@@ -123,6 +123,57 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
+// Phase accounting of the level kernel (tools/level_phases.py): built with -DMIPNERF_LEVEL_PHASES, thread 0 of each
+// consumer warpgroup and the producer thread charge the clock64 cycles since their previous mark to a phase, per CTA
+// and per level (slot 0: coarse fenceposts, slot 1: resampled).  Without the define, PhaseClock is empty and every
+// mark compiles to nothing.
+enum LevelPhase : int {
+  kPhPrologue,   // warp 0: fenceposts / resampler, view bias
+  kPhIpe,        // Gaussians + IPE features
+  kPhWFull,      // consumers: waiting for a weight stage (w_full)
+  kPhMma,        // consumers: wgmma issue and retire
+  kPhEpilogue,   // layer epilogues, view layer + colour head, head reductions, activation-dump issue
+  kPhComposite,  // warpgroup 0: activations + compositing (or the raw heads of MLP-only mode)
+  kPhBarrier,    // consumers: named-barrier waits
+  kPhWEmpty,     // producer: waiting for a free ring slot (w_empty)
+  kPhIssue,      // producer: everything else
+  kPhTotal,      // clock64 cycles from the role's first mark to its last
+  kNumPhases
+};
+#ifdef MIPNERF_LEVEL_PHASES
+constexpr int kPhaseMaxCtas = 1024;
+constexpr uint32_t kPhaseBytes = 3 * kNumPhases * 8;  // shared-memory accumulators, one row per role
+// [slot][cta][role: consumer wg 0, consumer wg 1, producer][phase]
+__device__ unsigned long long g_level_phases[2][kPhaseMaxCtas][3][kNumPhases];
+struct PhaseClock {
+  unsigned long long* acc;  // this role's row in shared memory; null on the threads that do not measure
+  long long start, last;
+  __device__ __forceinline__ void begin(unsigned long long* row, bool measuring) {
+    acc = measuring ? row : nullptr;
+    if (acc)
+      for (int i = 0; i < kNumPhases; ++i) acc[i] = 0;
+    start = last = clock64();
+  }
+  __device__ __forceinline__ void mark(int ph) {
+    const long long now = clock64();
+    if (acc) acc[ph] += (unsigned long long)(now - last);
+    last = now;
+  }
+  __device__ __forceinline__ void end(int slot, int role) {
+    if (!acc || blockIdx.x >= kPhaseMaxCtas) return;
+    acc[kPhTotal] = (unsigned long long)(last - start);
+    for (int i = 0; i < kNumPhases; ++i) atomicAdd(&g_level_phases[slot][blockIdx.x][role][i], acc[i]);
+  }
+};
+#else
+constexpr uint32_t kPhaseBytes = 0;
+struct PhaseClock {
+  __device__ __forceinline__ void begin(unsigned long long*, bool) {}
+  __device__ __forceinline__ void mark(int) {}
+  __device__ __forceinline__ void end(int, int) {}
+};
+#endif
+
 template <int kFmt>
 __device__ __forceinline__ void store8(uint8_t* dst, const float (&x)[8]) {
   *reinterpret_cast<uint4*>(dst) = make_uint4(pack2<kFmt>(x[0], x[1]), pack2<kFmt>(x[2], x[3]),
@@ -218,7 +269,10 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
 constexpr int kThreads = 384;
 template <bool kX3>
 struct LevelLayout {
-  static constexpr int kStages = kX3 ? 2 : 8;
+  // bf16 / fp16: the ring is kept at 4 stages so that the CTA fits the 132 KB shared-memory carveout and L1 keeps
+  // ~124 KB for the consumers' stack frames and the epilogue's bias loads.  Measured on H100: 4.31 ms per 4096-ray bf16
+  // forward at 4 stages, 4.58 ms at 8 (164 KB carveout), 5.84 / 5.99 ms at 12 / 16 (L1 down to 60 / 28 KB).
+  static constexpr int kStages = kX3 ? 2 : 4;
   static constexpr uint32_t kStage = kX3 ? 2 * kWStage : kWStage;  // split modes: W_hi stage, then W_lo
   static constexpr uint32_t kA = 0;
   static constexpr uint32_t kF = kA + (kX3 ? 2 : 1) * kABytes;  // split modes: hi tile, then lo tile
@@ -226,8 +280,11 @@ struct LevelLayout {
   static constexpr uint32_t kMisc = kW + kStages * kStage;
   // mbarriers, raw heads [2][128][4] (ray parity), scan carries [4], partial sums [4][8], resampler scratch [129]
   static constexpr uint32_t kMiscBytes = 2 * kStages * 8 + 2 * kN * 4 * 4 + 4 * 4 + 4 * 8 * 4 + (kN + 1) * 4;
-  static constexpr uint32_t kTotal = kMisc + kMiscBytes + 1024;  // + slack for the 1024-B alignment of the tiles
+  static constexpr uint32_t kPhase = (kMisc + kMiscBytes + 7) & ~7u;  // phase accumulators (MIPNERF_LEVEL_PHASES)
+  // + slack for the 1024-B alignment of the tiles
+  static constexpr uint32_t kTotal = kMisc + kMiscBytes + (kPhaseBytes ? kPhaseBytes + 8 : 0) + 1024;
   static_assert(kTotal <= 232448, "exceeds 227 KB of shared memory per CTA");
+  static_assert(kX3 || kTotal + 1024 <= 132 * 1024, "bf16 / fp16 layout no longer fits the 132 KB carveout");
 };
 
 // A-operand descriptor of K step j (16 wide) of K-slab s (32 wide) of layer l, for the rows of one warpgroup
@@ -243,12 +300,14 @@ __device__ __forceinline__ uint64_t level_a_desc(int l, int s, int j, uint32_t a
 template <int kFmt, bool kX3>
 __device__ __forceinline__ void level_mma_half(float (&acc)[64], int l, int nk, uint32_t a_u, uint32_t f_u,
                                                uint32_t ft_u, uint32_t w_u, uint64_t* w_full, uint64_t* w_empty,
-                                               int& st, uint32_t& ph, bool leader) {
+                                               int& st, uint32_t& ph, bool leader, PhaseClock& clk) {
   using Lay = LevelLayout<kX3>;
   int prev = -1;
   wgmma_fence_acc(acc);
   for (int s = 0; s < nk; ++s) {
+    clk.mark(kPhMma);
     mbar_wait(&w_full[st], ph);
+    clk.mark(kPhWFull);
     wgmma_fence();
     const uint32_t b_u = w_u + (uint32_t)st * Lay::kStage;
 #pragma unroll
@@ -273,6 +332,7 @@ __device__ __forceinline__ void level_mma_half(float (&acc)[64], int l, int nk, 
   wgmma_wait<0>();
   wgmma_fence_acc(acc);
   if (leader) mbar_arrive(&w_empty[prev]);
+  clk.mark(kPhMma);
 }
 
 // Epilogue of one N = 128 half (columns c_base..) of trunk layer / bottleneck l: + bias -> ReLU (l < 8) -> 16-bit ->
@@ -329,6 +389,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   float* cs = heads + 2 * kN * 4;                                      // [4] scan carries
   float* ps = cs + 4;                                                  // [4][8] partial sums
   float* rs_scratch = ps + 32;                                         // [129] resampler scratch
+  unsigned long long* phase_rows = reinterpret_cast<unsigned long long*>(smem + Lay::kPhase);
+  const int phase_slot = p.t_mode == 2 ? 1 : 0;
+  PhaseClock clk;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0) {
     for (int i = 0; i < Lay::kStages; ++i) {
@@ -343,6 +406,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
     // ============================ weight producer (warp 8; warps 9-11 only give their registers away) ============
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
     if (warp == 8 && lane == 0) {
+      clk.begin(phase_rows + 2 * kNumPhases, true);
       int st = 0;
       uint32_t ph = 0;
       const uint64_t pol = l2_policy_evict_last();  // the image is re-read by every CTA for every ray
@@ -351,7 +415,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
           const uint8_t* src = p.wimage + layer_offset(l);
           const int n = num_halves(l) * num_k32(l);  // stages in issue order: N-half major, then K-slab
           for (int i = 0; i < n; ++i) {
+            clk.mark(kPhIssue);
             mbar_wait(&w_empty[st], ph ^ 1);
+            clk.mark(kPhWEmpty);
             mbar_arrive_expect_tx(&w_full[st], Lay::kStage);
             bulk_g2s_hint(sW + st * Lay::kStage, src + (size_t)i * kWStage, kWStage, &w_full[st], pol);
             if (kX3) bulk_g2s_hint(sW + st * Lay::kStage + kWStage, src + kLoOffset + (size_t)i * kWStage, kWStage,
@@ -362,6 +428,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             }
           }
         }
+      clk.mark(kPhIssue);
+      clk.end(phase_slot, 2);
     }
     return;
   }
@@ -381,6 +449,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   bool dump_pending = false;
   int st = 0, par = 0;
   uint32_t ph = 0;
+  clk.begin(phase_rows + wg * kNumPhases, leader);
   for (int64_t ray = blockIdx.x; ray < p.num_rays; ray += gridDim.x, par ^= 1) {
     if (p.t_mode != 0 || p.vb_mode != 0) {
       // ---- ray prologue (warp 0); its global stores are read back by this CTA only, through L2 (ld.cg)
@@ -424,8 +493,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
           for (int j = 0; j < 4; ++j) __stcg(p.view_bias + ray * kCond + lane + 32 * j, acc[j]);
         }
         __threadfence_block();
+        clk.mark(kPhPrologue);
       }
       named_bar_sync(4, 256);
+      clk.mark(kPhBarrier);
     }
     {  // ---- Gaussians + IPE features of this warpgroup's rows: two threads per row, three 8-feature groups each
       const int row = 64 * wg + (t & 63), part = t >> 6;
@@ -438,24 +509,30 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       ipe_row_group<kFmt, kX3>(p, g, ray, row, t0, t1, sF, 3 * part, 3 * part + 3);
     }
     fence_proxy_async_smem();
+    clk.mark(kPhIpe);
     named_bar_sync(1 + wg, 128);
+    clk.mark(kPhBarrier);
 
     float d0 = 0.f, d1 = 0.f;  // density head, rows r0 / r0 + 8 (partial over this thread's columns)
     float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
     for (int l = 0; l < kNumLayers; ++l) {
       float acc0[64], acc1[64];
-      level_mma_half<kFmt, kX3>(acc0, l, num_k32(l), a_u, f_u, ft_u, w_u, w_full, w_empty, st, ph, leader);
+      level_mma_half<kFmt, kX3>(acc0, l, num_k32(l), a_u, f_u, ft_u, w_u, w_full, w_empty, st, ph, leader, clk);
       if (l < 9) {
-        level_mma_half<kFmt, kX3>(acc1, l, num_k32(l), a_u, f_u, ft_u, w_u, w_full, w_empty, st, ph, leader);
+        level_mma_half<kFmt, kX3>(acc1, l, num_k32(l), a_u, f_u, ft_u, w_u, w_full, w_empty, st, ph, leader, clk);
         if (dump_pending) {  // the previous layer's bulk store must have READ the tile before it is overwritten
           if (leader) bulk_store_wait_read();
           dump_pending = false;
+          clk.mark(kPhEpilogue);
           named_bar_sync(1 + wg, 128);
+          clk.mark(kPhBarrier);
         }
         level_epilogue_half<kFmt, kX3>(acc0, l, 0, r0, cq, sA, gsp, d0, d1);
         level_epilogue_half<kFmt, kX3>(acc1, l, 128, r0, cq, sA, gsp, d0, d1);
         fence_proxy_async_smem();
+        clk.mark(kPhEpilogue);
         named_bar_sync(1 + wg, 128);
+        clk.mark(kPhBarrier);
         if (p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core reads it
           if (leader) {
 #pragma unroll
@@ -465,6 +542,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             }
           }
           dump_pending = true;
+          clk.mark(kPhEpilogue);
         }
       } else {
         // view layer + colour head (models/mip_nerf.py:106-110); view_bias = the per-ray view-direction term
@@ -502,7 +580,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       *reinterpret_cast<float4*>(hd + r0 * 4) = make_float4(d0, rgb[0][0], rgb[0][1], rgb[0][2]);
       *reinterpret_cast<float4*>(hd + (r0 + 8) * 4) = make_float4(d1, rgb[1][0], rgb[1][1], rgb[1][2]);
     }
+    clk.mark(kPhEpilogue);
     named_bar_sync(3, 256);
+    clk.mark(kPhBarrier);
     if (wg == 1) continue;  // warpgroup 0 composites; warpgroup 1 goes on with the next ray
 
     // ============ activations + compositing over the ray's 128 samples (warpgroup 0, thread = sample row) ============
@@ -514,6 +594,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       p.raw_rgb_out[sidx * 3 + 1] = h4.z + c_small.b_color[1];
       p.raw_rgb_out[sidx * 3 + 2] = h4.w + c_small.b_color[2];
       p.raw_density_out[sidx] = h4.x + c_small.b_density;
+      clk.mark(kPhComposite);
       continue;
     }
     float raw_dens = h4.x + c_small.b_density;
@@ -542,7 +623,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
     float excl = __shfl_up_sync(0xffffffffu, incl, 1);
     if (lane == 0) excl = 0.f;
     if (lane == 31) cs[q] = incl;
+    clk.mark(kPhComposite);
     named_bar_sync(1, 128);
+    clk.mark(kPhBarrier);
     float before = 0.f;
     for (int qq = 0; qq < q; ++qq) before += cs[qq];
     const float w = -expm1f(-dd) * expf(-(before + excl));
@@ -553,7 +636,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       float* dst = ps + q * 8;
       dst[0] = pr, dst[1] = pg, dst[2] = pb, dst[3] = pw, dst[4] = pd;
     }
+    clk.mark(kPhComposite);
     named_bar_sync(1, 128);
+    clk.mark(kPhBarrier);
     if (row == 0) {
       float s[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
       for (int qq = 0; qq < 4; ++qq)
@@ -570,9 +655,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       p.distance[ray] = d;
       p.acc[ray] = s[3];
     }
+    clk.mark(kPhComposite);
     named_bar_sync(1, 128);  // row 0 has consumed ps / everyone cs before the next ray reuses them
+    clk.mark(kPhBarrier);
   }
   if (dump_pending && leader) bulk_store_wait_all();  // the last tile's store has left shared memory
+  clk.mark(kPhEpilogue);
+  clk.end(phase_slot, wg);
 }
 
 // MLP-only mode: same per-ray bias from a caller-supplied [B,27] view encoding
@@ -1002,3 +1091,18 @@ cudaError_t launch_view_bias_from_enc(const float* venc, const float* w, const f
 size_t tc_mlp_workspace_bytes(int64_t num_rays) { return (size_t)(num_rays > 0 ? num_rays : 1) * kCond * sizeof(float); }
 
 }  // namespace mipnerf
+
+#ifdef MIPNERF_LEVEL_PHASES
+// Instrumented builds only (tools/level_phases.py): copies the per-CTA phase cycles accumulated since the last call,
+// [2 slots][ctas][3 roles][phases] as uint64, into `out` and zeroes them.  Returns the phase count, or -1 on error.
+extern "C" int mipnerf_b200_level_phases(unsigned long long* out, int* ctas) {
+  using namespace mipnerf;
+  *ctas = kPhaseMaxCtas;
+  if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+  if (cudaMemcpyFromSymbol(out, g_level_phases, sizeof(g_level_phases)) != cudaSuccess) return -1;
+  void* dev = nullptr;
+  if (cudaGetSymbolAddress(&dev, g_level_phases) != cudaSuccess || cudaMemset(dev, 0, sizeof(g_level_phases)) != cudaSuccess)
+    return -1;
+  return kNumPhases;
+}
+#endif
