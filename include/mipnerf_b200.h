@@ -200,6 +200,36 @@ int mipnerf_b200_forward_backward_rng(const mipnerf_b200_config* cfg, const mipn
                                       const mipnerf_b200_linear_grad* grads, int num_grads, int accumulate,
                                       void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- backward pass of MipNerf.forward for any loss (autograd) ----------------------------------------
+ * Cotangents d L / d output of one level's rendered outputs; any pointer may be NULL (= zero). */
+typedef struct mipnerf_b200_level_cotangent {
+  const float* d_comp_rgb; /* [B,3] */
+  const float* d_distance; /* [B]   */
+  const float* d_acc;      /* [B]   */
+  const float* d_weights;  /* [B,N] */
+} mipnerf_b200_level_cotangent;
+
+/* Gradients of  L = sum_l <cots[l], (comp_rgb, distance, acc, weights)_l>  with respect to the MLP tensors, into
+ * `grads` (overwritten, or added to when `accumulate` != 0; same layout as mipnerf_b200_forward_backward).  The MLP
+ * is re-evaluated at the fenceposts a forward produced, `t_samples[l]` [B,N+1] (read only; they carry no gradient,
+ * stop_resample_grad=True), with the density noise of that forward: in-kernel Philox when `rng` is given (the
+ * forward's seed / offset), else density_normal[l] [B,N] (required when randomized and cfg->density_noise > 0).
+ * `randomized` only selects the density noise.  Same 4096-ray chunking and workspace as the training step
+ * (mipnerf_b200_train_workspace_bytes).  precision FP32 or BF16; FP16 is refused (its fixed gradient scale is sized
+ * for the training loss), the split precisions are forward-only. */
+int mipnerf_b200_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* weights,
+                          const mipnerf_b200_rays* rays, const float* const* t_samples, int randomized,
+                          const mipnerf_b200_rng* rng, const float* const* density_normal, int white_bkgd,
+                          int precision, const mipnerf_b200_level_cotangent* cots,
+                          const mipnerf_b200_linear_grad* grads, int num_grads, int accumulate, void* workspace,
+                          size_t workspace_bytes, void* stream);
+
+/* Gradient of distloss with respect to the weights (samples are constants):
+ * d_weights[r,i] = grad_out[0] * scale * d per_ray_loss_r / d w_ri  (grad_out: device scalar, NULL = 1; the
+ * reference's .mean() is scale = 1/num_rays). */
+int mipnerf_b200_distloss_backward(const float* weights, const float* samples, int64_t num_rays, int num_samples,
+                                   const float* grad_out, float scale, float* d_weights, void* stream);
+
 /* Stand-alone tensor-core linear layer  y[m,n] = act(x[m,k] . weight[n,k]^T + bias)  (wgmma, 16-bit operands, fp32
  * accumulate; n in {128,256}, k in {96,128,256}): the GEMM the training step uses for its forward and dgrad passes in
  * BF16 / FP16 mode.  `scratch` receives the packed weight image (n * ceil(k/64) * 128 bytes). */

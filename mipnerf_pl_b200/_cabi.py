@@ -70,6 +70,11 @@ class Loss(C.Structure):
                 ("per_ray_distloss", C.c_void_p)]
 
 
+class LevelCotangent(C.Structure):
+    _fields_ = [("d_comp_rgb", C.c_void_p), ("d_distance", C.c_void_p), ("d_acc", C.c_void_p),
+                ("d_weights", C.c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/mipnerf_b200.h declares.
 _V = C.c_void_p
 _SIGNATURES = {
@@ -92,6 +97,10 @@ _SIGNATURES = {
     "mipnerf_b200_forward_backward_rng": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), C.POINTER(RaysStruct),
                                                     C.POINTER(Rng), C.c_int, C.c_int, C.POINTER(Loss), C.POINTER(LevelOut),
                                                     C.POINTER(LinearGrad), C.c_int, C.c_int, _V, C.c_size_t, _V]),
+    "mipnerf_b200_backward": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), C.POINTER(RaysStruct), _V, C.c_int,
+                                        C.POINTER(Rng), _V, C.c_int, C.c_int, C.POINTER(LevelCotangent),
+                                        C.POINTER(LinearGrad), C.c_int, C.c_int, _V, C.c_size_t, _V]),
+    "mipnerf_b200_distloss_backward": (C.c_int, [_V, _V, C.c_int64, C.c_int, _V, C.c_float, _V, _V]),
     "mipnerf_b200_linear_tc": (C.c_int, [_V, _V, _V, _V, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),
     "mipnerf_b200_wgrad_tc_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "mipnerf_b200_wgrad_tc": (C.c_int, [_V, C.c_int, _V, C.c_int, _V, C.c_int, C.c_int, C.c_int64, _V, _V, C.c_int, _V,

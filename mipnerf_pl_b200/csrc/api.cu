@@ -439,6 +439,13 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
     return p;
   };
   auto take = [&](size_t elems) { return reinterpret_cast<float*>(take_bytes(elems * sizeof(float))); };
+  // chunk-invariant buffers first: the weight images are packed once per call into the first chunk's carve and read
+  // by every chunk, so no per-ray buffer of a shorter last chunk may move onto them
+  const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
+  const size_t max_k = (size_t)c->net_width + (d.xyz_dim > d.view_dim ? d.xyz_dim : d.view_dim) + 1;
+  s.part = take((size_t)mipnerf::kWgradMaxSlices * max_n * max_k);
+  s.images = take_bytes((size_t)kTrainImages * kTrainImageBytes);
+  s.packed = take_bytes(mipnerf::tc_packed_bytes(c, precision));
   for (int l = 0; l < 2; ++l) {
     s.act[l] = take_bytes((size_t)9 * rays * 65536);
     s.v[l] = take_bytes((size_t)rays * 32768);
@@ -456,11 +463,6 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
   s.d_v = take_bytes((size_t)rays * 32768);
   s.d_a = take_bytes((size_t)rays * 65536);
   s.d_b = take_bytes((size_t)rays * 65536);
-  const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
-  const size_t max_k = (size_t)c->net_width + (d.xyz_dim > d.view_dim ? d.xyz_dim : d.view_dim) + 1;
-  s.part = take((size_t)mipnerf::kWgradMaxSlices * max_n * max_k);
-  s.images = take_bytes((size_t)kTrainImages * kTrainImageBytes);
-  s.packed = take_bytes(mipnerf::tc_packed_bytes(c, precision));
   s.tcws_bytes = mipnerf::tc_workspace_bytes(c, rays, precision);
   s.tcws = take_bytes(s.tcws_bytes);
   s.bytes = off;
@@ -498,6 +500,37 @@ int check_train_config(const mipnerf_b200_config* c) {
 inline bool takes_skip(const mipnerf_b200_config* c, int layer) {  // models/mip_nerf.py:40-42
   return layer > 1 && (layer - 1) % c->skip_index == 0;
 }
+
+// Where the backward pass of a training driver starts: the loss of mipnerf_b200_loss, or cotangents of the rendered
+// outputs (one entry per level).  Everything after the render backward only sees d raw_rgb / d raw_density.
+struct GradSource {
+  const mipnerf_b200_loss* loss;
+  const mipnerf_b200_level_cotangent* cots;
+};
+
+// d raw_rgb / d raw_density of level l for the chunk [off, off + cnt) of a B-ray call.  `gscale` multiplies the loss
+// gradient (the fp16 step's fixed scale, 1 otherwise).
+cudaError_t launch_grad_source(const GradSource& g, const mipnerf_b200_config* c, int l, int64_t off, int64_t B,
+                               int64_t cnt, const float* raw_rgb, const float* raw_dens, const float* t,
+                               const float* dirs, int white_bkgd, float rgb_scale, float gscale, float* d_raw_rgb,
+                               float* d_raw_dens, cudaStream_t st) {
+  const int n = c->num_samples;
+  if (g.cots) {
+    const mipnerf_b200_level_cotangent& k = g.cots[l];
+    const mipnerf::RenderCot cot{k.d_comp_rgb ? k.d_comp_rgb + off * 3 : nullptr,
+                                 k.d_distance ? k.d_distance + off : nullptr, k.d_acc ? k.d_acc + off : nullptr,
+                                 k.d_weights ? k.d_weights + off * n : nullptr};
+    return mipnerf::launch_render_vjp(raw_rgb, raw_dens, t, dirs, cot, white_bkgd, c->density_bias, rgb_scale,
+                                      c->rgb_padding, d_raw_rgb, d_raw_dens, cnt, n, st);
+  }
+  const mipnerf_b200_loss* loss = g.loss;
+  return mipnerf::launch_render_backward(
+      raw_rgb, raw_dens, t, dirs, loss->target_rgb + off * 3, loss->lossmult ? loss->lossmult + off : nullptr,
+      loss->mask_sum, loss->level_mse_mult[l] * gscale, loss->level_dist_mult[l] * loss->dist_scale * gscale,
+      white_bkgd, c->density_bias, rgb_scale, c->rgb_padding, d_raw_rgb, d_raw_dens,
+      loss->per_ray_sqerr ? loss->per_ray_sqerr + (int64_t)l * B + off : nullptr,
+      loss->per_ray_distloss ? loss->per_ray_distloss + (int64_t)l * B + off : nullptr, cnt, n, st);
+}
 }  // namespace
 
 size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_rays) {
@@ -517,7 +550,7 @@ size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_
 static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d, const mipnerf_b200_weights* w,
                                   const mipnerf_b200_rays* rays, int randomized, const float* t_rand,
                                   const float* u_jitter, const mipnerf_b200_rng* rng, int white_bkgd, int precision,
-                                  const mipnerf_b200_loss* loss, mipnerf_b200_level_out* outs,
+                                  const GradSource& src, bool given_t, mipnerf_b200_level_out* outs,
                                   const mipnerf_b200_linear_grad* grads, bool* touched, void* workspace,
                                   cudaStream_t st) {
   const int n = cfg->num_samples, depth = cfg->net_depth, W = cfg->net_width, Wc = cfg->net_width_condition;
@@ -559,7 +592,11 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
     mipnerf::TcTrainDump dump{};
     for (int l = 0; l < cfg->num_levels; ++l) {
       lo[l] = outs[l];
-      lo[l].comp_rgb = outs[l].comp_rgb + off * 3, lo[l].distance = outs[l].distance + off, lo[l].acc = outs[l].acc + off;
+      if (given_t) {  // the recompute's pixels are not needed: they go to the (unused) fencepost scratch
+        lo[l].comp_rgb = s.t[l], lo[l].distance = s.t[l] + 3 * cnt, lo[l].acc = s.t[l] + 4 * cnt;
+      } else {
+        lo[l].comp_rgb = outs[l].comp_rgb + off * 3, lo[l].distance = outs[l].distance + off, lo[l].acc = outs[l].acc + off;
+      }
       lo[l].t_samples = outs[l].t_samples ? outs[l].t_samples + off * (n + 1) : s.t[l];
       lo[l].weights = outs[l].weights ? outs[l].weights + off * n : s.w[l];
       lo[l].inds = outs[l].inds ? outs[l].inds + off * (n + 1) : nullptr;
@@ -568,7 +605,7 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
     }
     CUDA_TRY(mipnerf::tc_forward(cfg, &wl, &rc_, randomized, t_rand ? t_rand + off * (n + 1) : nullptr,
                                  u_jitter ? u_jitter + off * (n + 1) : nullptr, rng, white_bkgd, precision, lo, s.tcws,
-                                 s.tcws_bytes, st, &dump, off));
+                                 s.tcws_bytes, st, &dump, off, given_t ? 1 : 0));
     // MIPNERF_B200_TRAIN_MASKBITS=0: the dgrad GEMMs read the ReLU mask from the activation tile images again (A/B)
     const char* bits_env = getenv("MIPNERF_B200_TRAIN_MASKBITS");
     const bool use_bits = !(bits_env && bits_env[0] == '0');
@@ -593,13 +630,8 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
       // straight into a tile image so that those wgrads stage them by bulk copy like every other operand
       CUDA_TRY(mipnerf::launch_ipe_t16(rc_.origins, rc_.directions, rc_.radii, t_cur, s.enc16, cnt, n,
                                        cfg->disable_integration, precision, st));
-      CUDA_TRY(mipnerf::launch_render_backward(
-          s.raw_rgb[l], s.raw_density[l], t_cur, rc_.directions, loss->target_rgb + off * 3,
-          loss->lossmult ? loss->lossmult + off : nullptr, loss->mask_sum, loss->level_mse_mult[l] * gscale,
-          loss->level_dist_mult[l] * loss->dist_scale * gscale, white_bkgd, cfg->density_bias, rgb_scale,
-          cfg->rgb_padding, s.d_raw_rgb, s.d_raw_density,
-          loss->per_ray_sqerr ? loss->per_ray_sqerr + (int64_t)l * B + off : nullptr,
-          loss->per_ray_distloss ? loss->per_ray_distloss + (int64_t)l * B + off : nullptr, cnt, n, st));
+      CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb[l], s.raw_density[l], t_cur, rc_.directions,
+                                  white_bkgd, rgb_scale, gscale, s.d_raw_rgb, s.d_raw_density, st));
       // colour head, view layer                                          (models/mip_nerf.py:106-110)
       CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(s.d_raw_rgb, 3, s.v[l], Wc, s.part, grads[d.n_lin - 1].weight_grad,
                                                  grads[d.n_lin - 1].bias_grad, touched[d.n_lin - 1] ? 1 : 0, m,
@@ -638,10 +670,13 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
   return MIPNERF_B200_OK;
 }
 
+// The training drivers: forward with every activation the backward needs, then the backward pass from `src`.
+// given_t: each level's fenceposts come from outs[l].t_samples (read-only) instead of being sampled / resampled, and
+// the recomputed pixels are not returned (the backward pass of MipNerf.forward, mipnerf_b200_backward).
 static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
                                  const mipnerf_b200_rays* rays, int randomized, const float* t_rand,
                                  const float* u_jitter, const mipnerf_b200_rng* rng, int white_bkgd, int precision,
-                                 const mipnerf_b200_loss* loss, mipnerf_b200_level_out* outs,
+                                 const GradSource& src, bool given_t, mipnerf_b200_level_out* outs,
                                  const mipnerf_b200_linear_grad* grads, int num_grads, int accumulate,
                                  void* workspace, size_t workspace_bytes, void* stream) {
   Dims d;
@@ -658,20 +693,28 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   if (tc && !train_tc_supported(cfg, d))
     return fail(MIPNERF_B200_EUNSUPPORTED,
                 "tensor-core training GEMMs: 8x256 trunk / 128 view layer / 96-d IPE only; use MIPNERF_B200_FP32");
-  if (!outs || !loss || !grads) return fail(MIPNERF_B200_EINVAL, "outs / loss / grads is NULL");
+  if (!outs || !(src.loss || src.cots) || !grads) return fail(MIPNERF_B200_EINVAL, "outs / loss / grads is NULL");
+  if (src.cots && precision == MIPNERF_B200_FP16)
+    return fail(MIPNERF_B200_EUNSUPPORTED,
+                "backward from arbitrary cotangents: FP16's fixed gradient scale is sized for the training loss; use "
+                "BF16 (same tensor-core path, fp32 range) or FP32");
   if (num_grads != d.n_lin) return fail(MIPNERF_B200_EINVAL, "expected %d gradient pairs, got %d", d.n_lin, num_grads);
   for (int i = 0; i < d.n_lin; ++i)
     if (!grads[i].weight_grad || !grads[i].bias_grad) return fail(MIPNERF_B200_EINVAL, "grads[%d] has a NULL tensor", i);
-  if (!loss->level_mse_mult || !loss->level_dist_mult)
+  if (src.loss && (!src.loss->level_mse_mult || !src.loss->level_dist_mult))
     return fail(MIPNERF_B200_EINVAL, "loss multipliers are NULL");
-  if (rays->num_rays > 0 && (!loss->target_rgb || !loss->mask_sum || !rays->viewdirs))
+  if (src.loss && rays->num_rays > 0 && (!src.loss->target_rgb || !src.loss->mask_sum || !rays->viewdirs))
     return fail(MIPNERF_B200_EINVAL, "target_rgb / mask_sum / viewdirs is NULL");
-  if (randomized && !rng && (!t_rand || (cfg->num_levels > 1 && !u_jitter)))
+  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "viewdirs is NULL");
+  if (!given_t && randomized && !rng && (!t_rand || (cfg->num_levels > 1 && !u_jitter)))
     return fail(MIPNERF_B200_EINVAL,
                 "randomized=1 needs t_rand and u_jitter (injected noise) or the _rng entry point (in-kernel Philox)");
-  for (int l = 0; l < cfg->num_levels; ++l)
-    if (rays->num_rays > 0 && (!outs[l].comp_rgb || !outs[l].distance || !outs[l].acc))
+  for (int l = 0; l < cfg->num_levels; ++l) {
+    if (!given_t && rays->num_rays > 0 && (!outs[l].comp_rgb || !outs[l].distance || !outs[l].acc))
       return fail(MIPNERF_B200_EINVAL, "outs[%d] misses comp_rgb/distance/acc", l);
+    if (given_t && rays->num_rays > 0 && !outs[l].t_samples)
+      return fail(MIPNERF_B200_EINVAL, "t_samples[%d] is NULL", l);
+  }
   {
     const int rcn = check_density_normals(cfg, randomized, rng, outs, rays->num_rays);
     if (rcn) return rcn;
@@ -695,8 +738,8 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   {
     const char* fused_env = getenv("MIPNERF_B200_TRAIN_FUSED");
     if (tc && B > 0 && train_fused_supported(cfg, precision) && !(fused_env && fused_env[0] == '0'))
-      return forward_backward_fused(cfg, d, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision, loss, outs,
-                                    grads, touched, workspace, st);
+      return forward_backward_fused(cfg, d, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision, src,
+                                    given_t, outs, grads, touched, workspace, st);
   }
   // ---- tensor-core mode: B operands of every forward / dgrad GEMM, packed once per call (the weights change every
   //      optimiser step).  fwd[i] = W_i[:, :k_main], fwd_skip[i] = W_i[:, 256:352], bwd[i] = W_i[:, :256]^T;
@@ -759,8 +802,14 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
     for (int l = 0; l < cfg->num_levels; ++l) {
       float* t_cur = outs[l].t_samples ? outs[l].t_samples + off * (n + 1) : s.t[l & 1];
       float* w_cur = outs[l].weights ? outs[l].weights + off * n : s.w[l & 1];
+      // given fenceposts: the recomputed pixels go to the (unused) fencepost scratch
+      float* comp_cur = given_t ? s.t[l & 1] : outs[l].comp_rgb + off * 3;
+      float* dist_cur = given_t ? s.t[l & 1] + 3 * cnt : outs[l].distance + off;
+      float* acc_cur = given_t ? s.t[l & 1] + 4 * cnt : outs[l].acc + off;
       // ---- forward of this level, every activation kept (models/mip_nerf.py:203-240)
-      if (l == 0) {
+      if (given_t) {
+        // the caller's fenceposts: nothing to sample
+      } else if (l == 0) {
         CUDA_TRY(mipnerf::launch_coarse_t(rc_.near, rc_.far, mipnerf::level_draws(randomized, t_rand, rng, off, 0, n + 1),
                                           t_cur, cnt, n, randomized, cfg->disparity, st));
       } else {
@@ -810,17 +859,13 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
       }
       CUDA_TRY(mipnerf::launch_linear_f32(s.v, Wc, Wc, nullptr, 0, 0, 1, cl.weight, cl.bias, s.raw_rgb, 3, m, 3, 0,
                                           st));
-      CUDA_TRY(mipnerf::launch_composite(s.raw_rgb, s.raw_density, t_cur, rc_.directions, outs[l].comp_rgb + off * 3,
-                                         outs[l].distance + off, outs[l].acc + off, w_cur, cnt, n, white_bkgd, 1,
-                                         cfg->density_bias, rgb_scale, cfg->rgb_padding, st));
+      CUDA_TRY(mipnerf::launch_composite(s.raw_rgb, s.raw_density, t_cur, rc_.directions, comp_cur, dist_cur, acc_cur,
+                                         w_cur, cnt, n, white_bkgd, 1, cfg->density_bias, rgb_scale, cfg->rgb_padding,
+                                         st));
 
       // ---- backward of this level (its fenceposts are constants, so levels are independent here)
-      CUDA_TRY(mipnerf::launch_render_backward(
-          s.raw_rgb, s.raw_density, t_cur, rc_.directions, loss->target_rgb + off * 3,
-          loss->lossmult ? loss->lossmult + off : nullptr, loss->mask_sum, loss->level_mse_mult[l],
-          loss->level_dist_mult[l] * loss->dist_scale, white_bkgd, cfg->density_bias, rgb_scale, cfg->rgb_padding,
-          s.d_raw_rgb, s.d_raw_density, loss->per_ray_sqerr ? loss->per_ray_sqerr + (int64_t)l * B + off : nullptr,
-          loss->per_ray_distloss ? loss->per_ray_distloss + (int64_t)l * B + off : nullptr, cnt, n, st));
+      CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb, s.raw_density, t_cur, rc_.directions, white_bkgd,
+                                  rgb_scale, 1.f, s.d_raw_rgb, s.d_raw_density, st));
       // colour head, view layer                                          (models/mip_nerf.py:106-110)
       CUDA_TRY(wgrad(d.n_lin - 1, s.d_raw_rgb, s.v, Wc, nullptr, 0, 1));
       CUDA_TRY(mipnerf::launch_color_dgrad(s.d_raw_rgb, cl.weight, s.v, s.d_v, m, Wc, st));
@@ -871,8 +916,9 @@ int mipnerf_b200_forward_backward(const mipnerf_b200_config* cfg, const mipnerf_
                                   const mipnerf_b200_loss* loss, mipnerf_b200_level_out* outs,
                                   const mipnerf_b200_linear_grad* grads, int num_grads, int accumulate,
                                   void* workspace, size_t workspace_bytes, void* stream) {
-  return forward_backward_impl(cfg, w, rays, randomized, t_rand, u_jitter, nullptr, white_bkgd, precision, loss, outs,
-                               grads, num_grads, accumulate, workspace, workspace_bytes, stream);
+  return forward_backward_impl(cfg, w, rays, randomized, t_rand, u_jitter, nullptr, white_bkgd, precision,
+                               GradSource{loss, nullptr}, false, outs, grads, num_grads, accumulate, workspace,
+                               workspace_bytes, stream);
 }
 
 int mipnerf_b200_forward_backward_rng(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
@@ -881,8 +927,29 @@ int mipnerf_b200_forward_backward_rng(const mipnerf_b200_config* cfg, const mipn
                                       const mipnerf_b200_linear_grad* grads, int num_grads, int accumulate,
                                       void* workspace, size_t workspace_bytes, void* stream) {
   if (!rng) return fail(MIPNERF_B200_EINVAL, "rng is NULL");
-  return forward_backward_impl(cfg, w, rays, 1, nullptr, nullptr, rng, white_bkgd, precision, loss, outs, grads, num_grads,
-                               accumulate, workspace, workspace_bytes, stream);
+  return forward_backward_impl(cfg, w, rays, 1, nullptr, nullptr, rng, white_bkgd, precision, GradSource{loss, nullptr},
+                               false, outs, grads, num_grads, accumulate, workspace, workspace_bytes, stream);
+}
+
+int mipnerf_b200_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const mipnerf_b200_rays* rays,
+                          const float* const* t_samples, int randomized, const mipnerf_b200_rng* rng,
+                          const float* const* density_normal, int white_bkgd, int precision,
+                          const mipnerf_b200_level_cotangent* cots, const mipnerf_b200_linear_grad* grads,
+                          int num_grads, int accumulate, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!cfg) return fail(MIPNERF_B200_EINVAL, "config is NULL");
+  if (!t_samples || !cots) return fail(MIPNERF_B200_EINVAL, "t_samples / cots is NULL");
+  if (cfg->num_levels < 1 || cfg->num_levels > 64) return fail(MIPNERF_B200_EINVAL, "num_levels=%d", cfg->num_levels);
+  mipnerf_b200_level_out outs[64];
+  for (int l = 0; l < cfg->num_levels; ++l) {
+    outs[l] = mipnerf_b200_level_out{};
+    outs[l].t_samples = const_cast<float*>(t_samples[l]);  // read only (given_t)
+    outs[l].density_normal = density_normal ? density_normal[l] : nullptr;
+  }
+  if (rng)  // in-kernel normals: injected ones are ignored, as by the _rng forward
+    for (int l = 0; l < cfg->num_levels; ++l) outs[l].density_normal = nullptr;
+  return forward_backward_impl(cfg, w, rays, randomized, nullptr, nullptr, rng, white_bkgd, precision,
+                               GradSource{nullptr, cots}, true, outs, grads, num_grads, accumulate, workspace,
+                               workspace_bytes, stream);
 }
 
 int mipnerf_b200_linear_tc(const float* x, const float* weight, const float* bias, float* y, int64_t m, int n,
@@ -963,6 +1030,15 @@ int mipnerf_b200_distloss(const float* weights, const float* samples, int64_t nu
   if (num_rays < 0 || num_samples < 1) return fail(MIPNERF_B200_EINVAL, "bad sizes");
   if (num_rays > 0 && (!weights || !samples || !per_ray_loss)) return fail(MIPNERF_B200_EINVAL, "NULL tensor");
   CUDA_TRY(mipnerf::launch_distloss(weights, samples, per_ray_loss, num_rays, num_samples, (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_distloss_backward(const float* weights, const float* samples, int64_t num_rays, int num_samples,
+                                   const float* grad_out, float scale, float* d_weights, void* stream) {
+  if (num_rays < 0 || num_samples < 1) return fail(MIPNERF_B200_EINVAL, "bad sizes");
+  if (num_rays > 0 && (!weights || !samples || !d_weights)) return fail(MIPNERF_B200_EINVAL, "NULL tensor");
+  CUDA_TRY(mipnerf::launch_distloss_backward(weights, samples, grad_out, scale, d_weights, num_rays, num_samples,
+                                             (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

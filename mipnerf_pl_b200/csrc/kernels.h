@@ -12,6 +12,9 @@ namespace mipnerf {
 // ---- ray_kernels.cu ----
 cudaError_t launch_distloss(const float* weights, const float* t, float* out, int64_t num_rays, int n,
                             cudaStream_t st);
+// d_w[r,i] = grad_out * scale * ((2/3) (t_{i+1} - t_i) w_i + 2 S_i),  S_i = sum_j w_j |m_i - m_j|  (grad_out NULL = 1)
+cudaError_t launch_distloss_backward(const float* weights, const float* t, const float* grad_out, float scale,
+                                     float* d_w, int64_t num_rays, int n, cudaStream_t st);
 cudaError_t launch_generate_rays(const float* c2w_host, int height, int width, float focal, float near_v,
                                  float far_v, int row0, int rows, float* origins, float* directions,
                                  float* viewdirs, float* radii, float* near_o, float* far_o, cudaStream_t st);
@@ -62,6 +65,15 @@ cudaError_t launch_render_backward(const float* raw_rgb, const float* raw_dens, 
                                    float mse_mult, float dist_mult, int white_bkgd, float density_bias,
                                    float rgb_scale, float rgb_padding, float* d_raw_rgb, float* d_raw_dens,
                                    float* sqerr_out, float* dist_out, int64_t num_rays, int n, cudaStream_t st);
+// cotangents of one level's rendered outputs (each [B,3] / [B] / [B] / [B,N], NULL = zero), for launch_render_vjp
+struct RenderCot {
+  const float *d_comp_rgb, *d_distance, *d_acc, *d_weights;
+};
+// d raw_rgb / d raw_density of  sum <cot, (comp_rgb, distance, acc, weights)>  (render_backward_kernel's recompute)
+cudaError_t launch_render_vjp(const float* raw_rgb, const float* raw_dens, const float* t, const float* dirs,
+                              const RenderCot& cot, int white_bkgd, float density_bias, float rgb_scale,
+                              float rgb_padding, float* d_raw_rgb, float* d_raw_dens, int64_t num_rays, int n,
+                              cudaStream_t st);
 cudaError_t launch_color_dgrad(const float* d_rgb, const float* wc, const float* v, float* d_v, int64_t m,
                                int k_dim, cudaStream_t st);
 // dX[m,k] = (act[m,k] > 0 or act == NULL) * (dY[m,:n_dim] @ W[:n_dim, :k_dim] (row stride ldw) + r1[m] * r1w[k])

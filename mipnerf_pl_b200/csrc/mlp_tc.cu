@@ -989,7 +989,8 @@ Draws density_noise_draws(const mipnerf_b200_config* c, int randomized, const fl
 cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, const mipnerf_b200_rays* rays,
                        int randomized, const float* t_rand, const float* u_jitter, const mipnerf_b200_rng* rng,
                        int white_bkgd, int precision, mipnerf_b200_level_out* outs, void* workspace,
-                       size_t workspace_bytes, cudaStream_t st, const TcTrainDump* dump, int64_t ray_base) {
+                       size_t workspace_bytes, cudaStream_t st, const TcTrainDump* dump, int64_t ray_base,
+                       int given_t) {
   const uint8_t* img = static_cast<const uint8_t*>(w->packed);
   SmallUpload small(img, st);  // biases / heads -> constant bank, ordered against other streams' forwards
   cudaError_t e = small.error();
@@ -1019,7 +1020,7 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
       p.origins = origins, p.directions = directions, p.radii = radii;
       p.t = t_cur;
       p.view_bias = s.vbias;
-      p.t_mode = l == 0 ? 1 : 2;
+      p.t_mode = given_t ? 0 : (l == 0 ? 1 : 2);  // 0: the caller's fenceposts in outs[l].t_samples
       p.vb_mode = l == 0 ? 1 : 0;  // level 0 leaves the per-ray bias in s.vbias for the later levels
       p.near = rays->near + off, p.far = rays->far + off;
       p.t_rand = draws(t_rand, 0);

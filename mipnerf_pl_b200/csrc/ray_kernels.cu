@@ -277,6 +277,43 @@ __global__ void distloss_kernel(const float* __restrict__ weights, const float* 
   if (lane == 0) out[ray] = (float)v;
 }
 
+// Its gradient with respect to the weights (samples are constants: stop_resample_grad), the same two scans:
+//   d/dw_i = (2/3) d_i w_i + 2 S_i,   S_i = sum_j w_j |m_i - m_j| = m_i (W_<i - W_>i) - (M_<i - M_>i).
+__global__ void distloss_backward_kernel(const float* __restrict__ weights, const float* __restrict__ t,
+                                         const float* __restrict__ grad_out, float scale, float* __restrict__ d_w,
+                                         int64_t num_rays, int n) {
+  const int lane = threadIdx.x & 31;
+  const int64_t ray = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (ray >= num_rays) return;
+  const float* w = weights + ray * n;
+  const float* tr = t + ray * (n + 1);
+  const int per = (n + 31) / 32;
+  double w_run = 0.0, m_run = 0.0;
+  for (int p = 0; p < per; ++p) {
+    const int i = lane * per + p;
+    if (i < n) {
+      const double wi = w[i], mi = 0.5 * ((double)tr[i] + (double)tr[i + 1]);
+      w_run += wi;
+      m_run += wi * mi;
+    }
+  }
+  double w_tot, m_tot;
+  double w_lt = warp_excl_scan_f64(w_run, lane, w_tot);
+  double m_lt = warp_excl_scan_f64(m_run, lane, m_tot);
+  const double up = (double)(grad_out ? __ldg(grad_out) : 1.0f) * (double)scale;
+  for (int p = 0; p < per; ++p) {
+    const int i = lane * per + p;
+    if (i < n) {
+      const double wi = w[i], t0 = tr[i], t1 = tr[i + 1], mi = 0.5 * (t0 + t1);
+      const double w_gt = w_tot - w_lt - wi, m_gt = m_tot - m_lt - wi * mi;
+      const double s_i = mi * (w_lt - w_gt) - (m_lt - m_gt);
+      d_w[ray * n + i] = (float)(up * ((2.0 / 3.0) * (t1 - t0) * wi + 2.0 * s_i));
+      w_lt += wi;
+      m_lt += wi * mi;
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // Blender-style pinhole rays for rows [row0, row0+rows) of an H x W frame, straight into HBM
 // (datasets/datasets.py:214-263, render_video.py:29-105): one thread per pixel.
@@ -414,6 +451,14 @@ cudaError_t launch_distloss(const float* weights, const float* t, float* out, in
   if (num_rays == 0) return cudaSuccess;
   LaunchScope scope(kKernDistloss, st);
   distloss_kernel<<<blocks_for(num_rays, 4), 128, 0, st>>>(weights, t, out, num_rays, n);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_distloss_backward(const float* weights, const float* t, const float* grad_out, float scale,
+                                     float* d_w, int64_t num_rays, int n, cudaStream_t st) {
+  if (num_rays == 0) return cudaSuccess;
+  LaunchScope scope(kKernDistloss, st);
+  distloss_backward_kernel<<<blocks_for(num_rays, 4), 128, 0, st>>>(weights, t, grad_out, scale, d_w, num_rays, n);
   return cudaGetLastError();
 }
 

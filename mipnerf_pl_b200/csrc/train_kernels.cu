@@ -9,7 +9,8 @@
 //   loss -> comp_rgb / weights -> (rgb, density) -> raw heads -> MLP.
 //
 // Kernels:
-//   render_backward_kernel   warp per ray: d loss / d raw_rgb, d raw_density (+ the per-ray loss terms)
+//   render_backward_kernel   warp per ray: d loss / d raw_rgb, d raw_density (+ the per-ray loss terms); the
+//                            same kernel turns arbitrary cotangents of the rendered outputs into them (render VJP)
 //   color_dgrad_kernel       d v   = relu'(v)  * (d raw_rgb @ Wc)                     (N = 3)
 //   dgrad_f32_kernel         d X   = relu'(act) * (d Y @ W[:, :k] + r[m] * rw[k])       128x128x16 FFMA tiles
 //   wgrad_f32_kernel         per M-slice partials of  dY^T @ [X1 | X2 | 1]  (last column = bias grad)
@@ -35,7 +36,13 @@ inline unsigned blocks_of(int64_t n, int per_block) { return (unsigned)((n + per
 // distloss (models/mip.py:8-20) with sorted midpoints:  d/dw_i = (2/3) len_i w_i + 2 S_i,
 //   S_i = sum_j w_j |m_i - m_j| = m_i (W_<i - W_>i) - (M_<i - M_>i)      (two prefix sums)
 // -------------------------------------------------------------------------------------------------
-template <int P>
+// kCot = false: (g, gw) come from the training loss above.  kCot = true (render VJP): from arbitrary cotangents of
+// the outputs (comp_rgb, distance, acc, weights), any of them NULL = zero:
+//   g = d comp_rgb,  gw_i = d w_i + g . rgb_i - [white_bkgd] sum_c g_c + d acc + g_D tmid_i,
+//   g_D = d distance where D = sum_i w_i tmid_i is finite and t_0 <= D <= t_N, else 0 (torch's backward of
+//   clamp(nan_to_num(D), t_0, t_N) with tensor bounds, models/mip.py:395-397).
+// Both share the recompute and the transmittance suffix scan.
+template <int P, bool kCot>
 __global__ void render_backward_kernel(const float* __restrict__ raw_rgb, const float* __restrict__ raw_dens,
                                        const float* __restrict__ t, const float* __restrict__ dirs,
                                        const float* __restrict__ target, const float* __restrict__ lossmult,
@@ -43,7 +50,7 @@ __global__ void render_backward_kernel(const float* __restrict__ raw_rgb, const 
                                        int white_bkgd, float density_bias, float rgb_scale, float rgb_padding,
                                        float* __restrict__ d_raw_rgb, float* __restrict__ d_raw_dens,
                                        float* __restrict__ sqerr_out, float* __restrict__ dist_out,
-                                       int64_t num_rays) {
+                                       int64_t num_rays, RenderCot cot) {
   constexpr int N = P * 32;
   const int lane = threadIdx.x & 31;
   const int64_t ray = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -93,45 +100,72 @@ __global__ void render_backward_kernel(const float* __restrict__ raw_rgb, const 
   const float comp[3] = {cr + bg, cg + bg, cb + bg};
 
   // ---- d loss / d comp_rgb                                   (models/nerf_system.py:104-105)
-  const float mask = lossmult ? __ldg(lossmult + ray) : 1.0f;
-  const float inv_ms = 1.0f / __ldg(mask_sum);
-  float g[3], sq = 0.f;
+  float g[3], mask = 1.0f, sq = 0.f;
+  if constexpr (!kCot) {
+    mask = lossmult ? __ldg(lossmult + ray) : 1.0f;
+    const float inv_ms = 1.0f / __ldg(mask_sum);
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const float e = comp[c] - __ldg(target + ray * 3 + c);
-    sq += e * e;
-    g[c] = mse_mult * 2.0f * mask * e * inv_ms;
+    for (int c = 0; c < 3; ++c) {
+      const float e = comp[c] - __ldg(target + ray * 3 + c);
+      sq += e * e;
+      g[c] = mse_mult * 2.0f * mask * e * inv_ms;
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g[c] = cot.d_comp_rgb ? __ldg(cot.d_comp_rgb + ray * 3 + c) : 0.f;
   }
   const float gsum_bg = white_bkgd ? (g[0] + g[1] + g[2]) : 0.0f;
 
-  // ---- distloss prefix sums (midpoints relative to t_0: |m_i - m_j| is shift invariant)
-  double w_run = 0.0, m_run = 0.0;
-  float mid[P];
-#pragma unroll
-  for (int p = 0; p < P; ++p) {
-    mid[p] = 0.5f * ((tt[p] - t_first) + (tt[p + 1] - t_first));
-    w_run += (double)w[p];
-    m_run += (double)w[p] * (double)mid[p];
-  }
-  double w_tot, m_tot;
-  double w_lt = warp_excl_scan_f64(w_run, lane, w_tot);
-  double m_lt = warp_excl_scan_f64(m_run, lane, m_tot);
-
   float gw[P];
-  double gww_run = 0.0, gww_incl[P], dist_val = 0.0;
+  double dist_val = 0.0;
+  if constexpr (!kCot) {
+    // ---- distloss prefix sums (midpoints relative to t_0: |m_i - m_j| is shift invariant)
+    double w_run = 0.0, m_run = 0.0;
+    float mid[P];
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      mid[p] = 0.5f * ((tt[p] - t_first) + (tt[p + 1] - t_first));
+      w_run += (double)w[p];
+      m_run += (double)w[p] * (double)mid[p];
+    }
+    double w_tot, m_tot;
+    double w_lt = warp_excl_scan_f64(w_run, lane, w_tot);
+    double m_lt = warp_excl_scan_f64(m_run, lane, m_tot);
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      const double wi = w[p], mi = mid[p];
+      const double w_gt = w_tot - w_lt - wi, m_gt = m_tot - m_lt - wi * mi;
+      const double s_i = mi * (w_lt - w_gt) - (m_lt - m_gt);
+      const double len = (double)tt[p + 1] - (double)tt[p];
+      dist_val += len * wi * wi / 3.0 + wi * s_i;
+      const float gdist = dist_mult * (float)((2.0 / 3.0) * len * wi + 2.0 * s_i);
+      gw[p] = g[0] * rgb[p][0] + g[1] * rgb[p][1] + g[2] * rgb[p][2] - gsum_bg + gdist;
+      w_lt += wi;
+      m_lt += wi * mi;
+    }
+  } else {
+    float tmid[P], dsum = 0.f;
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      tmid[p] = 0.5f * (tt[p] + tt[p + 1]);
+      dsum += w[p] * tmid[p];
+    }
+    dsum = warp_sum(dsum);
+    const float t_last = __shfl_sync(0xffffffffu, tt[P], 31);
+    const float g_d = (cot.d_distance && isfinite(dsum) && dsum >= t_first && dsum <= t_last)
+                          ? __ldg(cot.d_distance + ray) : 0.f;
+    const float g_acc = cot.d_acc ? __ldg(cot.d_acc + ray) : 0.f;
+#pragma unroll
+    for (int p = 0; p < P; ++p) {
+      const float dw = cot.d_weights ? __ldg(cot.d_weights + ray * N + lane * P + p) : 0.f;
+      gw[p] = dw + (g[0] * rgb[p][0] + g[1] * rgb[p][1] + g[2] * rgb[p][2]) - gsum_bg + g_acc + g_d * tmid[p];
+    }
+  }
+  double gww_run = 0.0, gww_incl[P];
 #pragma unroll
   for (int p = 0; p < P; ++p) {
-    const double wi = w[p], mi = mid[p];
-    const double w_gt = w_tot - w_lt - wi, m_gt = m_tot - m_lt - wi * mi;
-    const double s_i = mi * (w_lt - w_gt) - (m_lt - m_gt);
-    const double len = (double)tt[p + 1] - (double)tt[p];
-    dist_val += len * wi * wi / 3.0 + wi * s_i;
-    const float gdist = dist_mult * (float)((2.0 / 3.0) * len * wi + 2.0 * s_i);
-    gw[p] = g[0] * rgb[p][0] + g[1] * rgb[p][1] + g[2] * rgb[p][2] - gsum_bg + gdist;
-    gww_run += (double)gw[p] * wi;
+    gww_run += (double)gw[p] * (double)w[p];
     gww_incl[p] = gww_run;
-    w_lt += wi;
-    m_lt += wi * mi;
   }
   double gww_tot;
   const double gww_before = warp_excl_scan_f64(gww_run, lane, gww_tot);
@@ -145,28 +179,32 @@ __global__ void render_backward_kernel(const float* __restrict__ raw_rgb, const 
     for (int c = 0; c < 3; ++c)
       d_raw_rgb[s * 3 + c] = g[c] * w[p] * rgb_scale * srgb[p][c] * (1.0f - srgb[p][c]);
   }
+  if constexpr (!kCot) {
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) dist_val += __shfl_xor_sync(0xffffffffu, dist_val, o);
-  if (lane == 0) {
-    if (sqerr_out) sqerr_out[ray] = mask * sq;
-    if (dist_out) dist_out[ray] = (float)dist_val;
+    for (int o = 16; o > 0; o >>= 1) dist_val += __shfl_xor_sync(0xffffffffu, dist_val, o);
+    if (lane == 0) {
+      if (sqerr_out) sqerr_out[ray] = mask * sq;
+      if (dist_out) dist_out[ray] = (float)dist_val;
+    }
   }
 }
 
-cudaError_t launch_render_backward(const float* raw_rgb, const float* raw_dens, const float* t, const float* dirs,
-                                   const float* target, const float* lossmult, const float* mask_sum,
-                                   float mse_mult, float dist_mult, int white_bkgd, float density_bias,
-                                   float rgb_scale, float rgb_padding, float* d_raw_rgb, float* d_raw_dens,
-                                   float* sqerr_out, float* dist_out, int64_t num_rays, int n, cudaStream_t st) {
+template <bool kCot>
+static cudaError_t launch_render_grad(const float* raw_rgb, const float* raw_dens, const float* t, const float* dirs,
+                                      const float* target, const float* lossmult, const float* mask_sum,
+                                      float mse_mult, float dist_mult, int white_bkgd, float density_bias,
+                                      float rgb_scale, float rgb_padding, float* d_raw_rgb, float* d_raw_dens,
+                                      float* sqerr_out, float* dist_out, const RenderCot& cot, int64_t num_rays, int n,
+                                      cudaStream_t st) {
   if (num_rays == 0) return cudaSuccess;
   LaunchScope scope(kKernRenderBackward, st);
   const unsigned grid = blocks_of(num_rays, 4);
 #define MIPNERF_RB_CASE(PP)                                                                                    \
   case PP:                                                                                                     \
-    render_backward_kernel<PP><<<grid, 128, 0, st>>>(raw_rgb, raw_dens, t, dirs, target, lossmult, mask_sum,   \
-                                                     mse_mult, dist_mult, white_bkgd, density_bias, rgb_scale, \
-                                                     rgb_padding, d_raw_rgb, d_raw_dens, sqerr_out, dist_out,  \
-                                                     num_rays);                                                \
+    render_backward_kernel<PP, kCot><<<grid, 128, 0, st>>>(raw_rgb, raw_dens, t, dirs, target, lossmult,       \
+                                                           mask_sum, mse_mult, dist_mult, white_bkgd,          \
+                                                           density_bias, rgb_scale, rgb_padding, d_raw_rgb,    \
+                                                           d_raw_dens, sqerr_out, dist_out, num_rays, cot);    \
     break;
   switch (n / 32) {
     MIPNERF_RB_CASE(1)
@@ -180,6 +218,25 @@ cudaError_t launch_render_backward(const float* raw_rgb, const float* raw_dens, 
   }
 #undef MIPNERF_RB_CASE
   return cudaGetLastError();
+}
+
+cudaError_t launch_render_backward(const float* raw_rgb, const float* raw_dens, const float* t, const float* dirs,
+                                   const float* target, const float* lossmult, const float* mask_sum,
+                                   float mse_mult, float dist_mult, int white_bkgd, float density_bias,
+                                   float rgb_scale, float rgb_padding, float* d_raw_rgb, float* d_raw_dens,
+                                   float* sqerr_out, float* dist_out, int64_t num_rays, int n, cudaStream_t st) {
+  return launch_render_grad<false>(raw_rgb, raw_dens, t, dirs, target, lossmult, mask_sum, mse_mult, dist_mult,
+                                   white_bkgd, density_bias, rgb_scale, rgb_padding, d_raw_rgb, d_raw_dens, sqerr_out,
+                                   dist_out, RenderCot{}, num_rays, n, st);
+}
+
+cudaError_t launch_render_vjp(const float* raw_rgb, const float* raw_dens, const float* t, const float* dirs,
+                              const RenderCot& cot, int white_bkgd, float density_bias, float rgb_scale,
+                              float rgb_padding, float* d_raw_rgb, float* d_raw_dens, int64_t num_rays, int n,
+                              cudaStream_t st) {
+  return launch_render_grad<true>(raw_rgb, raw_dens, t, dirs, nullptr, nullptr, nullptr, 0.f, 0.f, white_bkgd,
+                                  density_bias, rgb_scale, rgb_padding, d_raw_rgb, d_raw_dens, nullptr, nullptr, cot,
+                                  num_rays, n, st);
 }
 
 // -------------------------------------------------------------------------------------------------

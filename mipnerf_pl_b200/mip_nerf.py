@@ -4,9 +4,18 @@ the sm_90a kernels of libmipnerf_b200.so through the C ABI.
 
 The modules own ordinary fp32 `torch.nn.Linear` parameters, so Lightning
 checkpoints of the reference (`mip_nerf.mlp.layers.{i}.0.weight`, ...) load with
-`load_state_dict` unchanged.  `forward` builds no autograd graph; training goes
-through `mipnerf_pl_b200.train` (`fused_loss` / `forward_backward`), where one library call runs forward and
-backward and hands the gradients to autograd or `param.grad`.
+`load_state_dict` unchanged.
+
+Training, two ways:
+  * `mipnerf_pl_b200.train` (`fused_loss` / `forward_backward`): one library call runs forward and backward of the
+    reference's loss (masked MSE per level + 0.01 distloss, coarse multiplier) and hands the gradients to autograd
+    or `param.grad`.  The fastest step, but the loss is fixed.
+  * `MipNerf(autograd=True)`: `forward` returns outputs with a `grad_fn` over the 24 MLP tensors (when grad mode is
+    on and a parameter requires grad), so any loss on comp_rgb / distance / acc / weights trains through
+    `loss.backward()`.  Only the rays, the fenceposts and the density noise are kept between the two passes
+    (O(B*N) floats, no activations); the backward re-runs the training forward at those fenceposts chunk by chunk
+    and then the library's backward chain (`mipnerf_b200_backward`).  fp32 and bf16; t_samples carry no gradient
+    (stop_resample_grad=True).
 """
 from __future__ import annotations
 
@@ -15,6 +24,7 @@ import os
 from typing import List, Optional
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _cabi
 from .ops import _dev, _f32, _ptr, _stream, draw_density_normal, draw_t_rand, draw_u_jitter
@@ -198,7 +208,7 @@ class MipNerf(torch.nn.Module):
                  disable_integration: bool = False, append_identity: bool = True, mlp_net_depth: int = 8,
                  mlp_net_width: int = 256, mlp_net_depth_condition: int = 1, mlp_net_width_condition: int = 128,
                  mlp_skip_index: int = 4, mlp_num_rgb_channels: int = 3, mlp_num_density_channels: int = 1,
-                 mlp_net_activation: str = 'relu', precision: Optional[str] = None):
+                 mlp_net_activation: str = 'relu', precision: Optional[str] = None, autograd: bool = False):
         super().__init__()
         self.num_levels = num_levels
         self.num_samples = num_samples
@@ -233,6 +243,9 @@ class MipNerf(torch.nn.Module):
         # seed from torch's global generator at first use, offset advanced by one per call.
         self.rng_seed: Optional[int] = None
         self.rng_offset = 0
+        # forward builds an autograd graph (grad mode on, some MLP parameter requires grad): any loss on the outputs
+        # can call backward(); the gradients come from mipnerf_b200_backward
+        self.autograd = bool(autograd)
 
     def next_rng(self) -> "_cabi.Rng":
         """(seed, offset) of the next randomized call; advances the offset (the role of torch's generator offset)."""
@@ -255,7 +268,20 @@ class MipNerf(torch.nn.Module):
         """rays -> [(comp_rgb [B,3], distance [B], acc [B], weights [B,N], t_samples [B,N+1])] * levels
         (models/mip_nerf.py:172-248).  `t_rand` / `u_jitter` / `density_normal` (one [B,N] tensor of standard normals
         per level, models/mip_nerf.py:233) inject the noise of randomized mode; without any of them the kernels draw
-        in-kernel.  With `return_inds` a sixth element (searchsorted indices, None for level 0) is appended."""
+        in-kernel.  With `return_inds` a sixth element (searchsorted indices, None for level 0) is appended.
+
+        With `autograd=True`, grad mode on and a parameter that requires grad, comp_rgb / distance / acc / weights of
+        every level carry a `grad_fn` over the MLP tensors (values identical: the same launches run); t_samples and
+        inds are constants (stop_resample_grad) and `.pixels` has no grad.  fp32 and bf16 only; ray tensors that
+        require grad are refused."""
+        if self.autograd and torch.is_grad_enabled() and any(p.requires_grad for p in self.mlp.parameters()):
+            return _forward_with_grad(self, rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds)
+        return self._forward(rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds)[0]
+
+    def _forward(self, rays: Rays, randomized: bool, white_bkgd: bool, t_rand, u_jitter, density_normal,
+                 return_inds: bool):
+        """The launches of `forward` -> (LevelOutputs, config, rng or None, per-level density normals or None,
+        the fp32 ray tensors handed to the library)."""
         if self.ray_shape == 'cylinder':
             raise NotImplementedError  # models/mip.py:97-98
         assert self.ray_shape == 'cone'
@@ -328,4 +354,122 @@ class MipNerf(torch.nn.Module):
         else:
             with torch.cuda.device(dev):
                 _cabi.check(fn(*args), "MipNerf.forward")
-        return ret
+        return ret, cfg, rng, normals, keep
+
+
+def _check_autograd(model: MipNerf, rays: Rays, b: int) -> None:
+    """Refuse, at forward time, what the backward pass cannot differentiate."""
+    if model.precision in ("fp16x3", "bf16x3"):
+        raise NotImplementedError(f"MipNerf(autograd=True): precision={model.precision!r} is forward-only; "
+                                  "use 'fp32' or 'bf16'")
+    if model.precision == "fp16":
+        raise NotImplementedError("MipNerf(autograd=True): fp16's fixed gradient scale is sized for the reference loss "
+                                  "and arbitrary losses can overflow or underflow it; use precision='bf16'")
+    if model.precision not in ("fp32", "bf16"):
+        raise ValueError(f"precision={model.precision!r}")
+    if not model.stop_resample_grad:
+        raise NotImplementedError("MipNerf(autograd=True): gradients through the resampled fenceposts "
+                                  "(stop_resample_grad=False) are not implemented")
+    if any(isinstance(x, torch.Tensor) and x.requires_grad for x in rays):
+        raise NotImplementedError("MipNerf(autograd=True): gradients with respect to the rays are not implemented; "
+                                  "pass ray tensors that do not require grad")
+    cfg = model._config()
+    if _cabi.lib().mipnerf_b200_train_workspace_bytes(C.byref(cfg), max(b, 1)) == 0:
+        raise NotImplementedError(f"MipNerf(autograd=True): {_cabi.last_error() or 'no training kernels'}; the "
+                                  "backward pass needs use_viewdirs=True with one view layer and net_depth <= 16")
+    if model.precision == "bf16":
+        m = model.mlp
+        # the 16-bit training GEMMs exist for the default widths and encodings only (api.cu train_tc_supported)
+        if not (m.net_width == 256 and m.net_width_condition == 128 and m.xyz_dim == 96 and m.view_dim == 27):
+            raise NotImplementedError("MipNerf(autograd=True, precision='bf16'): the tensor-core backward supports the "
+                                      "8x256 / 1x128 MLP with max_deg_point=16, deg_view=4; use precision='fp32'")
+
+
+def _forward_with_grad(model: MipNerf, rays: Rays, randomized, white_bkgd, t_rand, u_jitter, density_normal,
+                       return_inds):
+    _dev(rays.origins)
+    _check_autograd(model, rays, rays.origins.shape[0])
+    holder = {}
+    params = [p for lin in model.mlp.linears() for p in (lin.weight, lin.bias)]
+    flat = _ForwardWithGrad.apply(model, rays, randomized, white_bkgd, t_rand, u_jitter, density_normal,
+                                  return_inds, holder, *params)
+    per = 6 if return_inds else 5
+    ret = LevelOutputs(tuple(flat[i:i + per]) for i in range(0, len(flat), per))
+    ret.pixels = holder["pixels"]
+    return ret
+
+
+class _ForwardWithGrad(torch.autograd.Function):
+    """MipNerf.forward as a function of the 24 MLP tensors.  Saved: the rays, each level's fenceposts, the density
+    noise (Philox seed / offset or the normals) and the parameters; backward re-evaluates the MLP at those fenceposts
+    and runs the library's backward chain from the output cotangents."""
+
+    @staticmethod
+    def forward(ctx, model, rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds, holder,
+                *params):
+        ret, cfg, rng, normals, keep = model._forward(rays, randomized, white_bkgd, t_rand, u_jitter, density_normal,
+                                                      return_inds)
+        holder["pixels"] = ret.pixels
+        levels = len(ret)
+        ts = [lvl[4] for lvl in ret]
+        given = [x for x in normals if x is not None]
+        ctx.model, ctx.cfg, ctx.white_bkgd = model, cfg, bool(white_bkgd)
+        ctx.randomized, ctx.precision, ctx.levels, ctx.per = bool(randomized), model.precision, levels, len(ret[0])
+        ctx.rng = None if rng is None else (rng.seed, rng.offset)
+        ctx.normal_levels = [i for i, x in enumerate(normals) if x is not None]
+        ctx.num_params = len(params)
+        ctx.save_for_backward(*params, *keep, *ts, *given)
+        ctx.set_materialize_grads(False)
+        outs = [x for lvl in ret for x in lvl]
+        ctx.mark_non_differentiable(*[x for lvl in ret for x in lvl[4:] if x is not None])
+        return tuple(outs)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *grads):
+        saved = ctx.saved_tensors  # raises if a parameter was updated in place since the forward
+        np_, levels, per = ctx.num_params, ctx.levels, ctx.per
+        params = saved[:np_]
+        keep = saved[np_:np_ + 6]
+        ts = saved[np_ + 6:np_ + 6 + levels]
+        given = saved[np_ + 6 + levels:]
+        model, cfg = ctx.model, ctx.cfg
+        dev = keep[0].device
+        b = keep[0].shape[0]
+        out_grads = [torch.empty_like(p) for p in params]
+        if all(g is None for g in grads) or b == 0:
+            return (None,) * 9 + tuple(g.zero_() for g in out_grads)
+        rs = _cabi.RaysStruct(*[k.data_ptr() for k in keep], b)
+        cots = (_cabi.LevelCotangent * levels)()
+        cot_keep = []
+        for lvl in range(levels):
+            ptrs = []
+            for g in grads[lvl * per:lvl * per + 4]:
+                if g is None:
+                    ptrs.append(None)
+                else:
+                    g = _f32(g)
+                    cot_keep.append(g)
+                    ptrs.append(g.data_ptr())
+            cots[lvl] = _cabi.LevelCotangent(*ptrs)
+        t_arr = (C.c_void_p * levels)(*[t.data_ptr() for t in ts])
+        normal_arr = None
+        if ctx.normal_levels:
+            normal_arr = (C.c_void_p * levels)()
+            for i, x in zip(ctx.normal_levels, given):
+                normal_arr[i] = x.data_ptr()
+        rng = _cabi.Rng(*ctx.rng) if ctx.rng is not None else None
+        ws, wkeep = model.mlp._weights_struct(cfg, _cabi.FP32, dev)
+        garr = (_cabi.LinearGrad * (np_ // 2))()
+        for i in range(np_ // 2):
+            garr[i] = _cabi.LinearGrad(out_grads[2 * i].data_ptr(), out_grads[2 * i + 1].data_ptr())
+        lib = _cabi.lib()
+        nbytes = lib.mipnerf_b200_train_workspace_bytes(C.byref(cfg), b)
+        scratch = _Workspace.get(dev, nbytes)
+        with torch.cuda.device(dev):
+            _cabi.check(lib.mipnerf_b200_backward(
+                C.byref(cfg), C.byref(ws), C.byref(rs), t_arr, int(ctx.randomized),
+                C.byref(rng) if rng is not None else None, normal_arr, int(ctx.white_bkgd),
+                _cabi.PRECISIONS[ctx.precision], cots, garr, np_ // 2, 0, scratch.data_ptr(), scratch.numel(),
+                _stream(dev)), "MipNerf.backward")
+        return (None,) * 9 + tuple(out_grads)

@@ -16,6 +16,7 @@ import ctypes as C
 from typing import Optional
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _cabi
 
@@ -228,15 +229,45 @@ def volumetric_rendering(rgb, density, t_samples, dirs, white_bkgd):
     return comp, dist, acc, w
 
 
-def distloss(weight, samples):
-    """Distortion loss value (models/mip.py:8-20): weight [B,N], samples [B,N+1] -> scalar.
-    Value only (its gradient is part of `train.forward_backward`); O(N) per ray instead of the
-    reference's two [B,N,N] temporaries."""
-    dev = _dev(weight)
-    w, t = _f32(weight), _f32(samples)
+def _distloss_value(w: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
+    dev = _dev(w)
     b, n = w.shape
     out = torch.empty(b, device=dev)
     with torch.cuda.device(dev):
         _cabi.check(_cabi.lib().mipnerf_b200_distloss(w.data_ptr(), t.data_ptr(), b, n, out.data_ptr(), _stream(dev)),
                     "distloss")
     return out.mean()
+
+
+class _DistLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, weight, samples):
+        w, t = _f32(weight), _f32(samples)
+        ctx.save_for_backward(w, t)
+        ctx.weight_dtype = weight.dtype
+        return _distloss_value(w, t)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        w, t = ctx.saved_tensors
+        b, n = w.shape
+        dev = w.device
+        d_w = torch.empty_like(w)
+        g = _f32(grad_out).reshape(1)
+        with torch.cuda.device(dev):
+            _cabi.check(_cabi.lib().mipnerf_b200_distloss_backward(w.data_ptr(), t.data_ptr(), b, n, g.data_ptr(),
+                                                                    1.0 / max(b, 1), d_w.data_ptr(), _stream(dev)),
+                        "distloss_backward")
+        return d_w.to(ctx.weight_dtype), None
+
+
+def distloss(weight, samples):
+    """Distortion loss (models/mip.py:8-20): weight [B,N], samples [B,N+1] -> scalar; O(N) per ray instead of the
+    reference's two [B,N,N] temporaries.  Differentiable with respect to `weight` when it requires grad (the
+    gradient is the same prefix-sum form, `mipnerf_b200_distloss_backward`); `samples` is a constant, as under
+    stop_resample_grad.  Inside `train.forward_backward` the gradient is part of the fused step."""
+    _dev(weight)
+    if torch.is_grad_enabled() and weight.requires_grad:
+        return _DistLoss.apply(weight, samples)
+    return _distloss_value(_f32(weight), _f32(samples))

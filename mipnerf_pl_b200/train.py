@@ -13,6 +13,9 @@ the tensor cores (wgmma) with 16-bit operands and fp32 accumulation, wgrad / hea
 
 Gradients do not flow into the fenceposts (stop_resample_grad=True, the reference default); a model built
 with stop_resample_grad=False is refused rather than silently trained with different gradients.
+
+Both functions differentiate the reference loss only.  For any other loss on the rendered outputs, build the model
+with `MipNerf(autograd=True)` and call `loss.backward()` (mip_nerf.py).
 """
 from __future__ import annotations
 

@@ -2,10 +2,18 @@
 BASELINE configs[1] shape, with the per-kernel breakdown from the library's launch accounting.
 
     python tools/train_bench.py [--rays 4096] [--steps 5]
+    python tools/train_bench.py --autograd [--rounds 5]
+
+--autograd times MipNerf(autograd=True): forward -> the reference loss written in torch (masked MSE per level +
+0.01 distloss, coarse multiplier 0.1) -> loss.backward() -> FusedAdam, alternating it with the fused step
+(`forward_backward` + FusedAdam) on the same rays in the same process, fp32 and bf16, and prints one JSON line per
+precision with the median ms of each and the card's name and power limit.
 """
 import argparse
 import json
 import os
+import statistics
+import subprocess
 import sys
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
@@ -23,7 +31,11 @@ def main():
     ap.add_argument("--rays", type=int, default=4096)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--precision", default="fp32", choices=["fp32", "bf16", "fp16"])
+    ap.add_argument("--autograd", action="store_true", help="time the autograd step against the fused step")
+    ap.add_argument("--rounds", type=int, default=5, help="--autograd: alternations of the two steps")
     args = ap.parse_args()
+    if args.autograd:
+        return autograd_vs_fused(args)
     dev = torch.device("cuda", 0)
     model = mp.MipNerf(precision=args.precision)
     model.load_state_dict(mp.make_state_dict(seed=0, kind="xavier"))
@@ -64,6 +76,74 @@ def main():
                       "approx_tflops": flops / (ms * 1e-3) / 1e12, "loss": float(out["loss"]),
                       "kernel_ms_per_step": {k: round(v[1] / args.steps, 3) for k, v in prof.items() if v[2]},
                       "launches_per_step": {k: v[0] / args.steps for k, v in prof.items() if v[0]}}))
+
+
+def _card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        return q[0] if q else torch.cuda.get_device_name(0)
+    except (OSError, subprocess.SubprocessError):
+        return torch.cuda.get_device_name(0)
+
+
+def reference_loss(ret, rays, rgbs):
+    """models/nerf_system.py:95-111 as the reference writes it."""
+    mask = rays.lossmult
+    losses, dls = [], []
+    for (rgb, _, _, weights, t_samples) in ret:
+        losses.append((mask * (rgb - rgbs[..., :3]) ** 2).sum() / mask.sum())
+        dls.append(mp.distloss(weights, t_samples))
+    return 0.1 * (losses[0] + 0.01 * dls[0]) + losses[-1] + 0.01 * dls[-1]
+
+
+def autograd_vs_fused(args):
+    dev = torch.device("cuda", 0)
+    card = _card()
+    rays = mp.namedtuple_map(lambda t: t.to(dev), mp.random_ray_batch(args.rays, seed=0, multiscale=True))
+    rgbs = torch.rand(args.rays, 3, device=dev)
+    for precision in ("fp32", "bf16"):
+        models = {}
+        for kind in ("fused", "autograd"):
+            m = mp.MipNerf(precision=precision, autograd=kind == "autograd")
+            m.load_state_dict(mp.make_state_dict(seed=0, kind="xavier"))
+            m = m.to(dev)
+            models[kind] = (m, mp.FusedAdam(m.parameters(), lr=5e-4))
+
+        def fused():
+            m, opt = models["fused"]
+            mp.forward_backward(m, rays, rgbs, True, True)
+            opt.step()
+
+        def autograd():
+            m, opt = models["autograd"]
+            opt.zero_grad()
+            reference_loss(m(rays, True, True), rays, rgbs).backward()
+            opt.step()
+
+        steps = {"fused": fused, "autograd": autograd}
+        for fn in steps.values():                # warm-up: modules loaded, workspaces and caches allocated
+            for _ in range(2):
+                fn()
+        torch.cuda.synchronize()
+        times = {k: [] for k in steps}
+        for _ in range(args.rounds):             # alternate the two so that drift of the shared host hits both
+            for k, fn in steps.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(args.steps):
+                    fn()
+                e1.record()
+                torch.cuda.synchronize()
+                times[k].append(e0.elapsed_time(e1) / args.steps)
+        print(json.dumps({"what": f"{precision} training step, {args.rays} rays, randomized, 128+128 samples: "
+                                  "forward_backward + FusedAdam vs MipNerf(autograd=True) forward -> reference loss "
+                                  "in torch -> backward -> FusedAdam",
+                          "card": card, "rays": args.rays, "steps_per_round": args.steps, "rounds": args.rounds,
+                          "fused_ms_median": statistics.median(times["fused"]),
+                          "autograd_ms_median": statistics.median(times["autograd"]),
+                          "fused_ms": [round(x, 3) for x in times["fused"]],
+                          "autograd_ms": [round(x, 3) for x in times["autograd"]]}), flush=True)
 
 
 if __name__ == "__main__":
