@@ -132,7 +132,8 @@ enum LevelPhase : int {
   kPhIpe,        // Gaussians + IPE features
   kPhWFull,      // consumers: waiting for a weight stage (w_full)
   kPhMma,        // consumers: wgmma issue and retire
-  kPhEpilogue,   // layer epilogues, view layer + colour head, head reductions, activation-dump issue
+  kPhEpilogue,   // layer epilogue chunks (their K-slab's wgmmas run meanwhile), view layer + colour head, head
+                 // reductions, activation-dump issue
   kPhComposite,  // warpgroup 0: activations + compositing (or the raw heads of MLP-only mode)
   kPhBarrier,    // consumers: named-barrier waits
   kPhWEmpty,     // producer: waiting for a free ring slot (w_empty)
@@ -251,8 +252,9 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
 //   * warps 0-3 / 4-7: two consumer warpgroups, warpgroup g owns sample rows 64 g .. 64 g + 63 of the ray.  Each
 //     computes the IPE features of its rows, issues the wgmma (M = 64, N = 128, K = 16) of every layer for its rows
 //     (A operand: its rows of the activation / feature tile in shared memory; B: the weight stage both warpgroups
-//     share), and runs the epilogue from the register accumulators straight into the next layer's A operand, in place.
-//     The rows of a warpgroup are private to it, so a layer boundary is a 128-thread barrier, not a CTA barrier.
+//     share), and runs the epilogue from the register accumulators straight into the next layer's A operand, in place,
+//     in chunks under the wgmmas of later K-slabs (software-pipelined layer loop).  The rows of a warpgroup are private
+//     to it, so a layer boundary is a 128-thread barrier, not a CTA barrier.
 //   * warps 8-11: producer warpgroup (setmaxnreg gives its registers to the consumers); warp 8 is the weight producer
 //     — cp.async.bulk of the pre-swizzled [128 x 32] (SW64, 8 KB) stages of the packed image
 //     (+ the low-half stage in the split modes) into a ring; a stage is free once both warpgroups' wgmmas reading it
@@ -295,69 +297,101 @@ __device__ __forceinline__ uint64_t level_a_desc(int l, int s, int j, uint32_t a
   return make_sw64_desc(ft_u + 32u * j);
 }
 
-// One N = 128 half of layer l for the rows of one warpgroup: nk K-slabs through the weight ring.  A stage is released
-// (one arrive per warpgroup) as soon as the wgmmas that read it have completed; one stage's wgmmas stay in flight.
+// Where a consumer warpgroup stands in the weight ring: the slot and phase of its next stage, and the slot of its newest
+// wgmma group (-1: none in flight).
+struct RingPos {
+  int st;
+  uint32_t ph;
+  int prev;
+};
+
+// K-slab s (32 wide) of one N = 128 half of layer l into acc, for the rows of one warpgroup: wait for the weight stage,
+// issue its wgmmas as one group, then wait until only that group is in flight.  The wait retires the previous group,
+// whose stage is released (one arrive per warpgroup); so one stage's wgmmas stay in flight across calls, also from one
+// half or layer to the next.
 template <int kFmt, bool kX3>
-__device__ __forceinline__ void level_mma_half(float (&acc)[64], int l, int nk, uint32_t a_u, uint32_t f_u,
+__device__ __forceinline__ void level_mma_slab(float (&acc)[64], int l, int s, uint32_t a_u, uint32_t f_u,
                                                uint32_t ft_u, uint32_t w_u, uint64_t* w_full, uint64_t* w_empty,
-                                               int& st, uint32_t& ph, bool leader, PhaseClock& clk) {
+                                               RingPos& rp, bool leader, PhaseClock& clk) {
   using Lay = LevelLayout<kX3>;
-  int prev = -1;
-  wgmma_fence_acc(acc);
-  for (int s = 0; s < nk; ++s) {
-    clk.mark(kPhMma);
-    mbar_wait(&w_full[st], ph);
-    clk.mark(kPhWFull);
-    wgmma_fence();
-    const uint32_t b_u = w_u + (uint32_t)st * Lay::kStage;
+  mbar_wait(&w_full[rp.st], rp.ph);
+  clk.mark(kPhWFull);
+  wgmma_fence();
+  const uint32_t b_u = w_u + (uint32_t)rp.st * Lay::kStage;
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const uint64_t a_hi = level_a_desc(l, s, j, a_u, f_u, ft_u);
-      const uint64_t b_hi = make_sw64_desc(b_u + 32u * j);
-      wgmma_m64n128k16<kFmt>(acc, a_hi, b_hi, (s | j) ? 1u : 0u);
-      if (kX3) {  // A_lo . W_hi + A_hi . W_lo (the lo tiles sit one tile size behind the hi tiles)
-        wgmma_m64n128k16<kFmt>(acc, a_hi + ((l == 0 || (l == 5 && s >= 8)) ? kFBytes : kABytes) / 16, b_hi, 1u);
-        wgmma_m64n128k16<kFmt>(acc, a_hi, b_hi + kWStage / 16, 1u);
-      }
-    }
-    wgmma_commit();
-    wgmma_wait<1>();
-    if (prev >= 0 && leader) mbar_arrive(&w_empty[prev]);
-    prev = st;
-    if (++st == Lay::kStages) {
-      st = 0;
-      ph ^= 1;
+  for (int j = 0; j < 2; ++j) {
+    const uint64_t a_hi = level_a_desc(l, s, j, a_u, f_u, ft_u);
+    const uint64_t b_hi = make_sw64_desc(b_u + 32u * j);
+    wgmma_m64n128k16<kFmt>(acc, a_hi, b_hi, (s | j) ? 1u : 0u);
+    if (kX3) {  // A_lo . W_hi + A_hi . W_lo (the lo tiles sit one tile size behind the hi tiles)
+      wgmma_m64n128k16<kFmt>(acc, a_hi + ((l == 0 || (l == 5 && s >= 8)) ? kFBytes : kABytes) / 16, b_hi, 1u);
+      wgmma_m64n128k16<kFmt>(acc, a_hi, b_hi + kWStage / 16, 1u);
     }
   }
-  wgmma_wait<0>();
-  wgmma_fence_acc(acc);
-  if (leader) mbar_arrive(&w_empty[prev]);
+  wgmma_commit();
+  wgmma_wait<1>();
+  if (rp.prev >= 0 && leader) mbar_arrive(&w_empty[rp.prev]);
+  rp.prev = rp.st;
+  if (++rp.st == Lay::kStages) {
+    rp.st = 0;
+    rp.ph ^= 1;
+  }
   clk.mark(kPhMma);
 }
 
-// Epilogue of one N = 128 half (columns c_base..) of trunk layer / bottleneck l: + bias -> ReLU (l < 8) -> 16-bit ->
-// the A operand of the next layer (rows r0, r0 + 8 of the fragment); l == 7 also accumulates the density head on the
-// fp32 (un-rounded) h7 (models/mip_nerf.py:98).
-template <int kFmt, bool kX3>
-__device__ __forceinline__ void level_epilogue_half(const float (&acc)[64], int l, int c_base, int r0, int cq,
-                                                    uint8_t* sA, const SmallParams* __restrict__ gsp, float& d0,
-                                                    float& d1) {
-  const bool relu = l < 8;
+// The layer epilogues run in chunks under the wgmmas of K-slabs (see the layer loop of mlp_level_kernel): kEpiChunks
+// chunks per N = 128 half, each after the wait of one K-slab; chunk c covers the accumulator's column groups
+// 4 c .. 4 c + 3, i.e. columns c_base + 32 c .. + 31, which are exactly the A-operand columns that K-slab c
+// (c_base = 0) or 4 + c (c_base = 128) of the next layer reads.
+constexpr int kEpiChunks = 4;
+constexpr int kEpiGroups = 16 / kEpiChunks;
+// First K-slab of a trunk layer's N-half 1 that carries a chunk of N-half 0's epilogue (chunk c after K-slab
+// kEpiOverlap + c).  Any value in 1..4 is safe: chunk c overwrites the columns of K-slab c, retired by then.  Measured
+// on an H100 80GB HBM3 at 400 W (bench.py bf16 step, before the bias loads moved ahead of the K-slab): 4.13-4.15 ms
+// with 1, 4.22 / 4.35 / 4.48 ms with 2 / 3 / 4.
+constexpr int kEpiOverlap = 1;
+static_assert(kEpiOverlap >= 1 && kEpiOverlap + kEpiChunks <= 8, "chunk c must follow the retirement of K-slab c");
+
+// The bias of one epilogue chunk, loaded before the K-slab that the chunk follows, so that the load latency hides
+// under that slab's wgmmas.
+struct EpiConsts {
+  float2 b[kEpiGroups];
+};
+__device__ __forceinline__ void level_epilogue_consts(EpiConsts& e, int l, int c_base, int chunk, int cq,
+                                                      const SmallParams* __restrict__ gsp) {
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const int c = c_base + 8 * j + cq;
-    const float2 b = __ldg(reinterpret_cast<const float2*>(gsp->bias[l] + c));
+  for (int jj = 0; jj < kEpiGroups; ++jj)
+    e.b[jj] = __ldg(reinterpret_cast<const float2*>(gsp->bias[l] + c_base + 8 * (kEpiGroups * chunk + jj) + cq));
+}
+
+// Epilogue chunk `chunk` of one N = 128 half (columns c_base..) of trunk layer / bottleneck l: + bias -> ReLU (l < 8)
+// -> 16-bit -> the A operand of the next layer (rows r0, r0 + 8 of the fragment); l == 7 also accumulates the density
+// head on the fp32 (un-rounded) h7 (models/mip_nerf.py:98).  `chunk` must be a compile-time constant after unrolling,
+// so that the accumulator stays in registers.
+template <int kFmt, bool kX3>
+__device__ __forceinline__ void level_epilogue_chunk(const float (&acc)[64], const EpiConsts& e, int l, int c_base,
+                                                     int chunk, int r0, int cq, uint8_t* sA,
+                                                     const SmallParams* __restrict__ gsp, float& d0, float& d1) {
+  const bool relu = l < 8;
+  // sw128_offset(r0, c & 63) = row_off | ((j & 7) << 4 ^ sw): one LOP3 per store.  Opaque per chunk, so that the
+  // compiler recomputes the offsets instead of computing them once and keeping them in local memory across the layers.
+  uint32_t row_off = (uint32_t)r0 * 128u + 2u * (uint32_t)cq, sw = (uint32_t)(r0 & 7) << 4;
+  asm volatile("" : "+r"(row_off), "+r"(sw));
+#pragma unroll
+  for (int jj = 0; jj < kEpiGroups; ++jj) {
+    const int j = kEpiGroups * chunk + jj;
+    const float2 b = e.b[jj];
     float a0 = acc[4 * j], a1 = acc[4 * j + 1], a2 = acc[4 * j + 2], a3 = acc[4 * j + 3];
     fadd2(a0, a1, b.x, b.y);
     fadd2(a2, a3, b.x, b.y);
     if (l == 7) {
-      const float2 wd = __ldg(reinterpret_cast<const float2*>(gsp->w_density + c));
+      const float2 wd = __ldg(reinterpret_cast<const float2*>(gsp->w_density + c_base + 8 * j + cq));
       ffma2(d0, d1, fmaxf(a0, 0.f), fmaxf(a2, 0.f), wd.x, wd.x);
       ffma2(d0, d1, fmaxf(a1, 0.f), fmaxf(a3, 0.f), wd.y, wd.y);
     }
     if (relu) a0 = fmaxf(a0, 0.f), a1 = fmaxf(a1, 0.f), a2 = fmaxf(a2, 0.f), a3 = fmaxf(a3, 0.f);
-    const uint32_t o0 = (uint32_t)(c >> 6) * kStageBytes + sw128_offset(r0, c & 63);
-    const uint32_t o1 = (uint32_t)(c >> 6) * kStageBytes + sw128_offset(r0 + 8, c & 63);
+    const uint32_t o0 = (uint32_t)((c_base >> 6) + (j >> 3)) * kStageBytes + (row_off | ((uint32_t)(j & 7) << 4 ^ sw));
+    const uint32_t o1 = o0 + 8u * 128u;  // row r0 + 8: same swizzle phase
     const uint32_t h0 = pack2<kFmt>(a0, a1), h1 = pack2<kFmt>(a2, a3);
     *reinterpret_cast<uint32_t*>(sA + o0) = h0;
     *reinterpret_cast<uint32_t*>(sA + o1) = h1;
@@ -447,8 +481,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   const uint32_t w_u = smem_u32(sW);
   const uint64_t dump_policy = p.act_dump ? l2_policy_evict_first() : 0ull;  // the dump must not evict the weights
   bool dump_pending = false;
-  int st = 0, par = 0;
-  uint32_t ph = 0;
+  RingPos rp{0, 0u, -1};
+  int par = 0;
   clk.begin(phase_rows + wg * kNumPhases, leader);
   for (int64_t ray = blockIdx.x; ray < p.num_rays; ray += gridDim.x, par ^= 1) {
     if (p.t_mode != 0 || p.vb_mode != 0) {
@@ -515,59 +549,125 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
 
     float d0 = 0.f, d1 = 0.f;  // density head, rows r0 / r0 + 8 (partial over this thread's columns)
     float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-    for (int l = 0; l < kNumLayers; ++l) {
-      float acc0[64], acc1[64];
-      level_mma_half<kFmt, kX3>(acc0, l, num_k32(l), a_u, f_u, ft_u, w_u, w_full, w_empty, st, ph, leader, clk);
-      if (l < 9) {
-        level_mma_half<kFmt, kX3>(acc1, l, num_k32(l), a_u, f_u, ft_u, w_u, w_full, w_empty, st, ph, leader, clk);
-        if (dump_pending) {  // the previous layer's bulk store must have READ the tile before it is overwritten
-          if (leader) bulk_store_wait_read();
-          dump_pending = false;
-          clk.mark(kPhEpilogue);
-          named_bar_sync(1 + wg, 128);
-          clk.mark(kPhBarrier);
+    // ---- the layers, software-pipelined so that each epilogue runs under wgmmas instead of after them.  The epilogue
+    // of trunk layer / bottleneck l overwrites, in place, the activation columns that layer l read; wgmmas consume K in
+    // order, and K-slab s of layers 1..9 reads only columns 32 s .. 32 s + 31 (layer 5's slabs 8-10 and layer 0 read
+    // the feature tile).  Per layer l:
+    //   1. N-half 0 into acc0: K-slabs 0..3 were issued under the previous layer's acc1 epilogue (step 4); the rest here.
+    //   2. N-half 1 into acc1; after K-slab kEpiOverlap + c has been committed and waited for, chunk c of acc0's
+    //      epilogue (columns 32 c .. 32 c + 31).  That wait leaves only K-slab kEpiOverlap + c in flight: all of N-half
+    //      0 has retired (acc0 is final), and so has K-slab c of N-half 1, the last reader of those columns.  Layer 0
+    //      reads none of the columns it writes, so its chunks follow K-slabs 0, 1, 2, 2.
+    //   3. fence + barrier: columns 0..127 of layer l + 1's input are complete for this warpgroup's rows.
+    //   4. Layer l + 1's N-half 0, K-slabs 0..3 (columns 0..127 only); the chunks of acc1's epilogue (columns 128..255)
+    //      follow the waits of K-slabs 0, 1, 2, 2, and K-slab 3 runs under the barrier instead of a chunk.  The first
+    //      wait retires all of layer l.
+    //   5. fence + barrier: layer l + 1's input is complete (and goes out with bulk stores in the training forward).
+    // A chunk's bias loads are issued before the K-slab it follows.  The wgmmas into each accumulator, their operands and
+    // order, and the epilogue arithmetic are those of an unpipelined loop, so the results are the same bit for bit.
+    float acc0[64], acc1[64];
+    wgmma_fence_acc(acc0);
+#pragma unroll
+    for (int s = 0; s < num_k32(0); ++s)
+      level_mma_slab<kFmt, kX3>(acc0, 0, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+    for (int l = 0; l < 9; ++l) {
+      // 1. the rest of N-half 0
+      if (l > 0)
+        for (int s = kEpiChunks; s < num_k32(l); ++s)
+          level_mma_slab<kFmt, kX3>(acc0, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+      // 2. N-half 1, with acc0's epilogue under it
+      wgmma_fence_acc(acc1);
+      const int first = l == 0 ? 0 : kEpiOverlap;  // K-slab that carries chunk 0
+      for (int s = 0; s < first; ++s)
+        level_mma_slab<kFmt, kX3>(acc1, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+#pragma unroll
+      for (int c = 0; c < kEpiChunks; ++c) {
+        EpiConsts e;
+        level_epilogue_consts(e, l, 0, c, cq, gsp);
+        if (first + c < num_k32(l))
+          level_mma_slab<kFmt, kX3>(acc1, l, first + c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+        if (c == 0) {
+          wgmma_fence_acc(acc0);
+          if (dump_pending) {  // the previous tile's bulk stores must have READ it before it is overwritten
+            if (leader) bulk_store_wait_read();
+            dump_pending = false;
+            clk.mark(kPhEpilogue);
+            named_bar_sync(1 + wg, 128);
+            clk.mark(kPhBarrier);
+          }
         }
-        level_epilogue_half<kFmt, kX3>(acc0, l, 0, r0, cq, sA, gsp, d0, d1);
-        level_epilogue_half<kFmt, kX3>(acc1, l, 128, r0, cq, sA, gsp, d0, d1);
-        fence_proxy_async_smem();
+        level_epilogue_chunk<kFmt, kX3>(acc0, e, l, 0, c, r0, cq, sA, gsp, d0, d1);
         clk.mark(kPhEpilogue);
-        named_bar_sync(1 + wg, 128);
-        clk.mark(kPhBarrier);
-        if (p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core reads it
-          if (leader) {
+      }
+      for (int s = first + kEpiChunks; s < num_k32(l); ++s)
+        level_mma_slab<kFmt, kX3>(acc1, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+      // 3.
+      fence_proxy_async_smem();
+      clk.mark(kPhEpilogue);
+      named_bar_sync(1 + wg, 128);
+      clk.mark(kPhBarrier);
+      // 4. the next layer's N-half 0, K-slabs 0..3, with acc1's epilogue under the first three
+      wgmma_fence_acc(acc0);
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint32_t o = (uint32_t)k * kStageBytes + (uint32_t)wg * 8192u;
-              bulk_s2g_hint(p.act_dump + ((size_t)l * p.dump_tiles + ray) * kABytes + o, sA + o, 8192u, dump_policy);
-            }
-          }
-          dump_pending = true;
-          clk.mark(kPhEpilogue);
+      for (int c = 0; c < kEpiChunks; ++c) {
+        EpiConsts e;
+        level_epilogue_consts(e, l, 128, c, cq, gsp);
+        if (c < kEpiChunks - 1) {
+          level_mma_slab<kFmt, kX3>(acc0, l + 1, c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+          if (c == 0) wgmma_fence_acc(acc1);
         }
-      } else {
-        // view layer + colour head (models/mip_nerf.py:106-110); view_bias = the per-ray view-direction term
-        const float* vb = p.view_bias + ray * kCond;
-        uint8_t* vd = p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
+        level_epilogue_chunk<kFmt, kX3>(acc1, e, l, 128, c, r0, cq, sA, gsp, d0, d1);
+        clk.mark(kPhEpilogue);
+      }
+      level_mma_slab<kFmt, kX3>(acc0, l + 1, kEpiChunks - 1, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+      // 5.
+      fence_proxy_async_smem();
+      clk.mark(kPhEpilogue);
+      named_bar_sync(1 + wg, 128);
+      clk.mark(kPhBarrier);
+      if (p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core reads it
+        if (leader) {
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int c = 8 * j + cq;
-          const float2 b = __ldcg(reinterpret_cast<const float2*>(vb + c));
-          float y[4] = {acc0[4 * j], acc0[4 * j + 1], acc0[4 * j + 2], acc0[4 * j + 3]};
-          fadd2(y[0], y[1], b.x, b.y);
-          fadd2(y[2], y[3], b.x, b.y);
-#pragma unroll
-          for (int e = 0; e < 4; ++e) y[e] = fmaxf(y[e], 0.f);
-#pragma unroll
-          for (int ch = 0; ch < 3; ++ch) {
-            const float2 wc = __ldg(reinterpret_cast<const float2*>(gsp->w_color[ch] + c));
-            ffma2(rgb[0][ch], rgb[1][ch], y[0], y[2], wc.x, wc.x);
-            ffma2(rgb[0][ch], rgb[1][ch], y[1], y[3], wc.y, wc.y);
+          for (int k = 0; k < 4; ++k) {
+            const uint32_t o = (uint32_t)k * kStageBytes + (uint32_t)wg * 8192u;
+            bulk_s2g_hint(p.act_dump + ((size_t)l * p.dump_tiles + ray) * kABytes + o, sA + o, 8192u, dump_policy);
           }
-          if (vd) {  // training: the 16-bit view-layer output, same tile layout as the trunk's activation slabs
-            *reinterpret_cast<uint32_t*>(vd + (c >> 6) * kStageBytes + sw128_offset(r0, c & 63)) = pack2<kFmt>(y[0], y[1]);
-            *reinterpret_cast<uint32_t*>(vd + (c >> 6) * kStageBytes + sw128_offset(r0 + 8, c & 63)) =
-                pack2<kFmt>(y[2], y[3]);
-          }
+        }
+        dump_pending = true;
+        clk.mark(kPhEpilogue);
+      }
+    }
+    // the rest of the view layer's one N-half, then its epilogue from the registers
+    for (int s = kEpiChunks; s < num_k32(9); ++s)
+      level_mma_slab<kFmt, kX3>(acc0, 9, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc0);
+    if (leader) mbar_arrive(&w_empty[rp.prev]);
+    rp.prev = -1;
+    clk.mark(kPhMma);
+    {
+      // view layer + colour head (models/mip_nerf.py:106-110); view_bias = the per-ray view-direction term
+      const float* vb = p.view_bias + ray * kCond;
+      uint8_t* vd = p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = 8 * j + cq;
+        const float2 b = __ldcg(reinterpret_cast<const float2*>(vb + c));
+        float y[4] = {acc0[4 * j], acc0[4 * j + 1], acc0[4 * j + 2], acc0[4 * j + 3]};
+        fadd2(y[0], y[1], b.x, b.y);
+        fadd2(y[2], y[3], b.x, b.y);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) y[e] = fmaxf(y[e], 0.f);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) {
+          const float2 wc = __ldg(reinterpret_cast<const float2*>(gsp->w_color[ch] + c));
+          ffma2(rgb[0][ch], rgb[1][ch], y[0], y[2], wc.x, wc.x);
+          ffma2(rgb[0][ch], rgb[1][ch], y[1], y[3], wc.y, wc.y);
+        }
+        if (vd) {  // training: the 16-bit view-layer output, same tile layout as the trunk's activation slabs
+          *reinterpret_cast<uint32_t*>(vd + (c >> 6) * kStageBytes + sw128_offset(r0, c & 63)) = pack2<kFmt>(y[0], y[1]);
+          *reinterpret_cast<uint32_t*>(vd + (c >> 6) * kStageBytes + sw128_offset(r0 + 8, c & 63)) =
+              pack2<kFmt>(y[2], y[3]);
         }
       }
     }
