@@ -95,8 +95,9 @@ struct LevelParams {
   float* raw_rgb_out;      // MLP-only mode: [B,128,3] / [B,128] raw heads instead of compositing
   float* raw_density_out;
   // Training forward: every activation the backward pass needs leaves the SM exactly as the tensor core saw it — the
-  // 16-bit SW128 activation tile of each trunk layer / the bottleneck is copied out by bulk stores (shared -> global)
-  // after its epilogue; the view layer's output and the raw heads go out from registers.
+  // 16-bit SW128 activation tile of each trunk layer / the bottleneck is stored from the epilogue's registers (bf16 /
+  // fp16) or copied out of shared memory by bulk stores after its epilogue (split modes); the view layer's output and
+  // the raw heads go out from registers.
   uint8_t* act_dump;       // [9][dump_tiles][64 KB]: h_0..h_7 (post-ReLU), bottleneck; tile = ray
   uint8_t* v_dump;         // [dump_tiles][32 KB]: view-layer output (post-ReLU), two SW128 slabs
   float* raw_rgb_keep;     // [B,128,3] / [B,128]: raw heads (before the activations) for render_backward
@@ -133,9 +134,9 @@ enum LevelPhase : int {
   kPhWFull,      // consumers: waiting for a weight stage (w_full)
   kPhMma,        // consumers: wgmma issue and retire
   kPhEpilogue,   // layer epilogue chunks (their K-slab's wgmmas run meanwhile), view layer + colour head, head
-                 // reductions, activation-dump issue
+                 // reductions, activation-dump stores
   kPhComposite,  // warpgroup 0: activations + compositing (or the raw heads of MLP-only mode)
-  kPhBarrier,    // consumers: named-barrier waits
+  kPhBarrier,    // consumers: named-barrier waits (bf16 / fp16: none inside the layer loop)
   kPhWEmpty,     // producer: waiting for a free ring slot (w_empty)
   kPhIssue,      // producer: everything else
   kPhTotal,      // clock64 cycles from the role's first mark to its last
@@ -251,10 +252,11 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
 // The level kernel (sm_90a): one persistent CTA per SM, 384 threads, one ray (= 128 sample rows) at a time.
 //   * warps 0-3 / 4-7: two consumer warpgroups, warpgroup g owns sample rows 64 g .. 64 g + 63 of the ray.  Each
 //     computes the IPE features of its rows, issues the wgmma (M = 64, N = 128, K = 16) of every layer for its rows
-//     (A operand: its rows of the activation / feature tile in shared memory; B: the weight stage both warpgroups
-//     share), and runs the epilogue from the register accumulators straight into the next layer's A operand, in place,
-//     in chunks under the wgmmas of later K-slabs (software-pipelined layer loop).  The rows of a warpgroup are private
-//     to it, so a layer boundary is a 128-thread barrier, not a CTA barrier.
+//     (A operand: its rows of the feature tile in shared memory for layer 0 and layer 5's skip slabs; otherwise the
+//     layer input in registers (bf16 / fp16) or its rows of the activation tile in shared memory (split modes); B: the
+//     weight stage both warpgroups share), and runs the epilogue from the register accumulators straight into the next
+//     layer's A operand in chunks under the wgmmas of later K-slabs (software-pipelined layer loop).  The rows of a
+//     warpgroup are private to it, so a layer boundary is at most a 128-thread barrier, not a CTA barrier.
 //   * warps 8-11: producer warpgroup (setmaxnreg gives its registers to the consumers); warp 8 is the weight producer
 //     — cp.async.bulk of the pre-swizzled [128 x 32] (SW64, 8 KB) stages of the packed image
 //     (+ the low-half stage in the split modes) into a ring; a stage is free once both warpgroups' wgmmas reading it
@@ -269,15 +271,21 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
 // 384 threads = three warpgroups; the producer warpgroup hands its registers to the consumers (setmaxnreg): 2 x 128 x 232
 // + 128 x 40 fill the register file, and the consumers' two live N = 128 accumulators fit without spills.
 constexpr int kThreads = 384;
+// Weight-ring depth of the bf16 / fp16 kernel (a -D flag overrides it for experiments).
+#ifndef MIPNERF_LEVEL_STAGES
+#define MIPNERF_LEVEL_STAGES 12
+#endif
 template <bool kX3>
 struct LevelLayout {
-  // bf16 / fp16: the ring is kept at 4 stages so that the CTA fits the 132 KB shared-memory carveout and L1 keeps
-  // ~124 KB for the consumers' stack frames and the epilogue's bias loads.  Measured on H100: 4.31 ms per 4096-ray bf16
-  // forward at 4 stages, 4.58 ms at 8 (164 KB carveout), 5.84 / 5.99 ms at 12 / 16 (L1 down to 60 / 28 KB).
-  static constexpr int kStages = kX3 ? 2 : 4;
+  // bf16 / fp16: the layer inputs live in registers, so the CTA holds only the feature tile and the weight ring, and
+  // the ring is as deep as the 132 KB shared-memory carveout allows (L1 keeps ~124 KB for the epilogue's bias loads).
+  // Measured on an H100 80GB HBM3 at 400 W (bench.py bf16 step, two runs each): 3.60-3.62 ms with 4 stages, 3.53-3.54
+  // ms with 8, 3.51-3.53 ms with 12.  With the shared-memory activation tile, 8 stages (164 KB carveout) and 12 / 16
+  // (L1 down to 60 / 28 KB) had been slower than 4.
+  static constexpr int kStages = kX3 ? 2 : MIPNERF_LEVEL_STAGES;
   static constexpr uint32_t kStage = kX3 ? 2 * kWStage : kWStage;  // split modes: W_hi stage, then W_lo
-  static constexpr uint32_t kA = 0;
-  static constexpr uint32_t kF = kA + (kX3 ? 2 : 1) * kABytes;  // split modes: hi tile, then lo tile
+  static constexpr uint32_t kA = 0;  // split modes only: the activation tile, hi then lo
+  static constexpr uint32_t kF = kA + (kX3 ? 2 * kABytes : 0);
   static constexpr uint32_t kW = kF + (kX3 ? 2 : 1) * kFBytes;
   static constexpr uint32_t kMisc = kW + kStages * kStage;
   // mbarriers, raw heads [2][128][4] (ray parity), scan carries [4], partial sums [4][8], resampler scratch [129]
@@ -309,15 +317,31 @@ struct RingPos {
 // issue its wgmmas as one group, then wait until only that group is in flight.  The wait retires the previous group,
 // whose stage is released (one arrive per warpgroup); so one stage's wgmmas stay in flight across calls, also from one
 // half or layer to the next.
+template <bool kX3>
+__device__ __forceinline__ uint32_t level_stage_acquire(uint32_t w_u, uint64_t* w_full, const RingPos& rp,
+                                                        PhaseClock& clk) {
+  mbar_wait(&w_full[rp.st], rp.ph);
+  clk.mark(kPhWFull);
+  wgmma_fence();
+  return w_u + (uint32_t)rp.st * LevelLayout<kX3>::kStage;
+}
+template <bool kX3>
+__device__ __forceinline__ void level_stage_commit(uint64_t* w_empty, RingPos& rp, bool leader, PhaseClock& clk) {
+  wgmma_commit();
+  wgmma_wait<1>();
+  if (rp.prev >= 0 && leader) mbar_arrive(&w_empty[rp.prev]);
+  rp.prev = rp.st;
+  if (++rp.st == LevelLayout<kX3>::kStages) {
+    rp.st = 0;
+    rp.ph ^= 1;
+  }
+  clk.mark(kPhMma);
+}
 template <int kFmt, bool kX3>
 __device__ __forceinline__ void level_mma_slab(float (&acc)[64], int l, int s, uint32_t a_u, uint32_t f_u,
                                                uint32_t ft_u, uint32_t w_u, uint64_t* w_full, uint64_t* w_empty,
                                                RingPos& rp, bool leader, PhaseClock& clk) {
-  using Lay = LevelLayout<kX3>;
-  mbar_wait(&w_full[rp.st], rp.ph);
-  clk.mark(kPhWFull);
-  wgmma_fence();
-  const uint32_t b_u = w_u + (uint32_t)rp.st * Lay::kStage;
+  const uint32_t b_u = level_stage_acquire<kX3>(w_u, w_full, rp, clk);
 #pragma unroll
   for (int j = 0; j < 2; ++j) {
     const uint64_t a_hi = level_a_desc(l, s, j, a_u, f_u, ft_u);
@@ -328,15 +352,22 @@ __device__ __forceinline__ void level_mma_slab(float (&acc)[64], int l, int s, u
       wgmma_m64n128k16<kFmt>(acc, a_hi, b_hi + kWStage / 16, 1u);
     }
   }
-  wgmma_commit();
-  wgmma_wait<1>();
-  if (rp.prev >= 0 && leader) mbar_arrive(&w_empty[rp.prev]);
-  rp.prev = rp.st;
-  if (++rp.st == Lay::kStages) {
-    rp.st = 0;
-    rp.ph ^= 1;
+  level_stage_commit<kX3>(w_empty, rp, leader, clk);
+}
+// The same for K-slab s < 8 of layers 1..9 in the bf16 / fp16 kernel, with A from registers: x is the layer input as
+// wgmma A fragments (see level_epilogue_chunk_rs), and K-slab s reads x[8 s .. 8 s + 7].  `s` must be a compile-time
+// constant after unrolling, so that x stays in registers.
+template <int kFmt>
+__device__ __forceinline__ void level_mma_slab_rs(float (&acc)[64], const uint32_t (&x)[64], int s, uint32_t w_u,
+                                                  uint64_t* w_full, uint64_t* w_empty, RingPos& rp, bool leader,
+                                                  PhaseClock& clk) {
+  const uint32_t b_u = level_stage_acquire<false>(w_u, w_full, rp, clk);
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const uint32_t a[4] = {x[8 * s + 4 * j], x[8 * s + 4 * j + 1], x[8 * s + 4 * j + 2], x[8 * s + 4 * j + 3]};
+    wgmma_m64n128k16_rs<kFmt>(acc, a, make_sw64_desc(b_u + 32u * j), (s | j) ? 1u : 0u);
   }
-  clk.mark(kPhMma);
+  level_stage_commit<false>(w_empty, rp, leader, clk);
 }
 
 // The layer epilogues run in chunks under the wgmmas of K-slabs (see the layer loop of mlp_level_kernel): kEpiChunks
@@ -401,6 +432,146 @@ __device__ __forceinline__ void level_epilogue_chunk(const float (&acc)[64], con
       *reinterpret_cast<uint32_t*>(sA + kABytes + o1) = pack2<kFmt>(a2 - f1.x, a3 - f1.y);
     }
   }
+}
+
+// ---- the register-chained layer loop of the bf16 / fp16 kernel ----
+// First K-slab of a layer's N-half 1 that carries a chunk of N-half 0's epilogue (chunk c after K-slab
+// kEpiFirstRs + c).  The chunks write registers that no wgmma in flight reads, and the wait of N-half 1's first K-slab
+// retires all of N-half 0, so any value in 0..4 is safe; a -D flag overrides it for experiments.  Measured on an H100
+// 80GB HBM3 at 400 W (bench.py bf16 step, 12 stages): 3.86-3.89 ms with 0, 3.81-3.82 ms with 1, 3.51-3.53 ms with 2,
+// 3.52-3.54 ms with 3, 3.52-3.59 ms with 4.
+#ifndef MIPNERF_LEVEL_EPI_FIRST
+#define MIPNERF_LEVEL_EPI_FIRST 2
+#endif
+constexpr int kEpiFirstRs = MIPNERF_LEVEL_EPI_FIRST;
+static_assert(kEpiFirstRs >= 0 && kEpiFirstRs + kEpiChunks <= 8, "the chunks must follow K-slabs 0..7");
+
+// What the layer loop needs besides its accumulators and A arrays.
+struct LevelRsCtx {
+  uint32_t f_u, ft_u, w_u;  // this warpgroup's feature tile (SW128 slab, SW64 tail), the weight ring
+  uint64_t* w_full;
+  uint64_t* w_empty;
+  const SmallParams* gsp;
+  uint8_t* dump;           // training forward: this ray's tile of h_0 in p.act_dump (h_l: + l dump_stride); else null
+  size_t dump_stride;
+  uint64_t dump_policy;
+  int r0, cq;
+  bool leader;
+};
+
+// Epilogue chunk of the bf16 / fp16 kernel: the arithmetic of level_epilogue_chunk, with the 16-bit pairs kept in
+// registers as the next layer's wgmma A fragments instead of stored to shared memory.  The accumulator fragment of
+// column group j (columns 8 j + cq, + 1 of rows r0 and r0 + 8, j counted over all 256 columns) is half of the A
+// fragment of K-step j / 2: x[2 j] holds row r0, x[2 j + 1] row r0 + 8.  In the training forward the same pairs also
+// go to the layer's activation tile in global memory, at their SW128 tile-image offsets.
+template <int kFmt>
+__device__ __forceinline__ void level_epilogue_chunk_rs(const float (&acc)[64], const EpiConsts& e, int l, int c_base,
+                                                        int chunk, uint32_t (&x)[64], const LevelRsCtx& k, float& d0,
+                                                        float& d1) {
+  const bool relu = l < 8;
+  uint8_t* dump = k.dump ? k.dump + (size_t)l * k.dump_stride : nullptr;
+#pragma unroll
+  for (int jj = 0; jj < kEpiGroups; ++jj) {
+    const int j = kEpiGroups * chunk + jj;
+    const float2 b = e.b[jj];
+    float a0 = acc[4 * j], a1 = acc[4 * j + 1], a2 = acc[4 * j + 2], a3 = acc[4 * j + 3];
+    fadd2(a0, a1, b.x, b.y);
+    fadd2(a2, a3, b.x, b.y);
+    if (l == 7) {
+      const float2 wd = __ldg(reinterpret_cast<const float2*>(k.gsp->w_density + c_base + 8 * j + k.cq));
+      ffma2(d0, d1, fmaxf(a0, 0.f), fmaxf(a2, 0.f), wd.x, wd.x);
+      ffma2(d0, d1, fmaxf(a1, 0.f), fmaxf(a3, 0.f), wd.y, wd.y);
+    }
+    if (relu) a0 = fmaxf(a0, 0.f), a1 = fmaxf(a1, 0.f), a2 = fmaxf(a2, 0.f), a3 = fmaxf(a3, 0.f);
+    const int jg = (c_base >> 3) + j;
+    x[2 * jg] = pack2<kFmt>(a0, a1);
+    x[2 * jg + 1] = pack2<kFmt>(a2, a3);
+  }
+  if (dump) {
+    // The four threads of a quad hold the four 4-byte quarters of the chunk's four 16-byte column groups (per row): a
+    // 4 x 4 transpose in the quad (two butterfly steps) gives thread q all of group 4 chunk + q, one 16-byte store per
+    // row, so that every store fills whole L2 sectors.
+    const int q = k.cq >> 1;
+    const int jg = (c_base >> 3) + kEpiGroups * chunk + q;
+    const uint32_t o0 = (uint32_t)(jg >> 3) * kStageBytes + sw128_offset(k.r0, 8 * (jg & 7));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {  // row r0, row r0 + 8
+      uint32_t v[4];
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) v[jj] = x[2 * ((c_base >> 3) + kEpiGroups * chunk + jj) + h];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {  // exchange the 2 x 2 blocks off the diagonal with quad thread q ^ 2
+        const uint32_t r = __shfl_xor_sync(0xffffffffu, (q & 2) ? v[i] : v[2 + i], 2);
+        if (q & 2) v[i] = r;
+        else v[2 + i] = r;
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {  // then the elements off the diagonal of each block with quad thread q ^ 1
+        const uint32_t r = __shfl_xor_sync(0xffffffffu, (q & 1) ? v[2 * i] : v[2 * i + 1], 1);
+        if (q & 1) v[2 * i] = r;
+        else v[2 * i + 1] = r;
+      }
+      st_global_v4_hint(dump + o0 + (uint32_t)h * 8u * 128u, make_uint4(v[0], v[1], v[2], v[3]), k.dump_policy);
+    }
+  }
+}
+
+// Layer l + 1's N-half 0, K-slabs 0..3 (x[0..31], from acc0's epilogue of layer l) into acc0, with acc1's epilogue of
+// layer l (x[32..63]) in chunks after them.  The wait of the first K-slab retires all of layer l.
+template <int kFmt>
+__device__ __forceinline__ void level_rs_next_head(float (&acc0)[64], float (&acc1)[64], uint32_t (&x)[64], int l,
+                                                   const LevelRsCtx& k, RingPos& rp, PhaseClock& clk, float& d0,
+                                                   float& d1) {
+  wgmma_fence_acc(acc0);
+#pragma unroll
+  for (int c = 0; c < kEpiChunks; ++c) {
+    EpiConsts e;
+    level_epilogue_consts(e, l, 128, c, k.cq, k.gsp);
+    level_mma_slab_rs<kFmt>(acc0, x, c, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+    if (c == 0) wgmma_fence_acc(acc1);
+    level_epilogue_chunk_rs<kFmt>(acc1, e, l, 128, c, x, k, d0, d1);
+    clk.mark(kPhEpilogue);
+  }
+}
+
+// Trunk layer / bottleneck l (1..8) from x_in into x_out: the rest of N-half 0 into acc0, N-half 1 into acc1 with
+// acc0's epilogue in chunks under it, then level_rs_next_head.  kSkip: l may be 5, whose K-slabs 8..10 read the
+// feature tile.
+template <int kFmt, bool kSkip>
+__device__ __forceinline__ void level_rs_layer(float (&acc0)[64], float (&acc1)[64], const uint32_t (&x_in)[64],
+                                               uint32_t (&x_out)[64], int l, const LevelRsCtx& k, RingPos& rp,
+                                               PhaseClock& clk, float& d0, float& d1) {
+  const bool skip = kSkip && l == 5;
+  // the feature tile's addresses, opaque here so that the compiler recomputes the skip slabs' descriptors instead of
+  // keeping them in local memory across the layers
+  uint32_t f_u = k.f_u, ft_u = k.ft_u;
+  asm volatile("" : "+r"(f_u), "+r"(ft_u));
+#pragma unroll
+  for (int s = kEpiChunks; s < 8; ++s)
+    level_mma_slab_rs<kFmt>(acc0, x_in, s, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+  if (skip)
+    for (int s = 8; s < num_k32(5); ++s)
+      level_mma_slab<kFmt, false>(acc0, 5, s, 0u, f_u, ft_u, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+  wgmma_fence_acc(acc1);
+#pragma unroll
+  for (int s = 0; s < kEpiFirstRs; ++s)
+    level_mma_slab_rs<kFmt>(acc1, x_in, s, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+#pragma unroll
+  for (int c = 0; c < kEpiChunks; ++c) {
+    EpiConsts e;
+    level_epilogue_consts(e, l, 0, c, k.cq, k.gsp);
+    level_mma_slab_rs<kFmt>(acc1, x_in, kEpiFirstRs + c, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+    if (c == 0) wgmma_fence_acc(acc0);
+    level_epilogue_chunk_rs<kFmt>(acc0, e, l, 0, c, x_out, k, d0, d1);
+    clk.mark(kPhEpilogue);
+  }
+#pragma unroll
+  for (int s = kEpiFirstRs + kEpiChunks; s < 8; ++s)
+    level_mma_slab_rs<kFmt>(acc1, x_in, s, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+  if (skip)
+    for (int s = 8; s < num_k32(5); ++s)
+      level_mma_slab<kFmt, false>(acc1, 5, s, 0u, f_u, ft_u, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+  level_rs_next_head<kFmt>(acc0, acc1, x_out, l, k, rp, clk, d0, d1);
 }
 
 __device__ __forceinline__ float quad_sum(float v) {
@@ -549,10 +720,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
 
     float d0 = 0.f, d1 = 0.f;  // density head, rows r0 / r0 + 8 (partial over this thread's columns)
     float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-    // ---- the layers, software-pipelined so that each epilogue runs under wgmmas instead of after them.  The epilogue
-    // of trunk layer / bottleneck l overwrites, in place, the activation columns that layer l read; wgmmas consume K in
-    // order, and K-slab s of layers 1..9 reads only columns 32 s .. 32 s + 31 (layer 5's slabs 8-10 and layer 0 read
-    // the feature tile).  Per layer l:
+    // ---- the layers, software-pipelined so that each epilogue runs under wgmmas instead of after them.  In the split
+    // modes the epilogue of trunk layer / bottleneck l overwrites, in place, the activation columns (hi and lo tiles)
+    // that layer l read; wgmmas consume K in order, and K-slab s of layers 1..9 reads only columns 32 s .. 32 s + 31
+    // (layer 5's slabs 8-10 and layer 0 read the feature tile).  Per layer l:
     //   1. N-half 0 into acc0: K-slabs 0..3 were issued under the previous layer's acc1 epilogue (step 4); the rest here.
     //   2. N-half 1 into acc1; after K-slab kEpiOverlap + c has been committed and waited for, chunk c of acc0's
     //      epilogue (columns 32 c .. 32 c + 31).  That wait leaves only K-slab kEpiOverlap + c in flight: all of N-half
@@ -565,81 +736,117 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
     //   5. fence + barrier: layer l + 1's input is complete (and goes out with bulk stores in the training forward).
     // A chunk's bias loads are issued before the K-slab it follows.  The wgmmas into each accumulator, their operands and
     // order, and the epilogue arithmetic are those of an unpipelined loop, so the results are the same bit for bit.
+    // bf16 / fp16 keep the layer input in registers instead (below): the same steps without 3 and 5.
     float acc0[64], acc1[64];
     wgmma_fence_acc(acc0);
 #pragma unroll
     for (int s = 0; s < num_k32(0); ++s)
       level_mma_slab<kFmt, kX3>(acc0, 0, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
-    for (int l = 0; l < 9; ++l) {
-      // 1. the rest of N-half 0
-      if (l > 0)
-        for (int s = kEpiChunks; s < num_k32(l); ++s)
-          level_mma_slab<kFmt, kX3>(acc0, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
-      // 2. N-half 1, with acc0's epilogue under it
+    if constexpr (!kX3) {
+      // bf16 / fp16: the layers are chained through registers (wgmma with A from registers), the schedule above with
+      // no activation tile: each epilogue chunk writes its 16-bit pairs into the A fragments of the next layer's input,
+      // one of two arrays (layer l reads xa or xb, writes the other), so no layer's writes touch what its own wgmmas
+      // read, and there is no fence or barrier between layers.  acc0's chunks follow N-half 1's K-slabs kEpiFirstRs + c
+      // and acc1's the next layer's K-slabs 0..3.  Layer 0 and layer 5's K-slabs 8..10 read the feature tile; layer 0
+      // has three K-slabs, so its acc0 chunks follow K-slabs 0, 1, 2, 2.  The training forward's activation tiles go
+      // out from the epilogue's registers.
+      const LevelRsCtx k{f_u, ft_u, w_u, w_full, w_empty, gsp,
+                         p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
+                         (size_t)p.dump_tiles * kABytes, dump_policy, r0, cq, leader};
+      uint32_t xa[64], xb[64];
       wgmma_fence_acc(acc1);
-      const int first = l == 0 ? 0 : kEpiOverlap;  // K-slab that carries chunk 0
-      for (int s = 0; s < first; ++s)
-        level_mma_slab<kFmt, kX3>(acc1, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
 #pragma unroll
       for (int c = 0; c < kEpiChunks; ++c) {
         EpiConsts e;
-        level_epilogue_consts(e, l, 0, c, cq, gsp);
-        if (first + c < num_k32(l))
-          level_mma_slab<kFmt, kX3>(acc1, l, first + c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
-        if (c == 0) {
-          wgmma_fence_acc(acc0);
-          if (dump_pending) {  // the previous tile's bulk stores must have READ it before it is overwritten
-            if (leader) bulk_store_wait_read();
-            dump_pending = false;
-            clk.mark(kPhEpilogue);
-            named_bar_sync(1 + wg, 128);
-            clk.mark(kPhBarrier);
-          }
-        }
-        level_epilogue_chunk<kFmt, kX3>(acc0, e, l, 0, c, r0, cq, sA, gsp, d0, d1);
+        level_epilogue_consts(e, 0, 0, c, cq, gsp);
+        if (c < num_k32(0))
+          level_mma_slab<kFmt, false>(acc1, 0, c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+        if (c == 0) wgmma_fence_acc(acc0);
+        level_epilogue_chunk_rs<kFmt>(acc0, e, 0, 0, c, xb, k, d0, d1);
         clk.mark(kPhEpilogue);
       }
-      for (int s = first + kEpiChunks; s < num_k32(l); ++s)
-        level_mma_slab<kFmt, kX3>(acc1, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
-      // 3.
-      fence_proxy_async_smem();
-      clk.mark(kPhEpilogue);
-      named_bar_sync(1 + wg, 128);
-      clk.mark(kPhBarrier);
-      // 4. the next layer's N-half 0, K-slabs 0..3, with acc1's epilogue under the first three
-      wgmma_fence_acc(acc0);
+      level_rs_next_head<kFmt>(acc0, acc1, xb, 0, k, rp, clk, d0, d1);
+#pragma unroll 1
+      for (int l = 1; l < 9; l += 2) {
+        level_rs_layer<kFmt, true>(acc0, acc1, xb, xa, l, k, rp, clk, d0, d1);
+        level_rs_layer<kFmt, false>(acc0, acc1, xa, xb, l + 1, k, rp, clk, d0, d1);
+      }
+      // the rest of the view layer's one N-half, from the bottleneck in xb
 #pragma unroll
-      for (int c = 0; c < kEpiChunks; ++c) {
-        EpiConsts e;
-        level_epilogue_consts(e, l, 128, c, cq, gsp);
-        if (c < kEpiChunks - 1) {
-          level_mma_slab<kFmt, kX3>(acc0, l + 1, c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
-          if (c == 0) wgmma_fence_acc(acc1);
-        }
-        level_epilogue_chunk<kFmt, kX3>(acc1, e, l, 128, c, r0, cq, sA, gsp, d0, d1);
-        clk.mark(kPhEpilogue);
-      }
-      level_mma_slab<kFmt, kX3>(acc0, l + 1, kEpiChunks - 1, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
-      // 5.
-      fence_proxy_async_smem();
-      clk.mark(kPhEpilogue);
-      named_bar_sync(1 + wg, 128);
-      clk.mark(kPhBarrier);
-      if (p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core reads it
-        if (leader) {
+      for (int s = kEpiChunks; s < 8; ++s) level_mma_slab_rs<kFmt>(acc0, xb, s, w_u, w_full, w_empty, rp, leader, clk);
+    } else {
+      for (int l = 0; l < 9; ++l) {
+        // 1. the rest of N-half 0
+        if (l > 0)
+          for (int s = kEpiChunks; s < num_k32(l); ++s)
+            level_mma_slab<kFmt, kX3>(acc0, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+        // 2. N-half 1, with acc0's epilogue under it
+        wgmma_fence_acc(acc1);
+        const int first = l == 0 ? 0 : kEpiOverlap;  // K-slab that carries chunk 0
+        for (int s = 0; s < first; ++s)
+          level_mma_slab<kFmt, kX3>(acc1, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint32_t o = (uint32_t)k * kStageBytes + (uint32_t)wg * 8192u;
-            bulk_s2g_hint(p.act_dump + ((size_t)l * p.dump_tiles + ray) * kABytes + o, sA + o, 8192u, dump_policy);
+        for (int c = 0; c < kEpiChunks; ++c) {
+          EpiConsts e;
+          level_epilogue_consts(e, l, 0, c, cq, gsp);
+          if (first + c < num_k32(l))
+            level_mma_slab<kFmt, kX3>(acc1, l, first + c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+          if (c == 0) {
+            wgmma_fence_acc(acc0);
+            if (dump_pending) {  // the previous tile's bulk stores must have READ it before it is overwritten
+              if (leader) bulk_store_wait_read();
+              dump_pending = false;
+              clk.mark(kPhEpilogue);
+              named_bar_sync(1 + wg, 128);
+              clk.mark(kPhBarrier);
+            }
           }
+          level_epilogue_chunk<kFmt, kX3>(acc0, e, l, 0, c, r0, cq, sA, gsp, d0, d1);
+          clk.mark(kPhEpilogue);
         }
-        dump_pending = true;
+        for (int s = first + kEpiChunks; s < num_k32(l); ++s)
+          level_mma_slab<kFmt, kX3>(acc1, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+        // 3.
+        fence_proxy_async_smem();
         clk.mark(kPhEpilogue);
+        named_bar_sync(1 + wg, 128);
+        clk.mark(kPhBarrier);
+        // 4. the next layer's N-half 0, K-slabs 0..3, with acc1's epilogue under the first three
+        wgmma_fence_acc(acc0);
+#pragma unroll
+        for (int c = 0; c < kEpiChunks; ++c) {
+          EpiConsts e;
+          level_epilogue_consts(e, l, 128, c, cq, gsp);
+          if (c < kEpiChunks - 1) {
+            level_mma_slab<kFmt, kX3>(acc0, l + 1, c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+            if (c == 0) wgmma_fence_acc(acc1);
+          }
+          level_epilogue_chunk<kFmt, kX3>(acc1, e, l, 128, c, r0, cq, sA, gsp, d0, d1);
+          clk.mark(kPhEpilogue);
+        }
+        level_mma_slab<kFmt, kX3>(acc0, l + 1, kEpiChunks - 1, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+        // 5.
+        fence_proxy_async_smem();
+        clk.mark(kPhEpilogue);
+        named_bar_sync(1 + wg, 128);
+        clk.mark(kPhBarrier);
+        if (p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core reads it
+          if (leader) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const uint32_t o = (uint32_t)k * kStageBytes + (uint32_t)wg * 8192u;
+              bulk_s2g_hint(p.act_dump + ((size_t)l * p.dump_tiles + ray) * kABytes + o, sA + o, 8192u, dump_policy);
+            }
+          }
+          dump_pending = true;
+          clk.mark(kPhEpilogue);
+        }
       }
+      // the rest of the view layer's one N-half
+      for (int s = kEpiChunks; s < num_k32(9); ++s)
+        level_mma_slab<kFmt, kX3>(acc0, 9, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
     }
-    // the rest of the view layer's one N-half, then its epilogue from the registers
-    for (int s = kEpiChunks; s < num_k32(9); ++s)
-      level_mma_slab<kFmt, kX3>(acc0, 9, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+    // the view layer's epilogue from the registers
     wgmma_wait<0>();
     wgmma_fence_acc(acc0);
     if (leader) mbar_arrive(&w_empty[rp.prev]);

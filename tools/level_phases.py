@@ -2,7 +2,9 @@
 
 Builds the `phases` variant of the library (-DMIPNERF_LEVEL_PHASES: clock64 phase accounting in mlp_level_kernel), runs
 the benchmark's forward (4096 rays, xavier weights) in bf16 and fp16x3, and prints, per level launch and per role, the
-share of each phase in the role's cycles, averaged over CTAs, next to the GPU's name and power limit.
+share of each phase in the role's cycles, averaged over CTAs, next to the GPU's name and power limit.  Phases a role
+never enters are left out: in bf16 / fp16 the layer loop has no barrier, so `barrier` counts only the waits around
+the feature tile, the ray prologue and the raw heads.
 
     python tools/level_phases.py [--rays 4096] [--reps 20] [--precisions bf16,fp16x3] [--json OUT]
 
