@@ -75,7 +75,7 @@ struct LevelParams {
   const float* radii;
   float* t;                // [B,129] fenceposts of this level (read; written first when t_mode != 0)
   float* view_bias;        // [B,128]  b_view + W_view[:,256:] . pos_enc(viewdir) (written first when vb_mode != 0)
-  // Ray prologue, run by warp 0 in front of each ray's features: fenceposts / view bias produced in the level kernel
+  // Ray prologue, run by the helper warps ahead of each ray's features: fenceposts / view bias produced in the level kernel
   // instead of by launches of their own.
   int t_mode;              // 0: read p.t; 1: coarse fenceposts from near/far (models/mip.py:143-160);
                            // 2: resample t_prev / w_prev (models/mip.py:232-280)
@@ -125,28 +125,32 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
 }
 
 // Phase accounting of the level kernel (tools/level_phases.py): built with -DMIPNERF_LEVEL_PHASES, thread 0 of each
-// consumer warpgroup and the producer thread charge the clock64 cycles since their previous mark to a phase, per CTA
-// and per level (slot 0: coarse fenceposts, slot 1: resampled).  Without the define, PhaseClock is empty and every
-// mark compiles to nothing.
+// consumer warpgroup, the producer thread and the first helper thread charge the clock64 cycles since their previous
+// mark to a phase, per CTA and per level (slot 0: coarse fenceposts, slot 1: resampled).  Without the define,
+// PhaseClock is empty and every mark compiles to nothing.
 enum LevelPhase : int {
-  kPhPrologue,   // warp 0: fenceposts / resampler, view bias
-  kPhIpe,        // Gaussians + IPE features
+  kPhPrologue,   // helpers: fenceposts / resampler, view bias
+  kPhIpe,        // helpers: Gaussians + IPE features
   kPhWFull,      // consumers: waiting for a weight stage (w_full)
   kPhMma,        // consumers: wgmma issue and retire
   kPhEpilogue,   // layer epilogue chunks (their K-slab's wgmmas run meanwhile), view layer + colour head, head
                  // reductions, activation-dump stores
-  kPhComposite,  // warpgroup 0: activations + compositing (or the raw heads of MLP-only mode)
-  kPhBarrier,    // consumers: named-barrier waits (bf16 / fp16: none inside the layer loop)
+  kPhComposite,  // helpers: activations + compositing (or the raw heads of MLP-only mode)
+  kPhBarrier,    // named-barrier waits (bf16 / fp16 consumers: none inside the layer loop), consumers' heads_empty
   kPhWEmpty,     // producer: waiting for a free ring slot (w_empty)
   kPhIssue,      // producer: everything else
+  kPhFeatFull,   // consumers: waiting for the ray's feature buffer (feat_full)
+  kPhFeatEmpty,  // helpers: waiting for a free feature buffer (feat_empty)
+  kPhHeadsFull,  // helpers: waiting for the raw heads of the ray to composite (heads_full)
   kPhTotal,      // clock64 cycles from the role's first mark to its last
   kNumPhases
 };
 #ifdef MIPNERF_LEVEL_PHASES
+constexpr int kNumRoles = 4;  // consumer warpgroup 0, consumer warpgroup 1, weight producer, helpers
 constexpr int kPhaseMaxCtas = 1024;
-constexpr uint32_t kPhaseBytes = 3 * kNumPhases * 8;  // shared-memory accumulators, one row per role
-// [slot][cta][role: consumer wg 0, consumer wg 1, producer][phase]
-__device__ unsigned long long g_level_phases[2][kPhaseMaxCtas][3][kNumPhases];
+constexpr uint32_t kPhaseBytes = kNumRoles * kNumPhases * 8;  // shared-memory accumulators, one row per role
+// [slot][cta][role][phase]
+__device__ unsigned long long g_level_phases[2][kPhaseMaxCtas][kNumRoles][kNumPhases];
 struct PhaseClock {
   unsigned long long* acc;  // this role's row in shared memory; null on the threads that do not measure
   long long start, last;
@@ -249,52 +253,75 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
 }
 
 // =================================================================================================
-// The level kernel (sm_90a): one persistent CTA per SM, 384 threads, one ray (= 128 sample rows) at a time.
+// The level kernel (sm_90a): one persistent CTA per SM, 384 threads, one ray (= 128 sample rows) at a time in the
+// tensor core, with the scalar work of the neighbouring rays beside it.
 //   * warps 0-3 / 4-7: two consumer warpgroups, warpgroup g owns sample rows 64 g .. 64 g + 63 of the ray.  Each
-//     computes the IPE features of its rows, issues the wgmma (M = 64, N = 128, K = 16) of every layer for its rows
-//     (A operand: its rows of the feature tile in shared memory for layer 0 and layer 5's skip slabs; otherwise the
-//     layer input in registers (bf16 / fp16) or its rows of the activation tile in shared memory (split modes); B: the
-//     weight stage both warpgroups share), and runs the epilogue from the register accumulators straight into the next
-//     layer's A operand in chunks under the wgmmas of later K-slabs (software-pipelined layer loop).  The rows of a
-//     warpgroup are private to it, so a layer boundary is at most a 128-thread barrier, not a CTA barrier.
-//   * warps 8-11: producer warpgroup (setmaxnreg gives its registers to the consumers); warp 8 is the weight producer
+//     issues the wgmma (M = 64, N = 128, K = 16) of every layer for its rows (A operand: its rows of the ray's feature
+//     buffer in shared memory for layer 0 and layer 5's skip slabs; otherwise the layer input in registers (bf16 /
+//     fp16) or its rows of the activation tile in shared memory (split modes); B: the weight stage both warpgroups
+//     share), runs the epilogue from the register accumulators straight into the next layer's A operand in chunks
+//     under the wgmmas of later K-slabs (software-pipelined layer loop), and leaves the raw heads of its rows in shared
+//     memory.  The rows of a warpgroup are private to it, so a layer boundary is at most a 128-thread barrier.
+//   * warps 8-11: producer warpgroup (setmaxnreg gives registers to the consumers).  Warp 8 is the weight producer
 //     — cp.async.bulk of the pre-swizzled [128 x 32] (SW64, 8 KB) stages of the packed image
 //     (+ the low-half stage in the split modes) into a ring; a stage is free once both warpgroups' wgmmas reading it
 //     have completed.
-//   * in front of each ray's features, warp 0 runs the ray prologue: the coarse fenceposts (level 0) or the bit-exact
-//     inverse-CDF resampler (levels >= 1), and the per-ray view-layer bias (level 0; later levels read it back);
-//   * after the view layer both warpgroups leave the raw heads of their rows in shared memory and warpgroup 0
-//     composites the ray (thread = sample row) while warpgroup 1 starts on the next ray's features.
-// A forward is one launch of this kernel per level and nothing else.  The layer-5 skip connection is three extra K
-// slabs read from the feature tile (no concat).
+//   * warps 9-11 are the helpers: while the consumers run the layers of ray r, they run the ray prologue of ray r + 1
+//     (the coarse fenceposts (level 0) or the bit-exact inverse-CDF resampler (levels >= 1), and the per-ray
+//     view-layer bias (level 0; later levels read it back)), write its Gaussians + IPE features into a free feature
+//     buffer, and then composite ray r once its raw heads are in.
+// Hand-offs (mbarriers): feat_full[b] (helpers -> consumers: the features of buffer b are written and fenced for the
+// async proxy), feat_empty[b] (consumers -> helpers: the wait that retires layer 5's last skip K-slab has returned, the
+// last read of the buffer), heads_full[par] / heads_empty[par] (the raw heads of rays of parity par).  A forward is one
+// launch of this kernel per level and nothing else.  The layer-5 skip connection is three extra K slabs read from the
+// feature buffer (no concat).
 // =================================================================================================
-// 384 threads = three warpgroups; the producer warpgroup hands its registers to the consumers (setmaxnreg): 2 x 128 x 232
-// + 128 x 40 fill the register file, and the consumers' two live N = 128 accumulators fit without spills.
+// 384 threads = three warpgroups; the producer warpgroup hands its registers to the consumers (setmaxnreg): 2 x 128 x
+// kConsumerRegs + 128 x kProducerRegs fill the register file, and the consumers' two live N = 128 accumulators fit
+// without spills.
 constexpr int kThreads = 384;
+constexpr int kHelperWarp0 = 9;  // warps 9-11
+constexpr int kHelperThreads = 96;
+constexpr int kHelperBar = 3;  // named barrier of the helper warps (1 and 2: the consumer warpgroups' own)
+constexpr int kHeadsWriters = 2 * 128 / 4;  // one consumer thread per quad stores the raw heads of its two rows
+#ifndef MIPNERF_LEVEL_PRODUCER_REGS
+#define MIPNERF_LEVEL_PRODUCER_REGS 40
+#endif
+constexpr int kProducerRegs = MIPNERF_LEVEL_PRODUCER_REGS;
+constexpr int kConsumerRegs = (65536 / 128 - kProducerRegs) / 2 / 8 * 8;
+static_assert(2 * 128 * kConsumerRegs + 128 * kProducerRegs <= 65536 && kProducerRegs % 8 == 0, "setmaxnreg split");
 // Weight-ring depth of the bf16 / fp16 kernel (a -D flag overrides it for experiments).
 #ifndef MIPNERF_LEVEL_STAGES
 #define MIPNERF_LEVEL_STAGES 12
 #endif
 template <bool kX3>
 struct LevelLayout {
-  // bf16 / fp16: the layer inputs live in registers, so the CTA holds only the feature tile and the weight ring, and
-  // the ring is as deep as the 132 KB shared-memory carveout allows (L1 keeps ~124 KB for the epilogue's bias loads).
-  // Measured on an H100 80GB HBM3 at 400 W (bench.py bf16 step, two runs each): 3.60-3.62 ms with 4 stages, 3.53-3.54
-  // ms with 8, 3.51-3.53 ms with 12.  With the shared-memory activation tile, 8 stages (164 KB carveout) and 12 / 16
-  // (L1 down to 60 / 28 KB) had been slower than 4.
+  // Feature buffers: bf16 / fp16 have two, so that the helpers write ray r + 1's features while layer 0 / layer 5 of
+  // ray r read the other; the split modes (hi + lo tiles next to the 128 KB activation tile) have room for one only,
+  // and the helpers write the next ray's features once layer 5's skip slabs have retired.
+  static constexpr int kFeatBufs = kX3 ? 1 : 2;
+  static constexpr uint32_t kFBuf = (kX3 ? 2 : 1) * kFBytes;  // one buffer: the feature tile (split modes: hi, lo)
+  // bf16 / fp16: the layer inputs live in registers, so the CTA holds only the feature buffers and the weight ring, and
+  // the ring is as deep as the carveout allows: 9 stages within 132 KB (L1 keeps ~124 KB for the epilogue's bias
+  // loads), 12 within 164 KB.
   static constexpr int kStages = kX3 ? 2 : MIPNERF_LEVEL_STAGES;
   static constexpr uint32_t kStage = kX3 ? 2 * kWStage : kWStage;  // split modes: W_hi stage, then W_lo
   static constexpr uint32_t kA = 0;  // split modes only: the activation tile, hi then lo
   static constexpr uint32_t kF = kA + (kX3 ? 2 * kABytes : 0);
-  static constexpr uint32_t kW = kF + (kX3 ? 2 : 1) * kFBytes;
+  static constexpr uint32_t kW = kF + kFeatBufs * kFBuf;
   static constexpr uint32_t kMisc = kW + kStages * kStage;
+  // mbarriers: w_full / w_empty [kStages], feat_full / feat_empty [kFeatBufs], heads_full / heads_empty [2]
+  static constexpr int kNumMbars = 2 * kStages + 2 * kFeatBufs + 2 * 2;
   // mbarriers, raw heads [2][128][4] (ray parity), scan carries [4], partial sums [4][8], resampler scratch [129]
-  static constexpr uint32_t kMiscBytes = 2 * kStages * 8 + 2 * kN * 4 * 4 + 4 * 4 + 4 * 8 * 4 + (kN + 1) * 4;
+  static constexpr uint32_t kMiscBytes = kNumMbars * 8 + 2 * kN * 4 * 4 + 4 * 4 + 4 * 8 * 4 + (kN + 1) * 4;
   static constexpr uint32_t kPhase = (kMisc + kMiscBytes + 7) & ~7u;  // phase accumulators (MIPNERF_LEVEL_PHASES)
   // + slack for the 1024-B alignment of the tiles
   static constexpr uint32_t kTotal = kMisc + kMiscBytes + (kPhaseBytes ? kPhaseBytes + 8 : 0) + 1024;
+  static_assert(kNumMbars % 2 == 0, "the raw heads behind the mbarriers must be 16-B aligned");
   static_assert(kTotal <= 232448, "exceeds 227 KB of shared memory per CTA");
-  static_assert(kX3 || kTotal + 1024 <= 132 * 1024, "bf16 / fp16 layout no longer fits the 132 KB carveout");
+  static_assert(kX3 || kStages > 9 || kTotal + 1024 <= 132 * 1024,
+                "bf16 / fp16 with up to 9 stages no longer fits the 132 KB carveout");
+  static_assert(kX3 || kTotal + 1024 <= 164 * 1024, "bf16 / fp16 layout no longer fits the 164 KB carveout");
 };
 
 // A-operand descriptor of K step j (16 wide) of K-slab s (32 wide) of layer l, for the rows of one warpgroup
@@ -448,9 +475,10 @@ static_assert(kEpiFirstRs >= 0 && kEpiFirstRs + kEpiChunks <= 8, "the chunks mus
 
 // What the layer loop needs besides its accumulators and A arrays.
 struct LevelRsCtx {
-  uint32_t f_u, ft_u, w_u;  // this warpgroup's feature tile (SW128 slab, SW64 tail), the weight ring
+  uint32_t f_u, ft_u, w_u;  // this warpgroup's rows of the ray's feature buffer (SW128 slab, SW64 tail), the weight ring
   uint64_t* w_full;
   uint64_t* w_empty;
+  uint64_t* feat_empty;    // the ray's feature buffer is free once layer 5's skip slabs have retired
   const SmallParams* gsp;
   uint8_t* dump;           // training forward: this ray's tile of h_0 in p.act_dump (h_l: + l dump_stride); else null
   size_t dump_stride;
@@ -517,17 +545,19 @@ __device__ __forceinline__ void level_epilogue_chunk_rs(const float (&acc)[64], 
 }
 
 // Layer l + 1's N-half 0, K-slabs 0..3 (x[0..31], from acc0's epilogue of layer l) into acc0, with acc1's epilogue of
-// layer l (x[32..63]) in chunks after them.  The wait of the first K-slab retires all of layer l.
+// layer l (x[32..63]) in chunks after them.  The wait of the first K-slab retires all of layer l; after layer 5
+// (release_feat) that is the last read of the feature buffer, which goes back to the helpers.
 template <int kFmt>
 __device__ __forceinline__ void level_rs_next_head(float (&acc0)[64], float (&acc1)[64], uint32_t (&x)[64], int l,
-                                                   const LevelRsCtx& k, RingPos& rp, PhaseClock& clk, float& d0,
-                                                   float& d1) {
+                                                   bool release_feat, const LevelRsCtx& k, RingPos& rp, PhaseClock& clk,
+                                                   float& d0, float& d1) {
   wgmma_fence_acc(acc0);
 #pragma unroll
   for (int c = 0; c < kEpiChunks; ++c) {
     EpiConsts e;
     level_epilogue_consts(e, l, 128, c, k.cq, k.gsp);
     level_mma_slab_rs<kFmt>(acc0, x, c, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+    if (c == 0 && release_feat && k.leader) mbar_arrive(k.feat_empty);
     if (c == 0) wgmma_fence_acc(acc1);
     level_epilogue_chunk_rs<kFmt>(acc1, e, l, 128, c, x, k, d0, d1);
     clk.mark(kPhEpilogue);
@@ -571,12 +601,179 @@ __device__ __forceinline__ void level_rs_layer(float (&acc0)[64], float (&acc1)[
   if (skip)
     for (int s = 8; s < num_k32(5); ++s)
       level_mma_slab<kFmt, false>(acc1, 5, s, 0u, f_u, ft_u, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
-  level_rs_next_head<kFmt>(acc0, acc1, x_out, l, k, rp, clk, d0, d1);
+  level_rs_next_head<kFmt>(acc0, acc1, x_out, l, skip, k, rp, clk, d0, d1);
 }
 
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// ---- the helper warps' per-ray work (ht = helper thread 0..95, hw = helper warp 0..2) ----
+// Ray prologue and features of `ray` into the feature buffer fbuf.  The prologue's global stores (fenceposts, view
+// bias) are read back by this CTA only, through L2 (ld.cg): by the helpers after the helper barrier, by the consumers
+// after feat_full.
+template <int kFmt, bool kX3>
+__device__ __forceinline__ void level_prepare_ray(const LevelParams& p, int64_t ray, uint8_t* fbuf, float* rs_scratch,
+                                                  int ht, int hw, int lane, PhaseClock& clk) {
+  if (p.t_mode != 0 || p.vb_mode != 0) {
+    if (hw == 0) {
+      float* t_ray = p.t + ray * (kN + 1);
+      if (p.t_mode == 1) {  // coarse fenceposts (bit-identical to coarse_t_kernel)
+        const float nr = __ldg(p.near + ray), fr = __ldg(p.far + ray);
+        const bool jit = draws_active(p.t_rand);
+        for (int j = lane; j <= kN; j += 32)
+          __stcg(t_ray + j, coarse_fencepost(nr, fr, j, kN, p.disparity, jit,
+                                             jit ? draw_uniform(p.t_rand, ray, j, kN + 1) : 0.f));
+      } else if (p.t_mode == 2) {
+        resample_warp_lean<true>(p.t_prev + ray * (kN + 1), p.w_prev + ray * kN, kN, kN + 1, p.randomized,
+                                 p.u_jitter, ray, p.resample_padding, rs_scratch, t_ray,
+                                 p.inds ? p.inds + ray * (kN + 1) : nullptr, lane);
+      }
+    } else if (hw == 1 && p.vb_mode == 1) {
+      // per-ray view-layer bias  b[n] + W[n, 256:283] . pos_enc(viewdir)   (models/mip.py:353-363,
+      // models/mip_nerf.py:106-108): lane f < 27 owns encoding element f, lane owns outputs n = lane + 32 j
+      float enc = 0.f;
+      if (lane < kViewDim) {
+        if (lane < 3) {
+          enc = __ldg(p.viewdirs + ray * 3 + lane);  // append_identity
+        } else {
+          const int gidx = lane - 3, is_cos = gidx >= 12, h = is_cos ? gidx - 12 : gidx;  // scale-major, then xyz
+          const float y = __fmul_rn(__ldg(p.viewdirs + ray * 3 + h % 3), __int_as_float((127 + h / 3) << 23));
+          enc = sinf(is_cos ? __fadd_rn(y, MIPNERF_HALF_PI_F32) : y);
+        }
+      }
+      const float* wt = reinterpret_cast<const float*>(p.wimage + kViewDirOffset);  // [27][128] | bias[128]
+      float acc[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[j] = __ldg(wt + kViewDim * kCond + lane + 32 * j);
+#pragma unroll
+      for (int k = 0; k < kViewDim; ++k) {
+        const float e = __shfl_sync(0xffffffffu, enc, k);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[j] = fmaf(__ldg(wt + k * kCond + lane + 32 * j), e, acc[j]);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) __stcg(p.view_bias + ray * kCond + lane + 32 * j, acc[j]);
+    }
+    __threadfence_block();
+    clk.mark(kPhPrologue);
+    named_bar_sync(kHelperBar, kHelperThreads);
+    clk.mark(kPhBarrier);
+  }
+  // Gaussians + IPE features: 128 rows x 3 parts of two 8-feature groups = 384 units, four per helper thread; a warp's
+  // 32 units share their part
+  RayGeom g{};
+  if (!p.feat_in) g = load_ray_geom(p.origins, p.directions, p.radii, ray);
+#pragma unroll 1
+  for (int u = ht; u < 3 * kN; u += kHelperThreads) {
+    const int row = u & (kN - 1), part = u / kN;
+    float t0 = 0.f, t1 = 0.f;
+    if (!p.feat_in) t0 = __ldcg(p.t + ray * (kN + 1) + row), t1 = __ldcg(p.t + ray * (kN + 1) + row + 1);
+    ipe_row_group<kFmt, kX3>(p, g, ray, row, t0, t1, fbuf, 2 * part, 2 * part + 2);
+  }
+  fence_proxy_async_smem();  // the features are read by wgmma (async proxy)
+  clk.mark(kPhIpe);
+}
+
+// Activations + compositing of `ray` from its raw heads hd[128][4] (or, in MLP-only mode, the raw heads out), with the
+// summation order of a thread-per-row warpgroup: rows in four chunks of 32, chunk q on helper warp q % 3, each chunk
+// scanned / reduced within its warp, the chunks' carries and partial sums added in chunk order.  Each helper thread
+// arrives on heads_empty once it has read its rows' heads.
+__device__ __forceinline__ void level_composite_ray(const LevelParams& p, int64_t ray, const float* hd,
+                                                    uint64_t* heads_empty, float* cs, float* ps, int ht, int hw,
+                                                    int lane, PhaseClock& clk) {
+  if (p.raw_rgb_out) {  // MLP-only mode: hand back the raw heads (models/mip_nerf.py:98,110)
+    for (int row = ht; row < kN; row += kHelperThreads) {
+      const float4 h4 = *reinterpret_cast<const float4*>(hd + row * 4);
+      const int64_t sidx = ray * kN + row;
+      p.raw_rgb_out[sidx * 3 + 0] = h4.y + c_small.b_color[0];
+      p.raw_rgb_out[sidx * 3 + 1] = h4.z + c_small.b_color[1];
+      p.raw_rgb_out[sidx * 3 + 2] = h4.w + c_small.b_color[2];
+      p.raw_density_out[sidx] = h4.x + c_small.b_density;
+    }
+    mbar_arrive(heads_empty);
+    clk.mark(kPhComposite);
+    return;
+  }
+  const float* t_ray = p.t + ray * (kN + 1);
+  const float dx = __ldg(p.directions + ray * 3), dy = __ldg(p.directions + ray * 3 + 1),
+              dz = __ldg(p.directions + ray * 3 + 2);
+  const float dnorm = sqrtf(dx * dx + dy * dy + dz * dz);
+  constexpr int kChunksPerWarp = 2;  // chunks hw, hw + 3
+  float dd[kChunksPerWarp], excl[kChunksPerWarp], crgb[kChunksPerWarp][3], tmid[kChunksPerWarp];
+#pragma unroll
+  for (int k = 0; k < kChunksPerWarp; ++k) {
+    const int q = hw + 3 * k, row = 32 * q + lane;
+    if (q >= 4) break;
+    const float4 h4 = *reinterpret_cast<const float4*>(hd + row * 4);
+    const int64_t sidx = ray * kN + row;
+    float raw_dens = h4.x + c_small.b_density;
+    if (draws_active(p.dnoise)) raw_dens = noisy_raw_density(raw_dens, p.dnoise, ray, row);  // models/mip_nerf.py:232-233
+    if (p.raw_rgb_keep) {  // training: the raw heads as well (render_backward recomputes the rest; the density head
+      p.raw_rgb_keep[sidx * 3 + 0] = h4.y + c_small.b_color[0];  // WITH its noise, so that softplus' is taken at the
+      p.raw_rgb_keep[sidx * 3 + 1] = h4.z + c_small.b_color[1];  // same point)
+      p.raw_rgb_keep[sidx * 3 + 2] = h4.w + c_small.b_color[2];
+      p.raw_density_keep[sidx] = raw_dens;
+    }
+    const float t0 = __ldcg(t_ray + row), t1 = __ldcg(t_ray + row + 1);
+    const float density = density_activation(raw_dens, p.density_bias);
+    crgb[k][0] = rgb_activation(h4.y + c_small.b_color[0], p.rgb_scale, p.rgb_padding);
+    crgb[k][1] = rgb_activation(h4.z + c_small.b_color[1], p.rgb_scale, p.rgb_padding);
+    crgb[k][2] = rgb_activation(h4.w + c_small.b_color[2], p.rgb_scale, p.rgb_padding);
+    tmid[k] = 0.5f * (t0 + t1);
+    dd[k] = density * ((t1 - t0) * dnorm);
+    float incl = dd[k];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const float n = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += n;
+    }
+    excl[k] = __shfl_up_sync(0xffffffffu, incl, 1);
+    if (lane == 0) excl[k] = 0.f;
+    if (lane == 31) cs[q] = incl;
+  }
+  mbar_arrive(heads_empty);
+  clk.mark(kPhComposite);
+  named_bar_sync(kHelperBar, kHelperThreads);
+  clk.mark(kPhBarrier);
+#pragma unroll
+  for (int k = 0; k < kChunksPerWarp; ++k) {
+    const int q = hw + 3 * k;
+    if (q >= 4) break;
+    float before = 0.f;
+    for (int qq = 0; qq < q; ++qq) before += cs[qq];
+    const float w = -expm1f(-dd[k]) * expf(-(before + excl[k]));
+    p.weights[ray * kN + 32 * q + lane] = w;
+    const float pr = warp_sum(w * crgb[k][0]), pg = warp_sum(w * crgb[k][1]), pb = warp_sum(w * crgb[k][2]),
+                pw = warp_sum(w), pd = warp_sum(w * tmid[k]);
+    if (lane == 0) {
+      float* dst = ps + q * 8;
+      dst[0] = pr, dst[1] = pg, dst[2] = pb, dst[3] = pw, dst[4] = pd;
+    }
+  }
+  clk.mark(kPhComposite);
+  named_bar_sync(kHelperBar, kHelperThreads);
+  clk.mark(kPhBarrier);
+  if (ht == 0) {
+    float s[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int qq = 0; qq < 4; ++qq)
+      for (int k = 0; k < 5; ++k) s[k] += ps[qq * 8 + k];
+    const float t_first = __ldcg(t_ray), t_last = __ldcg(t_ray + kN);
+    float d = s[4];
+    if (isnan(d)) d = 0.f;
+    else if (isinf(d)) d = d > 0 ? 3.4028234663852886e38f : -3.4028234663852886e38f;
+    d = fminf(fmaxf(d, t_first), t_last);
+    const float bg = p.white_bkgd ? 1.0f - s[3] : 0.f;
+    p.comp_rgb[ray * 3 + 0] = s[0] + bg;
+    p.comp_rgb[ray * 3 + 1] = s[1] + bg;
+    p.comp_rgb[ray * 3 + 2] = s[2] + bg;
+    p.distance[ray] = d;
+    p.acc[ray] = s[3];
+  }
+  clk.mark(kPhComposite);
+  named_bar_sync(kHelperBar, kHelperThreads);  // ht 0 has consumed ps / everyone cs before the next ray reuses them
+  clk.mark(kPhBarrier);
 }
 
 template <int kFmt, bool kX3>
@@ -590,10 +787,14 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   uint8_t* sW = smem + Lay::kW;
   uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + Lay::kMisc);  // [kStages] producer -> consumers (tx bytes)
   uint64_t* w_empty = w_full + Lay::kStages;                           // [kStages] consumers (2 arrives) -> producer
-  float* heads = reinterpret_cast<float*>(w_empty + Lay::kStages);     // [2][128][4] raw density, rgb dots
-  float* cs = heads + 2 * kN * 4;                                      // [4] scan carries
-  float* ps = cs + 4;                                                  // [4][8] partial sums
-  float* rs_scratch = ps + 32;                                         // [129] resampler scratch
+  uint64_t* feat_full = w_empty + Lay::kStages;     // [kFeatBufs] helpers (kHelperThreads arrives) -> consumers
+  uint64_t* feat_empty = feat_full + Lay::kFeatBufs;  // [kFeatBufs] consumers (2 arrives) -> helpers
+  uint64_t* heads_full = feat_empty + Lay::kFeatBufs;  // [2] consumers (kHeadsWriters arrives) -> helpers
+  uint64_t* heads_empty = heads_full + 2;              // [2] helpers (kHelperThreads arrives) -> consumers
+  float* heads = reinterpret_cast<float*>(heads_empty + 2);  // [2][128][4] raw density, rgb dots
+  float* cs = heads + 2 * kN * 4;                            // [4] scan carries
+  float* ps = cs + 4;                                        // [4][8] partial sums
+  float* rs_scratch = ps + 32;                               // [129] resampler scratch
   unsigned long long* phase_rows = reinterpret_cast<unsigned long long*>(smem + Lay::kPhase);
   const int phase_slot = p.t_mode == 2 ? 1 : 0;
   PhaseClock clk;
@@ -603,14 +804,48 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       mbar_init(&w_full[i], 1);
       mbar_init(&w_empty[i], 2);
     }
+    for (int i = 0; i < Lay::kFeatBufs; ++i) {
+      mbar_init(&feat_full[i], kHelperThreads);
+      mbar_init(&feat_empty[i], 2);
+    }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&heads_full[i], kHeadsWriters);
+      mbar_init(&heads_empty[i], kHelperThreads);
+    }
     fence_mbar_init();
   }
   __syncthreads();
 
   if (warp >= 8) {
-    // ============================ weight producer (warp 8; warps 9-11 only give their registers away) ============
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    if (warp == 8 && lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(kProducerRegs) : "memory");
+    if (warp >= kHelperWarp0) {
+      // ============================ helpers (warps 9-11): a two-stage ray pipeline ============================
+      // prepare ray i (into feature buffer i % kFeatBufs, once the consumers are done with its previous ray), then
+      // composite ray i - 1; the consumers meanwhile run the layers of ray i - 1 and then ray i.
+      const int ht = tid - 32 * kHelperWarp0, hw = warp - kHelperWarp0;
+      clk.begin(phase_rows + 3 * kNumPhases, ht == 0);
+      for (int64_t ray = blockIdx.x, i = 0;; ray += gridDim.x, ++i) {
+        const bool more = ray < p.num_rays;
+        if (more) {
+          const int fb = (int)(i % Lay::kFeatBufs);
+          mbar_wait(&feat_empty[fb], ((uint32_t)(i / Lay::kFeatBufs) & 1u) ^ 1u);
+          clk.mark(kPhFeatEmpty);
+          level_prepare_ray<kFmt, kX3>(p, ray, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane, clk);
+          mbar_arrive(&feat_full[fb]);
+        }
+        if (i > 0) {  // ray - gridDim.x, the (i - 1)-th ray of the CTA
+          const int par = (int)((i - 1) & 1);
+          mbar_wait(&heads_full[par], (uint32_t)((i - 1) >> 1) & 1u);
+          clk.mark(kPhHeadsFull);
+          level_composite_ray(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], cs, ps, ht, hw, lane, clk);
+        }
+        if (!more) break;
+      }
+      clk.end(phase_slot, 3);
+      return;
+    }
+    // ============================ weight producer (warp 8, one lane) ============================
+    if (lane == 0) {
       clk.begin(phase_rows + 2 * kNumPhases, true);
       int st = 0;
       uint32_t ph = 0;
@@ -640,83 +875,27 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   }
 
   // ============================ consumer warpgroups ============================
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(kConsumerRegs) : "memory");
   const int wg = warp >> 2, t = tid & 127, wq = warp & 3;
   const int r0 = 64 * wg + 16 * wq + (lane >> 2);  // accumulator rows r0, r0 + 8 of this thread
   const int cq = 2 * (lane & 3);                   // and columns 8 j + cq, + 1
   const bool leader = t == 0;
   const SmallParams* __restrict__ gsp = reinterpret_cast<const SmallParams*>(p.wimage + kSmallOffset);
   const uint32_t a_u = smem_u32(sA) + (uint32_t)wg * 64u * 128u;
-  const uint32_t f_u = smem_u32(sF) + (uint32_t)wg * 64u * 128u;
-  const uint32_t ft_u = smem_u32(sF) + kStageBytes + (uint32_t)wg * 64u * 64u;
   const uint32_t w_u = smem_u32(sW);
   const uint64_t dump_policy = p.act_dump ? l2_policy_evict_first() : 0ull;  // the dump must not evict the weights
   bool dump_pending = false;
   RingPos rp{0, 0u, -1};
-  int par = 0;
   clk.begin(phase_rows + wg * kNumPhases, leader);
-  for (int64_t ray = blockIdx.x; ray < p.num_rays; ray += gridDim.x, par ^= 1) {
-    if (p.t_mode != 0 || p.vb_mode != 0) {
-      // ---- ray prologue (warp 0); its global stores are read back by this CTA only, through L2 (ld.cg)
-      if (warp == 0) {
-        float* t_ray = p.t + ray * (kN + 1);
-        if (p.t_mode == 1) {  // coarse fenceposts (bit-identical to coarse_t_kernel)
-          const float nr = __ldg(p.near + ray), fr = __ldg(p.far + ray);
-          const bool jit = draws_active(p.t_rand);
-          for (int j = lane; j <= kN; j += 32)
-            __stcg(t_ray + j, coarse_fencepost(nr, fr, j, kN, p.disparity, jit,
-                                               jit ? draw_uniform(p.t_rand, ray, j, kN + 1) : 0.f));
-        } else if (p.t_mode == 2) {
-          resample_warp_lean<true>(p.t_prev + ray * (kN + 1), p.w_prev + ray * kN, kN, kN + 1, p.randomized,
-                                   p.u_jitter, ray, p.resample_padding, rs_scratch, t_ray,
-                                   p.inds ? p.inds + ray * (kN + 1) : nullptr, lane);
-        }
-        if (p.vb_mode == 1) {
-          // per-ray view-layer bias  b[n] + W[n, 256:283] . pos_enc(viewdir)   (models/mip.py:353-363,
-          // models/mip_nerf.py:106-108): lane f < 27 owns encoding element f, lane owns outputs n = lane + 32 j
-          float enc = 0.f;
-          if (lane < kViewDim) {
-            if (lane < 3) {
-              enc = __ldg(p.viewdirs + ray * 3 + lane);  // append_identity
-            } else {
-              const int gidx = lane - 3, is_cos = gidx >= 12, h = is_cos ? gidx - 12 : gidx;  // scale-major, then xyz
-              const float y = __fmul_rn(__ldg(p.viewdirs + ray * 3 + h % 3), __int_as_float((127 + h / 3) << 23));
-              enc = sinf(is_cos ? __fadd_rn(y, MIPNERF_HALF_PI_F32) : y);
-            }
-          }
-          const float* wt = reinterpret_cast<const float*>(p.wimage + kViewDirOffset);  // [27][128] | bias[128]
-          float acc[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc[j] = __ldg(wt + kViewDim * kCond + lane + 32 * j);
-#pragma unroll
-          for (int k = 0; k < kViewDim; ++k) {
-            const float e = __shfl_sync(0xffffffffu, enc, k);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) acc[j] = fmaf(__ldg(wt + k * kCond + lane + 32 * j), e, acc[j]);
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) __stcg(p.view_bias + ray * kCond + lane + 32 * j, acc[j]);
-        }
-        __threadfence_block();
-        clk.mark(kPhPrologue);
-      }
-      named_bar_sync(4, 256);
-      clk.mark(kPhBarrier);
-    }
-    {  // ---- Gaussians + IPE features of this warpgroup's rows: two threads per row, three 8-feature groups each
-      const int row = 64 * wg + (t & 63), part = t >> 6;
-      RayGeom g{};
-      float t0 = 0.f, t1 = 0.f;
-      if (!p.feat_in) {
-        g = load_ray_geom(p.origins, p.directions, p.radii, ray);
-        t0 = __ldcg(p.t + ray * (kN + 1) + row), t1 = __ldcg(p.t + ray * (kN + 1) + row + 1);
-      }
-      ipe_row_group<kFmt, kX3>(p, g, ray, row, t0, t1, sF, 3 * part, 3 * part + 3);
-    }
-    fence_proxy_async_smem();
-    clk.mark(kPhIpe);
-    named_bar_sync(1 + wg, 128);
-    clk.mark(kPhBarrier);
+  for (int64_t ray = blockIdx.x, i = 0; ray < p.num_rays; ray += gridDim.x, ++i) {
+    // the ray's feature buffer and raw-heads parity, and their mbarrier phases
+    const int fb = (int)(i % Lay::kFeatBufs), par = (int)(i & 1);
+    const uint32_t fph = (uint32_t)(i / Lay::kFeatBufs) & 1u, hph = (uint32_t)(i >> 1) & 1u;
+    // this warpgroup's rows of the ray's feature buffer (SW128 slab, SW64 tail)
+    const uint32_t f_u = smem_u32(sF) + (uint32_t)fb * Lay::kFBuf + (uint32_t)wg * 64u * 128u;
+    const uint32_t ft_u = smem_u32(sF) + (uint32_t)fb * Lay::kFBuf + kStageBytes + (uint32_t)wg * 64u * 64u;
+    mbar_wait(&feat_full[fb], fph);
+    clk.mark(kPhFeatFull);
 
     float d0 = 0.f, d1 = 0.f;  // density head, rows r0 / r0 + 8 (partial over this thread's columns)
     float rgb[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
@@ -750,7 +929,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       // and acc1's the next layer's K-slabs 0..3.  Layer 0 and layer 5's K-slabs 8..10 read the feature tile; layer 0
       // has three K-slabs, so its acc0 chunks follow K-slabs 0, 1, 2, 2.  The training forward's activation tiles go
       // out from the epilogue's registers.
-      const LevelRsCtx k{f_u, ft_u, w_u, w_full, w_empty, gsp,
+      const LevelRsCtx k{f_u, ft_u, w_u, w_full, w_empty, &feat_empty[fb], gsp,
                          p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
                          (size_t)p.dump_tiles * kABytes, dump_policy, r0, cq, leader};
       uint32_t xa[64], xb[64];
@@ -765,7 +944,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
         level_epilogue_chunk_rs<kFmt>(acc0, e, 0, 0, c, xb, k, d0, d1);
         clk.mark(kPhEpilogue);
       }
-      level_rs_next_head<kFmt>(acc0, acc1, xb, 0, k, rp, clk, d0, d1);
+      level_rs_next_head<kFmt>(acc0, acc1, xb, 0, false, k, rp, clk, d0, d1);
 #pragma unroll 1
       for (int l = 1; l < 9; l += 2) {
         level_rs_layer<kFmt, true>(acc0, acc1, xb, xa, l, k, rp, clk, d0, d1);
@@ -819,6 +998,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
           level_epilogue_consts(e, l, 128, c, cq, gsp);
           if (c < kEpiChunks - 1) {
             level_mma_slab<kFmt, kX3>(acc0, l + 1, c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+            if (c == 0 && l == 5 && leader) mbar_arrive(&feat_empty[fb]);  // layer 5's skip slabs have retired
             if (c == 0) wgmma_fence_acc(acc1);
           }
           level_epilogue_chunk<kFmt, kX3>(acc1, e, l, 128, c, r0, cq, sA, gsp, d0, d1);
@@ -882,89 +1062,17 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
     d0 = quad_sum(d0), d1 = quad_sum(d1);
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) rgb[0][ch] = quad_sum(rgb[0][ch]), rgb[1][ch] = quad_sum(rgb[1][ch]);
-    float* hd = heads + par * kN * 4;
+    // one thread per quad: wait until the helpers have composited the ray two back, store, hand the rows over
     if ((lane & 3) == 0) {
+      float* hd = heads + par * kN * 4;
+      clk.mark(kPhEpilogue);
+      mbar_wait(&heads_empty[par], hph ^ 1);
+      clk.mark(kPhBarrier);
       *reinterpret_cast<float4*>(hd + r0 * 4) = make_float4(d0, rgb[0][0], rgb[0][1], rgb[0][2]);
       *reinterpret_cast<float4*>(hd + (r0 + 8) * 4) = make_float4(d1, rgb[1][0], rgb[1][1], rgb[1][2]);
+      mbar_arrive(&heads_full[par]);
     }
     clk.mark(kPhEpilogue);
-    named_bar_sync(3, 256);
-    clk.mark(kPhBarrier);
-    if (wg == 1) continue;  // warpgroup 0 composites; warpgroup 1 goes on with the next ray
-
-    // ============ activations + compositing over the ray's 128 samples (warpgroup 0, thread = sample row) ============
-    const int row = t, q = wq;
-    const float4 h4 = *reinterpret_cast<const float4*>(hd + row * 4);
-    const int64_t sidx = ray * kN + row;
-    if (p.raw_rgb_out) {  // MLP-only mode: hand back the raw heads (models/mip_nerf.py:98,110)
-      p.raw_rgb_out[sidx * 3 + 0] = h4.y + c_small.b_color[0];
-      p.raw_rgb_out[sidx * 3 + 1] = h4.z + c_small.b_color[1];
-      p.raw_rgb_out[sidx * 3 + 2] = h4.w + c_small.b_color[2];
-      p.raw_density_out[sidx] = h4.x + c_small.b_density;
-      clk.mark(kPhComposite);
-      continue;
-    }
-    float raw_dens = h4.x + c_small.b_density;
-    if (draws_active(p.dnoise)) raw_dens = noisy_raw_density(raw_dens, p.dnoise, ray, row);  // models/mip_nerf.py:232-233
-    if (p.raw_rgb_keep) {  // training: the raw heads as well (render_backward recomputes the rest; the density head
-      p.raw_rgb_keep[sidx * 3 + 0] = h4.y + c_small.b_color[0];  // WITH its noise, so that softplus' is taken at the
-      p.raw_rgb_keep[sidx * 3 + 1] = h4.z + c_small.b_color[1];  // same point)
-      p.raw_rgb_keep[sidx * 3 + 2] = h4.w + c_small.b_color[2];
-      p.raw_density_keep[sidx] = raw_dens;
-    }
-    const float t0 = __ldcg(p.t + ray * (kN + 1) + row), t1 = __ldcg(p.t + ray * (kN + 1) + row + 1);
-    const float dx = __ldg(p.directions + ray * 3), dy = __ldg(p.directions + ray * 3 + 1),
-                dz = __ldg(p.directions + ray * 3 + 2);
-    const float dnorm = sqrtf(dx * dx + dy * dy + dz * dz);
-    const float density = density_activation(raw_dens, p.density_bias);
-    const float cr = rgb_activation(h4.y + c_small.b_color[0], p.rgb_scale, p.rgb_padding);
-    const float cg = rgb_activation(h4.z + c_small.b_color[1], p.rgb_scale, p.rgb_padding);
-    const float cb = rgb_activation(h4.w + c_small.b_color[2], p.rgb_scale, p.rgb_padding);
-    const float dd = density * ((t1 - t0) * dnorm);
-    float incl = dd;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const float n = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += n;
-    }
-    float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0) excl = 0.f;
-    if (lane == 31) cs[q] = incl;
-    clk.mark(kPhComposite);
-    named_bar_sync(1, 128);
-    clk.mark(kPhBarrier);
-    float before = 0.f;
-    for (int qq = 0; qq < q; ++qq) before += cs[qq];
-    const float w = -expm1f(-dd) * expf(-(before + excl));
-    p.weights[sidx] = w;
-    const float pr = warp_sum(w * cr), pg = warp_sum(w * cg), pb = warp_sum(w * cb), pw = warp_sum(w),
-                pd = warp_sum(w * (0.5f * (t0 + t1)));
-    if (lane == 0) {
-      float* dst = ps + q * 8;
-      dst[0] = pr, dst[1] = pg, dst[2] = pb, dst[3] = pw, dst[4] = pd;
-    }
-    clk.mark(kPhComposite);
-    named_bar_sync(1, 128);
-    clk.mark(kPhBarrier);
-    if (row == 0) {
-      float s[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-      for (int qq = 0; qq < 4; ++qq)
-        for (int k = 0; k < 5; ++k) s[k] += ps[qq * 8 + k];
-      const float t_first = __ldcg(p.t + ray * (kN + 1)), t_last = __ldcg(p.t + ray * (kN + 1) + kN);
-      float d = s[4];
-      if (isnan(d)) d = 0.f;
-      else if (isinf(d)) d = d > 0 ? 3.4028234663852886e38f : -3.4028234663852886e38f;
-      d = fminf(fmaxf(d, t_first), t_last);
-      const float bg = p.white_bkgd ? 1.0f - s[3] : 0.f;
-      p.comp_rgb[ray * 3 + 0] = s[0] + bg;
-      p.comp_rgb[ray * 3 + 1] = s[1] + bg;
-      p.comp_rgb[ray * 3 + 2] = s[2] + bg;
-      p.distance[ray] = d;
-      p.acc[ray] = s[3];
-    }
-    clk.mark(kPhComposite);
-    named_bar_sync(1, 128);  // row 0 has consumed ps / everyone cs before the next ray reuses them
-    clk.mark(kPhBarrier);
   }
   if (dump_pending && leader) bulk_store_wait_all();  // the last tile's store has left shared memory
   clk.mark(kPhEpilogue);
@@ -1402,7 +1510,7 @@ size_t tc_mlp_workspace_bytes(int64_t num_rays) { return (size_t)(num_rays > 0 ?
 
 #ifdef MIPNERF_LEVEL_PHASES
 // Instrumented builds only (tools/level_phases.py): copies the per-CTA phase cycles accumulated since the last call,
-// [2 slots][ctas][3 roles][phases] as uint64, into `out` and zeroes them.  Returns the phase count, or -1 on error.
+// [2 slots][ctas][4 roles][phases] as uint64, into `out` and zeroes them.  Returns the phase count, or -1 on error.
 extern "C" int mipnerf_b200_level_phases(unsigned long long* out, int* ctas) {
   using namespace mipnerf;
   *ctas = kPhaseMaxCtas;

@@ -3,8 +3,9 @@
 Builds the `phases` variant of the library (-DMIPNERF_LEVEL_PHASES: clock64 phase accounting in mlp_level_kernel), runs
 the benchmark's forward (4096 rays, xavier weights) in bf16 and fp16x3, and prints, per level launch and per role, the
 share of each phase in the role's cycles, averaged over CTAs, next to the GPU's name and power limit.  Phases a role
-never enters are left out: in bf16 / fp16 the layer loop has no barrier, so `barrier` counts only the waits around
-the feature tile, the ray prologue and the raw heads.
+never enters are left out: in bf16 / fp16 the consumers' layer loop has no barrier, so their `barrier` counts only the
+wait for a free raw-heads buffer; the helpers' `barrier` is their own named barrier (prologue -> features, the
+compositing scans).
 
     python tools/level_phases.py [--rays 4096] [--reps 20] [--precisions bf16,fp16x3] [--json OUT]
 
@@ -18,8 +19,9 @@ import subprocess
 import sys
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-PHASES = ["prologue", "ipe", "w_full_wait", "mma", "epilogue", "composite", "barrier", "w_empty_wait", "issue"]
-ROLES = ["consumer_wg0", "consumer_wg1", "producer"]
+PHASES = ["prologue", "ipe", "w_full_wait", "mma", "epilogue", "composite", "barrier", "w_empty_wait", "issue",
+          "feat_full_wait", "feat_empty_wait", "heads_full_wait"]
+ROLES = ["consumer_wg0", "consumer_wg1", "producer", "helpers"]
 LEVELS = ["level0", "level1"]
 
 
@@ -72,7 +74,7 @@ def main():
         torch.cuda.synchronize()
         nph = read(buf.ctypes.data_as(C.POINTER(C.c_ulonglong)), C.byref(max_ctas))
         assert nph == len(PHASES) + 1, nph
-        data = buf.reshape(2, max_ctas.value, 3, nph).astype(np.float64)
+        data = buf.reshape(2, max_ctas.value, len(ROLES), nph).astype(np.float64)
         run = {"forward_ms": start.elapsed_time(stop) / args.reps}
         for s, level in enumerate(LEVELS):
             d = data[s]
