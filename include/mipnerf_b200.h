@@ -185,8 +185,11 @@ size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_
  * above into `grads` (overwritten, or added to when `accumulate` != 0).  Replaces
  * `loss = training_step(...); loss.backward()` (models/nerf_system.py:95-121 + autograd).  Fenceposts carry
  * no gradient (stop_resample_grad=True semantics, models/mip.py:250-264).  precision FP32: every GEMM in fp32 FFMA
- * (the parity mode); BF16 / FP16: forward and dgrad GEMMs on wgmma with 16-bit operands, wgrad / heads / rendering
- * in fp32 (default 8x256 architecture only). */
+ * (the parity mode); BF16 / FP16: forward, dgrad and wgrad GEMMs of the 128- and 256-wide layers on wgmma with
+ * 16-bit operands, heads / rendering in fp32.  The fused step (level kernels + 16-bit activation tile images) runs for
+ * the level kernel's shapes (the default architecture and encodings, 128 samples) with at most two levels; other
+ * shapes with the default widths and encoding sizes (96-d IPE, 27-d view encoding) and net_depth <= 16 run per-layer
+ * GEMMs on fp32 activations. */
 int mipnerf_b200_forward_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* weights,
                                   const mipnerf_b200_rays* rays, int randomized, const float* t_rand,
                                   const float* u_jitter, int white_bkgd, int precision,
@@ -239,7 +242,8 @@ int mipnerf_b200_linear_tc(const float* x, const float* weight, const float* bia
 /* Stand-alone tensor-core weight gradient of one nn.Linear (what loss.backward() accumulates into layer.weight.grad /
  * layer.bias.grad, models/nerf_system.py:108-111):  dw[n, k1+k2] = dy[m,n]^T . [x1[m,k1] | x2[m / x2_row_div, k2]],
  * db[n] = column sums of dy; n in {128,256}, 16-bit operands rounded while staging, fp32 accumulation, per-slice
- * partials reduced in a fixed order (bit-reproducible).  x2 may be NULL (k2 = 0). */
+ * partials reduced in a fixed order (bit-reproducible).  x2 may be NULL (k2 = 0).  With k2 > 0, k1 must be a multiple
+ * of 256 (MIPNERF_B200_EUNSUPPORTED otherwise); dy must be 16-byte aligned (MIPNERF_B200_EINVAL otherwise). */
 size_t mipnerf_b200_wgrad_tc_scratch_bytes(int n, int k);
 int mipnerf_b200_wgrad_tc(const float* dy, int n, const float* x1, int k1, const float* x2, int k2, int x2_row_div,
                           int64_t m, float* dw, float* db, int precision, void* scratch, size_t scratch_bytes,

@@ -469,8 +469,8 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
   return s;
 }
 
-// The fused step needs the level kernels' architecture (8 x 256 trunk, 128 samples, ...) and at most two levels.
-// MIPNERF_B200_TRAIN_FUSED=0 keeps the per-layer tensor-core path (A/B runs).
+// The fused step needs the level kernels' architecture (8 x 256 trunk, 128 samples, ...) and at most two levels;
+// other shapes that train_tc_supported accepts take the per-layer tensor-core path.
 bool train_fused_supported(const mipnerf_b200_config* c, int precision) {
   return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_FP16) && mipnerf::tc_supported(c, precision) &&
          mipnerf::tc_default_degrees(c) &&  // the backward's tile images carry the full 96 / 27 encodings
@@ -735,12 +735,9 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
       CUDA_TRY(cudaMemsetAsync(grads[i].bias_grad, 0, sizeof(float) * l.out_features, st));
     }
 
-  {
-    const char* fused_env = getenv("MIPNERF_B200_TRAIN_FUSED");
-    if (tc && B > 0 && train_fused_supported(cfg, precision) && !(fused_env && fused_env[0] == '0'))
-      return forward_backward_fused(cfg, d, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision, src,
-                                    given_t, outs, grads, touched, workspace, st);
-  }
+  if (tc && B > 0 && train_fused_supported(cfg, precision))
+    return forward_backward_fused(cfg, d, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision, src,
+                                  given_t, outs, grads, touched, workspace, st);
   // ---- tensor-core mode: B operands of every forward / dgrad GEMM, packed once per call (the weights change every
   //      optimiser step).  fwd[i] = W_i[:, :k_main], fwd_skip[i] = W_i[:, 256:352], bwd[i] = W_i[:, :256]^T;
   //      slots depth / depth+1 hold the bottleneck and the view layer.
@@ -776,16 +773,14 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
       const mipnerf_b200_linear& vl0 = w->linears[depth + 2];
       CUDA_TRY(mipnerf::launch_view_bias_from_enc(s.venc, vl0.weight, vl0.bias, s.vrow, cnt, st));
     }
-    // tensor-core mode: wgrad partials on the tensor cores as well.  MIPNERF_B200_WGRAD_TC=0 keeps wgrad on the fp32
-    // FFMA tiles (A/B runs).
-    const char* wgrad_env = getenv("MIPNERF_B200_WGRAD_TC");
-    const bool wgrad_on_tc = !(wgrad_env && wgrad_env[0] == '0');
+    // tensor-core mode: the wgrad partials of the 128- and 256-wide layers on the tensor cores as well (dy comes from
+    // the 256-byte-aligned workspace carves, and an x2 always follows k1 = 256 columns); the two heads on fp32 FFMA
     auto wgrad = [&](int idx, const float* dy, const float* x1, int k1, const float* x2, int k2, int div) {
       const mipnerf_b200_linear& l = w->linears[idx];
-      if (tc && wgrad_on_tc && mipnerf::wgrad_tc_shape_ok(l.out_features)) {  // tensor-core partials + same reduction
+      if (tc && mipnerf::wgrad_tc_shape_ok(l.out_features)) {  // tensor-core partials + same reduction
         int slices = 0;
-        cudaError_t e2 = mipnerf::launch_wgrad_tc_partials(dy, l.out_features, x1, k1, k1, x2, k2, k2, div, s.part, m,
-                                                           mipnerf::kWgradMaxSlices, precision, &slices, st);
+        cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy, 0, l.out_features, x1, 0, k1, k1, x2, 0, k2, k2, div,
+                                                           s.part, m, mipnerf::kWgradMaxSlices, precision, &slices, st);
         if (e2 != cudaSuccess) return e2;
         e2 = mipnerf::launch_wgrad_reduce(s.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
                                           grads[idx].bias_grad, touched[idx] ? 1 : 0, st);
@@ -978,14 +973,18 @@ int mipnerf_b200_wgrad_tc(const float* dy, int n, const float* x1, int k1, const
                           void* stream) {
   if (m < 0 || k1 < 1 || k2 < 0 || !mipnerf::wgrad_tc_shape_ok(n))
     return fail(MIPNERF_B200_EUNSUPPORTED, "wgrad_tc: n in {128,256} (got n=%d)", n);
+  if (k2 > 0 && k1 % 256 != 0)  // no k tile of the kernel may straddle x1 and x2 (launch_wgrad_mn_partials)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "wgrad_tc: with x2, k1 must be a multiple of 256 (got k1=%d)", k1);
   if (precision != MIPNERF_B200_BF16 && precision != MIPNERF_B200_FP16)
     return fail(MIPNERF_B200_EINVAL, "wgrad_tc: precision must be BF16 or FP16");
   if (!dw || !db || (m > 0 && (!dy || !x1 || (k2 > 0 && !x2)))) return fail(MIPNERF_B200_EINVAL, "NULL tensor");
+  if (m > 0 && (reinterpret_cast<uintptr_t>(dy) & 15) != 0)  // dy rows are staged with float4 loads
+    return fail(MIPNERF_B200_EINVAL, "wgrad_tc: dy must be 16-byte aligned");
   const size_t need = mipnerf_b200_wgrad_tc_scratch_bytes(n, k1 + k2);
   if (!scratch || scratch_bytes < need) return fail(MIPNERF_B200_EWORKSPACE, "scratch %zu < %zu bytes", scratch_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
   int slices = 0;
-  CUDA_TRY(mipnerf::launch_wgrad_tc_partials(dy, n, x1, k1, k1, k2 > 0 ? x2 : nullptr, k2, k2, x2_row_div,
+  CUDA_TRY(mipnerf::launch_wgrad_mn_partials(dy, 0, n, x1, 0, k1, k1, k2 > 0 ? x2 : nullptr, 0, k2, k2, x2_row_div,
                                              static_cast<float*>(scratch), m, mipnerf::kWgradMaxSlices, precision,
                                              &slices, st));
   CUDA_TRY(mipnerf::launch_wgrad_reduce(static_cast<float*>(scratch), slices, n, k1 + k2, dw, db, 0, st));

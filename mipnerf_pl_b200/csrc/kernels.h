@@ -113,9 +113,6 @@ cudaError_t launch_linear_tc(const float* x, int ldx, const void* image, float* 
                              cudaStream_t st);
 
 bool wgrad_tc_shape_ok(int n_dim);
-cudaError_t launch_wgrad_tc_partials(const float* dy, int n_dim, const float* x1, int ld1, int k1, const float* x2,
-                                     int ld2, int k2, int x2_row_div, float* part, int64_t m, int max_slices,
-                                     int precision, int* slices_out, cudaStream_t st);
 cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, const void* x1, int x1_t16, int ld1, int k1,
                                      const void* x2, int x2_t16, int ld2, int k2, int x2_row_div, float* part,
                                      int64_t m, int max_slices, int precision, int* slices_out, cudaStream_t st,

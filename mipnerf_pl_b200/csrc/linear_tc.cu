@@ -11,8 +11,6 @@
 //     then warpgroup g issues the wgmma (M = 64, N = 128, K = 16) of rows 64 g.. and applies the epilogue from its
 //     register accumulators straight to global memory:  + bias[col]  + row_bias[row / row_div][col]  + prev[row][col]
 //     + r1[row]*r1w[col], ReLU, ReLU-mask by another activation (dgrad).
-#include <cstdlib>
-
 #include "kernels.h"
 #include "profile.h"
 #include "tc_common.cuh"
@@ -166,14 +164,19 @@ __global__ void __launch_bounds__(256, 1) linear_tc_kernel(const LinearTcParams 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// wgrad on the tensor core:  part[s][n][kg] = sum_{m in slice s} dY[m, n0+n] * Xc[m, kg0+kg],
-//   Xc = [X1 (k1 cols) | X2[m / x2_row_div] (k2 cols)], one CTA per (slice, 128-wide n tile, <=256-wide k tile).
-// The reduction index is the row m, so BOTH operands are needed "m-major"; they are transposed while staging:
-// thread t < 128 owns output row n = t of A, threads 128.. own columns of B; each reads its column of dY / Xc for the
-// 64 rows of a slab (a warp reads 128 contiguous bytes per row: coalesced) and writes eight 16-byte chunks of 8
-// consecutive m into the SW128 K-major slab.  Warpgroup g accumulates rows 64 g .. of the [128 x nk] partial in
-// registers over the whole slice (4 wgmma K steps per slab and 128-column chunk); the bias gradient (column sums of
-// dY) falls out of the A staging.  Partials have the layout wgrad_reduce_kernel expects.
+// wgrad on the tensor core:  part[s][n][kg] = sum_{m in slice s} dY[m, n] * Xc[m, kg],
+//   Xc = [X1 (k1 cols) | X2[m / x2_row_div] (k2 cols)], column K of each partial row = the bias gradient (column sums
+//   of dY): the layout wgrad_reduce_kernel expects.
+// The reduction index of dW = dY^T . X is the row m, and a row-major [m][col] tile IS the canonical "MN-major" wgmma
+// operand (transpose bits of the instruction): 64 consecutive columns (128 B) x 8 rows form one 128-byte-swizzle atom,
+// column blocks LBO apart, 8-row groups SBO apart.  Staging is therefore a straight copy: a warp reads one whole row
+// (1 KB, coalesced), rounds to 16 bit and stores one 16-byte chunk per lane at the swizzled position of the same row.
+//   grid (slices, 128-column k tiles); one CTA per SM covers ALL n_dim <= 256 output rows (warpgroup g: rows 128 g..,
+//   two M = 64 register accumulators), so dY is read once per k tile;
+//   warps 0-7 stage 64-row slabs into a 3-deep ring (tile-image operands arrive by bulk copy from warp 8), then run
+//   4 K-steps of wgmma per slab and free the stage (one arrive per warpgroup); after the last slab they write the
+//   partial rows from the accumulators and add up the bias gradient (column sums of dY, kept in fp32 by the thread
+//   that staged the column) in a fixed order.
 // ---------------------------------------------------------------------------------------------------------------
 struct WgradTcParams {
   const float* dy;  // [M, n_dim]
@@ -184,8 +187,8 @@ struct WgradTcParams {
   int ld2, k2, x2_row_div;
   float* part;      // [slices, n_dim, K + 1]
   int64_t m, slice_rows;
-  // second-generation kernel only: dy / x1 are 16-bit tile images (train_t16.cu) instead of fp32 row-major matrices;
-  // x1's / x2's image has ceil(k / 64) slabs per tile (x2 as an image: x2_row_div == 1).
+  // dy / x1 / x2 are 16-bit tile images (train_t16.cu) instead of fp32 row-major matrices; x1's / x2's image has
+  // ceil(k / 64) slabs per tile (x2 as an image: x2_row_div == 1).
   int dy_t16, x1_t16, x2_t16;
   // optional by-product when x1 is a 256-column tile image: its sign mask, [m][32 bytes], bit c of a row = x1[row][c] > 0.
   // The dgrad GEMM that follows needs exactly this (the ReLU mask of the layer input) and then reads 32 bytes per row
@@ -193,118 +196,6 @@ struct WgradTcParams {
   uint8_t* mask_out;
 };
 
-template <int kFmt>
-__global__ void __launch_bounds__(256, 1) wgrad_tc_kernel(const WgradTcParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-  uint8_t* sA = smem;        // [128 n x 64 m] 16 KB
-  uint8_t* sB = sA + 16384;  // [nk  x 64 m] <= 32 KB
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3;
-  const int K = p.k1 + p.k2;
-  const int n0 = blockIdx.y * 128, kg0 = blockIdx.z * 256;
-  const int nk = K - kg0 < 256 ? K - kg0 : 256;  // valid output columns of this k tile
-  const int nk_pad = (nk + 127) & ~127;         // wgmma N = 128 chunks (padding columns are staged as zeros)
-  const int64_t m_begin = (int64_t)blockIdx.x * p.slice_rows;
-  const int64_t m_end = (m_begin + p.slice_rows) < p.m ? (m_begin + p.slice_rows) : p.m;
-  float bsum = 0.f;
-  const int n = n0 + tid;  // threads 0..127 stage A row n (and keep its bias-gradient sum)
-  const bool n_ok = tid < 128 && n < p.n_dim;
-  auto xcol = [&](int64_t row, int c) -> float {  // Xc[row][c], zero outside
-    if (c < p.k1) return __ldg(p.x1 + row * (int64_t)p.ld1 + c);
-    if (c < K) return __ldg(p.x2 + (row / p.x2_row_div) * (int64_t)p.ld2 + (c - p.k1));
-    return 0.f;
-  };
-  float acc0[64], acc1[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) acc0[i] = 0.f, acc1[i] = 0.f;
-  const uint32_t a_u = smem_u32(sA) + (uint32_t)wg * 8192u, b_u = smem_u32(sB);
-  for (int64_t m0 = m_begin; m0 < m_end; m0 += 64) {
-    if (tid < 128) {
-      // ---- A: row n = tid, 64 consecutive m -> 8 chunks of 16 bytes
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int64_t row = m0 + half * 32 + i;
-          v[i] = (n_ok && row < m_end) ? __ldg(p.dy + row * (int64_t)p.n_dim + n) : 0.f;
-          bsum += v[i];
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          *reinterpret_cast<uint4*>(sA + sw128_offset(tid, (half * 4 + c) * 8)) =
-              make_uint4(pack2<kFmt>(v[c * 8], v[c * 8 + 1]), pack2<kFmt>(v[c * 8 + 2], v[c * 8 + 3]),
-                         pack2<kFmt>(v[c * 8 + 4], v[c * 8 + 5]), pack2<kFmt>(v[c * 8 + 6], v[c * 8 + 7]));
-      }
-    } else {
-      // ---- B: rows (output columns) tid - 128 and tid of this k tile
-      for (int rb = tid - 128; rb < nk_pad; rb += 128) {
-        const int col = kg0 + rb;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          float v[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int64_t row = m0 + half * 32 + i;
-            v[i] = (rb < nk && row < m_end) ? xcol(row, col) : 0.f;
-          }
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-            *reinterpret_cast<uint4*>(sB + sw128_offset(rb, (half * 4 + c) * 8)) =
-                make_uint4(pack2<kFmt>(v[c * 8], v[c * 8 + 1]), pack2<kFmt>(v[c * 8 + 2], v[c * 8 + 3]),
-                           pack2<kFmt>(v[c * 8 + 4], v[c * 8 + 5]), pack2<kFmt>(v[c * 8 + 6], v[c * 8 + 7]));
-        }
-      }
-    }
-    fence_proxy_async_smem();
-    __syncthreads();
-    wgmma_fence_acc(acc0);
-    wgmma_fence_acc(acc1);
-    wgmma_fence();
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      wgmma_m64n128k16<kFmt>(acc0, make_sw128_desc(a_u + 32u * j), make_sw128_desc(b_u + 32u * j), 1u);
-      if (nk_pad > 128)
-        wgmma_m64n128k16<kFmt>(acc1, make_sw128_desc(a_u + 32u * j), make_sw128_desc(b_u + 16384u + 32u * j), 1u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_acc(acc0);
-    wgmma_fence_acc(acc1);
-    __syncthreads();  // the slab has been consumed: it may be overwritten
-  }
-  // ---- partial sums of this slice
-  float* out = p.part + (size_t)blockIdx.x * p.n_dim * (K + 1);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int nr = n0 + 64 * wg + 16 * wq + (lane >> 2) + 8 * h;
-    if (nr >= p.n_dim) continue;
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int c = 8 * j + 2 * (lane & 3) + e;
-        if (c < nk) out[(size_t)nr * (K + 1) + kg0 + c] = acc0[4 * j + 2 * h + e];
-        if (128 + c < nk) out[(size_t)nr * (K + 1) + kg0 + 128 + c] = acc1[4 * j + 2 * h + e];
-      }
-  }
-  if (blockIdx.z == 0 && n_ok) out[(size_t)n * (K + 1) + K] = bsum;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// wgrad, second generation: NO transposition.  The reduction index of dW = dY^T . X is the row m, and a row-major
-// [m][col] tile IS the canonical "MN-major" wgmma operand (transpose bits of the instruction): 64 consecutive
-// columns (128 B) x 8 rows form one 128-byte-swizzle atom, column blocks LBO apart, 8-row groups SBO apart.  Staging
-// is therefore a straight copy: a warp reads one whole row (1 KB, coalesced), rounds to 16 bit and stores one 16-byte
-// chunk per lane at the swizzled position of the same row — no per-thread column walks, no 32-row register tiles.
-//   grid (slices, 128-column k tiles); one CTA per SM covers ALL n_dim <= 256 output rows (warpgroup g: rows 128 g..,
-//   two M = 64 register accumulators), so dY is read once per k tile;
-//   warps 0-7 stage 64-row slabs into a 3-deep ring (tile-image operands arrive by bulk copy from warp 8), then run
-//   4 K-steps of wgmma per slab and free the stage (one arrive per warpgroup); after the last slab they write the
-//   partial rows from the accumulators and add up the bias gradient (column sums of dY, kept in fp32 by the thread
-//   that staged the column) in a fixed order.
-// ---------------------------------------------------------------------------------------------------------------
 constexpr int kWgStages = 3;
 constexpr int kWgSlab = 64;                    // rows (reduction steps) per stage
 constexpr uint32_t kWgOperand = kWgSlab * 512; // 64 rows x 256 cols x 2 B
@@ -614,8 +505,10 @@ cudaError_t launch_linear_tc(const float* x, int ldx, const void* image, float* 
 
 bool wgrad_tc_shape_ok(int n_dim) { return n_dim == 128 || n_dim == 256; }
 
-// Second-generation wgrad partials.  dy / x1 are fp32 row-major matrices, or (dy_t16 / x1_t16 != 0) 16-bit tile images
-// (then m must be a multiple of 128 and x1 has k1 / 64 slabs per tile); x2 is fp32 row-major.
+// Wgrad partials only; the caller runs the fixed-order reduction (train_kernels.cu) afterwards with the slice count
+// returned in *slices_out.  dy / x1 / x2 are fp32 row-major matrices (an fp32 dy 16-byte aligned), or (*_t16 != 0)
+// 16-bit tile images (then m must be a multiple of 128 and x1 has k1 / 64 slabs per tile).  No k tile may straddle
+// x1 and x2: k2 > 0 needs k1 % 256 == 0.
 cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, const void* x1, int x1_t16, int ld1, int k1,
                                      const void* x2, int x2_t16, int ld2, int k2, int x2_row_div, float* part,
                                      int64_t m, int max_slices, int precision, int* slices_out, cudaStream_t st,
@@ -640,13 +533,13 @@ cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, cons
   if (slices < 1) slices = 1;
   int64_t slice_rows = (m + slices - 1) / slices;
   slice_rows = (slice_rows + kWgSlab - 1) / kWgSlab * kWgSlab;
-  static bool attr2[2] = {false, false};
+  static bool attr[2] = {false, false};
   const size_t smem = 1024 + (size_t)kWgStages * kWgStage + 8 * 256 * sizeof(float) + 128;
-  if (!attr2[fmt]) {
+  if (!attr[fmt]) {
     cudaError_t e = fmt ? cudaFuncSetAttribute(wgrad_mn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
                         : cudaFuncSetAttribute(wgrad_mn_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    attr2[fmt] = true;
+    attr[fmt] = true;
   }
   WgradTcParams p{};
   p.dy = static_cast<const float*>(dy), p.n_dim = n_dim, p.x1 = static_cast<const float*>(x1), p.ld1 = ld1, p.k1 = k1;
@@ -657,53 +550,6 @@ cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, cons
   LaunchScope scope(kKernWgradTc, st);
   if (fmt) wgrad_mn_kernel<1><<<grid, 288, smem, st>>>(p);
   else wgrad_mn_kernel<0><<<grid, 288, smem, st>>>(p);
-  *slices_out = (int)slices;
-  return cudaGetLastError();
-}
-
-// Partials only; the caller runs the fixed-order reduction (train_kernels.cu) afterwards.  Returns the slice count.
-// MIPNERF_B200_WGRAD_TC=1 selects the first-generation (transposing) kernel for A/B runs.
-cudaError_t launch_wgrad_tc_partials(const float* dy, int n_dim, const float* x1, int ld1, int k1, const float* x2,
-                                     int ld2, int k2, int x2_row_div, float* part, int64_t m, int max_slices,
-                                     int precision, int* slices_out, cudaStream_t st) {
-  if (!x2) x2 = x1, ld2 = ld1, k2 = 0;
-  if (x2_row_div < 1) x2_row_div = 1;
-  const int K = k1 + k2;
-  if (g_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  const int fmt = precision == 1 ? 1 : 0;
-  const char* gen_env = getenv("MIPNERF_B200_WGRAD_TC");  // read per call: the tests flip it inside one process
-  const int generation = (gen_env && gen_env[0] == '1') ? 1 : 2;
-  const bool mn_ok = (k2 == 0 || k1 % 256 == 0) && (n_dim & 7) == 0 && (reinterpret_cast<uintptr_t>(dy) & 15) == 0;
-  if (generation == 2 && mn_ok)
-    return launch_wgrad_mn_partials(dy, 0, n_dim, x1, 0, ld1, k1, x2, 0, ld2, k2, x2_row_div, part, m, max_slices,
-                                    precision, slices_out, st);
-  const int n_tiles = (n_dim + 127) / 128, k_tiles = (K + 255) / 256;
-  int64_t slices = ((int64_t)g_sms + n_tiles * k_tiles - 1) / (n_tiles * k_tiles);  // one wave of CTAs
-  const int64_t by_rows = (m + 63) / 64;
-  if (slices > by_rows) slices = by_rows;
-  if (slices > max_slices) slices = max_slices;
-  if (slices < 1) slices = 1;
-  int64_t slice_rows = (m + slices - 1) / slices;
-  slice_rows = (slice_rows + 63) / 64 * 64;
-  static bool attr[2] = {false, false};
-  const size_t smem = 1024 + 16384 + 32768 + 64;
-  if (!attr[fmt]) {
-    cudaError_t e = fmt ? cudaFuncSetAttribute(wgrad_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                        : cudaFuncSetAttribute(wgrad_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    attr[fmt] = true;
-  }
-  WgradTcParams p{};
-  p.dy = dy, p.n_dim = n_dim, p.x1 = x1, p.ld1 = ld1, p.k1 = k1, p.x2 = x2, p.ld2 = ld2, p.k2 = k2;
-  p.x2_row_div = x2_row_div, p.part = part, p.m = m, p.slice_rows = slice_rows;
-  dim3 grid((unsigned)slices, (unsigned)n_tiles, (unsigned)k_tiles);
-  LaunchScope scope(kKernWgradTc, st);
-  if (fmt) wgrad_tc_kernel<1><<<grid, 256, smem, st>>>(p);
-  else wgrad_tc_kernel<0><<<grid, 256, smem, st>>>(p);
   *slices_out = (int)slices;
   return cudaGetLastError();
 }

@@ -274,17 +274,15 @@ def test_linear_tc_matches_fp32_linear(precision, tol, n, k):
     assert float((y.double() - exact).abs().max()) <= tol * scale
 
 
-@pytest.mark.parametrize("generation", ["1", "2"])
 @pytest.mark.parametrize("precision", ["bf16", "fp16"])
 @pytest.mark.parametrize("n,k1,k2,div,m", [(256, 256, 0, 1, 128 * 173 + 37), (256, 96, 0, 1, 9000), (256, 256, 96, 1, 20000),
                                            (128, 256, 27, 128, 128 * 100), (256, 256, 0, 1, 40)])
-def test_wgrad_tc_matches_rounded_operands(precision, n, k1, k2, div, m, generation, monkeypatch):
+def test_wgrad_tc_matches_rounded_operands(precision, n, k1, k2, div, m):
     """dW = dY^T [X1 | X2[row / div]] and db = colsum(dY) on the tensor cores: against the exact product of the SAME 16-bit
     operands (isolates layout / descriptor bugs from rounding: only the fp32 accumulation order differs), ragged row
     counts, the skip concat (K = 352 -> two k tiles), the per-ray view-direction operand, fewer rows than one slab.
-    generation 2 = both operands MN-major straight from their row-major tiles, 1 = the transposing kernel."""
+    Both operands are MN-major, staged straight from their row-major tiles."""
     from mipnerf_pl_b200 import _cabi
-    monkeypatch.setenv("MIPNERF_B200_WGRAD_TC", generation)
     gen = torch.Generator(device="cpu").manual_seed(5)
     dy = torch.randn(m, n, generator=gen).to(DEV)
     x1 = torch.randn(m, k1, generator=gen).to(DEV)
@@ -345,32 +343,41 @@ def test_fused_step_relu_bitmask_is_exact(precision, monkeypatch):
         assert torch.equal(grads["0"][k], grads["1"][k]), k
 
 
-@pytest.mark.parametrize("wgrad_tc", ["0", "1", "2", "fused"])
+# The tensor-core training step takes one of two paths, chosen by the config: the fused step for the level kernel's
+# shapes, per-layer GEMMs (linear_tc_kernel, wgrad_mn_kernel on fp32 operands) for every other shape it covers.
+TC_STEP_SHAPES = {"fused": {}, "per-layer": {"num_samples": 64, "num_levels": 3}}
+
+
+@pytest.mark.parametrize("path", list(TC_STEP_SHAPES))
 @pytest.mark.parametrize("precision,loss_tol,grad_tol", [("bf16", 5e-3, 1.5e-1), ("fp16", 1e-3, 1.5e-1)])
-def test_tensor_core_training_mode_tracks_fp32(precision, loss_tol, grad_tol, wgrad_tc, monkeypatch):
+def test_tensor_core_training_mode_tracks_fp32(precision, loss_tol, grad_tol, path):
     """precision='bf16'|'fp16': forward and dgrad GEMMs on the tensor cores.  Loss and every gradient tensor stay within
-    the operand-rounding distance of the fp32 step (which is pinned to the reference's autograd).  That distance is
-    NOT the operand epsilon for the trunk: an activation perturbed by eps flips the ReLU masks of a fraction ~eps of
-    the units, each flip adds/removes a full-size term, so the gradient moves by ~sqrt(eps) (observed: 5e-2 for fp16
-    on layers.0, 6e-2 for bf16) — the same mechanism that limits the fp32 trunk bar to 2e-3."""
-    # "fused" (default): forward = the level kernels with the activation dump, backward on 16-bit tile images;
-    # otherwise the per-layer tensor-core path with "2": MN-major wgmma wgrad, "1": transposing wgmma wgrad,
-    # "0": fp32 FFMA wgrad
-    monkeypatch.setenv("MIPNERF_B200_TRAIN_FUSED", "1" if wgrad_tc == "fused" else "0")
-    if wgrad_tc != "fused":
-        monkeypatch.setenv("MIPNERF_B200_WGRAD_TC", wgrad_tc)
+    the operand-rounding distance of the fp32 step of the same model (which is pinned to the reference's autograd).
+    That distance is NOT the operand epsilon for the trunk: an activation perturbed by eps flips the ReLU masks of a
+    fraction ~eps of the units, each flip adds/removes a full-size term, so the gradient moves by ~sqrt(eps) (observed:
+    5e-2 for fp16 on layers.0, 6e-2 for bf16) — the same mechanism that limits the fp32 trunk bar to 2e-3."""
+    from mipnerf_pl_b200 import _cabi
+    shape = TC_STEP_SHAPES[path]
     b = 200
     rays = to_dev(mp.random_ray_batch(b, seed=41, multiscale=True))
     rgbs = torch.rand(b, 3, device=DEV)
-    ref_model = gpu_model(6, "xavier")
+    ref_model = gpu_model(6, "xavier", **shape)
     ref = mp.forward_backward(ref_model, rays, rgbs, False, True)
     g_ref = {k: p.grad.clone() for k, p in ref_model.named_parameters()}
-    model = gpu_model(6, "xavier", precision=precision)
+    model = gpu_model(6, "xavier", precision=precision, **shape)
+    _cabi.profile_snapshot(reset=True)
     out = mp.forward_backward(model, rays, rgbs, False, True)
     torch.cuda.synchronize()
+    ran = {k: v[0] for k, v in _cabi.profile_snapshot(reset=True).items()}
+    # linear_t16 of the fused step counts under linear_tc as well: the level kernel tells the two paths apart
+    if path == "fused":
+        assert ran["mlp_level_tc"] > 0, ran
+    else:
+        assert ran["mlp_level_tc"] == 0 and ran["linear_tc"] > 0 and ran["wgrad_tc"] > 0, ran
     assert float(out["loss"]) == pytest.approx(float(ref["loss"]), rel=loss_tol)
     errs = {k: float((p.grad - g_ref[k]).norm() / g_ref[k].norm()) for k, p in model.named_parameters()}
-    print(f"{precision} [{wgrad_tc}]: per-tensor gradient distance to the fp32 step "
+    print(f"{precision} [{path}]: loss {float(out['loss']):.6e} vs fp32 {float(ref['loss']):.6e}; "
+          f"per-tensor gradient distance to the fp32 step "
           f"{ {k.replace('mlp.', ''): float(f'{v:.1e}') for k, v in errs.items()} }")
     assert max(errs.values()) <= grad_tol, errs
     # and it trains

@@ -208,6 +208,12 @@ def test_training_and_dataset_entry_points_validate_arguments_without_gpu(lib):
     assert lib.mipnerf_b200_linear_tc(None, None, None, None, 0, 64, 256, 0, _cabi.BF16, None, 0, None) == _cabi.EUNSUPPORTED
     assert lib.mipnerf_b200_linear_tc(None, None, None, None, 0, 256, 256, 0, _cabi.FP32, None, 0, None) == _cabi.EINVAL
     assert lib.mipnerf_b200_linear_tc(None, None, None, None, 0, 256, 256, 0, _cabi.BF16, None, 0, None) == _cabi.EWORKSPACE
+    # tensor-core wgrad: the second operand's columns must start on a 256-column boundary, dy must be 16-byte aligned
+    # (fake device pointers: the library refuses before it touches them)
+    dy, x1, x2, dw, db = 0x10000, 0x20000, 0x30000, 0x40000, 0x50000
+    assert lib.mipnerf_b200_wgrad_tc(dy, 256, x1, 128, x2, 96, 1, 640, dw, db, _cabi.BF16, None, 0, None) == _cabi.EUNSUPPORTED
+    assert lib.mipnerf_b200_wgrad_tc(dy + 4, 256, x1, 256, None, 0, 1, 640, dw, db, _cabi.BF16, None, 0, None) == _cabi.EINVAL
+    assert lib.mipnerf_b200_wgrad_tc(dy, 256, x1, 256, None, 0, 1, 640, dw, db, _cabi.BF16, None, 0, None) == _cabi.EWORKSPACE
     # ray bank / distloss
     assert lib.mipnerf_b200_rays_from_pixels(None, None, None, 0, None, 0, None, None, None, None, None, None, None, None,
                                              None, None) == _cabi.EINVAL
