@@ -32,7 +32,6 @@ constexpr int kViewDim = 27;
 constexpr int kNumLayers = 10;  // 8 trunk + extra_layer + view layer
 constexpr uint32_t kStageBytes = 16384;  // A-operand slab: [128 x 64] 16-bit, SW128
 constexpr uint32_t kTailBytes = 8192;    // feature tail slab: [128 x 32] 16-bit, SW64
-constexpr uint32_t kWStage = 8192;       // weight stage: [128 x 32] 16-bit, SW64 (K = 32 = two MMA steps)
 constexpr uint32_t kABytes = 65536;      // 4 slabs
 constexpr uint32_t kFBytes = kStageBytes + kTailBytes;  // feature tile: SW128 slab (K 0..63) + SW64 slab (K 64..95)
 // Biases and the two CUDA-core heads, broadcast-read by every thread: constant bank.
@@ -45,16 +44,57 @@ struct SmallParams {
 };
 __constant__ SmallParams c_small;
 
-// Packed weight image: per layer, per N-half (rows h*128..), K-slabs of 32 as [128 x 64 B] SW64 stages.
-// number of 32-wide K slabs of layer l (96, 256, .., 352 = [h | x], .., view layer uses the first 256)
-__host__ __device__ constexpr int num_k32(int l) { return l == 0 ? 3 : (l == 5 ? 11 : 8); }
+// The weight stages.  The packed image holds, per layer and per N-half (rows h*128..), the layer's K extent as K-slabs
+// in the order the producer streams them.  One K-slab is one weight stage: [128 rows x kw] 16-bit, K-major and
+// pre-swizzled, so that loading it is one contiguous cp.async.bulk.
+//   * bf16 / fp16 ("wide" stages): 64-wide K-slabs as [128 x 128 B] SW128 stages of 16 KB, four wgmma K steps per
+//     commit group.  Layer 0 (K = 96) and layer 5 (K = 352 = [h | x]) end in a 32-wide [128 x 64 B] SW64 tail of 8 KB.
+//   * split modes: 32-wide SW64 stages of 8 KB throughout; the hi and lo stages of a K-slab share one 16 KB ring slot.
+//     Wide hi + lo stages would need 32 KB slots: the two-slot ring would add 32 KB to the split modes' 213 KB layout,
+//     beyond the 227 KB a CTA may have.
+// Per layer, the image has the same size in both.  The packer, the producer and the consumers take the layout from
+// w_stage / w_stage_offset only.
+__host__ __device__ constexpr int layer_k(int l) {  // the view layer's K is its 256 trunk columns (the view-direction
+  return l == 0 ? kFeat : (l == 5 ? kWidth + kFeat : kWidth);  // columns go into the per-ray bias)
+}
 __host__ __device__ constexpr int num_halves(int l) { return l == 9 ? 1 : 2; }
-__host__ __device__ constexpr uint32_t layer_bytes(int l) { return (uint32_t)num_halves(l) * num_k32(l) * kWStage; }
+__host__ __device__ constexpr int slab_width(bool wide) { return wide ? 64 : 32; }
+__host__ __device__ constexpr int num_slabs(bool wide, int l) {
+  return (layer_k(l) + slab_width(wide) - 1) / slab_width(wide);
+}
+struct WStage {
+  int k0, kw;      // K offset and width: 64, or 32 (a wide layout's tail, or any split-mode stage)
+  uint32_t bytes;  // 128 rows x kw 16-bit
+  bool sw128;      // SW128 (kw = 64) or SW64 (kw = 32)
+};
+// K-slab s of either N-half of layer l
+__host__ __device__ constexpr WStage w_stage(bool wide, int l, int s) {
+  const int k0 = s * slab_width(wide), kw = wide && layer_k(l) - k0 < 64 ? 32 : slab_width(wide);
+  return WStage{k0, kw, (uint32_t)kw * 256u, kw == 64};
+}
+static_assert(kFeat % 32 == 0 && kWidth % 64 == 0, "every K extent is whole 32-wide K-slabs; only layers 0 / 5 have tails");
+__host__ __device__ constexpr uint32_t layer_bytes(int l) { return (uint32_t)num_halves(l) * layer_k(l) * 256u; }
 __host__ __device__ constexpr uint32_t layer_offset(int l) {
   uint32_t o = 0;
   for (int i = 0; i < l; ++i) o += layer_bytes(i);
   return o;
 }
+// image offset of K-slab s of N-half h of layer l (its stages are contiguous in streaming order)
+__host__ __device__ constexpr uint32_t w_stage_offset(bool wide, int l, int h, int s) {
+  return layer_offset(l) + ((uint32_t)h * layer_k(l) + w_stage(wide, l, s).k0) * 256u;
+}
+// the producer streams the image front to back: stage after stage, in issue order, with no gaps
+constexpr bool w_stages_contiguous(bool wide) {
+  uint32_t o = 0;
+  for (int l = 0; l < kNumLayers; ++l)
+    for (int h = 0; h < num_halves(l); ++h)
+      for (int s = 0; s < num_slabs(wide, l); ++s) {
+        if (w_stage_offset(wide, l, h, s) != o) return false;
+        o += w_stage(wide, l, s).bytes;
+      }
+  return o == layer_offset(kNumLayers);
+}
+static_assert(w_stages_contiguous(true) && w_stages_contiguous(false), "stage table and image layout disagree");
 constexpr uint32_t kImageStageBytes = layer_offset(kNumLayers);
 constexpr size_t kSmallOffset = ((size_t)kImageStageBytes + 255) / 256 * 256;
 // view-direction part of the view layer, transposed for coalesced per-ray reads by the ray prologue:
@@ -263,9 +303,8 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
 //     under the wgmmas of later K-slabs (software-pipelined layer loop), and leaves the raw heads of its rows in shared
 //     memory.  The rows of a warpgroup are private to it, so a layer boundary is at most a 128-thread barrier.
 //   * warps 8-11: producer warpgroup (setmaxnreg gives registers to the consumers).  Warp 8 is the weight producer
-//     — cp.async.bulk of the pre-swizzled [128 x 32] (SW64, 8 KB) stages of the packed image
-//     (+ the low-half stage in the split modes) into a ring; a stage is free once both warpgroups' wgmmas reading it
-//     have completed.
+//     — cp.async.bulk of the pre-swizzled weight stages of the packed image (w_stage; + the low-half stage in the
+//     split modes) into a ring of 16 KB slots; a slot is free once both warpgroups' wgmmas reading it have completed.
 //   * warps 9-11 are the helpers: while the consumers run the layers of ray r, they run the ray prologue of ray r + 1
 //     (the coarse fenceposts (level 0) or the bit-exact inverse-CDF resampler (levels >= 1), and the per-ray
 //     view-layer bias (level 0; later levels read it back)), write its Gaussians + IPE features into a free feature
@@ -290,9 +329,9 @@ constexpr int kHeadsWriters = 2 * 128 / 4;  // one consumer thread per quad stor
 constexpr int kProducerRegs = MIPNERF_LEVEL_PRODUCER_REGS;
 constexpr int kConsumerRegs = (65536 / 128 - kProducerRegs) / 2 / 8 * 8;
 static_assert(2 * 128 * kConsumerRegs + 128 * kProducerRegs <= 65536 && kProducerRegs % 8 == 0, "setmaxnreg split");
-// Weight-ring depth of the bf16 / fp16 kernel (a -D flag overrides it for experiments).
+// Weight-ring depth of the bf16 / fp16 kernel in 16 KB slots (a -D flag overrides it for experiments).
 #ifndef MIPNERF_LEVEL_STAGES
-#define MIPNERF_LEVEL_STAGES 12
+#define MIPNERF_LEVEL_STAGES 6
 #endif
 template <bool kX3>
 struct LevelLayout {
@@ -302,10 +341,10 @@ struct LevelLayout {
   static constexpr int kFeatBufs = kX3 ? 1 : 2;
   static constexpr uint32_t kFBuf = (kX3 ? 2 : 1) * kFBytes;  // one buffer: the feature tile (split modes: hi, lo)
   // bf16 / fp16: the layer inputs live in registers, so the CTA holds only the feature buffers and the weight ring, and
-  // the ring is as deep as the carveout allows: 9 stages within 132 KB (L1 keeps ~124 KB for the epilogue's bias
-  // loads), 12 within 164 KB.
+  // the ring is as deep as the 164 KB carveout allows: 6 slots (96 KB).
   static constexpr int kStages = kX3 ? 2 : MIPNERF_LEVEL_STAGES;
-  static constexpr uint32_t kStage = kX3 ? 2 * kWStage : kWStage;  // split modes: W_hi stage, then W_lo
+  // a ring slot: one wide stage (or a tail), or the W_hi then W_lo stage of a split-mode K-slab
+  static constexpr uint32_t kStage = 16384;
   static constexpr uint32_t kA = 0;  // split modes only: the activation tile, hi then lo
   static constexpr uint32_t kF = kA + (kX3 ? 2 * kABytes : 0);
   static constexpr uint32_t kW = kF + kFeatBufs * kFBuf;
@@ -319,17 +358,23 @@ struct LevelLayout {
   static constexpr uint32_t kTotal = kMisc + kMiscBytes + (kPhaseBytes ? kPhaseBytes + 8 : 0) + 1024;
   static_assert(kNumMbars % 2 == 0, "the raw heads behind the mbarriers must be 16-B aligned");
   static_assert(kTotal <= 232448, "exceeds 227 KB of shared memory per CTA");
-  static_assert(kX3 || kStages > 9 || kTotal + 1024 <= 132 * 1024,
-                "bf16 / fp16 with up to 9 stages no longer fits the 132 KB carveout");
-  static_assert(kX3 || kTotal + 1024 <= 164 * 1024, "bf16 / fp16 layout no longer fits the 164 KB carveout");
+  static_assert(kX3 || kStages * kStage > 72 * 1024 || kTotal + 1024 <= 132 * 1024,
+                "bf16 / fp16 with a weight ring of up to 72 KB no longer fits the 132 KB carveout");
+  static_assert(kX3 || kStages * kStage > 96 * 1024 || kTotal + 1024 <= 164 * 1024,
+                "bf16 / fp16 with a weight ring of up to 96 KB no longer fits the 164 KB carveout");
+  static_assert(kX3 ? kStage == 2 * w_stage(false, 0, 0).bytes : kStage == w_stage(true, 1, 0).bytes,
+                "a ring slot holds one stage (split modes: its hi and lo stages)");
 };
 
-// A-operand descriptor of K step j (16 wide) of K-slab s (32 wide) of layer l, for the rows of one warpgroup
-__device__ __forceinline__ uint64_t level_a_desc(int l, int s, int j, uint32_t a_u, uint32_t f_u, uint32_t ft_u) {
-  const int fs = l == 0 ? s : (l == 5 && s >= 8 ? s - 8 : -1);  // >= 0: K-slab fs of the feature tile
-  if (fs < 0) return make_sw128_desc(a_u + (uint32_t)(s >> 1) * kStageBytes + (uint32_t)(s & 1) * 64u + 32u * j);
-  if (fs < 2) return make_sw128_desc(f_u + (uint32_t)fs * 64u + 32u * j);
-  return make_sw64_desc(ft_u + 32u * j);
+// does column k of layer l's input come from the feature tile (layer 0, layer 5's skip columns)?
+__device__ __forceinline__ bool level_reads_feat(int l, int k) { return l == 0 || (l == 5 && k >= kWidth); }
+// A-operand descriptor of the K step (16 wide) at column k of layer l, for the rows of one warpgroup: the activation
+// tile (split modes), or the feature tile's SW128 slab (K 0..63) and SW64 tail (K 64..95)
+__device__ __forceinline__ uint64_t level_a_desc(int l, int k, uint32_t a_u, uint32_t f_u, uint32_t ft_u) {
+  if (!level_reads_feat(l, k)) return make_sw128_desc(a_u + (uint32_t)(k >> 6) * kStageBytes + 2u * (uint32_t)(k & 63));
+  const int kf = l == 0 ? k : k - kWidth;
+  if (kf < 64) return make_sw128_desc(f_u + 2u * (uint32_t)kf);
+  return make_sw64_desc(ft_u + 2u * (uint32_t)(kf - 64));
 }
 
 // Where a consumer warpgroup stands in the weight ring: the slot and phase of its next stage, and the slot of its newest
@@ -340,7 +385,7 @@ struct RingPos {
   int prev;
 };
 
-// K-slab s (32 wide) of one N = 128 half of layer l into acc, for the rows of one warpgroup: wait for the weight stage,
+// K-slab s (w_stage) of one N = 128 half of layer l into acc, for the rows of one warpgroup: wait for the weight stage,
 // issue its wgmmas as one group, then wait until only that group is in flight.  The wait retires the previous group,
 // whose stage is released (one arrive per warpgroup); so one stage's wgmmas stay in flight across calls, also from one
 // half or layer to the next.
@@ -369,38 +414,40 @@ __device__ __forceinline__ void level_mma_slab(float (&acc)[64], int l, int s, u
                                                uint32_t ft_u, uint32_t w_u, uint64_t* w_full, uint64_t* w_empty,
                                                RingPos& rp, bool leader, PhaseClock& clk) {
   const uint32_t b_u = level_stage_acquire<kX3>(w_u, w_full, rp, clk);
+  const WStage ws = w_stage(!kX3, l, s);  // bf16 / fp16: l and s are compile-time constants here
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const uint64_t a_hi = level_a_desc(l, s, j, a_u, f_u, ft_u);
-    const uint64_t b_hi = make_sw64_desc(b_u + 32u * j);
+  for (int j = 0; j < 4; ++j) {
+    if (16 * j >= ws.kw) break;
+    const uint64_t a_hi = level_a_desc(l, ws.k0 + 16 * j, a_u, f_u, ft_u);
+    const uint64_t b_hi = ws.sw128 ? make_sw128_desc(b_u + 32u * j) : make_sw64_desc(b_u + 32u * j);
     wgmma_m64n128k16<kFmt>(acc, a_hi, b_hi, (s | j) ? 1u : 0u);
     if (kX3) {  // A_lo . W_hi + A_hi . W_lo (the lo tiles sit one tile size behind the hi tiles)
-      wgmma_m64n128k16<kFmt>(acc, a_hi + ((l == 0 || (l == 5 && s >= 8)) ? kFBytes : kABytes) / 16, b_hi, 1u);
-      wgmma_m64n128k16<kFmt>(acc, a_hi, b_hi + kWStage / 16, 1u);
+      wgmma_m64n128k16<kFmt>(acc, a_hi + (level_reads_feat(l, ws.k0) ? kFBytes : kABytes) / 16, b_hi, 1u);
+      wgmma_m64n128k16<kFmt>(acc, a_hi, b_hi + ws.bytes / 16, 1u);
     }
   }
   level_stage_commit<kX3>(w_empty, rp, leader, clk);
 }
-// The same for K-slab s < 8 of layers 1..9 in the bf16 / fp16 kernel, with A from registers: x is the layer input as
-// wgmma A fragments (see level_epilogue_chunk_rs), and K-slab s reads x[8 s .. 8 s + 7].  `s` must be a compile-time
-// constant after unrolling, so that x stays in registers.
+// The same for the 64-wide K-slab s < 4 of layers 1..9 in the bf16 / fp16 kernel, with A from registers: x is the layer
+// input as wgmma A fragments (see level_epilogue_chunk_rs), and K-slab s reads x[16 s .. 16 s + 15].  `s` must be a
+// compile-time constant after unrolling, so that x stays in registers.
 template <int kFmt>
 __device__ __forceinline__ void level_mma_slab_rs(float (&acc)[64], const uint32_t (&x)[64], int s, uint32_t w_u,
                                                   uint64_t* w_full, uint64_t* w_empty, RingPos& rp, bool leader,
                                                   PhaseClock& clk) {
   const uint32_t b_u = level_stage_acquire<false>(w_u, w_full, rp, clk);
 #pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    const uint32_t a[4] = {x[8 * s + 4 * j], x[8 * s + 4 * j + 1], x[8 * s + 4 * j + 2], x[8 * s + 4 * j + 3]};
-    wgmma_m64n128k16_rs<kFmt>(acc, a, make_sw64_desc(b_u + 32u * j), (s | j) ? 1u : 0u);
+  for (int j = 0; j < 4; ++j) {
+    const uint32_t a[4] = {x[16 * s + 4 * j], x[16 * s + 4 * j + 1], x[16 * s + 4 * j + 2], x[16 * s + 4 * j + 3]};
+    wgmma_m64n128k16_rs<kFmt>(acc, a, make_sw128_desc(b_u + 32u * j), (s | j) ? 1u : 0u);
   }
   level_stage_commit<false>(w_empty, rp, leader, clk);
 }
 
 // The layer epilogues run in chunks under the wgmmas of K-slabs (see the layer loop of mlp_level_kernel): kEpiChunks
-// chunks per N = 128 half, each after the wait of one K-slab; chunk c covers the accumulator's column groups
-// 4 c .. 4 c + 3, i.e. columns c_base + 32 c .. + 31, which are exactly the A-operand columns that K-slab c
-// (c_base = 0) or 4 + c (c_base = 128) of the next layer reads.
+// chunks per N = 128 half, each after the wait of a K-slab; chunk c covers the accumulator's column groups
+// 4 c .. 4 c + 3, i.e. columns c_base + 32 c .. + 31, which are exactly the A-operand columns that the 32-wide
+// K-slab c (c_base = 0) or 4 + c (c_base = 128) of the next layer reads in the split modes.
 constexpr int kEpiChunks = 4;
 constexpr int kEpiGroups = 16 / kEpiChunks;
 // First K-slab of a trunk layer's N-half 1 that carries a chunk of N-half 0's epilogue (chunk c after K-slab
@@ -461,17 +508,23 @@ __device__ __forceinline__ void level_epilogue_chunk(const float (&acc)[64], con
   }
 }
 
-// ---- the register-chained layer loop of the bf16 / fp16 kernel ----
-// First K-slab of a layer's N-half 1 that carries a chunk of N-half 0's epilogue (chunk c after K-slab
-// kEpiFirstRs + c).  The chunks write registers that no wgmma in flight reads, and the wait of N-half 1's first K-slab
-// retires all of N-half 0, so any value in 0..4 is safe; a -D flag overrides it for experiments.  Measured on an H100
-// 80GB HBM3 at 400 W (bench.py bf16 step, 12 stages): 3.86-3.89 ms with 0, 3.81-3.82 ms with 1, 3.51-3.53 ms with 2,
-// 3.52-3.54 ms with 3, 3.52-3.59 ms with 4.
+// ---- the register-chained layer loop of the bf16 / fp16 kernel (64-wide K-slabs) ----
+// Where acc0's epilogue chunks run under a layer's N-half 1, counted in 32-wide halves of its K-slabs: chunk c follows
+// the K-slab (kEpiFirstRs + c) / 2.  The default 4 puts chunks 0, 1 after K-slab 2 and chunks 2, 3 after K-slab 3.
+// The chunks write registers that no wgmma in flight reads, and the wait of N-half 1's first K-slab retires all of
+// N-half 0, so any value in 0..4 is safe; a -D flag overrides it for experiments.  0 and 1 make ptxas serialise the
+// wgmmas (too few registers); 2 and 3 leave a local-memory load in the layer loop.  Measured with bench.py (bf16 step,
+// 6 slots, H100 80GB HBM3 at 400 W): 2.86-2.88 ms with 2, 2.84 ms with 3, 2.83-2.85 ms with 4.
 #ifndef MIPNERF_LEVEL_EPI_FIRST
-#define MIPNERF_LEVEL_EPI_FIRST 2
+#define MIPNERF_LEVEL_EPI_FIRST 4
 #endif
 constexpr int kEpiFirstRs = MIPNERF_LEVEL_EPI_FIRST;
-static_assert(kEpiFirstRs >= 0 && kEpiFirstRs + kEpiChunks <= 8, "the chunks must follow K-slabs 0..7");
+static_assert(kEpiFirstRs >= 0 && kEpiFirstRs + kEpiChunks <= 8, "the chunks must follow K-slabs 0..3");
+__host__ __device__ constexpr int epi_slab_acc0(int c) { return (kEpiFirstRs + c) / 2; }
+// acc1's chunks c = 0..3 follow the next layer's N-half-0 K-slab c / 2: chunk c writes x[32 + 8 c .. 32 + 8 c + 7],
+// which K-slab 2 (chunks 0, 1) and K-slab 3 (chunks 2, 3) read, and the wait of K-slab 0 retires all of the layer.
+__host__ __device__ constexpr int epi_slab_acc1(int c) { return c / 2; }
+static_assert(epi_slab_acc1(kEpiChunks - 1) < 2, "acc1's chunks must land before the next layer's K-slab 2 reads them");
 
 // What the layer loop needs besides its accumulators and A arrays.
 struct LevelRsCtx {
@@ -544,29 +597,33 @@ __device__ __forceinline__ void level_epilogue_chunk_rs(const float (&acc)[64], 
   }
 }
 
-// Layer l + 1's N-half 0, K-slabs 0..3 (x[0..31], from acc0's epilogue of layer l) into acc0, with acc1's epilogue of
-// layer l (x[32..63]) in chunks after them.  The wait of the first K-slab retires all of layer l; after layer 5
-// (release_feat) that is the last read of the feature buffer, which goes back to the helpers.
+// Layer l + 1's N-half 0, K-slabs 0, 1 (x[0..31], from acc0's epilogue of layer l) into acc0, with acc1's epilogue of
+// layer l (x[32..63]) in chunks after them (epi_slab_acc1).  The wait of the first K-slab retires all of layer l; after
+// layer 5 (release_feat) that is the last read of the feature buffer, which goes back to the helpers.
 template <int kFmt>
 __device__ __forceinline__ void level_rs_next_head(float (&acc0)[64], float (&acc1)[64], uint32_t (&x)[64], int l,
                                                    bool release_feat, const LevelRsCtx& k, RingPos& rp, PhaseClock& clk,
                                                    float& d0, float& d1) {
   wgmma_fence_acc(acc0);
 #pragma unroll
-  for (int c = 0; c < kEpiChunks; ++c) {
-    EpiConsts e;
-    level_epilogue_consts(e, l, 128, c, k.cq, k.gsp);
-    level_mma_slab_rs<kFmt>(acc0, x, c, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
-    if (c == 0 && release_feat && k.leader) mbar_arrive(k.feat_empty);
-    if (c == 0) wgmma_fence_acc(acc1);
-    level_epilogue_chunk_rs<kFmt>(acc1, e, l, 128, c, x, k, d0, d1);
+  for (int s = 0; s < 2; ++s) {
+    EpiConsts e[kEpiChunks];
+#pragma unroll
+    for (int c = 0; c < kEpiChunks; ++c)
+      if (epi_slab_acc1(c) == s) level_epilogue_consts(e[c], l, 128, c, k.cq, k.gsp);
+    level_mma_slab_rs<kFmt>(acc0, x, s, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+    if (s == 0 && release_feat && k.leader) mbar_arrive(k.feat_empty);
+    if (s == 0) wgmma_fence_acc(acc1);
+#pragma unroll
+    for (int c = 0; c < kEpiChunks; ++c)
+      if (epi_slab_acc1(c) == s) level_epilogue_chunk_rs<kFmt>(acc1, e[c], l, 128, c, x, k, d0, d1);
     clk.mark(kPhEpilogue);
   }
 }
 
 // Trunk layer / bottleneck l (1..8) from x_in into x_out: the rest of N-half 0 into acc0, N-half 1 into acc1 with
-// acc0's epilogue in chunks under it, then level_rs_next_head.  kSkip: l may be 5, whose K-slabs 8..10 read the
-// feature tile.
+// acc0's epilogue in chunks under it (epi_slab_acc0), then level_rs_next_head.  kSkip: l may be 5, whose K-slabs 4
+// (SW128) and 5 (SW64 tail) read the feature tile.
 template <int kFmt, bool kSkip>
 __device__ __forceinline__ void level_rs_layer(float (&acc0)[64], float (&acc1)[64], const uint32_t (&x_in)[64],
                                                uint32_t (&x_out)[64], int l, const LevelRsCtx& k, RingPos& rp,
@@ -577,30 +634,32 @@ __device__ __forceinline__ void level_rs_layer(float (&acc0)[64], float (&acc1)[
   uint32_t f_u = k.f_u, ft_u = k.ft_u;
   asm volatile("" : "+r"(f_u), "+r"(ft_u));
 #pragma unroll
-  for (int s = kEpiChunks; s < 8; ++s)
+  for (int s = 2; s < kWidth / 64; ++s)
     level_mma_slab_rs<kFmt>(acc0, x_in, s, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
-  if (skip)
-    for (int s = 8; s < num_k32(5); ++s)
+  if (skip) {
+#pragma unroll
+    for (int s = kWidth / 64; s < num_slabs(true, 5); ++s)
       level_mma_slab<kFmt, false>(acc0, 5, s, 0u, f_u, ft_u, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+  }
   wgmma_fence_acc(acc1);
 #pragma unroll
-  for (int s = 0; s < kEpiFirstRs; ++s)
-    level_mma_slab_rs<kFmt>(acc1, x_in, s, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+  for (int s = 0; s < kWidth / 64; ++s) {
+    EpiConsts e[kEpiChunks];  // the biases of the chunks that follow K-slab s, loaded before it
 #pragma unroll
-  for (int c = 0; c < kEpiChunks; ++c) {
-    EpiConsts e;
-    level_epilogue_consts(e, l, 0, c, k.cq, k.gsp);
-    level_mma_slab_rs<kFmt>(acc1, x_in, kEpiFirstRs + c, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
-    if (c == 0) wgmma_fence_acc(acc0);
-    level_epilogue_chunk_rs<kFmt>(acc0, e, l, 0, c, x_out, k, d0, d1);
+    for (int c = 0; c < kEpiChunks; ++c)
+      if (epi_slab_acc0(c) == s) level_epilogue_consts(e[c], l, 0, c, k.cq, k.gsp);
+    level_mma_slab_rs<kFmt>(acc1, x_in, s, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+    if (s == epi_slab_acc0(0)) wgmma_fence_acc(acc0);
+#pragma unroll
+    for (int c = 0; c < kEpiChunks; ++c)
+      if (epi_slab_acc0(c) == s) level_epilogue_chunk_rs<kFmt>(acc0, e[c], l, 0, c, x_out, k, d0, d1);
     clk.mark(kPhEpilogue);
   }
+  if (skip) {
 #pragma unroll
-  for (int s = kEpiFirstRs + kEpiChunks; s < 8; ++s)
-    level_mma_slab_rs<kFmt>(acc1, x_in, s, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
-  if (skip)
-    for (int s = 8; s < num_k32(5); ++s)
+    for (int s = kWidth / 64; s < num_slabs(true, 5); ++s)
       level_mma_slab<kFmt, false>(acc1, 5, s, 0u, f_u, ft_u, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
+  }
   level_rs_next_head<kFmt>(acc0, acc1, x_out, l, skip, k, rp, clk, d0, d1);
 }
 
@@ -850,24 +909,25 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       int st = 0;
       uint32_t ph = 0;
       const uint64_t pol = l2_policy_evict_last();  // the image is re-read by every CTA for every ray
-      for (int64_t ray = blockIdx.x; ray < p.num_rays; ray += gridDim.x)
-        for (int l = 0; l < kNumLayers; ++l) {
-          const uint8_t* src = p.wimage + layer_offset(l);
-          const int n = num_halves(l) * num_k32(l);  // stages in issue order: N-half major, then K-slab
-          for (int i = 0; i < n; ++i) {
-            clk.mark(kPhIssue);
-            mbar_wait(&w_empty[st], ph ^ 1);
-            clk.mark(kPhWEmpty);
-            mbar_arrive_expect_tx(&w_full[st], Lay::kStage);
-            bulk_g2s_hint(sW + st * Lay::kStage, src + (size_t)i * kWStage, kWStage, &w_full[st], pol);
-            if (kX3) bulk_g2s_hint(sW + st * Lay::kStage + kWStage, src + kLoOffset + (size_t)i * kWStage, kWStage,
-                                   &w_full[st], pol);
-            if (++st == Lay::kStages) {
-              st = 0;
-              ph ^= 1;
+      for (int64_t ray = blockIdx.x; ray < p.num_rays; ray += gridDim.x) {
+        const uint8_t* src = p.wimage;  // the stages are contiguous in issue order (w_stages_contiguous)
+        for (int l = 0; l < kNumLayers; ++l)
+          for (int h = 0; h < num_halves(l); ++h)  // N-half major, then K-slab
+            for (int s = 0; s < num_slabs(!kX3, l); ++s) {
+              const uint32_t bytes = w_stage(!kX3, l, s).bytes;
+              clk.mark(kPhIssue);
+              mbar_wait(&w_empty[st], ph ^ 1);
+              clk.mark(kPhWEmpty);
+              mbar_arrive_expect_tx(&w_full[st], kX3 ? 2 * bytes : bytes);
+              bulk_g2s_hint(sW + st * Lay::kStage, src, bytes, &w_full[st], pol);
+              if (kX3) bulk_g2s_hint(sW + st * Lay::kStage + bytes, src + kLoOffset, bytes, &w_full[st], pol);
+              src += bytes;
+              if (++st == Lay::kStages) {
+                st = 0;
+                ph ^= 1;
+              }
             }
-          }
-        }
+      }
       clk.mark(kPhIssue);
       clk.end(phase_slot, 2);
     }
@@ -919,29 +979,31 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
     float acc0[64], acc1[64];
     wgmma_fence_acc(acc0);
 #pragma unroll
-    for (int s = 0; s < num_k32(0); ++s)
+    for (int s = 0; s < num_slabs(!kX3, 0); ++s)
       level_mma_slab<kFmt, kX3>(acc0, 0, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
     if constexpr (!kX3) {
       // bf16 / fp16: the layers are chained through registers (wgmma with A from registers), the schedule above with
-      // no activation tile: each epilogue chunk writes its 16-bit pairs into the A fragments of the next layer's input,
-      // one of two arrays (layer l reads xa or xb, writes the other), so no layer's writes touch what its own wgmmas
-      // read, and there is no fence or barrier between layers.  acc0's chunks follow N-half 1's K-slabs kEpiFirstRs + c
-      // and acc1's the next layer's K-slabs 0..3.  Layer 0 and layer 5's K-slabs 8..10 read the feature tile; layer 0
-      // has three K-slabs, so its acc0 chunks follow K-slabs 0, 1, 2, 2.  The training forward's activation tiles go
-      // out from the epilogue's registers.
+      // no activation tile and 64-wide K-slabs: each epilogue chunk writes its 16-bit pairs into the A fragments of the
+      // next layer's input, one of two arrays (layer l reads xa or xb, writes the other), so no layer's writes touch
+      // what its own wgmmas read, and there is no fence or barrier between layers.  acc0's chunks follow N-half 1's
+      // K-slabs epi_slab_acc0(c) and acc1's the next layer's K-slabs 0, 1.  Layer 0 and layer 5's K-slabs 4, 5 read the
+      // feature tile; layer 0 has two K-slabs (64 wide + the 32-wide tail), and two of its acc0 chunks follow each.  The
+      // training forward's activation tiles go out from the epilogue's registers.
       const LevelRsCtx k{f_u, ft_u, w_u, w_full, w_empty, &feat_empty[fb], gsp,
                          p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
                          (size_t)p.dump_tiles * kABytes, dump_policy, r0, cq, leader};
       uint32_t xa[64], xb[64];
+      static_assert(2 * num_slabs(true, 0) == kEpiChunks, "layer 0: two acc0 chunks after each of its K-slabs");
       wgmma_fence_acc(acc1);
 #pragma unroll
-      for (int c = 0; c < kEpiChunks; ++c) {
-        EpiConsts e;
-        level_epilogue_consts(e, 0, 0, c, cq, gsp);
-        if (c < num_k32(0))
-          level_mma_slab<kFmt, false>(acc1, 0, c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
-        if (c == 0) wgmma_fence_acc(acc0);
-        level_epilogue_chunk_rs<kFmt>(acc0, e, 0, 0, c, xb, k, d0, d1);
+      for (int s = 0; s < num_slabs(true, 0); ++s) {
+        EpiConsts e[2];
+        level_epilogue_consts(e[0], 0, 0, 2 * s, cq, gsp);
+        level_epilogue_consts(e[1], 0, 0, 2 * s + 1, cq, gsp);
+        level_mma_slab<kFmt, false>(acc1, 0, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+        if (s == 0) wgmma_fence_acc(acc0);
+        level_epilogue_chunk_rs<kFmt>(acc0, e[0], 0, 0, 2 * s, xb, k, d0, d1);
+        level_epilogue_chunk_rs<kFmt>(acc0, e[1], 0, 0, 2 * s + 1, xb, k, d0, d1);
         clk.mark(kPhEpilogue);
       }
       level_rs_next_head<kFmt>(acc0, acc1, xb, 0, false, k, rp, clk, d0, d1);
@@ -952,12 +1014,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       }
       // the rest of the view layer's one N-half, from the bottleneck in xb
 #pragma unroll
-      for (int s = kEpiChunks; s < 8; ++s) level_mma_slab_rs<kFmt>(acc0, xb, s, w_u, w_full, w_empty, rp, leader, clk);
+      for (int s = 2; s < num_slabs(true, 9); ++s)
+        level_mma_slab_rs<kFmt>(acc0, xb, s, w_u, w_full, w_empty, rp, leader, clk);
     } else {
       for (int l = 0; l < 9; ++l) {
         // 1. the rest of N-half 0
         if (l > 0)
-          for (int s = kEpiChunks; s < num_k32(l); ++s)
+          for (int s = kEpiChunks; s < num_slabs(false, l); ++s)
             level_mma_slab<kFmt, kX3>(acc0, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
         // 2. N-half 1, with acc0's epilogue under it
         wgmma_fence_acc(acc1);
@@ -968,7 +1031,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
         for (int c = 0; c < kEpiChunks; ++c) {
           EpiConsts e;
           level_epilogue_consts(e, l, 0, c, cq, gsp);
-          if (first + c < num_k32(l))
+          if (first + c < num_slabs(false, l))
             level_mma_slab<kFmt, kX3>(acc1, l, first + c, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
           if (c == 0) {
             wgmma_fence_acc(acc0);
@@ -983,7 +1046,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
           level_epilogue_chunk<kFmt, kX3>(acc0, e, l, 0, c, r0, cq, sA, gsp, d0, d1);
           clk.mark(kPhEpilogue);
         }
-        for (int s = first + kEpiChunks; s < num_k32(l); ++s)
+        for (int s = first + kEpiChunks; s < num_slabs(false, l); ++s)
           level_mma_slab<kFmt, kX3>(acc1, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
         // 3.
         fence_proxy_async_smem();
@@ -1023,7 +1086,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
         }
       }
       // the rest of the view layer's one N-half
-      for (int s = kEpiChunks; s < num_k32(9); ++s)
+      for (int s = kEpiChunks; s < num_slabs(false, 9); ++s)
         level_mma_slab<kFmt, kX3>(acc0, 9, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
     }
     // the view layer's epilogue from the registers
@@ -1107,33 +1170,35 @@ __global__ void pack_stage_kernel(const float* __restrict__ w, int in_features, 
   *reinterpret_cast<uint16_t*>(dst + off) = to16<kFmt>(v);
 }
 
-// All stages of one (hi or lo) v1 image in ONE launch: block = stage.  Main stages: layer l, N-half h, K-slab s of 32
-// (K order of layer 5 is the reference's concat [h (256) | x (96)], mip_nerf.py:96-97) -> [128 x 64 B] SW64.
+// All stages of one (hi or lo) v1 image in ONE launch: block = stage.  Stage (layer l, N-half h, K-slab s) as w_stage
+// lays it out (K order of layer 5 is the reference's concat [h (256) | x (96)], mip_nerf.py:96-97): [128 x kw] at K
+// offset k0, SW128 for 64-wide stages, SW64 for 32-wide ones.
 struct PackV1Src {
   const float* weight[kNumLayers];
   int in_features[kNumLayers];
 };
-__host__ __device__ constexpr int v1_stage_begin(int l) {
+__host__ __device__ constexpr int v1_stage_begin(bool wide, int l) {
   int n = 0;
-  for (int i = 0; i < l; ++i) n += num_halves(i) * num_k32(i);
+  for (int i = 0; i < l; ++i) n += num_halves(i) * num_slabs(wide, i);
   return n;
 }
-constexpr int kV1MainStages = v1_stage_begin(kNumLayers);
 template <int kFmt>
-__global__ void __launch_bounds__(256) pack_v1_image_kernel(const PackV1Src src, uint8_t* __restrict__ base, int lo) {
+__global__ void __launch_bounds__(256) pack_v1_image_kernel(const PackV1Src src, uint8_t* __restrict__ base, int lo,
+                                                            bool wide) {
   const int stage = blockIdx.x;
   int l = 0;
-  while (l + 1 < kNumLayers && stage >= v1_stage_begin(l + 1)) ++l;
-  const int local = stage - v1_stage_begin(l);
-  const int h = local / num_k32(l), sl = local % num_k32(l);
+  while (l + 1 < kNumLayers && stage >= v1_stage_begin(wide, l + 1)) ++l;
+  const int local = stage - v1_stage_begin(wide, l);
+  const int h = local / num_slabs(wide, l), sl = local % num_slabs(wide, l);
+  const WStage ws = w_stage(wide, l, sl);
   const float* w = src.weight[l];
-  const int in_features = src.in_features[l], row0 = h * 128, kbase = sl * 32, nrows = 128;
-  uint8_t* dst = base + layer_offset(l) + (size_t)local * kWStage;
-  for (int idx = threadIdx.x; idx < nrows * 32; idx += 256) {
-    const int i = idx >> 5, j = idx & 31;
-    float v = w[(size_t)(row0 + i) * in_features + kbase + j];
+  const int in_features = src.in_features[l], row0 = h * 128, nrows = 128;
+  uint8_t* dst = base + w_stage_offset(wide, l, h, sl);
+  for (int idx = threadIdx.x; idx < nrows * ws.kw; idx += 256) {
+    const int i = idx / ws.kw, j = idx % ws.kw;
+    float v = w[(size_t)(row0 + i) * in_features + ws.k0 + j];
     if (lo) v = v - from16<kFmt>(to16<kFmt>(v));
-    *reinterpret_cast<uint16_t*>(dst + sw64_offset(i, j)) = to16<kFmt>(v);
+    *reinterpret_cast<uint16_t*>(dst + (ws.sw128 ? sw128_offset(i, j) : sw64_offset(i, j))) = to16<kFmt>(v);
   }
 }
 
@@ -1360,10 +1425,12 @@ cudaError_t tc_pack_weights(const mipnerf_b200_config* c, const mipnerf_b200_wei
     const int li = l < 8 ? l : (l == 8 ? 9 : 10);  // layers.l | extra_layer | view_layers.0
     v1.weight[l] = lin[li].weight, v1.in_features[l] = lin[li].in_features;
   }
+  const bool wide = !is_x3(precision);  // the stage layout the level kernel of this precision streams
+  const int stages = v1_stage_begin(wide, kNumLayers);
   for (int part = 0; part < parts; ++part) {
     uint8_t* base = img + (part ? kLoOffset : 0);
-    if (bf) pack_v1_image_kernel<1><<<kV1MainStages, 256, 0, st>>>(v1, base, part);
-    else pack_v1_image_kernel<0><<<kV1MainStages, 256, 0, st>>>(v1, base, part);
+    if (bf) pack_v1_image_kernel<1><<<stages, 256, 0, st>>>(v1, base, part, wide);
+    else pack_v1_image_kernel<0><<<stages, 256, 0, st>>>(v1, base, part, wide);
   }
   SmallSrc src;
   for (int l = 0; l < 8; ++l) src.bias[l] = lin[l].bias;
