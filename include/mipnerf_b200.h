@@ -33,10 +33,11 @@ extern "C" {
 
 /* Arithmetic the MLP contraction runs in (everything else on the path is always fp32).
  * FP32 takes any config check_config accepts.  The tensor-core precisions take the reference's shipped architecture:
- * 8x256 trunk with the skip after layer 4, one 128-wide view layer, num_samples = 128, use_viewdirs, min_deg_point = 0,
- * max_deg_point 1..16 and deg_view 1..4 (narrower encodings are zero-padded into the operand image by
- * mipnerf_b200_pack_weights); the tensor-core TRAINING step and mipnerf_b200_mlp_forward need max_deg_point = 16 and
- * deg_view = 4.  Anything else answers MIPNERF_B200_EUNSUPPORTED (mipnerf_b200_packed_weights_bytes() == 0). */
+ * 8x256 trunk with the skip after layer 4, one 128-wide view layer, num_samples = 128 or 256, use_viewdirs,
+ * min_deg_point = 0, max_deg_point 1..16 and deg_view 1..4 (narrower encodings are zero-padded into the operand image
+ * by mipnerf_b200_pack_weights; the image does not depend on num_samples); the tensor-core TRAINING step and
+ * mipnerf_b200_mlp_forward need max_deg_point = 16 and deg_view = 4, and mipnerf_b200_mlp_forward 128 samples per ray.
+ * Anything else answers MIPNERF_B200_EUNSUPPORTED (mipnerf_b200_packed_weights_bytes() == 0). */
 #define MIPNERF_B200_FP32 0 /* CUDA-core FFMA, fp32 operands: the 1e-4 parity mode                   */
 #define MIPNERF_B200_BF16 1 /* wgmma, bf16 operands, fp32 accumulate                                */
 #define MIPNERF_B200_FP16 2 /* wgmma, fp16 operands, fp32 accumulate                                */
@@ -187,7 +188,7 @@ size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_
  * no gradient (stop_resample_grad=True semantics, models/mip.py:250-264).  precision FP32: every GEMM in fp32 FFMA
  * (the parity mode); BF16 / FP16: forward, dgrad and wgrad GEMMs of the 128- and 256-wide layers on wgmma with
  * 16-bit operands, heads / rendering in fp32.  The fused step (level kernels + 16-bit activation tile images) runs for
- * the level kernel's shapes (the default architecture and encodings, 128 samples) with at most two levels; other
+ * the level kernel's shapes (the default architecture and encodings, 128 samples only) with at most two levels; other
  * shapes with the default widths and encoding sizes (96-d IPE, 27-d view encoding) and net_depth <= 16 run per-layer
  * GEMMs on fp32 activations. */
 int mipnerf_b200_forward_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* weights,

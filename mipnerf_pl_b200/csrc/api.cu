@@ -286,7 +286,8 @@ static int forward_impl(const mipnerf_b200_config* cfg, const mipnerf_b200_weigh
   if (precision != MIPNERF_B200_FP32) {
     if (!mipnerf::tc_supported(cfg, precision))
       return fail(MIPNERF_B200_EUNSUPPORTED,
-                  "tensor-core path supports the 8x256 / 1x128 / N=128 model with min_deg_point 0, max_deg_point 1..16, "
+                  "tensor-core path supports the 8x256 / 1x128 model with num_samples 128 or 256, min_deg_point 0, "
+                  "max_deg_point 1..16, "
                   "deg_view 1..4 and precision bf16|fp16|fp16x3|bf16x3; use MIPNERF_B200_FP32 for other shapes");
     if (!w->packed || w->packed_precision != precision ||
         w->packed_bytes < mipnerf::tc_packed_bytes(cfg, precision))
@@ -469,10 +470,12 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
   return s;
 }
 
-// The fused step needs the level kernels' architecture (8 x 256 trunk, 128 samples, ...) and at most two levels;
-// other shapes that train_tc_supported accepts take the per-layer tensor-core path.
+// The fused step needs the level kernels' architecture (8 x 256 trunk, ...) with one 128-row tile per ray (its
+// activation dump is one tile per ray) and at most two levels; other shapes that train_tc_supported accepts, 256
+// samples included, take the per-layer tensor-core path.
 bool train_fused_supported(const mipnerf_b200_config* c, int precision) {
   return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_FP16) && mipnerf::tc_supported(c, precision) &&
+         c->num_samples == 128 &&
          mipnerf::tc_default_degrees(c) &&  // the backward's tile images carry the full 96 / 27 encodings
          c->num_levels <= 2 && c->net_depth == 8;
 }

@@ -24,7 +24,7 @@ namespace {
 
 using namespace tc;
 
-constexpr int kN = 128;         // samples per ray (the M of a ray's GEMMs)
+constexpr int kN = 128;         // sample rows per tile (the M of a tile's GEMMs); a ray is kT = 1 or 2 tiles
 constexpr int kWidth = 256;     // trunk width
 constexpr int kCond = 128;      // view layer width
 constexpr int kFeat = 96;       // IPE width
@@ -108,6 +108,8 @@ constexpr size_t kLoOffset = kImageBytes;
 constexpr size_t kLoBytes = ((size_t)kImageStageBytes + 255) / 256 * 256;
 constexpr size_t kImageEnd = kLoOffset + kLoBytes;
 
+// Shapes below are for n = 128 samples per ray (kT = 1); a kT = 2 launch has n = 256: [B,257] fenceposts, [B,256]
+// weights and density normals.  The training dump and MLP-only mode exist for kT = 1 only.
 struct LevelParams {
   const uint8_t* wimage;
   const float* origins;
@@ -154,10 +156,11 @@ struct LevelParams {
   Draws dnoise;  // density noise of randomized mode (models/mip_nerf.py:232-233): normals [B,128] or in-kernel; scale = std
 };
 
-// raw density of (ray, row) with the density noise added; kept out of line so that the (default) noise-free
-// path carries none of the generator's registers
+// raw density of (ray, row) of a ray of kNs samples with the density noise added; kept out of line so that the
+// (default) noise-free path carries none of the generator's registers
+template <int kNs>
 __device__ __noinline__ float noisy_raw_density(float raw, const Draws d, int64_t ray, int row) {
-  return add_density_noise(raw, d, ray, row, kN);
+  return add_density_noise(raw, d, ray, row, kNs);
 }
 
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
@@ -246,13 +249,14 @@ __device__ __forceinline__ void store8_split(uint8_t* dst_hi, uint8_t* dst_lo, c
 }
 
 // Gaussian + IPE features [8 gi_begin, 8 gi_end) and [48 + 8 gi_begin, 48 + 8 gi_end) of one sample row of a ray (or,
-// in MLP-only mode, the caller's features) into the feature tile: SW128 slab (K 0..63) + SW64 tail (K 64..95).
-template <int kFmt, bool kX3>
+// in MLP-only mode, the caller's features) into the feature tile: SW128 slab (K 0..63) + SW64 tail (K 64..95).  `row`
+// is the row of the tile; MLP-only mode has one tile per ray.
+template <int kFmt, bool kX3, int kT>
 __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeom& g, int64_t ray, int row, float t0,
                                               float t1, uint8_t* myF, int gi_begin, int gi_end) {
   float mean[3] = {0.f, 0.f, 0.f}, cov[3] = {0.f, 0.f, 0.f};
   const float* fin = nullptr;
-  if (p.feat_in) {
+  if (kT == 1 && p.feat_in) {
     fin = p.feat_in + (ray * kN + row) * kFeat;  // MLP-only mode: the caller's encoding
   } else {
     float tm, tv, rv;
@@ -293,8 +297,9 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
 }
 
 // =================================================================================================
-// The level kernel (sm_90a): one persistent CTA per SM, 384 threads, one ray (= 128 sample rows) at a time in the
-// tensor core, with the scalar work of the neighbouring rays beside it.
+// The level kernel (sm_90a): one persistent CTA per SM, 384 threads, one tile of 128 sample rows at a time in the
+// tensor core, with the scalar work of the neighbouring tiles beside it.  A ray is kT = 1 or 2 consecutive tiles
+// (128 or 256 samples); below, "ray" is a tile when kT = 2, except for the per-ray prologue and compositing.
 //   * warps 0-3 / 4-7: two consumer warpgroups, warpgroup g owns sample rows 64 g .. 64 g + 63 of the ray.  Each
 //     issues the wgmma (M = 64, N = 128, K = 16) of every layer for its rows (A operand: its rows of the ray's feature
 //     buffer in shared memory for layer 0 and layer 5's skip slabs; otherwise the layer input in registers (bf16 /
@@ -333,11 +338,11 @@ static_assert(2 * 128 * kConsumerRegs + 128 * kProducerRegs <= 65536 && kProduce
 #ifndef MIPNERF_LEVEL_STAGES
 #define MIPNERF_LEVEL_STAGES 6
 #endif
-template <bool kX3>
+template <bool kX3, int kT>
 struct LevelLayout {
-  // Feature buffers: bf16 / fp16 have two, so that the helpers write ray r + 1's features while layer 0 / layer 5 of
-  // ray r read the other; the split modes (hi + lo tiles next to the 128 KB activation tile) have room for one only,
-  // and the helpers write the next ray's features once layer 5's skip slabs have retired.
+  // Feature buffers, one tile each: bf16 / fp16 have two, so that the helpers write tile i + 1's features while layer
+  // 0 / layer 5 of tile i read the other; the split modes (hi + lo tiles next to the 128 KB activation tile) have room
+  // for one only, and the helpers write the next tile's features once layer 5's skip slabs have retired.
   static constexpr int kFeatBufs = kX3 ? 1 : 2;
   static constexpr uint32_t kFBuf = (kX3 ? 2 : 1) * kFBytes;  // one buffer: the feature tile (split modes: hi, lo)
   // bf16 / fp16: the layer inputs live in registers, so the CTA holds only the feature buffers and the weight ring, and
@@ -351,11 +356,14 @@ struct LevelLayout {
   static constexpr uint32_t kMisc = kW + kStages * kStage;
   // mbarriers: w_full / w_empty [kStages], feat_full / feat_empty [kFeatBufs], heads_full / heads_empty [2]
   static constexpr int kNumMbars = 2 * kStages + 2 * kFeatBufs + 2 * 2;
-  // mbarriers, raw heads [2][128][4] (ray parity), scan carries [4], partial sums [4][8], resampler scratch [129]
-  static constexpr uint32_t kMiscBytes = kNumMbars * 8 + 2 * kN * 4 * 4 + 4 * 4 + 4 * 8 * 4 + (kN + 1) * 4;
+  // mbarriers, raw heads [2][128][4] (tile parity; with kT = 2 the two tiles of a ray), scan carries [4 kT], partial
+  // sums [4 kT][8] (one per 32-row chunk of the ray), resampler scratch [128 kT + 1]
+  static constexpr uint32_t kMiscBytes =
+      kNumMbars * 8 + 2 * kN * 4 * 4 + 4 * kT * 4 + 4 * kT * 8 * 4 + (kT * kN + 1) * 4;
   static constexpr uint32_t kPhase = (kMisc + kMiscBytes + 7) & ~7u;  // phase accumulators (MIPNERF_LEVEL_PHASES)
   // + slack for the 1024-B alignment of the tiles
   static constexpr uint32_t kTotal = kMisc + kMiscBytes + (kPhaseBytes ? kPhaseBytes + 8 : 0) + 1024;
+  static_assert(kT == 1 || kT == 2, "a ray is one or two 128-row tiles");
   static_assert(kNumMbars % 2 == 0, "the raw heads behind the mbarriers must be 16-B aligned");
   static_assert(kTotal <= 232448, "exceeds 227 KB of shared memory per CTA");
   static_assert(kX3 || kStages * kStage > 72 * 1024 || kTotal + 1024 <= 132 * 1024,
@@ -395,7 +403,7 @@ __device__ __forceinline__ uint32_t level_stage_acquire(uint32_t w_u, uint64_t* 
   mbar_wait(&w_full[rp.st], rp.ph);
   clk.mark(kPhWFull);
   wgmma_fence();
-  return w_u + (uint32_t)rp.st * LevelLayout<kX3>::kStage;
+  return w_u + (uint32_t)rp.st * LevelLayout<kX3, 1>::kStage;
 }
 template <bool kX3>
 __device__ __forceinline__ void level_stage_commit(uint64_t* w_empty, RingPos& rp, bool leader, PhaseClock& clk) {
@@ -403,7 +411,7 @@ __device__ __forceinline__ void level_stage_commit(uint64_t* w_empty, RingPos& r
   wgmma_wait<1>();
   if (rp.prev >= 0 && leader) mbar_arrive(&w_empty[rp.prev]);
   rp.prev = rp.st;
-  if (++rp.st == LevelLayout<kX3>::kStages) {
+  if (++rp.st == LevelLayout<kX3, 1>::kStages) {
     rp.st = 0;
     rp.ph ^= 1;
   }
@@ -668,26 +676,27 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// ---- the helper warps' per-ray work (ht = helper thread 0..95, hw = helper warp 0..2) ----
-// Ray prologue and features of `ray` into the feature buffer fbuf.  The prologue's global stores (fenceposts, view
-// bias) are read back by this CTA only, through L2 (ld.cg): by the helpers after the helper barrier, by the consumers
-// after feat_full.
-template <int kFmt, bool kX3>
-__device__ __forceinline__ void level_prepare_ray(const LevelParams& p, int64_t ray, uint8_t* fbuf, float* rs_scratch,
-                                                  int ht, int hw, int lane, PhaseClock& clk) {
-  if (p.t_mode != 0 || p.vb_mode != 0) {
+// ---- the helper warps' work (ht = helper thread 0..95, hw = helper warp 0..2) ----
+// Tile tt of `ray` into the feature buffer fbuf: first (tt == 0) the ray prologue, once per ray, then the tile's
+// features.  The prologue's global stores (fenceposts, view bias) are read back by this CTA only, through L2 (ld.cg):
+// by the helpers after the helper barrier, by the consumers after feat_full.
+template <int kFmt, bool kX3, int kT>
+__device__ __forceinline__ void level_prepare_tile(const LevelParams& p, int64_t ray, int tt, uint8_t* fbuf,
+                                                   float* rs_scratch, int ht, int hw, int lane, PhaseClock& clk) {
+  constexpr int kNs = kT * kN;  // samples per ray
+  if ((kT == 1 || tt == 0) && (p.t_mode != 0 || p.vb_mode != 0)) {
     if (hw == 0) {
-      float* t_ray = p.t + ray * (kN + 1);
+      float* t_ray = p.t + ray * (kNs + 1);
       if (p.t_mode == 1) {  // coarse fenceposts (bit-identical to coarse_t_kernel)
         const float nr = __ldg(p.near + ray), fr = __ldg(p.far + ray);
         const bool jit = draws_active(p.t_rand);
-        for (int j = lane; j <= kN; j += 32)
-          __stcg(t_ray + j, coarse_fencepost(nr, fr, j, kN, p.disparity, jit,
-                                             jit ? draw_uniform(p.t_rand, ray, j, kN + 1) : 0.f));
+        for (int j = lane; j <= kNs; j += 32)
+          __stcg(t_ray + j, coarse_fencepost(nr, fr, j, kNs, p.disparity, jit,
+                                             jit ? draw_uniform(p.t_rand, ray, j, kNs + 1) : 0.f));
       } else if (p.t_mode == 2) {
-        resample_warp_lean<true>(p.t_prev + ray * (kN + 1), p.w_prev + ray * kN, kN, kN + 1, p.randomized,
+        resample_warp_lean<true>(p.t_prev + ray * (kNs + 1), p.w_prev + ray * kNs, kNs, kNs + 1, p.randomized,
                                  p.u_jitter, ray, p.resample_padding, rs_scratch, t_ray,
-                                 p.inds ? p.inds + ray * (kN + 1) : nullptr, lane);
+                                 p.inds ? p.inds + ray * (kNs + 1) : nullptr, lane);
       }
     } else if (hw == 1 && p.vb_mode == 1) {
       // per-ray view-layer bias  b[n] + W[n, 256:283] . pos_enc(viewdir)   (models/mip.py:353-363,
@@ -724,25 +733,29 @@ __device__ __forceinline__ void level_prepare_ray(const LevelParams& p, int64_t 
   // 32 units share their part
   RayGeom g{};
   if (!p.feat_in) g = load_ray_geom(p.origins, p.directions, p.radii, ray);
+  const int row0 = kT == 1 ? 0 : tt * kN;  // the tile's first row of the ray
 #pragma unroll 1
   for (int u = ht; u < 3 * kN; u += kHelperThreads) {
     const int row = u & (kN - 1), part = u / kN;
     float t0 = 0.f, t1 = 0.f;
-    if (!p.feat_in) t0 = __ldcg(p.t + ray * (kN + 1) + row), t1 = __ldcg(p.t + ray * (kN + 1) + row + 1);
-    ipe_row_group<kFmt, kX3>(p, g, ray, row, t0, t1, fbuf, 2 * part, 2 * part + 2);
+    if (!p.feat_in) t0 = __ldcg(p.t + ray * (kNs + 1) + row0 + row), t1 = __ldcg(p.t + ray * (kNs + 1) + row0 + row + 1);
+    ipe_row_group<kFmt, kX3, kT>(p, g, ray, row, t0, t1, fbuf, 2 * part, 2 * part + 2);
   }
   fence_proxy_async_smem();  // the features are read by wgmma (async proxy)
   clk.mark(kPhIpe);
 }
 
-// Activations + compositing of `ray` from its raw heads hd[128][4] (or, in MLP-only mode, the raw heads out), with the
-// summation order of a thread-per-row warpgroup: rows in four chunks of 32, chunk q on helper warp q % 3, each chunk
-// scanned / reduced within its warp, the chunks' carries and partial sums added in chunk order.  Each helper thread
-// arrives on heads_empty once it has read its rows' heads.
+// Activations + compositing of `ray` from its raw heads hd[128 kT][4] (or, in MLP-only mode, the raw heads out), with
+// the summation order of a thread-per-row warpgroup: rows in 4 kT chunks of 32, chunk q on helper warp q % 3, each
+// chunk scanned / reduced within its warp, the chunks' carries and partial sums added in chunk order, across the tile
+// boundary too.  One round per tile (chunks 4 u .. 4 u + 3 of tile u); each helper thread arrives on heads_empty[u]
+// once it has read its rows of tile u's heads.
+template <int kT>
 __device__ __forceinline__ void level_composite_ray(const LevelParams& p, int64_t ray, const float* hd,
                                                     uint64_t* heads_empty, float* cs, float* ps, int ht, int hw,
                                                     int lane, PhaseClock& clk) {
-  if (p.raw_rgb_out) {  // MLP-only mode: hand back the raw heads (models/mip_nerf.py:98,110)
+  constexpr int kNs = kT * kN;  // samples per ray
+  if (kT == 1 && p.raw_rgb_out) {  // MLP-only mode: hand back the raw heads (models/mip_nerf.py:98,110)
     for (int row = ht; row < kN; row += kHelperThreads) {
       const float4 h4 = *reinterpret_cast<const float4*>(hd + row * 4);
       const int64_t sidx = ray * kN + row;
@@ -755,60 +768,64 @@ __device__ __forceinline__ void level_composite_ray(const LevelParams& p, int64_
     clk.mark(kPhComposite);
     return;
   }
-  const float* t_ray = p.t + ray * (kN + 1);
+  const float* t_ray = p.t + ray * (kNs + 1);
   const float dx = __ldg(p.directions + ray * 3), dy = __ldg(p.directions + ray * 3 + 1),
               dz = __ldg(p.directions + ray * 3 + 2);
   const float dnorm = sqrtf(dx * dx + dy * dy + dz * dz);
-  constexpr int kChunksPerWarp = 2;  // chunks hw, hw + 3
-  float dd[kChunksPerWarp], excl[kChunksPerWarp], crgb[kChunksPerWarp][3], tmid[kChunksPerWarp];
+  constexpr int kChunksPerWarp = 2;  // chunks hw, hw + 3 of a tile
+#pragma unroll 1
+  for (int u = 0; u < kT; ++u) {
+    float dd[kChunksPerWarp], excl[kChunksPerWarp], crgb[kChunksPerWarp][3], tmid[kChunksPerWarp];
 #pragma unroll
-  for (int k = 0; k < kChunksPerWarp; ++k) {
-    const int q = hw + 3 * k, row = 32 * q + lane;
-    if (q >= 4) break;
-    const float4 h4 = *reinterpret_cast<const float4*>(hd + row * 4);
-    const int64_t sidx = ray * kN + row;
-    float raw_dens = h4.x + c_small.b_density;
-    if (draws_active(p.dnoise)) raw_dens = noisy_raw_density(raw_dens, p.dnoise, ray, row);  // models/mip_nerf.py:232-233
-    if (p.raw_rgb_keep) {  // training: the raw heads as well (render_backward recomputes the rest; the density head
-      p.raw_rgb_keep[sidx * 3 + 0] = h4.y + c_small.b_color[0];  // WITH its noise, so that softplus' is taken at the
-      p.raw_rgb_keep[sidx * 3 + 1] = h4.z + c_small.b_color[1];  // same point)
-      p.raw_rgb_keep[sidx * 3 + 2] = h4.w + c_small.b_color[2];
-      p.raw_density_keep[sidx] = raw_dens;
+    for (int k = 0; k < kChunksPerWarp; ++k) {
+      const int q = hw + 3 * k, row = 32 * (4 * u + q) + lane;  // row of the ray
+      if (q >= 4) break;
+      const float4 h4 = *reinterpret_cast<const float4*>(hd + row * 4);
+      const int64_t sidx = ray * kNs + row;
+      float raw_dens = h4.x + c_small.b_density;
+      if (draws_active(p.dnoise))  // models/mip_nerf.py:232-233
+        raw_dens = noisy_raw_density<kNs>(raw_dens, p.dnoise, ray, row);
+      if (kT == 1 && p.raw_rgb_keep) {  // training: the raw heads as well (render_backward recomputes the rest; the
+        p.raw_rgb_keep[sidx * 3 + 0] = h4.y + c_small.b_color[0];  // density head WITH its noise, so that softplus'
+        p.raw_rgb_keep[sidx * 3 + 1] = h4.z + c_small.b_color[1];  // is taken at the same point)
+        p.raw_rgb_keep[sidx * 3 + 2] = h4.w + c_small.b_color[2];
+        p.raw_density_keep[sidx] = raw_dens;
+      }
+      const float t0 = __ldcg(t_ray + row), t1 = __ldcg(t_ray + row + 1);
+      const float density = density_activation(raw_dens, p.density_bias);
+      crgb[k][0] = rgb_activation(h4.y + c_small.b_color[0], p.rgb_scale, p.rgb_padding);
+      crgb[k][1] = rgb_activation(h4.z + c_small.b_color[1], p.rgb_scale, p.rgb_padding);
+      crgb[k][2] = rgb_activation(h4.w + c_small.b_color[2], p.rgb_scale, p.rgb_padding);
+      tmid[k] = 0.5f * (t0 + t1);
+      dd[k] = density * ((t1 - t0) * dnorm);
+      float incl = dd[k];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const float n = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += n;
+      }
+      excl[k] = __shfl_up_sync(0xffffffffu, incl, 1);
+      if (lane == 0) excl[k] = 0.f;
+      if (lane == 31) cs[4 * u + q] = incl;
     }
-    const float t0 = __ldcg(t_ray + row), t1 = __ldcg(t_ray + row + 1);
-    const float density = density_activation(raw_dens, p.density_bias);
-    crgb[k][0] = rgb_activation(h4.y + c_small.b_color[0], p.rgb_scale, p.rgb_padding);
-    crgb[k][1] = rgb_activation(h4.z + c_small.b_color[1], p.rgb_scale, p.rgb_padding);
-    crgb[k][2] = rgb_activation(h4.w + c_small.b_color[2], p.rgb_scale, p.rgb_padding);
-    tmid[k] = 0.5f * (t0 + t1);
-    dd[k] = density * ((t1 - t0) * dnorm);
-    float incl = dd[k];
+    mbar_arrive(heads_empty + u);
+    clk.mark(kPhComposite);
+    named_bar_sync(kHelperBar, kHelperThreads);
+    clk.mark(kPhBarrier);
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const float n = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += n;
-    }
-    excl[k] = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0) excl[k] = 0.f;
-    if (lane == 31) cs[q] = incl;
-  }
-  mbar_arrive(heads_empty);
-  clk.mark(kPhComposite);
-  named_bar_sync(kHelperBar, kHelperThreads);
-  clk.mark(kPhBarrier);
-#pragma unroll
-  for (int k = 0; k < kChunksPerWarp; ++k) {
-    const int q = hw + 3 * k;
-    if (q >= 4) break;
-    float before = 0.f;
-    for (int qq = 0; qq < q; ++qq) before += cs[qq];
-    const float w = -expm1f(-dd[k]) * expf(-(before + excl[k]));
-    p.weights[ray * kN + 32 * q + lane] = w;
-    const float pr = warp_sum(w * crgb[k][0]), pg = warp_sum(w * crgb[k][1]), pb = warp_sum(w * crgb[k][2]),
-                pw = warp_sum(w), pd = warp_sum(w * tmid[k]);
-    if (lane == 0) {
-      float* dst = ps + q * 8;
-      dst[0] = pr, dst[1] = pg, dst[2] = pb, dst[3] = pw, dst[4] = pd;
+    for (int k = 0; k < kChunksPerWarp; ++k) {
+      const int q = hw + 3 * k, qr = 4 * u + q;  // chunk of the tile, of the ray
+      if (q >= 4) break;
+      float before = 0.f;
+      for (int qq = 0; qq < qr; ++qq) before += cs[qq];
+      const float w = -expm1f(-dd[k]) * expf(-(before + excl[k]));
+      p.weights[ray * kNs + 32 * qr + lane] = w;
+      const float pr = warp_sum(w * crgb[k][0]), pg = warp_sum(w * crgb[k][1]), pb = warp_sum(w * crgb[k][2]),
+                  pw = warp_sum(w), pd = warp_sum(w * tmid[k]);
+      if (lane == 0) {
+        float* dst = ps + qr * 8;
+        dst[0] = pr, dst[1] = pg, dst[2] = pb, dst[3] = pw, dst[4] = pd;
+      }
     }
   }
   clk.mark(kPhComposite);
@@ -816,9 +833,9 @@ __device__ __forceinline__ void level_composite_ray(const LevelParams& p, int64_
   clk.mark(kPhBarrier);
   if (ht == 0) {
     float s[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-    for (int qq = 0; qq < 4; ++qq)
+    for (int qq = 0; qq < 4 * kT; ++qq)
       for (int k = 0; k < 5; ++k) s[k] += ps[qq * 8 + k];
-    const float t_first = __ldcg(t_ray), t_last = __ldcg(t_ray + kN);
+    const float t_first = __ldcg(t_ray), t_last = __ldcg(t_ray + kNs);
     float d = s[4];
     if (isnan(d)) d = 0.f;
     else if (isinf(d)) d = d > 0 ? 3.4028234663852886e38f : -3.4028234663852886e38f;
@@ -835,9 +852,9 @@ __device__ __forceinline__ void level_composite_ray(const LevelParams& p, int64_
   clk.mark(kPhBarrier);
 }
 
-template <int kFmt, bool kX3>
+template <int kFmt, bool kX3, int kT>
 __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParams p) {
-  using Lay = LevelLayout<kX3>;
+  using Lay = LevelLayout<kX3, kT>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
@@ -851,9 +868,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   uint64_t* heads_full = feat_empty + Lay::kFeatBufs;  // [2] consumers (kHeadsWriters arrives) -> helpers
   uint64_t* heads_empty = heads_full + 2;              // [2] helpers (kHelperThreads arrives) -> consumers
   float* heads = reinterpret_cast<float*>(heads_empty + 2);  // [2][128][4] raw density, rgb dots
-  float* cs = heads + 2 * kN * 4;                            // [4] scan carries
-  float* ps = cs + 4;                                        // [4][8] partial sums
-  float* rs_scratch = ps + 32;                               // [129] resampler scratch
+  float* cs = heads + 2 * kN * 4;                            // [4 kT] scan carries
+  float* ps = cs + 4 * kT;                                   // [4 kT][8] partial sums
+  float* rs_scratch = ps + 32 * kT;                          // [128 kT + 1] resampler scratch
   unsigned long long* phase_rows = reinterpret_cast<unsigned long long*>(smem + Lay::kPhase);
   const int phase_slot = p.t_mode == 2 ? 1 : 0;
   PhaseClock clk;
@@ -879,24 +896,33 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(kProducerRegs) : "memory");
     if (warp >= kHelperWarp0) {
       // ============================ helpers (warps 9-11): a two-stage ray pipeline ============================
-      // prepare ray i (into feature buffer i % kFeatBufs, once the consumers are done with its previous ray), then
-      // composite ray i - 1; the consumers meanwhile run the layers of ray i - 1 and then ray i.
+      // prepare tile 0 of ray i (into feature buffer j % kFeatBufs, j the tile's index in the CTA, once the consumers
+      // are done with its previous tile), composite ray i - 1, then prepare the other tile of ray i; the consumers
+      // meanwhile run the layers of the tiles of ray i - 1 and then of ray i.  With kT = 2 the raw heads of a ray's
+      // tiles 0 / 1 are in heads[0] / heads[1], i.e. rows 0..255 of heads.
       const int ht = tid - 32 * kHelperWarp0, hw = warp - kHelperWarp0;
       clk.begin(phase_rows + 3 * kNumPhases, ht == 0);
       for (int64_t ray = blockIdx.x, i = 0;; ray += gridDim.x, ++i) {
         const bool more = ray < p.num_rays;
-        if (more) {
-          const int fb = (int)(i % Lay::kFeatBufs);
-          mbar_wait(&feat_empty[fb], ((uint32_t)(i / Lay::kFeatBufs) & 1u) ^ 1u);
-          clk.mark(kPhFeatEmpty);
-          level_prepare_ray<kFmt, kX3>(p, ray, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane, clk);
-          mbar_arrive(&feat_full[fb]);
-        }
-        if (i > 0) {  // ray - gridDim.x, the (i - 1)-th ray of the CTA
-          const int par = (int)((i - 1) & 1);
-          mbar_wait(&heads_full[par], (uint32_t)((i - 1) >> 1) & 1u);
-          clk.mark(kPhHeadsFull);
-          level_composite_ray(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], cs, ps, ht, hw, lane, clk);
+#pragma unroll 1
+        for (int tt = 0; tt < kT; ++tt) {
+          const int64_t j = i * kT + tt;
+          if (more) {
+            const int fb = (int)(j % Lay::kFeatBufs);
+            mbar_wait(&feat_empty[fb], ((uint32_t)(j / Lay::kFeatBufs) & 1u) ^ 1u);
+            clk.mark(kPhFeatEmpty);
+            level_prepare_tile<kFmt, kX3, kT>(p, ray, tt, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane, clk);
+            mbar_arrive(&feat_full[fb]);
+          }
+          if (tt == 0 && i > 0) {  // ray - gridDim.x, the (i - 1)-th ray of the CTA: tiles (i - 1) kT ..
+            const int par = (int)(((i - 1) * kT) & 1);  // kT = 2: 0
+#pragma unroll
+            for (int u = 0; u < kT; ++u)
+              mbar_wait(&heads_full[par + u], (uint32_t)(((i - 1) * kT + u) >> 1) & 1u);
+            clk.mark(kPhHeadsFull);
+            level_composite_ray<kT>(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], cs, ps, ht, hw, lane,
+                                    clk);
+          }
         }
         if (!more) break;
       }
@@ -909,7 +935,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       int st = 0;
       uint32_t ph = 0;
       const uint64_t pol = l2_policy_evict_last();  // the image is re-read by every CTA for every ray
-      for (int64_t ray = blockIdx.x; ray < p.num_rays; ray += gridDim.x) {
+      for (int64_t tile = 0, ray = blockIdx.x; ray < p.num_rays; ray += ++tile % kT == 0 ? gridDim.x : 0) {
         const uint8_t* src = p.wimage;  // the stages are contiguous in issue order (w_stages_contiguous)
         for (int l = 0; l < kNumLayers; ++l)
           for (int h = 0; h < num_halves(l); ++h)  // N-half major, then K-slab
@@ -943,15 +969,17 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   const SmallParams* __restrict__ gsp = reinterpret_cast<const SmallParams*>(p.wimage + kSmallOffset);
   const uint32_t a_u = smem_u32(sA) + (uint32_t)wg * 64u * 128u;
   const uint32_t w_u = smem_u32(sW);
-  const uint64_t dump_policy = p.act_dump ? l2_policy_evict_first() : 0ull;  // the dump must not evict the weights
+  // the training forward's dump (p.act_dump, p.v_dump) exists for kT = 1 only
+  const uint64_t dump_policy = kT == 1 && p.act_dump ? l2_policy_evict_first() : 0ull;  // must not evict the weights
   bool dump_pending = false;
   RingPos rp{0, 0u, -1};
   clk.begin(phase_rows + wg * kNumPhases, leader);
-  for (int64_t ray = blockIdx.x, i = 0; ray < p.num_rays; ray += gridDim.x, ++i) {
-    // the ray's feature buffer and raw-heads parity, and their mbarrier phases
+  // tile i of the CTA is tile i % kT of `ray`; every tile of a ray adds the ray's one view bias
+  for (int64_t ray = blockIdx.x, i = 0; ray < p.num_rays; ray += ++i % kT == 0 ? gridDim.x : 0) {
+    // the tile's feature buffer and raw-heads parity, and their mbarrier phases
     const int fb = (int)(i % Lay::kFeatBufs), par = (int)(i & 1);
     const uint32_t fph = (uint32_t)(i / Lay::kFeatBufs) & 1u, hph = (uint32_t)(i >> 1) & 1u;
-    // this warpgroup's rows of the ray's feature buffer (SW128 slab, SW64 tail)
+    // this warpgroup's rows of the tile's feature buffer (SW128 slab, SW64 tail)
     const uint32_t f_u = smem_u32(sF) + (uint32_t)fb * Lay::kFBuf + (uint32_t)wg * 64u * 128u;
     const uint32_t ft_u = smem_u32(sF) + (uint32_t)fb * Lay::kFBuf + kStageBytes + (uint32_t)wg * 64u * 64u;
     mbar_wait(&feat_full[fb], fph);
@@ -990,7 +1018,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       // feature tile; layer 0 has two K-slabs (64 wide + the 32-wide tail), and two of its acc0 chunks follow each.  The
       // training forward's activation tiles go out from the epilogue's registers.
       const LevelRsCtx k{f_u, ft_u, w_u, w_full, w_empty, &feat_empty[fb], gsp,
-                         p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
+                         kT == 1 && p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
                          (size_t)p.dump_tiles * kABytes, dump_policy, r0, cq, leader};
       uint32_t xa[64], xb[64];
       static_assert(2 * num_slabs(true, 0) == kEpiChunks, "layer 0: two acc0 chunks after each of its K-slabs");
@@ -1073,7 +1101,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
         clk.mark(kPhEpilogue);
         named_bar_sync(1 + wg, 128);
         clk.mark(kPhBarrier);
-        if (p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core reads it
+        if (kT == 1 && p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core
+          // reads it
           if (leader) {
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
@@ -1098,7 +1127,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
     {
       // view layer + colour head (models/mip_nerf.py:106-110); view_bias = the per-ray view-direction term
       const float* vb = p.view_bias + ray * kCond;
-      uint8_t* vd = p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
+      uint8_t* vd = kT == 1 && p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int c = 8 * j + cq;
@@ -1297,11 +1326,14 @@ struct TcScratch {
   float *vbias, *t[2], *w[2];
   size_t bytes;
 };
+// rays per launch of the level kernels: 65536 at 128 samples, 32768 at 256 (the same scratch per chunk, and still
+// 500 rays per SM)
 constexpr int64_t kChunkRaysTc = 65536;
+inline int64_t tc_chunk_rays(int n) { return kChunkRaysTc * kN / n; }
 
 inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
-TcScratch carve_tc(int64_t rays, void* base) {
+TcScratch carve_tc(int64_t rays, int n, void* base) {
   TcScratch s{};
   size_t off = 0;
   auto take = [&](size_t elems) {
@@ -1311,8 +1343,8 @@ TcScratch carve_tc(int64_t rays, void* base) {
   };
   s.vbias = take((size_t)rays * kCond);
   for (int i = 0; i < 2; ++i) {
-    s.t[i] = take((size_t)rays * (kN + 1));
-    s.w[i] = take((size_t)rays * kN);
+    s.t[i] = take((size_t)rays * (n + 1));
+    s.w[i] = take((size_t)rays * n);
   }
   s.bytes = off;
   return s;
@@ -1324,10 +1356,10 @@ int g_num_sms = 0;
 inline int fmt_of(int precision) { return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_BF16X3) ? 1 : 0; }
 inline bool is_x3(int precision) { return precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3; }
 
-template <int kFmt, bool kX3>
+template <int kFmt, bool kX3, int kT>
 cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
-  auto kern = mlp_level_kernel<kFmt, kX3>;
-  constexpr uint32_t smem = LevelLayout<kX3>::kTotal;
+  auto kern = mlp_level_kernel<kFmt, kX3, kT>;
+  constexpr uint32_t smem = LevelLayout<kX3, kT>::kTotal;
   static bool attr_set = false;  // one flag per instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -1345,11 +1377,16 @@ cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_level(const LevelParams& p, int precision, cudaStream_t st) {
-  if (p.num_rays <= 0) return cudaSuccess;
+// n = 128 or 256 samples per ray: one or two 128-row tiles per ray
+template <int kT>
+cudaError_t launch_level_tiles(const LevelParams& p, int precision, cudaStream_t st) {
   if (is_x3(precision))
-    return fmt_of(precision) ? launch_level_t<1, true>(p, st) : launch_level_t<0, true>(p, st);
-  return fmt_of(precision) ? launch_level_t<1, false>(p, st) : launch_level_t<0, false>(p, st);
+    return fmt_of(precision) ? launch_level_t<1, true, kT>(p, st) : launch_level_t<0, true, kT>(p, st);
+  return fmt_of(precision) ? launch_level_t<1, false, kT>(p, st) : launch_level_t<0, false, kT>(p, st);
+}
+cudaError_t launch_level(const LevelParams& p, int precision, int n, cudaStream_t st) {
+  if (p.num_rays <= 0) return cudaSuccess;
+  return n == 2 * kN ? launch_level_tiles<2>(p, precision, st) : launch_level_tiles<1>(p, precision, st);
 }
 
 }  // namespace
@@ -1363,7 +1400,7 @@ cudaError_t launch_level(const LevelParams& p, int precision, cudaStream_t st) {
 bool tc_default_degrees(const mipnerf_b200_config* c) { return c->max_deg_point == 16 && c->deg_view == 4; }
 bool tc_supported(const mipnerf_b200_config* c, int precision) {
   return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_FP16 || is_x3(precision)) &&
-         c->num_samples == kN &&
+         (c->num_samples == kN || c->num_samples == 2 * kN) &&
          c->min_deg_point == 0 && c->max_deg_point >= 1 && c->max_deg_point <= 16 && c->deg_view >= 1 &&
          c->deg_view <= 4 && c->use_viewdirs &&
          c->net_depth == 8 && c->net_width == kWidth && c->net_depth_condition == 1 &&
@@ -1390,8 +1427,8 @@ size_t tc_packed_bytes(const mipnerf_b200_config* c, int precision) {
 
 size_t tc_workspace_bytes(const mipnerf_b200_config* c, int64_t num_rays, int precision) {
   if (!tc_supported(c, precision)) return 0;
-  const int64_t r = num_rays < kChunkRaysTc ? num_rays : kChunkRaysTc;
-  return carve_tc(r > 0 ? r : 1, nullptr).bytes;
+  const int64_t chunk = tc_chunk_rays(c->num_samples), r = num_rays < chunk ? num_rays : chunk;
+  return carve_tc(r > 0 ? r : 1, c->num_samples, nullptr).bytes;
 }
 
 cudaError_t tc_pack_weights(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, int precision,
@@ -1478,25 +1515,28 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
   cudaError_t e = small.error();
   if (e != cudaSuccess) return e;
   const float rgb_scale = (float)(1.0 + 2.0 * (double)c->rgb_padding);
-  for (int64_t off = 0; off < rays->num_rays; off += kChunkRaysTc) {
-    const int64_t cnt = (rays->num_rays - off) < kChunkRaysTc ? (rays->num_rays - off) : kChunkRaysTc;
-    const TcScratch s = carve_tc(cnt, workspace);
+  const int n = c->num_samples;
+  const int64_t chunk = tc_chunk_rays(n);
+  if (dump && n != kN) return cudaErrorNotSupported;  // the training dump is one tile per ray
+  for (int64_t off = 0; off < rays->num_rays; off += chunk) {
+    const int64_t cnt = (rays->num_rays - off) < chunk ? (rays->num_rays - off) : chunk;
+    const TcScratch s = carve_tc(cnt, n, workspace);
     if (s.bytes > workspace_bytes) return cudaErrorInvalidValue;
     const float* origins = rays->origins + off * 3;
     const float* directions = rays->directions + off * 3;
     const float* radii = rays->radii + off;
     // in-kernel Philox: the counter is the ray index of the caller's whole batch (ray_base = offset of `rays` in it)
     auto draws = [&](const float* array, int stream) {
-      Draws d = level_draws(randomized, array, rng, off, stream, kN + 1);
+      Draws d = level_draws(randomized, array, rng, off, stream, n + 1);
       if (!array) d.ray_base += ray_base;
       return d;
     };
     const float *t_prev = nullptr, *w_prev = nullptr;
     for (int l = 0; l < c->num_levels; ++l) {
-      float* t_cur = outs[l].t_samples ? outs[l].t_samples + off * (kN + 1) : s.t[l & 1];
-      float* w_cur = outs[l].weights ? outs[l].weights + off * kN : s.w[l & 1];
+      float* t_cur = outs[l].t_samples ? outs[l].t_samples + off * (n + 1) : s.t[l & 1];
+      float* w_cur = outs[l].weights ? outs[l].weights + off * n : s.w[l & 1];
       const Draws jit = draws(u_jitter, 1 + l);  // one stream per level
-      int64_t* inds = outs[l].inds ? outs[l].inds + off * (kN + 1) : nullptr;
+      int64_t* inds = outs[l].inds ? outs[l].inds + off * (n + 1) : nullptr;
       LevelParams p{};
       p.wimage = img;
       p.origins = origins, p.directions = directions, p.radii = radii;
@@ -1526,9 +1566,9 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
       p.white_bkgd = white_bkgd;
       p.disable_integration = c->disable_integration;
       p.density_bias = c->density_bias, p.rgb_scale = rgb_scale, p.rgb_padding = c->rgb_padding;
-      p.dnoise = density_noise_draws(c, randomized, outs[l].density_normal, rng, off, l, kN);
+      p.dnoise = density_noise_draws(c, randomized, outs[l].density_normal, rng, off, l, n);
       if (!outs[l].density_normal) p.dnoise.ray_base += ray_base;
-      e = launch_level(p, precision, st);
+      e = launch_level(p, precision, n, st);
       if (e != cudaSuccess) return e;
       t_prev = t_cur;
       w_prev = w_cur;
@@ -1560,7 +1600,7 @@ cudaError_t tc_mlp_forward(const mipnerf_b200_config* c, const mipnerf_b200_weig
   p.raw_rgb_out = raw_rgb;
   p.raw_density_out = raw_density;
   p.num_rays = num_rays;
-  return launch_level(p, precision, st);
+  return launch_level(p, precision, kN, st);
 }
 
 cudaError_t launch_view_bias_from_enc(const float* venc, const float* w, const float* b, float* out,

@@ -147,8 +147,9 @@ class MLP(torch.nn.Module):
         lib = _cabi.lib()
         nbytes = lib.mipnerf_b200_packed_weights_bytes(C.byref(cfg), precision)
         if nbytes == 0:
-            raise NotImplementedError("tensor-core path: the 8x256 / 1x128 MLP with num_samples=128, min_deg_point=0, "
-                                      "max_deg_point 1..16 and deg_view 1..4 is implemented; use precision='fp32'")
+            raise NotImplementedError("tensor-core path: the 8x256 / 1x128 MLP with num_samples 128 or 256, "
+                                      "min_deg_point=0, max_deg_point 1..16 and deg_view 1..4 is implemented; "
+                                      "use precision='fp32'")
         packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
         with torch.cuda.device(device):
             _cabi.check(lib.mipnerf_b200_pack_weights(C.byref(cfg), C.byref(ws), precision, packed.data_ptr(),
