@@ -339,6 +339,33 @@ int mipnerf_b200_resample_along_rays(const mipnerf_b200_rays* rays, const float*
                                      float* new_t_samples, float* means, float* covs, int64_t* inds,
                                      void* stream);
 
+/* ---- density queries and meshes ----
+ * Density of the field at Gaussians: means [P,3], diagonal covs [P,3] (NULL: zero covariance, i.e. plain positional
+ * encoding) -> the IPE (models/mip.py:322-350) -> trunk (layers 0-7, skip after 4) -> density_layer
+ * (models/mip_nerf.py:93-98).  raw_density [P] = MLP.forward's raw density (no noise); density [P] =
+ * softplus(raw + cfg->density_bias).  Either output may be NULL, not both; cfg->disable_integration zeroes covs.
+ * FP32 takes any config check_config accepts; the tensor-core precisions the configs the forward takes on the tensor
+ * cores (see the precision list above), through the density-only mode of the level kernel.  Points run in launch
+ * chunks; results do not depend on how a query is split. */
+size_t mipnerf_b200_density_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points, int precision);
+int mipnerf_b200_query_density(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                               const float* covs, int64_t num_points, int precision, float* raw_density,
+                               float* density, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Isosurface of a scalar grid [nz, ny, nx] fp32 (x fastest, every dimension >= 2) by marching tetrahedra (6 Kuhn
+ * tetrahedra per cell): a watertight indexed mesh whose normals point from inside (value > iso; NaN is outside) to
+ * outside.  Pass 1 writes counts[2] (device int64: vertices, faces); pass 2, with the same scratch, writes verts [V,3]
+ * fp32 and faces [F,3] int32 (lo_host / hi_host: HOST float[3], the positions of lattice points 0 and n-1 per axis).
+ * Vertex ids follow (lattice point in x-fastest order, edge direction x, y, z, x+y, x+z, y+z, x+y+z), faces (cell,
+ * tetrahedron, triangle): the output is bit-reproducible.  Emit reads the vertex count back (one stream synchronise)
+ * and answers MIPNERF_B200_EUNSUPPORTED when int32 indices cannot address it. */
+size_t mipnerf_b200_isosurface_scratch_bytes(int nx, int ny, int nz);
+int mipnerf_b200_isosurface_count(const float* grid, int nx, int ny, int nz, float iso, void* scratch,
+                                  size_t scratch_bytes, int64_t* counts, void* stream);
+int mipnerf_b200_isosurface_emit(const float* grid, int nx, int ny, int nz, const float* lo_host,
+                                 const float* hi_host, float iso, const void* scratch, float* verts,
+                                 int32_t* faces, void* stream);
+
 /* Hardware self-test of the wgmma building blocks (descriptor / swizzle / accumulator-fragment conventions):
  * d[128,n] = a[128,k] . b[n,k]^T, 16-bit operands (precision BF16|FP16), fp32 accumulate; n in {128, 256}.
  * variant bit 0: B through a pre-swizzled image + cp.async.bulk (needs `scratch`); bit 1: A in registers (the RS form

@@ -125,6 +125,13 @@ _SIGNATURES = {
     "mipnerf_b200_sorted_piecewise_constant_pdf": (C.c_int, [_V, _V, C.c_int64, C.c_int, C.c_int, C.c_int, _V, _V, _V, _V]),
     "mipnerf_b200_resample_along_rays": (C.c_int, [C.POINTER(RaysStruct), _V, _V, C.c_int, C.c_int, _V, C.c_float,
                                                    _V, _V, _V, _V, _V]),
+    "mipnerf_b200_density_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int]),
+    "mipnerf_b200_query_density": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), _V, _V, C.c_int64, C.c_int, _V, _V,
+                                             _V, C.c_size_t, _V]),
+    "mipnerf_b200_isosurface_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "mipnerf_b200_isosurface_count": (C.c_int, [_V, C.c_int, C.c_int, C.c_int, C.c_float, _V, C.c_size_t, _V, _V]),
+    "mipnerf_b200_isosurface_emit": (C.c_int, [_V, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.c_float, _V, _V, _V,
+                                               _V]),
     "mipnerf_b200_selftest_umma": (C.c_int, [_V, _V, _V, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),
     "mipnerf_b200_profile_enable": (C.c_int, [C.c_int]),
     "mipnerf_b200_profile_num_kernels": (C.c_int, []),

@@ -154,17 +154,15 @@ Fp32Scratch carve_fp32(const mipnerf_b200_config* c, const Dims& d, int64_t rays
   return s;
 }
 
-// MLP.forward on the fp32 path (models/mip_nerf.py:75-111).
-int mlp_forward_fp32(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w,
-                     const float* x, const float* venc, int64_t rays, int n, const Fp32Scratch& s,
-                     float* raw_rgb, float* raw_density, cudaStream_t st) {
-  const int64_t m = rays * n;
+// The trunk on the fp32 path (models/mip_nerf.py:93-97): x [m, xyz_dim] -> *out (h0 or h1), [m, net_width].
+int trunk_fp32(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w, const float* x, int64_t m,
+               float* h0, float* h1, const float** out_h, cudaStream_t st) {
   const float* cur = x;
   int cur_k = d.xyz_dim;
   bool concat = false;
   for (int i = 0; i < c->net_depth; ++i) {
     const mipnerf_b200_linear& l = w->linears[i];
-    float* out = (i & 1) ? s.h1 : s.h0;
+    float* out = (i & 1) ? h1 : h0;
     CUDA_TRY(mipnerf::launch_linear_f32(cur, cur_k, cur_k, concat ? x : nullptr, d.xyz_dim,
                                         concat ? d.xyz_dim : 0, 1, l.weight, l.bias, out, c->net_width, m,
                                         c->net_width, 1, st));
@@ -172,6 +170,19 @@ int mlp_forward_fp32(const mipnerf_b200_config* c, const Dims& d, const mipnerf_
     cur_k = c->net_width;
     concat = (i % c->skip_index == 0 && i > 0);  // models/mip_nerf.py:96-97
   }
+  *out_h = cur;
+  return MIPNERF_B200_OK;
+}
+
+// MLP.forward on the fp32 path (models/mip_nerf.py:75-111).
+int mlp_forward_fp32(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w,
+                     const float* x, const float* venc, int64_t rays, int n, const Fp32Scratch& s,
+                     float* raw_rgb, float* raw_density, cudaStream_t st) {
+  const int64_t m = rays * n;
+  const float* cur;
+  int rc;
+  if ((rc = trunk_fp32(c, d, w, x, m, s.h0, s.h1, &cur, st))) return rc;
+  const int cur_k = c->net_width;
   const mipnerf_b200_linear& dl = w->linears[c->net_depth];
   CUDA_TRY(mipnerf::launch_linear_f32(cur, cur_k, cur_k, nullptr, 0, 0, 1, dl.weight, dl.bias, raw_density,
                                       1, m, 1, 0, st));
@@ -1242,6 +1253,126 @@ int mipnerf_b200_resample_along_rays(const mipnerf_b200_rays* rays, const float*
   if (means && covs)
     CUDA_TRY(mipnerf::launch_cast_rays(rays->origins, rays->directions, rays->radii, new_t_samples, means,
                                        covs, rays->num_rays, num_samples, st));
+  return MIPNERF_B200_OK;
+}
+
+// ---- density queries and isosurface extraction ----------------------------------------------------
+namespace {
+// the fp32 density query runs as many points per chunk as the fp32 forward has samples per chunk
+constexpr int64_t kChunkPointsFp32 = kChunkRaysFp32 * 128;
+
+struct DensityScratch {
+  float *zero_covs, *enc, *h0, *h1, *raw;
+  size_t bytes;
+};
+DensityScratch carve_density(const mipnerf_b200_config* c, const Dims& d, int64_t m, void* base) {
+  DensityScratch s{};
+  size_t off = 0;
+  auto take = [&](size_t elems) {
+    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
+    off += align_up(elems * sizeof(float));
+    return p;
+  };
+  s.zero_covs = take((size_t)m * 3);
+  s.enc = take((size_t)m * d.xyz_dim);
+  s.h0 = take((size_t)m * c->net_width);
+  s.h1 = take((size_t)m * c->net_width);
+  s.raw = take((size_t)m);
+  s.bytes = off;
+  return s;
+}
+}  // namespace
+
+size_t mipnerf_b200_density_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points, int precision) {
+  Dims d;
+  if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0 || precision != MIPNERF_B200_FP32) return 0;
+  const int64_t m = num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32;
+  return carve_density(cfg, d, m > 0 ? m : 1, nullptr).bytes;
+}
+
+int mipnerf_b200_query_density(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                               const float* covs, int64_t num_points, int precision, float* raw_density,
+                               float* density, void* workspace, size_t workspace_bytes, void* stream) {
+  Dims d;
+  int rc;
+  if ((rc = check_config(cfg, &d))) return rc;
+  if ((rc = check_weights(cfg, d, w))) return rc;
+  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if (!raw_density && !density) return fail(MIPNERF_B200_EINVAL, "raw_density and density are both NULL");
+  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
+  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
+    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
+  if (precision != MIPNERF_B200_FP32) {
+    if (!mipnerf::tc_supported(cfg, precision))
+      return fail(MIPNERF_B200_EUNSUPPORTED,
+                  "tensor-core density query: the forward's tensor-core shapes only (8x256 / 1x128 model, "
+                  "num_samples 128 or 256, min_deg_point 0, max_deg_point 1..16, deg_view 1..4); use MIPNERF_B200_FP32");
+    if (!w->packed || w->packed_precision != precision || w->packed_bytes < mipnerf::tc_packed_bytes(cfg, precision))
+      return fail(MIPNERF_B200_EINVAL, "weights->packed missing or packed for another precision");
+  }
+  const size_t need = mipnerf_b200_density_workspace_bytes(cfg, num_points, precision);
+  if (num_points > 0 && need > 0 && (!workspace || workspace_bytes < need))
+    return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
+  if (num_points == 0) return MIPNERF_B200_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (precision != MIPNERF_B200_FP32) {
+    cudaError_t e = mipnerf::tc_query_density(cfg, w, means, covs, num_points, precision, raw_density, density, st);
+    if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "tc_query_density: %s", cudaGetErrorString(e));
+    return MIPNERF_B200_OK;
+  }
+  // fp32: the IPE stage kernel, the fp32 trunk and density_layer (models/mip.py:322-350, models/mip_nerf.py:93-98)
+  const mipnerf_b200_linear& dl = w->linears[cfg->net_depth];
+  for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
+    const int64_t m = (num_points - off) < kChunkPointsFp32 ? (num_points - off) : kChunkPointsFp32;
+    const DensityScratch s = carve_density(cfg, d, m, workspace);
+    const float* cv = covs ? covs + off * 3 : nullptr;
+    if (!cv || cfg->disable_integration) {
+      CUDA_TRY(cudaMemsetAsync(s.zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
+      cv = s.zero_covs;
+    }
+    CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, s.enc, m, cfg->min_deg_point, cfg->max_deg_point, st));
+    const float* h;
+    if ((rc = trunk_fp32(cfg, d, w, s.enc, m, s.h0, s.h1, &h, st))) return rc;
+    float* raw = raw_density ? raw_density + off : s.raw;
+    CUDA_TRY(mipnerf::launch_linear_f32(h, cfg->net_width, cfg->net_width, nullptr, 0, 0, 1, dl.weight, dl.bias, raw, 1,
+                                        m, 1, 0, st));
+    if (density) CUDA_TRY(mipnerf::launch_density_activation(raw, density + off, m, cfg->density_bias, st));
+  }
+  return MIPNERF_B200_OK;
+}
+
+size_t mipnerf_b200_isosurface_scratch_bytes(int nx, int ny, int nz) {
+  if (nx < 2 || ny < 2 || nz < 2) return 0;
+  return mipnerf::isosurface_scratch_bytes(nx, ny, nz);
+}
+
+int mipnerf_b200_isosurface_count(const float* grid, int nx, int ny, int nz, float iso, void* scratch,
+                                  size_t scratch_bytes, int64_t* counts, void* stream) {
+  if (nx < 2 || ny < 2 || nz < 2) return fail(MIPNERF_B200_EINVAL, "grid %d x %d x %d: need >= 2 per axis", nx, ny, nz);
+  if (!grid || !counts) return fail(MIPNERF_B200_EINVAL, "grid / counts is NULL");
+  const size_t need = mipnerf::isosurface_scratch_bytes(nx, ny, nz);
+  if (!scratch || scratch_bytes < need) return fail(MIPNERF_B200_EWORKSPACE, "scratch %zu < %zu bytes", scratch_bytes, need);
+  CUDA_TRY(mipnerf::launch_isosurface_count(grid, nx, ny, nz, iso, scratch, counts, (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_isosurface_emit(const float* grid, int nx, int ny, int nz, const float* lo_host, const float* hi_host,
+                                 float iso, const void* scratch, float* verts, int32_t* faces, void* stream) {
+  if (nx < 2 || ny < 2 || nz < 2) return fail(MIPNERF_B200_EINVAL, "grid %d x %d x %d: need >= 2 per axis", nx, ny, nz);
+  if (!grid || !lo_host || !hi_host || !scratch) return fail(MIPNERF_B200_EINVAL, "grid / bounds / scratch is NULL");
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t totals[2];
+  CUDA_TRY(cudaMemcpyAsync(totals, mipnerf::isosurface_totals(scratch), sizeof(totals), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (totals[0] > INT32_MAX)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "%lld vertices: int32 face indices cannot address them",
+                (long long)totals[0]);
+  if ((totals[0] > 0 && !verts) || (totals[1] > 0 && !faces)) return fail(MIPNERF_B200_EINVAL, "verts / faces is NULL");
+  if (totals[0] == 0) return MIPNERF_B200_OK;
+  const int n[3] = {nx, ny, nz};
+  float step[3];
+  for (int a = 0; a < 3; ++a) step[a] = (hi_host[a] - lo_host[a]) / (float)(n[a] - 1);
+  CUDA_TRY(mipnerf::launch_isosurface_emit(grid, nx, ny, nz, lo_host, step, iso, scratch, verts, faces, st));
   return MIPNERF_B200_OK;
 }
 

@@ -45,6 +45,18 @@ cudaError_t launch_composite(const float* rgb, const float* dens, const float* t
 cudaError_t launch_resample(const float* bins, const float* weights, const Draws& jitter, float* out,
                             int64_t* inds, int64_t num_rays, int nb, int ns, int randomized, int blur,
                             float padding, cudaStream_t st);
+// density[i] = softplus(raw[i] + density_bias)  (models/mip_nerf.py:237)
+cudaError_t launch_density_activation(const float* raw, float* density, int64_t n, float density_bias, cudaStream_t st);
+
+// ---- isosurface.cu (marching tetrahedra; grid [nz, ny, nx], x fastest) ----
+size_t isosurface_scratch_bytes(int nx, int ny, int nz);
+// the device int64 [2] (vertices, faces) that launch_isosurface_count leaves at the start of the scratch
+const int64_t* isosurface_totals(const void* scratch);
+cudaError_t launch_isosurface_count(const float* grid, int nx, int ny, int nz, float iso, void* scratch,
+                                    int64_t* counts, cudaStream_t st);
+// lo / step: HOST float[3] (lattice point idx at lo + idx * step per axis)
+cudaError_t launch_isosurface_emit(const float* grid, int nx, int ny, int nz, const float* lo, const float* step,
+                                   float iso, const void* scratch, float* verts, int32_t* faces, cudaStream_t st);
 
 // ---- metrics.cu ----
 size_t image_metrics_scratch_bytes(int height, int width, int channels);

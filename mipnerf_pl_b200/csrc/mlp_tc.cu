@@ -154,6 +154,13 @@ struct LevelParams {
   int disable_integration;
   float density_bias, rgb_scale, rgb_padding;
   Draws dnoise;  // density noise of randomized mode (models/mip_nerf.py:232-233): normals [B,128] or in-kernel; scale = std
+  // Density-only mode (mipnerf_b200_query_density): tile i holds points 128 i .. 128 i + 127 of the Gaussians
+  // q_means / q_covs [num_points, 3] (q_covs null: zero covariance); raw density into raw_density_out, softplus(raw +
+  // density_bias) into density_out (either may be null).  num_rays counts the tiles.
+  const float* q_means;
+  const float* q_covs;
+  int64_t num_points;
+  float* density_out;
 };
 
 // raw density of (ray, row) of a ray of kNs samples with the density noise added; kept out of line so that the
@@ -250,13 +257,24 @@ __device__ __forceinline__ void store8_split(uint8_t* dst_hi, uint8_t* dst_lo, c
 
 // Gaussian + IPE features [8 gi_begin, 8 gi_end) and [48 + 8 gi_begin, 48 + 8 gi_end) of one sample row of a ray (or,
 // in MLP-only mode, the caller's features) into the feature tile: SW128 slab (K 0..63) + SW64 tail (K 64..95).  `row`
-// is the row of the tile; MLP-only mode has one tile per ray.
-template <int kFmt, bool kX3, int kT>
+// is the row of the tile; MLP-only mode has one tile per ray.  kDensity: the row is query point 128 ray + row (zero
+// past the last one), encoded with the IPE of mipnerf_b200_integrated_pos_enc (ipe_pair<false>), so that the 16-bit
+// features equal MLP-only mode's rounding of that entry point's output.
+template <int kFmt, bool kX3, int kT, bool kDensity = false>
 __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeom& g, int64_t ray, int row, float t0,
                                               float t1, uint8_t* myF, int gi_begin, int gi_end) {
   float mean[3] = {0.f, 0.f, 0.f}, cov[3] = {0.f, 0.f, 0.f};
   const float* fin = nullptr;
-  if (kT == 1 && p.feat_in) {
+  if (kDensity) {
+    const int64_t pt = ray * kN + row;
+    if (pt < p.num_points) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        mean[c] = __ldg(p.q_means + pt * 3 + c);
+        cov[c] = p.q_covs && !p.disable_integration ? __ldg(p.q_covs + pt * 3 + c) : 0.f;
+      }
+    }
+  } else if (kT == 1 && p.feat_in) {
     fin = p.feat_in + (ray * kN + row) * kFeat;  // MLP-only mode: the caller's encoding
   } else {
     float tm, tv, rv;
@@ -280,7 +298,7 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
         const int f = gi * 8 + e;  // feature index = degree*3 + coord   (models/mip.py:335-341)
         // (measured: the accurate sinf / expf in place of the MUFU pair changes the split modes' error against the
         //  reference goldens by < 3 % — 1.06e-4 vs 1.08e-4 on the worst one — and costs 7x the IPE time: not used)
-        ipe_pair<true>(mean[f % 3], cov[f % 3], f / 3, fsin[e], fcos[e]);
+        ipe_pair<!kDensity>(mean[f % 3], cov[f % 3], f / 3, fsin[e], fcos[e]);
       }
     }
     const uint32_t o_sin = sw128_offset(row, gi * 8);                                     // K = f
@@ -631,8 +649,10 @@ __device__ __forceinline__ void level_rs_next_head(float (&acc0)[64], float (&ac
 
 // Trunk layer / bottleneck l (1..8) from x_in into x_out: the rest of N-half 0 into acc0, N-half 1 into acc1 with
 // acc0's epilogue in chunks under it (epi_slab_acc0), then level_rs_next_head.  kSkip: l may be 5, whose K-slabs 4
-// (SW128) and 5 (SW64 tail) read the feature tile.
-template <int kFmt, bool kSkip>
+// (SW128) and 5 (SW64 tail) read the feature tile.  kLast (density-only mode, l = 7): no next layer; the wgmmas retire
+// and acc1's epilogue chunks follow in the order level_rs_next_head runs them, so the density head sums the same terms
+// in the same order.
+template <int kFmt, bool kSkip, bool kLast = false>
 __device__ __forceinline__ void level_rs_layer(float (&acc0)[64], float (&acc1)[64], const uint32_t (&x_in)[64],
                                                uint32_t (&x_out)[64], int l, const LevelRsCtx& k, RingPos& rp,
                                                PhaseClock& clk, float& d0, float& d1) {
@@ -668,7 +688,22 @@ __device__ __forceinline__ void level_rs_layer(float (&acc0)[64], float (&acc1)[
     for (int s = kWidth / 64; s < num_slabs(true, 5); ++s)
       level_mma_slab<kFmt, false>(acc1, 5, s, 0u, f_u, ft_u, k.w_u, k.w_full, k.w_empty, rp, k.leader, clk);
   }
-  level_rs_next_head<kFmt>(acc0, acc1, x_out, l, skip, k, rp, clk, d0, d1);
+  if constexpr (kLast) {
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc1);
+    if (k.leader) mbar_arrive(&k.w_empty[rp.prev]);
+    rp.prev = -1;
+    clk.mark(kPhMma);
+#pragma unroll
+    for (int c = 0; c < kEpiChunks; ++c) {
+      EpiConsts e;
+      level_epilogue_consts(e, l, 128, c, k.cq, k.gsp);
+      level_epilogue_chunk_rs<kFmt>(acc1, e, l, 128, c, x_out, k, d0, d1);
+    }
+    clk.mark(kPhEpilogue);
+  } else {
+    level_rs_next_head<kFmt>(acc0, acc1, x_out, l, skip, k, rp, clk, d0, d1);
+  }
 }
 
 __device__ __forceinline__ float quad_sum(float v) {
@@ -679,12 +714,13 @@ __device__ __forceinline__ float quad_sum(float v) {
 // ---- the helper warps' work (ht = helper thread 0..95, hw = helper warp 0..2) ----
 // Tile tt of `ray` into the feature buffer fbuf: first (tt == 0) the ray prologue, once per ray, then the tile's
 // features.  The prologue's global stores (fenceposts, view bias) are read back by this CTA only, through L2 (ld.cg):
-// by the helpers after the helper barrier, by the consumers after feat_full.
-template <int kFmt, bool kX3, int kT>
+// by the helpers after the helper barrier, by the consumers after feat_full.  Density-only mode: the tile's query
+// points' features only.
+template <int kFmt, bool kX3, int kT, bool kDensity = false>
 __device__ __forceinline__ void level_prepare_tile(const LevelParams& p, int64_t ray, int tt, uint8_t* fbuf,
                                                    float* rs_scratch, int ht, int hw, int lane, PhaseClock& clk) {
   constexpr int kNs = kT * kN;  // samples per ray
-  if ((kT == 1 || tt == 0) && (p.t_mode != 0 || p.vb_mode != 0)) {
+  if (!kDensity && (kT == 1 || tt == 0) && (p.t_mode != 0 || p.vb_mode != 0)) {
     if (hw == 0) {
       float* t_ray = p.t + ray * (kNs + 1);
       if (p.t_mode == 1) {  // coarse fenceposts (bit-identical to coarse_t_kernel)
@@ -732,14 +768,15 @@ __device__ __forceinline__ void level_prepare_tile(const LevelParams& p, int64_t
   // Gaussians + IPE features: 128 rows x 3 parts of two 8-feature groups = 384 units, four per helper thread; a warp's
   // 32 units share their part
   RayGeom g{};
-  if (!p.feat_in) g = load_ray_geom(p.origins, p.directions, p.radii, ray);
+  if (!kDensity && !p.feat_in) g = load_ray_geom(p.origins, p.directions, p.radii, ray);
   const int row0 = kT == 1 ? 0 : tt * kN;  // the tile's first row of the ray
 #pragma unroll 1
   for (int u = ht; u < 3 * kN; u += kHelperThreads) {
     const int row = u & (kN - 1), part = u / kN;
     float t0 = 0.f, t1 = 0.f;
-    if (!p.feat_in) t0 = __ldcg(p.t + ray * (kNs + 1) + row0 + row), t1 = __ldcg(p.t + ray * (kNs + 1) + row0 + row + 1);
-    ipe_row_group<kFmt, kX3, kT>(p, g, ray, row, t0, t1, fbuf, 2 * part, 2 * part + 2);
+    if (!kDensity && !p.feat_in)
+      t0 = __ldcg(p.t + ray * (kNs + 1) + row0 + row), t1 = __ldcg(p.t + ray * (kNs + 1) + row0 + row + 1);
+    ipe_row_group<kFmt, kX3, kT, kDensity>(p, g, ray, row, t0, t1, fbuf, 2 * part, 2 * part + 2);
   }
   fence_proxy_async_smem();  // the features are read by wgmma (async proxy)
   clk.mark(kPhIpe);
@@ -852,8 +889,27 @@ __device__ __forceinline__ void level_composite_ray(const LevelParams& p, int64_
   clk.mark(kPhBarrier);
 }
 
-template <int kFmt, bool kX3, int kT>
+// Density-only mode: the raw density of tile `tile`'s query points from its raw heads hd[128][4] (the sum MLP-only mode
+// hands back, models/mip_nerf.py:98) and its activation (models/mip_nerf.py:237); rows past the last point are masked.
+__device__ __forceinline__ void level_density_out(const LevelParams& p, int64_t tile, const float* hd,
+                                                  uint64_t* heads_empty, int ht, PhaseClock& clk) {
+  for (int row = ht; row < kN; row += kHelperThreads) {
+    const int64_t pt = tile * kN + row;
+    if (pt >= p.num_points) break;
+    const float raw = hd[row * 4] + c_small.b_density;
+    if (p.raw_density_out) p.raw_density_out[pt] = raw;
+    if (p.density_out) p.density_out[pt] = density_activation(raw, p.density_bias);
+  }
+  mbar_arrive(heads_empty);
+  clk.mark(kPhComposite);
+}
+
+// kDensity (kT = 1): density-only mode.  The producer streams the stages of layers 0-7 only (a prefix of the image),
+// the consumers run layers 0-7 and finish the density head in layer 7's epilogue, and the helpers encode the query
+// points and write the densities; everything else is the forward's schedule.
+template <int kFmt, bool kX3, int kT, bool kDensity = false>
 __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParams p) {
+  static_assert(!kDensity || kT == 1, "density-only mode takes one 128-point tile at a time");
   using Lay = LevelLayout<kX3, kT>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -911,7 +967,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             const int fb = (int)(j % Lay::kFeatBufs);
             mbar_wait(&feat_empty[fb], ((uint32_t)(j / Lay::kFeatBufs) & 1u) ^ 1u);
             clk.mark(kPhFeatEmpty);
-            level_prepare_tile<kFmt, kX3, kT>(p, ray, tt, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane, clk);
+            level_prepare_tile<kFmt, kX3, kT, kDensity>(p, ray, tt, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane,
+                                                        clk);
             mbar_arrive(&feat_full[fb]);
           }
           if (tt == 0 && i > 0) {  // ray - gridDim.x, the (i - 1)-th ray of the CTA: tiles (i - 1) kT ..
@@ -920,8 +977,11 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             for (int u = 0; u < kT; ++u)
               mbar_wait(&heads_full[par + u], (uint32_t)(((i - 1) * kT + u) >> 1) & 1u);
             clk.mark(kPhHeadsFull);
-            level_composite_ray<kT>(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], cs, ps, ht, hw, lane,
-                                    clk);
+            if constexpr (kDensity)
+              level_density_out(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], ht, clk);
+            else
+              level_composite_ray<kT>(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], cs, ps, ht, hw, lane,
+                                      clk);
           }
         }
         if (!more) break;
@@ -937,7 +997,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       const uint64_t pol = l2_policy_evict_last();  // the image is re-read by every CTA for every ray
       for (int64_t tile = 0, ray = blockIdx.x; ray < p.num_rays; ray += ++tile % kT == 0 ? gridDim.x : 0) {
         const uint8_t* src = p.wimage;  // the stages are contiguous in issue order (w_stages_contiguous)
-        for (int l = 0; l < kNumLayers; ++l)
+        for (int l = 0; l < (kDensity ? 8 : kNumLayers); ++l)
           for (int h = 0; h < num_halves(l); ++h)  // N-half major, then K-slab
             for (int s = 0; s < num_slabs(!kX3, l); ++s) {
               const uint32_t bytes = w_stage(!kX3, l, s).bytes;
@@ -1018,7 +1078,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       // feature tile; layer 0 has two K-slabs (64 wide + the 32-wide tail), and two of its acc0 chunks follow each.  The
       // training forward's activation tiles go out from the epilogue's registers.
       const LevelRsCtx k{f_u, ft_u, w_u, w_full, w_empty, &feat_empty[fb], gsp,
-                         kT == 1 && p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
+                         !kDensity && kT == 1 && p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
                          (size_t)p.dump_tiles * kABytes, dump_policy, r0, cq, leader};
       uint32_t xa[64], xb[64];
       static_assert(2 * num_slabs(true, 0) == kEpiChunks, "layer 0: two acc0 chunks after each of its K-slabs");
@@ -1036,14 +1096,18 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       }
       level_rs_next_head<kFmt>(acc0, acc1, xb, 0, false, k, rp, clk, d0, d1);
 #pragma unroll 1
-      for (int l = 1; l < 9; l += 2) {
+      for (int l = 1; l < (kDensity ? 7 : 9); l += 2) {
         level_rs_layer<kFmt, true>(acc0, acc1, xb, xa, l, k, rp, clk, d0, d1);
         level_rs_layer<kFmt, false>(acc0, acc1, xa, xb, l + 1, k, rp, clk, d0, d1);
       }
-      // the rest of the view layer's one N-half, from the bottleneck in xb
+      if constexpr (kDensity) {
+        level_rs_layer<kFmt, false, true>(acc0, acc1, xb, xa, 7, k, rp, clk, d0, d1);
+      } else {
+        // the rest of the view layer's one N-half, from the bottleneck in xb
 #pragma unroll
-      for (int s = 2; s < num_slabs(true, 9); ++s)
-        level_mma_slab_rs<kFmt>(acc0, xb, s, w_u, w_full, w_empty, rp, leader, clk);
+        for (int s = 2; s < num_slabs(true, 9); ++s)
+          level_mma_slab_rs<kFmt>(acc0, xb, s, w_u, w_full, w_empty, rp, leader, clk);
+      }
     } else {
       for (int l = 0; l < 9; ++l) {
         // 1. the rest of N-half 0
@@ -1076,6 +1140,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
         }
         for (int s = first + kEpiChunks; s < num_slabs(false, l); ++s)
           level_mma_slab<kFmt, kX3>(acc1, l, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+        if (kDensity && l == 7) break;  // density-only mode: layer 7 has no next layer (acc1's epilogue below)
         // 3.
         fence_proxy_async_smem();
         clk.mark(kPhEpilogue);
@@ -1114,17 +1179,32 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
           clk.mark(kPhEpilogue);
         }
       }
-      // the rest of the view layer's one N-half
-      for (int s = kEpiChunks; s < num_slabs(false, 9); ++s)
-        level_mma_slab<kFmt, kX3>(acc0, 9, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+      if constexpr (kDensity) {  // layer 7's acc1 epilogue, as step 4 runs it
+        wgmma_wait<0>();
+        wgmma_fence_acc(acc1);
+        if (leader) mbar_arrive(&w_empty[rp.prev]);
+        rp.prev = -1;
+        clk.mark(kPhMma);
+#pragma unroll
+        for (int c = 0; c < kEpiChunks; ++c) {
+          EpiConsts e;
+          level_epilogue_consts(e, 7, 128, c, cq, gsp);
+          level_epilogue_chunk<kFmt, kX3>(acc1, e, 7, 128, c, r0, cq, sA, gsp, d0, d1);
+        }
+        clk.mark(kPhEpilogue);
+      } else {
+        // the rest of the view layer's one N-half
+        for (int s = kEpiChunks; s < num_slabs(false, 9); ++s)
+          level_mma_slab<kFmt, kX3>(acc0, 9, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
+      }
     }
-    // the view layer's epilogue from the registers
-    wgmma_wait<0>();
-    wgmma_fence_acc(acc0);
-    if (leader) mbar_arrive(&w_empty[rp.prev]);
-    rp.prev = -1;
-    clk.mark(kPhMma);
-    {
+    if constexpr (!kDensity) {
+      // the view layer's epilogue from the registers
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc0);
+      if (leader) mbar_arrive(&w_empty[rp.prev]);
+      rp.prev = -1;
+      clk.mark(kPhMma);
       // view layer + colour head (models/mip_nerf.py:106-110); view_bias = the per-ray view-direction term
       const float* vb = p.view_bias + ray * kCond;
       uint8_t* vd = kT == 1 && p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
@@ -1356,9 +1436,9 @@ int g_num_sms = 0;
 inline int fmt_of(int precision) { return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_BF16X3) ? 1 : 0; }
 inline bool is_x3(int precision) { return precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3; }
 
-template <int kFmt, bool kX3, int kT>
+template <int kFmt, bool kX3, int kT, bool kDensity = false>
 cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
-  auto kern = mlp_level_kernel<kFmt, kX3, kT>;
+  auto kern = mlp_level_kernel<kFmt, kX3, kT, kDensity>;
   constexpr uint32_t smem = LevelLayout<kX3, kT>::kTotal;
   static bool attr_set = false;  // one flag per instantiation
   if (!attr_set) {
@@ -1371,7 +1451,7 @@ cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
   }
-  LaunchScope scope(p.feat_in ? kKernMlpTc : kKernMlpLevelTc, st);
+  LaunchScope scope(kDensity ? kKernDensityTc : (p.feat_in ? kKernMlpTc : kKernMlpLevelTc), st);
   const int grid = (int)(p.num_rays < g_num_sms ? p.num_rays : g_num_sms);
   kern<<<grid, kThreads, smem, st>>>(p);
   return cudaGetLastError();
@@ -1387,6 +1467,12 @@ cudaError_t launch_level_tiles(const LevelParams& p, int precision, cudaStream_t
 cudaError_t launch_level(const LevelParams& p, int precision, int n, cudaStream_t st) {
   if (p.num_rays <= 0) return cudaSuccess;
   return n == 2 * kN ? launch_level_tiles<2>(p, precision, st) : launch_level_tiles<1>(p, precision, st);
+}
+cudaError_t launch_density(const LevelParams& p, int precision, cudaStream_t st) {
+  if (p.num_rays <= 0) return cudaSuccess;
+  if (is_x3(precision))
+    return fmt_of(precision) ? launch_level_t<1, true, 1, true>(p, st) : launch_level_t<0, true, 1, true>(p, st);
+  return fmt_of(precision) ? launch_level_t<1, false, 1, true>(p, st) : launch_level_t<0, false, 1, true>(p, st);
 }
 
 }  // namespace
@@ -1601,6 +1687,30 @@ cudaError_t tc_mlp_forward(const mipnerf_b200_config* c, const mipnerf_b200_weig
   p.raw_density_out = raw_density;
   p.num_rays = num_rays;
   return launch_level(p, precision, kN, st);
+}
+
+cudaError_t tc_query_density(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, const float* means,
+                             const float* covs, int64_t num_points, int precision, float* raw_density, float* density,
+                             cudaStream_t st) {
+  const uint8_t* img = static_cast<const uint8_t*>(w->packed);
+  SmallUpload small(img, st);
+  cudaError_t e = small.error();
+  if (e != cudaSuccess) return e;
+  for (int64_t off = 0; off < num_points; off += kDensityChunkPoints) {
+    const int64_t cnt = (num_points - off) < kDensityChunkPoints ? (num_points - off) : kDensityChunkPoints;
+    LevelParams p{};
+    p.wimage = img;
+    p.q_means = means + off * 3;
+    p.q_covs = covs ? covs + off * 3 : nullptr;
+    p.num_points = cnt;
+    p.num_rays = (cnt + kN - 1) / kN;
+    p.raw_density_out = raw_density ? raw_density + off : nullptr;
+    p.density_out = density ? density + off : nullptr;
+    p.disable_integration = c->disable_integration;
+    p.density_bias = c->density_bias;
+    if ((e = launch_density(p, precision, st)) != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 cudaError_t launch_view_bias_from_enc(const float* venc, const float* w, const float* b, float* out,

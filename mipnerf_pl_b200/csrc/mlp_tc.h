@@ -42,5 +42,11 @@ cudaError_t tc_mlp_forward(const mipnerf_b200_config* cfg, const mipnerf_b200_we
                            const float* view_enc, int64_t num_rays, int precision, float* raw_rgb,
                            float* raw_density, void* workspace, cudaStream_t st);
 size_t tc_mlp_workspace_bytes(int64_t num_rays);
+// Density-only mode of the level kernels (mipnerf_b200_query_density), kDensityChunkPoints points per launch; needs
+// tc_supported(cfg, precision) and w->packed for that precision.
+constexpr int64_t kDensityChunkPoints = 4096 * 128;
+cudaError_t tc_query_density(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                             const float* covs, int64_t num_points, int precision, float* raw_density, float* density,
+                             cudaStream_t st);
 
 }  // namespace mipnerf

@@ -28,6 +28,8 @@ enum KernelId : int {
   kKernLinearTc,     // stand-alone wgmma linear layer (training forward / dgrad)
   kKernWgradTc,      // wgmma wgrad partials
   kKernImageMetrics, // PSNR + SSIM of a rendered frame
+  kKernDensityTc,    // density-only mode of the wgmma level kernel (IPE + trunk + density head)
+  kKernIsosurface,   // marching-tetrahedra isosurface extraction (count / scan / emit)
   kKernCount
 };
 

@@ -587,4 +587,17 @@ cudaError_t launch_resample(const float* bins, const float* weights, const Draws
   return cudaGetLastError();
 }
 
+__global__ void density_activation_kernel(const float* __restrict__ raw, float* __restrict__ density, int64_t n,
+                                          float density_bias) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) density[i] = density_activation(raw[i], density_bias);
+}
+
+cudaError_t launch_density_activation(const float* raw, float* density, int64_t n, float density_bias, cudaStream_t st) {
+  if (n == 0) return cudaSuccess;
+  LaunchScope scope(kKernComposite, st);
+  density_activation_kernel<<<blocks_for(n, 256), 256, 0, st>>>(raw, density, n, density_bias);
+  return cudaGetLastError();
+}
+
 }  // namespace mipnerf

@@ -1,0 +1,119 @@
+"""Looking at the geometry of a trained field: density on a 3D lattice and its isosurface as a mesh.
+
+* `MipNerf.query_density` evaluates the density at Gaussians (means, diagonal covariances); on the tensor cores it is
+  the density-only mode of the level kernel (IPE -> trunk -> density head, nothing else).
+* `density_grid` queries a lattice in z-slabs.  By default each lattice point is the Gaussian of its voxel (variance
+  step**2 / 12 per axis, a uniform voxel's), so the IPE integrates the field over the voxel's footprint and the grid is
+  anti-aliased at its own scale.
+* `isosurface` extracts the `grid > iso` surface with the library's marching-tetrahedra kernels; `extract_mesh` is both.
+* `write_ply` writes a binary PLY with no dependency.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Optional, Sequence, Tuple, Union
+
+import numpy as np
+import torch
+
+from . import _cabi
+from .ops import _dev, _f32, _stream
+
+DEFAULT_BOUNDS = ((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5))
+Resolution = Union[int, Sequence[int]]
+
+
+def _resolution(resolution: Resolution) -> Tuple[int, int, int]:
+    """(nx, ny, nz)."""
+    res = (int(resolution),) * 3 if isinstance(resolution, (int, np.integer)) else tuple(int(r) for r in resolution)
+    if len(res) != 3 or min(res) < 2:
+        raise ValueError(f"resolution {resolution!r}: need an int or (nx, ny, nz), each >= 2")
+    return res
+
+
+def lattice_axes(resolution: Resolution, bounds=DEFAULT_BOUNDS, device="cuda"):
+    """The lattice coordinates per axis, fp32: lo[a] + idx * step[a] with step[a] = (hi[a] - lo[a]) / (n[a] - 1), each
+    operation rounded to fp32 (the positions the isosurface kernels give the lattice points)."""
+    n = _resolution(resolution)
+    lo = np.asarray(bounds[0], dtype=np.float32)
+    hi = np.asarray(bounds[1], dtype=np.float32)
+    step = (hi - lo) / (np.asarray(n, dtype=np.float32) - np.float32(1))
+    axes = [torch.arange(n[a], dtype=torch.float32, device=device) * float(step[a]) + float(lo[a]) for a in range(3)]
+    return axes, step
+
+
+def density_grid(model, resolution: Resolution, bounds=DEFAULT_BOUNDS, variance=None,
+                 slab_points: int = 1 << 22) -> torch.Tensor:
+    """Density (softplus(raw + density_bias)) of `model` on a lattice -> [nz, ny, nx] on the model's device.  Point
+    (i, j, k) sits at lo + (i, j, k) * step; `variance` (a float or one per axis) is the diagonal covariance of every
+    query, by default step**2 / 12 per axis; 0 gives a point-sampled grid.  Queried in z-slabs of at most
+    `slab_points` points, so that the memory beyond the grid stays bounded."""
+    dev = next(model.parameters()).device
+    nx, ny, nz = _resolution(resolution)
+    (xs, ys, zs), step = lattice_axes((nx, ny, nz), bounds, dev)
+    var = step.astype(np.float32) ** 2 / np.float32(12) if variance is None else np.broadcast_to(
+        np.asarray(variance, dtype=np.float32), (3,))
+    covs_row = torch.tensor(np.asarray(var, dtype=np.float32), device=dev)
+    out = torch.empty(nz, ny, nx, device=dev)
+    slab = max(1, slab_points // (nx * ny))
+    yy, xx = torch.meshgrid(ys, xs, indexing="ij")
+    for z0 in range(0, nz, slab):
+        z = zs[z0:z0 + slab]
+        means = torch.stack([xx.expand(len(z), ny, nx), yy.expand(len(z), ny, nx),
+                             z[:, None, None].expand(len(z), ny, nx)], dim=-1)
+        covs = covs_row.expand(len(z), ny, nx, 3)
+        out[z0:z0 + len(z)] = model.query_density(means, covs)
+    return out
+
+
+def isosurface(grid: torch.Tensor, iso: float, bounds=DEFAULT_BOUNDS) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The surface `grid > iso` of a [nz, ny, nx] grid whose lattice spans `bounds` -> (verts [V,3] fp32, faces [F,3]
+    int32) on the grid's device.  Marching tetrahedra (6 per cell): a watertight, consistently oriented mesh whose
+    normals point from inside (> iso) to outside; NaN counts as outside.  Bit-reproducible."""
+    dev = _dev(grid)
+    if grid.dim() != 3:
+        raise ValueError(f"grid must be [nz, ny, nx], got {tuple(grid.shape)}")
+    g = _f32(grid)
+    nz, ny, nx = g.shape
+    lib = _cabi.lib()
+    nbytes = lib.mipnerf_b200_isosurface_scratch_bytes(nx, ny, nz)
+    if nbytes == 0:
+        raise ValueError(f"grid {tuple(grid.shape)}: need at least 2 points per axis")
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    counts = torch.empty(2, dtype=torch.int64, device=dev)
+    lo = (C.c_float * 3)(*[float(v) for v in bounds[0]])
+    hi = (C.c_float * 3)(*[float(v) for v in bounds[1]])
+    with torch.cuda.device(dev):
+        st = _stream(dev)
+        _cabi.check(lib.mipnerf_b200_isosurface_count(g.data_ptr(), nx, ny, nz, float(iso), scratch.data_ptr(), nbytes,
+                                                      counts.data_ptr(), st), "isosurface")
+        nv, nf = (int(v) for v in counts.tolist())
+        verts = torch.empty(nv, 3, device=dev)
+        faces = torch.empty(nf, 3, dtype=torch.int32, device=dev)
+        _cabi.check(lib.mipnerf_b200_isosurface_emit(g.data_ptr(), nx, ny, nz, lo, hi, float(iso), scratch.data_ptr(),
+                                                     verts.data_ptr() if nv else None,
+                                                     faces.data_ptr() if nf else None, st), "isosurface")
+    return verts, faces
+
+
+def extract_mesh(model, threshold: float, resolution: Resolution = 256, bounds=DEFAULT_BOUNDS,
+                 variance=None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The surface density > threshold of `model` inside `bounds` -> (verts, faces) on the model's device."""
+    grid = density_grid(model, resolution, bounds, variance)
+    return isosurface(grid, threshold, bounds)
+
+
+def write_ply(path: str, verts, faces) -> None:
+    """Binary little-endian PLY: float x, y, z per vertex; uchar-counted int vertex_indices per face."""
+    v = np.ascontiguousarray(torch.as_tensor(verts).detach().cpu().numpy(), dtype="<f4").reshape(-1, 3)
+    f = np.ascontiguousarray(torch.as_tensor(faces).detach().cpu().numpy(), dtype="<i4").reshape(-1, 3)
+    rec = np.empty(len(f), dtype=[("n", "u1"), ("idx", "<i4", (3,))])
+    rec["n"] = 3
+    rec["idx"] = f
+    header = ("ply\nformat binary_little_endian 1.0\n"
+              f"element vertex {len(v)}\nproperty float x\nproperty float y\nproperty float z\n"
+              f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(v.tobytes())
+        fh.write(rec.tobytes())

@@ -279,6 +279,36 @@ class MipNerf(torch.nn.Module):
             return _forward_with_grad(self, rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds)
         return self._forward(rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds)[0]
 
+    @torch.no_grad()
+    def query_density(self, means: torch.Tensor, covs: Optional[torch.Tensor] = None, *, raw: bool = False):
+        """Density of the field at Gaussians: means / diagonal covs [..., 3] (covs None: zero covariance) -> [...] on
+        `self.precision`: the IPE (models/mip.py:322-350), trunk and density_layer of MLP.forward
+        (models/mip_nerf.py:93-98), then softplus(raw + density_bias) unless `raw` (no density noise).  The result has
+        no grad_fn.  The tensor-core precisions take the configs `forward` takes on the tensor cores; fp32 any."""
+        dev = _dev(means)
+        if means.shape[-1] != 3 or (covs is not None and covs.shape != means.shape):
+            raise ValueError(f"means {tuple(means.shape)} / covs {None if covs is None else tuple(covs.shape)}: "
+                             "need [..., 3] of the same shape")
+        shape = means.shape[:-1]
+        m = _f32(means).reshape(-1, 3)
+        c = _f32(covs).reshape(-1, 3) if covs is not None else None
+        p = m.shape[0]
+        prec = _cabi.PRECISIONS[self.precision]
+        cfg = self._config()
+        ws, keep = self.mlp._weights_struct(cfg, prec, dev)
+        out = torch.empty(p, device=dev)
+        if p == 0:
+            return out.reshape(shape)
+        lib = _cabi.lib()
+        nbytes = lib.mipnerf_b200_density_workspace_bytes(C.byref(cfg), p, prec)
+        scratch = _Workspace.get(dev, nbytes)
+        with torch.cuda.device(dev):
+            _cabi.check(lib.mipnerf_b200_query_density(
+                C.byref(cfg), C.byref(ws), m.data_ptr(), _ptr(c), p, prec,
+                out.data_ptr() if raw else None, None if raw else out.data_ptr(), scratch.data_ptr(), scratch.numel(),
+                _stream(dev)), "MipNerf.query_density")
+        return out.reshape(shape)
+
     def _forward(self, rays: Rays, randomized: bool, white_bkgd: bool, t_rand, u_jitter, density_normal,
                  return_inds: bool):
         """The launches of `forward` -> (LevelOutputs, config, rng or None, per-level density normals or None,
