@@ -352,6 +352,21 @@ int mipnerf_b200_query_density(const mipnerf_b200_config* cfg, const mipnerf_b20
                                const float* covs, int64_t num_points, int precision, float* raw_density,
                                float* density, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Radiance of the field at Gaussians, each seen from its own direction: means / covs as for the density query,
+ * viewdirs [P,3] (encoded as given; the reference encodes unit directions) -> MLP.forward(x [P,1,xyz_dim],
+ * pos_enc(viewdirs) [P,view_dim]) (models/mip_nerf.py:75-111).  raw_rgb [P,3] / raw_density [P] are its raw heads (no
+ * noise); rgb [P,3] = sigmoid(raw) * (1 + 2 rgb_padding) - rgb_padding and density [P] = softplus(raw +
+ * cfg->density_bias).  Any output may be NULL, not all.  viewdirs may be NULL only when !cfg->use_viewdirs (FP32 only:
+ * the colour head then reads the trunk output, as the reference's).  Refusals and precisions as for the density query.
+ * The tensor-core precisions run the radiance mode of the level kernel; their workspace is two [128][128] fp32 slots
+ * of view-direction terms per CTA of a launch, min(ceil(P / 128), 4096, SMs) CTAs, so it is sized by the device the
+ * call runs on.  Results do not depend on how a query is split. */
+size_t mipnerf_b200_radiance_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points, int precision);
+int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                                const float* covs, const float* viewdirs, int64_t num_points, int precision,
+                                float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
+                                size_t workspace_bytes, void* stream);
+
 /* Isosurface of a scalar grid [nz, ny, nx] fp32 (x fastest, every dimension >= 2) by marching tetrahedra (6 Kuhn
  * tetrahedra per cell): a watertight indexed mesh whose normals point from inside (value > iso; NaN is outside) to
  * outside.  Pass 1 writes counts[2] (device int64: vertices, faces); pass 2, with the same scratch, writes verts [V,3]
@@ -365,6 +380,13 @@ int mipnerf_b200_isosurface_count(const float* grid, int nx, int ny, int nz, flo
 int mipnerf_b200_isosurface_emit(const float* grid, int nx, int ny, int nz, const float* lo_host,
                                  const float* hi_host, float iso, const void* scratch, float* verts,
                                  int32_t* faces, void* stream);
+/* Vertex normals of the mesh _emit wrote, from the same grid, bounds, iso and scratch (after _emit): normals [V,3] fp32,
+ * vertex v's at row v.  The grid gradient at both ends of the vertex's lattice edge (central differences over 2 step
+ * per axis, one-sided over step at the box faces), interpolated with the vertex's t, negated and normalised: the unit
+ * direction from inside to outside, the faces' orientation.  (0, 0, 0) where that gradient is zero or not finite (a NaN
+ * neighbour).  Every operation is explicitly rounded: the normals are bit-reproducible. */
+int mipnerf_b200_isosurface_normals(const float* grid, int nx, int ny, int nz, const float* lo_host,
+                                    const float* hi_host, float iso, const void* scratch, float* normals, void* stream);
 
 /* Hardware self-test of the wgmma building blocks (descriptor / swizzle / accumulator-fragment conventions):
  * d[128,n] = a[128,k] . b[n,k]^T, 16-bit operands (precision BF16|FP16), fp32 accumulate; n in {128, 256}.

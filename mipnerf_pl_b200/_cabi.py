@@ -128,6 +128,11 @@ _SIGNATURES = {
     "mipnerf_b200_density_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int]),
     "mipnerf_b200_query_density": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), _V, _V, C.c_int64, C.c_int, _V, _V,
                                              _V, C.c_size_t, _V]),
+    "mipnerf_b200_radiance_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int]),
+    "mipnerf_b200_query_radiance": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), _V, _V, _V, C.c_int64, C.c_int,
+                                              _V, _V, _V, _V, _V, C.c_size_t, _V]),
+    "mipnerf_b200_isosurface_normals": (C.c_int, [_V, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.c_float, _V, _V,
+                                                  _V]),
     "mipnerf_b200_isosurface_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "mipnerf_b200_isosurface_count": (C.c_int, [_V, C.c_int, C.c_int, C.c_int, C.c_float, _V, C.c_size_t, _V, _V]),
     "mipnerf_b200_isosurface_emit": (C.c_int, [_V, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.c_float, _V, _V, _V,

@@ -1341,6 +1341,100 @@ int mipnerf_b200_query_density(const mipnerf_b200_config* cfg, const mipnerf_b20
   return MIPNERF_B200_OK;
 }
 
+namespace {
+struct RadianceScratch {
+  float *zero_covs, *enc, *venc, *raw_rgb, *raw_density;
+  Fp32Scratch mlp;  // h0, h1, c0, c1 of mlp_forward_fp32
+  size_t bytes;
+};
+RadianceScratch carve_radiance(const mipnerf_b200_config* c, const Dims& d, int64_t m, void* base) {
+  RadianceScratch s{};
+  size_t off = 0;
+  auto take = [&](size_t elems) {
+    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
+    off += align_up(elems * sizeof(float));
+    return p;
+  };
+  s.zero_covs = take((size_t)m * 3);
+  s.enc = take((size_t)m * d.xyz_dim);
+  s.venc = take((size_t)m * d.view_dim);
+  s.raw_rgb = take((size_t)m * 3);
+  s.raw_density = take((size_t)m);
+  s.mlp.h0 = take((size_t)m * c->net_width);
+  s.mlp.h1 = take((size_t)m * c->net_width);
+  s.mlp.c0 = take((size_t)m * c->net_width_condition);
+  s.mlp.c1 = take((size_t)m * c->net_width_condition);
+  s.bytes = off;
+  return s;
+}
+}  // namespace
+
+size_t mipnerf_b200_radiance_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points, int precision) {
+  Dims d;
+  if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0) return 0;
+  if (precision != MIPNERF_B200_FP32)
+    return mipnerf::tc_supported(cfg, precision) ? mipnerf::tc_radiance_workspace_bytes(num_points) : 0;
+  const int64_t m = num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32;
+  return carve_radiance(cfg, d, m > 0 ? m : 1, nullptr).bytes;
+}
+
+int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                                const float* covs, const float* viewdirs, int64_t num_points, int precision,
+                                float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
+                                size_t workspace_bytes, void* stream) {
+  Dims d;
+  int rc;
+  if ((rc = check_config(cfg, &d))) return rc;
+  if ((rc = check_weights(cfg, d, w))) return rc;
+  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if (!raw_rgb && !raw_density && !rgb && !density) return fail(MIPNERF_B200_EINVAL, "every output is NULL");
+  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
+  if (num_points > 0 && cfg->use_viewdirs && !viewdirs)
+    return fail(MIPNERF_B200_EINVAL, "viewdirs is NULL with use_viewdirs");
+  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
+    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
+  if (precision != MIPNERF_B200_FP32) {
+    if (!mipnerf::tc_supported(cfg, precision))
+      return fail(MIPNERF_B200_EUNSUPPORTED,
+                  "tensor-core radiance query: the forward's tensor-core shapes only (8x256 / 1x128 model, "
+                  "num_samples 128 or 256, min_deg_point 0, max_deg_point 1..16, deg_view 1..4); use MIPNERF_B200_FP32");
+    if (!w->packed || w->packed_precision != precision || w->packed_bytes < mipnerf::tc_packed_bytes(cfg, precision))
+      return fail(MIPNERF_B200_EINVAL, "weights->packed missing or packed for another precision");
+  }
+  const size_t need = mipnerf_b200_radiance_workspace_bytes(cfg, num_points, precision);
+  if (num_points > 0 && (need == 0 || !workspace || workspace_bytes < need))
+    return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
+  if (num_points == 0) return MIPNERF_B200_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (precision != MIPNERF_B200_FP32) {
+    cudaError_t e = mipnerf::tc_query_radiance(cfg, w, means, covs, viewdirs, num_points, precision, raw_rgb,
+                                               raw_density, rgb, density, workspace, workspace_bytes, st);
+    if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "tc_query_radiance: %s", cudaGetErrorString(e));
+    return MIPNERF_B200_OK;
+  }
+  // fp32: the IPE stage kernel, the view-direction encoding and the fp32 MLP with one sample per "ray" (each point its
+  // own view encoding), then the activations (models/mip.py:322-363, models/mip_nerf.py:75-111, 236-237)
+  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
+    const int64_t m = (num_points - off) < kChunkPointsFp32 ? (num_points - off) : kChunkPointsFp32;
+    const RadianceScratch s = carve_radiance(cfg, d, m, workspace);
+    const float* cv = covs ? covs + off * 3 : nullptr;
+    if (!cv || cfg->disable_integration) {
+      CUDA_TRY(cudaMemsetAsync(s.zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
+      cv = s.zero_covs;
+    }
+    CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, s.enc, m, cfg->min_deg_point, cfg->max_deg_point, st));
+    if (cfg->use_viewdirs) CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, s.venc, m, 0, cfg->deg_view, 1, st));
+    float* rr = raw_rgb ? raw_rgb + off * 3 : s.raw_rgb;
+    float* rd = raw_density ? raw_density + off : s.raw_density;
+    if ((rc = mlp_forward_fp32(cfg, d, w, s.enc, cfg->use_viewdirs ? s.venc : nullptr, m, 1, s.mlp, rr, rd, st)))
+      return rc;
+    CUDA_TRY(mipnerf::launch_radiance_activation(rr, rd, rgb ? rgb + off * 3 : nullptr, density ? density + off : nullptr,
+                                                 m, cfg->density_bias, rgb_scale, cfg->rgb_padding, st));
+  }
+  return MIPNERF_B200_OK;
+}
+
 size_t mipnerf_b200_isosurface_scratch_bytes(int nx, int ny, int nz) {
   if (nx < 2 || ny < 2 || nz < 2) return 0;
   return mipnerf::isosurface_scratch_bytes(nx, ny, nz);
@@ -1373,6 +1467,23 @@ int mipnerf_b200_isosurface_emit(const float* grid, int nx, int ny, int nz, cons
   float step[3];
   for (int a = 0; a < 3; ++a) step[a] = (hi_host[a] - lo_host[a]) / (float)(n[a] - 1);
   CUDA_TRY(mipnerf::launch_isosurface_emit(grid, nx, ny, nz, lo_host, step, iso, scratch, verts, faces, st));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_isosurface_normals(const float* grid, int nx, int ny, int nz, const float* lo_host,
+                                    const float* hi_host, float iso, const void* scratch, float* normals, void* stream) {
+  if (nx < 2 || ny < 2 || nz < 2) return fail(MIPNERF_B200_EINVAL, "grid %d x %d x %d: need >= 2 per axis", nx, ny, nz);
+  if (!grid || !lo_host || !hi_host || !scratch) return fail(MIPNERF_B200_EINVAL, "grid / bounds / scratch is NULL");
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t totals[2];
+  CUDA_TRY(cudaMemcpyAsync(totals, mipnerf::isosurface_totals(scratch), sizeof(totals), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (totals[0] > 0 && !normals) return fail(MIPNERF_B200_EINVAL, "normals is NULL");
+  if (totals[0] == 0) return MIPNERF_B200_OK;
+  const int n[3] = {nx, ny, nz};
+  float step[3];
+  for (int a = 0; a < 3; ++a) step[a] = (hi_host[a] - lo_host[a]) / (float)(n[a] - 1);
+  CUDA_TRY(mipnerf::launch_isosurface_normals(grid, nx, ny, nz, step, iso, scratch, normals, st));
   return MIPNERF_B200_OK;
 }
 

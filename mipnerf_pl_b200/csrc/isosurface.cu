@@ -1,4 +1,5 @@
-// isosurface.cu — marching tetrahedra over a scalar grid (mipnerf_b200_isosurface_count / _emit).
+// isosurface.cu — marching tetrahedra over a scalar grid (mipnerf_b200_isosurface_count / _emit), and the vertex
+// normals of the emitted mesh from the grid's gradient (mipnerf_b200_isosurface_normals).
 //
 // Lattice point (i, j, k) of a grid [nz, ny, nx] (x fastest) sits at lo + idx * step per axis.  Each cell is split into
 // the 6 Kuhn tetrahedra v0 -> v0 + e_a -> v0 + e_a + e_b -> v0 + (1,1,1), one per axis permutation (a, b, c), so that
@@ -280,6 +281,56 @@ __global__ void __launch_bounds__(kIsoThreads) iso_face_kernel(const IsoGrid g, 
   }
 }
 
+// d(grid)/d(axis a) at lattice point idx (p its flat index): (v[+1] - v[-1]) / (2 step) inside, one-sided over step at
+// the box faces
+__device__ __forceinline__ float grid_partial(const IsoGrid& g, int64_t p, const int (&idx)[3], int a, float step) {
+  const int n = a == 0 ? g.nx : (a == 1 ? g.ny : g.nz);
+  const int64_t stride = a == 0 ? 1 : (a == 1 ? (int64_t)g.nx : (int64_t)g.nx * g.ny);
+  const bool lo = idx[a] == 0, hi = idx[a] == n - 1;
+  const float vp = __ldg(g.v + (hi ? p : p + stride)), vm = __ldg(g.v + (lo ? p : p - stride));
+  return __fdiv_rn(__fsub_rn(vp, vm), (lo || hi) ? step : __fmul_rn(2.f, step));
+}
+
+// pass 3 (after pass 2a): vertex normals, in the vertex order of iso_vertex_kernel (one thread per lattice point)
+__global__ void __launch_bounds__(kIsoThreads) iso_normal_kernel(const IsoGrid g, const IsoFrame fr,
+                                                                 const uint8_t* __restrict__ mask,
+                                                                 const int32_t* __restrict__ vbase,
+                                                                 float* __restrict__ normals) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= g.n) return;
+  const uint32_t m = mask[p];
+  if (!m) return;
+  int64_t id = vbase[p];
+  const int i = (int)(p % g.nx);
+  const int64_t q = p / g.nx;
+  const int j = (int)(q % g.ny), k = (int)(q / g.ny);
+  const int ia[3] = {i, j, k};
+  const float va = __ldg(g.v + p);
+  float ga[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) ga[a] = grid_partial(g, p, ia, a, fr.step[a]);
+  for (int d = 0; d < 7; ++d) {
+    if (!((m >> d) & 1u)) continue;
+    const int b = c_bits_of_dir[d];
+    const int ib[3] = {i + (b & 1), j + ((b >> 1) & 1), k + (b >> 2)};
+    const int64_t pb = p + (b & 1) + (int64_t)g.nx * (((b >> 1) & 1) + (int64_t)g.ny * (b >> 2));
+    const float vb = __ldg(g.v + pb);
+    float t = __fdiv_rn(__fsub_rn(g.iso, va), __fsub_rn(vb, va));  // the vertex's t (iso_vertex_kernel)
+    if (t != t) t = 0.5f;
+    float n[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const float gb = grid_partial(g, pb, ib, a, fr.step[a]);
+      n[a] = __fadd_rn(ga[a], __fmul_rn(t, __fsub_rn(gb, ga[a])));
+    }
+    const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(n[0], n[0]), __fmul_rn(n[1], n[1])), __fmul_rn(n[2], n[2])));
+    const bool ok = len > 0.f && len < INFINITY;  // false for NaN too
+#pragma unroll
+    for (int a = 0; a < 3; ++a) normals[id * 3 + a] = ok ? __fdiv_rn(-n[a], len) : 0.f;
+    ++id;
+  }
+}
+
 // scratch: [totals 2] [tile_v tiles] [tile_f tiles] (int64) | vbase [n] int32 | mask [n] uint8
 struct IsoScratch {
   int64_t *totals, *tile_v, *tile_f;
@@ -334,6 +385,18 @@ cudaError_t launch_isosurface_emit(const float* grid, int nx, int ny, int nz, co
   LaunchScope scope(kKernIsosurface, st);
   iso_vertex_kernel<<<(unsigned)s.tiles, kIsoThreads, 0, st>>>(g, fr, s.tile_v, s.mask, s.vbase, verts);
   iso_face_kernel<<<(unsigned)s.tiles, kIsoThreads, 0, st>>>(g, s.tile_f, s.mask, s.vbase, faces);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_isosurface_normals(const float* grid, int nx, int ny, int nz, const float* step, float iso,
+                                      const void* scratch, float* normals, cudaStream_t st) {
+  const IsoScratch s = carve_iso(nx, ny, nz, const_cast<void*>(scratch));
+  const IsoGrid g{grid, nx, ny, nz, iso, (int64_t)nx * ny * nz};
+  IsoFrame fr;
+  for (int a = 0; a < 3; ++a) fr.lo[a] = 0.f, fr.step[a] = step[a];
+  LaunchScope scope(kKernIsosurface, st);
+  iso_normal_kernel<<<(unsigned)((g.n + kIsoThreads - 1) / kIsoThreads), kIsoThreads, 0, st>>>(g, fr, s.mask, s.vbase,
+                                                                                                normals);
   return cudaGetLastError();
 }
 

@@ -47,6 +47,11 @@ cudaError_t launch_resample(const float* bins, const float* weights, const Draws
                             float padding, cudaStream_t st);
 // density[i] = softplus(raw[i] + density_bias)  (models/mip_nerf.py:237)
 cudaError_t launch_density_activation(const float* raw, float* density, int64_t n, float density_bias, cudaStream_t st);
+// rgb[i,c] = rgb_activation(raw_rgb[i,c]), density[i] = softplus(raw_density[i] + density_bias) (models/mip_nerf.py:
+// 236-237); either output may be null
+cudaError_t launch_radiance_activation(const float* raw_rgb, const float* raw_density, float* rgb, float* density,
+                                       int64_t n, float density_bias, float rgb_scale, float rgb_padding,
+                                       cudaStream_t st);
 
 // ---- isosurface.cu (marching tetrahedra; grid [nz, ny, nx], x fastest) ----
 size_t isosurface_scratch_bytes(int nx, int ny, int nz);
@@ -57,6 +62,9 @@ cudaError_t launch_isosurface_count(const float* grid, int nx, int ny, int nz, f
 // lo / step: HOST float[3] (lattice point idx at lo + idx * step per axis)
 cudaError_t launch_isosurface_emit(const float* grid, int nx, int ny, int nz, const float* lo, const float* step,
                                    float iso, const void* scratch, float* verts, int32_t* faces, cudaStream_t st);
+// after launch_isosurface_emit on the same scratch: the unit normal of every vertex (step: HOST float[3])
+cudaError_t launch_isosurface_normals(const float* grid, int nx, int ny, int nz, const float* step, float iso,
+                                      const void* scratch, float* normals, cudaStream_t st);
 
 // ---- metrics.cu ----
 size_t image_metrics_scratch_bytes(int height, int width, int channels);

@@ -161,7 +161,16 @@ struct LevelParams {
   const float* q_covs;
   int64_t num_points;
   float* density_out;
+  // Radiance mode (mipnerf_b200_query_radiance): the query points as in density-only mode, each with its own direction
+  // viewdirs [num_points, 3]; view_bias is the per-CTA slots [gridDim.x][2][128][128] of the points' view-direction
+  // terms (tile parity); raw heads into raw_rgb_out / raw_density_out, their activations into rgb_out / density_out (any
+  // may be null).
+  float* rgb_out;
 };
+
+// Compile-time modes of the level kernel: the forward (rays in, composited pixels out; MLP-only mode and the training
+// forward are runtime variants of it), density-only queries, and radiance queries with a view direction per point.
+enum LevelMode : int { kModeForward = 0, kModeDensity = 1, kModeRadiance = 2 };
 
 // raw density of (ray, row) of a ray of kNs samples with the density noise added; kept out of line so that the
 // (default) noise-free path carries none of the generator's registers
@@ -257,9 +266,9 @@ __device__ __forceinline__ void store8_split(uint8_t* dst_hi, uint8_t* dst_lo, c
 
 // Gaussian + IPE features [8 gi_begin, 8 gi_end) and [48 + 8 gi_begin, 48 + 8 gi_end) of one sample row of a ray (or,
 // in MLP-only mode, the caller's features) into the feature tile: SW128 slab (K 0..63) + SW64 tail (K 64..95).  `row`
-// is the row of the tile; MLP-only mode has one tile per ray.  kDensity: the row is query point 128 ray + row (zero
-// past the last one), encoded with the IPE of mipnerf_b200_integrated_pos_enc (ipe_pair<false>), so that the 16-bit
-// features equal MLP-only mode's rounding of that entry point's output.
+// is the row of the tile; MLP-only mode has one tile per ray.  kDensity (the query modes, density and radiance): the
+// row is query point 128 ray + row (zero past the last one), encoded with the IPE of mipnerf_b200_integrated_pos_enc
+// (ipe_pair<false>), so that the 16-bit features equal MLP-only mode's rounding of that entry point's output.
 template <int kFmt, bool kX3, int kT, bool kDensity = false>
 __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeom& g, int64_t ray, int row, float t0,
                                               float t1, uint8_t* myF, int gi_begin, int gi_end) {
@@ -711,15 +720,74 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+// Radiance mode: the view-direction term  b_view[n] + W_view[n, 256:283] . pos_enc(viewdir)  of each query point of
+// `tile` into its row of `slot` [128][128] (models/mip.py:353-363, models/mip_nerf.py:106-108).  fp32, with the
+// encoding and the fmaf order (the bias, then k = 0..26) of the level-0 prologue and view_bias_from_enc_kernel, so that
+// every term is theirs bit for bit.  A helper warp takes kViewPts points at a time: lane f < 27 encodes element f of
+// each, and the lane owns outputs n = 4 lane .. 4 lane + 3, whose weights it loads once per k for all kViewPts points.
+// Rows past the last point get the bias alone.  The stores go to L2 (st.cg); the consumers read them back with ld.cg
+// after feat_full, as the forward's view bias.
+constexpr int kViewPts = 4;
+__device__ __forceinline__ void level_view_terms(const LevelParams& p, int64_t tile, float* slot, int hw, int lane) {
+  const float4* wt = reinterpret_cast<const float4*>(p.wimage + kViewDirOffset);  // [27][128] | bias[128]
+  const float4 b4 = __ldg(wt + kViewDim * kCond / 4 + lane);
+#pragma unroll 1
+  for (int r = kViewPts * hw; r < kN; r += kViewPts * (kHelperThreads / 32)) {
+    float enc[kViewPts];
+#pragma unroll
+    for (int q = 0; q < kViewPts; ++q) {
+      const int64_t pt = tile * kN + r + q;
+      enc[q] = 0.f;
+      if (lane < kViewDim && pt < p.num_points) {
+        const float* vd = p.viewdirs + pt * 3;
+        if (lane < 3) {
+          enc[q] = __ldg(vd + lane);  // append_identity
+        } else {
+          const int gidx = lane - 3, is_cos = gidx >= 12, h = is_cos ? gidx - 12 : gidx;  // scale-major, then xyz
+          const float y = __fmul_rn(__ldg(vd + h % 3), __int_as_float((127 + h / 3) << 23));
+          enc[q] = sinf(is_cos ? __fadd_rn(y, MIPNERF_HALF_PI_F32) : y);
+        }
+      }
+    }
+    float acc[kViewPts][4];
+#pragma unroll
+    for (int q = 0; q < kViewPts; ++q) acc[q][0] = b4.x, acc[q][1] = b4.y, acc[q][2] = b4.z, acc[q][3] = b4.w;
+#pragma unroll 3
+    for (int k = 0; k < kViewDim; ++k) {
+      const float4 w4 = __ldg(wt + k * (kCond / 4) + lane);
+#pragma unroll
+      for (int q = 0; q < kViewPts; ++q) {
+        const float e = __shfl_sync(0xffffffffu, enc[q], k);
+        acc[q][0] = fmaf(w4.x, e, acc[q][0]);
+        acc[q][1] = fmaf(w4.y, e, acc[q][1]);
+        acc[q][2] = fmaf(w4.z, e, acc[q][2]);
+        acc[q][3] = fmaf(w4.w, e, acc[q][3]);
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < kViewPts; ++q)
+      __stcg(reinterpret_cast<float4*>(slot + (r + q) * kCond) + lane,
+             make_float4(acc[q][0], acc[q][1], acc[q][2], acc[q][3]));
+  }
+  __threadfence_block();
+}
+
 // ---- the helper warps' work (ht = helper thread 0..95, hw = helper warp 0..2) ----
 // Tile tt of `ray` into the feature buffer fbuf: first (tt == 0) the ray prologue, once per ray, then the tile's
 // features.  The prologue's global stores (fenceposts, view bias) are read back by this CTA only, through L2 (ld.cg):
 // by the helpers after the helper barrier, by the consumers after feat_full.  Density-only mode: the tile's query
-// points' features only.
-template <int kFmt, bool kX3, int kT, bool kDensity = false>
+// points' features only.  Radiance mode: first the view-direction terms of the tile's points into its slot `vslot`
+// (level_view_terms), then their features.
+template <int kFmt, bool kX3, int kT, int kMode = kModeForward>
 __device__ __forceinline__ void level_prepare_tile(const LevelParams& p, int64_t ray, int tt, uint8_t* fbuf,
-                                                   float* rs_scratch, int ht, int hw, int lane, PhaseClock& clk) {
+                                                   float* rs_scratch, int ht, int hw, int lane, PhaseClock& clk,
+                                                   float* vslot = nullptr) {
   constexpr int kNs = kT * kN;  // samples per ray
+  constexpr bool kDensity = kMode != kModeForward;  // a query mode: the tile is 128 query points
+  if constexpr (kMode == kModeRadiance) {
+    level_view_terms(p, ray, vslot, hw, lane);
+    clk.mark(kPhPrologue);
+  }
   if (!kDensity && (kT == 1 || tt == 0) && (p.t_mode != 0 || p.vb_mode != 0)) {
     if (hw == 0) {
       float* t_ray = p.t + ray * (kNs + 1);
@@ -904,12 +972,43 @@ __device__ __forceinline__ void level_density_out(const LevelParams& p, int64_t 
   clk.mark(kPhComposite);
 }
 
-// kDensity (kT = 1): density-only mode.  The producer streams the stages of layers 0-7 only (a prefix of the image),
-// the consumers run layers 0-7 and finish the density head in layer 7's epilogue, and the helpers encode the query
-// points and write the densities; everything else is the forward's schedule.
-template <int kFmt, bool kX3, int kT, bool kDensity = false>
+// Radiance mode: tile `tile`'s raw heads hd[128][4] plus the head biases (the sums MLP-only mode hands back,
+// models/mip_nerf.py:98,110) and their activations (models/mip_nerf.py:236-237); rows past the last point are masked.
+__device__ __forceinline__ void level_radiance_out(const LevelParams& p, int64_t tile, const float* hd,
+                                                   uint64_t* heads_empty, int ht, PhaseClock& clk) {
+  for (int row = ht; row < kN; row += kHelperThreads) {
+    const int64_t pt = tile * kN + row;
+    if (pt >= p.num_points) break;
+    const float4 h4 = *reinterpret_cast<const float4*>(hd + row * 4);
+    const float raw[4] = {h4.x + c_small.b_density, h4.y + c_small.b_color[0], h4.z + c_small.b_color[1],
+                          h4.w + c_small.b_color[2]};
+    if (p.raw_density_out) p.raw_density_out[pt] = raw[0];
+    if (p.density_out) p.density_out[pt] = density_activation(raw[0], p.density_bias);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      if (p.raw_rgb_out) p.raw_rgb_out[pt * 3 + ch] = raw[1 + ch];
+      if (p.rgb_out) p.rgb_out[pt * 3 + ch] = rgb_activation(raw[1 + ch], p.rgb_scale, p.rgb_padding);
+    }
+  }
+  mbar_arrive(heads_empty);
+  clk.mark(kPhComposite);
+}
+
+// kMode = kModeDensity (kT = 1): density-only mode.  The producer streams the stages of layers 0-7 only (a prefix of
+// the image), the consumers run layers 0-7 and finish the density head in layer 7's epilogue, and the helpers encode
+// the query points and write the densities; everything else is the forward's schedule.
+// kMode = kModeRadiance (kT = 1): radiance mode.  The producer and the consumers run the forward's schedule, except that
+// the view layer's epilogue adds to each row its own point's view-direction term instead of one per-ray bias.  The
+// helpers write those terms (level_view_terms) and the features of tile i ahead of the consumers, and the raw heads and
+// activations of tile i - 1 after them.  The terms of tile i go to slot i % 2 of this CTA; two slots are enough: the
+// helpers write slot i % 2 for tile i only after they have waited on heads_full of tile i - 2 (in the previous round
+// of their loop, with one feature buffer or two), and the consumers arrive on heads_full of a tile only after its view
+// layer's epilogue has read the tile's terms (the quad sums that the arriving thread stores depend on every loaded term).
+template <int kFmt, bool kX3, int kT, int kMode = kModeForward>
 __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParams p) {
-  static_assert(!kDensity || kT == 1, "density-only mode takes one 128-point tile at a time");
+  constexpr bool kDensity = kMode == kModeDensity;
+  constexpr bool kQuery = kMode != kModeForward;  // density or radiance: 128 query points per tile, no dumps
+  static_assert(!kQuery || kT == 1, "the query modes take one 128-point tile at a time");
   using Lay = LevelLayout<kX3, kT>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -967,8 +1066,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             const int fb = (int)(j % Lay::kFeatBufs);
             mbar_wait(&feat_empty[fb], ((uint32_t)(j / Lay::kFeatBufs) & 1u) ^ 1u);
             clk.mark(kPhFeatEmpty);
-            level_prepare_tile<kFmt, kX3, kT, kDensity>(p, ray, tt, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane,
-                                                        clk);
+            level_prepare_tile<kFmt, kX3, kT, kMode>(
+                p, ray, tt, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane, clk,
+                kMode == kModeRadiance ? p.view_bias + ((size_t)blockIdx.x * 2 + (j & 1)) * (kN * kCond) : nullptr);
             mbar_arrive(&feat_full[fb]);
           }
           if (tt == 0 && i > 0) {  // ray - gridDim.x, the (i - 1)-th ray of the CTA: tiles (i - 1) kT ..
@@ -979,6 +1079,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             clk.mark(kPhHeadsFull);
             if constexpr (kDensity)
               level_density_out(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], ht, clk);
+            else if constexpr (kMode == kModeRadiance)
+              level_radiance_out(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], ht, clk);
             else
               level_composite_ray<kT>(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], cs, ps, ht, hw, lane,
                                       clk);
@@ -1030,7 +1132,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   const uint32_t a_u = smem_u32(sA) + (uint32_t)wg * 64u * 128u;
   const uint32_t w_u = smem_u32(sW);
   // the training forward's dump (p.act_dump, p.v_dump) exists for kT = 1 only
-  const uint64_t dump_policy = kT == 1 && p.act_dump ? l2_policy_evict_first() : 0ull;  // must not evict the weights
+  const uint64_t dump_policy = kMode != kModeRadiance && kT == 1 && p.act_dump ? l2_policy_evict_first() : 0ull;  // must not evict the weights
   bool dump_pending = false;
   RingPos rp{0, 0u, -1};
   clk.begin(phase_rows + wg * kNumPhases, leader);
@@ -1078,7 +1180,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       // feature tile; layer 0 has two K-slabs (64 wide + the 32-wide tail), and two of its acc0 chunks follow each.  The
       // training forward's activation tiles go out from the epilogue's registers.
       const LevelRsCtx k{f_u, ft_u, w_u, w_full, w_empty, &feat_empty[fb], gsp,
-                         !kDensity && kT == 1 && p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
+                         !kQuery && kT == 1 && p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
                          (size_t)p.dump_tiles * kABytes, dump_policy, r0, cq, leader};
       uint32_t xa[64], xb[64];
       static_assert(2 * num_slabs(true, 0) == kEpiChunks, "layer 0: two acc0 chunks after each of its K-slabs");
@@ -1166,7 +1268,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
         clk.mark(kPhEpilogue);
         named_bar_sync(1 + wg, 128);
         clk.mark(kPhBarrier);
-        if (kT == 1 && p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core
+        if (kMode != kModeRadiance && kT == 1 && p.act_dump) {  // training forward: this warpgroup's rows of the 16-bit tile, as the tensor core
           // reads it
           if (leader) {
 #pragma unroll
@@ -1205,16 +1307,20 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       if (leader) mbar_arrive(&w_empty[rp.prev]);
       rp.prev = -1;
       clk.mark(kPhMma);
-      // view layer + colour head (models/mip_nerf.py:106-110); view_bias = the per-ray view-direction term
-      const float* vb = p.view_bias + ray * kCond;
-      uint8_t* vd = kT == 1 && p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
+      // view layer + colour head (models/mip_nerf.py:106-110); view_bias = the per-ray view-direction term (radiance
+      // mode: row r0 of the tile's slot; row r0 + 8 adds its own term b1)
+      const float* vb = kMode == kModeRadiance
+                            ? p.view_bias + ((size_t)blockIdx.x * 2 + par) * (kN * kCond) + (size_t)r0 * kCond
+                            : p.view_bias + ray * kCond;
+      uint8_t* vd = !kQuery && kT == 1 && p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int c = 8 * j + cq;
         const float2 b = __ldcg(reinterpret_cast<const float2*>(vb + c));
+        const float2 b1 = kMode == kModeRadiance ? __ldcg(reinterpret_cast<const float2*>(vb + 8 * kCond + c)) : b;
         float y[4] = {acc0[4 * j], acc0[4 * j + 1], acc0[4 * j + 2], acc0[4 * j + 3]};
         fadd2(y[0], y[1], b.x, b.y);
-        fadd2(y[2], y[3], b.x, b.y);
+        fadd2(y[2], y[3], b1.x, b1.y);
 #pragma unroll
         for (int e = 0; e < 4; ++e) y[e] = fmaxf(y[e], 0.f);
 #pragma unroll
@@ -1436,9 +1542,18 @@ int g_num_sms = 0;
 inline int fmt_of(int precision) { return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_BF16X3) ? 1 : 0; }
 inline bool is_x3(int precision) { return precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3; }
 
-template <int kFmt, bool kX3, int kT, bool kDensity = false>
+int num_sms() {
+  if (g_num_sms == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return g_num_sms;
+}
+
+template <int kFmt, bool kX3, int kT, int kMode = kModeForward>
 cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
-  auto kern = mlp_level_kernel<kFmt, kX3, kT, kDensity>;
+  auto kern = mlp_level_kernel<kFmt, kX3, kT, kMode>;
   constexpr uint32_t smem = LevelLayout<kX3, kT>::kTotal;
   static bool attr_set = false;  // one flag per instantiation
   if (!attr_set) {
@@ -1446,12 +1561,11 @@ cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  if (g_num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  LaunchScope scope(kDensity ? kKernDensityTc : (p.feat_in ? kKernMlpTc : kKernMlpLevelTc), st);
+  num_sms();
+  LaunchScope scope(kMode == kModeDensity    ? kKernDensityTc
+                    : kMode == kModeRadiance ? kKernRadianceTc
+                                             : (p.feat_in ? kKernMlpTc : kKernMlpLevelTc),
+                    st);
   const int grid = (int)(p.num_rays < g_num_sms ? p.num_rays : g_num_sms);
   kern<<<grid, kThreads, smem, st>>>(p);
   return cudaGetLastError();
@@ -1471,8 +1585,26 @@ cudaError_t launch_level(const LevelParams& p, int precision, int n, cudaStream_
 cudaError_t launch_density(const LevelParams& p, int precision, cudaStream_t st) {
   if (p.num_rays <= 0) return cudaSuccess;
   if (is_x3(precision))
-    return fmt_of(precision) ? launch_level_t<1, true, 1, true>(p, st) : launch_level_t<0, true, 1, true>(p, st);
-  return fmt_of(precision) ? launch_level_t<1, false, 1, true>(p, st) : launch_level_t<0, false, 1, true>(p, st);
+    return fmt_of(precision) ? launch_level_t<1, true, 1, kModeDensity>(p, st)
+                             : launch_level_t<0, true, 1, kModeDensity>(p, st);
+  return fmt_of(precision) ? launch_level_t<1, false, 1, kModeDensity>(p, st)
+                           : launch_level_t<0, false, 1, kModeDensity>(p, st);
+}
+cudaError_t launch_radiance(const LevelParams& p, int precision, cudaStream_t st) {
+  if (p.num_rays <= 0) return cudaSuccess;
+  if (is_x3(precision))
+    return fmt_of(precision) ? launch_level_t<1, true, 1, kModeRadiance>(p, st)
+                             : launch_level_t<0, true, 1, kModeRadiance>(p, st);
+  return fmt_of(precision) ? launch_level_t<1, false, 1, kModeRadiance>(p, st)
+                           : launch_level_t<0, false, 1, kModeRadiance>(p, st);
+}
+
+// radiance mode: the view-direction slots [ctas][2][128][128] fp32, one pair per CTA of a launch of min(tiles, SMs)
+constexpr size_t kRadianceSlotBytes = 2 * (size_t)kN * kCond * sizeof(float);
+int64_t radiance_ctas(int64_t num_points) {
+  const int64_t tiles = (num_points + kN - 1) / kN, chunk = kDensityChunkPoints / kN;
+  const int64_t t = tiles < chunk ? tiles : chunk;
+  return t < num_sms() ? t : num_sms();
 }
 
 }  // namespace
@@ -1709,6 +1841,42 @@ cudaError_t tc_query_density(const mipnerf_b200_config* c, const mipnerf_b200_we
     p.disable_integration = c->disable_integration;
     p.density_bias = c->density_bias;
     if ((e = launch_density(p, precision, st)) != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+size_t tc_radiance_workspace_bytes(int64_t num_points) {
+  return (size_t)radiance_ctas(num_points > 0 ? num_points : 1) * kRadianceSlotBytes;
+}
+
+cudaError_t tc_query_radiance(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, const float* means,
+                              const float* covs, const float* viewdirs, int64_t num_points, int precision,
+                              float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
+                              size_t workspace_bytes, cudaStream_t st) {
+  if (workspace_bytes < tc_radiance_workspace_bytes(num_points)) return cudaErrorInvalidValue;
+  const uint8_t* img = static_cast<const uint8_t*>(w->packed);
+  SmallUpload small(img, st);
+  cudaError_t e = small.error();
+  if (e != cudaSuccess) return e;
+  for (int64_t off = 0; off < num_points; off += kDensityChunkPoints) {
+    const int64_t cnt = (num_points - off) < kDensityChunkPoints ? (num_points - off) : kDensityChunkPoints;
+    LevelParams p{};
+    p.wimage = img;
+    p.q_means = means + off * 3;
+    p.q_covs = covs ? covs + off * 3 : nullptr;
+    p.viewdirs = viewdirs + off * 3;
+    p.view_bias = static_cast<float*>(workspace);  // the per-CTA slots, reused launch after launch on `st`
+    p.num_points = cnt;
+    p.num_rays = (cnt + kN - 1) / kN;
+    p.raw_rgb_out = raw_rgb ? raw_rgb + off * 3 : nullptr;
+    p.raw_density_out = raw_density ? raw_density + off : nullptr;
+    p.rgb_out = rgb ? rgb + off * 3 : nullptr;
+    p.density_out = density ? density + off : nullptr;
+    p.disable_integration = c->disable_integration;
+    p.density_bias = c->density_bias;
+    p.rgb_scale = (float)(1.0 + 2.0 * (double)c->rgb_padding);
+    p.rgb_padding = c->rgb_padding;
+    if ((e = launch_radiance(p, precision, st)) != cudaSuccess) return e;
   }
   return cudaSuccess;
 }

@@ -48,5 +48,13 @@ constexpr int64_t kDensityChunkPoints = 4096 * 128;
 cudaError_t tc_query_density(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
                              const float* covs, int64_t num_points, int precision, float* raw_density, float* density,
                              cudaStream_t st);
+// Radiance mode of the level kernels (mipnerf_b200_query_radiance), launched in the same chunks as the density query.
+// The workspace is two [128][128] fp32 slots of view-direction terms per CTA of a launch, min(tiles, SMs) CTAs with
+// tiles = ceil(points / 128) capped at one chunk's 4096.
+size_t tc_radiance_workspace_bytes(int64_t num_points);
+cudaError_t tc_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                              const float* covs, const float* viewdirs, int64_t num_points, int precision,
+                              float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
+                              size_t workspace_bytes, cudaStream_t st);
 
 }  // namespace mipnerf

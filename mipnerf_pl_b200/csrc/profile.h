@@ -30,6 +30,7 @@ enum KernelId : int {
   kKernImageMetrics, // PSNR + SSIM of a rendered frame
   kKernDensityTc,    // density-only mode of the wgmma level kernel (IPE + trunk + density head)
   kKernIsosurface,   // marching-tetrahedra isosurface extraction (count / scan / emit)
+  kKernRadianceTc,   // radiance mode of the wgmma level kernel (IPE + per-point view term + the whole MLP)
   kKernCount
 };
 

@@ -600,4 +600,24 @@ cudaError_t launch_density_activation(const float* raw, float* density, int64_t 
   return cudaGetLastError();
 }
 
+__global__ void radiance_activation_kernel(const float* __restrict__ raw_rgb, const float* __restrict__ raw_density,
+                                           float* __restrict__ rgb, float* __restrict__ density, int64_t n,
+                                           float density_bias, float rgb_scale, float rgb_padding) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (density) density[i] = density_activation(raw_density[i], density_bias);
+  if (rgb)
+    for (int c = 0; c < 3; ++c) rgb[i * 3 + c] = rgb_activation(raw_rgb[i * 3 + c], rgb_scale, rgb_padding);
+}
+
+cudaError_t launch_radiance_activation(const float* raw_rgb, const float* raw_density, float* rgb, float* density,
+                                       int64_t n, float density_bias, float rgb_scale, float rgb_padding,
+                                       cudaStream_t st) {
+  if (n == 0 || (!rgb && !density)) return cudaSuccess;
+  LaunchScope scope(kKernComposite, st);
+  radiance_activation_kernel<<<blocks_for(n, 256), 256, 0, st>>>(raw_rgb, raw_density, rgb, density, n, density_bias,
+                                                                 rgb_scale, rgb_padding);
+  return cudaGetLastError();
+}
+
 }  // namespace mipnerf

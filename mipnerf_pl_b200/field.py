@@ -5,8 +5,11 @@
 * `density_grid` queries a lattice in z-slabs.  By default each lattice point is the Gaussian of its voxel (variance
   step**2 / 12 per axis, a uniform voxel's), so the IPE integrates the field over the voxel's footprint and the grid is
   anti-aliased at its own scale.
-* `isosurface` extracts the `grid > iso` surface with the library's marching-tetrahedra kernels; `extract_mesh` is both.
-* `write_ply` writes a binary PLY with no dependency.
+* `isosurface` extracts the `grid > iso` surface with the library's marching-tetrahedra kernels, and optionally vertex
+  normals from the grid's gradient; `extract_mesh` is both.
+* `mesh_colors` colours vertices with `MipNerf.query_radiance` (the radiance mode of the level kernel on the tensor
+  cores), each vertex seen along its inward normal; `extract_mesh(colors=True)` adds normals and colours.
+* `write_ply` writes a binary PLY (optionally with normals and colours) with no dependency.
 """
 from __future__ import annotations
 
@@ -66,10 +69,12 @@ def density_grid(model, resolution: Resolution, bounds=DEFAULT_BOUNDS, variance=
     return out
 
 
-def isosurface(grid: torch.Tensor, iso: float, bounds=DEFAULT_BOUNDS) -> Tuple[torch.Tensor, torch.Tensor]:
+def isosurface(grid: torch.Tensor, iso: float, bounds=DEFAULT_BOUNDS, normals: bool = False):
     """The surface `grid > iso` of a [nz, ny, nx] grid whose lattice spans `bounds` -> (verts [V,3] fp32, faces [F,3]
     int32) on the grid's device.  Marching tetrahedra (6 per cell): a watertight, consistently oriented mesh whose
-    normals point from inside (> iso) to outside; NaN counts as outside.  Bit-reproducible."""
+    normals point from inside (> iso) to outside; NaN counts as outside.  Bit-reproducible.  With `normals`, also the
+    unit vertex normals [V,3] from the grid's gradient (central differences, interpolated along each vertex's edge),
+    pointing outside; (0, 0, 0) where the gradient is zero or not finite: (verts, faces, normals)."""
     dev = _dev(grid)
     if grid.dim() != 3:
         raise ValueError(f"grid must be [nz, ny, nx], got {tuple(grid.shape)}")
@@ -93,27 +98,76 @@ def isosurface(grid: torch.Tensor, iso: float, bounds=DEFAULT_BOUNDS) -> Tuple[t
         _cabi.check(lib.mipnerf_b200_isosurface_emit(g.data_ptr(), nx, ny, nz, lo, hi, float(iso), scratch.data_ptr(),
                                                      verts.data_ptr() if nv else None,
                                                      faces.data_ptr() if nf else None, st), "isosurface")
-    return verts, faces
+        if not normals:
+            return verts, faces
+        nrm = torch.empty(nv, 3, device=dev)
+        _cabi.check(lib.mipnerf_b200_isosurface_normals(g.data_ptr(), nx, ny, nz, lo, hi, float(iso),
+                                                        scratch.data_ptr(), nrm.data_ptr() if nv else None, st),
+                    "isosurface")
+    return verts, faces, nrm
+
+
+def mesh_colors(model, verts: torch.Tensor, normals: torch.Tensor, variance, slab_points: int = 1 << 22) -> torch.Tensor:
+    """The colour [V,3] of `model` at mesh vertices: the radiance (`MipNerf.query_radiance`) of each vertex's Gaussian
+    (diagonal `variance`, a float or one per axis, e.g. the voxel's step**2 / 12) seen along -normal, a ray arriving at
+    the surface from outside.  Queried in chunks of at most `slab_points` vertices."""
+    dev = next(model.parameters()).device
+    v = _f32(verts).to(dev).reshape(-1, 3)
+    d = -_f32(normals).to(dev).reshape(-1, 3)
+    var = torch.tensor(np.broadcast_to(np.asarray(variance, dtype=np.float32), (3,)).copy(), device=dev)
+    out = torch.empty(v.shape[0], 3, device=dev)
+    for o in range(0, v.shape[0], slab_points):
+        vv = v[o:o + slab_points]
+        out[o:o + len(vv)] = model.query_radiance(vv, var.expand(len(vv), 3), d[o:o + slab_points])[0]
+    return out
+
+
+def voxel_variance(resolution: Resolution, bounds=DEFAULT_BOUNDS) -> np.ndarray:
+    """step**2 / 12 per axis: the variance of a uniform voxel of the lattice (density_grid's default)."""
+    _, step = lattice_axes(resolution, bounds, "cpu")
+    return step.astype(np.float32) ** 2 / np.float32(12)
 
 
 def extract_mesh(model, threshold: float, resolution: Resolution = 256, bounds=DEFAULT_BOUNDS,
-                 variance=None) -> Tuple[torch.Tensor, torch.Tensor]:
-    """The surface density > threshold of `model` inside `bounds` -> (verts, faces) on the model's device."""
+                 variance=None, colors: bool = False):
+    """The surface density > threshold of `model` inside `bounds` -> (verts, faces) on the model's device.  With
+    `colors`: (verts, faces, normals, colors), the normals from the density grid's gradient and the colours from
+    `mesh_colors` with the grid's variance (by default the voxel's, step**2 / 12)."""
     grid = density_grid(model, resolution, bounds, variance)
-    return isosurface(grid, threshold, bounds)
+    if not colors:
+        return isosurface(grid, threshold, bounds)
+    verts, faces, normals = isosurface(grid, threshold, bounds, normals=True)
+    var = voxel_variance(resolution, bounds) if variance is None else variance
+    return verts, faces, normals, mesh_colors(model, verts, normals, var)
 
 
-def write_ply(path: str, verts, faces) -> None:
-    """Binary little-endian PLY: float x, y, z per vertex; uchar-counted int vertex_indices per face."""
+def write_ply(path: str, verts, faces, colors=None, normals=None) -> None:
+    """Binary little-endian PLY: float x, y, z per vertex, then (with `normals`) float nx, ny, nz and (with `colors`,
+    [V,3] in [0, 1]) uchar red, green, blue = round(255 clamp(c, 0, 1)); uchar-counted int vertex_indices per face."""
     v = np.ascontiguousarray(torch.as_tensor(verts).detach().cpu().numpy(), dtype="<f4").reshape(-1, 3)
     f = np.ascontiguousarray(torch.as_tensor(faces).detach().cpu().numpy(), dtype="<i4").reshape(-1, 3)
     rec = np.empty(len(f), dtype=[("n", "u1"), ("idx", "<i4", (3,))])
     rec["n"] = 3
     rec["idx"] = f
+    fields = [("xyz", "<f4", (3,))]
+    props = "property float x\nproperty float y\nproperty float z\n"
+    if normals is not None:
+        fields.append(("n", "<f4", (3,)))
+        props += "property float nx\nproperty float ny\nproperty float nz\n"
+    if colors is not None:
+        fields.append(("rgb", "u1", (3,)))
+        props += "property uchar red\nproperty uchar green\nproperty uchar blue\n"
+    vert = np.empty(len(v), dtype=fields)
+    vert["xyz"] = v
+    if normals is not None:
+        vert["n"] = np.asarray(torch.as_tensor(normals).detach().cpu().numpy(), dtype=np.float32).reshape(-1, 3)
+    if colors is not None:
+        c = np.asarray(torch.as_tensor(colors).detach().float().cpu().numpy(), dtype=np.float32).reshape(-1, 3)
+        vert["rgb"] = np.round(np.clip(c, 0.0, 1.0) * np.float32(255)).astype(np.uint8)
     header = ("ply\nformat binary_little_endian 1.0\n"
-              f"element vertex {len(v)}\nproperty float x\nproperty float y\nproperty float z\n"
+              f"element vertex {len(v)}\n{props}"
               f"element face {len(f)}\nproperty list uchar int vertex_indices\nend_header\n")
     with open(path, "wb") as fh:
         fh.write(header.encode("ascii"))
-        fh.write(v.tobytes())
+        fh.write(vert.tobytes())
         fh.write(rec.tobytes())

@@ -309,6 +309,46 @@ class MipNerf(torch.nn.Module):
                 _stream(dev)), "MipNerf.query_density")
         return out.reshape(shape)
 
+    @torch.no_grad()
+    def query_radiance(self, means: torch.Tensor, covs: Optional[torch.Tensor] = None,
+                       viewdirs: Optional[torch.Tensor] = None, *, raw: bool = False):
+        """Radiance of the field at Gaussians, each seen from its own direction: means / diagonal covs / viewdirs
+        [..., 3] -> (rgb [..., 3], density [...]) on `self.precision`: MLP.forward of the points' IPE features and view
+        encodings (models/mip_nerf.py:75-111), then the activations (models/mip_nerf.py:236-237), or the raw heads
+        (raw_rgb, raw_density) when `raw`.  No density noise and no grad_fn.  viewdirs are encoded as given; the
+        reference encodes unit directions.  They may be None only for a model with use_viewdirs=False (fp32: the colour
+        head then reads the trunk).  The tensor-core precisions take the configs `forward` takes on the tensor cores
+        (the radiance mode of the level kernel); fp32 any."""
+        if (means.shape[-1] != 3 or (covs is not None and covs.shape != means.shape) or
+                (viewdirs is not None and viewdirs.shape != means.shape)):
+            raise ValueError(f"means {tuple(means.shape)} / covs {None if covs is None else tuple(covs.shape)} / "
+                             f"viewdirs {None if viewdirs is None else tuple(viewdirs.shape)}: need [..., 3] of the "
+                             "same shape")
+        if viewdirs is None and self.use_viewdirs:
+            raise ValueError("query_radiance: viewdirs are required when use_viewdirs=True")
+        dev = _dev(means)
+        shape = means.shape[:-1]
+        m = _f32(means).reshape(-1, 3)
+        c = _f32(covs).reshape(-1, 3) if covs is not None else None
+        v = _f32(viewdirs).reshape(-1, 3) if viewdirs is not None else None
+        p = m.shape[0]
+        prec = _cabi.PRECISIONS[self.precision]
+        cfg = self._config()
+        ws, keep = self.mlp._weights_struct(cfg, prec, dev)
+        out_rgb = torch.empty(p, 3, device=dev)
+        out_dens = torch.empty(p, device=dev)
+        if p > 0:
+            lib = _cabi.lib()
+            nbytes = lib.mipnerf_b200_radiance_workspace_bytes(C.byref(cfg), p, prec)
+            scratch = _Workspace.get(dev, nbytes)
+            rgb_ptrs = (out_rgb.data_ptr(), out_dens.data_ptr(), None, None) if raw else \
+                (None, None, out_rgb.data_ptr(), out_dens.data_ptr())
+            with torch.cuda.device(dev):
+                _cabi.check(lib.mipnerf_b200_query_radiance(
+                    C.byref(cfg), C.byref(ws), m.data_ptr(), _ptr(c), _ptr(v), p, prec, *rgb_ptrs,
+                    scratch.data_ptr(), scratch.numel(), _stream(dev)), "MipNerf.query_radiance")
+        return out_rgb.reshape(*shape, 3), out_dens.reshape(shape)
+
     def _forward(self, rays: Rays, randomized: bool, white_bkgd: bool, t_rand, u_jitter, density_normal,
                  return_inds: bool):
         """The launches of `forward` -> (LevelOutputs, config, rng or None, per-level density normals or None,

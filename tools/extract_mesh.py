@@ -1,10 +1,12 @@
 """Extract the density isosurface of a trained MipNeRFSystem checkpoint as a binary PLY.
 
     python tools/extract_mesh.py --ckpt last.ckpt --threshold 50 --out mesh.ply \
-        [--resolution 256] [--bounds -1.5 -1.5 -1.5 1.5 1.5 1.5] [--precision bf16] [--point-sampled]
+        [--resolution 256] [--bounds -1.5 -1.5 -1.5 1.5 1.5 1.5] [--precision bf16] [--point-sampled] [--colors]
 
 The density is queried on a resolution^3 lattice over the bounds (each lattice point the Gaussian of its voxel unless
---point-sampled), and the surface density > threshold is extracted with marching tetrahedra on the GPU.
+--point-sampled), and the surface density > threshold is extracted with marching tetrahedra on the GPU.  With
+--colors the PLY also carries vertex normals (from the grid's gradient) and colours: the field's radiance at each
+vertex's Gaussian, seen along the inward normal.
 """
 import argparse
 import os
@@ -29,6 +31,7 @@ def main(argv=None):
                     metavar=("X0", "Y0", "Z0", "X1", "Y1", "Z1"))
     ap.add_argument("--precision", default="bf16", choices=sorted(mp._cabi.PRECISIONS))
     ap.add_argument("--point-sampled", action="store_true", help="zero covariance instead of the voxel's")
+    ap.add_argument("--colors", action="store_true", help="add vertex normals and colours (query_radiance)")
     ap.add_argument("--out", required=True)
     ap.add_argument("--device", default="cuda:0")
     args = ap.parse_args(argv)
@@ -38,10 +41,15 @@ def main(argv=None):
     bounds = (tuple(args.bounds[:3]), tuple(args.bounds[3:]))
     t0 = time.perf_counter()
     grid = mp.density_grid(model, res, bounds, variance=0.0 if args.point_sampled else None)
-    verts, faces = mp.isosurface(grid, args.threshold, bounds)
+    normals = colors = None
+    if args.colors:
+        verts, faces, normals = mp.isosurface(grid, args.threshold, bounds, normals=True)
+        colors = mp.mesh_colors(model, verts, normals, 0.0 if args.point_sampled else mp.voxel_variance(res, bounds))
+    else:
+        verts, faces = mp.isosurface(grid, args.threshold, bounds)
     torch.cuda.synchronize()
     t1 = time.perf_counter()
-    mp.write_ply(args.out, verts, faces)
+    mp.write_ply(args.out, verts, faces, colors=colors, normals=normals)
     print(f"{args.out}: {len(verts)} vertices, {len(faces)} faces (grid {tuple(grid.shape[::-1])}, density "
           f"{float(grid.min()):.3g}..{float(grid.max()):.3g}, {t1 - t0:.2f} s on the GPU)")
 

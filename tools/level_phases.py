@@ -8,6 +8,10 @@ wait for a free raw-heads buffer; the helpers' `barrier` is their own named barr
 compositing scans).
 
     python tools/level_phases.py [--rays 4096] [--reps 20] [--precisions bf16,fp16x3] [--json OUT]
+    python tools/level_phases.py --query 4194304 ...   # query_radiance and query_density on that many points instead
+
+In query mode the helpers' `prologue` is the radiance mode's per-point view-direction terms and `composite` the
+writing of the outputs; both query modes charge slot `level0`.
 
 With MIPNERF_B200_LIB set, that (instrumented) library is used instead of building one.
 """
@@ -37,6 +41,7 @@ def main():
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--precisions", default="bf16,fp16x3")
     ap.add_argument("--json", default=None, help="also write the result as JSON to this path")
+    ap.add_argument("--query", type=int, default=0, help="points of a query_radiance / query_density run instead")
     args = ap.parse_args()
 
     if not os.environ.get("MIPNERF_B200_LIB"):  # a prebuilt instrumented library may be passed in
@@ -58,25 +63,34 @@ def main():
     max_ctas = C.c_int(0)
     buf = np.zeros(2 * 1024 * len(ROLES) * (len(PHASES) + 1), dtype=np.uint64)  # [slot][cta][role][phase + total]
     result = {"gpu": gpu_info(), "rays": args.rays, "reps": args.reps, "runs": {}}
-    for precision in args.precisions.split(","):
+    if args.query:
+        g = torch.Generator().manual_seed(0)
+        q_means = (3.0 * torch.rand(args.query, 3, generator=g) - 1.5).to(dev)
+        q_covs = (10 ** (-6 + 5 * torch.rand(args.query, 3, generator=g))).to(dev)
+        q_dirs = torch.nn.functional.normalize(torch.randn(args.query, 3, generator=g), dim=-1).to(dev)
+    for precision, what in [(p, w) for p in args.precisions.split(",")
+                            for w in (("radiance", "density") if args.query else ("forward",))]:
         model = mp.MipNerf(precision=precision)
         model.load_state_dict(sd)
         model = model.to(dev).eval()
+        call = {"forward": lambda: model(rays, False, True),
+                "radiance": lambda: model.query_radiance(q_means, q_covs, q_dirs),
+                "density": lambda: model.query_density(q_means, q_covs)}[what]
         for _ in range(3):
-            model(rays, False, True)
+            call()
         torch.cuda.synchronize()
         read(buf.ctypes.data_as(C.POINTER(C.c_ulonglong)), C.byref(max_ctas))  # reset
         start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         start.record()
         for _ in range(args.reps):
-            model(rays, False, True)
+            call()
         stop.record()
         torch.cuda.synchronize()
         nph = read(buf.ctypes.data_as(C.POINTER(C.c_ulonglong)), C.byref(max_ctas))
         assert nph == len(PHASES) + 1, nph
         data = buf.reshape(2, max_ctas.value, len(ROLES), nph).astype(np.float64)
-        run = {"forward_ms": start.elapsed_time(stop) / args.reps}
-        for s, level in enumerate(LEVELS):
+        run = {f"{what}_ms": start.elapsed_time(stop) / args.reps}
+        for s, level in enumerate(LEVELS[:1] if args.query else LEVELS):
             d = data[s]
             ctas = d[:, 0, -1] > 0
             row = {"ctas": int(ctas.sum()),
@@ -86,7 +100,7 @@ def main():
                 row[role] = {ph: round(float((d[ctas, r, i] / tot).mean()), 4) for i, ph in enumerate(PHASES)
                              if d[ctas, r, i].any()}
             run[level] = row
-        result["runs"][precision] = run
+        result["runs"][precision if what == "forward" else f"{precision}_{what}"] = run
     print(json.dumps(result, indent=1))
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
