@@ -339,8 +339,9 @@ __device__ __forceinline__ void ipe_row_group(const LevelParams& p, const RayGeo
 //     split modes) into a ring of 16 KB slots; a slot is free once both warpgroups' wgmmas reading it have completed.
 //   * warps 9-11 are the helpers: while the consumers run the layers of ray r, they run the ray prologue of ray r + 1
 //     (the coarse fenceposts (level 0) or the bit-exact inverse-CDF resampler (levels >= 1), and the per-ray
-//     view-layer bias (level 0; later levels read it back)), write its Gaussians + IPE features into a free feature
-//     buffer, and then composite ray r once its raw heads are in.
+//     view-layer bias (level 0; later levels read it back), which they leave in a shared-memory slot for the view
+//     layer's epilogue), write its Gaussians + IPE features into a free feature buffer, and then composite ray r once
+//     its raw heads are in.
 // Hand-offs (mbarriers): feat_full[b] (helpers -> consumers: the features of buffer b are written and fenced for the
 // async proxy), feat_empty[b] (consumers -> helpers: the wait that retires layer 5's last skip K-slab has returned, the
 // last read of the buffer), heads_full[par] / heads_empty[par] (the raw heads of rays of parity par).  A forward is one
@@ -387,9 +388,13 @@ struct LevelLayout {
   // sums [4 kT][8] (one per 32-row chunk of the ray), resampler scratch [128 kT + 1]
   static constexpr uint32_t kMiscBytes =
       kNumMbars * 8 + 2 * kN * 4 * 4 + 4 * kT * 4 + 4 * kT * 8 * 4 + (kT * kN + 1) * 4;
-  static constexpr uint32_t kPhase = (kMisc + kMiscBytes + 7) & ~7u;  // phase accumulators (MIPNERF_LEVEL_PHASES)
+  // the forward's per-ray view bias [2][128] fp32 (parity of the ray's index in the CTA): the helpers fill it in the
+  // ray prologue, the consumers' view-layer epilogue reads it
+  static constexpr uint32_t kVBias = (kMisc + kMiscBytes + 15) & ~15u;
+  static constexpr uint32_t kVBiasBytes = 2 * kCond * 4;
+  static constexpr uint32_t kPhase = kVBias + kVBiasBytes;  // phase accumulators (MIPNERF_LEVEL_PHASES)
   // + slack for the 1024-B alignment of the tiles
-  static constexpr uint32_t kTotal = kMisc + kMiscBytes + (kPhaseBytes ? kPhaseBytes + 8 : 0) + 1024;
+  static constexpr uint32_t kTotal = kPhase + kPhaseBytes + 1024;
   static_assert(kT == 1 || kT == 2, "a ray is one or two 128-row tiles");
   static_assert(kNumMbars % 2 == 0, "the raw heads behind the mbarriers must be 16-B aligned");
   static_assert(kTotal <= 232448, "exceeds 227 KB of shared memory per CTA");
@@ -774,21 +779,22 @@ __device__ __forceinline__ void level_view_terms(const LevelParams& p, int64_t t
 
 // ---- the helper warps' work (ht = helper thread 0..95, hw = helper warp 0..2) ----
 // Tile tt of `ray` into the feature buffer fbuf: first (tt == 0) the ray prologue, once per ray, then the tile's
-// features.  The prologue's global stores (fenceposts, view bias) are read back by this CTA only, through L2 (ld.cg):
-// by the helpers after the helper barrier, by the consumers after feat_full.  Density-only mode: the tile's query
-// points' features only.  Radiance mode: first the view-direction terms of the tile's points into its slot `vslot`
-// (level_view_terms), then their features.
+// features.  The prologue leaves the ray's view bias in its shared-memory slot vb_slot[128] for the consumers (computed
+// at level 0, which also stores it to p.view_bias for the later levels; copied from p.view_bias otherwise, MLP-only
+// mode included).  Its global stores (fenceposts, view bias) are read back by this CTA only, through L2 (ld.cg), by the
+// helpers after the helper barrier.  Density-only mode: the tile's query points' features only.  Radiance mode: first
+// the view-direction terms of the tile's points into its slot `vslot` (level_view_terms), then their features.
 template <int kFmt, bool kX3, int kT, int kMode = kModeForward>
 __device__ __forceinline__ void level_prepare_tile(const LevelParams& p, int64_t ray, int tt, uint8_t* fbuf,
                                                    float* rs_scratch, int ht, int hw, int lane, PhaseClock& clk,
-                                                   float* vslot = nullptr) {
+                                                   float* vb_slot, float* vslot = nullptr) {
   constexpr int kNs = kT * kN;  // samples per ray
   constexpr bool kDensity = kMode != kModeForward;  // a query mode: the tile is 128 query points
   if constexpr (kMode == kModeRadiance) {
     level_view_terms(p, ray, vslot, hw, lane);
     clk.mark(kPhPrologue);
   }
-  if (!kDensity && (kT == 1 || tt == 0) && (p.t_mode != 0 || p.vb_mode != 0)) {
+  if (!kDensity && (kT == 1 || tt == 0)) {
     if (hw == 0) {
       float* t_ray = p.t + ray * (kNs + 1);
       if (p.t_mode == 1) {  // coarse fenceposts (bit-identical to coarse_t_kernel)
@@ -802,9 +808,13 @@ __device__ __forceinline__ void level_prepare_tile(const LevelParams& p, int64_t
                                  p.u_jitter, ray, p.resample_padding, rs_scratch, t_ray,
                                  p.inds ? p.inds + ray * (kNs + 1) : nullptr, lane);
       }
-    } else if (hw == 1 && p.vb_mode == 1) {
+    } else if (hw == 1 && p.vb_mode == 0) {  // the ray's view bias from p.view_bias into its slot
+#pragma unroll
+      for (int j = 0; j < 4; ++j) vb_slot[lane + 32 * j] = __ldcg(p.view_bias + ray * kCond + lane + 32 * j);
+    } else if (hw == 1) {
       // per-ray view-layer bias  b[n] + W[n, 256:283] . pos_enc(viewdir)   (models/mip.py:353-363,
-      // models/mip_nerf.py:106-108): lane f < 27 owns encoding element f, lane owns outputs n = lane + 32 j
+      // models/mip_nerf.py:106-108): lane f < 27 owns encoding element f, lane owns outputs n = lane + 32 j; into the
+      // ray's slot, and into p.view_bias for the later levels
       float enc = 0.f;
       if (lane < kViewDim) {
         if (lane < 3) {
@@ -826,12 +836,17 @@ __device__ __forceinline__ void level_prepare_tile(const LevelParams& p, int64_t
         for (int j = 0; j < 4; ++j) acc[j] = fmaf(__ldg(wt + k * kCond + lane + 32 * j), e, acc[j]);
       }
 #pragma unroll
-      for (int j = 0; j < 4; ++j) __stcg(p.view_bias + ray * kCond + lane + 32 * j, acc[j]);
+      for (int j = 0; j < 4; ++j) {
+        vb_slot[lane + 32 * j] = acc[j];
+        __stcg(p.view_bias + ray * kCond + lane + 32 * j, acc[j]);
+      }
     }
     __threadfence_block();
     clk.mark(kPhPrologue);
-    named_bar_sync(kHelperBar, kHelperThreads);
-    clk.mark(kPhBarrier);
+    if (p.t_mode != 0 || p.vb_mode != 0) {  // the prologue's global stores are read back after the helper barrier
+      named_bar_sync(kHelperBar, kHelperThreads);
+      clk.mark(kPhBarrier);
+    }
   }
   // Gaussians + IPE features: 128 rows x 3 parts of two 8-feature groups = 384 units, four per helper thread; a warp's
   // 32 units share their part
@@ -1004,6 +1019,12 @@ __device__ __forceinline__ void level_radiance_out(const LevelParams& p, int64_t
 // helpers write slot i % 2 for tile i only after they have waited on heads_full of tile i - 2 (in the previous round
 // of their loop, with one feature buffer or two), and the consumers arrive on heads_full of a tile only after its view
 // layer's epilogue has read the tile's terms (the quad sums that the arriving thread stores depend on every loaded term).
+// kMode = kModeForward: the per-ray view bias of the i-th ray of the CTA is in shared-memory slot vbias[i % 2], which
+// the helpers fill in the ray prologue of its tile 0 and the view-layer epilogues of all its tiles read.  The same
+// argument holds per ray: the helpers fill the slot of ray i only after they have waited on heads_full of every tile of
+// ray i - 2 (in round i - 1 of their loop, with kT = 1 or 2 and one feature buffer or two), and the consumers arrive on
+// heads_full of a tile only after its view-layer epilogue has read the slot; the slot of ray i is written before the
+// feat_full arrive of its tile 0, which the consumers wait on before any tile of ray i.
 template <int kFmt, bool kX3, int kT, int kMode = kModeForward>
 __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParams p) {
   constexpr bool kDensity = kMode == kModeDensity;
@@ -1026,6 +1047,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   float* cs = heads + 2 * kN * 4;                            // [4 kT] scan carries
   float* ps = cs + 4 * kT;                                   // [4 kT][8] partial sums
   float* rs_scratch = ps + 32 * kT;                          // [128 kT + 1] resampler scratch
+  float* vbias = reinterpret_cast<float*>(smem + Lay::kVBias);  // [2][128] forward: per-ray view bias (ray parity)
   unsigned long long* phase_rows = reinterpret_cast<unsigned long long*>(smem + Lay::kPhase);
   const int phase_slot = p.t_mode == 2 ? 1 : 0;
   PhaseClock clk;
@@ -1067,7 +1089,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             mbar_wait(&feat_empty[fb], ((uint32_t)(j / Lay::kFeatBufs) & 1u) ^ 1u);
             clk.mark(kPhFeatEmpty);
             level_prepare_tile<kFmt, kX3, kT, kMode>(
-                p, ray, tt, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane, clk,
+                p, ray, tt, sF + fb * Lay::kFBuf, rs_scratch, ht, hw, lane, clk, vbias + (i & 1) * kCond,
                 kMode == kModeRadiance ? p.view_bias + ((size_t)blockIdx.x * 2 + (j & 1)) * (kN * kCond) : nullptr);
             mbar_arrive(&feat_full[fb]);
           }
@@ -1141,6 +1163,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
     // the tile's feature buffer and raw-heads parity, and their mbarrier phases
     const int fb = (int)(i % Lay::kFeatBufs), par = (int)(i & 1);
     const uint32_t fph = (uint32_t)(i / Lay::kFeatBufs) & 1u, hph = (uint32_t)(i >> 1) & 1u;
+    const int vpar = kT == 1 ? par : (int)hph;  // the ray's view-bias slot: the parity of i / kT
     // this warpgroup's rows of the tile's feature buffer (SW128 slab, SW64 tail)
     const uint32_t f_u = smem_u32(sF) + (uint32_t)fb * Lay::kFBuf + (uint32_t)wg * 64u * 128u;
     const uint32_t ft_u = smem_u32(sF) + (uint32_t)fb * Lay::kFBuf + kStageBytes + (uint32_t)wg * 64u * 64u;
@@ -1301,22 +1324,30 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       }
     }
     if constexpr (!kDensity) {
-      // the view layer's epilogue from the registers
+      // the view layer's epilogue from the registers; the forward reads its columns of the ray's view bias from the
+      // ray's slot, in bf16 / fp16 while the last K-slab's wgmmas run (the split modes' training forward has no
+      // registers to spare there: ptxas spills 32 values)
+      const float* vs = vbias + vpar * kCond + cq;
+      float2 vbr[16];
+      if constexpr (kMode == kModeForward && !kX3) {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) vbr[j] = *reinterpret_cast<const float2*>(vs + 8 * j);
+      }
       wgmma_wait<0>();
       wgmma_fence_acc(acc0);
       if (leader) mbar_arrive(&w_empty[rp.prev]);
       rp.prev = -1;
       clk.mark(kPhMma);
-      // view layer + colour head (models/mip_nerf.py:106-110); view_bias = the per-ray view-direction term (radiance
-      // mode: row r0 of the tile's slot; row r0 + 8 adds its own term b1)
-      const float* vb = kMode == kModeRadiance
-                            ? p.view_bias + ((size_t)blockIdx.x * 2 + par) * (kN * kCond) + (size_t)r0 * kCond
-                            : p.view_bias + ray * kCond;
+      // view layer + colour head (models/mip_nerf.py:106-110); view bias = the per-ray view-direction term (radiance
+      // mode: row r0 of the tile's global slot; row r0 + 8 adds its own term b1)
+      const float* vb = p.view_bias + ((size_t)blockIdx.x * 2 + par) * (kN * kCond) + (size_t)r0 * kCond;
       uint8_t* vd = !kQuery && kT == 1 && p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int c = 8 * j + cq;
-        const float2 b = __ldcg(reinterpret_cast<const float2*>(vb + c));
+        const float2 b = kMode == kModeRadiance ? __ldcg(reinterpret_cast<const float2*>(vb + c))
+                         : kX3                  ? *reinterpret_cast<const float2*>(vs + 8 * j)
+                                                : vbr[j];
         const float2 b1 = kMode == kModeRadiance ? __ldcg(reinterpret_cast<const float2*>(vb + 8 * kCond + c)) : b;
         float y[4] = {acc0[4 * j], acc0[4 * j + 1], acc0[4 * j + 2], acc0[4 * j + 3]};
         fadd2(y[0], y[1], b.x, b.y);
