@@ -180,7 +180,12 @@ typedef struct mipnerf_b200_loss {
   float* per_ray_distloss;      /* [num_levels, B] device, nullable                                  */
 } mipnerf_b200_loss;
 
+/* Workspace of the training step for every non-split precision (FP32, BF16, FP16): the largest of
+ * mipnerf_b200_train_workspace_bytes_for over the three.  0 for configs the training step does not take. */
 size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_rays);
+/* Workspace of the training step in one precision.  BF16X3 (chunks of 2048 rays, 5.7 GiB at the default
+ * architecture, the 16-bit step's 4096-ray chunk 6.3 GiB) is non-zero only for the configs its fused step takes. */
+size_t mipnerf_b200_train_workspace_bytes_for(const mipnerf_b200_config* cfg, int64_t num_rays, int precision);
 
 /* MipNerf.forward (outputs in `outs`, as mipnerf_b200_forward) followed by the backward pass of the loss
  * above into `grads` (overwritten, or added to when `accumulate` != 0).  Replaces
@@ -190,7 +195,11 @@ size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_
  * 16-bit operands, heads / rendering in fp32.  The fused step (level kernels + 16-bit activation tile images) runs for
  * the level kernel's shapes (the default architecture and encodings, 128 samples only) with at most two levels; other
  * shapes with the default widths and encoding sizes (96-d IPE, 27-d view encoding) and net_depth <= 16 run per-layer
- * GEMMs on fp32 activations. */
+ * GEMMs on fp32 activations.  BF16X3 (the fused step only, at the same shapes; workspace from
+ * mipnerf_b200_train_workspace_bytes_for): every operand of the forward, dgrad and wgrad GEMMs is split into bf16 hi +
+ * lo halves (16 significant bits, fp32's range) and each product is hi.hi + lo.hi + hi.lo into fp32; gradients land an
+ * order of magnitude closer to FP32's than BF16's.  FP16X3 is forward-only: MIPNERF_B200_EUNSUPPORTED, as is BF16X3 at
+ * other shapes. */
 int mipnerf_b200_forward_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* weights,
                                   const mipnerf_b200_rays* rays, int randomized, const float* t_rand,
                                   const float* u_jitter, int white_bkgd, int precision,
@@ -220,7 +229,7 @@ typedef struct mipnerf_b200_level_cotangent {
  * forward's seed / offset), else density_normal[l] [B,N] (required when randomized and cfg->density_noise > 0).
  * `randomized` only selects the density noise.  Same 4096-ray chunking and workspace as the training step
  * (mipnerf_b200_train_workspace_bytes).  precision FP32 or BF16; FP16 is refused (its fixed gradient scale is sized
- * for the training loss), the split precisions are forward-only. */
+ * for the training loss), the split precisions are refused (BF16X3 trains through mipnerf_b200_forward_backward only). */
 int mipnerf_b200_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* weights,
                           const mipnerf_b200_rays* rays, const float* const* t_samples, int randomized,
                           const mipnerf_b200_rng* rng, const float* const* density_normal, int white_bkgd,
@@ -249,6 +258,18 @@ size_t mipnerf_b200_wgrad_tc_scratch_bytes(int n, int k);
 int mipnerf_b200_wgrad_tc(const float* dy, int n, const float* x1, int k1, const float* x2, int k2, int x2_row_div,
                           int64_t m, float* dw, float* db, int precision, void* scratch, size_t scratch_bytes,
                           void* stream);
+
+/* The bf16x3 training step's GEMMs on their own, for tests: the fp32 operands are split into bf16 hi + lo tile images
+ * and run through the step's kernels.  linear_x3: y[m,n] = [mask > 0] * (x[m,k] . weight[n,k]^T + r1[m] r1w[n]) (mask,
+ * r1 nullable; r1 needs m % 128 == 0), y = hi + lo of the output images; n, k in {128, 256}.  wgrad_x3: as
+ * mipnerf_b200_wgrad_tc; x2 is split into images when x2_row_div == 1 and read as fp32 rows otherwise (then
+ * x2_row_div % 64 == 0 and m % 128 == 0). */
+size_t mipnerf_b200_linear_x3_scratch_bytes(int64_t m, int n, int k);
+int mipnerf_b200_linear_x3(const float* x, const float* weight, const float* r1, const float* r1w, const float* mask,
+                           float* y, int64_t m, int n, int k, void* scratch, size_t scratch_bytes, void* stream);
+size_t mipnerf_b200_wgrad_x3_scratch_bytes(int64_t m, int n, int k1, int k2, int x2_row_div);
+int mipnerf_b200_wgrad_x3(const float* dy, int n, const float* x1, int k1, const float* x2, int k2, int x2_row_div,
+                          int64_t m, float* dw, float* db, void* scratch, size_t scratch_bytes, void* stream);
 
 /* torch.optim.Adam.step() for one flat fp32 tensor (models/nerf_system.py:70-72; amsgrad off, no weight
  * decay): `step` is the 1-based step count after this update; the gradient is read as grad * grad_scale

@@ -91,6 +91,7 @@ _SIGNATURES = {
     "mipnerf_b200_philox_normal": (C.c_int, [C.POINTER(Rng), C.c_int, C.c_int64, C.c_int, _V, _V]),
     "mipnerf_b200_distloss": (C.c_int, [_V, _V, C.c_int64, C.c_int, _V, _V]),
     "mipnerf_b200_train_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64]),
+    "mipnerf_b200_train_workspace_bytes_for": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int]),
     "mipnerf_b200_forward_backward": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), C.POINTER(RaysStruct), C.c_int,
                                                 _V, _V, C.c_int, C.c_int, C.POINTER(Loss), C.POINTER(LevelOut),
                                                 C.POINTER(LinearGrad), C.c_int, C.c_int, _V, C.c_size_t, _V]),
@@ -104,6 +105,11 @@ _SIGNATURES = {
     "mipnerf_b200_linear_tc": (C.c_int, [_V, _V, _V, _V, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),
     "mipnerf_b200_wgrad_tc_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "mipnerf_b200_wgrad_tc": (C.c_int, [_V, C.c_int, _V, C.c_int, _V, C.c_int, C.c_int, C.c_int64, _V, _V, C.c_int, _V,
+                                        C.c_size_t, _V]),
+    "mipnerf_b200_linear_x3_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int]),
+    "mipnerf_b200_linear_x3": (C.c_int, [_V, _V, _V, _V, _V, _V, C.c_int64, C.c_int, C.c_int, _V, C.c_size_t, _V]),
+    "mipnerf_b200_wgrad_x3_scratch_bytes": (C.c_size_t, [C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mipnerf_b200_wgrad_x3": (C.c_int, [_V, C.c_int, _V, C.c_int, _V, C.c_int, C.c_int, C.c_int64, _V, _V, _V,
                                         C.c_size_t, _V]),
     "mipnerf_b200_adam_step": (C.c_int, [_V, _V, _V, _V, C.c_int64, C.c_double, C.c_double, C.c_double, C.c_double,
                                          C.c_int64, C.c_double, _V]),

@@ -34,6 +34,9 @@ int fail(int code, const char* fmt, ...) {
   } while (0)
 
 constexpr int64_t kChunkRaysFp32 = 4096;  // bounds the fp32 path's activation scratch (~1.8 GB)
+// the bf16x3 training step carries every tile image twice (hi, lo): half the chunk keeps its scratch at the 16-bit
+// step's (5.7 GiB instead of 11 GiB at the default architecture)
+constexpr int64_t kChunkRaysX3 = 2048;
 
 inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
@@ -431,6 +434,8 @@ TrainScratch carve_train(const mipnerf_b200_config* c, const Dims& d, int64_t ra
 // Scratch of the fused tensor-core training step (forward = the level kernels with the activation dump, backward on
 // 16-bit tile images, train_t16.cu).  Overlays the same workspace as TrainScratch.
 struct FusedScratch {
+  // bf16x3: every tile image below is followed by its lo image of the same size (act: [2][9][rays][64 KB]), and the
+  // images carve holds the lo images of the dgrad B operands as well
   uint8_t *act[2], *v[2];                // forward dump per level: [9][rays][64 KB], [rays][32 KB]
   float *raw_rgb[2], *raw_density[2];    // raw heads per level
   float *enc, *venc, *d_raw_rgb, *d_raw_density, *part, *t[2], *w[2];
@@ -451,6 +456,7 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
     return p;
   };
   auto take = [&](size_t elems) { return reinterpret_cast<float*>(take_bytes(elems * sizeof(float))); };
+  const size_t x = precision == MIPNERF_B200_BF16X3 ? 2 : 1;  // tile images per operand: hi (, lo)
   // chunk-invariant buffers first: the weight images are packed once per call into the first chunk's carve and read
   // by every chunk, so no per-ray buffer of a shorter last chunk may move onto them
   const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
@@ -459,8 +465,8 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
   s.images = take_bytes((size_t)kTrainImages * kTrainImageBytes);
   s.packed = take_bytes(mipnerf::tc_packed_bytes(c, precision));
   for (int l = 0; l < 2; ++l) {
-    s.act[l] = take_bytes((size_t)9 * rays * 65536);
-    s.v[l] = take_bytes((size_t)rays * 32768);
+    s.act[l] = take_bytes(x * 9 * rays * 65536);
+    s.v[l] = take_bytes(x * rays * 32768);
     s.raw_rgb[l] = take(m * 3);
     s.raw_density[l] = take(m);
     s.t[l] = take((size_t)rays * (c->num_samples + 1));
@@ -470,11 +476,11 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
   s.venc = take((size_t)rays * d.view_dim);
   s.d_raw_rgb = take(m * 3);
   s.d_raw_density = take(m);
-  s.enc16 = take_bytes((size_t)rays * 32768);
+  s.enc16 = take_bytes(x * rays * 32768);
   s.relu_bits = take_bytes(m * 32);
-  s.d_v = take_bytes((size_t)rays * 32768);
-  s.d_a = take_bytes((size_t)rays * 65536);
-  s.d_b = take_bytes((size_t)rays * 65536);
+  s.d_v = take_bytes(x * rays * 32768);
+  s.d_a = take_bytes(x * rays * 65536);
+  s.d_b = take_bytes(x * rays * 65536);
   s.tcws_bytes = mipnerf::tc_workspace_bytes(c, rays, precision);
   s.tcws = take_bytes(s.tcws_bytes);
   s.bytes = off;
@@ -485,7 +491,8 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
 // activation dump is one tile per ray) and at most two levels; other shapes that train_tc_supported accepts, 256
 // samples included, take the per-layer tensor-core path.
 bool train_fused_supported(const mipnerf_b200_config* c, int precision) {
-  return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_FP16) && mipnerf::tc_supported(c, precision) &&
+  return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_FP16 || precision == MIPNERF_B200_BF16X3) &&
+         mipnerf::tc_supported(c, precision) &&
          c->num_samples == 128 &&
          mipnerf::tc_default_degrees(c) &&  // the backward's tile images carry the full 96 / 27 encodings
          c->num_levels <= 2 && c->net_depth == 8;
@@ -547,17 +554,32 @@ cudaError_t launch_grad_source(const GradSource& g, const mipnerf_b200_config* c
 }
 }  // namespace
 
-size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_rays) {
+size_t mipnerf_b200_train_workspace_bytes_for(const mipnerf_b200_config* cfg, int64_t num_rays, int precision) {
   Dims d;
   if (check_config(cfg, &d) != MIPNERF_B200_OK || check_train_config(cfg) != MIPNERF_B200_OK || num_rays < 0)
     return 0;
+  if (precision == MIPNERF_B200_BF16X3) {  // the fused step only, in chunks of kChunkRaysX3
+    if (!train_fused_supported(cfg, precision)) return 0;
+    const int64_t r = num_rays < kChunkRaysX3 ? num_rays : kChunkRaysX3;
+    return carve_fused(cfg, d, r > 0 ? r : 1, precision, nullptr).bytes;
+  }
+  if (precision != MIPNERF_B200_FP32 && precision != MIPNERF_B200_BF16 && precision != MIPNERF_B200_FP16) return 0;
   const int64_t r = num_rays < kChunkRaysFp32 ? num_rays : kChunkRaysFp32;
   size_t bytes = carve_train(cfg, d, r > 0 ? r : 1, nullptr).bytes;
-  for (int precision : {MIPNERF_B200_BF16, MIPNERF_B200_FP16})  // the fused tensor-core step overlays the same buffer
-    if (train_fused_supported(cfg, precision)) {
-      const size_t f = carve_fused(cfg, d, r > 0 ? r : 1, precision, nullptr).bytes;
-      if (f > bytes) bytes = f;
-    }
+  if (train_fused_supported(cfg, precision)) {  // the fused tensor-core step overlays the same buffer
+    const size_t f = carve_fused(cfg, d, r > 0 ? r : 1, precision, nullptr).bytes;
+    if (f > bytes) bytes = f;
+  }
+  return bytes;
+}
+
+// one size for every non-split precision (what callers allocated before the split step existed)
+size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_rays) {
+  size_t bytes = 0;
+  for (int precision : {MIPNERF_B200_FP32, MIPNERF_B200_BF16, MIPNERF_B200_FP16}) {
+    const size_t b = mipnerf_b200_train_workspace_bytes_for(cfg, num_rays, precision);
+    if (b > bytes) bytes = b;
+  }
   return bytes;
 }
 
@@ -570,19 +592,32 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
   const int n = cfg->num_samples, depth = cfg->net_depth, W = cfg->net_width, Wc = cfg->net_width_condition;
   const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
   const int64_t B = rays->num_rays;
-  const FusedScratch s0 = carve_fused(cfg, d, B < kChunkRaysFp32 ? B : kChunkRaysFp32, precision, workspace);
+  // bf16x3: every operand of the backward is a pair of bf16 tile images, hi and lo (the 16-bit launchers' format
+  // argument is then bf16, and the *_lo arguments select their split kernels)
+  const bool x3 = precision == MIPNERF_B200_BF16X3;
+  const int fmt = x3 ? MIPNERF_B200_BF16 : precision;
+  const int64_t chunk = x3 ? kChunkRaysX3 : kChunkRaysFp32;
+  const FusedScratch s0 = carve_fused(cfg, d, B < chunk ? B : chunk, precision, workspace);
   // ---- once per call (the weights change every optimiser step): the level kernels' packed image, and the
   //      transposed B operands of the dgrad chain  bwd[i] = W_i[:, :256]^T  (slots depth / depth+1: bottleneck, view)
   mipnerf_b200_weights wl = *w;
   wl.packed = s0.packed;
   CUDA_TRY(mipnerf::tc_pack_weights(cfg, w, precision, s0.packed, st));
   const uint8_t* img_bwd[kMaxTrainDepth + 2] = {nullptr};
+  const uint8_t* img_bwd_lo[kMaxTrainDepth + 2] = {nullptr};  // bf16x3: slot + kMaxTrainDepth + 2
   {
     int slot = 0;
     auto pack = [&](const mipnerf_b200_linear& l, int nn, int kk, const uint8_t** out) {
-      uint8_t* dst = s0.images + (size_t)(slot++) * kTrainImageBytes;
+      uint8_t* dst = s0.images + (size_t)slot * kTrainImageBytes;
       *out = dst;
-      return mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, dst, nn, kk, precision, st);
+      if (x3) {
+        uint8_t* lo = s0.images + (size_t)(slot + kMaxTrainDepth + 2) * kTrainImageBytes;
+        img_bwd_lo[out - img_bwd] = lo;
+        cudaError_t e = mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, lo, nn, kk, fmt, st, 1);
+        if (e != cudaSuccess) return e;
+      }
+      ++slot;
+      return mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, dst, nn, kk, fmt, st);
     };
     for (int i = 1; i < depth; ++i) CUDA_TRY(pack(w->linears[i], W, W, &img_bwd[i]));
     CUDA_TRY(pack(w->linears[depth + 1], W, W, &img_bwd[depth]));
@@ -595,11 +630,15 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
   // scaled by 2^10 (it is bounded by 2/3 per sample: no overflow), every gradient tile image carries that factor, and
   // the fixed-order reduction of the wgrad partials takes it out again.  bf16 has fp32's range: scale 1.
   const float gscale = precision == MIPNERF_B200_FP16 ? 1024.f : 1.f, inv_gscale = 1.f / gscale;
-  for (int64_t off = 0; off < B; off += kChunkRaysFp32) {
-    const int64_t cnt = (B - off) < kChunkRaysFp32 ? (B - off) : kChunkRaysFp32;
+  for (int64_t off = 0; off < B; off += chunk) {
+    const int64_t cnt = (B - off) < chunk ? (B - off) : chunk;
     const int64_t m = cnt * n;
     const mipnerf_b200_rays rc_ = offset_rays(*rays, off, cnt);
     const FusedScratch s = carve_fused(cfg, d, cnt, precision, workspace);
+    // bf16x3: the lo image behind a hi image of `bytes_per_ray` bytes per ray (null in the 16-bit step)
+    auto lo_img = [&](const uint8_t* hi, size_t bytes_per_ray) {
+      return x3 ? const_cast<uint8_t*>(hi) + (size_t)cnt * bytes_per_ray : nullptr;
+    };
     CUDA_TRY(mipnerf::launch_pos_enc(rc_.viewdirs, s.venc, cnt, 0, cfg->deg_view, 1, st));
     // ---- forward of all levels: two launches, everything the backward needs is left behind as tile images
     mipnerf_b200_level_out lo[2];
@@ -623,57 +662,74 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
     // MIPNERF_B200_TRAIN_MASKBITS=0: the dgrad GEMMs read the ReLU mask from the activation tile images again (A/B)
     const char* bits_env = getenv("MIPNERF_B200_TRAIN_MASKBITS");
     const bool use_bits = !(bits_env && bits_env[0] == '0');
+    // dy16_lo / x1_lo / x2_lo: bf16x3's lo images (null otherwise)
     auto wgrad = [&](int idx, const void* dy16, const void* x1, int k1, const void* x2, int x2_t16, int k2, int div,
-                     bool emit_mask = false) {
+                     bool emit_mask, const void* dy16_lo, const void* x1_lo, const void* x2_lo) {
       const mipnerf_b200_linear& l = w->linears[idx];
       int slices = 0;
       cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy16, 1, l.out_features, x1, 1, k1, k1, x2, x2_t16, k2, k2, div,
-                                                         s.part, m, mipnerf::kWgradMaxSlices, precision, &slices, st,
-                                                         emit_mask && use_bits ? s.relu_bits : nullptr);
+                                                         s.part, m, mipnerf::kWgradMaxSlices, fmt, &slices, st,
+                                                         emit_mask && use_bits ? s.relu_bits : nullptr, dy16_lo, x1_lo,
+                                                         x2_lo);
       if (e2 != cudaSuccess) return e2;
       e2 = mipnerf::launch_wgrad_reduce(s.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
                                         grads[idx].bias_grad, touched[idx] ? 1 : 0, st, inv_gscale);
       touched[idx] = true;
       return e2;
     };
+    // y = [mask] (x . B^T + r1 r1w) on tile images, in bf16x3 on the hi / lo pairs
+    // (act: the layer input whose ReLU masks the output, read as the sign bits the preceding wgrad left behind, or
+    // null for no mask)
+    auto dgrad = [&](const uint8_t* xi, int slot, uint8_t* y, int nn, int kk, const float* r1, const float* r1w,
+                     const uint8_t* act_in) {
+      const void* mask = act_in && !use_bits ? act_in : nullptr;
+      const void* bits = act_in && use_bits ? s.relu_bits : nullptr;
+      if (x3)
+        return mipnerf::launch_linear_t16_x3(xi, lo_img(xi, (size_t)kk * 256), img_bwd[slot], img_bwd_lo[slot], y,
+                                             lo_img(y, (size_t)nn * 256), m, nn, kk, r1, r1w, mask, st, bits);
+      return mipnerf::launch_linear_t16(xi, img_bwd[slot], y, m, nn, kk, r1, r1w, mask, fmt, st, bits);
+    };
     for (int l = 0; l < cfg->num_levels; ++l) {
       const float* t_cur = lo[l].t_samples;
       const uint8_t* act = s.act[l];
       auto h16 = [&](int i) { return act + (size_t)i * cnt * 65536; };  // h_0..h_7, 8 = bottleneck
+      auto h16_lo = [&](int i) { return x3 ? h16(9 + i) : nullptr; };
       // the IPE features again (operand of two wgrads; the level kernel keeps its own 16-bit copy on chip), written
       // straight into a tile image so that those wgrads stage them by bulk copy like every other operand
+      uint8_t* enc16_lo = lo_img(s.enc16, 32768);
       CUDA_TRY(mipnerf::launch_ipe_t16(rc_.origins, rc_.directions, rc_.radii, t_cur, s.enc16, cnt, n,
-                                       cfg->disable_integration, precision, st));
+                                       cfg->disable_integration, fmt, st, enc16_lo));
       CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb[l], s.raw_density[l], t_cur, rc_.directions,
                                   white_bkgd, rgb_scale, gscale, s.d_raw_rgb, s.d_raw_density, st));
       // colour head, view layer                                          (models/mip_nerf.py:106-110)
       CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(s.d_raw_rgb, 3, s.v[l], Wc, s.part, grads[d.n_lin - 1].weight_grad,
                                                  grads[d.n_lin - 1].bias_grad, touched[d.n_lin - 1] ? 1 : 0, m,
-                                                 precision, st, inv_gscale));
+                                                 fmt, st, inv_gscale, lo_img(s.v[l], 32768)));
       touched[d.n_lin - 1] = true;
-      CUDA_TRY(mipnerf::launch_color_dgrad_t16(s.d_raw_rgb, cl.weight, s.v[l], s.d_v, m, Wc, precision, st));
-      CUDA_TRY(wgrad(depth + 2, s.d_v, h16(8), W, s.venc, 0, d.view_dim, n));
-      CUDA_TRY(mipnerf::launch_linear_t16(s.d_v, img_bwd[depth + 1], s.d_a, m, W, Wc, nullptr, nullptr, nullptr,
-                                          precision, st));
+      CUDA_TRY(mipnerf::launch_color_dgrad_t16(s.d_raw_rgb, cl.weight, s.v[l], s.d_v, m, Wc, fmt, st,
+                                               lo_img(s.d_v, 32768)));
+      CUDA_TRY(wgrad(depth + 2, s.d_v, h16(8), W, s.venc, 0, d.view_dim, n, false, lo_img(s.d_v, 32768), h16_lo(8),
+                     nullptr));
+      CUDA_TRY(dgrad(s.d_v, depth + 1, s.d_a, W, Wc, nullptr, nullptr, nullptr));
       // bottleneck + density head share h_7                              (models/mip_nerf.py:98-101)
-      CUDA_TRY(wgrad(depth + 1, s.d_a, h16(depth - 1), W, nullptr, 0, 0, 1, /*emit_mask=*/true));  // sign mask of h_7
+      CUDA_TRY(wgrad(depth + 1, s.d_a, h16(depth - 1), W, nullptr, 0, 0, 1, /*emit_mask=*/true, lo_img(s.d_a, 65536),
+                     h16_lo(depth - 1), nullptr));  // sign mask of h_7
       CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(s.d_raw_density, 1, h16(depth - 1), W, s.part,
                                                  grads[depth].weight_grad, grads[depth].bias_grad,
-                                                 touched[depth] ? 1 : 0, m, precision, st, inv_gscale));
+                                                 touched[depth] ? 1 : 0, m, fmt, st, inv_gscale, h16_lo(depth - 1)));
       touched[depth] = true;
-      CUDA_TRY(mipnerf::launch_linear_t16(s.d_a, img_bwd[depth], s.d_b, m, W, W, s.d_raw_density, dl.weight,
-                                          use_bits ? nullptr : h16(depth - 1), precision, st,
-                                          use_bits ? s.relu_bits : nullptr));
+      CUDA_TRY(dgrad(s.d_a, depth, s.d_b, W, W, s.d_raw_density, dl.weight, h16(depth - 1)));
       // trunk                                                            (models/mip_nerf.py:93-97)
       uint8_t *cur = s.d_b, *other = s.d_a;
       for (int i = depth - 1; i >= 0; --i) {
         const bool skip = takes_skip(cfg, i);
-        if (i == 0) CUDA_TRY(wgrad(0, cur, s.enc16, d.xyz_dim, nullptr, 0, 0, 1));
-        else CUDA_TRY(wgrad(i, cur, h16(i - 1), W, skip ? s.enc16 : nullptr, 1, skip ? d.xyz_dim : 0, 1, true));
+        if (i == 0)
+          CUDA_TRY(wgrad(0, cur, s.enc16, d.xyz_dim, nullptr, 0, 0, 1, false, lo_img(cur, 65536), enc16_lo, nullptr));
+        else
+          CUDA_TRY(wgrad(i, cur, h16(i - 1), W, skip ? s.enc16 : nullptr, 1, skip ? d.xyz_dim : 0, 1, true,
+                         lo_img(cur, 65536), h16_lo(i - 1), skip ? enc16_lo : nullptr));
         if (i > 0) {  // the wgrad just streamed h_{i-1} and left its sign mask behind: 32 B per row instead of 512
-          CUDA_TRY(mipnerf::launch_linear_t16(cur, img_bwd[i], other, m, W, W, nullptr, nullptr,
-                                              use_bits ? nullptr : h16(i - 1), precision, st,
-                                              use_bits ? s.relu_bits : nullptr));
+          CUDA_TRY(dgrad(cur, i, other, W, W, nullptr, nullptr, h16(i - 1)));
           uint8_t* tmp = cur;
           cur = other;
           other = tmp;
@@ -699,10 +755,13 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   if ((rc = check_train_config(cfg))) return rc;
   if ((rc = check_weights(cfg, d, w))) return rc;
   if ((rc = check_rays(rays))) return rc;
-  const bool tc = precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_FP16;
-  if (precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3)
+  const bool x3 = precision == MIPNERF_B200_BF16X3;
+  const bool tc = precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_FP16 || x3;
+  if (precision == MIPNERF_B200_FP16X3 || (x3 && (src.cots || !train_fused_supported(cfg, precision))))
     return fail(MIPNERF_B200_EUNSUPPORTED,
-                "training: the split-operand precisions are forward-only; use FP32 (parity) or BF16 / FP16");
+                "training: BF16X3 is the one split-operand training precision, for the fused training-loss step only "
+                "(8x256 / 1x128 MLP, default encodings, 128 samples, at most two levels; no backward from cotangents); "
+                "use FP32 (parity), BF16 or FP16");
   if (precision != MIPNERF_B200_FP32 && !tc) return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
   if (tc && !train_tc_supported(cfg, d))
     return fail(MIPNERF_B200_EUNSUPPORTED,
@@ -733,7 +792,8 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
     const int rcn = check_density_normals(cfg, randomized, rng, outs, rays->num_rays);
     if (rcn) return rcn;
   }
-  const size_t need = mipnerf_b200_train_workspace_bytes(cfg, rays->num_rays);
+  const size_t need = x3 ? mipnerf_b200_train_workspace_bytes_for(cfg, rays->num_rays, precision)
+                        : mipnerf_b200_train_workspace_bytes(cfg, rays->num_rays);
   if (rays->num_rays > 0 && (!workspace || workspace_bytes < need))
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
@@ -1002,6 +1062,87 @@ int mipnerf_b200_wgrad_tc(const float* dy, int n, const float* x1, int k1, const
                                              static_cast<float*>(scratch), m, mipnerf::kWgradMaxSlices, precision,
                                              &slices, st));
   CUDA_TRY(mipnerf::launch_wgrad_reduce(static_cast<float*>(scratch), slices, n, k1 + k2, dw, db, 0, st));
+  return MIPNERF_B200_OK;
+}
+
+// ---- the bf16x3 training step's GEMMs on their own (operands split into hi / lo tile images here) ----
+namespace {
+size_t t16_pair(int64_t m, int cols) { return align_up(2 * mipnerf::t16_image_bytes(m, cols)); }
+}  // namespace
+
+size_t mipnerf_b200_linear_x3_scratch_bytes(int64_t m, int n, int k) {
+  if (m < 0 || !(n == 128 || n == 256) || !(k == 128 || k == 256)) return 0;
+  return t16_pair(m, k) + t16_pair(m, n) + align_up(mipnerf::t16_image_bytes(m, n)) +
+         align_up(2 * mipnerf::linear_tc_image_bytes(n, k));
+}
+
+int mipnerf_b200_linear_x3(const float* x, const float* weight, const float* r1, const float* r1w, const float* mask,
+                           float* y, int64_t m, int n, int k, void* scratch, size_t scratch_bytes, void* stream) {
+  const size_t need = mipnerf_b200_linear_x3_scratch_bytes(m, n, k);
+  if (need == 0) return fail(MIPNERF_B200_EUNSUPPORTED, "linear_x3: n, k in {128,256} (got n=%d k=%d)", n, k);
+  if (m > 0 && (!x || !weight || !y || (r1 && !r1w))) return fail(MIPNERF_B200_EINVAL, "NULL tensor");
+  if (!scratch || scratch_bytes < need) return fail(MIPNERF_B200_EWORKSPACE, "scratch %zu < %zu bytes", scratch_bytes, need);
+  if (m == 0) return MIPNERF_B200_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* base = static_cast<uint8_t*>(scratch);
+  const size_t xi = mipnerf::t16_image_bytes(m, k), yi = mipnerf::t16_image_bytes(m, n);
+  uint8_t *xh = base, *yh = base + t16_pair(m, k), *mk = yh + t16_pair(m, n);
+  uint8_t* img = mk + align_up(yi);
+  const size_t ib = mipnerf::linear_tc_image_bytes(n, k);
+  const int64_t mp = (m + 127) / 128 * 128;  // the images are whole 128-row tiles (zero rows past m)
+  CUDA_TRY(mipnerf::launch_t16_pack(x, k, k, m, xh, MIPNERF_B200_BF16, st, xh + xi));
+  if (mask) CUDA_TRY(mipnerf::launch_t16_pack(mask, n, n, m, mk, MIPNERF_B200_BF16, st));
+  CUDA_TRY(mipnerf::launch_pack_linear_image(weight, k, 0, 0, img, n, k, MIPNERF_B200_BF16, st));
+  CUDA_TRY(mipnerf::launch_pack_linear_image(weight, k, 0, 0, img + ib, n, k, MIPNERF_B200_BF16, st, 1));
+  const float* r1p = r1;
+  if (r1 && mp != m) return fail(MIPNERF_B200_EINVAL, "linear_x3: r1 needs m a multiple of 128");
+  CUDA_TRY(mipnerf::launch_linear_t16_x3(xh, xh + xi, img, img + ib, yh, yh + yi, mp, n, k, r1p, r1w,
+                                         mask ? mk : nullptr, st));
+  CUDA_TRY(mipnerf::launch_t16_unpack(yh, n, y, n, m, MIPNERF_B200_BF16, st, yh + yi));
+  return MIPNERF_B200_OK;
+}
+
+size_t mipnerf_b200_wgrad_x3_scratch_bytes(int64_t m, int n, int k1, int k2, int x2_row_div) {
+  if (m < 0 || n < 1 || k1 < 1 || k2 < 0) return 0;
+  return align_up(mipnerf_b200_wgrad_tc_scratch_bytes(n, k1 + k2)) + t16_pair(m, n) + t16_pair(m, k1) +
+         (k2 > 0 && x2_row_div <= 1 ? t16_pair(m, k2) : 0);
+}
+
+int mipnerf_b200_wgrad_x3(const float* dy, int n, const float* x1, int k1, const float* x2, int k2, int x2_row_div,
+                          int64_t m, float* dw, float* db, void* scratch, size_t scratch_bytes, void* stream) {
+  if (m < 0 || k1 < 1 || k2 < 0 || !mipnerf::wgrad_tc_shape_ok(n))
+    return fail(MIPNERF_B200_EUNSUPPORTED, "wgrad_x3: n in {128,256} (got n=%d)", n);
+  if (k2 > 0 && k1 % 256 != 0)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "wgrad_x3: with x2, k1 must be a multiple of 256 (got k1=%d)", k1);
+  if (!dw || !db || (m > 0 && (!dy || !x1 || (k2 > 0 && !x2)))) return fail(MIPNERF_B200_EINVAL, "NULL tensor");
+  if (x2_row_div < 1) x2_row_div = 1;
+  const size_t need = mipnerf_b200_wgrad_x3_scratch_bytes(m, n, k1, k2, x2_row_div);
+  if (!scratch || scratch_bytes < need) return fail(MIPNERF_B200_EWORKSPACE, "scratch %zu < %zu bytes", scratch_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* base = static_cast<uint8_t*>(scratch);
+  float* part = reinterpret_cast<float*>(base);
+  uint8_t* dyh = base + align_up(mipnerf_b200_wgrad_tc_scratch_bytes(n, k1 + k2));
+  uint8_t* x1h = dyh + t16_pair(m, n);
+  uint8_t* x2h = x1h + t16_pair(m, k1);
+  const int64_t mp = (m + 127) / 128 * 128;  // zero rows past m add nothing
+  const bool x2_img = k2 > 0 && x2_row_div == 1;
+  if (x2_row_div > 1 && mp != m) return fail(MIPNERF_B200_EINVAL, "wgrad_x3: x2_row_div > 1 needs m a multiple of 128");
+  CUDA_TRY(mipnerf::launch_t16_pack(dy, n, n, m, dyh, MIPNERF_B200_BF16, st, dyh + mipnerf::t16_image_bytes(m, n)));
+  CUDA_TRY(mipnerf::launch_t16_pack(x1, k1, k1, m, x1h, MIPNERF_B200_BF16, st, x1h + mipnerf::t16_image_bytes(m, k1)));
+  if (x2_img)
+    CUDA_TRY(mipnerf::launch_t16_pack(x2, k2, k2, m, x2h, MIPNERF_B200_BF16, st, x2h + mipnerf::t16_image_bytes(m, k2)));
+  int slices = 0;
+  if (mp > 0) {
+    CUDA_TRY(mipnerf::launch_wgrad_mn_partials(
+        dyh, 1, n, x1h, 1, k1, k1, k2 > 0 ? (x2_img ? (const void*)x2h : (const void*)x2) : nullptr, x2_img ? 1 : 0, k2,
+        k2, x2_row_div, part, mp, mipnerf::kWgradMaxSlices, MIPNERF_B200_BF16, &slices, st, nullptr,
+        dyh + mipnerf::t16_image_bytes(m, n), x1h + mipnerf::t16_image_bytes(m, k1),
+        x2_img ? x2h + mipnerf::t16_image_bytes(m, k2) : nullptr));
+    CUDA_TRY(mipnerf::launch_wgrad_reduce(part, slices, n, k1 + k2, dw, db, 0, st));
+  } else {
+    CUDA_TRY(cudaMemsetAsync(dw, 0, sizeof(float) * n * (k1 + k2), st));
+    CUDA_TRY(cudaMemsetAsync(db, 0, sizeof(float) * n, st));
+  }
   return MIPNERF_B200_OK;
 }
 

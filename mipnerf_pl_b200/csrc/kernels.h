@@ -124,8 +124,9 @@ cudaError_t launch_adam_multi(const AdamMulti& t, float beta1, float beta2, floa
 size_t linear_tc_image_bytes(int n, int k);
 bool linear_tc_shape_ok(int n, int k);
 // B image of  W[:, off:off+k]  (transposed == 0, n rows)  or of  W[off:off+k, :n]^T  (transposed == 1)
+// lo != 0: the low halves fl16(w - fl16(w)) of the split precisions (the level kernel's lo stage image convention)
 cudaError_t launch_pack_linear_image(const float* w, int ldw, int off, int transposed, void* image, int n, int k,
-                                     int precision, cudaStream_t st);
+                                     int precision, cudaStream_t st, int lo = 0);
 // Y = [mask>0] * relu?( X[M,:k] . B^T + bias[col] + row_bias[row/row_div][col] + prev[row][col] + r1[row]*r1w[col] )
 cudaError_t launch_linear_tc(const float* x, int ldx, const void* image, float* y, int ldy, int64_t m, int n, int k,
                              const float* bias, const float* row_bias, int row_div, const float* prev,
@@ -136,28 +137,37 @@ bool wgrad_tc_shape_ok(int n_dim);
 cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, const void* x1, int x1_t16, int ld1, int k1,
                                      const void* x2, int x2_t16, int ld2, int k2, int x2_row_div, float* part,
                                      int64_t m, int max_slices, int precision, int* slices_out, cudaStream_t st,
-                                     void* mask_out = nullptr);
+                                     void* mask_out = nullptr, const void* dy_lo = nullptr,
+                                     const void* x1_lo = nullptr, const void* x2_lo = nullptr);
 // fixed-order reduction of [slices, n_dim, k_dim + 1] partials into dW / db (train_kernels.cu)
 cudaError_t launch_wgrad_reduce(const float* part, int slices, int n_dim, int k_dim, float* dw, float* db,
                                 int accumulate, cudaStream_t st, float scale = 1.f);
 
 // ---- train_t16.cu (backward pass on 16-bit tile images: [tile = 128 rows][64-column slab][128 rows x 128 B, SW128]) ----
+// The split (bf16x3) backward carries every operand as two such images, hi = fl16(x) and lo = fl16(x - hi): the `*_lo`
+// arguments below (null: the 16-bit path; non-null: bf16x3, precision must be 1 = bf16).
 size_t t16_image_bytes(int64_t rows, int cols);
-cudaError_t launch_t16_pack(const float* src, int ld, int cols, int64_t m, void* image, int precision, cudaStream_t st);
+cudaError_t launch_t16_pack(const float* src, int ld, int cols, int64_t m, void* image, int precision, cudaStream_t st,
+                            void* image_lo = nullptr);
 cudaError_t launch_ipe_t16(const float* origins, const float* directions, const float* radii, const float* t, void* image,
-                           int64_t num_rays, int n, int disable_integration, int precision, cudaStream_t st);
+                           int64_t num_rays, int n, int disable_integration, int precision, cudaStream_t st,
+                           void* image_lo = nullptr);
+// image_lo: dst = hi + lo
 cudaError_t launch_t16_unpack(const void* image, int cols, float* dst, int ld, int64_t m, int precision,
-                              cudaStream_t st);
+                              cudaStream_t st, const void* image_lo = nullptr);
 // mask: a tile image like y (zero where mask <= 0), or mask_bits: [m][32 B] sign bits of a 256-column image
 // (wgrad_mn_kernel's by-product); at most one of them
 cudaError_t launch_linear_t16(const void* x, const void* image, void* y, int64_t m, int n, int k, const float* r1,
                               const float* r1w, const void* mask, int precision, cudaStream_t st,
                               const void* mask_bits = nullptr);
+cudaError_t launch_linear_t16_x3(const void* x, const void* x_lo, const void* image, const void* image_lo, void* y,
+                                 void* y_lo, int64_t m, int n, int k, const float* r1, const float* r1w,
+                                 const void* mask, cudaStream_t st, const void* mask_bits = nullptr);
 cudaError_t launch_color_dgrad_t16(const float* d_rgb, const float* wc, const void* v, void* d_v, int64_t m, int k_dim,
-                                   int precision, cudaStream_t st);
+                                   int precision, cudaStream_t st, void* d_v_lo = nullptr);
 cudaError_t launch_wgrad_small_n_t16(const float* dy, int n_dim, const void* x, int k_dim, float* part, float* dw,
                                      float* db, int accumulate, int64_t m, int precision, cudaStream_t st,
-                                     float scale = 1.f);
+                                     float scale = 1.f, const void* x_lo = nullptr);
 
 // ---- mlp_tc.cu ----
 // out[ray][n] = b[n] + W[n, in_main : in_main + view_dim] . venc[ray]   (view-direction part of the view layer)

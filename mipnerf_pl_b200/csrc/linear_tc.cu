@@ -23,9 +23,10 @@ using namespace tc;
 // B[n][k] = w[n * ldw + col0 + k]            (transposed == 0: forward, rows of W, columns col0.. of its input dim)
 //         = w[(row0 + k) * ldw + n]          (transposed == 1: dgrad, B = W[row0.., :n_dim]^T)
 // written as slabs of [n rows x 128 B] in the 128-byte-swizzle K-major layout, zero padded to whole slabs.
+// lo != 0: fl16(v - fl16(v)), the low half of the split precisions
 template <int kFmt>
 __global__ void pack_linear_image_kernel(const float* __restrict__ w, int ldw, int off, int transposed,
-                                         uint8_t* __restrict__ image, int n, int k) {
+                                         uint8_t* __restrict__ image, int n, int k, int lo) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int slabs = (k + 63) / 64;
   if (idx >= n * slabs * 64) return;
@@ -33,6 +34,7 @@ __global__ void pack_linear_image_kernel(const float* __restrict__ w, int ldw, i
   const int kk = idx % (slabs * 64);
   float v = 0.f;
   if (kk < k) v = transposed ? w[(size_t)(off + kk) * ldw + row] : w[(size_t)row * ldw + off + kk];
+  if (lo) v -= from16<kFmt>(to16<kFmt>(v));
   uint16_t* dst = reinterpret_cast<uint16_t*>(image + (size_t)(kk / 64) * n * 128 + sw128_offset(row, kk % 64));
   *dst = to16<kFmt>(v);
 }
@@ -194,6 +196,9 @@ struct WgradTcParams {
   // The dgrad GEMM that follows needs exactly this (the ReLU mask of the layer input) and then reads 32 bytes per row
   // instead of the 512-byte activation row again.
   uint8_t* mask_out;
+  // bf16x3: the lo images of the tile-image operands (dy, x1 and x2 when they are images); fp32 operands are split
+  // while staging.
+  const uint8_t *dy_lo, *x1_lo, *x2_lo;
 };
 
 constexpr int kWgStages = 3;
@@ -202,6 +207,10 @@ constexpr uint32_t kWgOperand = kWgSlab * 512; // 64 rows x 256 cols x 2 B
 constexpr uint32_t kWgStage = 2 * kWgOperand;
 constexpr uint32_t kWgBlock = kWgSlab * 128;   // one 64-column block of a slab
 constexpr int kWgK = 128;                      // output columns per CTA (the wgmma N)
+// bf16x3 keeps the three 64 KB stages and halves the slab instead: 32 rows of dY hi, X hi, dY lo and X lo per stage
+// (4 x 16 KB), so the ring stays 192 KB and as deep; the partial sums are added in the same fixed order either way.
+constexpr int kWgSlabX3 = 32;
+static_assert(4 * kWgSlabX3 * 512 == kWgStage, "a bf16x3 stage is as large as a 16-bit one");
 
 template <int kFmt>
 __device__ __forceinline__ float2 unpack16x2(uint32_t v) {
@@ -209,8 +218,26 @@ __device__ __forceinline__ float2 unpack16x2(uint32_t v) {
   return __half22float2(*reinterpret_cast<__half2*>(&v));
 }
 
+// eight fp32 values as hi = fl16(x) and lo = fl16(x - hi), 16 bytes each
 template <int kFmt>
+__device__ __forceinline__ void stage8_split(uint8_t* hi, uint8_t* lo, const float4 (&f)[2]) {
+  const float v[8] = {f[0].x, f[0].y, f[0].z, f[0].w, f[1].x, f[1].y, f[1].z, f[1].w};
+  uint32_t h[4], l[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    h[e] = pack2<kFmt>(v[2 * e], v[2 * e + 1]);
+    l[e] = pack2_low<kFmt>(v[2 * e], v[2 * e + 1], h[e]);
+  }
+  *reinterpret_cast<uint4*>(hi) = make_uint4(h[0], h[1], h[2], h[3]);
+  *reinterpret_cast<uint4*>(lo) = make_uint4(l[0], l[1], l[2], l[3]);
+}
+
+template <int kFmt, bool kX3 = false>
 __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p) {
+  // rows per slab, and the operand / 64-column block sizes of a slab; kX3 adds the lo operands kLo bytes behind the hi
+  // ones in the stage: [dY hi][X hi][dY lo][X lo]
+  constexpr int kWgSlab = kX3 ? kWgSlabX3 : ::mipnerf::kWgSlab;
+  constexpr uint32_t kWgOperand = kWgSlab * 512, kWgBlock = kWgSlab * 128, kLo = 2 * kWgOperand;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
@@ -261,8 +288,9 @@ __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p)
     if (lane == 0 && (a16 || b16)) {
       const uint8_t* dy16 = reinterpret_cast<const uint8_t*>(p.dy);
       const uint8_t* x16 = reinterpret_cast<const uint8_t*>(in_x1 ? p.x1 : p.x2);
+      const uint8_t* x16_lo = in_x1 ? p.x1_lo : p.x2_lo;
       const int x_slabs = ((in_x1 ? p.k1 : p.k2) + 63) >> 6;
-      const uint32_t bytes = (uint32_t)((a16 ? a_blocks : 0) + (b16 ? b_blocks : 0)) * kWgBlock;
+      const uint32_t bytes = (uint32_t)((a16 ? a_blocks : 0) + (b16 ? b_blocks : 0)) * kWgBlock * (kX3 ? 2u : 1u);
       // the operand tiles stream through once (0.5 GB per launch): evict-first, so that the 39 MB of partial sums this
       // launch writes are still in L2 when the reduction kernel reads them
       const uint64_t stream_policy = l2_policy_evict_first();
@@ -271,17 +299,21 @@ __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p)
         if (it >= kWgStages) mbar_wait(&empty[s], (uint32_t)(it / kWgStages - 1) & 1u);
         uint8_t* sa = ring + (size_t)s * kWgStage;
         uint8_t* sb = sa + kWgOperand;
-        const int64_t row0 = m_begin + (int64_t)it * kWgSlab;  // a multiple of 64: one half of a 128-row tile
-        const size_t tile = (size_t)(row0 >> 7), half = (size_t)((row0 >> 6) & 1) * kWgBlock;
+        const int64_t row0 = m_begin + (int64_t)it * kWgSlab;  // a multiple of the slab: a part of a 128-row tile
+        const size_t tile = (size_t)(row0 >> 7), half = (size_t)(row0 & 127) * 128;
         mbar_arrive_expect_tx(&full[s], bytes);
         if (a16)
-          for (int b = 0; b < a_blocks; ++b)
-            bulk_g2s_hint(sa + (size_t)b * kWgBlock, dy16 + (tile * a_blocks + b) * 16384 + half, kWgBlock, &full[s],
-                          stream_policy);
+          for (int b = 0; b < a_blocks; ++b) {
+            const size_t o = (tile * a_blocks + b) * 16384 + half;
+            bulk_g2s_hint(sa + (size_t)b * kWgBlock, dy16 + o, kWgBlock, &full[s], stream_policy);
+            if (kX3) bulk_g2s_hint(sa + kLo + (size_t)b * kWgBlock, p.dy_lo + o, kWgBlock, &full[s], stream_policy);
+          }
         if (b16)
-          for (int b = 0; b < b_blocks; ++b)
-            bulk_g2s_hint(sb + (size_t)b * kWgBlock, x16 + (tile * x_slabs + (xc0 >> 6) + b) * 16384 + half, kWgBlock,
-                          &full[s], stream_policy);
+          for (int b = 0; b < b_blocks; ++b) {
+            const size_t o = (tile * x_slabs + (xc0 >> 6) + b) * 16384 + half;
+            bulk_g2s_hint(sb + (size_t)b * kWgBlock, x16 + o, kWgBlock, &full[s], stream_policy);
+            if (kX3) bulk_g2s_hint(sb + kLo + (size_t)b * kWgBlock, x16_lo + o, kWgBlock, &full[s], stream_policy);
+          }
       }
     }
   } else {
@@ -314,7 +346,7 @@ __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p)
         xs0 = make_float4(t[0], t[1], t[2], t[3]), xs1 = make_float4(t[4], t[5], t[6], t[7]);
       }
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
+      for (int half = 0; half < kWgSlab / 32; ++half) {
         float4 fa[4][2], fb[4][2];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -348,14 +380,23 @@ __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p)
           if (a_on && !a16) {
             bs[0] += fa[i][0].x, bs[1] += fa[i][0].y, bs[2] += fa[i][0].z, bs[3] += fa[i][0].w;
             bs[4] += fa[i][1].x, bs[5] += fa[i][1].y, bs[6] += fa[i][1].z, bs[7] += fa[i][1].w;
+            if constexpr (kX3) {
+              stage8_split<kFmt>(sa + off, sa + kLo + off, fa[i]);
+            } else {
             *reinterpret_cast<uint4*>(sa + off) =
                 make_uint4(pack2<kFmt>(fa[i][0].x, fa[i][0].y), pack2<kFmt>(fa[i][0].z, fa[i][0].w),
                            pack2<kFmt>(fa[i][1].x, fa[i][1].y), pack2<kFmt>(fa[i][1].z, fa[i][1].w));
+            }
           }
-          if (b_on && !b16)
+          if (b_on && !b16) {
+            if constexpr (kX3) {
+              stage8_split<kFmt>(sb + off, sb + kLo + off, fb[i]);
+            } else {
             *reinterpret_cast<uint4*>(sb + off) =
                 make_uint4(pack2<kFmt>(fb[i][0].x, fb[i][0].y), pack2<kFmt>(fb[i][0].z, fb[i][0].w),
                            pack2<kFmt>(fb[i][1].x, fb[i][1].y), pack2<kFmt>(fb[i][1].z, fb[i][1].w));
+            }
+          }
         }
       }
       fence_proxy_async_smem();  // this thread's st.shared -> visible to the tensor core's (async-proxy) reads
@@ -371,9 +412,18 @@ __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p)
 #pragma unroll
         for (int j = 0; j < kWgSlab / 16; ++j) {  // 16 rows = two 8-row groups = 2 KB further into every block
           const uint64_t bd = gmma_desc(sb_u + j * 2048, kWgBlock, 1024, 1);
-          wgmma_m64n128k16<kFmt, 1, 1>(acc0, gmma_desc(sa_u + (2 * wg) * kWgBlock + j * 2048, kWgBlock, 1024, 1), bd, 1u);
-          wgmma_m64n128k16<kFmt, 1, 1>(acc1, gmma_desc(sa_u + (2 * wg + 1) * kWgBlock + j * 2048, kWgBlock, 1024, 1), bd,
-                                       1u);
+          const uint64_t ad0 = gmma_desc(sa_u + (2 * wg) * kWgBlock + j * 2048, kWgBlock, 1024, 1);
+          const uint64_t ad1 = gmma_desc(sa_u + (2 * wg + 1) * kWgBlock + j * 2048, kWgBlock, 1024, 1);
+          wgmma_m64n128k16<kFmt, 1, 1>(acc0, ad0, bd, 1u);
+          if (kX3) {  // dY_lo . X_hi + dY_hi . X_lo, the level kernel's order
+            wgmma_m64n128k16<kFmt, 1, 1>(acc0, ad0 + kLo / 16, bd, 1u);
+            wgmma_m64n128k16<kFmt, 1, 1>(acc0, ad0, bd + kLo / 16, 1u);
+          }
+          wgmma_m64n128k16<kFmt, 1, 1>(acc1, ad1, bd, 1u);
+          if (kX3) {
+            wgmma_m64n128k16<kFmt, 1, 1>(acc1, ad1 + kLo / 16, bd, 1u);
+            wgmma_m64n128k16<kFmt, 1, 1>(acc1, ad1, bd + kLo / 16, 1u);
+          }
         }
         wgmma_commit();
       }
@@ -382,7 +432,7 @@ __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p)
           const uint32_t mblk = (uint32_t)((lane - mlane0) >> 3) * kWgBlock;
           const int64_t m0r = m_begin + (int64_t)it * kWgSlab;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
+          for (int i = 0; i < kWgSlab / 8; ++i) {
             const int r = warp + 8 * i;
             const uint4 w = *reinterpret_cast<const uint4*>(sb + mblk + (uint32_t)r * 128u + ((chunk ^ (uint32_t)(r & 7)) << 4));
             const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
@@ -397,11 +447,19 @@ __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p)
         }
         if (bias_read && a_on) {
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
+          for (int i = 0; i < kWgSlab / 8; ++i) {
             const int r = warp + 8 * i;
-            const uint4 w = *reinterpret_cast<const uint4*>(sa + blk + (uint32_t)r * 128u + ((chunk ^ (uint32_t)(r & 7)) << 4));
-            const float2 f0 = unpack16x2<kFmt>(w.x), f1 = unpack16x2<kFmt>(w.y), f2 = unpack16x2<kFmt>(w.z),
-                         f3 = unpack16x2<kFmt>(w.w);
+            const uint32_t o = blk + (uint32_t)r * 128u + ((chunk ^ (uint32_t)(r & 7)) << 4);
+            const uint4 w = *reinterpret_cast<const uint4*>(sa + o);
+            float2 f0 = unpack16x2<kFmt>(w.x), f1 = unpack16x2<kFmt>(w.y), f2 = unpack16x2<kFmt>(w.z),
+                   f3 = unpack16x2<kFmt>(w.w);
+            if (kX3) {  // dY = hi + lo
+              const uint4 wl = *reinterpret_cast<const uint4*>(sa + kLo + o);
+              const float2 l0 = unpack16x2<kFmt>(wl.x), l1 = unpack16x2<kFmt>(wl.y), l2 = unpack16x2<kFmt>(wl.z),
+                           l3 = unpack16x2<kFmt>(wl.w);
+              f0.x += l0.x, f0.y += l0.y, f1.x += l1.x, f1.y += l1.y;
+              f2.x += l2.x, f2.y += l2.y, f3.x += l3.x, f3.y += l3.y;
+            }
             bs[0] += f0.x, bs[1] += f0.y, bs[2] += f1.x, bs[3] += f1.y;
             bs[4] += f2.x, bs[5] += f2.y, bs[6] += f3.x, bs[7] += f3.y;
           }
@@ -458,13 +516,13 @@ size_t linear_tc_image_bytes(int n, int k) { return (size_t)((k + 63) / 64) * n 
 bool linear_tc_shape_ok(int n, int k) { return (n == 128 || n == 256) && (k == 96 || k == 128 || k == 256); }
 
 cudaError_t launch_pack_linear_image(const float* w, int ldw, int off, int transposed, void* image, int n, int k,
-                                     int precision, cudaStream_t st) {
+                                     int precision, cudaStream_t st, int lo) {
   const int total = n * ((k + 63) / 64) * 64;
   LaunchScope scope(kKernPackWeights, st);
   if (precision == 1)
-    pack_linear_image_kernel<1><<<(total + 255) / 256, 256, 0, st>>>(w, ldw, off, transposed, (uint8_t*)image, n, k);
+    pack_linear_image_kernel<1><<<(total + 255) / 256, 256, 0, st>>>(w, ldw, off, transposed, (uint8_t*)image, n, k, lo);
   else
-    pack_linear_image_kernel<0><<<(total + 255) / 256, 256, 0, st>>>(w, ldw, off, transposed, (uint8_t*)image, n, k);
+    pack_linear_image_kernel<0><<<(total + 255) / 256, 256, 0, st>>>(w, ldw, off, transposed, (uint8_t*)image, n, k, lo);
   return cudaGetLastError();
 }
 
@@ -512,8 +570,12 @@ bool wgrad_tc_shape_ok(int n_dim) { return n_dim == 128 || n_dim == 256; }
 cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, const void* x1, int x1_t16, int ld1, int k1,
                                      const void* x2, int x2_t16, int ld2, int k2, int x2_row_div, float* part,
                                      int64_t m, int max_slices, int precision, int* slices_out, cudaStream_t st,
-                                     void* mask_out) {
-  if (!x2) x2 = x1, x2_t16 = x1_t16, ld2 = ld1, k2 = 0;
+                                     void* mask_out, const void* dy_lo, const void* x1_lo, const void* x2_lo) {
+  // bf16x3 (dy_lo given): dy and x1 are tile images with their lo images, x2 an image with its lo image or fp32
+  const bool x3 = dy_lo != nullptr;
+  if (x3 && (precision != 1 || !dy_t16 || !x1_t16 || !x1_lo || (x2 && x2_t16 && k2 > 0 && !x2_lo)))
+    return cudaErrorInvalidValue;
+  if (!x2) x2 = x1, x2_t16 = x1_t16, ld2 = ld1, k2 = 0, x2_lo = x1_lo;
   if (x2_row_div < 1) x2_row_div = 1;
   const int K = k1 + k2;
   if (!(k2 == 0 || k1 % 256 == 0) || !(n_dim == 128 || n_dim == 256)) return cudaErrorInvalidValue;
@@ -527,28 +589,34 @@ cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, cons
   const int fmt = precision == 1 ? 1 : 0;
   const int k_tiles = (K + kWgK - 1) / kWgK;
   int64_t slices = g_sms / k_tiles;  // one CTA per SM, one wave
-  const int64_t by_rows = (m + kWgSlab - 1) / kWgSlab;
+  const int slab = x3 ? kWgSlabX3 : kWgSlab;
+  const int64_t by_rows = (m + slab - 1) / slab;
   if (slices > by_rows) slices = by_rows;
   if (slices > max_slices) slices = max_slices;
   if (slices < 1) slices = 1;
   int64_t slice_rows = (m + slices - 1) / slices;
-  slice_rows = (slice_rows + kWgSlab - 1) / kWgSlab * kWgSlab;
-  static bool attr[2] = {false, false};
+  slice_rows = (slice_rows + slab - 1) / slab * slab;
+  static bool attr[3] = {false, false, false};
   const size_t smem = 1024 + (size_t)kWgStages * kWgStage + 8 * 256 * sizeof(float) + 128;
-  if (!attr[fmt]) {
-    cudaError_t e = fmt ? cudaFuncSetAttribute(wgrad_mn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                        : cudaFuncSetAttribute(wgrad_mn_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  const int variant = x3 ? 2 : fmt;
+  if (!attr[variant]) {
+    cudaError_t e = x3    ? cudaFuncSetAttribute(wgrad_mn_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                    : fmt ? cudaFuncSetAttribute(wgrad_mn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                          : cudaFuncSetAttribute(wgrad_mn_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    attr[fmt] = true;
+    attr[variant] = true;
   }
   WgradTcParams p{};
   p.dy = static_cast<const float*>(dy), p.n_dim = n_dim, p.x1 = static_cast<const float*>(x1), p.ld1 = ld1, p.k1 = k1;
   p.x2 = static_cast<const float*>(x2), p.ld2 = ld2, p.k2 = k2, p.x2_row_div = x2_row_div, p.part = part, p.m = m;
   p.slice_rows = slice_rows, p.dy_t16 = dy_t16, p.x1_t16 = x1_t16, p.x2_t16 = x2_t16;
   p.mask_out = (x1_t16 && k1 == 256) ? static_cast<uint8_t*>(mask_out) : nullptr;
+  p.dy_lo = static_cast<const uint8_t*>(dy_lo), p.x1_lo = static_cast<const uint8_t*>(x1_lo);
+  p.x2_lo = static_cast<const uint8_t*>(x2_lo);
   dim3 grid((unsigned)slices, (unsigned)k_tiles);
   LaunchScope scope(kKernWgradTc, st);
-  if (fmt) wgrad_mn_kernel<1><<<grid, 288, smem, st>>>(p);
+  if (x3) wgrad_mn_kernel<1, true><<<grid, 288, smem, st>>>(p);
+  else if (fmt) wgrad_mn_kernel<1><<<grid, 288, smem, st>>>(p);
   else wgrad_mn_kernel<0><<<grid, 288, smem, st>>>(p);
   *slices_out = (int)slices;
   return cudaGetLastError();

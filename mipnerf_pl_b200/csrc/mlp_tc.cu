@@ -1025,8 +1025,12 @@ __device__ __forceinline__ void level_radiance_out(const LevelParams& p, int64_t
 // ray i - 2 (in round i - 1 of their loop, with kT = 1 or 2 and one feature buffer or two), and the consumers arrive on
 // heads_full of a tile only after its view-layer epilogue has read the slot; the slot of ray i is written before the
 // feat_full arrive of its tile 0, which the consumers wait on before any tile of ray i.
-template <int kFmt, bool kX3, int kT, int kMode = kModeForward>
+// kTrain (bf16x3 / fp16x3 forward with the training dump only): the dump also carries the lo halves of the split
+// activation tiles, at act_dump + 9 dump_tiles 64 KB (same [9][dump_tiles] layout), and of the view-layer output, at
+// v_dump + dump_tiles 32 KB.  A compile-time flag, so that the inference instantiations carry none of it.
+template <int kFmt, bool kX3, int kT, int kMode = kModeForward, bool kTrain = false>
 __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParams p) {
+  static_assert(!kTrain || (kX3 && kT == 1 && kMode == kModeForward), "the split training forward: 128 samples");
   constexpr bool kDensity = kMode == kModeDensity;
   constexpr bool kQuery = kMode != kModeForward;  // density or radiance: 128 query points per tile, no dumps
   static_assert(!kQuery || kT == 1, "the query modes take one 128-point tile at a time");
@@ -1298,6 +1302,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             for (int k = 0; k < 4; ++k) {
               const uint32_t o = (uint32_t)k * kStageBytes + (uint32_t)wg * 8192u;
               bulk_s2g_hint(p.act_dump + ((size_t)l * p.dump_tiles + ray) * kABytes + o, sA + o, 8192u, dump_policy);
+              if constexpr (kTrain)
+                bulk_s2g_hint(p.act_dump + ((size_t)(9 + l) * p.dump_tiles + ray) * kABytes + o, sA + kABytes + o, 8192u,
+                              dump_policy);
             }
           }
           dump_pending = true;
@@ -1364,6 +1371,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
           *reinterpret_cast<uint32_t*>(vd + (c >> 6) * kStageBytes + sw128_offset(r0, c & 63)) = pack2<kFmt>(y[0], y[1]);
           *reinterpret_cast<uint32_t*>(vd + (c >> 6) * kStageBytes + sw128_offset(r0 + 8, c & 63)) =
               pack2<kFmt>(y[2], y[3]);
+          if constexpr (kTrain) {  // and its lo halves
+            uint8_t* vl = vd + (size_t)p.dump_tiles * (2 * kStageBytes);
+            *reinterpret_cast<uint32_t*>(vl + (c >> 6) * kStageBytes + sw128_offset(r0, c & 63)) =
+                pack2_low<kFmt>(y[0], y[1], pack2<kFmt>(y[0], y[1]));
+            *reinterpret_cast<uint32_t*>(vl + (c >> 6) * kStageBytes + sw128_offset(r0 + 8, c & 63)) =
+                pack2_low<kFmt>(y[2], y[3], pack2<kFmt>(y[2], y[3]));
+          }
         }
       }
     }
@@ -1582,9 +1596,9 @@ int num_sms() {
   return g_num_sms;
 }
 
-template <int kFmt, bool kX3, int kT, int kMode = kModeForward>
+template <int kFmt, bool kX3, int kT, int kMode = kModeForward, bool kTrain = false>
 cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
-  auto kern = mlp_level_kernel<kFmt, kX3, kT, kMode>;
+  auto kern = mlp_level_kernel<kFmt, kX3, kT, kMode, kTrain>;
   constexpr uint32_t smem = LevelLayout<kX3, kT>::kTotal;
   static bool attr_set = false;  // one flag per instantiation
   if (!attr_set) {
@@ -1817,7 +1831,11 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
       p.density_bias = c->density_bias, p.rgb_scale = rgb_scale, p.rgb_padding = c->rgb_padding;
       p.dnoise = density_noise_draws(c, randomized, outs[l].density_normal, rng, off, l, n);
       if (!outs[l].density_normal) p.dnoise.ray_base += ray_base;
-      e = launch_level(p, precision, n, st);
+      // the split precisions' training forward dumps the lo halves as well (kTrain); bf16x3 is the one that trains
+      if (dump && is_x3(precision))
+        e = fmt_of(precision) ? launch_level_t<1, true, 1, kModeForward, true>(p, st) : cudaErrorNotSupported;
+      else
+        e = launch_level(p, precision, n, st);
       if (e != cudaSuccess) return e;
       t_prev = t_cur;
       w_prev = w_cur;

@@ -250,6 +250,13 @@ __device__ __forceinline__ float from16(uint16_t h) {
   if (kFmt == 1) return __bfloat162float(*reinterpret_cast<__nv_bfloat16*>(&h));
   return __half2float(*reinterpret_cast<__half*>(&h));
 }
+// The low halves of a pair whose high halves are `hi` = pack2(lo_el, hi_el): fl16(x - fl16(x)), the second operand of the
+// split ("x3") precisions, as the level kernel rounds it
+template <int kFmt>
+__device__ __forceinline__ uint32_t pack2_low(float a, float b, uint32_t hi) {
+  const float fa = from16<kFmt>((uint16_t)(hi & 0xffffu)), fb = from16<kFmt>((uint16_t)(hi >> 16));
+  return pack2<kFmt>(a - fa, b - fb);
+}
 
 }  // namespace tc
 }  // namespace mipnerf

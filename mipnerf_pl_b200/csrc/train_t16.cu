@@ -126,11 +126,135 @@ __global__ void __launch_bounds__(256, 1) linear_t16_kernel(const LinearT16Param
   }
 }
 
-// d v[row][c] = [v[row][c] > 0] * sum_j d_rgb[row][j] * wc[j][c]      thread = (row, 8-column chunk), k_dim = 128
+// The split-operand (bf16x3) dgrad: x = x_hi + x_lo and B = B_hi + B_lo, each K-step x_hi.B_hi + x_lo.B_hi + x_hi.B_lo
+// into one fp32 accumulator (the level kernel's order; x_lo.B_lo, below 2^-16 relative, is dropped), the output written
+// as y_hi = fl16(y) and y_lo = fl16(y - y_hi).  Hi + lo copies of the layout above would take 384 KB, so a CTA owns one
+// 128-column N-half for good and keeps that half of B, hi and lo, resident: 2 x k/64 x 16 KB = 128 KB at k = 256.  A
+// streams per 64-wide K-slab, hi + lo = 32 KB, through a two-slot ring: 64 KB.  192 KB in all at n = k = 256 (plus the
+// 1 KB alignment slack and the mbarriers).  Warps 0-7 are the two wgmma warpgroups (rows 64 g ..), warp 8 issues the
+// bulk copies.
+struct LinearT16X3Params {
+  LinearT16Params hi;  // x, image, y: the hi images; mask / mask_bits / r1 as for linear_t16_kernel
+  const uint8_t* x_lo;
+  const uint8_t* image_lo;
+  uint8_t* y_lo;
+};
+
 template <int kFmt>
+__global__ void __launch_bounds__(288, 1) linear_t16_x3_kernel(const LinearT16X3Params q) {
+  const LinearT16Params& p = q.hi;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
+  const int slabs = p.k >> 6, halves = p.n >> 7;
+  uint8_t* sB = smem;                                       // [hi, lo][slabs][128 rows x 128 B]
+  uint8_t* sA = sB + (size_t)2 * slabs * kSlab;             // [2 slots][hi, lo][16 KB]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sA + 4 * kSlab);
+  uint64_t* bar_b = bars;
+  uint64_t* full = bars + 1;   // [2] producer (tx bytes) -> warpgroups
+  uint64_t* empty = bars + 3;  // [2] one arrive per warpgroup once its wgmmas have read the slot
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int nc = 128 * (int)(blockIdx.x % halves);
+  const int64_t tile0 = blockIdx.x / halves, tstep = gridDim.x / halves;
+  if (tid == 0) {
+    mbar_init(bar_b, 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 2);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (warp == 8) {
+    if (lane == 0) {
+      mbar_arrive_expect_tx(bar_b, (uint32_t)(2 * slabs) * kSlab);
+      for (int s = 0; s < slabs; ++s) {
+        const size_t src = ((size_t)s * p.n + nc) * 128;
+        bulk_g2s(sB + (size_t)s * kSlab, p.image + src, kSlab, bar_b);
+        bulk_g2s(sB + (size_t)(slabs + s) * kSlab, q.image_lo + src, kSlab, bar_b);
+      }
+      int it = 0;
+      for (int64_t tile = tile0; tile < p.tiles; tile += tstep)
+        for (int s = 0; s < slabs; ++s, ++it) {
+          const int b = it & 1;
+          if (it >= 2) mbar_wait(&empty[b], (uint32_t)((it >> 1) - 1) & 1u);
+          mbar_arrive_expect_tx(&full[b], 2 * kSlab);
+          const size_t src = ((size_t)tile * slabs + s) * kSlab;
+          bulk_g2s(sA + (size_t)(2 * b) * kSlab, p.x + src, kSlab, &full[b]);
+          bulk_g2s(sA + (size_t)(2 * b + 1) * kSlab, q.x_lo + src, kSlab, &full[b]);
+        }
+    }
+    return;
+  }
+  const int wg = warp >> 2, wq = warp & 3;
+  const bool leader = (tid & 127) == 0;
+  const int r_lo = 64 * wg + 16 * wq + (lane >> 2);
+  const int y_slabs = p.n >> 6;
+  const uint32_t a_u = smem_u32(sA) + (uint32_t)wg * 8192u, b_u = smem_u32(sB);
+  const uint32_t b_lo = (uint32_t)slabs * kSlab / 16u;  // descriptor offsets of the lo operands
+  constexpr uint32_t a_lo = kSlab / 16u;
+  mbar_wait(bar_b, 0);
+  int it = 0;
+  for (int64_t tile = tile0; tile < p.tiles; tile += tstep) {
+    float acc[64];
+    wgmma_fence_acc(acc);
+    for (int s = 0; s < slabs; ++s, ++it) {
+      const int b = it & 1;
+      mbar_wait(&full[b], (uint32_t)(it >> 1) & 1u);
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint64_t ad = make_sw128_desc(a_u + (uint32_t)(2 * b) * kSlab + 32u * j);
+        const uint64_t bd = make_sw128_desc(b_u + (uint32_t)s * kSlab + 32u * j);
+        wgmma_m64n128k16<kFmt>(acc, ad, bd, (s | j) ? 1u : 0u);
+        wgmma_m64n128k16<kFmt>(acc, ad + a_lo, bd, 1u);
+        wgmma_m64n128k16<kFmt>(acc, ad, bd + b_lo, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (leader) mbar_arrive(&empty[b]);
+    }
+    uint8_t* ytile = p.y + (size_t)tile * y_slabs * kSlab;
+    uint8_t* ltile = q.y_lo + (size_t)tile * y_slabs * kSlab;
+    const uint8_t* mtile = p.mask ? p.mask + (size_t)tile * y_slabs * kSlab : nullptr;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r_lo + 8 * h;
+      const float rv = p.r1 ? __ldg(p.r1 + tile * 128 + row) : 0.f;
+      const uint8_t* mb = p.mask_bits ? p.mask_bits + ((size_t)tile * 128 + row) * 32 : nullptr;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = nc + 8 * j + 2 * (lane & 3);
+        float o0 = acc[4 * j + 2 * h], o1 = acc[4 * j + 2 * h + 1];
+        if (p.r1) {
+          const float2 w = __ldg(reinterpret_cast<const float2*>(p.r1w + col));
+          o0 = fmaf(rv, w.x, o0), o1 = fmaf(rv, w.y, o1);
+        }
+        const uint32_t off = (uint32_t)(col >> 6) * kSlab + sw128_offset(row, col & 63);
+        if (mtile) {  // the hi image's sign: fl16(x) > 0 iff x > 0
+          const uint32_t mw = __ldg(reinterpret_cast<const uint32_t*>(mtile + off));
+          if (!((int16_t)(mw & 0xffffu) > 0)) o0 = 0.f;
+          if (!((int32_t)mw >= 0x00010000)) o1 = 0.f;
+        } else if (mb) {
+          const uint32_t byte = __ldg(mb + (col >> 3));
+          if (!((byte >> (col & 7)) & 1u)) o0 = 0.f;
+          if (!((byte >> ((col & 7) + 1)) & 1u)) o1 = 0.f;
+        }
+        const uint32_t hv = pack2<kFmt>(o0, o1);
+        *reinterpret_cast<uint32_t*>(ytile + off) = hv;
+        *reinterpret_cast<uint32_t*>(ltile + off) = pack2_low<kFmt>(o0, o1, hv);
+      }
+    }
+  }
+}
+
+// d v[row][c] = [v[row][c] > 0] * sum_j d_rgb[row][j] * wc[j][c]      thread = (row, 8-column chunk), k_dim = 128
+// kX3: v is the hi image (its sign is v's), d v goes out as hi and lo images
+template <int kFmt, bool kX3 = false>
 __global__ void color_dgrad_t16_kernel(const float* __restrict__ d_rgb, const float* __restrict__ wc,
                                        const uint8_t* __restrict__ v, uint8_t* __restrict__ d_v, int64_t m,
-                                       int k_dim) {
+                                       int k_dim, uint8_t* __restrict__ d_v_lo = nullptr) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int chunks = k_dim >> 3;
   if (idx >= m * chunks) return;
@@ -159,8 +283,19 @@ __global__ void color_dgrad_t16_kernel(const float* __restrict__ d_rgb, const fl
     if (!((int16_t)(mw[e] & 0xffffu) > 0)) o[2 * e] = 0.f;
     if (!((int32_t)mw[e] >= 0x00010000)) o[2 * e + 1] = 0.f;
   }
-  *reinterpret_cast<uint4*>(d_v + off) =
-      make_uint4(pack2<kFmt>(o[0], o[1]), pack2<kFmt>(o[2], o[3]), pack2<kFmt>(o[4], o[5]), pack2<kFmt>(o[6], o[7]));
+  if constexpr (kX3) {
+    uint32_t hv[4], lv[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      hv[e] = pack2<kFmt>(o[2 * e], o[2 * e + 1]);
+      lv[e] = pack2_low<kFmt>(o[2 * e], o[2 * e + 1], hv[e]);
+    }
+    *reinterpret_cast<uint4*>(d_v + off) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
+    *reinterpret_cast<uint4*>(d_v_lo + off) = make_uint4(lv[0], lv[1], lv[2], lv[3]);
+  } else {
+    *reinterpret_cast<uint4*>(d_v + off) =
+        make_uint4(pack2<kFmt>(o[0], o[1]), pack2<kFmt>(o[2], o[3]), pack2<kFmt>(o[4], o[5]), pack2<kFmt>(o[6], o[7]));
+  }
 }
 
 template <int kFmt>
@@ -174,10 +309,12 @@ __device__ __forceinline__ float t16_load(const uint8_t* base, int64_t row, int 
 // streaming pass.  A warp (k_dim = 256) or half-warp (128) owns a row at a time, each lane one 16-byte chunk (8 columns,
 // coalesced 512 / 256 B per row), eight rows in flight per lane; the dY values of the row are warp-uniform fp32 loads.
 // Lane partials are combined through shared memory in a fixed order; same partial layout as wgrad_small_n_kernel.
-template <int kFmt, int kN>
+// kX3: X = hi + lo (x_lo the lo image), the two halves summed in fp32.
+template <int kFmt, int kN, bool kX3 = false>
 __global__ void __launch_bounds__(256)
 wgrad_small_n_t16_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ x, int k_dim,
-                         float* __restrict__ part, int64_t m, int64_t slice_rows) {
+                         float* __restrict__ part, int64_t m, int64_t slice_rows,
+                         const uint8_t* __restrict__ x_lo = nullptr) {
   __shared__ float red[8][32][kN * 8 + 1];
   __shared__ float bred[16][kN];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -197,25 +334,31 @@ wgrad_small_n_t16_kernel(const float* __restrict__ dy, const uint8_t* __restrict
   const uint32_t ci = (uint32_t)chunk & 7u;
   const int step = 8 * rpw;
   for (int64_t row0 = m_begin + warp * rpw + sub; row0 < m_end; row0 += (int64_t)step * 8) {
-    uint4 xv[8];
+    uint4 xv[8], xl[8];
     float d[8][kN];
 #pragma unroll
     for (int u = 0; u < 8; ++u) {  // eight independent rows in flight
       const int64_t row = row0 + (int64_t)u * step;
       const bool ok = row < m_end;
       const int r = (int)(row & 127);
-      xv[u] = ok ? __ldg(reinterpret_cast<const uint4*>(x + (size_t)(row >> 7) * (cpr >> 3) * kSlab + slab_off +
-                                                        (uint32_t)r * 128u + ((ci ^ ((uint32_t)r & 7u)) << 4)))
-                 : make_uint4(0u, 0u, 0u, 0u);
+      const size_t xo = (size_t)(row >> 7) * (cpr >> 3) * kSlab + slab_off + (uint32_t)r * 128u +
+                        ((ci ^ ((uint32_t)r & 7u)) << 4);
+      xv[u] = ok ? __ldg(reinterpret_cast<const uint4*>(x + xo)) : make_uint4(0u, 0u, 0u, 0u);
+      if (kX3) xl[u] = ok ? __ldg(reinterpret_cast<const uint4*>(x_lo + xo)) : make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
       for (int j = 0; j < kN; ++j) d[u][j] = ok ? __ldg(dy + row * kN + j) : 0.f;
     }
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       const uint32_t w[4] = {xv[u].x, xv[u].y, xv[u].z, xv[u].w};
+      const uint32_t wl[4] = {kX3 ? xl[u].x : 0u, kX3 ? xl[u].y : 0u, kX3 ? xl[u].z : 0u, kX3 ? xl[u].w : 0u};
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float x0 = from16<kFmt>((uint16_t)(w[e] & 0xffffu)), x1 = from16<kFmt>((uint16_t)(w[e] >> 16));
+        float x0 = from16<kFmt>((uint16_t)(w[e] & 0xffffu)), x1 = from16<kFmt>((uint16_t)(w[e] >> 16));
+        if (kX3) {
+          x0 += from16<kFmt>((uint16_t)(wl[e] & 0xffffu));
+          x1 += from16<kFmt>((uint16_t)(wl[e] >> 16));
+        }
 #pragma unroll
         for (int j = 0; j < kN; ++j) {
           acc[j][2 * e] = fmaf(d[u][j], x0, acc[j][2 * e]);
@@ -258,23 +401,30 @@ wgrad_small_n_t16_kernel(const float* __restrict__ dy, const uint8_t* __restrict
 // (mlp_tc.cu: ipe_row_group), so these are bit for bit the features the forward multiplied with.  Thread = (sample row,
 // k): k < 6 computes the Gaussian once and the eight (degree, coordinate) pairs 8k..8k+7, i.e. sin chunk k and cos
 // chunk 6 + k; k = 6, 7 zero the padding chunks.
-template <int kFmt>
+// kX3: hi and lo images (out_lo), split as the split level kernel's feature tile (mlp_tc.cu: store8_split).
+template <int kFmt, bool kX3 = false>
 __global__ void __launch_bounds__(256) ipe_t16_kernel(const float* __restrict__ origins,
                                                       const float* __restrict__ directions,
                                                       const float* __restrict__ radii, const float* __restrict__ t,
                                                       uint8_t* __restrict__ out, int64_t num_rays, int n,
-                                                      int disable_integration) {
+                                                      int disable_integration, uint8_t* __restrict__ out_lo = nullptr) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= num_rays * n * 8) return;
   const int64_t p = idx >> 3;  // sample index = ray * n + j   (n = 128: tile = ray, row = j)
   const int k = (int)(idx & 7);
   const int r = (int)(p & 127);
-  uint8_t* tile = out + (size_t)(p >> 7) * (2 * kSlab) + (uint32_t)r * 128u;
+  const size_t tile_off = (size_t)(p >> 7) * (2 * kSlab) + (uint32_t)r * 128u;
+  uint8_t* tile = out + tile_off;
   const uint32_t rx = (uint32_t)r & 7u;
-  auto chunk_ptr = [&](int ch) { return tile + (size_t)(ch >> 3) * kSlab + ((((uint32_t)ch & 7u) ^ rx) << 4); };
+  auto chunk_off = [&](int ch) { return (size_t)(ch >> 3) * kSlab + ((((uint32_t)ch & 7u) ^ rx) << 4); };
+  auto chunk_ptr = [&](int ch) { return tile + chunk_off(ch); };
   if (k >= 6) {
     *reinterpret_cast<uint4*>(chunk_ptr(12 + 2 * (k - 6))) = make_uint4(0u, 0u, 0u, 0u);
     *reinterpret_cast<uint4*>(chunk_ptr(13 + 2 * (k - 6))) = make_uint4(0u, 0u, 0u, 0u);
+    if (kX3) {
+      *reinterpret_cast<uint4*>(out_lo + tile_off + chunk_off(12 + 2 * (k - 6))) = make_uint4(0u, 0u, 0u, 0u);
+      *reinterpret_cast<uint4*>(out_lo + tile_off + chunk_off(13 + 2 * (k - 6))) = make_uint4(0u, 0u, 0u, 0u);
+    }
     return;
   }
   const int64_t ray = p / n;
@@ -291,6 +441,21 @@ __global__ void __launch_bounds__(256) ipe_t16_kernel(const float* __restrict__ 
     const int f = k * 8 + e;  // feature index = degree * 3 + coord   (models/mip.py:335-341)
     ipe_pair<true>(mean[f % 3], cov[f % 3], f / 3, fs[e], fc[e]);
   }
+  if constexpr (kX3) {
+    auto split8 = [&](const float (&v)[8], size_t o) {
+      uint32_t hv[4], lv[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        hv[e] = pack2<kFmt>(v[2 * e], v[2 * e + 1]);
+        lv[e] = pack2_low<kFmt>(v[2 * e], v[2 * e + 1], hv[e]);
+      }
+      *reinterpret_cast<uint4*>(out + tile_off + o) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
+      *reinterpret_cast<uint4*>(out_lo + tile_off + o) = make_uint4(lv[0], lv[1], lv[2], lv[3]);
+    };
+    split8(fs, chunk_off(k));
+    split8(fc, chunk_off(6 + k));
+    return;
+  }
   *reinterpret_cast<uint4*>(chunk_ptr(k)) =
       make_uint4(pack2<kFmt>(fs[0], fs[1]), pack2<kFmt>(fs[2], fs[3]), pack2<kFmt>(fs[4], fs[5]), pack2<kFmt>(fs[6], fs[7]));
   *reinterpret_cast<uint4*>(chunk_ptr(6 + k)) =
@@ -301,7 +466,7 @@ __global__ void __launch_bounds__(256) ipe_t16_kernel(const float* __restrict__ 
 // thread = (row, 16-byte chunk of 8 columns): two float4 loads when the source allows it, one 16-byte store
 template <int kFmt>
 __global__ void t16_pack_kernel(const float* __restrict__ src, int ld, int cols, int64_t m, uint8_t* __restrict__ dst,
-                                int img_cols, int64_t padded_rows, int vec) {
+                                int img_cols, int64_t padded_rows, int vec, uint8_t* __restrict__ dst_lo) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int chunks = img_cols >> 3;
   if (idx >= padded_rows * chunks) return;
@@ -320,18 +485,28 @@ __global__ void t16_pack_kernel(const float* __restrict__ src, int ld, int cols,
     }
   }
   const int r = (int)(row & 127);
-  *reinterpret_cast<uint4*>(dst + ((size_t)(row >> 7) * (img_cols >> 6) + (ch >> 3)) * kSlab + (uint32_t)r * 128u +
-                            ((((uint32_t)ch & 7u) ^ ((uint32_t)r & 7u)) << 4)) =
-      make_uint4(pack2<kFmt>(v[0], v[1]), pack2<kFmt>(v[2], v[3]), pack2<kFmt>(v[4], v[5]), pack2<kFmt>(v[6], v[7]));
+  const size_t o = ((size_t)(row >> 7) * (img_cols >> 6) + (ch >> 3)) * kSlab + (uint32_t)r * 128u +
+                   ((((uint32_t)ch & 7u) ^ ((uint32_t)r & 7u)) << 4);
+  uint32_t hv[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) hv[e] = pack2<kFmt>(v[2 * e], v[2 * e + 1]);
+  *reinterpret_cast<uint4*>(dst + o) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
+  if (dst_lo)  // the split precisions' low halves
+    *reinterpret_cast<uint4*>(dst_lo + o) =
+        make_uint4(pack2_low<kFmt>(v[0], v[1], hv[0]), pack2_low<kFmt>(v[2], v[3], hv[1]),
+                   pack2_low<kFmt>(v[4], v[5], hv[2]), pack2_low<kFmt>(v[6], v[7], hv[3]));
 }
+// src_lo (or null): the lo image of a split pair, added in fp32
 template <int kFmt>
 __global__ void t16_unpack_kernel(const uint8_t* __restrict__ src, int img_cols, float* __restrict__ dst, int ld,
-                                  int cols, int64_t m) {
+                                  int cols, int64_t m, const uint8_t* __restrict__ src_lo) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= m * cols) return;
   const int64_t row = idx / cols;
   const int col = (int)(idx % cols);
-  dst[row * ld + col] = t16_load<kFmt>(src, row, col, img_cols);
+  float v = t16_load<kFmt>(src, row, col, img_cols);
+  if (src_lo) v += t16_load<kFmt>(src_lo, row, col, img_cols);
+  dst[row * ld + col] = v;
 }
 
 int g_sms_t16 = 0;
@@ -344,28 +519,33 @@ size_t t16_image_bytes(int64_t rows, int cols) {
 }
 
 cudaError_t launch_t16_pack(const float* src, int ld, int cols, int64_t m, void* image, int precision,
-                            cudaStream_t st) {
+                            cudaStream_t st, void* image_lo) {
   const int img_cols = (cols + 63) / 64 * 64;
   const int64_t padded = (m + 127) / 128 * 128;
   if (padded == 0) return cudaSuccess;
   LaunchScope scope(kKernIpe, st);  // accounted with the feature kernels (its use in the training step)
   const int vec = (ld & 3) == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
   const int64_t total = padded * (img_cols / 8);
+  uint8_t* lo = static_cast<uint8_t*>(image_lo);
   if (precision == 1)
-    t16_pack_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(src, ld, cols, m, (uint8_t*)image, img_cols, padded, vec);
+    t16_pack_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(src, ld, cols, m, (uint8_t*)image, img_cols, padded, vec, lo);
   else
-    t16_pack_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(src, ld, cols, m, (uint8_t*)image, img_cols, padded, vec);
+    t16_pack_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(src, ld, cols, m, (uint8_t*)image, img_cols, padded, vec, lo);
   return cudaGetLastError();
 }
 
 // min_deg = 0, max_deg = 16 (96 features), n = 128 samples per ray: the level kernels' shape
 cudaError_t launch_ipe_t16(const float* origins, const float* directions, const float* radii, const float* t, void* image,
-                           int64_t num_rays, int n, int disable_integration, int precision, cudaStream_t st) {
+                           int64_t num_rays, int n, int disable_integration, int precision, cudaStream_t st,
+                           void* image_lo) {
   if (num_rays == 0) return cudaSuccess;
-  if (n != 128) return cudaErrorInvalidValue;
+  if (n != 128 || (image_lo && precision != 1)) return cudaErrorInvalidValue;
   LaunchScope scope(kKernIpe, st);
   const int64_t total = num_rays * n * 8;
-  if (precision == 1)
+  if (image_lo)
+    ipe_t16_kernel<1, true><<<blocks_of(total, 256), 256, 0, st>>>(origins, directions, radii, t, (uint8_t*)image,
+                                                                    num_rays, n, disable_integration, (uint8_t*)image_lo);
+  else if (precision == 1)
     ipe_t16_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(origins, directions, radii, t, (uint8_t*)image, num_rays, n,
                                                               disable_integration);
   else
@@ -375,13 +555,14 @@ cudaError_t launch_ipe_t16(const float* origins, const float* directions, const 
 }
 
 cudaError_t launch_t16_unpack(const void* image, int cols, float* dst, int ld, int64_t m, int precision,
-                              cudaStream_t st) {
+                              cudaStream_t st, const void* image_lo) {
   const int img_cols = (cols + 63) / 64 * 64;
   if (m == 0) return cudaSuccess;
+  const uint8_t* lo = static_cast<const uint8_t*>(image_lo);
   if (precision == 1)
-    t16_unpack_kernel<1><<<blocks_of(m * cols, 256), 256, 0, st>>>((const uint8_t*)image, img_cols, dst, ld, cols, m);
+    t16_unpack_kernel<1><<<blocks_of(m * cols, 256), 256, 0, st>>>((const uint8_t*)image, img_cols, dst, ld, cols, m, lo);
   else
-    t16_unpack_kernel<0><<<blocks_of(m * cols, 256), 256, 0, st>>>((const uint8_t*)image, img_cols, dst, ld, cols, m);
+    t16_unpack_kernel<0><<<blocks_of(m * cols, 256), 256, 0, st>>>((const uint8_t*)image, img_cols, dst, ld, cols, m, lo);
   return cudaGetLastError();
 }
 
@@ -418,13 +599,51 @@ cudaError_t launch_linear_t16(const void* x, const void* image, void* y, int64_t
   return cudaGetLastError();
 }
 
-cudaError_t launch_color_dgrad_t16(const float* d_rgb, const float* wc, const void* v, void* d_v, int64_t m, int k_dim,
-                                   int precision, cudaStream_t st) {
+// the same in bf16x3: x, B and y as hi and lo images (linear_t16_x3_kernel)
+cudaError_t launch_linear_t16_x3(const void* x, const void* x_lo, const void* image, const void* image_lo, void* y,
+                                 void* y_lo, int64_t m, int n, int k, const float* r1, const float* r1w,
+                                 const void* mask, cudaStream_t st, const void* mask_bits) {
   if (m == 0) return cudaSuccess;
-  if (k_dim % 64 != 0) return cudaErrorInvalidValue;
+  if (m % 128 != 0 || !(n == 128 || n == 256) || !(k == 128 || k == 256)) return cudaErrorInvalidValue;
+  if (mask_bits && (mask || n != 256)) return cudaErrorInvalidValue;
+  const int slabs = k / 64, halves = n / 128;
+  const size_t smem = 1024 + (size_t)(2 * slabs + 4) * kSlab + 64;
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(linear_t16_x3_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)(1024 + (size_t)(2 * 4 + 4) * kSlab + 64));
+    if (e != cudaSuccess) return e;
+    attr = true;
+  }
+  if (g_sms_t16 == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&g_sms_t16, cudaDevAttrMultiProcessorCount, dev);
+  }
+  LinearT16X3Params q{};
+  LinearT16Params& p = q.hi;
+  p.x = static_cast<const uint8_t*>(x), p.image = static_cast<const uint8_t*>(image), p.y = static_cast<uint8_t*>(y);
+  p.mask_bits = static_cast<const uint8_t*>(mask_bits);
+  p.mask = static_cast<const uint8_t*>(mask), p.r1 = r1, p.r1w = r1w, p.tiles = m / 128, p.n = n, p.k = k;
+  q.x_lo = static_cast<const uint8_t*>(x_lo), q.image_lo = static_cast<const uint8_t*>(image_lo);
+  q.y_lo = static_cast<uint8_t*>(y_lo);
+  // a CTA keeps one N-half for good: the grid is a whole number of CTAs per half
+  const int64_t per_half = p.tiles < g_sms_t16 / halves ? p.tiles : g_sms_t16 / halves;
+  LaunchScope scope(kKernLinearTc, st);
+  linear_t16_x3_kernel<1><<<(unsigned)(per_half * halves), 288, smem, st>>>(q);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_color_dgrad_t16(const float* d_rgb, const float* wc, const void* v, void* d_v, int64_t m, int k_dim,
+                                   int precision, cudaStream_t st, void* d_v_lo) {
+  if (m == 0) return cudaSuccess;
+  if (k_dim % 64 != 0 || (d_v_lo && precision != 1)) return cudaErrorInvalidValue;
   LaunchScope scope(kKernDgrad, st);
   const int64_t total = m * (k_dim / 8);
-  if (precision == 1)
+  if (d_v_lo)
+    color_dgrad_t16_kernel<1, true><<<blocks_of(total, 256), 256, 0, st>>>(d_rgb, wc, (const uint8_t*)v, (uint8_t*)d_v, m,
+                                                                          k_dim, (uint8_t*)d_v_lo);
+  else if (precision == 1)
     color_dgrad_t16_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(d_rgb, wc, (const uint8_t*)v, (uint8_t*)d_v, m, k_dim);
   else
     color_dgrad_t16_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(d_rgb, wc, (const uint8_t*)v, (uint8_t*)d_v, m, k_dim);
@@ -435,9 +654,10 @@ cudaError_t launch_color_dgrad_t16(const float* d_rgb, const float* wc, const vo
 // fixed-order sum
 cudaError_t launch_wgrad_small_n_t16(const float* dy, int n_dim, const void* x, int k_dim, float* part, float* dw,
                                      float* db, int accumulate, int64_t m, int precision, cudaStream_t st,
-                                     float scale) {
+                                     float scale, const void* x_lo) {
   if (m == 0 || n_dim == 0) return cudaSuccess;
   if (!(n_dim == 1 || n_dim == 3) || !(k_dim == 128 || k_dim == 256)) return cudaErrorInvalidValue;
+  if (x_lo && precision != 1) return cudaErrorInvalidValue;
   if (g_sms_t16 == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
@@ -452,7 +672,10 @@ cudaError_t launch_wgrad_small_n_t16(const float* dy, int n_dim, const void* x, 
   {
     LaunchScope scope(kKernWgrad, st);
     const int fmt = precision == 1 ? 1 : 0;
-    if (fmt && n_dim == 1) wgrad_small_n_t16_kernel<1, 1><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);
+    const uint8_t* xl = static_cast<const uint8_t*>(x_lo);
+    if (xl && n_dim == 1) wgrad_small_n_t16_kernel<1, 1, true><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows, xl);
+    else if (xl) wgrad_small_n_t16_kernel<1, 3, true><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows, xl);
+    else if (fmt && n_dim == 1) wgrad_small_n_t16_kernel<1, 1><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);
     else if (fmt) wgrad_small_n_t16_kernel<1, 3><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);
     else if (n_dim == 1) wgrad_small_n_t16_kernel<0, 1><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);
     else wgrad_small_n_t16_kernel<0, 3><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);

@@ -191,7 +191,7 @@ def _run(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized: bool, white
          grad_tensors: Sequence[torch.Tensor], accumulate: bool, mask_sum, global_rays, density_normal=None):
     if not model.stop_resample_grad:
         raise NotImplementedError("training kernels implement stop_resample_grad=True (the reference default)")
-    prec = _cabi.PRECISIONS[model.precision]   # fp32: the parity mode; bf16 / fp16: forward + dgrad GEMMs on the tensor cores
+    prec = _cabi.PRECISIONS[model.precision]   # fp32: the parity mode; bf16 / fp16 / bf16x3: GEMMs on the tensor cores
     if model.ray_shape != "cone":
         raise NotImplementedError
     dev = _dev(rays.origins)
@@ -242,7 +242,8 @@ def _run(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized: bool, white
                                    _ptr(normals[lvl]))
         ret.append((comp, dist, acc, w, t))
     lib = _cabi.lib()
-    nbytes = lib.mipnerf_b200_train_workspace_bytes(C.byref(cfg), b)
+    nbytes = (lib.mipnerf_b200_train_workspace_bytes_for(C.byref(cfg), b, prec) if prec == _cabi.BF16X3
+              else lib.mipnerf_b200_train_workspace_bytes(C.byref(cfg), b))
     scratch = _Workspace.get(dev, nbytes)
     tail = (int(bool(white_bkgd)), prec, C.byref(loss), outs, garr, len(lins), int(bool(accumulate)),
             scratch.data_ptr() if nbytes else None, scratch.numel() if nbytes else 0, _stream(dev))

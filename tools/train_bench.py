@@ -30,7 +30,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rays", type=int, default=4096)
     ap.add_argument("--steps", type=int, default=10)
-    ap.add_argument("--precision", default="fp32", choices=["fp32", "bf16", "fp16"])
+    ap.add_argument("--precision", default="fp32", choices=["fp32", "bf16", "fp16", "bf16x3"])
     ap.add_argument("--autograd", action="store_true", help="time the autograd step against the fused step")
     ap.add_argument("--rounds", type=int, default=5, help="--autograd: alternations of the two steps")
     args = ap.parse_args()
