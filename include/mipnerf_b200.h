@@ -388,6 +388,39 @@ int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b2
                                 float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
                                 size_t workspace_bytes, void* stream);
 
+/* ---- gradients of field queries with respect to the MLP tensors ----
+ * Cotangents of one query's outputs; any pointer may be NULL (= zero). */
+typedef struct mipnerf_b200_query_cotangent {
+  const float* d_raw_rgb;      /* [P,3] */
+  const float* d_raw_density;  /* [P]   */
+  const float* d_rgb;          /* [P,3]  rgb = sigmoid(raw) (1 + 2 rgb_padding) - rgb_padding          */
+  const float* d_density;      /* [P]    density = softplus(raw + density_bias), torch's threshold 20  */
+} mipnerf_b200_query_cotangent;
+
+/* Workspace of mipnerf_b200_query_backward for a radiance (radiance != 0) or density query of num_points points: one
+ * chunk of at most 524288 points, so the size stops growing there.  0 where the backward refuses the config or
+ * precision. */
+size_t mipnerf_b200_query_backward_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points,
+                                                   int radiance, int precision);
+/* Gradients of L = <cot, outputs of query_radiance (viewdirs != NULL) or query_density (viewdirs == NULL)> w.r.t. the
+ * MLP tensors, into `grads` (same layout and accumulate semantics as mipnerf_b200_backward).  covs NULL or
+ * cfg->disable_integration: zero covariance; no density noise.  The means, covs and viewdirs carry no gradient.  A
+ * density query reads only d_raw_density and d_density, and writes exact zeros to the bottleneck, view-layer and
+ * colour-head gradients (leaves them untouched when `accumulate` is set).
+ * BF16 runs the query again on the level kernel's query mode with the training dump (the outputs and 16-bit activation
+ * tiles are the forward query's own, bit for bit), then the fused training step's tile-image backward chain; it takes
+ * the default architecture and encodings.  FP32 re-evaluates the query with its fp32 activations kept (the IPE stage
+ * kernel, pos_enc, the fp32 MLP, the same values as the fp32 query) and runs the per-layer fp32 chain; it takes the
+ * configs mipnerf_b200_backward takes.  FP16 (its fixed gradient scale is sized for the training loss), the split
+ * precisions (forward-only here) and other configs: MIPNERF_B200_EUNSUPPORTED.  Points run in chunks of 524288 and the
+ * wgrad partials are reduced in a fixed order: the gradients are bit-reproducible, though a query split into two calls
+ * sums in a different order. */
+int mipnerf_b200_query_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
+                                const float* means, const float* covs, const float* viewdirs, int64_t num_points,
+                                int precision, const mipnerf_b200_query_cotangent* cot,
+                                const mipnerf_b200_linear_grad* grads, int num_grads, int accumulate,
+                                void* workspace, size_t workspace_bytes, void* stream);
+
 /* Isosurface of a scalar grid [nz, ny, nx] fp32 (x fastest, every dimension >= 2) by marching tetrahedra (6 Kuhn
  * tetrahedra per cell): a watertight indexed mesh whose normals point from inside (value > iso; NaN is outside) to
  * outside.  Pass 1 writes counts[2] (device int64: vertices, faces); pass 2, with the same scratch, writes verts [V,3]

@@ -75,6 +75,11 @@ class LevelCotangent(C.Structure):
                 ("d_weights", C.c_void_p)]
 
 
+class QueryCotangent(C.Structure):
+    _fields_ = [("d_raw_rgb", C.c_void_p), ("d_raw_density", C.c_void_p), ("d_rgb", C.c_void_p),
+                ("d_density", C.c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/mipnerf_b200.h declares.
 _V = C.c_void_p
 _SIGNATURES = {
@@ -137,6 +142,10 @@ _SIGNATURES = {
     "mipnerf_b200_radiance_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int]),
     "mipnerf_b200_query_radiance": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), _V, _V, _V, C.c_int64, C.c_int,
                                               _V, _V, _V, _V, _V, C.c_size_t, _V]),
+    "mipnerf_b200_query_backward_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int, C.c_int]),
+    "mipnerf_b200_query_backward": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), _V, _V, _V, C.c_int64, C.c_int,
+                                              C.POINTER(QueryCotangent), C.POINTER(LinearGrad), C.c_int, C.c_int, _V,
+                                              C.c_size_t, _V]),
     "mipnerf_b200_isosurface_normals": (C.c_int, [_V, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.c_float, _V, _V,
                                                   _V]),
     "mipnerf_b200_isosurface_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),

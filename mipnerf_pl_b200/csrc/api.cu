@@ -522,6 +522,162 @@ inline bool takes_skip(const mipnerf_b200_config* c, int layer) {  // models/mip
   return layer > 1 && (layer - 1) % c->skip_index == 0;
 }
 
+// B operands of the per-layer tensor-core GEMMs, packed once per call (the weights change every optimiser step) into
+// kTrainImageBytes slots at `base`.  fwd[i] = W_i[:, :k_main], skip[i] = W_i[:, 256:352], bwd[i] = W_i[:, :256]^T;
+// slots depth / depth+1 hold the bottleneck and the view layer.
+struct LayerImages {
+  const uint8_t *fwd[kMaxTrainDepth + 2], *skip[kMaxTrainDepth], *bwd[kMaxTrainDepth + 2];
+};
+
+cudaError_t pack_layer_images(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w, int precision,
+                              uint8_t* base, LayerImages* im, cudaStream_t st) {
+  const int depth = c->net_depth, W = c->net_width, Wc = c->net_width_condition;
+  *im = LayerImages{};
+  int slot = 0;
+  auto pack = [&](const mipnerf_b200_linear& l, int off, int transposed, int nn, int kk, const uint8_t** out) {
+    uint8_t* dst = base + (size_t)(slot++) * kTrainImageBytes;
+    *out = dst;
+    return mipnerf::launch_pack_linear_image(l.weight, l.in_features, off, transposed, dst, nn, kk, precision, st);
+  };
+  cudaError_t e;
+  for (int i = 0; i < depth; ++i) {
+    const mipnerf_b200_linear& l = w->linears[i];
+    if ((e = pack(l, 0, 0, W, i == 0 ? d.xyz_dim : W, &im->fwd[i]))) return e;
+    if (takes_skip(c, i) && (e = pack(l, W, 0, W, d.xyz_dim, &im->skip[i]))) return e;
+    if (i > 0 && (e = pack(l, 0, 1, W, W, &im->bwd[i]))) return e;  // B[k_out][n] = W_i[n][k_out]
+  }
+  if ((e = pack(w->linears[depth + 1], 0, 0, W, W, &im->fwd[depth]))) return e;  // bottleneck
+  if ((e = pack(w->linears[depth + 1], 0, 1, W, W, &im->bwd[depth]))) return e;
+  if ((e = pack(w->linears[depth + 2], 0, 0, Wc, W, &im->fwd[depth + 1]))) return e;  // view layer, bottleneck columns
+  return pack(w->linears[depth + 2], 0, 1, W, Wc, &im->bwd[depth + 1]);
+}
+
+// MLP.forward of m rows with every activation the backward needs kept in `s` (models/mip_nerf.py:75-111): the trunk
+// s.h[] from s.enc and the density head into s.raw_density; unless `density_only`, the bottleneck s.bott, the view layer
+// s.v (view encoding s.venc, or on the tensor cores its bias s.vrow, one row per `view_div` rows) and the colour head
+// into s.raw_rgb.  tc: the 128- and 256-wide layers on the tensor cores (images `im`), the heads in fp32.
+int mlp_forward_kept(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w, bool tc, int precision,
+                     const LayerImages& im, const TrainScratch& s, int64_t m, int view_div, bool density_only,
+                     cudaStream_t st) {
+  const int depth = c->net_depth, W = c->net_width, Wc = c->net_width_condition;
+  for (int i = 0; i < depth; ++i) {
+    const mipnerf_b200_linear& li = w->linears[i];
+    const bool skip = takes_skip(c, i);
+    const float* in = i == 0 ? s.enc : s.h[i - 1];
+    const int k1 = i == 0 ? d.xyz_dim : W;
+    if (!tc) {
+      CUDA_TRY(mipnerf::launch_linear_f32(in, k1, k1, skip ? s.enc : nullptr, d.xyz_dim, skip ? d.xyz_dim : 0, 1,
+                                          li.weight, li.bias, s.h[i], W, m, W, 1, st));
+    } else if (!skip) {
+      CUDA_TRY(mipnerf::launch_linear_tc(in, k1, im.fwd[i], s.h[i], W, m, W, k1, li.bias, nullptr, 1, nullptr, nullptr,
+                                         nullptr, nullptr, 1, precision, st));
+    } else {  // cat([h, enc]) as two K passes: the second adds the first's partial sums, the bias and the ReLU
+      CUDA_TRY(mipnerf::launch_linear_tc(in, k1, im.fwd[i], s.h[i], W, m, W, k1, nullptr, nullptr, 1, nullptr, nullptr,
+                                         nullptr, nullptr, 0, precision, st));
+      CUDA_TRY(mipnerf::launch_linear_tc(s.enc, d.xyz_dim, im.skip[i], s.h[i], W, m, W, d.xyz_dim, li.bias, nullptr, 1,
+                                         s.h[i], nullptr, nullptr, nullptr, 1, precision, st));
+    }
+  }
+  const float* h_last = s.h[depth - 1];
+  const mipnerf_b200_linear& dl = w->linears[depth];
+  const mipnerf_b200_linear& el = w->linears[depth + 1];
+  const mipnerf_b200_linear& vl = w->linears[depth + 2];
+  const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
+  CUDA_TRY(mipnerf::launch_linear_f32(h_last, W, W, nullptr, 0, 0, 1, dl.weight, dl.bias, s.raw_density, 1, m, 1, 0, st));
+  if (density_only) return MIPNERF_B200_OK;
+  if (!tc) {
+    CUDA_TRY(mipnerf::launch_linear_f32(h_last, W, W, nullptr, 0, 0, 1, el.weight, el.bias, s.bott, W, m, W, 0, st));
+    CUDA_TRY(mipnerf::launch_linear_f32(s.bott, W, W, s.venc, d.view_dim, d.view_dim, view_div, vl.weight, vl.bias, s.v,
+                                        Wc, m, Wc, 1, st));
+  } else {
+    CUDA_TRY(mipnerf::launch_linear_tc(h_last, W, im.fwd[depth], s.bott, W, m, W, W, el.bias, nullptr, 1, nullptr,
+                                       nullptr, nullptr, nullptr, 0, precision, st));
+    CUDA_TRY(mipnerf::launch_linear_tc(s.bott, W, im.fwd[depth + 1], s.v, Wc, m, Wc, W, nullptr, s.vrow, view_div,
+                                       nullptr, nullptr, nullptr, nullptr, 1, precision, st));
+  }
+  CUDA_TRY(mipnerf::launch_linear_f32(s.v, Wc, Wc, nullptr, 0, 0, 1, cl.weight, cl.bias, s.raw_rgb, 3, m, 3, 0, st));
+  return MIPNERF_B200_OK;
+}
+
+// The per-layer backward chain of m rows from d raw_rgb / d raw_density (s.d_raw_rgb, s.d_raw_density) through the
+// colour head, view layer, bottleneck + density head and trunk into `grads`, on the activations mlp_forward_kept left in
+// `s` (same `tc`, `view_div`, `density_only`).  With density_only it starts at the density head: d h_last is then the
+// rank-1 term d_raw_density . W_density alone, which dgrad_f32 with an empty dY computes without a GEMM.  touched[i]:
+// grads[i] already holds a sum to add to.
+int mlp_backward_chain(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w, bool tc,
+                       int precision, const LayerImages& im, const TrainScratch& s, int64_t m, int view_div,
+                       bool density_only, const mipnerf_b200_linear_grad* grads, bool* touched, cudaStream_t st) {
+  const int depth = c->net_depth, W = c->net_width, Wc = c->net_width_condition;
+  // tensor-core mode: the wgrad partials of the 128- and 256-wide layers on the tensor cores as well (dy comes from
+  // the 256-byte-aligned workspace carves, and an x2 always follows k1 = 256 columns); the two heads on fp32 FFMA
+  auto wgrad = [&](int idx, const float* dy, const float* x1, int k1, const float* x2, int k2, int div) {
+    const mipnerf_b200_linear& l = w->linears[idx];
+    if (tc && mipnerf::wgrad_tc_shape_ok(l.out_features)) {  // tensor-core partials + same reduction
+      int slices = 0;
+      cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy, 0, l.out_features, x1, 0, k1, k1, x2, 0, k2, k2, div,
+                                                         s.part, m, mipnerf::kWgradMaxSlices, precision, &slices, st);
+      if (e2 != cudaSuccess) return e2;
+      e2 = mipnerf::launch_wgrad_reduce(s.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
+                                        grads[idx].bias_grad, touched[idx] ? 1 : 0, st);
+      touched[idx] = true;
+      return e2;
+    }
+    cudaError_t e = mipnerf::launch_wgrad_f32(dy, l.out_features, x1, k1, k1, x2, k2, k2, div, s.part,
+                                              grads[idx].weight_grad, grads[idx].bias_grad, touched[idx] ? 1 : 0,
+                                              m, st);
+    touched[idx] = true;
+    return e;
+  };
+  const float* h_last = s.h[depth - 1];
+  const mipnerf_b200_linear& dl = w->linears[depth];
+  const mipnerf_b200_linear& el = w->linears[depth + 1];
+  const mipnerf_b200_linear& vl = w->linears[depth + 2];
+  const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
+  if (density_only) {
+    CUDA_TRY(wgrad(depth, s.d_raw_density, h_last, W, nullptr, 0, 1));
+    CUDA_TRY(mipnerf::launch_dgrad_f32(nullptr, 0, el.weight, W, s.d_raw_density, dl.weight, h_last, s.d_b, m, W, st));
+  } else {
+    // colour head, view layer                                          (models/mip_nerf.py:106-110)
+    CUDA_TRY(wgrad(d.n_lin - 1, s.d_raw_rgb, s.v, Wc, nullptr, 0, 1));
+    CUDA_TRY(mipnerf::launch_color_dgrad(s.d_raw_rgb, cl.weight, s.v, s.d_v, m, Wc, st));
+    CUDA_TRY(wgrad(depth + 2, s.d_v, s.bott, W, s.venc, d.view_dim, view_div));
+    if (!tc)
+      CUDA_TRY(mipnerf::launch_dgrad_f32(s.d_v, Wc, vl.weight, W + d.view_dim, nullptr, nullptr, nullptr, s.d_a, m, W,
+                                         st));
+    else
+      CUDA_TRY(mipnerf::launch_linear_tc(s.d_v, Wc, im.bwd[depth + 1], s.d_a, W, m, W, Wc, nullptr, nullptr, 1, nullptr,
+                                         nullptr, nullptr, nullptr, 0, precision, st));
+    // bottleneck + density head share h_last                           (models/mip_nerf.py:98-101)
+    CUDA_TRY(wgrad(depth + 1, s.d_a, h_last, W, nullptr, 0, 1));
+    CUDA_TRY(wgrad(depth, s.d_raw_density, h_last, W, nullptr, 0, 1));
+    if (!tc)
+      CUDA_TRY(mipnerf::launch_dgrad_f32(s.d_a, W, el.weight, W, s.d_raw_density, dl.weight, h_last, s.d_b, m, W, st));
+    else
+      CUDA_TRY(mipnerf::launch_linear_tc(s.d_a, W, im.bwd[depth], s.d_b, W, m, W, W, nullptr, nullptr, 1, nullptr,
+                                         s.d_raw_density, dl.weight, h_last, 0, precision, st));
+  }
+  // trunk                                                            (models/mip_nerf.py:93-97)
+  float *cur = s.d_b, *other = s.d_a;
+  for (int i = depth - 1; i >= 0; --i) {
+    const bool skip = takes_skip(c, i);
+    const float* in = i == 0 ? s.enc : s.h[i - 1];
+    const int k1 = i == 0 ? d.xyz_dim : W;
+    CUDA_TRY(wgrad(i, cur, in, k1, skip ? s.enc : nullptr, skip ? d.xyz_dim : 0, 1));
+    if (i > 0) {
+      if (!tc)
+        CUDA_TRY(mipnerf::launch_dgrad_f32(cur, W, w->linears[i].weight, k1 + (skip ? d.xyz_dim : 0), nullptr, nullptr,
+                                           s.h[i - 1], other, m, W, st));
+      else
+        CUDA_TRY(mipnerf::launch_linear_tc(cur, W, im.bwd[i], other, W, m, W, W, nullptr, nullptr, 1, nullptr, nullptr,
+                                           nullptr, s.h[i - 1], 0, precision, st));
+      float* tmp = cur;
+      cur = other;
+      other = tmp;
+    }
+  }
+  return MIPNERF_B200_OK;
+}
+
 // Where the backward pass of a training driver starts: the loss of mipnerf_b200_loss, or cotangents of the rendered
 // outputs (one entry per level).  Everything after the render backward only sees d raw_rgb / d raw_density.
 struct GradSource {
@@ -583,13 +739,154 @@ size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_
   return bytes;
 }
 
+// Operands of the tile-image backward chain for one chunk of `tiles` 128-row tiles: the forward's dump of the level
+// kernel (act [9][tiles][64 KB]: h_0..h_7, bottleneck; v [tiles][32 KB]: view-layer output), the IPE features enc16
+// [tiles][32 KB], the fp32 view encoding (one row per view_div rows), d raw_rgb / d raw_density [tiles * 128] and the
+// gradient tile images.  bf16x3: every image is followed by its lo image, `tiles` images further on.
+struct TileChainOps {
+  const uint8_t *act, *v, *enc16;
+  const float* venc;
+  int view_div;
+  const float *d_raw_rgb, *d_raw_density;
+  uint8_t *d_v, *d_a, *d_b, *relu_bits;
+  float* part;
+  int64_t tiles;
+};
+
+// The per-level backward chain of the fused training step, on 16-bit tile images: colour head, view layer, bottleneck
+// + density head, trunk, into `grads` (touched[i]: grads[i] already holds a sum to add to; inv_gscale takes the fp16
+// step's gradient scale out again).  img_bwd[i] = W_i[:, :256]^T (slots depth / depth + 1: bottleneck, view layer),
+// img_bwd_lo their lo images in bf16x3.  density_only (a density query): the chain starts at the density head; d h_7
+// is then the rank-1 term d_raw_density . W_density, masked by h_7 > 0, which the bottleneck's dgrad computes on an
+// all-zero d_a with the mask read from the h_7 tile (there is no bottleneck wgrad to leave its sign bits behind).
+int tile_backward_chain(const mipnerf_b200_config* cfg, const Dims& d, const mipnerf_b200_weights* w, int precision,
+                        const uint8_t* const* img_bwd, const uint8_t* const* img_bwd_lo, const TileChainOps& o,
+                        bool density_only, float inv_gscale, const mipnerf_b200_linear_grad* grads, bool* touched,
+                        cudaStream_t st) {
+  const int depth = cfg->net_depth, W = cfg->net_width, Wc = cfg->net_width_condition;
+  const bool x3 = precision == MIPNERF_B200_BF16X3;
+  const int fmt = x3 ? MIPNERF_B200_BF16 : precision;
+  const int64_t m = o.tiles * 128;
+  const mipnerf_b200_linear& dl = w->linears[depth];
+  const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
+  // bf16x3: the lo image behind a hi image of `bytes_per_tile` bytes per tile (null in the 16-bit step)
+  auto lo_img = [&](const uint8_t* hi, size_t bytes_per_tile) {
+    return x3 ? const_cast<uint8_t*>(hi) + (size_t)o.tiles * bytes_per_tile : nullptr;
+  };
+  // MIPNERF_B200_TRAIN_MASKBITS=0: the dgrad GEMMs read the ReLU mask from the activation tile images again (A/B)
+  const char* bits_env = getenv("MIPNERF_B200_TRAIN_MASKBITS");
+  const bool use_bits = !(bits_env && bits_env[0] == '0');
+  // dy16_lo / x1_lo / x2_lo: bf16x3's lo images (null otherwise)
+  auto wgrad = [&](int idx, const void* dy16, const void* x1, int k1, const void* x2, int x2_t16, int k2, int div,
+                   bool emit_mask, const void* dy16_lo, const void* x1_lo, const void* x2_lo) {
+    const mipnerf_b200_linear& l = w->linears[idx];
+    int slices = 0;
+    cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy16, 1, l.out_features, x1, 1, k1, k1, x2, x2_t16, k2, k2, div,
+                                                       o.part, m, mipnerf::kWgradMaxSlices, fmt, &slices, st,
+                                                       emit_mask && use_bits ? o.relu_bits : nullptr, dy16_lo, x1_lo,
+                                                       x2_lo);
+    if (e2 != cudaSuccess) return e2;
+    e2 = mipnerf::launch_wgrad_reduce(o.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
+                                      grads[idx].bias_grad, touched[idx] ? 1 : 0, st, inv_gscale);
+    touched[idx] = true;
+    return e2;
+  };
+  // y = [mask] (x . B^T + r1 r1w) on tile images, in bf16x3 on the hi / lo pairs
+  // (act: the layer input whose ReLU masks the output, read as the sign bits the preceding wgrad left behind, or
+  // null for no mask; image_mask: read it from the activation tile itself)
+  auto dgrad = [&](const uint8_t* xi, int slot, uint8_t* y, int nn, int kk, const float* r1, const float* r1w,
+                   const uint8_t* act_in, bool image_mask = false) {
+    const bool bits_ok = use_bits && !image_mask;
+    const void* mask = act_in && !bits_ok ? act_in : nullptr;
+    const void* bits = act_in && bits_ok ? o.relu_bits : nullptr;
+    if (x3)
+      return mipnerf::launch_linear_t16_x3(xi, lo_img(xi, (size_t)kk * 256), img_bwd[slot], img_bwd_lo[slot], y,
+                                           lo_img(y, (size_t)nn * 256), m, nn, kk, r1, r1w, mask, st, bits);
+    return mipnerf::launch_linear_t16(xi, img_bwd[slot], y, m, nn, kk, r1, r1w, mask, fmt, st, bits);
+  };
+  auto h16 = [&](int i) { return o.act + (size_t)i * o.tiles * 65536; };  // h_0..h_7, 8 = bottleneck
+  auto h16_lo = [&](int i) { return x3 ? h16(9 + i) : nullptr; };
+  const uint8_t* enc16_lo = lo_img(o.enc16, 32768);
+  if (density_only) {
+    CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(o.d_raw_density, 1, h16(depth - 1), W, o.part, grads[depth].weight_grad,
+                                               grads[depth].bias_grad, touched[depth] ? 1 : 0, m, fmt, st, inv_gscale,
+                                               h16_lo(depth - 1)));
+    touched[depth] = true;
+    CUDA_TRY(cudaMemsetAsync(o.d_a, 0, (size_t)o.tiles * 65536 * (x3 ? 2 : 1), st));
+    CUDA_TRY(dgrad(o.d_a, depth, o.d_b, W, W, o.d_raw_density, dl.weight, h16(depth - 1), /*image_mask=*/true));
+  } else {
+    // colour head, view layer                                          (models/mip_nerf.py:106-110)
+    CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(o.d_raw_rgb, 3, o.v, Wc, o.part, grads[d.n_lin - 1].weight_grad,
+                                               grads[d.n_lin - 1].bias_grad, touched[d.n_lin - 1] ? 1 : 0, m, fmt, st,
+                                               inv_gscale, lo_img(o.v, 32768)));
+    touched[d.n_lin - 1] = true;
+    CUDA_TRY(mipnerf::launch_color_dgrad_t16(o.d_raw_rgb, cl.weight, o.v, o.d_v, m, Wc, fmt, st, lo_img(o.d_v, 32768)));
+    CUDA_TRY(wgrad(depth + 2, o.d_v, h16(8), W, o.venc, 0, d.view_dim, o.view_div, false, lo_img(o.d_v, 32768),
+                   h16_lo(8), nullptr));
+    CUDA_TRY(dgrad(o.d_v, depth + 1, o.d_a, W, Wc, nullptr, nullptr, nullptr));
+    // bottleneck + density head share h_7                              (models/mip_nerf.py:98-101)
+    CUDA_TRY(wgrad(depth + 1, o.d_a, h16(depth - 1), W, nullptr, 0, 0, 1, /*emit_mask=*/true, lo_img(o.d_a, 65536),
+                   h16_lo(depth - 1), nullptr));  // sign mask of h_7
+    CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(o.d_raw_density, 1, h16(depth - 1), W, o.part, grads[depth].weight_grad,
+                                               grads[depth].bias_grad, touched[depth] ? 1 : 0, m, fmt, st, inv_gscale,
+                                               h16_lo(depth - 1)));
+    touched[depth] = true;
+    CUDA_TRY(dgrad(o.d_a, depth, o.d_b, W, W, o.d_raw_density, dl.weight, h16(depth - 1)));
+  }
+  // trunk                                                            (models/mip_nerf.py:93-97)
+  uint8_t *cur = o.d_b, *other = o.d_a;
+  for (int i = depth - 1; i >= 0; --i) {
+    const bool skip = takes_skip(cfg, i);
+    if (i == 0)
+      CUDA_TRY(wgrad(0, cur, o.enc16, d.xyz_dim, nullptr, 0, 0, 1, false, lo_img(cur, 65536), enc16_lo, nullptr));
+    else
+      CUDA_TRY(wgrad(i, cur, h16(i - 1), W, skip ? o.enc16 : nullptr, 1, skip ? d.xyz_dim : 0, 1, true,
+                     lo_img(cur, 65536), h16_lo(i - 1), skip ? enc16_lo : nullptr));
+    if (i > 0) {  // the wgrad just streamed h_{i-1} and left its sign mask behind: 32 B per row instead of 512
+      CUDA_TRY(dgrad(cur, i, other, W, W, nullptr, nullptr, h16(i - 1)));
+      uint8_t* tmp = cur;
+      cur = other;
+      other = tmp;
+    }
+  }
+  return MIPNERF_B200_OK;
+}
+
+// The B operands of the tile-image dgrad chain, packed once per call (the weights change every optimiser step) into
+// kTrainImageBytes slots at `base`: bwd[i] = W_i[:, :256]^T (slots depth / depth + 1: bottleneck, view layer); bf16x3
+// also their lo images, kMaxTrainDepth + 2 slots further on.
+cudaError_t pack_bwd_images(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, int precision, uint8_t* base,
+                            const uint8_t** img_bwd, const uint8_t** img_bwd_lo, cudaStream_t st) {
+  const int depth = cfg->net_depth, W = cfg->net_width, Wc = cfg->net_width_condition;
+  const bool x3 = precision == MIPNERF_B200_BF16X3;
+  const int fmt = x3 ? MIPNERF_B200_BF16 : precision;
+  int slot = 0;
+  auto pack = [&](const mipnerf_b200_linear& l, int nn, int kk, const uint8_t** out) {
+    uint8_t* dst = base + (size_t)slot * kTrainImageBytes;
+    *out = dst;
+    if (x3) {
+      uint8_t* lo = base + (size_t)(slot + kMaxTrainDepth + 2) * kTrainImageBytes;
+      img_bwd_lo[out - img_bwd] = lo;
+      cudaError_t e = mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, lo, nn, kk, fmt, st, 1);
+      if (e != cudaSuccess) return e;
+    }
+    ++slot;
+    return mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, dst, nn, kk, fmt, st);
+  };
+  cudaError_t e;
+  for (int i = 1; i < depth; ++i)
+    if ((e = pack(w->linears[i], W, W, &img_bwd[i]))) return e;
+  if ((e = pack(w->linears[depth + 1], W, W, &img_bwd[depth]))) return e;
+  return pack(w->linears[depth + 2], W, Wc, &img_bwd[depth + 1]);
+}
+
 static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d, const mipnerf_b200_weights* w,
                                   const mipnerf_b200_rays* rays, int randomized, const float* t_rand,
                                   const float* u_jitter, const mipnerf_b200_rng* rng, int white_bkgd, int precision,
                                   const GradSource& src, bool given_t, mipnerf_b200_level_out* outs,
                                   const mipnerf_b200_linear_grad* grads, bool* touched, void* workspace,
                                   cudaStream_t st) {
-  const int n = cfg->num_samples, depth = cfg->net_depth, W = cfg->net_width, Wc = cfg->net_width_condition;
+  const int n = cfg->num_samples;
   const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
   const int64_t B = rays->num_rays;
   // bf16x3: every operand of the backward is a pair of bf16 tile images, hi and lo (the 16-bit launchers' format
@@ -605,26 +902,7 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
   CUDA_TRY(mipnerf::tc_pack_weights(cfg, w, precision, s0.packed, st));
   const uint8_t* img_bwd[kMaxTrainDepth + 2] = {nullptr};
   const uint8_t* img_bwd_lo[kMaxTrainDepth + 2] = {nullptr};  // bf16x3: slot + kMaxTrainDepth + 2
-  {
-    int slot = 0;
-    auto pack = [&](const mipnerf_b200_linear& l, int nn, int kk, const uint8_t** out) {
-      uint8_t* dst = s0.images + (size_t)slot * kTrainImageBytes;
-      *out = dst;
-      if (x3) {
-        uint8_t* lo = s0.images + (size_t)(slot + kMaxTrainDepth + 2) * kTrainImageBytes;
-        img_bwd_lo[out - img_bwd] = lo;
-        cudaError_t e = mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, lo, nn, kk, fmt, st, 1);
-        if (e != cudaSuccess) return e;
-      }
-      ++slot;
-      return mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, dst, nn, kk, fmt, st);
-    };
-    for (int i = 1; i < depth; ++i) CUDA_TRY(pack(w->linears[i], W, W, &img_bwd[i]));
-    CUDA_TRY(pack(w->linears[depth + 1], W, W, &img_bwd[depth]));
-    CUDA_TRY(pack(w->linears[depth + 2], W, Wc, &img_bwd[depth + 1]));
-  }
-  const mipnerf_b200_linear& dl = w->linears[depth];
-  const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
+  CUDA_TRY(pack_bwd_images(cfg, w, precision, s0.images, img_bwd, img_bwd_lo, st));
   // fp16 gradients underflow: d loss / d activation is ~1e-7 .. 1e-4 per sample (the loss is a mean over the batch),
   // below fp16's 6e-5 normal range.  The backward pass is linear in d loss / d raw, so render_backward emits it
   // scaled by 2^10 (it is bounded by 2/3 per sample: no overflow), every gradient tile image carries that factor, and
@@ -632,7 +910,6 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
   const float gscale = precision == MIPNERF_B200_FP16 ? 1024.f : 1.f, inv_gscale = 1.f / gscale;
   for (int64_t off = 0; off < B; off += chunk) {
     const int64_t cnt = (B - off) < chunk ? (B - off) : chunk;
-    const int64_t m = cnt * n;
     const mipnerf_b200_rays rc_ = offset_rays(*rays, off, cnt);
     const FusedScratch s = carve_fused(cfg, d, cnt, precision, workspace);
     // bf16x3: the lo image behind a hi image of `bytes_per_ray` bytes per ray (null in the 16-bit step)
@@ -659,82 +936,20 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
     CUDA_TRY(mipnerf::tc_forward(cfg, &wl, &rc_, randomized, t_rand ? t_rand + off * (n + 1) : nullptr,
                                  u_jitter ? u_jitter + off * (n + 1) : nullptr, rng, white_bkgd, precision, lo, s.tcws,
                                  s.tcws_bytes, st, &dump, off, given_t ? 1 : 0));
-    // MIPNERF_B200_TRAIN_MASKBITS=0: the dgrad GEMMs read the ReLU mask from the activation tile images again (A/B)
-    const char* bits_env = getenv("MIPNERF_B200_TRAIN_MASKBITS");
-    const bool use_bits = !(bits_env && bits_env[0] == '0');
-    // dy16_lo / x1_lo / x2_lo: bf16x3's lo images (null otherwise)
-    auto wgrad = [&](int idx, const void* dy16, const void* x1, int k1, const void* x2, int x2_t16, int k2, int div,
-                     bool emit_mask, const void* dy16_lo, const void* x1_lo, const void* x2_lo) {
-      const mipnerf_b200_linear& l = w->linears[idx];
-      int slices = 0;
-      cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy16, 1, l.out_features, x1, 1, k1, k1, x2, x2_t16, k2, k2, div,
-                                                         s.part, m, mipnerf::kWgradMaxSlices, fmt, &slices, st,
-                                                         emit_mask && use_bits ? s.relu_bits : nullptr, dy16_lo, x1_lo,
-                                                         x2_lo);
-      if (e2 != cudaSuccess) return e2;
-      e2 = mipnerf::launch_wgrad_reduce(s.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
-                                        grads[idx].bias_grad, touched[idx] ? 1 : 0, st, inv_gscale);
-      touched[idx] = true;
-      return e2;
-    };
-    // y = [mask] (x . B^T + r1 r1w) on tile images, in bf16x3 on the hi / lo pairs
-    // (act: the layer input whose ReLU masks the output, read as the sign bits the preceding wgrad left behind, or
-    // null for no mask)
-    auto dgrad = [&](const uint8_t* xi, int slot, uint8_t* y, int nn, int kk, const float* r1, const float* r1w,
-                     const uint8_t* act_in) {
-      const void* mask = act_in && !use_bits ? act_in : nullptr;
-      const void* bits = act_in && use_bits ? s.relu_bits : nullptr;
-      if (x3)
-        return mipnerf::launch_linear_t16_x3(xi, lo_img(xi, (size_t)kk * 256), img_bwd[slot], img_bwd_lo[slot], y,
-                                             lo_img(y, (size_t)nn * 256), m, nn, kk, r1, r1w, mask, st, bits);
-      return mipnerf::launch_linear_t16(xi, img_bwd[slot], y, m, nn, kk, r1, r1w, mask, fmt, st, bits);
-    };
     for (int l = 0; l < cfg->num_levels; ++l) {
       const float* t_cur = lo[l].t_samples;
-      const uint8_t* act = s.act[l];
-      auto h16 = [&](int i) { return act + (size_t)i * cnt * 65536; };  // h_0..h_7, 8 = bottleneck
-      auto h16_lo = [&](int i) { return x3 ? h16(9 + i) : nullptr; };
       // the IPE features again (operand of two wgrads; the level kernel keeps its own 16-bit copy on chip), written
       // straight into a tile image so that those wgrads stage them by bulk copy like every other operand
-      uint8_t* enc16_lo = lo_img(s.enc16, 32768);
       CUDA_TRY(mipnerf::launch_ipe_t16(rc_.origins, rc_.directions, rc_.radii, t_cur, s.enc16, cnt, n,
-                                       cfg->disable_integration, fmt, st, enc16_lo));
+                                       cfg->disable_integration, fmt, st, lo_img(s.enc16, 32768)));
       CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb[l], s.raw_density[l], t_cur, rc_.directions,
                                   white_bkgd, rgb_scale, gscale, s.d_raw_rgb, s.d_raw_density, st));
-      // colour head, view layer                                          (models/mip_nerf.py:106-110)
-      CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(s.d_raw_rgb, 3, s.v[l], Wc, s.part, grads[d.n_lin - 1].weight_grad,
-                                                 grads[d.n_lin - 1].bias_grad, touched[d.n_lin - 1] ? 1 : 0, m,
-                                                 fmt, st, inv_gscale, lo_img(s.v[l], 32768)));
-      touched[d.n_lin - 1] = true;
-      CUDA_TRY(mipnerf::launch_color_dgrad_t16(s.d_raw_rgb, cl.weight, s.v[l], s.d_v, m, Wc, fmt, st,
-                                               lo_img(s.d_v, 32768)));
-      CUDA_TRY(wgrad(depth + 2, s.d_v, h16(8), W, s.venc, 0, d.view_dim, n, false, lo_img(s.d_v, 32768), h16_lo(8),
-                     nullptr));
-      CUDA_TRY(dgrad(s.d_v, depth + 1, s.d_a, W, Wc, nullptr, nullptr, nullptr));
-      // bottleneck + density head share h_7                              (models/mip_nerf.py:98-101)
-      CUDA_TRY(wgrad(depth + 1, s.d_a, h16(depth - 1), W, nullptr, 0, 0, 1, /*emit_mask=*/true, lo_img(s.d_a, 65536),
-                     h16_lo(depth - 1), nullptr));  // sign mask of h_7
-      CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(s.d_raw_density, 1, h16(depth - 1), W, s.part,
-                                                 grads[depth].weight_grad, grads[depth].bias_grad,
-                                                 touched[depth] ? 1 : 0, m, fmt, st, inv_gscale, h16_lo(depth - 1)));
-      touched[depth] = true;
-      CUDA_TRY(dgrad(s.d_a, depth, s.d_b, W, W, s.d_raw_density, dl.weight, h16(depth - 1)));
-      // trunk                                                            (models/mip_nerf.py:93-97)
-      uint8_t *cur = s.d_b, *other = s.d_a;
-      for (int i = depth - 1; i >= 0; --i) {
-        const bool skip = takes_skip(cfg, i);
-        if (i == 0)
-          CUDA_TRY(wgrad(0, cur, s.enc16, d.xyz_dim, nullptr, 0, 0, 1, false, lo_img(cur, 65536), enc16_lo, nullptr));
-        else
-          CUDA_TRY(wgrad(i, cur, h16(i - 1), W, skip ? s.enc16 : nullptr, 1, skip ? d.xyz_dim : 0, 1, true,
-                         lo_img(cur, 65536), h16_lo(i - 1), skip ? enc16_lo : nullptr));
-        if (i > 0) {  // the wgrad just streamed h_{i-1} and left its sign mask behind: 32 B per row instead of 512
-          CUDA_TRY(dgrad(cur, i, other, W, W, nullptr, nullptr, h16(i - 1)));
-          uint8_t* tmp = cur;
-          cur = other;
-          other = tmp;
-        }
-      }
+      const TileChainOps ops{s.act[l], s.v[l], s.enc16, s.venc, n, s.d_raw_rgb, s.d_raw_density,
+                             s.d_v, s.d_a, s.d_b, s.relu_bits, s.part, cnt};
+      int rc;
+      if ((rc = tile_backward_chain(cfg, d, w, precision, img_bwd, img_bwd_lo, ops, false, inv_gscale, grads, touched,
+                                    st)))
+        return rc;
     }
   }
   return MIPNERF_B200_OK;
@@ -797,7 +1012,7 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   if (rays->num_rays > 0 && (!workspace || workspace_bytes < need))
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
-  const int n = cfg->num_samples, depth = cfg->net_depth, W = cfg->net_width, Wc = cfg->net_width_condition;
+  const int n = cfg->num_samples, depth = cfg->net_depth;
   const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
   const int64_t B = rays->num_rays;
   bool touched[kMaxTrainDepth + 8];
@@ -812,30 +1027,11 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   if (tc && B > 0 && train_fused_supported(cfg, precision))
     return forward_backward_fused(cfg, d, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision, src,
                                   given_t, outs, grads, touched, workspace, st);
-  // ---- tensor-core mode: B operands of every forward / dgrad GEMM, packed once per call (the weights change every
-  //      optimiser step).  fwd[i] = W_i[:, :k_main], fwd_skip[i] = W_i[:, 256:352], bwd[i] = W_i[:, :256]^T;
-  //      slots depth / depth+1 hold the bottleneck and the view layer.
-  const uint8_t *img_fwd[kMaxTrainDepth + 2] = {nullptr}, *img_skip[kMaxTrainDepth] = {nullptr},
-                *img_bwd[kMaxTrainDepth + 2] = {nullptr};
-  if (tc && B > 0) {
-    uint8_t* base = carve_train(cfg, d, B < kChunkRaysFp32 ? B : kChunkRaysFp32, workspace).images;
-    int slot = 0;
-    auto pack = [&](const mipnerf_b200_linear& l, int off, int transposed, int nn, int kk, const uint8_t** out) {
-      uint8_t* dst = base + (size_t)(slot++) * kTrainImageBytes;
-      *out = dst;
-      return mipnerf::launch_pack_linear_image(l.weight, l.in_features, off, transposed, dst, nn, kk, precision, st);
-    };
-    for (int i = 0; i < depth; ++i) {
-      const mipnerf_b200_linear& l = w->linears[i];
-      CUDA_TRY(pack(l, 0, 0, W, i == 0 ? d.xyz_dim : W, &img_fwd[i]));
-      if (takes_skip(cfg, i)) CUDA_TRY(pack(l, W, 0, W, d.xyz_dim, &img_skip[i]));
-      if (i > 0) CUDA_TRY(pack(l, 0, 1, W, W, &img_bwd[i]));          // B[k_out][n] = W_i[n][k_out]
-    }
-    CUDA_TRY(pack(w->linears[depth + 1], 0, 0, W, W, &img_fwd[depth]));      // bottleneck
-    CUDA_TRY(pack(w->linears[depth + 1], 0, 1, W, W, &img_bwd[depth]));
-    CUDA_TRY(pack(w->linears[depth + 2], 0, 0, Wc, W, &img_fwd[depth + 1]));  // view layer, bottleneck columns
-    CUDA_TRY(pack(w->linears[depth + 2], 0, 1, W, Wc, &img_bwd[depth + 1]));
-  }
+  // ---- tensor-core mode: B operands of every forward / dgrad GEMM, packed once per call
+  LayerImages im{};
+  if (tc && B > 0)
+    CUDA_TRY(pack_layer_images(cfg, d, w, precision,
+                               carve_train(cfg, d, B < kChunkRaysFp32 ? B : kChunkRaysFp32, workspace).images, &im, st));
 
   for (int64_t off = 0; off < B; off += kChunkRaysFp32) {
     const int64_t cnt = (B - off) < kChunkRaysFp32 ? (B - off) : kChunkRaysFp32;
@@ -847,26 +1043,6 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
       const mipnerf_b200_linear& vl0 = w->linears[depth + 2];
       CUDA_TRY(mipnerf::launch_view_bias_from_enc(s.venc, vl0.weight, vl0.bias, s.vrow, cnt, st));
     }
-    // tensor-core mode: the wgrad partials of the 128- and 256-wide layers on the tensor cores as well (dy comes from
-    // the 256-byte-aligned workspace carves, and an x2 always follows k1 = 256 columns); the two heads on fp32 FFMA
-    auto wgrad = [&](int idx, const float* dy, const float* x1, int k1, const float* x2, int k2, int div) {
-      const mipnerf_b200_linear& l = w->linears[idx];
-      if (tc && mipnerf::wgrad_tc_shape_ok(l.out_features)) {  // tensor-core partials + same reduction
-        int slices = 0;
-        cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy, 0, l.out_features, x1, 0, k1, k1, x2, 0, k2, k2, div,
-                                                           s.part, m, mipnerf::kWgradMaxSlices, precision, &slices, st);
-        if (e2 != cudaSuccess) return e2;
-        e2 = mipnerf::launch_wgrad_reduce(s.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
-                                          grads[idx].bias_grad, touched[idx] ? 1 : 0, st);
-        touched[idx] = true;
-        return e2;
-      }
-      cudaError_t e = mipnerf::launch_wgrad_f32(dy, l.out_features, x1, k1, k1, x2, k2, k2, div, s.part,
-                                                grads[idx].weight_grad, grads[idx].bias_grad, touched[idx] ? 1 : 0,
-                                                m, st);
-      touched[idx] = true;
-      return e;
-    };
     const float *t_prev = nullptr, *w_prev = nullptr;
     for (int l = 0; l < cfg->num_levels; ++l) {
       float* t_cur = outs[l].t_samples ? outs[l].t_samples + off * (n + 1) : s.t[l & 1];
@@ -888,46 +1064,10 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
       }
       CUDA_TRY(mipnerf::launch_ipe_from_t(rc_.origins, rc_.directions, rc_.radii, t_cur, s.enc, cnt, n,
                                           cfg->min_deg_point, cfg->max_deg_point, cfg->disable_integration, st));
-      for (int i = 0; i < depth; ++i) {
-        const mipnerf_b200_linear& li = w->linears[i];
-        const bool skip = takes_skip(cfg, i);
-        const float* in = i == 0 ? s.enc : s.h[i - 1];
-        const int k1 = i == 0 ? d.xyz_dim : W;
-        if (!tc) {
-          CUDA_TRY(mipnerf::launch_linear_f32(in, k1, k1, skip ? s.enc : nullptr, d.xyz_dim, skip ? d.xyz_dim : 0, 1,
-                                              li.weight, li.bias, s.h[i], W, m, W, 1, st));
-        } else if (!skip) {
-          CUDA_TRY(mipnerf::launch_linear_tc(in, k1, img_fwd[i], s.h[i], W, m, W, k1, li.bias, nullptr, 1, nullptr,
-                                             nullptr, nullptr, nullptr, 1, precision, st));
-        } else {  // cat([h, enc]) as two K passes: the second adds the first's partial sums, the bias and the ReLU
-          CUDA_TRY(mipnerf::launch_linear_tc(in, k1, img_fwd[i], s.h[i], W, m, W, k1, nullptr, nullptr, 1, nullptr,
-                                             nullptr, nullptr, nullptr, 0, precision, st));
-          CUDA_TRY(mipnerf::launch_linear_tc(s.enc, d.xyz_dim, img_skip[i], s.h[i], W, m, W, d.xyz_dim, li.bias, nullptr,
-                                             1, s.h[i], nullptr, nullptr, nullptr, 1, precision, st));
-        }
-      }
-      const float* h_last = s.h[depth - 1];
-      const mipnerf_b200_linear& dl = w->linears[depth];
-      const mipnerf_b200_linear& el = w->linears[depth + 1];
-      const mipnerf_b200_linear& vl = w->linears[depth + 2];
-      const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
-      CUDA_TRY(mipnerf::launch_linear_f32(h_last, W, W, nullptr, 0, 0, 1, dl.weight, dl.bias, s.raw_density, 1, m, 1,
-                                          0, st));
+      if ((rc = mlp_forward_kept(cfg, d, w, tc, precision, im, s, m, n, false, st))) return rc;
       // density noise (models/mip_nerf.py:232-233), in place: render_backward then takes softplus' at the noisy point
       CUDA_TRY(mipnerf::launch_add_density_noise(
           s.raw_density, mipnerf::density_noise_draws(cfg, randomized, outs[l].density_normal, rng, off, l, n), cnt, n, st));
-      if (!tc) {
-        CUDA_TRY(mipnerf::launch_linear_f32(h_last, W, W, nullptr, 0, 0, 1, el.weight, el.bias, s.bott, W, m, W, 0, st));
-        CUDA_TRY(mipnerf::launch_linear_f32(s.bott, W, W, s.venc, d.view_dim, d.view_dim, n, vl.weight, vl.bias, s.v,
-                                            Wc, m, Wc, 1, st));
-      } else {
-        CUDA_TRY(mipnerf::launch_linear_tc(h_last, W, img_fwd[depth], s.bott, W, m, W, W, el.bias, nullptr, 1, nullptr,
-                                           nullptr, nullptr, nullptr, 0, precision, st));
-        CUDA_TRY(mipnerf::launch_linear_tc(s.bott, W, img_fwd[depth + 1], s.v, Wc, m, Wc, W, nullptr, s.vrow, n, nullptr,
-                                           nullptr, nullptr, nullptr, 1, precision, st));
-      }
-      CUDA_TRY(mipnerf::launch_linear_f32(s.v, Wc, Wc, nullptr, 0, 0, 1, cl.weight, cl.bias, s.raw_rgb, 3, m, 3, 0,
-                                          st));
       CUDA_TRY(mipnerf::launch_composite(s.raw_rgb, s.raw_density, t_cur, rc_.directions, comp_cur, dist_cur, acc_cur,
                                          w_cur, cnt, n, white_bkgd, 1, cfg->density_bias, rgb_scale, cfg->rgb_padding,
                                          st));
@@ -935,43 +1075,7 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
       // ---- backward of this level (its fenceposts are constants, so levels are independent here)
       CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb, s.raw_density, t_cur, rc_.directions, white_bkgd,
                                   rgb_scale, 1.f, s.d_raw_rgb, s.d_raw_density, st));
-      // colour head, view layer                                          (models/mip_nerf.py:106-110)
-      CUDA_TRY(wgrad(d.n_lin - 1, s.d_raw_rgb, s.v, Wc, nullptr, 0, 1));
-      CUDA_TRY(mipnerf::launch_color_dgrad(s.d_raw_rgb, cl.weight, s.v, s.d_v, m, Wc, st));
-      CUDA_TRY(wgrad(depth + 2, s.d_v, s.bott, W, s.venc, d.view_dim, n));
-      if (!tc)
-        CUDA_TRY(mipnerf::launch_dgrad_f32(s.d_v, Wc, vl.weight, W + d.view_dim, nullptr, nullptr, nullptr, s.d_a, m, W,
-                                           st));
-      else
-        CUDA_TRY(mipnerf::launch_linear_tc(s.d_v, Wc, img_bwd[depth + 1], s.d_a, W, m, W, Wc, nullptr, nullptr, 1,
-                                           nullptr, nullptr, nullptr, nullptr, 0, precision, st));
-      // bottleneck + density head share h_last                           (models/mip_nerf.py:98-101)
-      CUDA_TRY(wgrad(depth + 1, s.d_a, h_last, W, nullptr, 0, 1));
-      CUDA_TRY(wgrad(depth, s.d_raw_density, h_last, W, nullptr, 0, 1));
-      if (!tc)
-        CUDA_TRY(mipnerf::launch_dgrad_f32(s.d_a, W, el.weight, W, s.d_raw_density, dl.weight, h_last, s.d_b, m, W, st));
-      else
-        CUDA_TRY(mipnerf::launch_linear_tc(s.d_a, W, img_bwd[depth], s.d_b, W, m, W, W, nullptr, nullptr, 1, nullptr,
-                                           s.d_raw_density, dl.weight, h_last, 0, precision, st));
-      // trunk                                                            (models/mip_nerf.py:93-97)
-      float *cur = s.d_b, *other = s.d_a;
-      for (int i = depth - 1; i >= 0; --i) {
-        const bool skip = takes_skip(cfg, i);
-        const float* in = i == 0 ? s.enc : s.h[i - 1];
-        const int k1 = i == 0 ? d.xyz_dim : W;
-        CUDA_TRY(wgrad(i, cur, in, k1, skip ? s.enc : nullptr, skip ? d.xyz_dim : 0, 1));
-        if (i > 0) {
-          if (!tc)
-            CUDA_TRY(mipnerf::launch_dgrad_f32(cur, W, w->linears[i].weight, k1 + (skip ? d.xyz_dim : 0), nullptr,
-                                               nullptr, s.h[i - 1], other, m, W, st));
-          else
-            CUDA_TRY(mipnerf::launch_linear_tc(cur, W, img_bwd[i], other, W, m, W, W, nullptr, nullptr, 1, nullptr,
-                                               nullptr, nullptr, s.h[i - 1], 0, precision, st));
-          float* tmp = cur;
-          cur = other;
-          other = tmp;
-        }
-      }
+      if ((rc = mlp_backward_chain(cfg, d, w, tc, precision, im, s, m, n, false, grads, touched, st))) return rc;
       t_prev = t_cur;
       w_prev = w_cur;
     }
@@ -1573,6 +1677,246 @@ int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b2
     CUDA_TRY(mipnerf::launch_radiance_activation(rr, rd, rgb ? rgb + off * 3 : nullptr, density ? density + off : nullptr,
                                                  m, cfg->density_bias, rgb_scale, cfg->rgb_padding, st));
   }
+  return MIPNERF_B200_OK;
+}
+
+namespace {
+// Scratch of the fp32 query backward for one chunk of m points: the training step's activation layout (TrainScratch
+// with one row per point, view encoding included) without its per-ray buffers, and the zero covariances.
+struct QueryGradScratch {
+  TrainScratch t;
+  float* zero_covs;
+  size_t bytes;
+};
+QueryGradScratch carve_query_grad(const mipnerf_b200_config* c, const Dims& d, int64_t m, bool radiance, void* base) {
+  QueryGradScratch s{};
+  size_t off = 0;
+  auto take = [&](size_t elems) {
+    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
+    off += align_up(elems * sizeof(float));
+    return p;
+  };
+  const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
+  const size_t max_k = (size_t)c->net_width + (d.xyz_dim > d.view_dim ? d.xyz_dim : d.view_dim) + 1;
+  s.t.part = take((size_t)mipnerf::kWgradMaxSlices * max_n * max_k);
+  s.zero_covs = take((size_t)m * 3);
+  s.t.enc = take((size_t)m * d.xyz_dim);
+  for (int i = 0; i < c->net_depth; ++i) s.t.h[i] = take((size_t)m * c->net_width);
+  s.t.raw_density = take((size_t)m);
+  s.t.d_raw_density = take((size_t)m);
+  s.t.d_a = take((size_t)m * c->net_width);
+  s.t.d_b = take((size_t)m * c->net_width);
+  if (radiance) {
+    s.t.venc = take((size_t)m * d.view_dim);
+    s.t.bott = take((size_t)m * c->net_width);
+    s.t.v = take((size_t)m * c->net_width_condition);
+    s.t.raw_rgb = take((size_t)m * 3);
+    s.t.d_v = take((size_t)m * c->net_width_condition);
+    s.t.d_raw_rgb = take((size_t)m * 3);
+  }
+  s.bytes = off;
+  return s;
+}
+
+// Scratch of the bf16 query backward for one chunk of m points, T = ceil(m / 128) tiles: the level kernel's query dump
+// (act: h_0..h_7 and, radiance, the bottleneck; v), the raw heads, the IPE tile image, the fp32 view encoding and the
+// gradient tile images of the fused step's chain, all over whole tiles (rows past m: zero cotangents).
+struct QueryFusedScratch {
+  uint8_t *images, *packed, *act, *v, *enc16, *relu_bits, *d_v, *d_a, *d_b;
+  float *part, *slots, *raw_rgb, *raw_density, *venc, *d_raw_rgb, *d_raw_density;
+  size_t slots_bytes, bytes;
+};
+QueryFusedScratch carve_query_fused(const mipnerf_b200_config* c, const Dims& d, int64_t m, bool radiance,
+                                    void* base) {
+  QueryFusedScratch s{};
+  size_t off = 0;
+  auto take_bytes = [&](size_t bytes) {
+    uint8_t* p = base ? static_cast<uint8_t*>(base) + off : nullptr;
+    off += align_up(bytes);
+    return p;
+  };
+  auto take = [&](size_t elems) { return reinterpret_cast<float*>(take_bytes(elems * sizeof(float))); };
+  const int64_t tiles = (m + 127) / 128, rows = tiles * 128;
+  // chunk-invariant buffers first: the weight images are packed once per call into the first chunk's carve
+  const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
+  const size_t max_k = (size_t)c->net_width + (d.xyz_dim > d.view_dim ? d.xyz_dim : d.view_dim) + 1;
+  s.part = take((size_t)mipnerf::kWgradMaxSlices * max_n * max_k);
+  s.images = take_bytes((size_t)(kMaxTrainDepth + 2) * kTrainImageBytes);
+  s.packed = take_bytes(mipnerf::tc_packed_bytes(c, MIPNERF_B200_BF16));
+  s.slots_bytes = radiance ? mipnerf::tc_radiance_workspace_bytes(mipnerf::kDensityChunkPoints) : 0;
+  s.slots = reinterpret_cast<float*>(take_bytes(s.slots_bytes));
+  s.act = take_bytes((size_t)(radiance ? 9 : 8) * tiles * 65536);
+  s.raw_density = take((size_t)rows);
+  s.d_raw_density = take((size_t)rows);
+  s.enc16 = take_bytes((size_t)tiles * 32768);
+  s.relu_bits = take_bytes((size_t)rows * 32);
+  s.d_a = take_bytes((size_t)tiles * 65536);
+  s.d_b = take_bytes((size_t)tiles * 65536);
+  if (radiance) {
+    s.v = take_bytes((size_t)tiles * 32768);
+    s.raw_rgb = take((size_t)rows * 3);
+    s.d_raw_rgb = take((size_t)rows * 3);
+    s.venc = take((size_t)rows * d.view_dim);
+    s.d_v = take_bytes((size_t)tiles * 32768);
+  }
+  s.bytes = off;
+  return s;
+}
+
+// The configs the query backward takes: those of the training chain, and on the tensor cores (BF16) the default
+// architecture and encodings (the tile images of the fused step's chain carry the full 96 / 27 encodings).
+bool query_grad_supported(const mipnerf_b200_config* c, const Dims& d, int precision) {
+  if (check_train_config(c) != MIPNERF_B200_OK) return false;
+  if (precision == MIPNERF_B200_FP32) return true;
+  return precision == MIPNERF_B200_BF16 && mipnerf::tc_supported(c, precision) && mipnerf::tc_default_degrees(c) &&
+         c->net_depth == 8 && train_tc_supported(c, d);
+}
+
+// The cotangents of chunk [off, off + m) (radiance: all four; density: the density ones)
+mipnerf::QueryCot chunk_cot(const mipnerf_b200_query_cotangent* cot, int64_t off, bool radiance) {
+  return mipnerf::QueryCot{radiance && cot->d_raw_rgb ? cot->d_raw_rgb + off * 3 : nullptr,
+                           cot->d_raw_density ? cot->d_raw_density + off : nullptr,
+                           radiance && cot->d_rgb ? cot->d_rgb + off * 3 : nullptr,
+                           cot->d_density ? cot->d_density + off : nullptr};
+}
+
+// fp32: the IPE stage kernel, pos_enc, the fp32 MLP with its activations kept and the per-layer chain
+int query_backward_fp32(const mipnerf_b200_config* cfg, const Dims& d, const mipnerf_b200_weights* w,
+                        const float* means, const float* covs, const float* viewdirs, int64_t num_points,
+                        const mipnerf_b200_query_cotangent* cot, const mipnerf_b200_linear_grad* grads, bool* touched,
+                        void* workspace, cudaStream_t st) {
+  const bool radiance = viewdirs != nullptr;
+  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const LayerImages im{};
+  int rc;
+  for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
+    const int64_t m = (num_points - off) < kChunkPointsFp32 ? (num_points - off) : kChunkPointsFp32;
+    const QueryGradScratch s = carve_query_grad(cfg, d, m, radiance, workspace);
+    // the forward of the query (models/mip.py:322-363, models/mip_nerf.py:75-111), every activation kept
+    const float* cv = covs ? covs + off * 3 : nullptr;
+    if (!cv || cfg->disable_integration) {
+      CUDA_TRY(cudaMemsetAsync(s.zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
+      cv = s.zero_covs;
+    }
+    CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, s.t.enc, m, cfg->min_deg_point, cfg->max_deg_point, st));
+    if (radiance) CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, s.t.venc, m, 0, cfg->deg_view, 1, st));
+    if ((rc = mlp_forward_kept(cfg, d, w, false, MIPNERF_B200_FP32, im, s.t, m, 1, !radiance, st))) return rc;
+    // the activations' VJP, then the training step's per-layer chain
+    CUDA_TRY(mipnerf::launch_query_activation_vjp(s.t.raw_rgb, s.t.raw_density, chunk_cot(cot, off, radiance),
+                                                  cfg->density_bias, rgb_scale, radiance ? s.t.d_raw_rgb : nullptr,
+                                                  s.t.d_raw_density, m, st));
+    if ((rc = mlp_backward_chain(cfg, d, w, false, MIPNERF_B200_FP32, im, s.t, m, 1, !radiance, grads, touched, st)))
+      return rc;
+  }
+  return MIPNERF_B200_OK;
+}
+
+// bf16: the query itself on the level kernel with the training dump (its outputs are the raw heads the VJP takes the
+// activations' derivatives at), the IPE of the points as a tile image, then the fused training step's tile-image chain
+int query_backward_bf16(const mipnerf_b200_config* cfg, const Dims& d, const mipnerf_b200_weights* w,
+                        const float* means, const float* covs, const float* viewdirs, int64_t num_points,
+                        const mipnerf_b200_query_cotangent* cot, const mipnerf_b200_linear_grad* grads, bool* touched,
+                        void* workspace, cudaStream_t st) {
+  const bool radiance = viewdirs != nullptr;
+  const int prec = MIPNERF_B200_BF16;
+  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const int64_t chunk = mipnerf::kDensityChunkPoints;
+  const QueryFusedScratch s0 = carve_query_fused(cfg, d, num_points < chunk ? num_points : chunk, radiance, workspace);
+  mipnerf_b200_weights wl = *w;
+  wl.packed = s0.packed, wl.packed_precision = prec, wl.packed_bytes = mipnerf::tc_packed_bytes(cfg, prec);
+  CUDA_TRY(mipnerf::tc_pack_weights(cfg, w, prec, s0.packed, st));
+  const uint8_t* img_bwd[kMaxTrainDepth + 2] = {nullptr};
+  const uint8_t* img_bwd_lo[kMaxTrainDepth + 2] = {nullptr};
+  CUDA_TRY(pack_bwd_images(cfg, w, prec, s0.images, img_bwd, img_bwd_lo, st));
+  int rc;
+  for (int64_t off = 0; off < num_points; off += chunk) {
+    const int64_t m = (num_points - off) < chunk ? (num_points - off) : chunk;
+    const int64_t tiles = (m + 127) / 128, rows = tiles * 128;
+    const QueryFusedScratch s = carve_query_fused(cfg, d, m, radiance, workspace);
+    const float* mp = means + off * 3;
+    const float* cv = covs ? covs + off * 3 : nullptr;
+    const mipnerf::TcQueryDump dump{s.act, s.v};
+    cudaError_t e = radiance ? mipnerf::tc_query_radiance(cfg, &wl, mp, cv, viewdirs + off * 3, m, prec, s.raw_rgb,
+                                                          s.raw_density, nullptr, nullptr, s0.slots, s0.slots_bytes, st,
+                                                          &dump)
+                             : mipnerf::tc_query_density(cfg, &wl, mp, cv, m, prec, s.raw_density, nullptr, st, &dump);
+    if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "query backward, forward: %s", cudaGetErrorString(e));
+    CUDA_TRY(mipnerf::launch_ipe_points_t16(mp, cv, s.enc16, m, cfg->disable_integration, prec, st));
+    if (radiance) {
+      CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, s.venc, m, 0, cfg->deg_view, 1, st));
+      if (rows > m) CUDA_TRY(cudaMemsetAsync(s.venc + m * d.view_dim, 0, (size_t)(rows - m) * d.view_dim * 4, st));
+    }
+    // the activations' VJP; the rows of the last tile past the last point take no cotangent
+    CUDA_TRY(mipnerf::launch_query_activation_vjp(s.raw_rgb, s.raw_density, chunk_cot(cot, off, radiance),
+                                                  cfg->density_bias, rgb_scale, radiance ? s.d_raw_rgb : nullptr,
+                                                  s.d_raw_density, m, st));
+    if (rows > m) {
+      CUDA_TRY(cudaMemsetAsync(s.d_raw_density + m, 0, (size_t)(rows - m) * 4, st));
+      if (radiance) CUDA_TRY(cudaMemsetAsync(s.d_raw_rgb + m * 3, 0, (size_t)(rows - m) * 12, st));
+    }
+    const TileChainOps ops{s.act, s.v, s.enc16, s.venc, 1, s.d_raw_rgb, s.d_raw_density,
+                           s.d_v, s.d_a, s.d_b, s.relu_bits, s0.part, tiles};
+    if ((rc = tile_backward_chain(cfg, d, w, prec, img_bwd, img_bwd_lo, ops, !radiance, 1.f, grads, touched, st)))
+      return rc;
+  }
+  return MIPNERF_B200_OK;
+}
+}  // namespace
+
+size_t mipnerf_b200_query_backward_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points, int radiance,
+                                                   int precision) {
+  Dims d;
+  if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0 || !query_grad_supported(cfg, d, precision)) return 0;
+  const int64_t m = num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32;
+  if (precision == MIPNERF_B200_BF16) return carve_query_fused(cfg, d, m > 0 ? m : 1, radiance != 0, nullptr).bytes;
+  return carve_query_grad(cfg, d, m > 0 ? m : 1, radiance != 0, nullptr).bytes;
+}
+
+int mipnerf_b200_query_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                                const float* covs, const float* viewdirs, int64_t num_points, int precision,
+                                const mipnerf_b200_query_cotangent* cot, const mipnerf_b200_linear_grad* grads,
+                                int num_grads, int accumulate, void* workspace, size_t workspace_bytes, void* stream) {
+  Dims d;
+  int rc;
+  if ((rc = check_config(cfg, &d))) return rc;
+  if ((rc = check_weights(cfg, d, w))) return rc;
+  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if (!cot || !grads) return fail(MIPNERF_B200_EINVAL, "cot / grads is NULL");
+  if (num_grads != d.n_lin) return fail(MIPNERF_B200_EINVAL, "expected %d gradient pairs, got %d", d.n_lin, num_grads);
+  for (int i = 0; i < d.n_lin; ++i)
+    if (!grads[i].weight_grad || !grads[i].bias_grad) return fail(MIPNERF_B200_EINVAL, "grads[%d] has a NULL tensor", i);
+  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
+  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
+    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
+  if (precision == MIPNERF_B200_FP16)
+    return fail(MIPNERF_B200_EUNSUPPORTED,
+                "query backward: FP16's fixed gradient scale is sized for the training loss and arbitrary cotangents "
+                "can overflow or underflow it; use BF16 (fp32 range) or FP32");
+  if (precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "query backward: the split-operand precisions are forward-only; use FP32 or BF16");
+  if ((rc = check_train_config(cfg))) return rc;
+  if (!query_grad_supported(cfg, d, precision))
+    return fail(MIPNERF_B200_EUNSUPPORTED,
+                "query backward in BF16: the 8x256 / 1x128 MLP with max_deg_point=16, deg_view=4 only; use FP32");
+  const bool radiance = viewdirs != nullptr;
+  const size_t need = mipnerf_b200_query_backward_workspace_bytes(cfg, num_points, radiance, precision);
+  if (num_points > 0 && (!workspace || workspace_bytes < need))
+    return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  bool touched[kMaxTrainDepth + 8];
+  for (int i = 0; i < d.n_lin; ++i) touched[i] = accumulate != 0;
+  if (num_points > 0) {
+    rc = precision == MIPNERF_B200_BF16
+             ? query_backward_bf16(cfg, d, w, means, covs, viewdirs, num_points, cot, grads, touched, workspace, st)
+             : query_backward_fp32(cfg, d, w, means, covs, viewdirs, num_points, cot, grads, touched, workspace, st);
+    if (rc) return rc;
+  }
+  for (int i = 0; i < d.n_lin; ++i)  // no points, or the heads a density query does not reach: exact zeros
+    if (!touched[i]) {
+      const mipnerf_b200_linear& l = w->linears[i];
+      CUDA_TRY(cudaMemsetAsync(grads[i].weight_grad, 0, sizeof(float) * l.in_features * l.out_features, st));
+      CUDA_TRY(cudaMemsetAsync(grads[i].bias_grad, 0, sizeof(float) * l.out_features, st));
+    }
   return MIPNERF_B200_OK;
 }
 

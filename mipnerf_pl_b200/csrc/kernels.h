@@ -94,6 +94,14 @@ cudaError_t launch_render_vjp(const float* raw_rgb, const float* raw_dens, const
                               const RenderCot& cot, int white_bkgd, float density_bias, float rgb_scale,
                               float rgb_padding, float* d_raw_rgb, float* d_raw_dens, int64_t num_rays, int n,
                               cudaStream_t st);
+// cotangents of a field query's outputs (raw heads [P,3] / [P] and activated rgb / density), NULL = zero
+struct QueryCot {
+  const float *d_raw_rgb, *d_raw_density, *d_rgb, *d_density;
+};
+// d raw_rgb / d raw_density of  <cot, (raw_rgb, raw_density, rgb, density)>  of m points; d_raw_rgb null: density only
+cudaError_t launch_query_activation_vjp(const float* raw_rgb, const float* raw_dens, const QueryCot& cot,
+                                        float density_bias, float rgb_scale, float* d_raw_rgb, float* d_raw_dens,
+                                        int64_t m, cudaStream_t st);
 cudaError_t launch_color_dgrad(const float* d_rgb, const float* wc, const float* v, float* d_v, int64_t m,
                                int k_dim, cudaStream_t st);
 // dX[m,k] = (act[m,k] > 0 or act == NULL) * (dY[m,:n_dim] @ W[:n_dim, :k_dim] (row stride ldw) + r1[m] * r1w[k])
@@ -152,6 +160,10 @@ cudaError_t launch_t16_pack(const float* src, int ld, int cols, int64_t m, void*
 cudaError_t launch_ipe_t16(const float* origins, const float* directions, const float* radii, const float* t, void* image,
                            int64_t num_rays, int n, int disable_integration, int precision, cudaStream_t st,
                            void* image_lo = nullptr);
+// the IPE of query points [num_points, 3] (covs null: zero) as a tile image, whole tiles (rows past num_points: the IPE
+// of a zero Gaussian), with the query modes' ipe_pair<false>
+cudaError_t launch_ipe_points_t16(const float* means, const float* covs, void* image, int64_t num_points,
+                                  int disable_integration, int precision, cudaStream_t st);
 // image_lo: dst = hi + lo
 cudaError_t launch_t16_unpack(const void* image, int cols, float* dst, int ld, int64_t m, int precision,
                               cudaStream_t st, const void* image_lo = nullptr);

@@ -1028,11 +1028,17 @@ __device__ __forceinline__ void level_radiance_out(const LevelParams& p, int64_t
 // kTrain (bf16x3 / fp16x3 forward with the training dump only): the dump also carries the lo halves of the split
 // activation tiles, at act_dump + 9 dump_tiles 64 KB (same [9][dump_tiles] layout), and of the view-layer output, at
 // v_dump + dump_tiles 32 KB.  A compile-time flag, so that the inference instantiations carry none of it.
-template <int kFmt, bool kX3, int kT, int kMode = kModeForward, bool kTrain = false>
+// kQueryDump (bf16 / fp16 query modes, the backward of a query only): the query tiles leave the training forward's dump,
+// tile = query tile of the launch: h_0..h_7 (density mode: h_7 from layer 7's epilogue, which otherwise only finishes
+// the density head) and, in radiance mode, the bottleneck into act_dump, the view-layer output into v_dump.  The raw
+// heads are the query's own outputs.  Rows past the last point hold the features of a zero Gaussian: finite.
+template <int kFmt, bool kX3, int kT, int kMode = kModeForward, bool kTrain = false, bool kQueryDump = false>
 __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParams p) {
   static_assert(!kTrain || (kX3 && kT == 1 && kMode == kModeForward), "the split training forward: 128 samples");
+  static_assert(!kQueryDump || (!kX3 && kT == 1 && kMode != kModeForward), "the 16-bit query modes' dump");
   constexpr bool kDensity = kMode == kModeDensity;
-  constexpr bool kQuery = kMode != kModeForward;  // density or radiance: 128 query points per tile, no dumps
+  constexpr bool kQuery = kMode != kModeForward;  // density or radiance: 128 query points per tile
+  constexpr bool kDumps = !kQuery || kQueryDump;  // the training dump (p.act_dump, p.v_dump) may be set
   static_assert(!kQuery || kT == 1, "the query modes take one 128-point tile at a time");
   using Lay = LevelLayout<kX3, kT>;
   extern __shared__ uint8_t smem_raw[];
@@ -1158,7 +1164,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
   const uint32_t a_u = smem_u32(sA) + (uint32_t)wg * 64u * 128u;
   const uint32_t w_u = smem_u32(sW);
   // the training forward's dump (p.act_dump, p.v_dump) exists for kT = 1 only
-  const uint64_t dump_policy = kMode != kModeRadiance && kT == 1 && p.act_dump ? l2_policy_evict_first() : 0ull;  // must not evict the weights
+  const uint64_t dump_policy =
+      (kMode != kModeRadiance || kQueryDump) && kT == 1 && p.act_dump ? l2_policy_evict_first() : 0ull;  // must not evict the weights
   bool dump_pending = false;
   RingPos rp{0, 0u, -1};
   clk.begin(phase_rows + wg * kNumPhases, leader);
@@ -1207,7 +1214,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       // feature tile; layer 0 has two K-slabs (64 wide + the 32-wide tail), and two of its acc0 chunks follow each.  The
       // training forward's activation tiles go out from the epilogue's registers.
       const LevelRsCtx k{f_u, ft_u, w_u, w_full, w_empty, &feat_empty[fb], gsp,
-                         !kQuery && kT == 1 && p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
+                         kDumps && kT == 1 && p.act_dump ? p.act_dump + (size_t)ray * kABytes : nullptr,
                          (size_t)p.dump_tiles * kABytes, dump_policy, r0, cq, leader};
       uint32_t xa[64], xb[64];
       static_assert(2 * num_slabs(true, 0) == kEpiChunks, "layer 0: two acc0 chunks after each of its K-slabs");
@@ -1348,7 +1355,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
       // view layer + colour head (models/mip_nerf.py:106-110); view bias = the per-ray view-direction term (radiance
       // mode: row r0 of the tile's global slot; row r0 + 8 adds its own term b1)
       const float* vb = p.view_bias + ((size_t)blockIdx.x * 2 + par) * (kN * kCond) + (size_t)r0 * kCond;
-      uint8_t* vd = !kQuery && kT == 1 && p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
+      uint8_t* vd = kDumps && kT == 1 && p.v_dump ? p.v_dump + (size_t)ray * (2 * kStageBytes) : nullptr;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int c = 8 * j + cq;
@@ -1596,9 +1603,9 @@ int num_sms() {
   return g_num_sms;
 }
 
-template <int kFmt, bool kX3, int kT, int kMode = kModeForward, bool kTrain = false>
+template <int kFmt, bool kX3, int kT, int kMode = kModeForward, bool kTrain = false, bool kQueryDump = false>
 cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
-  auto kern = mlp_level_kernel<kFmt, kX3, kT, kMode, kTrain>;
+  auto kern = mlp_level_kernel<kFmt, kX3, kT, kMode, kTrain, kQueryDump>;
   constexpr uint32_t smem = LevelLayout<kX3, kT>::kTotal;
   static bool attr_set = false;  // one flag per instantiation
   if (!attr_set) {
@@ -1629,6 +1636,9 @@ cudaError_t launch_level(const LevelParams& p, int precision, int n, cudaStream_
 }
 cudaError_t launch_density(const LevelParams& p, int precision, cudaStream_t st) {
   if (p.num_rays <= 0) return cudaSuccess;
+  if (p.act_dump)  // the backward of a query: bf16 / fp16 only (tc_query_density)
+    return fmt_of(precision) ? launch_level_t<1, false, 1, kModeDensity, false, true>(p, st)
+                             : launch_level_t<0, false, 1, kModeDensity, false, true>(p, st);
   if (is_x3(precision))
     return fmt_of(precision) ? launch_level_t<1, true, 1, kModeDensity>(p, st)
                              : launch_level_t<0, true, 1, kModeDensity>(p, st);
@@ -1637,6 +1647,9 @@ cudaError_t launch_density(const LevelParams& p, int precision, cudaStream_t st)
 }
 cudaError_t launch_radiance(const LevelParams& p, int precision, cudaStream_t st) {
   if (p.num_rays <= 0) return cudaSuccess;
+  if (p.act_dump)
+    return fmt_of(precision) ? launch_level_t<1, false, 1, kModeRadiance, false, true>(p, st)
+                             : launch_level_t<0, false, 1, kModeRadiance, false, true>(p, st);
   if (is_x3(precision))
     return fmt_of(precision) ? launch_level_t<1, true, 1, kModeRadiance>(p, st)
                              : launch_level_t<0, true, 1, kModeRadiance>(p, st);
@@ -1872,7 +1885,8 @@ cudaError_t tc_mlp_forward(const mipnerf_b200_config* c, const mipnerf_b200_weig
 
 cudaError_t tc_query_density(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, const float* means,
                              const float* covs, int64_t num_points, int precision, float* raw_density, float* density,
-                             cudaStream_t st) {
+                             cudaStream_t st, const TcQueryDump* dump) {
+  if (dump && (is_x3(precision) || num_points > kDensityChunkPoints)) return cudaErrorInvalidValue;
   const uint8_t* img = static_cast<const uint8_t*>(w->packed);
   SmallUpload small(img, st);
   cudaError_t e = small.error();
@@ -1889,6 +1903,7 @@ cudaError_t tc_query_density(const mipnerf_b200_config* c, const mipnerf_b200_we
     p.density_out = density ? density + off : nullptr;
     p.disable_integration = c->disable_integration;
     p.density_bias = c->density_bias;
+    if (dump) p.act_dump = dump->act, p.dump_tiles = p.num_rays;
     if ((e = launch_density(p, precision, st)) != cudaSuccess) return e;
   }
   return cudaSuccess;
@@ -1901,8 +1916,9 @@ size_t tc_radiance_workspace_bytes(int64_t num_points) {
 cudaError_t tc_query_radiance(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, const float* means,
                               const float* covs, const float* viewdirs, int64_t num_points, int precision,
                               float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
-                              size_t workspace_bytes, cudaStream_t st) {
+                              size_t workspace_bytes, cudaStream_t st, const TcQueryDump* dump) {
   if (workspace_bytes < tc_radiance_workspace_bytes(num_points)) return cudaErrorInvalidValue;
+  if (dump && (is_x3(precision) || num_points > kDensityChunkPoints)) return cudaErrorInvalidValue;
   const uint8_t* img = static_cast<const uint8_t*>(w->packed);
   SmallUpload small(img, st);
   cudaError_t e = small.error();
@@ -1925,6 +1941,7 @@ cudaError_t tc_query_radiance(const mipnerf_b200_config* c, const mipnerf_b200_w
     p.density_bias = c->density_bias;
     p.rgb_scale = (float)(1.0 + 2.0 * (double)c->rgb_padding);
     p.rgb_padding = c->rgb_padding;
+    if (dump) p.act_dump = dump->act, p.v_dump = dump->v, p.dump_tiles = p.num_rays;
     if ((e = launch_radiance(p, precision, st)) != cudaSuccess) return e;
   }
   return cudaSuccess;

@@ -45,9 +45,16 @@ size_t tc_mlp_workspace_bytes(int64_t num_rays);
 // Density-only mode of the level kernels (mipnerf_b200_query_density), kDensityChunkPoints points per launch; needs
 // tc_supported(cfg, precision) and w->packed for that precision.
 constexpr int64_t kDensityChunkPoints = 4096 * 128;
+// The backward of a query: the query's tiles leave the training forward's dump (bf16 / fp16, at most one chunk of
+// points per call; tile = query tile): act [layers][tiles][64 KB] with h_0..h_7 and, in radiance mode, the bottleneck;
+// v [tiles][32 KB], the view-layer output (radiance mode).
+struct TcQueryDump {
+  uint8_t* act;
+  uint8_t* v;
+};
 cudaError_t tc_query_density(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
                              const float* covs, int64_t num_points, int precision, float* raw_density, float* density,
-                             cudaStream_t st);
+                             cudaStream_t st, const TcQueryDump* dump = nullptr);
 // Radiance mode of the level kernels (mipnerf_b200_query_radiance), launched in the same chunks as the density query.
 // The workspace is two [128][128] fp32 slots of view-direction terms per CTA of a launch, min(tiles, SMs) CTAs with
 // tiles = ceil(points / 128) capped at one chunk's 4096.
@@ -55,6 +62,6 @@ size_t tc_radiance_workspace_bytes(int64_t num_points);
 cudaError_t tc_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
                               const float* covs, const float* viewdirs, int64_t num_points, int precision,
                               float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
-                              size_t workspace_bytes, cudaStream_t st);
+                              size_t workspace_bytes, cudaStream_t st, const TcQueryDump* dump = nullptr);
 
 }  // namespace mipnerf

@@ -36,6 +36,11 @@ inline unsigned blocks_of(int64_t n, int per_block) { return (unsigned)((n + per
 // distloss (models/mip.py:8-20) with sorted midpoints:  d/dw_i = (2/3) len_i w_i + 2 S_i,
 //   S_i = sum_j w_j |m_i - m_j| = m_i (W_<i - W_>i) - (M_<i - M_>i)      (two prefix sums)
 // -------------------------------------------------------------------------------------------------
+// The activations' derivatives, shared by the render backward and the query VJP: sigmoid (rgb = sigmoid(raw) (1+2p) - p)
+// and softplus' at x = raw_density + density_bias, with torch's threshold 20 (models/mip_nerf.py:236-237).
+__device__ __forceinline__ float sigmoid_f32(float raw) { return 1.0f / (1.0f + expf(-raw)); }
+__device__ __forceinline__ float softplus_grad(float x) { return x > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-x)); }
+
 // kCot = false: (g, gw) come from the training loss above.  kCot = true (render VJP): from arbitrary cotangents of
 // the outputs (comp_rgb, distance, acc, weights), any of them NULL = zero:
 //   g = d comp_rgb,  gw_i = d w_i + g . rgb_i - [white_bkgd] sum_c g_c + d acc + g_D tmid_i,
@@ -70,7 +75,7 @@ __global__ void render_backward_kernel(const float* __restrict__ raw_rgb, const 
   for (int p = 0; p < P; ++p) {
     const float x = __ldg(raw_dens + ray * N + lane * P + p) + density_bias;
     const float dens = x > 20.0f ? x : log1pf(expf(x));
-    dsig[p] = x > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-x));  // softplus'
+    dsig[p] = softplus_grad(x);
     delta[p] = __fmul_rn(__fsub_rn(tt[p + 1], tt[p]), dnorm);
     dd[p] = __fmul_rn(dens, delta[p]);
     run += (double)dd[p];
@@ -89,7 +94,7 @@ __global__ void render_backward_kernel(const float* __restrict__ raw_rgb, const 
     const int64_t s = ray * N + lane * P + p;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float sg = 1.0f / (1.0f + expf(-__ldg(raw_rgb + s * 3 + c)));
+      const float sg = sigmoid_f32(__ldg(raw_rgb + s * 3 + c));
       srgb[p][c] = sg;
       rgb[p][c] = sg * rgb_scale - rgb_padding;
     }
@@ -237,6 +242,43 @@ cudaError_t launch_render_vjp(const float* raw_rgb, const float* raw_dens, const
   return launch_render_grad<true>(raw_rgb, raw_dens, t, dirs, nullptr, nullptr, nullptr, 0.f, 0.f, white_bkgd,
                                   density_bias, rgb_scale, rgb_padding, d_raw_rgb, d_raw_dens, nullptr, nullptr, cot,
                                   num_rays, n, st);
+}
+
+// -------------------------------------------------------------------------------------------------
+// VJP of a field query's activations, one thread per point (any cotangent NULL = zero):
+//   d raw_rgb     = cot.d_raw_rgb + cot.d_rgb * (1+2p) sigmoid'(raw_rgb)
+//   d raw_density = cot.d_raw_density + cot.d_density * softplus'(raw_density + density_bias)
+// d_raw_rgb null: a density query (raw_rgb is not read).
+// -------------------------------------------------------------------------------------------------
+__global__ void query_activation_vjp_kernel(const float* __restrict__ raw_rgb, const float* __restrict__ raw_dens,
+                                            QueryCot cot, float density_bias, float rgb_scale,
+                                            float* __restrict__ d_raw_rgb, float* __restrict__ d_raw_dens, int64_t m) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  if (d_raw_rgb) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float g = cot.d_raw_rgb ? __ldg(cot.d_raw_rgb + i * 3 + c) : 0.f;
+      if (cot.d_rgb) {
+        const float sg = sigmoid_f32(__ldg(raw_rgb + i * 3 + c));
+        g += __ldg(cot.d_rgb + i * 3 + c) * rgb_scale * sg * (1.0f - sg);
+      }
+      d_raw_rgb[i * 3 + c] = g;
+    }
+  }
+  float g = cot.d_raw_density ? __ldg(cot.d_raw_density + i) : 0.f;
+  if (cot.d_density) g += __ldg(cot.d_density + i) * softplus_grad(__ldg(raw_dens + i) + density_bias);
+  d_raw_dens[i] = g;
+}
+
+cudaError_t launch_query_activation_vjp(const float* raw_rgb, const float* raw_dens, const QueryCot& cot,
+                                        float density_bias, float rgb_scale, float* d_raw_rgb, float* d_raw_dens,
+                                        int64_t m, cudaStream_t st) {
+  if (m == 0) return cudaSuccess;
+  LaunchScope scope(kKernRenderBackward, st);
+  query_activation_vjp_kernel<<<blocks_of(m, 256), 256, 0, st>>>(raw_rgb, raw_dens, cot, density_bias, rgb_scale,
+                                                                 d_raw_rgb, d_raw_dens, m);
+  return cudaGetLastError();
 }
 
 // -------------------------------------------------------------------------------------------------

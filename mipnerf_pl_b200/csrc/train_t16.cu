@@ -462,6 +462,49 @@ __global__ void __launch_bounds__(256) ipe_t16_kernel(const float* __restrict__ 
       make_uint4(pack2<kFmt>(fc[0], fc[1]), pack2<kFmt>(fc[2], fc[3]), pack2<kFmt>(fc[4], fc[5]), pack2<kFmt>(fc[6], fc[7]));
 }
 
+// The sibling for query points (the backward of the level kernel's query modes): row p of the image is the IPE of
+// Gaussian p of means / covs [num_points, 3] (covs null or disable_integration: zero covariance), with ipe_pair<false>
+// as the query modes' helper warps (mlp_tc.cu: ipe_row_group<.., kDensity = true>) compute it, so these are bit for bit
+// the features the query multiplied with.  Rows past num_points up to the last whole tile are the IPE of a zero
+// Gaussian, as in the query's feature tile: finite.  Thread layout as ipe_t16_kernel.
+template <int kFmt>
+__global__ void __launch_bounds__(256) ipe_points_t16_kernel(const float* __restrict__ means,
+                                                             const float* __restrict__ covs, uint8_t* __restrict__ out,
+                                                             int64_t num_points, int64_t padded_rows,
+                                                             int disable_integration) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= padded_rows * 8) return;
+  const int64_t p = idx >> 3;
+  const int k = (int)(idx & 7);
+  const int r = (int)(p & 127);
+  uint8_t* tile = out + (size_t)(p >> 7) * (2 * kSlab) + (uint32_t)r * 128u;
+  const uint32_t rx = (uint32_t)r & 7u;
+  auto chunk_ptr = [&](int ch) { return tile + (size_t)(ch >> 3) * kSlab + ((((uint32_t)ch & 7u) ^ rx) << 4); };
+  if (k >= 6) {
+    *reinterpret_cast<uint4*>(chunk_ptr(12 + 2 * (k - 6))) = make_uint4(0u, 0u, 0u, 0u);
+    *reinterpret_cast<uint4*>(chunk_ptr(13 + 2 * (k - 6))) = make_uint4(0u, 0u, 0u, 0u);
+    return;
+  }
+  float mean[3] = {0.f, 0.f, 0.f}, cov[3] = {0.f, 0.f, 0.f};
+  if (p < num_points) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      mean[c] = __ldg(means + p * 3 + c);
+      cov[c] = covs && !disable_integration ? __ldg(covs + p * 3 + c) : 0.f;
+    }
+  }
+  float fs[8], fc[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const int f = k * 8 + e;  // feature index = degree * 3 + coord   (models/mip.py:335-341)
+    ipe_pair<false>(mean[f % 3], cov[f % 3], f / 3, fs[e], fc[e]);
+  }
+  *reinterpret_cast<uint4*>(chunk_ptr(k)) =
+      make_uint4(pack2<kFmt>(fs[0], fs[1]), pack2<kFmt>(fs[2], fs[3]), pack2<kFmt>(fs[4], fs[5]), pack2<kFmt>(fs[6], fs[7]));
+  *reinterpret_cast<uint4*>(chunk_ptr(6 + k)) =
+      make_uint4(pack2<kFmt>(fc[0], fc[1]), pack2<kFmt>(fc[2], fc[3]), pack2<kFmt>(fc[4], fc[5]), pack2<kFmt>(fc[6], fc[7]));
+}
+
 // fp32 row-major [m, cols] (ld) <-> tile image; rows beyond m / columns beyond cols are zero in the image.
 // thread = (row, 16-byte chunk of 8 columns): two float4 loads when the source allows it, one 16-byte store
 template <int kFmt>
@@ -551,6 +594,21 @@ cudaError_t launch_ipe_t16(const float* origins, const float* directions, const 
   else
     ipe_t16_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(origins, directions, radii, t, (uint8_t*)image, num_rays, n,
                                                               disable_integration);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ipe_points_t16(const float* means, const float* covs, void* image, int64_t num_points,
+                                  int disable_integration, int precision, cudaStream_t st) {
+  const int64_t padded = (num_points + 127) / 128 * 128;
+  if (padded == 0) return cudaSuccess;
+  LaunchScope scope(kKernIpe, st);
+  const int64_t total = padded * 8;
+  if (precision == 1)
+    ipe_points_t16_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(means, covs, (uint8_t*)image, num_points, padded,
+                                                                     disable_integration);
+  else
+    ipe_points_t16_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(means, covs, (uint8_t*)image, num_points, padded,
+                                                                     disable_integration);
   return cudaGetLastError();
 }
 

@@ -45,12 +45,14 @@ def lattice_axes(resolution: Resolution, bounds=DEFAULT_BOUNDS, device="cuda"):
     return axes, step
 
 
+@torch.no_grad()
 def density_grid(model, resolution: Resolution, bounds=DEFAULT_BOUNDS, variance=None,
                  slab_points: int = 1 << 22) -> torch.Tensor:
     """Density (softplus(raw + density_bias)) of `model` on a lattice -> [nz, ny, nx] on the model's device.  Point
     (i, j, k) sits at lo + (i, j, k) * step; `variance` (a float or one per axis) is the diagonal covariance of every
     query, by default step**2 / 12 per axis; 0 gives a point-sampled grid.  Queried in z-slabs of at most
-    `slab_points` points, so that the memory beyond the grid stays bounded."""
+    `slab_points` points, so that the memory beyond the grid stays bounded.  Under no_grad: no graph, even on an
+    autograd model."""
     dev = next(model.parameters()).device
     nx, ny, nz = _resolution(resolution)
     (xs, ys, zs), step = lattice_axes((nx, ny, nz), bounds, dev)
@@ -107,10 +109,11 @@ def isosurface(grid: torch.Tensor, iso: float, bounds=DEFAULT_BOUNDS, normals: b
     return verts, faces, nrm
 
 
+@torch.no_grad()
 def mesh_colors(model, verts: torch.Tensor, normals: torch.Tensor, variance, slab_points: int = 1 << 22) -> torch.Tensor:
     """The colour [V,3] of `model` at mesh vertices: the radiance (`MipNerf.query_radiance`) of each vertex's Gaussian
     (diagonal `variance`, a float or one per axis, e.g. the voxel's step**2 / 12) seen along -normal, a ray arriving at
-    the surface from outside.  Queried in chunks of at most `slab_points` vertices."""
+    the surface from outside.  Queried in chunks of at most `slab_points` vertices, under no_grad."""
     dev = next(model.parameters()).device
     v = _f32(verts).to(dev).reshape(-1, 3)
     d = -_f32(normals).to(dev).reshape(-1, 3)

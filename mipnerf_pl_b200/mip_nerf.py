@@ -275,20 +275,34 @@ class MipNerf(torch.nn.Module):
         every level carry a `grad_fn` over the MLP tensors (values identical: the same launches run); t_samples and
         inds are constants (stop_resample_grad) and `.pixels` has no grad.  fp32 and bf16 only; ray tensors that
         require grad are refused."""
-        if self.autograd and torch.is_grad_enabled() and any(p.requires_grad for p in self.mlp.parameters()):
+        if self._builds_graph():
             return _forward_with_grad(self, rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds)
         return self._forward(rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds)[0]
 
-    @torch.no_grad()
+    def _builds_graph(self) -> bool:
+        """`forward` and the queries return outputs with a grad_fn: autograd=True, grad mode on, and some MLP
+        parameter that requires grad."""
+        return self.autograd and torch.is_grad_enabled() and any(p.requires_grad for p in self.mlp.parameters())
+
     def query_density(self, means: torch.Tensor, covs: Optional[torch.Tensor] = None, *, raw: bool = False):
         """Density of the field at Gaussians: means / diagonal covs [..., 3] (covs None: zero covariance) -> [...] on
         `self.precision`: the IPE (models/mip.py:322-350), trunk and density_layer of MLP.forward
-        (models/mip_nerf.py:93-98), then softplus(raw + density_bias) unless `raw` (no density noise).  The result has
-        no grad_fn.  The tensor-core precisions take the configs `forward` takes on the tensor cores; fp32 any."""
-        dev = _dev(means)
+        (models/mip_nerf.py:93-98), then softplus(raw + density_bias) unless `raw` (no density noise).  The tensor-core
+        precisions take the configs `forward` takes on the tensor cores; fp32 any.
+
+        With `autograd=True`, grad mode on and a parameter that requires grad, the result carries a `grad_fn` over the
+        24 MLP tensors (same values: the same launches run); its backward is `mipnerf_b200_query_backward`.  fp32 and
+        bf16 (default encodings) only; means / covs that require grad are refused.  Otherwise no grad_fn."""
         if means.shape[-1] != 3 or (covs is not None and covs.shape != means.shape):
             raise ValueError(f"means {tuple(means.shape)} / covs {None if covs is None else tuple(covs.shape)}: "
                              "need [..., 3] of the same shape")
+        if self._builds_graph():
+            return _query_with_grad(self, means, covs, None, raw)
+        with torch.no_grad():
+            return self._query_density(means, covs, raw)
+
+    def _query_density(self, means: torch.Tensor, covs: Optional[torch.Tensor], raw: bool):
+        dev = _dev(means)
         shape = means.shape[:-1]
         m = _f32(means).reshape(-1, 3)
         c = _f32(covs).reshape(-1, 3) if covs is not None else None
@@ -309,16 +323,15 @@ class MipNerf(torch.nn.Module):
                 _stream(dev)), "MipNerf.query_density")
         return out.reshape(shape)
 
-    @torch.no_grad()
     def query_radiance(self, means: torch.Tensor, covs: Optional[torch.Tensor] = None,
                        viewdirs: Optional[torch.Tensor] = None, *, raw: bool = False):
         """Radiance of the field at Gaussians, each seen from its own direction: means / diagonal covs / viewdirs
         [..., 3] -> (rgb [..., 3], density [...]) on `self.precision`: MLP.forward of the points' IPE features and view
         encodings (models/mip_nerf.py:75-111), then the activations (models/mip_nerf.py:236-237), or the raw heads
-        (raw_rgb, raw_density) when `raw`.  No density noise and no grad_fn.  viewdirs are encoded as given; the
-        reference encodes unit directions.  They may be None only for a model with use_viewdirs=False (fp32: the colour
-        head then reads the trunk).  The tensor-core precisions take the configs `forward` takes on the tensor cores
-        (the radiance mode of the level kernel); fp32 any."""
+        (raw_rgb, raw_density) when `raw`.  No density noise.  viewdirs are encoded as given; the reference encodes
+        unit directions.  They may be None only for a model with use_viewdirs=False (fp32: the colour head then reads
+        the trunk).  The tensor-core precisions take the configs `forward` takes on the tensor cores (the radiance mode
+        of the level kernel); fp32 any.  Gradients with respect to the MLP tensors as for `query_density`."""
         if (means.shape[-1] != 3 or (covs is not None and covs.shape != means.shape) or
                 (viewdirs is not None and viewdirs.shape != means.shape)):
             raise ValueError(f"means {tuple(means.shape)} / covs {None if covs is None else tuple(covs.shape)} / "
@@ -326,6 +339,13 @@ class MipNerf(torch.nn.Module):
                              "same shape")
         if viewdirs is None and self.use_viewdirs:
             raise ValueError("query_radiance: viewdirs are required when use_viewdirs=True")
+        if self._builds_graph():
+            return _query_with_grad(self, means, covs, viewdirs, raw)
+        with torch.no_grad():
+            return self._query_radiance(means, covs, viewdirs, raw)
+
+    def _query_radiance(self, means: torch.Tensor, covs: Optional[torch.Tensor], viewdirs: Optional[torch.Tensor],
+                        raw: bool):
         dev = _dev(means)
         shape = means.shape[:-1]
         m = _f32(means).reshape(-1, 3)
@@ -544,3 +564,95 @@ class _ForwardWithGrad(torch.autograd.Function):
                 _cabi.PRECISIONS[ctx.precision], cots, garr, np_ // 2, 0, scratch.data_ptr(), scratch.numel(),
                 _stream(dev)), "MipNerf.backward")
         return (None,) * 9 + tuple(out_grads)
+
+
+def _check_query_autograd(model: MipNerf, tensors, radiance: bool) -> None:
+    """Refuse, at query time, what the query backward cannot differentiate."""
+    if model.precision in ("fp16x3", "bf16x3"):
+        raise NotImplementedError(f"MipNerf(autograd=True) queries: precision={model.precision!r} is forward-only; "
+                                  "use 'fp32' or 'bf16'")
+    if model.precision == "fp16":
+        raise NotImplementedError("MipNerf(autograd=True) queries: fp16's fixed gradient scale is sized for the "
+                                  "reference loss and arbitrary losses can overflow or underflow it; use "
+                                  "precision='bf16'")
+    if model.precision not in ("fp32", "bf16"):
+        raise ValueError(f"precision={model.precision!r}")
+    if any(isinstance(x, torch.Tensor) and x.requires_grad for x in tensors):
+        raise NotImplementedError("MipNerf(autograd=True) queries: gradients with respect to means, covs or viewdirs "
+                                  "are not implemented; pass tensors that do not require grad")
+    cfg = model._config()
+    lib = _cabi.lib()
+    if lib.mipnerf_b200_query_backward_workspace_bytes(C.byref(cfg), 1, int(radiance),
+                                                       _cabi.PRECISIONS[model.precision]) == 0:
+        raise NotImplementedError("MipNerf(autograd=True) queries: the backward needs use_viewdirs=True with one view "
+                                  "layer and net_depth <= 16, and in bf16 the 8x256 / 1x128 MLP with max_deg_point=16, "
+                                  "deg_view=4; use precision='fp32' or autograd=False")
+
+
+def _query_with_grad(model: MipNerf, means, covs, viewdirs, raw: bool):
+    radiance = viewdirs is not None
+    _check_query_autograd(model, (means, covs, viewdirs), radiance)
+    shape = means.shape[:-1]
+    m = _f32(means).reshape(-1, 3)
+    c = _f32(covs).reshape(-1, 3) if covs is not None else None
+    v = _f32(viewdirs).reshape(-1, 3) if viewdirs is not None else None
+    params = [p for lin in model.mlp.linears() for p in (lin.weight, lin.bias)]
+    outs = _QueryWithGrad.apply(model, m, c, v, bool(raw), *params)
+    if not radiance:
+        return outs[0].reshape(shape)
+    return outs[0].reshape(*shape, 3), outs[1].reshape(shape)
+
+
+class _QueryWithGrad(torch.autograd.Function):
+    """query_density (viewdirs None) / query_radiance as a function of the 24 MLP tensors.  Saved: the flattened fp32
+    means, covs and viewdirs and the parameters; backward re-evaluates the field at those points with every activation
+    kept and runs the library's backward chain from the output cotangents (mipnerf_b200_query_backward)."""
+
+    @staticmethod
+    def forward(ctx, model, means, covs, viewdirs, raw, *params):
+        radiance = viewdirs is not None
+        if radiance:
+            outs = model._query_radiance(means, covs, viewdirs, raw)
+        else:
+            outs = (model._query_density(means, covs, raw),)
+        ctx.model, ctx.cfg, ctx.raw, ctx.radiance = model, model._config(), raw, radiance
+        ctx.precision, ctx.num_params = model.precision, len(params)
+        ctx.save_for_backward(means, covs, viewdirs, *params)
+        ctx.set_materialize_grads(False)
+        return outs
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *grads):
+        saved = ctx.saved_tensors  # raises if a parameter was updated in place since the forward
+        means, covs, viewdirs = saved[:3]
+        params = saved[3:]
+        np_ = ctx.num_params
+        dev = means.device
+        p = means.shape[0]
+        out_grads = [torch.empty_like(x) for x in params]
+        if all(g is None for g in grads) or p == 0:
+            return (None,) * 5 + tuple(g.zero_() for g in out_grads)
+        keep = [None if g is None else _f32(g).reshape(-1) for g in grads]
+        if ctx.radiance:
+            pair = (_ptr(keep[0]), _ptr(keep[1]))
+            cot = _cabi.QueryCotangent(*pair, None, None) if ctx.raw else _cabi.QueryCotangent(None, None, *pair)
+        else:
+            cot = _cabi.QueryCotangent(None, _ptr(keep[0]), None, None) if ctx.raw else \
+                _cabi.QueryCotangent(None, None, None, _ptr(keep[0]))
+        model, cfg = ctx.model, ctx.cfg
+        prec = _cabi.PRECISIONS[ctx.precision]
+        ws, wkeep = model.mlp._weights_struct(cfg, _cabi.FP32, dev)
+        garr = (_cabi.LinearGrad * (np_ // 2))()
+        for i in range(np_ // 2):
+            garr[i] = _cabi.LinearGrad(out_grads[2 * i].data_ptr(), out_grads[2 * i + 1].data_ptr())
+        lib = _cabi.lib()
+        nbytes = lib.mipnerf_b200_query_backward_workspace_bytes(C.byref(cfg), p, int(ctx.radiance), prec)
+        # per call, not the per-stream _Workspace: up to one chunk's activations (GBs), which a forward-only process
+        # that ran one query backward should not keep reserved for small forwards
+        scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            _cabi.check(lib.mipnerf_b200_query_backward(
+                C.byref(cfg), C.byref(ws), means.data_ptr(), _ptr(covs), _ptr(viewdirs), p, prec, C.byref(cot), garr,
+                np_ // 2, 0, scratch.data_ptr(), scratch.numel(), _stream(dev)), "MipNerf.query backward")
+        return (None,) * 5 + tuple(out_grads)
