@@ -388,6 +388,28 @@ int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b2
                                 float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
                                 size_t workspace_bytes, void* stream);
 
+/* Radiance of the field at Gaussians under one shared set of directions: means / covs [P,3] as for the density query,
+ * dirs [D,3] (encoded as given), each point seen from every direction.  The view layer's pre-activation is split into
+ * W_view[:, :256] . bottleneck(p) (per point) and b_view + W_view[:, 256:] . pos_enc(dir d) (per direction); per pair
+ * remain the ReLU and the colour head.  Outputs, each may be NULL but not all:
+ *   raw_rgb / rgb [P,D,3]: query_radiance's raw head / activation of (point p, direction d);
+ *   raw_density / density [P]: query_density's;
+ *   proj_out [P,num_basis,3] = sum over d = 0..D-1, in order, in fp32, of table[d][k] c[p][d] with c = raw_rgb when
+ *   proj_raw, else rgb; table [D,num_basis] (device), num_basis 1..16.  Bit-reproducible, independent of chunking.
+ * The tensor-core precisions take the configs query_radiance takes on the tensor cores and return query_radiance's
+ * raw_rgb / rgb bit for bit (the view-accumulator mode of the level kernel, then the per-pair kernel in the level
+ * kernel's summation order); FP32 takes use_viewdirs configs with one 128-wide view layer, within fp32 round-off of
+ * query_radiance (the view layer's sum runs in another order).  use_viewdirs=0, num_dirs < 1, proj_out without table
+ * or with num_basis outside 1..16: refused.  Workspace: one chunk of at most 524288 points (256 MB of view
+ * accumulators on the tensor cores) plus D x 512 bytes. */
+size_t mipnerf_b200_radiance_dirs_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points, int64_t num_dirs,
+                                                  int precision);
+int mipnerf_b200_query_radiance_dirs(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                                     const float* covs, int64_t num_points, const float* dirs, int64_t num_dirs,
+                                     int precision, float* raw_rgb, float* rgb, float* raw_density, float* density,
+                                     const float* table, int num_basis, int proj_raw, float* proj_out,
+                                     void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- gradients of field queries with respect to the MLP tensors ----
  * Cotangents of one query's outputs; any pointer may be NULL (= zero). */
 typedef struct mipnerf_b200_query_cotangent {

@@ -17,7 +17,8 @@ from .datasets import (Blender, Multicam, DeviceRayBank, Scene, dataset_dict, lo
 from .render import generate_rays, render_frame, render_sharded, shard_bounds, shard_rows, gather_rows
 from .graph import GraphedForward
 from .metrics import eval_errors, ssim, evaluate, render_path, spheric_path, save_images
-from .field import density_grid, isosurface, extract_mesh, mesh_colors, voxel_variance, write_ply
+from .field import (density_grid, isosurface, extract_mesh, mesh_colors, voxel_variance, write_ply, sh_basis,
+                    sphere_quadrature, bake_sh, eval_sh, mesh_sh)
 
 __all__ = [
     "Rays", "Rays_keys", "namedtuple_map", "rearrange_render_image", "blender_rays", "spheric_pose",
@@ -29,5 +30,5 @@ __all__ = [
     "load_blender_scene", "load_multicam_scene", "image_rays", "convert_blender_to_multiscale",
     "write_synthetic_blender_scene", "GraphedForward", "philox_uniform", "philox_normal", "eval_errors", "ssim", "evaluate",
     "render_path", "spheric_path", "save_images", "density_grid", "isosurface", "extract_mesh", "write_ply",
-    "mesh_colors", "voxel_variance",
+    "mesh_colors", "voxel_variance", "sh_basis", "sphere_quadrature", "bake_sh", "eval_sh", "mesh_sh",
 ]

@@ -142,6 +142,10 @@ _SIGNATURES = {
     "mipnerf_b200_radiance_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int]),
     "mipnerf_b200_query_radiance": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), _V, _V, _V, C.c_int64, C.c_int,
                                               _V, _V, _V, _V, _V, C.c_size_t, _V]),
+    "mipnerf_b200_radiance_dirs_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int64, C.c_int]),
+    "mipnerf_b200_query_radiance_dirs": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), _V, _V, C.c_int64, _V,
+                                                   C.c_int64, C.c_int, _V, _V, _V, _V, _V, C.c_int, C.c_int, _V, _V,
+                                                   C.c_size_t, _V]),
     "mipnerf_b200_query_backward_workspace_bytes": (C.c_size_t, [C.POINTER(Config), C.c_int64, C.c_int, C.c_int]),
     "mipnerf_b200_query_backward": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), _V, _V, _V, C.c_int64, C.c_int,
                                               C.POINTER(QueryCotangent), C.POINTER(LinearGrad), C.c_int, C.c_int, _V,

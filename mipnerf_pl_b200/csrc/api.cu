@@ -1681,6 +1681,147 @@ int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b2
 }
 
 namespace {
+// Radiance under a shared direction set: per chunk of m points, the view layer's accumulators A [m rounded up to a
+// 128-point tile][128] (W_view[:, :width] . bottleneck), and once per call the direction terms T [D][128]; fp32 adds
+// the IPE, trunk and bottleneck activations, the raw densities and the zero bias / zero view row that let
+// launch_linear_f32 compute A from the view layer's own weights.
+struct RadianceDirsScratch {
+  float *acc, *terms, *zero_covs, *enc, *h0, *h1, *raw, *zeros;
+  size_t bytes;
+};
+RadianceDirsScratch carve_radiance_dirs(const mipnerf_b200_config* c, const Dims& d, int64_t m, int64_t num_dirs,
+                                        int precision, void* base) {
+  RadianceDirsScratch s{};
+  size_t off = 0;
+  auto take = [&](size_t elems) {
+    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
+    off += align_up(elems * sizeof(float));
+    return p;
+  };
+  s.acc = take((size_t)((m + 127) / 128 * 128) * c->net_width_condition);
+  s.terms = take((size_t)num_dirs * c->net_width_condition);
+  if (precision == MIPNERF_B200_FP32) {
+    s.zero_covs = take((size_t)m * 3);
+    s.enc = take((size_t)m * d.xyz_dim);
+    s.h0 = take((size_t)m * c->net_width);
+    s.h1 = take((size_t)m * c->net_width);
+    s.raw = take((size_t)m);
+    s.zeros = take((size_t)c->net_width_condition + d.view_dim);
+  }
+  s.bytes = off;
+  return s;
+}
+// the view layer splits into a per-point and a per-direction part only when it is the one layer before the colour head,
+// 128 wide (the pair kernel's width)
+bool radiance_dirs_supported(const mipnerf_b200_config* c, int precision) {
+  if (precision != MIPNERF_B200_FP32) return mipnerf::tc_supported(c, precision);
+  return c->use_viewdirs && c->net_depth_condition == 1 && c->net_width_condition == 128;
+}
+}  // namespace
+
+size_t mipnerf_b200_radiance_dirs_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points, int64_t num_dirs,
+                                                  int precision) {
+  Dims d;
+  if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0 || num_dirs < 1 ||
+      precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3 || !radiance_dirs_supported(cfg, precision))
+    return 0;
+  const int64_t m = num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32;
+  return carve_radiance_dirs(cfg, d, m > 0 ? m : 1, num_dirs, precision, nullptr).bytes;
+}
+
+int mipnerf_b200_query_radiance_dirs(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                                     const float* covs, int64_t num_points, const float* dirs, int64_t num_dirs,
+                                     int precision, float* raw_rgb, float* rgb, float* raw_density, float* density,
+                                     const float* table, int num_basis, int proj_raw, float* proj_out,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  static_assert(kChunkPointsFp32 == mipnerf::kDensityChunkPoints, "one chunk size for every precision");
+  Dims d;
+  int rc;
+  if ((rc = check_config(cfg, &d))) return rc;
+  if ((rc = check_weights(cfg, d, w))) return rc;
+  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if (num_dirs < 1) return fail(MIPNERF_B200_EINVAL, "num_dirs=%lld: need at least one direction", (long long)num_dirs);
+  if (!raw_rgb && !rgb && !raw_density && !density && !proj_out) return fail(MIPNERF_B200_EINVAL, "every output is NULL");
+  if (proj_out && !table) return fail(MIPNERF_B200_EINVAL, "proj_out without table");
+  if (proj_out && (num_basis < 1 || num_basis > 16))
+    return fail(MIPNERF_B200_EINVAL, "num_basis=%d: need 1..16 with proj_out", num_basis);
+  if (!dirs) return fail(MIPNERF_B200_EINVAL, "dirs is NULL");
+  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
+  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
+    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
+  if (!cfg->use_viewdirs)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "radiance under a direction set needs use_viewdirs (use query_radiance)");
+  if (!radiance_dirs_supported(cfg, precision)) {
+    if (precision == MIPNERF_B200_FP32)
+      return fail(MIPNERF_B200_EUNSUPPORTED, "radiance under a direction set: one 128-wide view layer only");
+    return fail(MIPNERF_B200_EUNSUPPORTED,
+                "tensor-core radiance query: the forward's tensor-core shapes only (8x256 / 1x128 model, "
+                "num_samples 128 or 256, min_deg_point 0, max_deg_point 1..16, deg_view 1..4); use MIPNERF_B200_FP32");
+  }
+  if (precision != MIPNERF_B200_FP32 &&
+      (!w->packed || w->packed_precision != precision || w->packed_bytes < mipnerf::tc_packed_bytes(cfg, precision)))
+    return fail(MIPNERF_B200_EINVAL, "weights->packed missing or packed for another precision");
+  const size_t need = mipnerf_b200_radiance_dirs_workspace_bytes(cfg, num_points, num_dirs, precision);
+  if (num_points > 0 && (need == 0 || !workspace || workspace_bytes < need))
+    return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
+  if (num_points == 0) return MIPNERF_B200_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const mipnerf_b200_linear& vl = w->linears[cfg->net_depth + 2];
+  const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
+  const RadianceDirsScratch s0 = carve_radiance_dirs(cfg, d, num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32,
+                                                     num_dirs, precision, workspace);
+  // T: radiance mode's view-direction term of each direction (the tensor-core precisions), or the same sum over the
+  // view layer's own weights (fp32)
+  if (precision != MIPNERF_B200_FP32) {
+    cudaError_t e = mipnerf::tc_view_terms(w, dirs, num_dirs, s0.terms, st);
+    if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "tc_view_terms: %s", cudaGetErrorString(e));
+  } else {
+    CUDA_TRY(mipnerf::launch_view_terms(dirs, num_dirs, vl.weight + cfg->net_width, 1, cfg->net_width + d.view_dim,
+                                        vl.bias, d.view_dim, cfg->deg_view, s0.terms, st));
+    CUDA_TRY(cudaMemsetAsync(s0.zeros, 0, (size_t)(cfg->net_width_condition + d.view_dim) * sizeof(float), st));
+  }
+  for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
+    const int64_t m = (num_points - off) < kChunkPointsFp32 ? (num_points - off) : kChunkPointsFp32;
+    const RadianceDirsScratch& s = s0;  // every chunk reuses the first one's scratch, in stream order
+    if (precision != MIPNERF_B200_FP32) {
+      cudaError_t e = mipnerf::tc_query_view_acc(cfg, w, means + off * 3, covs ? covs + off * 3 : nullptr, m, precision,
+                                                 s.acc, raw_density ? raw_density + off : nullptr,
+                                                 density ? density + off : nullptr, st);
+      if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "tc_query_view_acc: %s", cudaGetErrorString(e));
+    } else {
+      // the IPE stage kernel, the fp32 trunk, density_layer and extra_layer, then A = [bottleneck | 0] . W_view^T + 0:
+      // the view layer's sum over its bottleneck columns (models/mip.py:322-350, models/mip_nerf.py:93-107)
+      const float* cv = covs ? covs + off * 3 : nullptr;
+      if (!cv || cfg->disable_integration) {
+        CUDA_TRY(cudaMemsetAsync(s.zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
+        cv = s.zero_covs;
+      }
+      CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, s.enc, m, cfg->min_deg_point, cfg->max_deg_point, st));
+      const float* h;
+      if ((rc = trunk_fp32(cfg, d, w, s.enc, m, s.h0, s.h1, &h, st))) return rc;
+      const mipnerf_b200_linear& dl = w->linears[cfg->net_depth];
+      const mipnerf_b200_linear& el = w->linears[cfg->net_depth + 1];
+      float* raw = raw_density ? raw_density + off : s.raw;
+      CUDA_TRY(mipnerf::launch_linear_f32(h, cfg->net_width, cfg->net_width, nullptr, 0, 0, 1, dl.weight, dl.bias, raw, 1,
+                                          m, 1, 0, st));
+      if (density) CUDA_TRY(mipnerf::launch_density_activation(raw, density + off, m, cfg->density_bias, st));
+      float* bott = h == s.h0 ? s.h1 : s.h0;
+      CUDA_TRY(mipnerf::launch_linear_f32(h, cfg->net_width, cfg->net_width, nullptr, 0, 0, 1, el.weight, el.bias, bott,
+                                          cfg->net_width, m, cfg->net_width, 0, st));
+      CUDA_TRY(mipnerf::launch_linear_f32(bott, cfg->net_width, cfg->net_width, s.zeros + cfg->net_width_condition,
+                                          d.view_dim, d.view_dim, (int)m, vl.weight, s.zeros, s.acc,
+                                          cfg->net_width_condition, m, cfg->net_width_condition, 0, st));
+    }
+    CUDA_TRY(mipnerf::launch_radiance_pairs(
+        s.acc, s.terms, cl.weight, cl.bias, m, num_dirs, rgb_scale, cfg->rgb_padding,
+        raw_rgb ? raw_rgb + off * num_dirs * 3 : nullptr, rgb ? rgb + off * num_dirs * 3 : nullptr, table, num_basis,
+        proj_raw, proj_out ? proj_out + off * num_basis * 3 : nullptr, st));
+  }
+  return MIPNERF_B200_OK;
+}
+
+namespace {
 // Scratch of the fp32 query backward for one chunk of m points: the training step's activation layout (TrainScratch
 // with one row per point, view encoding included) without its per-ray buffers, and the zero covariances.
 struct QueryGradScratch {

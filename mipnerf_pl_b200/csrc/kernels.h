@@ -185,5 +185,16 @@ cudaError_t launch_wgrad_small_n_t16(const float* dy, int n_dim, const void* x, 
 // out[ray][n] = b[n] + W[n, in_main : in_main + view_dim] . venc[ray]   (view-direction part of the view layer)
 cudaError_t launch_view_bias_from_enc(const float* venc, const float* w, const float* b, float* out,
                                       int64_t num_rays, cudaStream_t st);
+// terms[d][n] = bias[n] + sum_{k < nk} w[k sk + n sn] enc_k(dirs[d])  (fmaf, k in order; enc: pos_enc of num_deg
+// degrees with append_identity, nk <= 27), n < 128
+cudaError_t launch_view_terms(const float* dirs, int64_t num_dirs, const float* w, int64_t sk, int64_t sn,
+                              const float* bias, int nk, int num_deg, float* terms, cudaStream_t st);
+// Per (point p, direction d): raw = W_color . max(acc[p] + terms[d], 0) + b_color (128 wide, the level kernel's order),
+// rgb = its activation, into raw_rgb / rgb [P][D][3] (either may be null); proj (may be null) [P][num_basis][3] =
+// sum over d in order of table[d][k] (raw if proj_raw else rgb), num_basis 1..16.
+cudaError_t launch_radiance_pairs(const float* acc, const float* terms, const float* w_color, const float* b_color,
+                                  int64_t num_points, int64_t num_dirs, float rgb_scale, float rgb_padding,
+                                  float* raw_rgb, float* rgb, const float* table, int num_basis, int proj_raw,
+                                  float* proj, cudaStream_t st);
 
 }  // namespace mipnerf

@@ -166,11 +166,16 @@ struct LevelParams {
   // terms (tile parity); raw heads into raw_rgb_out / raw_density_out, their activations into rgb_out / density_out (any
   // may be null).
   float* rgb_out;
+  // View-accumulator mode (mipnerf_b200_query_radiance_dirs): the query points as in density-only mode; the view layer's
+  // pre-activation without its bias and view-direction columns, W_view[:, :256] . bottleneck, of every row of tile i
+  // into view_acc + i [128][128] fp32 (rows past the last point hold garbage); densities as in density-only mode.
+  float* view_acc;
 };
 
 // Compile-time modes of the level kernel: the forward (rays in, composited pixels out; MLP-only mode and the training
-// forward are runtime variants of it), density-only queries, and radiance queries with a view direction per point.
-enum LevelMode : int { kModeForward = 0, kModeDensity = 1, kModeRadiance = 2 };
+// forward are runtime variants of it), density-only queries, radiance queries with a view direction per point, and
+// the view accumulators of radiance queries under a shared direction set.
+enum LevelMode : int { kModeForward = 0, kModeDensity = 1, kModeRadiance = 2, kModeViewAcc = 3 };
 
 // raw density of (ray, row) of a ray of kNs samples with the density noise added; kept out of line so that the
 // (default) noise-free path carries none of the generator's registers
@@ -733,6 +738,20 @@ __device__ __forceinline__ float quad_sum(float v) {
 // Rows past the last point get the bias alone.  The stores go to L2 (st.cg); the consumers read them back with ld.cg
 // after feat_full, as the forward's view bias.
 constexpr int kViewPts = 4;
+// Element f < 3 + 6 num_deg of the view encoding of direction vd (models/mip.py:353-363, append_identity): vd, then
+// sin(2^l vd) scale-major then xyz, then sin(2^l vd + pi/2); the arithmetic of pos_enc_kernel, of level_view_terms and
+// of the level-0 prologue.  (Those two keep their own copy of it: calling this function from them reorders their SASS.)
+__device__ __forceinline__ float view_enc_elem(const float* vd, int f, int num_deg) {
+  float enc;
+  if (f < 3) {
+    enc = __ldg(vd + f);  // append_identity
+  } else {
+    const int gidx = f - 3, half = 3 * num_deg, is_cos = gidx >= half, h = is_cos ? gidx - half : gidx;
+    const float y = __fmul_rn(__ldg(vd + h % 3), __int_as_float((127 + h / 3) << 23));
+    enc = sinf(is_cos ? __fadd_rn(y, MIPNERF_HALF_PI_F32) : y);
+  }
+  return enc;
+}
 __device__ __forceinline__ void level_view_terms(const LevelParams& p, int64_t tile, float* slot, int hw, int lane) {
   const float4* wt = reinterpret_cast<const float4*>(p.wimage + kViewDirOffset);  // [27][128] | bias[128]
   const float4 b4 = __ldg(wt + kViewDim * kCond / 4 + lane);
@@ -1019,6 +1038,11 @@ __device__ __forceinline__ void level_radiance_out(const LevelParams& p, int64_t
 // helpers write slot i % 2 for tile i only after they have waited on heads_full of tile i - 2 (in the previous round
 // of their loop, with one feature buffer or two), and the consumers arrive on heads_full of a tile only after its view
 // layer's epilogue has read the tile's terms (the quad sums that the arriving thread stores depend on every loaded term).
+// kMode = kModeViewAcc (kT = 1): view-accumulator mode.  The producer and the consumers run radiance mode's schedule
+// through the view layer's K-slabs (the same stages and wgmmas into acc0, in the same order), then the consumers store
+// acc0 as it is to p.view_acc instead of the view-layer epilogue and the colour head; the density head is finished and
+// handed over as in radiance mode.  The helpers compute no view terms: they encode the query points and write the
+// densities, as in density-only mode.
 // kMode = kModeForward: the per-ray view bias of the i-th ray of the CTA is in shared-memory slot vbias[i % 2], which
 // the helpers fill in the ray prologue of its tile 0 and the view-layer epilogues of all its tiles read.  The same
 // argument holds per ray: the helpers fill the slot of ray i only after they have waited on heads_full of every tile of
@@ -1109,7 +1133,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
             for (int u = 0; u < kT; ++u)
               mbar_wait(&heads_full[par + u], (uint32_t)(((i - 1) * kT + u) >> 1) & 1u);
             clk.mark(kPhHeadsFull);
-            if constexpr (kDensity)
+            if constexpr (kDensity || kMode == kModeViewAcc)
               level_density_out(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], ht, clk);
             else if constexpr (kMode == kModeRadiance)
               level_radiance_out(p, ray - gridDim.x, heads + par * kN * 4, &heads_empty[par], ht, clk);
@@ -1337,7 +1361,22 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_level_kernel(const LevelParam
           level_mma_slab<kFmt, kX3>(acc0, 9, s, a_u, f_u, ft_u, w_u, w_full, w_empty, rp, leader, clk);
       }
     }
-    if constexpr (!kDensity) {
+    if constexpr (kMode == kModeViewAcc) {
+      // the view layer's accumulators as they are, straight from the registers (evict-first: read once, by the pair
+      // kernel, after this launch)
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc0);
+      if (leader) mbar_arrive(&w_empty[rp.prev]);
+      rp.prev = -1;
+      clk.mark(kPhMma);
+      const uint64_t pol = l2_policy_evict_first();
+      float* va = p.view_acc + ((size_t)ray * kN + r0) * kCond + cq;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        st_global_v2_hint(va + 8 * j, acc0[4 * j], acc0[4 * j + 1], pol);
+        st_global_v2_hint(va + 8 * kCond + 8 * j, acc0[4 * j + 2], acc0[4 * j + 3], pol);
+      }
+    } else if constexpr (!kDensity) {
       // the view layer's epilogue from the registers; the forward reads its columns of the ray's view bias from the
       // ray's slot, in bf16 / fp16 while the last K-slab's wgmmas run (the split modes' training forward has no
       // registers to spare there: ptxas spills 32 values)
@@ -1421,6 +1460,118 @@ __global__ void view_bias_from_enc_kernel(const float* __restrict__ venc, const 
   for (int k = 0; k < kViewDim; ++k)
     acc = fmaf(__ldg(w + (size_t)n * (kWidth + kViewDim) + kWidth + k), __ldg(venc + ray * kViewDim + k), acc);
   out[idx] = acc;
+}
+
+// Radiance under a shared direction set: the view-direction term  b_view[n] + sum_k W(k, n) enc_k(dir d)  of direction
+// d into terms[d][n], one block of 128 threads per direction.  W(k, n) = w[k sk + n sn] over nk encoding elements of
+// num_deg degrees: the packed image's [27][128] (the tensor-core precisions; the fmaf order of level_view_terms, so
+// each term is radiance mode's bit for bit) or view_layers.0's own columns (fp32).
+__global__ void __launch_bounds__(kCond) view_terms_kernel(const float* __restrict__ dirs, const float* __restrict__ w,
+                                                           int64_t sk, int64_t sn, const float* __restrict__ bias,
+                                                           int nk, int num_deg, float* __restrict__ terms) {
+  __shared__ float enc[kViewDim];
+  const int64_t d = blockIdx.x;
+  const int n = threadIdx.x;
+  if (n < nk) enc[n] = view_enc_elem(dirs + d * 3, n, num_deg);
+  __syncthreads();
+  float acc = __ldg(bias + n);
+  for (int k = 0; k < nk; ++k) acc = fmaf(__ldg(w + k * sk + n * sn), enc[k], acc);
+  terms[d * kCond + n] = acc;
+}
+
+// The per-(point, direction) head: y = max(A[p] + T[d], 0) and the colour head on it in the level kernel's order (four
+// partial sums, one per quad lane q over columns 8 j + 2 q, + 1 for j = 0..15; combined as quad_sum combines them; then
+// b_color), so that raw_rgb is radiance mode's bit for bit.  One thread per point with its A row in registers; the
+// terms, the table and W_color are broadcast from shared memory, kPairDirs directions at a time.  kProj: proj[p][k][ch] =
+// sum over d = 0..D-1, in order, of table[d][k] c[p][d][ch] (c: raw_rgb when proj_raw, else rgb), in fp32.
+constexpr int kPairThreads = 128;
+constexpr int kPairDirs = 32;
+constexpr int kMaxBasis = 16;
+template <bool kProj>
+__global__ void __launch_bounds__(kPairThreads) radiance_pairs_kernel(
+    const float* __restrict__ acc, const float* __restrict__ terms, const float* __restrict__ w_color,
+    const float* __restrict__ b_color, int64_t num_points, int64_t num_dirs, float rgb_scale, float rgb_padding,
+    float* __restrict__ raw_rgb, float* __restrict__ rgb, const float* __restrict__ table, int num_basis, int proj_raw,
+    float* __restrict__ proj) {
+  __shared__ __align__(16) float s_w[3][kCond];
+  __shared__ __align__(16) float s_t[kPairDirs][kCond];
+  __shared__ float s_tab[kPairDirs][kMaxBasis];
+  const int tid = threadIdx.x;
+  const int64_t pt = (int64_t)blockIdx.x * kPairThreads + tid;
+  const bool live = pt < num_points;
+  for (int i = tid; i < 3 * kCond; i += kPairThreads) s_w[i / kCond][i % kCond] = __ldg(w_color + i);
+  float a[kCond];
+  const float4* ar = reinterpret_cast<const float4*>(acc + (live ? pt : 0) * kCond);
+#pragma unroll
+  for (int j = 0; j < kCond / 4; ++j) {
+    const float4 v = __ldcs(ar + j);  // read once
+    a[4 * j] = v.x, a[4 * j + 1] = v.y, a[4 * j + 2] = v.z, a[4 * j + 3] = v.w;
+  }
+  const float bc[3] = {__ldg(b_color), __ldg(b_color + 1), __ldg(b_color + 2)};
+  float pr[kProj ? kMaxBasis : 1][3];
+#pragma unroll
+  for (int k = 0; k < (kProj ? kMaxBasis : 1); ++k) pr[k][0] = pr[k][1] = pr[k][2] = 0.f;
+#pragma unroll 1
+  for (int64_t d0 = 0; d0 < num_dirs; d0 += kPairDirs) {
+    const int nd = (int)(num_dirs - d0 < kPairDirs ? num_dirs - d0 : kPairDirs);
+    __syncthreads();  // the previous round's reads of s_t / s_tab are done
+    for (int i = tid; i < nd * kCond; i += kPairThreads) s_t[i / kCond][i % kCond] = __ldg(terms + d0 * kCond + i);
+    if (kProj)
+      for (int i = tid; i < nd * kMaxBasis; i += kPairThreads) {
+        const int dd = i / kMaxBasis, k = i % kMaxBasis;
+        s_tab[dd][k] = k < num_basis ? __ldg(table + (d0 + dd) * num_basis + k) : 0.f;
+      }
+    __syncthreads();
+    if (!live) continue;
+#pragma unroll 1
+    for (int dd = 0; dd < nd; ++dd) {
+      // W_color re-read from shared memory per direction: opaque here, so that the compiler does not keep its 384
+      // loop-invariant values in registers beside the A row (ptxas spills 1.6 KB otherwise)
+      const float* wc = &s_w[0][0];
+      asm volatile("" : "+l"(wc));
+      float s[4][3];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) s[q][0] = s[q][1] = s[q][2] = 0.f;
+#pragma unroll
+      for (int j = 0; j < kCond / 8; ++j)
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * j + 2 * q + e;
+            const float y = fmaxf(__fadd_rn(a[c], s_t[dd][c]), 0.f);
+#pragma unroll
+            for (int ch = 0; ch < 3; ++ch) s[q][ch] = __fmaf_rn(y, wc[ch * kCond + c], s[q][ch]);
+          }
+      const int64_t o = (pt * num_dirs + d0 + dd) * 3;
+      float cv[3];
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const float raw = __fadd_rn(__fadd_rn(__fadd_rn(s[0][ch], s[1][ch]), __fadd_rn(s[2][ch], s[3][ch])), bc[ch]);
+        const float act = rgb_activation(raw, rgb_scale, rgb_padding);
+        if (raw_rgb) raw_rgb[o + ch] = raw;
+        if (rgb) rgb[o + ch] = act;
+        cv[ch] = proj_raw ? raw : act;
+      }
+      if (kProj) {
+#pragma unroll
+        for (int k = 0; k < (kProj ? kMaxBasis : 1); ++k) {
+          if (k >= num_basis) break;
+          const float t = s_tab[dd][k];
+#pragma unroll
+          for (int ch = 0; ch < 3; ++ch) pr[k][ch] = __fmaf_rn(t, cv[ch], pr[k][ch]);
+        }
+      }
+    }
+  }
+  if (kProj && live) {
+#pragma unroll
+    for (int k = 0; k < (kProj ? kMaxBasis : 1); ++k) {
+      if (k >= num_basis) break;
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) proj[(pt * num_basis + k) * 3 + ch] = pr[k][ch];
+    }
+  }
 }
 
 // ---- weight packing ---------------------------------------------------------------------------
@@ -1616,6 +1767,7 @@ cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
   num_sms();
   LaunchScope scope(kMode == kModeDensity    ? kKernDensityTc
                     : kMode == kModeRadiance ? kKernRadianceTc
+                    : kMode == kModeViewAcc  ? kKernRadianceDirsTc
                                              : (p.feat_in ? kKernMlpTc : kKernMlpLevelTc),
                     st);
   const int grid = (int)(p.num_rays < g_num_sms ? p.num_rays : g_num_sms);
@@ -1655,6 +1807,14 @@ cudaError_t launch_radiance(const LevelParams& p, int precision, cudaStream_t st
                              : launch_level_t<0, true, 1, kModeRadiance>(p, st);
   return fmt_of(precision) ? launch_level_t<1, false, 1, kModeRadiance>(p, st)
                            : launch_level_t<0, false, 1, kModeRadiance>(p, st);
+}
+cudaError_t launch_view_acc(const LevelParams& p, int precision, cudaStream_t st) {
+  if (p.num_rays <= 0) return cudaSuccess;
+  if (is_x3(precision))
+    return fmt_of(precision) ? launch_level_t<1, true, 1, kModeViewAcc>(p, st)
+                             : launch_level_t<0, true, 1, kModeViewAcc>(p, st);
+  return fmt_of(precision) ? launch_level_t<1, false, 1, kModeViewAcc>(p, st)
+                           : launch_level_t<0, false, 1, kModeViewAcc>(p, st);
 }
 
 // radiance mode: the view-direction slots [ctas][2][128][128] fp32, one pair per CTA of a launch of min(tiles, SMs)
@@ -1956,6 +2116,62 @@ cudaError_t launch_view_bias_from_enc(const float* venc, const float* w, const f
 }
 
 size_t tc_mlp_workspace_bytes(int64_t num_rays) { return (size_t)(num_rays > 0 ? num_rays : 1) * kCond * sizeof(float); }
+
+cudaError_t tc_query_view_acc(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, const float* means,
+                              const float* covs, int64_t num_points, int precision, float* view_acc,
+                              float* raw_density, float* density, cudaStream_t st) {
+  if (num_points > kDensityChunkPoints) return cudaErrorInvalidValue;
+  const uint8_t* img = static_cast<const uint8_t*>(w->packed);
+  SmallUpload small(img, st);
+  cudaError_t e = small.error();
+  if (e != cudaSuccess) return e;
+  LevelParams p{};
+  p.wimage = img;
+  p.q_means = means;
+  p.q_covs = covs;
+  p.num_points = num_points;
+  p.num_rays = (num_points + kN - 1) / kN;
+  p.view_acc = view_acc;
+  p.raw_density_out = raw_density;
+  p.density_out = density;
+  p.disable_integration = c->disable_integration;
+  p.density_bias = c->density_bias;
+  return launch_view_acc(p, precision, st);
+}
+
+cudaError_t tc_view_terms(const mipnerf_b200_weights* w, const float* dirs, int64_t num_dirs, float* terms,
+                          cudaStream_t st) {
+  const float* wt = reinterpret_cast<const float*>(static_cast<const uint8_t*>(w->packed) + kViewDirOffset);
+  return launch_view_terms(dirs, num_dirs, wt, kCond, 1, wt + kViewDim * kCond, kViewDim, (kViewDim - 3) / 6, terms, st);
+}
+
+cudaError_t launch_view_terms(const float* dirs, int64_t num_dirs, const float* w, int64_t sk, int64_t sn,
+                              const float* bias, int nk, int num_deg, float* terms, cudaStream_t st) {
+  if (num_dirs == 0) return cudaSuccess;
+  if (nk > kViewDim) return cudaErrorInvalidValue;
+  LaunchScope scope(kKernPosEnc, st);
+  view_terms_kernel<<<(unsigned)num_dirs, kCond, 0, st>>>(dirs, w, sk, sn, bias, nk, num_deg, terms);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_radiance_pairs(const float* acc, const float* terms, const float* w_color, const float* b_color,
+                                  int64_t num_points, int64_t num_dirs, float rgb_scale, float rgb_padding,
+                                  float* raw_rgb, float* rgb, const float* table, int num_basis, int proj_raw,
+                                  float* proj, cudaStream_t st) {
+  if (num_points == 0 || num_dirs == 0) return cudaSuccess;
+  if (proj && (num_basis < 1 || num_basis > kMaxBasis || !table)) return cudaErrorInvalidValue;
+  LaunchScope scope(kKernRadiancePairs, st);
+  const unsigned grid = (unsigned)((num_points + kPairThreads - 1) / kPairThreads);
+  if (proj)
+    radiance_pairs_kernel<true><<<grid, kPairThreads, 0, st>>>(acc, terms, w_color, b_color, num_points, num_dirs,
+                                                               rgb_scale, rgb_padding, raw_rgb, rgb, table, num_basis,
+                                                               proj_raw, proj);
+  else
+    radiance_pairs_kernel<false><<<grid, kPairThreads, 0, st>>>(acc, terms, w_color, b_color, num_points, num_dirs,
+                                                                rgb_scale, rgb_padding, raw_rgb, rgb, nullptr, 0, 0,
+                                                                nullptr);
+  return cudaGetLastError();
+}
 
 }  // namespace mipnerf
 

@@ -63,5 +63,15 @@ cudaError_t tc_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b200
                               const float* covs, const float* viewdirs, int64_t num_points, int precision,
                               float* raw_rgb, float* raw_density, float* rgb, float* density, void* workspace,
                               size_t workspace_bytes, cudaStream_t st, const TcQueryDump* dump = nullptr);
+// Radiance under a shared direction set (mipnerf_b200_query_radiance_dirs).  The view-accumulator mode of the level
+// kernels, one launch for at most kDensityChunkPoints points: view_acc [ceil(points / 128) * 128][128] gets W_view[:, :256]
+// . bottleneck of each point (the view layer's accumulators of radiance mode, before the view-direction term), raw_density
+// / density (either may be null) the density query's values.
+cudaError_t tc_query_view_acc(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
+                              const float* covs, int64_t num_points, int precision, float* view_acc,
+                              float* raw_density, float* density, cudaStream_t st);
+// terms [num_dirs][128]: radiance mode's view-direction term of each direction, from the packed image's view weights
+cudaError_t tc_view_terms(const mipnerf_b200_weights* w, const float* dirs, int64_t num_dirs, float* terms,
+                          cudaStream_t st);
 
 }  // namespace mipnerf

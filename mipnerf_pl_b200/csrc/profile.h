@@ -31,6 +31,8 @@ enum KernelId : int {
   kKernDensityTc,    // density-only mode of the wgmma level kernel (IPE + trunk + density head)
   kKernIsosurface,   // marching-tetrahedra isosurface extraction (count / scan / emit)
   kKernRadianceTc,   // radiance mode of the wgmma level kernel (IPE + per-point view term + the whole MLP)
+  kKernRadianceDirsTc,  // view-accumulator mode of the wgmma level kernel (IPE + the MLP up to the view layer's GEMM)
+  kKernRadiancePairs,   // per-(point, direction) view layer + colour head (+ projection) of a shared direction set
   kKernCount
 };
 

@@ -131,6 +131,9 @@ __device__ __forceinline__ void st_global_v4_hint(void* gdst, uint4 v, uint64_t 
   asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(gdst), "r"(v.x), "r"(v.y), "r"(v.z),
                "r"(v.w), "l"(policy));
 }
+__device__ __forceinline__ void st_global_v2_hint(float* gdst, float x, float y, uint64_t policy) {
+  asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1, %2}, %3;" ::"l"(gdst), "f"(x), "f"(y), "l"(policy));
+}
 __device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar,
                                               uint64_t policy) {
   asm volatile(

@@ -9,6 +9,9 @@
   normals from the grid's gradient; `extract_mesh` is both.
 * `mesh_colors` colours vertices with `MipNerf.query_radiance` (the radiance mode of the level kernel on the tensor
   cores), each vertex seen along its inward normal; `extract_mesh(colors=True)` adds normals and colours.
+* `MipNerf.query_radiance_dirs` / `query_radiance_proj` see every point from one shared set of directions (the trunk
+  once per point, the view layer's ReLU and the colour head per direction); `bake_sh` projects that colour onto real
+  spherical harmonics over `sphere_quadrature`, `mesh_sh` does so at mesh vertices, and `eval_sh` evaluates the result.
 * `write_ply` writes a binary PLY (optionally with normals and colours) with no dependency.
 """
 from __future__ import annotations
@@ -122,6 +125,120 @@ def mesh_colors(model, verts: torch.Tensor, normals: torch.Tensor, variance, sla
     for o in range(0, v.shape[0], slab_points):
         vv = v[o:o + slab_points]
         out[o:o + len(vv)] = model.query_radiance(vv, var.expand(len(vv), 3), d[o:o + slab_points])[0]
+    return out
+
+
+# Real spherical harmonics up to degree 3 in the convention of the common `eval_sh` (PlenOctrees / Plenoxels / 3D
+# Gaussian splatting): basis k = l^2 + l + m, orthonormal on the unit sphere, with these constants and signs.
+SH_C0 = 0.28209479177387814
+SH_C1 = 0.4886025119029199
+SH_C2 = (1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396)
+SH_C3 = (-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658,
+         1.445305721320277, -0.5900435899266435)
+SH_MAX_DEGREE = 3
+
+
+def _sh_terms(x, y, z, degree: int):
+    """The (degree + 1)^2 basis functions at (x, y, z), as a list (numpy or torch arithmetic alike)."""
+    if not 0 <= int(degree) <= SH_MAX_DEGREE:
+        raise ValueError(f"degree {degree}: need 0..{SH_MAX_DEGREE}")
+    out = [SH_C0 + 0 * x]
+    if degree >= 1:
+        out += [-SH_C1 * y, SH_C1 * z, -SH_C1 * x]
+    if degree >= 2:
+        xx, yy, zz = x * x, y * y, z * z
+        out += [SH_C2[0] * x * y, SH_C2[1] * y * z, SH_C2[2] * (2 * zz - xx - yy), SH_C2[3] * x * z,
+                SH_C2[4] * (xx - yy)]
+    if degree >= 3:
+        out += [SH_C3[0] * y * (3 * xx - yy), SH_C3[1] * x * y * z, SH_C3[2] * y * (4 * zz - xx - yy),
+                SH_C3[3] * z * (2 * zz - 3 * xx - 3 * yy), SH_C3[4] * x * (4 * zz - xx - yy),
+                SH_C3[5] * z * (xx - yy), SH_C3[6] * x * (xx - 3 * yy)]
+    return out
+
+
+def sh_basis(dirs, degree: int) -> np.ndarray:
+    """Real SH basis [..., (degree + 1)^2] at unit directions dirs [..., 3], float64 on the host; degree 0..3, the
+    `eval_sh` convention (SH_C0 = 0.28209479..., Y_1 = -C1 y, Y_2 = C1 z, Y_3 = -C1 x, ...)."""
+    d = np.asarray(torch.as_tensor(dirs).detach().cpu().numpy() if isinstance(dirs, torch.Tensor) else dirs,
+                   dtype=np.float64)
+    if d.shape[-1] != 3:
+        raise ValueError(f"dirs {d.shape}: need [..., 3]")
+    return np.stack(_sh_terms(d[..., 0], d[..., 1], d[..., 2], degree), axis=-1)
+
+
+def sh_degree(num_coeffs: int) -> int:
+    """The degree of an expansion with num_coeffs = (degree + 1)^2 coefficients."""
+    deg = int(round(num_coeffs ** 0.5)) - 1
+    if (deg + 1) ** 2 != num_coeffs or not 0 <= deg <= SH_MAX_DEGREE:
+        raise ValueError(f"{num_coeffs} coefficients: need (degree + 1)^2 with degree 0..{SH_MAX_DEGREE}")
+    return deg
+
+
+def eval_sh(coeffs: torch.Tensor, dirs: torch.Tensor) -> torch.Tensor:
+    """The colour of an SH expansion: coeffs [..., K, C] with K = (degree + 1)^2, dirs [..., 3] (unit; broadcast against
+    coeffs' leading dimensions) -> [..., C] = sum_k Y_k(dir) coeffs[..., k, :], in coeffs' dtype and device.  No
+    activation: a bake of activated colours evaluates to colours."""
+    deg = sh_degree(coeffs.shape[-2])
+    d = dirs.to(device=coeffs.device, dtype=coeffs.dtype)
+    y = torch.stack(_sh_terms(d[..., 0], d[..., 1], d[..., 2], deg), dim=-1)
+    return (y.unsqueeze(-1) * coeffs).sum(dim=-2)
+
+
+def sphere_quadrature(n_theta: int, n_phi: Optional[int] = None):
+    """A quadrature on the unit sphere: Gauss-Legendre in cos(theta) (n_theta nodes) times n_phi uniform azimuths
+    (default 2 n_theta, offset by half a step) -> (dirs [n_theta n_phi, 3], weights [n_theta n_phi]), float64 on the host,
+    weights summing to 4 pi.  Exact for every product of two spherical harmonics of degree <= n_theta - 1, so that SH
+    projections up to that degree are exact for band-limited functions."""
+    n_theta = int(n_theta)
+    n_phi = 2 * n_theta if n_phi is None else int(n_phi)
+    if n_theta < 1 or n_phi < 1:
+        raise ValueError(f"n_theta {n_theta}, n_phi {n_phi}: need >= 1")
+    z, wz = np.polynomial.legendre.leggauss(n_theta)
+    phi = 2.0 * np.pi * (np.arange(n_phi) + 0.5) / n_phi
+    zz, pp = np.meshgrid(z, phi, indexing="ij")
+    r = np.sqrt(np.maximum(0.0, 1.0 - zz * zz))
+    dirs = np.stack([r * np.cos(pp), r * np.sin(pp), zz], axis=-1).reshape(-1, 3)
+    weights = (wz[:, None] * np.full(n_phi, 2.0 * np.pi / n_phi)[None, :]).reshape(-1)
+    return dirs, weights
+
+
+def sh_table(degree: int, n_theta: int):
+    """The projection of `bake_sh`: (dirs [D, 3] float64, table [D, K] float64 = w_d Y_k(dir_d)) of
+    sphere_quadrature(n_theta)."""
+    if not 0 <= int(degree) <= min(SH_MAX_DEGREE, int(n_theta) - 1):
+        raise ValueError(f"degree {degree} with n_theta {n_theta}: need 0 <= degree <= min(3, n_theta - 1)")
+    dirs, w = sphere_quadrature(n_theta)
+    return dirs, w[:, None] * sh_basis(dirs, degree)
+
+
+@torch.no_grad()
+def bake_sh(model, means: torch.Tensor, covs: Optional[torch.Tensor] = None, degree: int = 2, n_theta: int = 8,
+            raw: bool = False) -> torch.Tensor:
+    """The view-dependent colour of `model` at Gaussians as real SH coefficients [..., (degree + 1)^2, 3] (`eval_sh`
+    convention, degree 0..3): coeffs_k = sum_d w_d Y_k(d) rgb(d) over sphere_quadrature(n_theta) (n_theta * 2 n_theta
+    directions; the default 8 gives 128), i.e. the L2 projection of the colour onto the basis, in one
+    `MipNerf.query_radiance_proj` call (the table w_d Y_k(d) built in float64 and rounded to fp32; no [..., D, 3] colour
+    array).  `raw`: the raw colour head instead of the activated colour.  Under no_grad."""
+    dirs, table = sh_table(degree, n_theta)
+    dev = means.device
+    d32 = torch.tensor(dirs, dtype=torch.float32, device=dev)
+    t32 = torch.tensor(table, dtype=torch.float32, device=dev)
+    return model.query_radiance_proj(means, covs, d32, t32, raw=raw)[0]
+
+
+@torch.no_grad()
+def mesh_sh(model, verts: torch.Tensor, variance, degree: int = 2, n_theta: int = 8,
+            slab_points: int = 1 << 22) -> torch.Tensor:
+    """The view-dependent colour [V, (degree + 1)^2, 3] of `model` at mesh vertices as SH coefficients (`bake_sh` of each
+    vertex's Gaussian, diagonal `variance`, a float or one per axis, e.g. the voxel's step**2 / 12): the counterpart
+    of `mesh_colors` for every direction at once.  Queried in chunks of at most `slab_points` vertices, under no_grad."""
+    dev = next(model.parameters()).device
+    v = _f32(verts).to(dev).reshape(-1, 3)
+    var = torch.tensor(np.broadcast_to(np.asarray(variance, dtype=np.float32), (3,)).copy(), device=dev)
+    out = torch.empty(v.shape[0], (int(degree) + 1) ** 2, 3, device=dev)
+    for o in range(0, v.shape[0], slab_points):
+        vv = v[o:o + slab_points]
+        out[o:o + len(vv)] = bake_sh(model, vv, var.expand(len(vv), 3), degree, n_theta)
     return out
 
 

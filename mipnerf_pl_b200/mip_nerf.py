@@ -369,6 +369,71 @@ class MipNerf(torch.nn.Module):
                     scratch.data_ptr(), scratch.numel(), _stream(dev)), "MipNerf.query_radiance")
         return out_rgb.reshape(*shape, 3), out_dens.reshape(shape)
 
+    def query_radiance_dirs(self, means: torch.Tensor, covs: Optional[torch.Tensor], dirs: torch.Tensor, *,
+                            raw: bool = False):
+        """Radiance of the field at Gaussians under one shared set of directions: means / diagonal covs [..., 3] (covs
+        None: zero covariance), dirs [D, 3] (encoded as given) -> (rgb [..., D, 3], density [...]); `raw`: the raw
+        heads instead.  `rgb[..., d, :]` is `query_radiance(means, covs, dirs[d].expand_as(means))[0]` (bit for bit on
+        the tensor cores; fp32 to round-off), but the trunk runs once per point and only the view layer's ReLU and the
+        colour head once per (point, direction).  Needs use_viewdirs; no autograd (refused where `forward` would build
+        a graph)."""
+        rgb, dens, _ = self._query_radiance_dirs(means, covs, dirs, None, raw, colors=True)
+        return rgb, dens
+
+    def query_radiance_proj(self, means: torch.Tensor, covs: Optional[torch.Tensor], dirs: torch.Tensor,
+                            table: torch.Tensor, *, raw: bool = False):
+        """The colours of `query_radiance_dirs` projected onto K <= 16 functions of the direction, without forming the
+        [..., D, 3] colours: coeffs[..., k, :] = sum over d = 0..D-1 (in order, fp32) of table[d, k] * rgb[..., d, :]
+        (raw heads when `raw`) -> (coeffs [..., K, 3], density [...]).  table [D, K], e.g. quadrature weights times a
+        basis (`field.bake_sh`).  Bit-reproducible and independent of how the points are batched."""
+        _, dens, proj = self._query_radiance_dirs(means, covs, dirs, table, raw, colors=False)
+        return proj, dens
+
+    def _query_radiance_dirs(self, means, covs, dirs, table, raw: bool, colors: bool):
+        name = "query_radiance_dirs" if colors else "query_radiance_proj"
+        if means.shape[-1] != 3 or (covs is not None and covs.shape != means.shape):
+            raise ValueError(f"{name}: means {tuple(means.shape)} / covs "
+                             f"{None if covs is None else tuple(covs.shape)}: need [..., 3] of the same shape")
+        if dirs.dim() != 2 or dirs.shape[1] != 3 or dirs.shape[0] < 1:
+            raise ValueError(f"{name}: dirs {tuple(dirs.shape)}: need [D, 3] with D >= 1")
+        if table is not None and (table.dim() != 2 or table.shape[0] != dirs.shape[0] or not 1 <= table.shape[1] <= 16):
+            raise ValueError(f"{name}: table {tuple(table.shape)}: need [D = {dirs.shape[0]}, K] with 1 <= K <= 16")
+        if not self.use_viewdirs:
+            raise NotImplementedError(f"{name}: the model has use_viewdirs=False (its colour does not depend on the "
+                                      "direction; use query_radiance)")
+        if self._builds_graph():
+            raise NotImplementedError(f"{name}: no gradients; call it under torch.no_grad() on an autograd model")
+        with torch.no_grad():
+            dev = _dev(means)
+            shape = means.shape[:-1]
+            m = _f32(means).reshape(-1, 3)
+            c = _f32(covs).reshape(-1, 3) if covs is not None else None
+            dd = _f32(dirs).to(dev)
+            tab = _f32(table).to(dev) if table is not None else None
+            p, nd = m.shape[0], dd.shape[0]
+            k = tab.shape[1] if tab is not None else 0
+            prec = _cabi.PRECISIONS[self.precision]
+            cfg = self._config()
+            ws, keep = self.mlp._weights_struct(cfg, prec, dev)
+            out_rgb = torch.empty(p, nd, 3, device=dev) if colors else None
+            out_dens = torch.empty(p, device=dev)
+            proj = torch.empty(p, k, 3, device=dev) if tab is not None else None
+            if p > 0:
+                lib = _cabi.lib()
+                nbytes = lib.mipnerf_b200_radiance_dirs_workspace_bytes(C.byref(cfg), p, nd, prec)
+                if nbytes == 0:
+                    raise NotImplementedError(f"{name}: precision {self.precision!r} does not take this model")
+                scratch = _Workspace.get(dev, nbytes)
+                rgb_ptr = _ptr(out_rgb)
+                with torch.cuda.device(dev):
+                    _cabi.check(lib.mipnerf_b200_query_radiance_dirs(
+                        C.byref(cfg), C.byref(ws), m.data_ptr(), _ptr(c), p, dd.data_ptr(), nd, prec,
+                        rgb_ptr if raw else None, None if raw else rgb_ptr, out_dens.data_ptr() if raw else None,
+                        None if raw else out_dens.data_ptr(), _ptr(tab), k, int(raw), _ptr(proj),
+                        scratch.data_ptr(), scratch.numel(), _stream(dev)), f"MipNerf.{name}")
+        return (out_rgb.reshape(*shape, nd, 3) if colors else None, out_dens.reshape(shape),
+                proj.reshape(*shape, k, 3) if proj is not None else None)
+
     def _forward(self, rays: Rays, randomized: bool, white_bkgd: bool, t_rand, u_jitter, density_normal,
                  return_inds: bool):
         """The launches of `forward` -> (LevelOutputs, config, rng or None, per-level density normals or None,
