@@ -322,7 +322,8 @@ int mipnerf_b200_sample_along_rays(const mipnerf_b200_rays* rays, int num_sample
 int mipnerf_b200_cast_rays(const mipnerf_b200_rays* rays, const float* t_samples, int num_samples,
                            float* means, float* covs, void* stream);
 
-/* integrated_pos_enc, diagonal (models/mip.py:322-350): means, covs [M,3] -> out [M, 6*(max-min)]. */
+/* integrated_pos_enc, diagonal (models/mip.py:322-350): means, covs [M,3] -> out [M, 6*(max-min)].
+ * -60 <= min_deg <= max_deg <= 60 (here and in pos_enc); an empty range is an [M, 0] output. */
 int mipnerf_b200_integrated_pos_enc(const float* means, const float* covs, int64_t num_points,
                                     int min_deg, int max_deg, float* out, void* stream);
 
@@ -340,20 +341,25 @@ int mipnerf_b200_mlp_forward(const mipnerf_b200_config* cfg, const mipnerf_b200_
 size_t mipnerf_b200_mlp_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_rays,
                                         int samples_per_ray, int precision);
 
-/* volumetric_rendering (models/mip.py:366-401): rgb [B,N,3], density [B,N,1] already activated. */
+/* volumetric_rendering (models/mip.py:366-401): rgb [B,N,3], density [B,N,1] already activated.
+ * num_samples N in {32, 64, 96, 128, 192, 256} (the forward's set); any other N >= 1 is EUNSUPPORTED. */
 int mipnerf_b200_volumetric_rendering(const float* rgb, const float* density,
                                       const float* t_samples, const float* dirs, int64_t num_rays,
                                       int num_samples, int white_bkgd, float* comp_rgb,
                                       float* distance, float* acc, float* weights, void* stream);
 
 /* sorted_piecewise_constant_pdf (models/mip.py:168-229): bins [B,nb+1], weights [B,nb] (NOT
- * modified) -> samples [B,num_samples]; inds (nullable) are the searchsorted(right=True) results. */
+ * modified) -> samples [B,num_samples]; inds (nullable) are the searchsorted(right=True) results.
+ * num_bins nb a multiple of 32, <= 512 (EUNSUPPORTED otherwise: above 544 bins CPU torch sums a row in another
+ * order, so the samples would stop being bit-exact); num_samples >= 2. */
 int mipnerf_b200_sorted_piecewise_constant_pdf(const float* bins, const float* weights,
                                                int64_t num_rays, int num_bins, int num_samples,
                                                int randomized, const float* u_jitter,
                                                float* samples, int64_t* inds, void* stream);
 
-/* resample_along_rays (models/mip.py:232-280): blur-pool + padding + inverse CDF + cast_rays. */
+/* resample_along_rays (models/mip.py:232-280): blur-pool + padding + inverse CDF + cast_rays.
+ * t_samples [B,N+1], weights [B,N] -> new_t_samples [B,N+1], means/covs [B,N,3] (nullable), inds [B,N+1] (nullable);
+ * num_samples N a multiple of 32, <= 512 (EUNSUPPORTED otherwise, as for sorted_piecewise_constant_pdf). */
 int mipnerf_b200_resample_along_rays(const mipnerf_b200_rays* rays, const float* t_samples,
                                      const float* weights, int num_samples, int randomized,
                                      const float* u_jitter, float resample_padding,

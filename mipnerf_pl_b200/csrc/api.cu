@@ -37,6 +37,10 @@ constexpr int64_t kChunkRaysFp32 = 4096;  // bounds the fp32 path's activation s
 // the bf16x3 training step carries every tile image twice (hi, lo): half the chunk keeps its scratch at the 16-bit
 // step's (5.7 GiB instead of 11 GiB at the default architecture)
 constexpr int64_t kChunkRaysX3 = 2048;
+// Largest histogram the stand-alone resampler entries take.  Its row sum restates torch.sum's fp32 order, which CPU
+// torch keeps for rows of up to 544 floats and changes above that; 512 also keeps the kernel's 4 x (3 nb + 2) floats of
+// shared memory inside the 48 KiB default.  The model itself resamples at most 256 bins.
+constexpr int kMaxResampleBins = 512;
 
 inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
@@ -44,12 +48,16 @@ struct Dims {
   int xyz_dim, view_dim, n_lin;
 };
 
+// The per-ray sample counts the compositing kernel is instantiated for (launch_composite: P = N/32 in 1,2,3,4,6,8).
+int check_num_samples(int n) {
+  if (n <= 0 || n % 32 != 0 || n > 256 || n / 32 == 5 || n / 32 == 7)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "num_samples=%d: need a multiple of 32 in {32,64,96,128,192,256}", n);
+  return MIPNERF_B200_OK;
+}
+
 int check_config(const mipnerf_b200_config* c, Dims* d) {
   if (!c) return fail(MIPNERF_B200_EINVAL, "config is NULL");
-  if (c->num_samples <= 0 || c->num_samples % 32 != 0 || c->num_samples > 256 ||
-      (c->num_samples / 32 == 5) || (c->num_samples / 32 == 7))
-    return fail(MIPNERF_B200_EUNSUPPORTED, "num_samples=%d: need a multiple of 32 in {32,64,96,128,192,256}",
-                c->num_samples);
+  if (int rc = check_num_samples(c->num_samples)) return rc;
   if (c->num_levels < 1) return fail(MIPNERF_B200_EINVAL, "num_levels=%d", c->num_levels);
   if (c->max_deg_point <= c->min_deg_point || c->min_deg_point < -60 || c->max_deg_point > 60)
     return fail(MIPNERF_B200_EINVAL, "bad point degrees [%d,%d)", c->min_deg_point, c->max_deg_point);
@@ -1371,8 +1379,9 @@ int mipnerf_b200_cast_rays(const mipnerf_b200_rays* rays, const float* t_samples
 
 int mipnerf_b200_integrated_pos_enc(const float* means, const float* covs, int64_t num_points, int min_deg,
                                     int max_deg, float* out, void* stream) {
-  if (num_points < 0 || (num_points > 0 && (!means || !covs || !out)) || max_deg <= min_deg ||
-      min_deg < -60 || max_deg > 60)
+  // an empty degree range is an [M, 0] encoding, as in the reference: nothing to read or write
+  if (num_points < 0 || max_deg < min_deg || min_deg < -60 || max_deg > 60 ||
+      (num_points > 0 && max_deg > min_deg && (!means || !covs || !out)))
     return fail(MIPNERF_B200_EINVAL, "bad argument");
   CUDA_TRY(mipnerf::launch_ipe(means, covs, out, num_points, min_deg, max_deg, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
@@ -1380,7 +1389,9 @@ int mipnerf_b200_integrated_pos_enc(const float* means, const float* covs, int64
 
 int mipnerf_b200_pos_enc(const float* x, int64_t num_points, int min_deg, int max_deg, int append_identity,
                          float* out, void* stream) {
-  if (num_points < 0 || (num_points > 0 && (!x || !out)) || max_deg < min_deg || min_deg < -60 || max_deg > 60)
+  const bool empty = max_deg == min_deg && !append_identity;  // an [M, 0] output: nothing to read or write
+  if (num_points < 0 || max_deg < min_deg || min_deg < -60 || max_deg > 60 ||
+      (num_points > 0 && !empty && (!x || !out)))
     return fail(MIPNERF_B200_EINVAL, "bad argument");
   CUDA_TRY(mipnerf::launch_pos_enc(x, out, num_points, min_deg, max_deg, append_identity, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
@@ -1454,15 +1465,13 @@ int mipnerf_b200_volumetric_rendering(const float* rgb, const float* density, co
                                       float* comp_rgb, float* distance, float* acc, float* weights,
                                       void* stream) {
   if (num_rays < 0 || num_samples < 1) return fail(MIPNERF_B200_EINVAL, "bad sizes");
+  // the kernel reads each ray's rows with a compile-time stride: any other count would be read as a smaller one
+  if (int rc = check_num_samples(num_samples)) return rc;
   if (num_rays == 0) return MIPNERF_B200_OK;
   if (!rgb || !density || !t_samples || !dirs || !comp_rgb || !distance || !acc)
     return fail(MIPNERF_B200_EINVAL, "NULL tensor");
-  cudaError_t e = mipnerf::launch_composite(rgb, density, t_samples, dirs, comp_rgb, distance, acc, weights,
-                                            num_rays, num_samples, white_bkgd, 0, 0.f, 1.f, 0.f,
-                                            (cudaStream_t)stream);
-  if (e == cudaErrorInvalidValue)
-    return fail(MIPNERF_B200_EUNSUPPORTED, "num_samples=%d: need a multiple of 32 in {32..256}", num_samples);
-  CUDA_TRY(e);
+  CUDA_TRY(mipnerf::launch_composite(rgb, density, t_samples, dirs, comp_rgb, distance, acc, weights, num_rays,
+                                     num_samples, white_bkgd, 0, 0.f, 1.f, 0.f, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 
@@ -1471,8 +1480,8 @@ int mipnerf_b200_sorted_piecewise_constant_pdf(const float* bins, const float* w
                                                const float* u_jitter, float* samples, int64_t* inds,
                                                void* stream) {
   if (num_rays < 0 || num_bins < 1 || num_samples < 2) return fail(MIPNERF_B200_EINVAL, "bad sizes");
-  if (num_bins % 32 != 0 || num_bins > 1024)
-    return fail(MIPNERF_B200_EUNSUPPORTED, "num_bins=%d: need a multiple of 32, <= 1024", num_bins);
+  if (num_bins % 32 != 0 || num_bins > kMaxResampleBins)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "num_bins=%d: need a multiple of 32, <= %d", num_bins, kMaxResampleBins);
   if (num_rays == 0) return MIPNERF_B200_OK;
   if (!bins || !weights || !samples || (randomized && !u_jitter)) return fail(MIPNERF_B200_EINVAL, "NULL tensor");
   CUDA_TRY(mipnerf::launch_resample(bins, weights, mipnerf::draws_from_array(randomized ? u_jitter : nullptr), samples,
@@ -1486,8 +1495,9 @@ int mipnerf_b200_resample_along_rays(const mipnerf_b200_rays* rays, const float*
                                      int64_t* inds, void* stream) {
   int rc;
   if ((rc = check_rays(rays))) return rc;
-  if (num_samples < 32 || num_samples % 32 != 0 || num_samples > 1024)
-    return fail(MIPNERF_B200_EUNSUPPORTED, "num_samples=%d: need a multiple of 32, <= 1024", num_samples);
+  if (num_samples < 32 || num_samples % 32 != 0 || num_samples > kMaxResampleBins)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "num_samples=%d: need a multiple of 32, <= %d", num_samples,
+                kMaxResampleBins);
   if (rays->num_rays == 0) return MIPNERF_B200_OK;
   if (!t_samples || !weights || !new_t_samples || (randomized && !u_jitter))
     return fail(MIPNERF_B200_EINVAL, "NULL tensor");

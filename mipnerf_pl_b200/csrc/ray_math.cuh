@@ -161,8 +161,9 @@ __device__ __forceinline__ void lift_gaussian(const RayGeom& g, float t_mean, fl
 // One IPE feature pair for coordinate value `m`, variance `v`, degree l (scale 2^l):
 //   sin-half  exp(-0.5*v*4^l) * sin(m*2^l)
 //   cos-half  exp(-0.5*v*4^l) * sin(fl32(m*2^l + fl32(pi/2)))        (models/mip.py:335-350,:286)
-// When the damping factor underflows to exactly 0 the feature is +-0 whatever sin returns, so the
-// sine (and its slow large-argument path) is skipped — bit-identical up to the sign of zero.
+// When the damping factor underflows to exactly 0 the feature is +-0 for any finite sin(y), so the
+// sine (and its slow large-argument path) is skipped — bit-identical up to the sign of zero, and NaN
+// where the reference's sin(y) is NaN.
 template <bool kFast>
 __device__ __forceinline__ void ipe_pair(float m, float v, int l, float& f_sin, float& f_cos);
 
@@ -179,13 +180,13 @@ __device__ __forceinline__ void ipe_pair<false>(float m, float v, int l, float& 
   const float scale = __int_as_float((127 + l) << 23);       // 2^l
   const float scale_sq = __int_as_float((127 + 2 * l) << 23);  // 4^l
   const float e_arg = __fmul_rn(-0.5f, __fmul_rn(v, scale_sq));
+  const float y = __fmul_rn(m, scale);
   if (e_arg < -104.0f) {  // expf(x) == 0 for x < -103.98
-    f_sin = 0.0f;
-    f_cos = 0.0f;
+    // the reference's 0 * sin(y) is NaN when y is NaN or infinite (a non-finite mean); +-0 otherwise
+    f_sin = f_cos = isfinite(y) ? 0.0f : CUDART_NAN_F;
     return;
   }
   const float e = expf(e_arg);
-  const float y = __fmul_rn(m, scale);
   f_sin = __fmul_rn(e, sinf(y));
   f_cos = __fmul_rn(e, sinf(__fadd_rn(y, MIPNERF_HALF_PI_F32)));
 }

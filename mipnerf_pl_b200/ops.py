@@ -139,7 +139,9 @@ def sample_along_rays(origins, directions, radii, num_samples, near, far, random
 
 def sorted_piecewise_constant_pdf(bins, weights, num_samples, randomized,
                                   u_jitter: Optional[torch.Tensor] = None, return_inds: bool = False):
-    """models/mip.py:168-229.  `weights` is NOT modified (the reference pads it in place)."""
+    """models/mip.py:168-229.  `weights` is NOT modified (the reference pads it in place).
+    weights [B, nb] with nb a multiple of 32 up to 512, num_samples >= 2; other sizes raise NotImplementedError
+    (above 544 bins CPU torch sums a row in another order, so the samples would stop being bit-exact)."""
     dev = _dev(bins)
     bn, w = _f32(bins), _f32(weights)
     b, nb = w.shape
@@ -158,7 +160,8 @@ def sorted_piecewise_constant_pdf(bins, weights, num_samples, randomized,
 def resample_along_rays(origins, directions, radii, t_samples, weights, randomized, ray_shape, stop_grad,
                         resample_padding, u_jitter: Optional[torch.Tensor] = None, return_inds: bool = False):
     """models/mip.py:232-280 -> (new_t [B,N+1], (means, covs)).  Forward only, so `stop_grad`
-    (which only changes autograd in the reference) has no effect on the values."""
+    (which only changes autograd in the reference) has no effect on the values.  weights [B, N] with N a multiple
+    of 32 up to 512; other sizes raise NotImplementedError, as in sorted_piecewise_constant_pdf."""
     if ray_shape == "cylinder":
         raise NotImplementedError
     assert ray_shape == "cone"
@@ -213,7 +216,8 @@ def pos_enc(x, min_deg, max_deg, append_identity=True):
 
 
 def volumetric_rendering(rgb, density, t_samples, dirs, white_bkgd):
-    """models/mip.py:366-401 -> (comp_rgb [B,3], distance [B], acc [B], weights [B,N])."""
+    """models/mip.py:366-401 -> (comp_rgb [B,3], distance [B], acc [B], weights [B,N]).
+    N in {32, 64, 96, 128, 192, 256}, the forward's sample counts; any other N raises NotImplementedError."""
     dev = _dev(rgb)
     r, d, t, dd = _f32(rgb), _f32(density), _f32(t_samples), _f32(dirs)
     b, n = r.shape[0], r.shape[1]

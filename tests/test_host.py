@@ -219,6 +219,30 @@ def test_training_and_dataset_entry_points_validate_arguments_without_gpu(lib):
                                              None, None) == _cabi.EINVAL
     assert lib.mipnerf_b200_distloss(None, None, -1, 128, None, None) == _cabi.EINVAL
     assert lib.mipnerf_b200_distloss(None, None, 0, 128, None, None) == _cabi.OK
+    # per-stage ray entry points: sample / bin counts the kernels do not take are refused before any launch
+    p = 0x10000
+    rc = lib.mipnerf_b200_volumetric_rendering(p, p, p, p, 4, 100, 1, p, p, p, p, None)
+    assert rc == _cabi.EUNSUPPORTED and b"num_samples=100" in lib.mipnerf_b200_last_error()
+    assert lib.mipnerf_b200_volumetric_rendering(None, None, None, None, 0, 256, 1, None, None, None, None,
+                                                 None) == _cabi.OK
+    for nb in (544, 1024):
+        rc = lib.mipnerf_b200_sorted_piecewise_constant_pdf(p, p, 4, nb, nb + 1, 0, None, p, p, None)
+        assert rc == _cabi.EUNSUPPORTED and b"num_bins" in lib.mipnerf_b200_last_error(), nb
+    assert lib.mipnerf_b200_sorted_piecewise_constant_pdf(None, None, 0, 512, 513, 0, None, None, None,
+                                                          None) == _cabi.OK
+    rays = _cabi.RaysStruct(p, p, None, p, p, p, 4)
+    rc = lib.mipnerf_b200_resample_along_rays(C.byref(rays), p, p, 1024, 0, None, 0.01, p, p, p, p, None)
+    assert rc == _cabi.EUNSUPPORTED and b"num_samples=1024" in lib.mipnerf_b200_last_error()
+    rays.num_rays = 0
+    assert lib.mipnerf_b200_resample_along_rays(C.byref(rays), None, None, 512, 0, None, 0.01, None, None, None, None,
+                                                None) == _cabi.OK
+    # encodings: -60 <= min_deg <= max_deg <= 60; an empty degree range is an [M, 0] output with nothing to touch
+    for lo, hi in ((5, 2), (-61, 0), (0, 61)):
+        assert lib.mipnerf_b200_integrated_pos_enc(p, p, 4, lo, hi, p, None) == _cabi.EINVAL, (lo, hi)
+        assert lib.mipnerf_b200_pos_enc(p, 4, lo, hi, 1, p, None) == _cabi.EINVAL, (lo, hi)
+    assert lib.mipnerf_b200_integrated_pos_enc(None, None, 4, 3, 3, None, None) == _cabi.OK
+    assert lib.mipnerf_b200_pos_enc(None, 4, 3, 3, 0, None, None) == _cabi.OK
+    assert lib.mipnerf_b200_pos_enc(None, 4, 3, 3, 1, None, None) == _cabi.EINVAL   # the identity columns remain
 
 
 def test_public_header_is_plain_c_and_links(tmp_path):
