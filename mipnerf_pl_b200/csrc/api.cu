@@ -1,5 +1,6 @@
 // api.cu — the extern "C" surface declared in include/mipnerf_b200.h and the level loop of
 // MipNerf.forward (models/mip_nerf.py:172-248) expressed as kernel launches on one stream.
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -42,7 +43,8 @@ constexpr int64_t kChunkRaysX3 = 2048;
 // shared memory inside the 48 KiB default.  The model itself resamples at most 256 bins.
 constexpr int kMaxResampleBins = 512;
 
-inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
+using mipnerf::align_up;
+using mipnerf::Carver;
 
 struct Dims {
   int xyz_dim, view_dim, n_lin;
@@ -109,6 +111,28 @@ int check_weights(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b20
   return expect(d.n_lin - 1, c->net_width_condition, 3, "color_layer");
 }
 
+// The precondition of the entry points that run the level kernels: `precision` runs on the tensor cores for this
+// config, and w->packed is an image of that precision, at least tc_packed_bytes long.
+int check_tc(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, int precision, const char* what) {
+  if (!mipnerf::tc_supported(c, precision))
+    return fail(MIPNERF_B200_EUNSUPPORTED,
+                "tensor-core %s: the 8x256 / 1x128 model with num_samples 128 or 256, min_deg_point 0, max_deg_point "
+                "1..16, deg_view 1..4 and precision bf16|fp16|fp16x3|bf16x3 only; use MIPNERF_B200_FP32",
+                what);
+  const size_t need = mipnerf::tc_packed_bytes(c, precision);
+  if (!w->packed || w->packed_precision != precision || w->packed_bytes < need)
+    return fail(MIPNERF_B200_EINVAL, "weights->packed missing, packed for another precision or shorter than %zu bytes",
+                need);
+  return MIPNERF_B200_OK;
+}
+
+// Floats of the wgrad partial sums: kWgradMaxSlices slices of [n, k + 1] for the widest layer of the MLP
+size_t wgrad_part_floats(const mipnerf_b200_config* c, const Dims& d) {
+  const size_t max_n = std::max(c->net_width, c->net_width_condition);
+  const size_t max_k = (size_t)c->net_width + std::max(d.xyz_dim, d.view_dim) + 1;
+  return (size_t)mipnerf::kWgradMaxSlices * max_n * max_k;
+}
+
 int check_rays(const mipnerf_b200_rays* r) {
   if (!r) return fail(MIPNERF_B200_EINVAL, "rays is NULL");
   if (r->num_rays < 0) return fail(MIPNERF_B200_EINVAL, "num_rays=%lld", (long long)r->num_rays);
@@ -139,29 +163,22 @@ Fp32Scratch carve_fp32(const mipnerf_b200_config* c, const Dims& d, int64_t rays
                        bool mlp_only = false) {
   Fp32Scratch s{};
   const size_t m = (size_t)rays * c->num_samples;
-  size_t off = 0;
-  auto take = [&](size_t elems) {
-    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-    off += align_up(elems * sizeof(float));
-    return p;
-  };
-  s.h0 = take(m * c->net_width);
-  s.h1 = take(m * c->net_width);
-  s.c0 = take(m * c->net_width_condition);
-  s.c1 = take(m * c->net_width_condition);
-  if (mlp_only) {
-    s.bytes = off;
-    return s;
+  Carver cv{base};
+  s.h0 = cv.floats(m * c->net_width);
+  s.h1 = cv.floats(m * c->net_width);
+  s.c0 = cv.floats(m * c->net_width_condition);
+  s.c1 = cv.floats(m * c->net_width_condition);
+  if (!mlp_only) {
+    s.enc = cv.floats(m * d.xyz_dim);
+    s.venc = cv.floats((size_t)rays * d.view_dim);
+    s.raw_rgb = cv.floats(m * 3);
+    s.raw_density = cv.floats(m);
+    for (int i = 0; i < 2; ++i) {
+      s.t[i] = cv.floats((size_t)rays * (c->num_samples + 1));
+      s.w[i] = cv.floats(m);
+    }
   }
-  s.enc = take(m * d.xyz_dim);
-  s.venc = take((size_t)rays * d.view_dim);
-  s.raw_rgb = take(m * 3);
-  s.raw_density = take(m);
-  for (int i = 0; i < 2; ++i) {
-    s.t[i] = take((size_t)rays * (c->num_samples + 1));
-    s.w[i] = take(m);
-  }
-  s.bytes = off;
+  s.bytes = cv.off;
   return s;
 }
 
@@ -237,10 +254,8 @@ int mipnerf_b200_abi_version(void) { return MIPNERF_B200_ABI_VERSION; }
 size_t mipnerf_b200_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_rays, int precision) {
   Dims d;
   if (check_config(cfg, &d) != MIPNERF_B200_OK || num_rays < 0) return 0;
-  if (precision == MIPNERF_B200_FP32) {
-    const int64_t r = num_rays < kChunkRaysFp32 ? num_rays : kChunkRaysFp32;
-    return carve_fp32(cfg, d, r > 0 ? r : 1, nullptr).bytes;
-  }
+  if (precision == MIPNERF_B200_FP32)
+    return carve_fp32(cfg, d, std::clamp<int64_t>(num_rays, 1, kChunkRaysFp32), nullptr).bytes;
   return mipnerf::tc_workspace_bytes(cfg, num_rays, precision);
 }
 
@@ -303,17 +318,10 @@ static int forward_impl(const mipnerf_b200_config* cfg, const mipnerf_b200_weigh
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
   const int n = cfg->num_samples;
-  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const float rgb_scale = mipnerf::rgb_scale_of(cfg);
 
   if (precision != MIPNERF_B200_FP32) {
-    if (!mipnerf::tc_supported(cfg, precision))
-      return fail(MIPNERF_B200_EUNSUPPORTED,
-                  "tensor-core path supports the 8x256 / 1x128 model with num_samples 128 or 256, min_deg_point 0, "
-                  "max_deg_point 1..16, "
-                  "deg_view 1..4 and precision bf16|fp16|fp16x3|bf16x3; use MIPNERF_B200_FP32 for other shapes");
-    if (!w->packed || w->packed_precision != precision ||
-        w->packed_bytes < mipnerf::tc_packed_bytes(cfg, precision))
-      return fail(MIPNERF_B200_EINVAL, "weights->packed missing or packed for another precision");
+    if ((rc = check_tc(cfg, w, precision, "forward"))) return rc;
     cudaError_t e = mipnerf::tc_forward(cfg, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision,
                                         outs, workspace, workspace_bytes, st);
     if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "tc_forward: %s", cudaGetErrorString(e));
@@ -408,34 +416,27 @@ constexpr size_t kTrainImageBytes = 131072;  // 256 x 256 x 16 bit
 TrainScratch carve_train(const mipnerf_b200_config* c, const Dims& d, int64_t rays, void* base) {
   TrainScratch s{};
   const size_t m = (size_t)rays * c->num_samples;
-  size_t off = 0;
-  auto take = [&](size_t elems) {
-    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-    off += align_up(elems * sizeof(float));
-    return p;
-  };
-  s.enc = take(m * d.xyz_dim);
-  s.venc = take((size_t)rays * d.view_dim);
-  for (int i = 0; i < c->net_depth; ++i) s.h[i] = take(m * c->net_width);
-  s.bott = take(m * c->net_width);
-  s.v = take(m * c->net_width_condition);
-  s.raw_rgb = take(m * 3);
-  s.raw_density = take(m);
-  s.d_a = take(m * c->net_width);
-  s.d_b = take(m * c->net_width);
-  s.d_v = take(m * c->net_width_condition);
-  s.d_raw_rgb = take(m * 3);
-  s.d_raw_density = take(m);
-  const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
-  const size_t max_k = (size_t)c->net_width + (d.xyz_dim > d.view_dim ? d.xyz_dim : d.view_dim) + 1;
-  s.part = take((size_t)mipnerf::kWgradMaxSlices * max_n * max_k);
+  Carver cv{base};
+  s.enc = cv.floats(m * d.xyz_dim);
+  s.venc = cv.floats((size_t)rays * d.view_dim);
+  for (int i = 0; i < c->net_depth; ++i) s.h[i] = cv.floats(m * c->net_width);
+  s.bott = cv.floats(m * c->net_width);
+  s.v = cv.floats(m * c->net_width_condition);
+  s.raw_rgb = cv.floats(m * 3);
+  s.raw_density = cv.floats(m);
+  s.d_a = cv.floats(m * c->net_width);
+  s.d_b = cv.floats(m * c->net_width);
+  s.d_v = cv.floats(m * c->net_width_condition);
+  s.d_raw_rgb = cv.floats(m * 3);
+  s.d_raw_density = cv.floats(m);
+  s.part = cv.floats(wgrad_part_floats(c, d));
   for (int i = 0; i < 2; ++i) {
-    s.t[i] = take((size_t)rays * (c->num_samples + 1));
-    s.w[i] = take(m);
+    s.t[i] = cv.floats((size_t)rays * (c->num_samples + 1));
+    s.w[i] = cv.floats(m);
   }
-  s.vrow = take((size_t)rays * c->net_width_condition);
-  s.images = reinterpret_cast<uint8_t*>(take(kTrainImages * kTrainImageBytes / sizeof(float)));
-  s.bytes = off;
+  s.vrow = cv.floats((size_t)rays * c->net_width_condition);
+  s.images = cv.bytes(kTrainImages * kTrainImageBytes);
+  s.bytes = cv.off;
   return s;
 }
 
@@ -457,41 +458,33 @@ struct FusedScratch {
 FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t rays, int precision, void* base) {
   FusedScratch s{};
   const size_t m = (size_t)rays * c->num_samples;
-  size_t off = 0;
-  auto take_bytes = [&](size_t bytes) {
-    uint8_t* p = base ? static_cast<uint8_t*>(base) + off : nullptr;
-    off += align_up(bytes);
-    return p;
-  };
-  auto take = [&](size_t elems) { return reinterpret_cast<float*>(take_bytes(elems * sizeof(float))); };
+  Carver cv{base};
   const size_t x = precision == MIPNERF_B200_BF16X3 ? 2 : 1;  // tile images per operand: hi (, lo)
   // chunk-invariant buffers first: the weight images are packed once per call into the first chunk's carve and read
   // by every chunk, so no per-ray buffer of a shorter last chunk may move onto them
-  const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
-  const size_t max_k = (size_t)c->net_width + (d.xyz_dim > d.view_dim ? d.xyz_dim : d.view_dim) + 1;
-  s.part = take((size_t)mipnerf::kWgradMaxSlices * max_n * max_k);
-  s.images = take_bytes((size_t)kTrainImages * kTrainImageBytes);
-  s.packed = take_bytes(mipnerf::tc_packed_bytes(c, precision));
+  s.part = cv.floats(wgrad_part_floats(c, d));
+  s.images = cv.bytes((size_t)kTrainImages * kTrainImageBytes);
+  s.packed = cv.bytes(mipnerf::tc_packed_bytes(c, precision));
   for (int l = 0; l < 2; ++l) {
-    s.act[l] = take_bytes(x * 9 * rays * 65536);
-    s.v[l] = take_bytes(x * rays * 32768);
-    s.raw_rgb[l] = take(m * 3);
-    s.raw_density[l] = take(m);
-    s.t[l] = take((size_t)rays * (c->num_samples + 1));
-    s.w[l] = take(m);
+    s.act[l] = cv.bytes(x * 9 * rays * 65536);
+    s.v[l] = cv.bytes(x * rays * 32768);
+    s.raw_rgb[l] = cv.floats(m * 3);
+    s.raw_density[l] = cv.floats(m);
+    s.t[l] = cv.floats((size_t)rays * (c->num_samples + 1));
+    s.w[l] = cv.floats(m);
   }
-  s.enc = take(m * d.xyz_dim);
-  s.venc = take((size_t)rays * d.view_dim);
-  s.d_raw_rgb = take(m * 3);
-  s.d_raw_density = take(m);
-  s.enc16 = take_bytes(x * rays * 32768);
-  s.relu_bits = take_bytes(m * 32);
-  s.d_v = take_bytes(x * rays * 32768);
-  s.d_a = take_bytes(x * rays * 65536);
-  s.d_b = take_bytes(x * rays * 65536);
+  s.enc = cv.floats(m * d.xyz_dim);
+  s.venc = cv.floats((size_t)rays * d.view_dim);
+  s.d_raw_rgb = cv.floats(m * 3);
+  s.d_raw_density = cv.floats(m);
+  s.enc16 = cv.bytes(x * rays * 32768);
+  s.relu_bits = cv.bytes(m * 32);
+  s.d_v = cv.bytes(x * rays * 32768);
+  s.d_a = cv.bytes(x * rays * 65536);
+  s.d_b = cv.bytes(x * rays * 65536);
   s.tcws_bytes = mipnerf::tc_workspace_bytes(c, rays, precision);
-  s.tcws = take_bytes(s.tcws_bytes);
-  s.bytes = off;
+  s.tcws = cv.bytes(s.tcws_bytes);
+  s.bytes = cv.off;
   return s;
 }
 
@@ -724,16 +717,13 @@ size_t mipnerf_b200_train_workspace_bytes_for(const mipnerf_b200_config* cfg, in
     return 0;
   if (precision == MIPNERF_B200_BF16X3) {  // the fused step only, in chunks of kChunkRaysX3
     if (!train_fused_supported(cfg, precision)) return 0;
-    const int64_t r = num_rays < kChunkRaysX3 ? num_rays : kChunkRaysX3;
-    return carve_fused(cfg, d, r > 0 ? r : 1, precision, nullptr).bytes;
+    return carve_fused(cfg, d, std::clamp<int64_t>(num_rays, 1, kChunkRaysX3), precision, nullptr).bytes;
   }
   if (precision != MIPNERF_B200_FP32 && precision != MIPNERF_B200_BF16 && precision != MIPNERF_B200_FP16) return 0;
-  const int64_t r = num_rays < kChunkRaysFp32 ? num_rays : kChunkRaysFp32;
-  size_t bytes = carve_train(cfg, d, r > 0 ? r : 1, nullptr).bytes;
-  if (train_fused_supported(cfg, precision)) {  // the fused tensor-core step overlays the same buffer
-    const size_t f = carve_fused(cfg, d, r > 0 ? r : 1, precision, nullptr).bytes;
-    if (f > bytes) bytes = f;
-  }
+  const int64_t r = std::clamp<int64_t>(num_rays, 1, kChunkRaysFp32);
+  size_t bytes = carve_train(cfg, d, r, nullptr).bytes;
+  if (train_fused_supported(cfg, precision))  // the fused tensor-core step overlays the same buffer
+    bytes = std::max(bytes, carve_fused(cfg, d, r, precision, nullptr).bytes);
   return bytes;
 }
 
@@ -895,7 +885,7 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
                                   const mipnerf_b200_linear_grad* grads, bool* touched, void* workspace,
                                   cudaStream_t st) {
   const int n = cfg->num_samples;
-  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   const int64_t B = rays->num_rays;
   // bf16x3: every operand of the backward is a pair of bf16 tile images, hi and lo (the 16-bit launchers' format
   // argument is then bf16, and the *_lo arguments select their split kernels)
@@ -1021,7 +1011,7 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
   const int n = cfg->num_samples, depth = cfg->net_depth;
-  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   const int64_t B = rays->num_rays;
   bool touched[kMaxTrainDepth + 8];
   for (int i = 0; i < d.n_lin; ++i) touched[i] = accumulate != 0;
@@ -1414,11 +1404,11 @@ int mipnerf_b200_mlp_forward(const mipnerf_b200_config* cfg, const mipnerf_b200_
   if (!x || !raw_rgb || !raw_density || (cfg->use_viewdirs && !view_enc))
     return fail(MIPNERF_B200_EINVAL, "NULL tensor");
   cudaStream_t st = (cudaStream_t)stream;
+  c2.num_samples = samples_per_ray;
   if (precision != MIPNERF_B200_FP32) {
     if (!mipnerf::tc_mlp_supported(cfg, samples_per_ray, precision))
       return fail(MIPNERF_B200_EUNSUPPORTED, "tensor-core MLP: default 8x256 model, 128 samples/ray only");
-    if (!w->packed || w->packed_precision != precision)
-      return fail(MIPNERF_B200_EINVAL, "weights->packed missing or packed for another precision");
+    if ((rc = check_tc(&c2, w, precision, "MLP"))) return rc;
     if (!workspace || workspace_bytes < mipnerf::tc_mlp_workspace_bytes(num_rays))
       return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes,
                   mipnerf::tc_mlp_workspace_bytes(num_rays));
@@ -1427,10 +1417,7 @@ int mipnerf_b200_mlp_forward(const mipnerf_b200_config* cfg, const mipnerf_b200_
     if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "tc_mlp_forward: %s", cudaGetErrorString(e));
     return MIPNERF_B200_OK;
   }
-  c2.num_samples = samples_per_ray;
-  const int64_t max_rows = kChunkRaysFp32 * 128;
-  int64_t per = max_rows / samples_per_ray;
-  if (per < 1) per = 1;
+  const int64_t per = std::max<int64_t>(kChunkRaysFp32 * 128 / samples_per_ray, 1);
   const size_t need = mipnerf_b200_mlp_workspace_bytes(cfg, num_rays, samples_per_ray, precision);
   if (!workspace || workspace_bytes < need)
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
@@ -1454,9 +1441,7 @@ size_t mipnerf_b200_mlp_workspace_bytes(const mipnerf_b200_config* cfg, int64_t 
   if (check_config(&c2, &d) != MIPNERF_B200_OK) return 0;
   if (precision != MIPNERF_B200_FP32) return mipnerf::tc_mlp_workspace_bytes(num_rays);
   c2.num_samples = samples_per_ray;
-  int64_t per = (kChunkRaysFp32 * 128) / samples_per_ray;
-  if (per < 1) per = 1;
-  if (per > num_rays) per = num_rays > 0 ? num_rays : 1;
+  const int64_t per = std::clamp<int64_t>(num_rays, 1, std::max<int64_t>(kChunkRaysFp32 * 128 / samples_per_ray, 1));
   return carve_fp32(&c2, d, per, nullptr, true).bytes;
 }
 
@@ -1522,27 +1507,60 @@ struct DensityScratch {
 };
 DensityScratch carve_density(const mipnerf_b200_config* c, const Dims& d, int64_t m, void* base) {
   DensityScratch s{};
-  size_t off = 0;
-  auto take = [&](size_t elems) {
-    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-    off += align_up(elems * sizeof(float));
-    return p;
-  };
-  s.zero_covs = take((size_t)m * 3);
-  s.enc = take((size_t)m * d.xyz_dim);
-  s.h0 = take((size_t)m * c->net_width);
-  s.h1 = take((size_t)m * c->net_width);
-  s.raw = take((size_t)m);
-  s.bytes = off;
+  Carver cv{base};
+  s.zero_covs = cv.floats((size_t)m * 3);
+  s.enc = cv.floats((size_t)m * d.xyz_dim);
+  s.h0 = cv.floats((size_t)m * c->net_width);
+  s.h1 = cv.floats((size_t)m * c->net_width);
+  s.raw = cv.floats((size_t)m);
+  s.bytes = cv.off;
   return s;
+}
+
+// The arguments every field query checks first: config, weights, point count, means and precision.
+int check_query(const mipnerf_b200_config* c, Dims* d, const mipnerf_b200_weights* w, int64_t num_points,
+                const float* means, int precision) {
+  int rc;
+  if ((rc = check_config(c, d))) return rc;
+  if ((rc = check_weights(c, *d, w))) return rc;
+  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
+  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
+    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
+  return MIPNERF_B200_OK;
+}
+
+// The IPE stage kernel on query points [off, off + m) into enc (models/mip.py:322-350): their covariances, or zero
+// ones in zero_covs when covs is NULL or integration is disabled.
+int query_ipe_fp32(const mipnerf_b200_config* c, const float* means, const float* covs, int64_t off, int64_t m,
+                   float* zero_covs, float* enc, cudaStream_t st) {
+  const float* cv = covs ? covs + off * 3 : nullptr;
+  if (!cv || c->disable_integration) {
+    CUDA_TRY(cudaMemsetAsync(zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
+    cv = zero_covs;
+  }
+  CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, enc, m, c->min_deg_point, c->max_deg_point, st));
+  return MIPNERF_B200_OK;
+}
+
+// The density of m points from their IPE features (models/mip_nerf.py:93-98, 237): the fp32 trunk in h0 / h1 (*h: its
+// output), density_layer into raw and, unless density is NULL, the softplus into density.
+int density_fp32(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w, const float* enc,
+                 int64_t m, float* h0, float* h1, const float** h, float* raw, float* density, cudaStream_t st) {
+  int rc;
+  if ((rc = trunk_fp32(c, d, w, enc, m, h0, h1, h, st))) return rc;
+  const mipnerf_b200_linear& dl = w->linears[c->net_depth];
+  CUDA_TRY(mipnerf::launch_linear_f32(*h, c->net_width, c->net_width, nullptr, 0, 0, 1, dl.weight, dl.bias, raw, 1, m,
+                                      1, 0, st));
+  if (density) CUDA_TRY(mipnerf::launch_density_activation(raw, density, m, c->density_bias, st));
+  return MIPNERF_B200_OK;
 }
 }  // namespace
 
 size_t mipnerf_b200_density_workspace_bytes(const mipnerf_b200_config* cfg, int64_t num_points, int precision) {
   Dims d;
   if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0 || precision != MIPNERF_B200_FP32) return 0;
-  const int64_t m = num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32;
-  return carve_density(cfg, d, m > 0 ? m : 1, nullptr).bytes;
+  return carve_density(cfg, d, std::clamp<int64_t>(num_points, 1, kChunkPointsFp32), nullptr).bytes;
 }
 
 int mipnerf_b200_query_density(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
@@ -1550,21 +1568,9 @@ int mipnerf_b200_query_density(const mipnerf_b200_config* cfg, const mipnerf_b20
                                float* density, void* workspace, size_t workspace_bytes, void* stream) {
   Dims d;
   int rc;
-  if ((rc = check_config(cfg, &d))) return rc;
-  if ((rc = check_weights(cfg, d, w))) return rc;
-  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if ((rc = check_query(cfg, &d, w, num_points, means, precision))) return rc;
   if (!raw_density && !density) return fail(MIPNERF_B200_EINVAL, "raw_density and density are both NULL");
-  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
-  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
-    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
-  if (precision != MIPNERF_B200_FP32) {
-    if (!mipnerf::tc_supported(cfg, precision))
-      return fail(MIPNERF_B200_EUNSUPPORTED,
-                  "tensor-core density query: the forward's tensor-core shapes only (8x256 / 1x128 model, "
-                  "num_samples 128 or 256, min_deg_point 0, max_deg_point 1..16, deg_view 1..4); use MIPNERF_B200_FP32");
-    if (!w->packed || w->packed_precision != precision || w->packed_bytes < mipnerf::tc_packed_bytes(cfg, precision))
-      return fail(MIPNERF_B200_EINVAL, "weights->packed missing or packed for another precision");
-  }
+  if (precision != MIPNERF_B200_FP32 && (rc = check_tc(cfg, w, precision, "density query"))) return rc;
   const size_t need = mipnerf_b200_density_workspace_bytes(cfg, num_points, precision);
   if (num_points > 0 && need > 0 && (!workspace || workspace_bytes < need))
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
@@ -1575,23 +1581,14 @@ int mipnerf_b200_query_density(const mipnerf_b200_config* cfg, const mipnerf_b20
     if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "tc_query_density: %s", cudaGetErrorString(e));
     return MIPNERF_B200_OK;
   }
-  // fp32: the IPE stage kernel, the fp32 trunk and density_layer (models/mip.py:322-350, models/mip_nerf.py:93-98)
-  const mipnerf_b200_linear& dl = w->linears[cfg->net_depth];
   for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
-    const int64_t m = (num_points - off) < kChunkPointsFp32 ? (num_points - off) : kChunkPointsFp32;
+    const int64_t m = std::min(num_points - off, kChunkPointsFp32);
     const DensityScratch s = carve_density(cfg, d, m, workspace);
-    const float* cv = covs ? covs + off * 3 : nullptr;
-    if (!cv || cfg->disable_integration) {
-      CUDA_TRY(cudaMemsetAsync(s.zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
-      cv = s.zero_covs;
-    }
-    CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, s.enc, m, cfg->min_deg_point, cfg->max_deg_point, st));
     const float* h;
-    if ((rc = trunk_fp32(cfg, d, w, s.enc, m, s.h0, s.h1, &h, st))) return rc;
-    float* raw = raw_density ? raw_density + off : s.raw;
-    CUDA_TRY(mipnerf::launch_linear_f32(h, cfg->net_width, cfg->net_width, nullptr, 0, 0, 1, dl.weight, dl.bias, raw, 1,
-                                        m, 1, 0, st));
-    if (density) CUDA_TRY(mipnerf::launch_density_activation(raw, density + off, m, cfg->density_bias, st));
+    if ((rc = query_ipe_fp32(cfg, means, covs, off, m, s.zero_covs, s.enc, st))) return rc;
+    if ((rc = density_fp32(cfg, d, w, s.enc, m, s.h0, s.h1, &h, raw_density ? raw_density + off : s.raw,
+                           density ? density + off : nullptr, st)))
+      return rc;
   }
   return MIPNERF_B200_OK;
 }
@@ -1604,22 +1601,17 @@ struct RadianceScratch {
 };
 RadianceScratch carve_radiance(const mipnerf_b200_config* c, const Dims& d, int64_t m, void* base) {
   RadianceScratch s{};
-  size_t off = 0;
-  auto take = [&](size_t elems) {
-    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-    off += align_up(elems * sizeof(float));
-    return p;
-  };
-  s.zero_covs = take((size_t)m * 3);
-  s.enc = take((size_t)m * d.xyz_dim);
-  s.venc = take((size_t)m * d.view_dim);
-  s.raw_rgb = take((size_t)m * 3);
-  s.raw_density = take((size_t)m);
-  s.mlp.h0 = take((size_t)m * c->net_width);
-  s.mlp.h1 = take((size_t)m * c->net_width);
-  s.mlp.c0 = take((size_t)m * c->net_width_condition);
-  s.mlp.c1 = take((size_t)m * c->net_width_condition);
-  s.bytes = off;
+  Carver cv{base};
+  s.zero_covs = cv.floats((size_t)m * 3);
+  s.enc = cv.floats((size_t)m * d.xyz_dim);
+  s.venc = cv.floats((size_t)m * d.view_dim);
+  s.raw_rgb = cv.floats((size_t)m * 3);
+  s.raw_density = cv.floats((size_t)m);
+  s.mlp.h0 = cv.floats((size_t)m * c->net_width);
+  s.mlp.h1 = cv.floats((size_t)m * c->net_width);
+  s.mlp.c0 = cv.floats((size_t)m * c->net_width_condition);
+  s.mlp.c1 = cv.floats((size_t)m * c->net_width_condition);
+  s.bytes = cv.off;
   return s;
 }
 }  // namespace
@@ -1629,8 +1621,7 @@ size_t mipnerf_b200_radiance_workspace_bytes(const mipnerf_b200_config* cfg, int
   if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0) return 0;
   if (precision != MIPNERF_B200_FP32)
     return mipnerf::tc_supported(cfg, precision) ? mipnerf::tc_radiance_workspace_bytes(num_points) : 0;
-  const int64_t m = num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32;
-  return carve_radiance(cfg, d, m > 0 ? m : 1, nullptr).bytes;
+  return carve_radiance(cfg, d, std::clamp<int64_t>(num_points, 1, kChunkPointsFp32), nullptr).bytes;
 }
 
 int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
@@ -1639,23 +1630,11 @@ int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b2
                                 size_t workspace_bytes, void* stream) {
   Dims d;
   int rc;
-  if ((rc = check_config(cfg, &d))) return rc;
-  if ((rc = check_weights(cfg, d, w))) return rc;
-  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if ((rc = check_query(cfg, &d, w, num_points, means, precision))) return rc;
   if (!raw_rgb && !raw_density && !rgb && !density) return fail(MIPNERF_B200_EINVAL, "every output is NULL");
-  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
   if (num_points > 0 && cfg->use_viewdirs && !viewdirs)
     return fail(MIPNERF_B200_EINVAL, "viewdirs is NULL with use_viewdirs");
-  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
-    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
-  if (precision != MIPNERF_B200_FP32) {
-    if (!mipnerf::tc_supported(cfg, precision))
-      return fail(MIPNERF_B200_EUNSUPPORTED,
-                  "tensor-core radiance query: the forward's tensor-core shapes only (8x256 / 1x128 model, "
-                  "num_samples 128 or 256, min_deg_point 0, max_deg_point 1..16, deg_view 1..4); use MIPNERF_B200_FP32");
-    if (!w->packed || w->packed_precision != precision || w->packed_bytes < mipnerf::tc_packed_bytes(cfg, precision))
-      return fail(MIPNERF_B200_EINVAL, "weights->packed missing or packed for another precision");
-  }
+  if (precision != MIPNERF_B200_FP32 && (rc = check_tc(cfg, w, precision, "radiance query"))) return rc;
   const size_t need = mipnerf_b200_radiance_workspace_bytes(cfg, num_points, precision);
   if (num_points > 0 && (need == 0 || !workspace || workspace_bytes < need))
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
@@ -1669,16 +1648,11 @@ int mipnerf_b200_query_radiance(const mipnerf_b200_config* cfg, const mipnerf_b2
   }
   // fp32: the IPE stage kernel, the view-direction encoding and the fp32 MLP with one sample per "ray" (each point its
   // own view encoding), then the activations (models/mip.py:322-363, models/mip_nerf.py:75-111, 236-237)
-  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
-    const int64_t m = (num_points - off) < kChunkPointsFp32 ? (num_points - off) : kChunkPointsFp32;
+    const int64_t m = std::min(num_points - off, kChunkPointsFp32);
     const RadianceScratch s = carve_radiance(cfg, d, m, workspace);
-    const float* cv = covs ? covs + off * 3 : nullptr;
-    if (!cv || cfg->disable_integration) {
-      CUDA_TRY(cudaMemsetAsync(s.zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
-      cv = s.zero_covs;
-    }
-    CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, s.enc, m, cfg->min_deg_point, cfg->max_deg_point, st));
+    if ((rc = query_ipe_fp32(cfg, means, covs, off, m, s.zero_covs, s.enc, st))) return rc;
     if (cfg->use_viewdirs) CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, s.venc, m, 0, cfg->deg_view, 1, st));
     float* rr = raw_rgb ? raw_rgb + off * 3 : s.raw_rgb;
     float* rd = raw_density ? raw_density + off : s.raw_density;
@@ -1702,23 +1676,18 @@ struct RadianceDirsScratch {
 RadianceDirsScratch carve_radiance_dirs(const mipnerf_b200_config* c, const Dims& d, int64_t m, int64_t num_dirs,
                                         int precision, void* base) {
   RadianceDirsScratch s{};
-  size_t off = 0;
-  auto take = [&](size_t elems) {
-    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-    off += align_up(elems * sizeof(float));
-    return p;
-  };
-  s.acc = take((size_t)((m + 127) / 128 * 128) * c->net_width_condition);
-  s.terms = take((size_t)num_dirs * c->net_width_condition);
+  Carver cv{base};
+  s.acc = cv.floats((size_t)((m + 127) / 128 * 128) * c->net_width_condition);
+  s.terms = cv.floats((size_t)num_dirs * c->net_width_condition);
   if (precision == MIPNERF_B200_FP32) {
-    s.zero_covs = take((size_t)m * 3);
-    s.enc = take((size_t)m * d.xyz_dim);
-    s.h0 = take((size_t)m * c->net_width);
-    s.h1 = take((size_t)m * c->net_width);
-    s.raw = take((size_t)m);
-    s.zeros = take((size_t)c->net_width_condition + d.view_dim);
+    s.zero_covs = cv.floats((size_t)m * 3);
+    s.enc = cv.floats((size_t)m * d.xyz_dim);
+    s.h0 = cv.floats((size_t)m * c->net_width);
+    s.h1 = cv.floats((size_t)m * c->net_width);
+    s.raw = cv.floats((size_t)m);
+    s.zeros = cv.floats((size_t)c->net_width_condition + d.view_dim);
   }
-  s.bytes = off;
+  s.bytes = cv.off;
   return s;
 }
 // the view layer splits into a per-point and a per-direction part only when it is the one layer before the colour head,
@@ -1735,8 +1704,8 @@ size_t mipnerf_b200_radiance_dirs_workspace_bytes(const mipnerf_b200_config* cfg
   if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0 || num_dirs < 1 ||
       precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3 || !radiance_dirs_supported(cfg, precision))
     return 0;
-  const int64_t m = num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32;
-  return carve_radiance_dirs(cfg, d, m > 0 ? m : 1, num_dirs, precision, nullptr).bytes;
+  return carve_radiance_dirs(cfg, d, std::clamp<int64_t>(num_points, 1, kChunkPointsFp32), num_dirs, precision, nullptr)
+      .bytes;
 }
 
 int mipnerf_b200_query_radiance_dirs(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
@@ -1747,40 +1716,30 @@ int mipnerf_b200_query_radiance_dirs(const mipnerf_b200_config* cfg, const mipne
   static_assert(kChunkPointsFp32 == mipnerf::kDensityChunkPoints, "one chunk size for every precision");
   Dims d;
   int rc;
-  if ((rc = check_config(cfg, &d))) return rc;
-  if ((rc = check_weights(cfg, d, w))) return rc;
-  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if ((rc = check_query(cfg, &d, w, num_points, means, precision))) return rc;
   if (num_dirs < 1) return fail(MIPNERF_B200_EINVAL, "num_dirs=%lld: need at least one direction", (long long)num_dirs);
   if (!raw_rgb && !rgb && !raw_density && !density && !proj_out) return fail(MIPNERF_B200_EINVAL, "every output is NULL");
   if (proj_out && !table) return fail(MIPNERF_B200_EINVAL, "proj_out without table");
   if (proj_out && (num_basis < 1 || num_basis > 16))
     return fail(MIPNERF_B200_EINVAL, "num_basis=%d: need 1..16 with proj_out", num_basis);
   if (!dirs) return fail(MIPNERF_B200_EINVAL, "dirs is NULL");
-  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
-  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
-    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
   if (!cfg->use_viewdirs)
     return fail(MIPNERF_B200_EUNSUPPORTED, "radiance under a direction set needs use_viewdirs (use query_radiance)");
-  if (!radiance_dirs_supported(cfg, precision)) {
-    if (precision == MIPNERF_B200_FP32)
-      return fail(MIPNERF_B200_EUNSUPPORTED, "radiance under a direction set: one 128-wide view layer only");
-    return fail(MIPNERF_B200_EUNSUPPORTED,
-                "tensor-core radiance query: the forward's tensor-core shapes only (8x256 / 1x128 model, "
-                "num_samples 128 or 256, min_deg_point 0, max_deg_point 1..16, deg_view 1..4); use MIPNERF_B200_FP32");
+  if (precision != MIPNERF_B200_FP32) {
+    if ((rc = check_tc(cfg, w, precision, "radiance query"))) return rc;
+  } else if (!radiance_dirs_supported(cfg, precision)) {
+    return fail(MIPNERF_B200_EUNSUPPORTED, "radiance under a direction set: one 128-wide view layer only");
   }
-  if (precision != MIPNERF_B200_FP32 &&
-      (!w->packed || w->packed_precision != precision || w->packed_bytes < mipnerf::tc_packed_bytes(cfg, precision)))
-    return fail(MIPNERF_B200_EINVAL, "weights->packed missing or packed for another precision");
   const size_t need = mipnerf_b200_radiance_dirs_workspace_bytes(cfg, num_points, num_dirs, precision);
   if (num_points > 0 && (need == 0 || !workspace || workspace_bytes < need))
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
   if (num_points == 0) return MIPNERF_B200_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   const mipnerf_b200_linear& vl = w->linears[cfg->net_depth + 2];
   const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
-  const RadianceDirsScratch s0 = carve_radiance_dirs(cfg, d, num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32,
-                                                     num_dirs, precision, workspace);
+  const RadianceDirsScratch s0 =
+      carve_radiance_dirs(cfg, d, std::min(num_points, kChunkPointsFp32), num_dirs, precision, workspace);
   // T: radiance mode's view-direction term of each direction (the tensor-core precisions), or the same sum over the
   // view layer's own weights (fp32)
   if (precision != MIPNERF_B200_FP32) {
@@ -1792,7 +1751,7 @@ int mipnerf_b200_query_radiance_dirs(const mipnerf_b200_config* cfg, const mipne
     CUDA_TRY(cudaMemsetAsync(s0.zeros, 0, (size_t)(cfg->net_width_condition + d.view_dim) * sizeof(float), st));
   }
   for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
-    const int64_t m = (num_points - off) < kChunkPointsFp32 ? (num_points - off) : kChunkPointsFp32;
+    const int64_t m = std::min(num_points - off, kChunkPointsFp32);
     const RadianceDirsScratch& s = s0;  // every chunk reuses the first one's scratch, in stream order
     if (precision != MIPNERF_B200_FP32) {
       cudaError_t e = mipnerf::tc_query_view_acc(cfg, w, means + off * 3, covs ? covs + off * 3 : nullptr, m, precision,
@@ -1802,20 +1761,12 @@ int mipnerf_b200_query_radiance_dirs(const mipnerf_b200_config* cfg, const mipne
     } else {
       // the IPE stage kernel, the fp32 trunk, density_layer and extra_layer, then A = [bottleneck | 0] . W_view^T + 0:
       // the view layer's sum over its bottleneck columns (models/mip.py:322-350, models/mip_nerf.py:93-107)
-      const float* cv = covs ? covs + off * 3 : nullptr;
-      if (!cv || cfg->disable_integration) {
-        CUDA_TRY(cudaMemsetAsync(s.zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
-        cv = s.zero_covs;
-      }
-      CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, s.enc, m, cfg->min_deg_point, cfg->max_deg_point, st));
       const float* h;
-      if ((rc = trunk_fp32(cfg, d, w, s.enc, m, s.h0, s.h1, &h, st))) return rc;
-      const mipnerf_b200_linear& dl = w->linears[cfg->net_depth];
+      if ((rc = query_ipe_fp32(cfg, means, covs, off, m, s.zero_covs, s.enc, st))) return rc;
+      if ((rc = density_fp32(cfg, d, w, s.enc, m, s.h0, s.h1, &h, raw_density ? raw_density + off : s.raw,
+                             density ? density + off : nullptr, st)))
+        return rc;
       const mipnerf_b200_linear& el = w->linears[cfg->net_depth + 1];
-      float* raw = raw_density ? raw_density + off : s.raw;
-      CUDA_TRY(mipnerf::launch_linear_f32(h, cfg->net_width, cfg->net_width, nullptr, 0, 0, 1, dl.weight, dl.bias, raw, 1,
-                                          m, 1, 0, st));
-      if (density) CUDA_TRY(mipnerf::launch_density_activation(raw, density + off, m, cfg->density_bias, st));
       float* bott = h == s.h0 ? s.h1 : s.h0;
       CUDA_TRY(mipnerf::launch_linear_f32(h, cfg->net_width, cfg->net_width, nullptr, 0, 0, 1, el.weight, el.bias, bott,
                                           cfg->net_width, m, cfg->net_width, 0, st));
@@ -1841,31 +1792,24 @@ struct QueryGradScratch {
 };
 QueryGradScratch carve_query_grad(const mipnerf_b200_config* c, const Dims& d, int64_t m, bool radiance, void* base) {
   QueryGradScratch s{};
-  size_t off = 0;
-  auto take = [&](size_t elems) {
-    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-    off += align_up(elems * sizeof(float));
-    return p;
-  };
-  const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
-  const size_t max_k = (size_t)c->net_width + (d.xyz_dim > d.view_dim ? d.xyz_dim : d.view_dim) + 1;
-  s.t.part = take((size_t)mipnerf::kWgradMaxSlices * max_n * max_k);
-  s.zero_covs = take((size_t)m * 3);
-  s.t.enc = take((size_t)m * d.xyz_dim);
-  for (int i = 0; i < c->net_depth; ++i) s.t.h[i] = take((size_t)m * c->net_width);
-  s.t.raw_density = take((size_t)m);
-  s.t.d_raw_density = take((size_t)m);
-  s.t.d_a = take((size_t)m * c->net_width);
-  s.t.d_b = take((size_t)m * c->net_width);
+  Carver cv{base};
+  s.t.part = cv.floats(wgrad_part_floats(c, d));
+  s.zero_covs = cv.floats((size_t)m * 3);
+  s.t.enc = cv.floats((size_t)m * d.xyz_dim);
+  for (int i = 0; i < c->net_depth; ++i) s.t.h[i] = cv.floats((size_t)m * c->net_width);
+  s.t.raw_density = cv.floats((size_t)m);
+  s.t.d_raw_density = cv.floats((size_t)m);
+  s.t.d_a = cv.floats((size_t)m * c->net_width);
+  s.t.d_b = cv.floats((size_t)m * c->net_width);
   if (radiance) {
-    s.t.venc = take((size_t)m * d.view_dim);
-    s.t.bott = take((size_t)m * c->net_width);
-    s.t.v = take((size_t)m * c->net_width_condition);
-    s.t.raw_rgb = take((size_t)m * 3);
-    s.t.d_v = take((size_t)m * c->net_width_condition);
-    s.t.d_raw_rgb = take((size_t)m * 3);
+    s.t.venc = cv.floats((size_t)m * d.view_dim);
+    s.t.bott = cv.floats((size_t)m * c->net_width);
+    s.t.v = cv.floats((size_t)m * c->net_width_condition);
+    s.t.raw_rgb = cv.floats((size_t)m * 3);
+    s.t.d_v = cv.floats((size_t)m * c->net_width_condition);
+    s.t.d_raw_rgb = cv.floats((size_t)m * 3);
   }
-  s.bytes = off;
+  s.bytes = cv.off;
   return s;
 }
 
@@ -1880,37 +1824,29 @@ struct QueryFusedScratch {
 QueryFusedScratch carve_query_fused(const mipnerf_b200_config* c, const Dims& d, int64_t m, bool radiance,
                                     void* base) {
   QueryFusedScratch s{};
-  size_t off = 0;
-  auto take_bytes = [&](size_t bytes) {
-    uint8_t* p = base ? static_cast<uint8_t*>(base) + off : nullptr;
-    off += align_up(bytes);
-    return p;
-  };
-  auto take = [&](size_t elems) { return reinterpret_cast<float*>(take_bytes(elems * sizeof(float))); };
+  Carver cv{base};
   const int64_t tiles = (m + 127) / 128, rows = tiles * 128;
   // chunk-invariant buffers first: the weight images are packed once per call into the first chunk's carve
-  const size_t max_n = c->net_width > c->net_width_condition ? c->net_width : c->net_width_condition;
-  const size_t max_k = (size_t)c->net_width + (d.xyz_dim > d.view_dim ? d.xyz_dim : d.view_dim) + 1;
-  s.part = take((size_t)mipnerf::kWgradMaxSlices * max_n * max_k);
-  s.images = take_bytes((size_t)(kMaxTrainDepth + 2) * kTrainImageBytes);
-  s.packed = take_bytes(mipnerf::tc_packed_bytes(c, MIPNERF_B200_BF16));
+  s.part = cv.floats(wgrad_part_floats(c, d));
+  s.images = cv.bytes((size_t)(kMaxTrainDepth + 2) * kTrainImageBytes);
+  s.packed = cv.bytes(mipnerf::tc_packed_bytes(c, MIPNERF_B200_BF16));
   s.slots_bytes = radiance ? mipnerf::tc_radiance_workspace_bytes(mipnerf::kDensityChunkPoints) : 0;
-  s.slots = reinterpret_cast<float*>(take_bytes(s.slots_bytes));
-  s.act = take_bytes((size_t)(radiance ? 9 : 8) * tiles * 65536);
-  s.raw_density = take((size_t)rows);
-  s.d_raw_density = take((size_t)rows);
-  s.enc16 = take_bytes((size_t)tiles * 32768);
-  s.relu_bits = take_bytes((size_t)rows * 32);
-  s.d_a = take_bytes((size_t)tiles * 65536);
-  s.d_b = take_bytes((size_t)tiles * 65536);
+  s.slots = reinterpret_cast<float*>(cv.bytes(s.slots_bytes));
+  s.act = cv.bytes((size_t)(radiance ? 9 : 8) * tiles * 65536);
+  s.raw_density = cv.floats((size_t)rows);
+  s.d_raw_density = cv.floats((size_t)rows);
+  s.enc16 = cv.bytes((size_t)tiles * 32768);
+  s.relu_bits = cv.bytes((size_t)rows * 32);
+  s.d_a = cv.bytes((size_t)tiles * 65536);
+  s.d_b = cv.bytes((size_t)tiles * 65536);
   if (radiance) {
-    s.v = take_bytes((size_t)tiles * 32768);
-    s.raw_rgb = take((size_t)rows * 3);
-    s.d_raw_rgb = take((size_t)rows * 3);
-    s.venc = take((size_t)rows * d.view_dim);
-    s.d_v = take_bytes((size_t)tiles * 32768);
+    s.v = cv.bytes((size_t)tiles * 32768);
+    s.raw_rgb = cv.floats((size_t)rows * 3);
+    s.d_raw_rgb = cv.floats((size_t)rows * 3);
+    s.venc = cv.floats((size_t)rows * d.view_dim);
+    s.d_v = cv.bytes((size_t)tiles * 32768);
   }
-  s.bytes = off;
+  s.bytes = cv.off;
   return s;
 }
 
@@ -1937,19 +1873,14 @@ int query_backward_fp32(const mipnerf_b200_config* cfg, const Dims& d, const mip
                         const mipnerf_b200_query_cotangent* cot, const mipnerf_b200_linear_grad* grads, bool* touched,
                         void* workspace, cudaStream_t st) {
   const bool radiance = viewdirs != nullptr;
-  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   const LayerImages im{};
   int rc;
   for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
-    const int64_t m = (num_points - off) < kChunkPointsFp32 ? (num_points - off) : kChunkPointsFp32;
+    const int64_t m = std::min(num_points - off, kChunkPointsFp32);
     const QueryGradScratch s = carve_query_grad(cfg, d, m, radiance, workspace);
     // the forward of the query (models/mip.py:322-363, models/mip_nerf.py:75-111), every activation kept
-    const float* cv = covs ? covs + off * 3 : nullptr;
-    if (!cv || cfg->disable_integration) {
-      CUDA_TRY(cudaMemsetAsync(s.zero_covs, 0, (size_t)m * 3 * sizeof(float), st));
-      cv = s.zero_covs;
-    }
-    CUDA_TRY(mipnerf::launch_ipe(means + off * 3, cv, s.t.enc, m, cfg->min_deg_point, cfg->max_deg_point, st));
+    if ((rc = query_ipe_fp32(cfg, means, covs, off, m, s.zero_covs, s.t.enc, st))) return rc;
     if (radiance) CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, s.t.venc, m, 0, cfg->deg_view, 1, st));
     if ((rc = mlp_forward_kept(cfg, d, w, false, MIPNERF_B200_FP32, im, s.t, m, 1, !radiance, st))) return rc;
     // the activations' VJP, then the training step's per-layer chain
@@ -1970,9 +1901,9 @@ int query_backward_bf16(const mipnerf_b200_config* cfg, const Dims& d, const mip
                         void* workspace, cudaStream_t st) {
   const bool radiance = viewdirs != nullptr;
   const int prec = MIPNERF_B200_BF16;
-  const float rgb_scale = (float)(1.0 + 2.0 * (double)cfg->rgb_padding);
+  const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   const int64_t chunk = mipnerf::kDensityChunkPoints;
-  const QueryFusedScratch s0 = carve_query_fused(cfg, d, num_points < chunk ? num_points : chunk, radiance, workspace);
+  const QueryFusedScratch s0 = carve_query_fused(cfg, d, std::min(num_points, chunk), radiance, workspace);
   mipnerf_b200_weights wl = *w;
   wl.packed = s0.packed, wl.packed_precision = prec, wl.packed_bytes = mipnerf::tc_packed_bytes(cfg, prec);
   CUDA_TRY(mipnerf::tc_pack_weights(cfg, w, prec, s0.packed, st));
@@ -1981,7 +1912,7 @@ int query_backward_bf16(const mipnerf_b200_config* cfg, const Dims& d, const mip
   CUDA_TRY(pack_bwd_images(cfg, w, prec, s0.images, img_bwd, img_bwd_lo, st));
   int rc;
   for (int64_t off = 0; off < num_points; off += chunk) {
-    const int64_t m = (num_points - off) < chunk ? (num_points - off) : chunk;
+    const int64_t m = std::min(num_points - off, chunk);
     const int64_t tiles = (m + 127) / 128, rows = tiles * 128;
     const QueryFusedScratch s = carve_query_fused(cfg, d, m, radiance, workspace);
     const float* mp = means + off * 3;
@@ -2018,9 +1949,9 @@ size_t mipnerf_b200_query_backward_workspace_bytes(const mipnerf_b200_config* cf
                                                    int precision) {
   Dims d;
   if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0 || !query_grad_supported(cfg, d, precision)) return 0;
-  const int64_t m = num_points < kChunkPointsFp32 ? num_points : kChunkPointsFp32;
-  if (precision == MIPNERF_B200_BF16) return carve_query_fused(cfg, d, m > 0 ? m : 1, radiance != 0, nullptr).bytes;
-  return carve_query_grad(cfg, d, m > 0 ? m : 1, radiance != 0, nullptr).bytes;
+  const int64_t m = std::clamp<int64_t>(num_points, 1, kChunkPointsFp32);
+  if (precision == MIPNERF_B200_BF16) return carve_query_fused(cfg, d, m, radiance != 0, nullptr).bytes;
+  return carve_query_grad(cfg, d, m, radiance != 0, nullptr).bytes;
 }
 
 int mipnerf_b200_query_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
@@ -2029,16 +1960,11 @@ int mipnerf_b200_query_backward(const mipnerf_b200_config* cfg, const mipnerf_b2
                                 int num_grads, int accumulate, void* workspace, size_t workspace_bytes, void* stream) {
   Dims d;
   int rc;
-  if ((rc = check_config(cfg, &d))) return rc;
-  if ((rc = check_weights(cfg, d, w))) return rc;
-  if (num_points < 0) return fail(MIPNERF_B200_EINVAL, "num_points=%lld", (long long)num_points);
+  if ((rc = check_query(cfg, &d, w, num_points, means, precision))) return rc;
   if (!cot || !grads) return fail(MIPNERF_B200_EINVAL, "cot / grads is NULL");
   if (num_grads != d.n_lin) return fail(MIPNERF_B200_EINVAL, "expected %d gradient pairs, got %d", d.n_lin, num_grads);
   for (int i = 0; i < d.n_lin; ++i)
     if (!grads[i].weight_grad || !grads[i].bias_grad) return fail(MIPNERF_B200_EINVAL, "grads[%d] has a NULL tensor", i);
-  if (num_points > 0 && !means) return fail(MIPNERF_B200_EINVAL, "means is NULL");
-  if (precision < MIPNERF_B200_FP32 || precision > MIPNERF_B200_BF16X3)
-    return fail(MIPNERF_B200_EINVAL, "precision %d", precision);
   if (precision == MIPNERF_B200_FP16)
     return fail(MIPNERF_B200_EUNSUPPORTED,
                 "query backward: FP16's fixed gradient scale is sized for the training loss and arbitrary cotangents "

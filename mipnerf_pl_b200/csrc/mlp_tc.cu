@@ -10,6 +10,7 @@
 // heads out: mipnerf_b200_mlp_forward).
 #include "mlp_tc.h"
 
+#include <algorithm>
 #include <cstdlib>
 #include <mutex>
 
@@ -1720,22 +1721,15 @@ struct TcScratch {
 constexpr int64_t kChunkRaysTc = 65536;
 inline int64_t tc_chunk_rays(int n) { return kChunkRaysTc * kN / n; }
 
-inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
-
 TcScratch carve_tc(int64_t rays, int n, void* base) {
   TcScratch s{};
-  size_t off = 0;
-  auto take = [&](size_t elems) {
-    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-    off += align_up(elems * sizeof(float));
-    return p;
-  };
-  s.vbias = take((size_t)rays * kCond);
+  Carver cv{base};
+  s.vbias = cv.floats((size_t)rays * kCond);
   for (int i = 0; i < 2; ++i) {
-    s.t[i] = take((size_t)rays * (n + 1));
-    s.w[i] = take((size_t)rays * n);
+    s.t[i] = cv.floats((size_t)rays * (n + 1));
+    s.w[i] = cv.floats((size_t)rays * n);
   }
-  s.bytes = off;
+  s.bytes = cv.off;
   return s;
 }
 
@@ -1775,46 +1769,38 @@ cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
   return cudaGetLastError();
 }
 
-// n = 128 or 256 samples per ray: one or two 128-row tiles per ray
-template <int kT>
-cudaError_t launch_level_tiles(const LevelParams& p, int precision, cudaStream_t st) {
-  if (is_x3(precision))
-    return fmt_of(precision) ? launch_level_t<1, true, kT>(p, st) : launch_level_t<0, true, kT>(p, st);
-  return fmt_of(precision) ? launch_level_t<1, false, kT>(p, st) : launch_level_t<0, false, kT>(p, st);
-}
-cudaError_t launch_level(const LevelParams& p, int precision, int n, cudaStream_t st) {
+// One launch of the level kernel in mode kMode with kT 128-row tiles per ray (n = 128 or 256 samples per ray), on the
+// operand format and split of `precision`.  A query's backward (p.act_dump in density / radiance mode) takes the query
+// dump variant, which exists for bf16 / fp16 only; the training forward of the split precisions is tc_forward's.
+template <int kMode, int kT = 1>
+cudaError_t launch_level(const LevelParams& p, int precision, cudaStream_t st) {
   if (p.num_rays <= 0) return cudaSuccess;
-  return n == 2 * kN ? launch_level_tiles<2>(p, precision, st) : launch_level_tiles<1>(p, precision, st);
-}
-cudaError_t launch_density(const LevelParams& p, int precision, cudaStream_t st) {
-  if (p.num_rays <= 0) return cudaSuccess;
-  if (p.act_dump)  // the backward of a query: bf16 / fp16 only (tc_query_density)
-    return fmt_of(precision) ? launch_level_t<1, false, 1, kModeDensity, false, true>(p, st)
-                             : launch_level_t<0, false, 1, kModeDensity, false, true>(p, st);
+  const bool bf = fmt_of(precision) == 1;
+  if constexpr (kMode == kModeDensity || kMode == kModeRadiance)
+    if (p.act_dump)
+      return bf ? launch_level_t<1, false, 1, kMode, false, true>(p, st)
+                : launch_level_t<0, false, 1, kMode, false, true>(p, st);
   if (is_x3(precision))
-    return fmt_of(precision) ? launch_level_t<1, true, 1, kModeDensity>(p, st)
-                             : launch_level_t<0, true, 1, kModeDensity>(p, st);
-  return fmt_of(precision) ? launch_level_t<1, false, 1, kModeDensity>(p, st)
-                           : launch_level_t<0, false, 1, kModeDensity>(p, st);
+    return bf ? launch_level_t<1, true, kT, kMode>(p, st) : launch_level_t<0, true, kT, kMode>(p, st);
+  return bf ? launch_level_t<1, false, kT, kMode>(p, st) : launch_level_t<0, false, kT, kMode>(p, st);
 }
-cudaError_t launch_radiance(const LevelParams& p, int precision, cudaStream_t st) {
-  if (p.num_rays <= 0) return cudaSuccess;
-  if (p.act_dump)
-    return fmt_of(precision) ? launch_level_t<1, false, 1, kModeRadiance, false, true>(p, st)
-                             : launch_level_t<0, false, 1, kModeRadiance, false, true>(p, st);
-  if (is_x3(precision))
-    return fmt_of(precision) ? launch_level_t<1, true, 1, kModeRadiance>(p, st)
-                             : launch_level_t<0, true, 1, kModeRadiance>(p, st);
-  return fmt_of(precision) ? launch_level_t<1, false, 1, kModeRadiance>(p, st)
-                           : launch_level_t<0, false, 1, kModeRadiance>(p, st);
-}
-cudaError_t launch_view_acc(const LevelParams& p, int precision, cudaStream_t st) {
-  if (p.num_rays <= 0) return cudaSuccess;
-  if (is_x3(precision))
-    return fmt_of(precision) ? launch_level_t<1, true, 1, kModeViewAcc>(p, st)
-                             : launch_level_t<0, true, 1, kModeViewAcc>(p, st);
-  return fmt_of(precision) ? launch_level_t<1, false, 1, kModeViewAcc>(p, st)
-                           : launch_level_t<0, false, 1, kModeViewAcc>(p, st);
+
+// The launch parameters every query mode shares: points [off, off + cnt) of the query's Gaussians as tiles of 128
+// points, their density outputs (either may be null) and, for a query's backward, the dump.
+LevelParams query_params(const mipnerf_b200_config* c, const uint8_t* img, const float* means, const float* covs,
+                         int64_t off, int64_t cnt, float* raw_density, float* density, const TcQueryDump* dump) {
+  LevelParams p{};
+  p.wimage = img;
+  p.q_means = means + off * 3;
+  p.q_covs = covs ? covs + off * 3 : nullptr;
+  p.num_points = cnt;
+  p.num_rays = (cnt + kN - 1) / kN;
+  p.raw_density_out = raw_density ? raw_density + off : nullptr;
+  p.density_out = density ? density + off : nullptr;
+  p.disable_integration = c->disable_integration;
+  p.density_bias = c->density_bias;
+  if (dump) p.act_dump = dump->act, p.v_dump = dump->v, p.dump_tiles = p.num_rays;
+  return p;
 }
 
 // radiance mode: the view-direction slots [ctas][2][128][128] fp32, one pair per CTA of a launch of min(tiles, SMs)
@@ -1863,8 +1849,7 @@ size_t tc_packed_bytes(const mipnerf_b200_config* c, int precision) {
 
 size_t tc_workspace_bytes(const mipnerf_b200_config* c, int64_t num_rays, int precision) {
   if (!tc_supported(c, precision)) return 0;
-  const int64_t chunk = tc_chunk_rays(c->num_samples), r = num_rays < chunk ? num_rays : chunk;
-  return carve_tc(r > 0 ? r : 1, c->num_samples, nullptr).bytes;
+  return carve_tc(std::clamp<int64_t>(num_rays, 1, tc_chunk_rays(c->num_samples)), c->num_samples, nullptr).bytes;
 }
 
 cudaError_t tc_pack_weights(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, int precision,
@@ -1950,7 +1935,7 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
   SmallUpload small(img, st);  // biases / heads -> constant bank, ordered against other streams' forwards
   cudaError_t e = small.error();
   if (e != cudaSuccess) return e;
-  const float rgb_scale = (float)(1.0 + 2.0 * (double)c->rgb_padding);
+  const float rgb_scale = rgb_scale_of(c);
   const int n = c->num_samples;
   const int64_t chunk = tc_chunk_rays(n);
   if (dump && n != kN) return cudaErrorNotSupported;  // the training dump is one tile per ray
@@ -2008,7 +1993,8 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
       if (dump && is_x3(precision))
         e = fmt_of(precision) ? launch_level_t<1, true, 1, kModeForward, true>(p, st) : cudaErrorNotSupported;
       else
-        e = launch_level(p, precision, n, st);
+        e = n == 2 * kN ? launch_level<kModeForward, 2>(p, precision, st)
+                        : launch_level<kModeForward>(p, precision, st);
       if (e != cudaSuccess) return e;
       t_prev = t_cur;
       w_prev = w_cur;
@@ -2040,7 +2026,7 @@ cudaError_t tc_mlp_forward(const mipnerf_b200_config* c, const mipnerf_b200_weig
   p.raw_rgb_out = raw_rgb;
   p.raw_density_out = raw_density;
   p.num_rays = num_rays;
-  return launch_level(p, precision, kN, st);
+  return launch_level<kModeForward>(p, precision, st);
 }
 
 cudaError_t tc_query_density(const mipnerf_b200_config* c, const mipnerf_b200_weights* w, const float* means,
@@ -2053,18 +2039,8 @@ cudaError_t tc_query_density(const mipnerf_b200_config* c, const mipnerf_b200_we
   if (e != cudaSuccess) return e;
   for (int64_t off = 0; off < num_points; off += kDensityChunkPoints) {
     const int64_t cnt = (num_points - off) < kDensityChunkPoints ? (num_points - off) : kDensityChunkPoints;
-    LevelParams p{};
-    p.wimage = img;
-    p.q_means = means + off * 3;
-    p.q_covs = covs ? covs + off * 3 : nullptr;
-    p.num_points = cnt;
-    p.num_rays = (cnt + kN - 1) / kN;
-    p.raw_density_out = raw_density ? raw_density + off : nullptr;
-    p.density_out = density ? density + off : nullptr;
-    p.disable_integration = c->disable_integration;
-    p.density_bias = c->density_bias;
-    if (dump) p.act_dump = dump->act, p.dump_tiles = p.num_rays;
-    if ((e = launch_density(p, precision, st)) != cudaSuccess) return e;
+    const LevelParams p = query_params(c, img, means, covs, off, cnt, raw_density, density, dump);
+    if ((e = launch_level<kModeDensity>(p, precision, st)) != cudaSuccess) return e;
   }
   return cudaSuccess;
 }
@@ -2085,24 +2061,14 @@ cudaError_t tc_query_radiance(const mipnerf_b200_config* c, const mipnerf_b200_w
   if (e != cudaSuccess) return e;
   for (int64_t off = 0; off < num_points; off += kDensityChunkPoints) {
     const int64_t cnt = (num_points - off) < kDensityChunkPoints ? (num_points - off) : kDensityChunkPoints;
-    LevelParams p{};
-    p.wimage = img;
-    p.q_means = means + off * 3;
-    p.q_covs = covs ? covs + off * 3 : nullptr;
+    LevelParams p = query_params(c, img, means, covs, off, cnt, raw_density, density, dump);
     p.viewdirs = viewdirs + off * 3;
     p.view_bias = static_cast<float*>(workspace);  // the per-CTA slots, reused launch after launch on `st`
-    p.num_points = cnt;
-    p.num_rays = (cnt + kN - 1) / kN;
     p.raw_rgb_out = raw_rgb ? raw_rgb + off * 3 : nullptr;
-    p.raw_density_out = raw_density ? raw_density + off : nullptr;
     p.rgb_out = rgb ? rgb + off * 3 : nullptr;
-    p.density_out = density ? density + off : nullptr;
-    p.disable_integration = c->disable_integration;
-    p.density_bias = c->density_bias;
-    p.rgb_scale = (float)(1.0 + 2.0 * (double)c->rgb_padding);
+    p.rgb_scale = rgb_scale_of(c);
     p.rgb_padding = c->rgb_padding;
-    if (dump) p.act_dump = dump->act, p.v_dump = dump->v, p.dump_tiles = p.num_rays;
-    if ((e = launch_radiance(p, precision, st)) != cudaSuccess) return e;
+    if ((e = launch_level<kModeRadiance>(p, precision, st)) != cudaSuccess) return e;
   }
   return cudaSuccess;
 }
@@ -2125,18 +2091,9 @@ cudaError_t tc_query_view_acc(const mipnerf_b200_config* c, const mipnerf_b200_w
   SmallUpload small(img, st);
   cudaError_t e = small.error();
   if (e != cudaSuccess) return e;
-  LevelParams p{};
-  p.wimage = img;
-  p.q_means = means;
-  p.q_covs = covs;
-  p.num_points = num_points;
-  p.num_rays = (num_points + kN - 1) / kN;
+  LevelParams p = query_params(c, img, means, covs, 0, num_points, raw_density, density, nullptr);
   p.view_acc = view_acc;
-  p.raw_density_out = raw_density;
-  p.density_out = density;
-  p.disable_integration = c->disable_integration;
-  p.density_bias = c->density_bias;
-  return launch_view_acc(p, precision, st);
+  return launch_level<kModeViewAcc>(p, precision, st);
 }
 
 cudaError_t tc_view_terms(const mipnerf_b200_weights* w, const float* dirs, int64_t num_dirs, float* terms,

@@ -9,6 +9,23 @@
 
 namespace mipnerf {
 
+// 1 + 2 rgb_padding, the scale of the padded sigmoid colour activation (models/mip_nerf.py:236)
+inline float rgb_scale_of(const mipnerf_b200_config* c) { return (float)(1.0 + 2.0 * (double)c->rgb_padding); }
+
+inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
+
+// The scratch layouts' bump allocator: 256-byte-aligned takes from `base` in call order; a null base only counts bytes.
+struct Carver {
+  void* base;
+  size_t off = 0;
+  uint8_t* bytes(size_t n) {
+    uint8_t* p = base ? static_cast<uint8_t*>(base) + off : nullptr;
+    off += align_up(n);
+    return p;
+  }
+  float* floats(size_t n) { return reinterpret_cast<float*>(bytes(n * sizeof(float))); }
+};
+
 // true iff (cfg, precision) is the shape the fused tensor-core kernels are specialised for.
 bool tc_supported(const mipnerf_b200_config* cfg, int precision);
 bool tc_default_degrees(const mipnerf_b200_config* cfg);  // max_deg_point == 16 && deg_view == 4 (no weight padding)

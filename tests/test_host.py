@@ -245,6 +245,54 @@ def test_training_and_dataset_entry_points_validate_arguments_without_gpu(lib):
     assert lib.mipnerf_b200_pos_enc(None, 4, 3, 3, 1, None, None) == _cabi.EINVAL   # the identity columns remain
 
 
+# Workspace sizes the scratch layouts have always had: every buffer keeps its place and size, so callers that size
+# their allocations with these entry points see the same numbers.  (model kwargs, entry point, arguments, bytes);
+# only cases that do not depend on the device's SM count.
+PINNED_WORKSPACES = [
+    ({}, "workspace_bytes", (4096 + 37, _cabi.FP32), 1829191680),
+    ({}, "workspace_bytes", (1 << 20, _cabi.BF16), 168296448),
+    (dict(num_samples=256), "workspace_bytes", (1 << 20, _cabi.BF16), 151257088),
+    (dict(mlp_net_width=128), "workspace_bytes", (4095, _cabi.FP32), 1292005376),
+    (dict(max_deg_point=10), "workspace_bytes", (4096 + 37, _cabi.FP16X3), 10613760),
+    ({}, "train_workspace_bytes", (1 << 20,), 6734594048),
+    ({}, "train_workspace_bytes_for", (4096 + 37, _cabi.BF16X3), 6102435584),
+    ({}, "train_workspace_bytes_for", (1, _cabi.FP32), 64707840),
+    (dict(mlp_net_depth=6), "train_workspace_bytes_for", (4096 + 37, _cabi.FP32), 5660852224),
+    ({}, "mlp_workspace_bytes", (4096 + 37, 128, _cabi.FP32), 1610612736),
+    ({}, "mlp_workspace_bytes", (4096 + 37, 1, _cabi.FP32), 12696576),
+    ({}, "density_workspace_bytes", (1 << 20, _cabi.FP32), 1283457024),
+    ({}, "radiance_workspace_bytes", (4095, _cabi.FP32), 14709504),
+    (dict(use_viewdirs=False, mlp_net_width_condition=256), "radiance_workspace_bytes", (4095, _cabi.FP32), 18902784),
+    ({}, "radiance_dirs_workspace_bytes", (4095, 128, _cabi.FP32), 12188160),
+    ({}, "radiance_dirs_workspace_bytes", (1 << 20, 1, _cabi.BF16), 268435968),
+    ({}, "radiance_dirs_workspace_bytes", (1, 128, _cabi.FP16), 131072),
+    ({}, "query_backward_workspace_bytes", (1, 0, _cabi.FP32), 57847040),
+    ({}, "query_backward_workspace_bytes", (1 << 20, 0, _cabi.BF16), 2902189824),
+    (dict(max_deg_point=10, deg_view=2), "query_backward_workspace_bytes", (4096 + 37, 1, _cabi.FP32), 104145920),
+]
+
+
+@pytest.mark.parametrize("kw,entry,args,want", PINNED_WORKSPACES)
+def test_workspace_sizes_are_pinned(lib, kw, entry, args, want):
+    cfg = mp.MipNerf(**kw)._config()
+    assert getattr(lib, "mipnerf_b200_" + entry)(C.byref(cfg), *args) == want
+
+
+def test_mlp_forward_refuses_a_short_packed_image(lib):
+    """MLP.forward on the tensor cores reads the whole packed image: one declared byte too few is a bad argument,
+    refused before any device work."""
+    model = mp.MipNerf()
+    cfg = model._config()
+    lins = model.mlp.linears()
+    arr = (_cabi.Linear * len(lins))(*[_cabi.Linear(0x10000, 0x10000, l.in_features, l.out_features) for l in lins])
+    need = lib.mipnerf_b200_packed_weights_bytes(C.byref(cfg), _cabi.BF16)
+    work = lib.mipnerf_b200_mlp_workspace_bytes(C.byref(cfg), 4, 128, _cabi.BF16)
+    ws = _cabi.Weights(arr, len(lins), _cabi.BF16, 0x20000, need - 1)
+    p = 0x30000
+    rc = lib.mipnerf_b200_mlp_forward(C.byref(cfg), C.byref(ws), p, p, 4, 128, _cabi.BF16, p, p, p, work, None)
+    assert rc == _cabi.EINVAL and b"packed" in lib.mipnerf_b200_last_error()
+
+
 def test_public_header_is_plain_c_and_links(tmp_path):
     """include/mipnerf_b200.h is a C header (no torch / C++ types): a C99 translation unit that includes it compiles
     with -Wall -Wextra -pedantic -Werror and links against the shared library."""
