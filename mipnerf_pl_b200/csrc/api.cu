@@ -76,6 +76,10 @@ int check_config(const mipnerf_b200_config* c, Dims* d) {
   if (!c->use_viewdirs && c->net_width != c->net_width_condition)
     return fail(MIPNERF_B200_EUNSUPPORTED,
                 "use_viewdirs=False needs net_width == net_width_condition (reference color_layer shape)");
+  // view_layers is then an empty Sequential: the colour head would see net_width + view_dim inputs, which the
+  // reference's color_layer (net_width_condition inputs) cannot take
+  if (c->use_viewdirs && c->net_depth_condition == 0)
+    return fail(MIPNERF_B200_EUNSUPPORTED, "net_depth_condition=0 with use_viewdirs");
   if (!(c->density_noise >= 0.f) || c->density_noise > 3.0e38f)
     return fail(MIPNERF_B200_EINVAL, "density_noise=%g: need a finite standard deviation >= 0", (double)c->density_noise);
   d->xyz_dim = (c->max_deg_point - c->min_deg_point) * 6;
@@ -223,7 +227,7 @@ int mlp_forward_fp32(const mipnerf_b200_config* c, const Dims& d, const mipnerf_
                                         c->net_width, m, c->net_width, 0, st));
     feat = bott;
     feat_k = c->net_width;
-    for (int j = 0; j < c->net_depth_condition; ++j) {
+    for (int j = 0; j < c->net_depth_condition; ++j) {  // check_config: at least one
       const mipnerf_b200_linear& vl = w->linears[c->net_depth + 2 + j];
       float* out = (j & 1) ? s.c1 : s.c0;
       CUDA_TRY(mipnerf::launch_linear_f32(feat, feat_k, feat_k, j == 0 ? venc : nullptr, d.view_dim,
@@ -231,11 +235,6 @@ int mlp_forward_fp32(const mipnerf_b200_config* c, const Dims& d, const mipnerf_
                                           c->net_width_condition, m, c->net_width_condition, 1, st));
       feat = out;
       feat_k = c->net_width_condition;
-    }
-    if (c->net_depth_condition == 0) {
-      // view_layers is an empty Sequential: the colour head would see width+view_dim inputs, which
-      // the reference's color_layer (net_width_condition inputs) cannot take.
-      return fail(MIPNERF_B200_EUNSUPPORTED, "net_depth_condition=0 with use_viewdirs");
     }
   }
   const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
@@ -604,10 +603,11 @@ int mlp_forward_kept(const mipnerf_b200_config* c, const Dims& d, const mipnerf_
 // colour head, view layer, bottleneck + density head and trunk into `grads`, on the activations mlp_forward_kept left in
 // `s` (same `tc`, `view_div`, `density_only`).  With density_only it starts at the density head: d h_last is then the
 // rank-1 term d_raw_density . W_density alone, which dgrad_f32 with an empty dY computes without a GEMM.  touched[i]:
-// grads[i] already holds a sum to add to.
+// grads[i] already holds a sum to add to.  inv_gscale takes the fp16 step's gradient scale out of the wgrad sums.
 int mlp_backward_chain(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w, bool tc,
                        int precision, const LayerImages& im, const TrainScratch& s, int64_t m, int view_div,
-                       bool density_only, const mipnerf_b200_linear_grad* grads, bool* touched, cudaStream_t st) {
+                       bool density_only, const mipnerf_b200_linear_grad* grads, bool* touched, cudaStream_t st,
+                       float inv_gscale = 1.f) {
   const int depth = c->net_depth, W = c->net_width, Wc = c->net_width_condition;
   // tensor-core mode: the wgrad partials of the 128- and 256-wide layers on the tensor cores as well (dy comes from
   // the 256-byte-aligned workspace carves, and an x2 always follows k1 = 256 columns); the two heads on fp32 FFMA
@@ -619,13 +619,13 @@ int mlp_backward_chain(const mipnerf_b200_config* c, const Dims& d, const mipner
                                                          s.part, m, mipnerf::kWgradMaxSlices, precision, &slices, st);
       if (e2 != cudaSuccess) return e2;
       e2 = mipnerf::launch_wgrad_reduce(s.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
-                                        grads[idx].bias_grad, touched[idx] ? 1 : 0, st);
+                                        grads[idx].bias_grad, touched[idx] ? 1 : 0, st, inv_gscale);
       touched[idx] = true;
       return e2;
     }
     cudaError_t e = mipnerf::launch_wgrad_f32(dy, l.out_features, x1, k1, k1, x2, k2, k2, div, s.part,
                                               grads[idx].weight_grad, grads[idx].bias_grad, touched[idx] ? 1 : 0,
-                                              m, st);
+                                              m, st, inv_gscale);
     touched[idx] = true;
     return e;
   };
@@ -720,6 +720,7 @@ size_t mipnerf_b200_train_workspace_bytes_for(const mipnerf_b200_config* cfg, in
     return carve_fused(cfg, d, std::clamp<int64_t>(num_rays, 1, kChunkRaysX3), precision, nullptr).bytes;
   }
   if (precision != MIPNERF_B200_FP32 && precision != MIPNERF_B200_BF16 && precision != MIPNERF_B200_FP16) return 0;
+  if (precision != MIPNERF_B200_FP32 && !train_tc_supported(cfg, d)) return 0;  // forward_backward refuses it
   const int64_t r = std::clamp<int64_t>(num_rays, 1, kChunkRaysFp32);
   size_t bytes = carve_train(cfg, d, r, nullptr).bytes;
   if (train_fused_supported(cfg, precision))  // the fused tensor-core step overlays the same buffer
@@ -1013,6 +1014,10 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   const int n = cfg->num_samples, depth = cfg->net_depth;
   const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   const int64_t B = rays->num_rays;
+  // the per-layer fp16 GEMMs carry the fused step's gradient scale (forward_backward_fused says why): without it the
+  // gradient operands of deep trunks fall below fp16's normal range (measured at depth 16: 62 % of layers.0's gradient
+  // lost against the fp32 step)
+  const float gscale = precision == MIPNERF_B200_FP16 ? 1024.f : 1.f;
   bool touched[kMaxTrainDepth + 8];
   for (int i = 0; i < d.n_lin; ++i) touched[i] = accumulate != 0;
   if (B == 0 && !accumulate)
@@ -1072,8 +1077,9 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
 
       // ---- backward of this level (its fenceposts are constants, so levels are independent here)
       CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb, s.raw_density, t_cur, rc_.directions, white_bkgd,
-                                  rgb_scale, 1.f, s.d_raw_rgb, s.d_raw_density, st));
-      if ((rc = mlp_backward_chain(cfg, d, w, tc, precision, im, s, m, n, false, grads, touched, st))) return rc;
+                                  rgb_scale, gscale, s.d_raw_rgb, s.d_raw_density, st));
+      if ((rc = mlp_backward_chain(cfg, d, w, tc, precision, im, s, m, n, false, grads, touched, st, 1.f / gscale)))
+        return rc;
       t_prev = t_cur;
       w_prev = w_cur;
     }

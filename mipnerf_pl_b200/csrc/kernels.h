@@ -109,10 +109,11 @@ cudaError_t launch_dgrad_f32(const float* dy, int n_dim, const float* w, int ldw
                              const float* r1w, const float* act, float* dx, int64_t m, int k_dim,
                              cudaStream_t st);
 // dW[n_dim, k1+k2] (+)= dY^T @ [X1 | X2[row / x2_row_div]],  db[n_dim] (+)= colsum(dY); `part` holds
-// up to kWgradMaxSlices * n_dim * (k1+k2+1) floats of per-slice partial sums.
+// up to kWgradMaxSlices * n_dim * (k1+k2+1) floats of per-slice partial sums.  `scale` multiplies the sums before
+// they are stored / added (1 / the fp16 step's gradient scale).
 cudaError_t launch_wgrad_f32(const float* dy, int n_dim, const float* x1, int ld1, int k1, const float* x2,
                              int ld2, int k2, int x2_row_div, float* part, float* dw, float* db,
-                             int accumulate, int64_t m, cudaStream_t st);
+                             int accumulate, int64_t m, cudaStream_t st, float scale = 1.f);
 cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, float beta1, float beta2,
                         float eps, float step_size, float bc2_sqrt, float grad_scale, cudaStream_t st);
 constexpr int kAdamMaxTensors = 32;

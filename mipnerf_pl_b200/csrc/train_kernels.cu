@@ -578,7 +578,7 @@ cudaError_t launch_wgrad_reduce(const float* part, int slices, int n_dim, int k_
 
 cudaError_t launch_wgrad_f32(const float* dy, int n_dim, const float* x1, int ld1, int k1, const float* x2,
                              int ld2, int k2, int x2_row_div, float* part, float* dw, float* db,
-                             int accumulate, int64_t m, cudaStream_t st) {
+                             int accumulate, int64_t m, cudaStream_t st, float scale) {
   if (m == 0 || n_dim == 0) return cudaSuccess;
   if (!x2) {
     x2 = x1, ld2 = ld1, k2 = 0;
@@ -598,7 +598,7 @@ cudaError_t launch_wgrad_f32(const float* dy, int n_dim, const float* x1, int ld
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     wgrad_reduce_kernel<<<blocks_of((int64_t)n_dim * (K + 1), 64), 256, 0, st>>>(part, slices, n_dim, K, dw, db,
-                                                                                 accumulate);
+                                                                                 accumulate, scale);
     return cudaGetLastError();
   }
   const int tiles = ((n_dim + 127) / 128) * ((K + 127) / 128);
@@ -614,7 +614,7 @@ cudaError_t launch_wgrad_f32(const float* dy, int n_dim, const float* x1, int ld
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   wgrad_reduce_kernel<<<blocks_of((int64_t)n_dim * (K + 1), 64), 256, 0, st>>>(part, slices, n_dim, K, dw, db,
-                                                                               accumulate);
+                                                                               accumulate, scale);
   return cudaGetLastError();
 }
 
