@@ -1260,8 +1260,9 @@ int mipnerf_b200_adam_step(float* param, const float* grad, float* exp_avg, floa
   if (n < 0 || step < 1) return fail(MIPNERF_B200_EINVAL, "bad n / step");
   if (n > 0 && (!param || !grad || !exp_avg || !exp_avg_sq)) return fail(MIPNERF_B200_EINVAL, "NULL tensor");
   const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
-  CUDA_TRY(mipnerf::launch_adam(param, grad, exp_avg, exp_avg_sq, n, (float)beta1, (float)beta2, (float)eps,
-                                (float)(lr / bc1), (float)sqrt(bc2), (float)grad_scale, (cudaStream_t)stream));
+  CUDA_TRY(mipnerf::launch_adam(param, grad, exp_avg, exp_avg_sq, n, (float)(1.0 - beta1), (float)beta2,
+                                (float)(1.0 - beta2), (float)eps, (float)(lr / bc1), (float)sqrt(bc2), (float)grad_scale,
+                                (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 
@@ -1270,19 +1271,20 @@ int mipnerf_b200_adam_step_multi(int count, float* const* params, const float* c
                                  double eps, int64_t step, double grad_scale, void* stream) {
   if (count < 0 || step < 1) return fail(MIPNERF_B200_EINVAL, "bad count / step");
   if (count > 0 && (!params || !grads || !exp_avg || !exp_avg_sq || !sizes)) return fail(MIPNERF_B200_EINVAL, "NULL array");
+  for (int i = 0; i < count; ++i)  // every tensor before the first launch: a refusal leaves all of them untouched
+    if (sizes[i] < 0 || (sizes[i] > 0 && (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i])))
+      return fail(MIPNERF_B200_EINVAL, "tensor %d: NULL pointer or negative size", i);
   const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
   for (int base = 0; base < count; base += mipnerf::kAdamMaxTensors) {
     mipnerf::AdamMulti t{};
     t.count = (count - base) < mipnerf::kAdamMaxTensors ? (count - base) : mipnerf::kAdamMaxTensors;
     for (int k = 0; k < t.count; ++k) {
       const int i = base + k;
-      if (sizes[i] < 0 || (sizes[i] > 0 && (!params[i] || !grads[i] || !exp_avg[i] || !exp_avg_sq[i])))
-        return fail(MIPNERF_B200_EINVAL, "tensor %d: NULL pointer or negative size", i);
       t.p[k] = params[i], t.g[k] = grads[i], t.m[k] = exp_avg[i], t.v[k] = exp_avg_sq[i], t.n[k] = sizes[i];
       t.blocks[k] = (int)((sizes[i] + 255) / 256);
     }
-    CUDA_TRY(mipnerf::launch_adam_multi(t, (float)beta1, (float)beta2, (float)eps, (float)(lr / bc1), (float)sqrt(bc2),
-                                        (float)grad_scale, (cudaStream_t)stream));
+    CUDA_TRY(mipnerf::launch_adam_multi(t, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps,
+                                        (float)(lr / bc1), (float)sqrt(bc2), (float)grad_scale, (cudaStream_t)stream));
   }
   return MIPNERF_B200_OK;
 }

@@ -114,7 +114,8 @@ cudaError_t launch_dgrad_f32(const float* dy, int n_dim, const float* w, int ldw
 cudaError_t launch_wgrad_f32(const float* dy, int n_dim, const float* x1, int ld1, int k1, const float* x2,
                              int ld2, int k2, int x2_row_div, float* part, float* dw, float* db,
                              int accumulate, int64_t m, cudaStream_t st, float scale = 1.f);
-cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, float beta1, float beta2,
+// c1 = fl32(1 - beta1), c2 = fl32(1 - beta2), each rounded once from double (torch's Adam weights)
+cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, float c1, float beta2, float c2,
                         float eps, float step_size, float bc2_sqrt, float grad_scale, cudaStream_t st);
 constexpr int kAdamMaxTensors = 32;
 struct AdamMulti {  // passed by value in the kernel parameters
@@ -126,8 +127,8 @@ struct AdamMulti {  // passed by value in the kernel parameters
   int blocks[kAdamMaxTensors];  // ceil(n / 256)
   int count;
 };
-cudaError_t launch_adam_multi(const AdamMulti& t, float beta1, float beta2, float eps, float step_size, float bc2_sqrt,
-                              float grad_scale, cudaStream_t st);
+cudaError_t launch_adam_multi(const AdamMulti& t, float c1, float beta2, float c2, float eps, float step_size,
+                              float bc2_sqrt, float grad_scale, cudaStream_t st);
 
 // ---- linear_tc.cu (wgmma linear layer for the training step's forward / dgrad GEMMs) ----
 size_t linear_tc_image_bytes(int n, int k);

@@ -621,15 +621,18 @@ cudaError_t launch_wgrad_f32(const float* dy, int n_dim, const float* x1, int ld
 // -------------------------------------------------------------------------------------------------
 // torch.optim.Adam (amsgrad=False, weight_decay=0, maximize=False), single-tensor form:
 //   m <- lerp(m, g, 1-b1);  v <- b2 v + (1-b2) g^2;  p <- p - (lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps)
+// c1 = fl32(1 - b1) and c2 = fl32(1 - b2) are formed in double on the host, as torch forms its scalar weights (1.0f -
+// fl32(0.999) is 1.3e-5 away from fl32(0.001)).  The g^2 term is (c2 g) g, addcmul's order: g g alone overflows for
+// |g| > 1.8e19, where torch's v stays finite.
 // -------------------------------------------------------------------------------------------------
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                            float* __restrict__ v, int64_t n, float beta1, float beta2, float eps, float step_size,
-                            float bc2_sqrt, float grad_scale) {
+                            float* __restrict__ v, int64_t n, float c1, float beta2, float c2, float eps,
+                            float step_size, float bc2_sqrt, float grad_scale) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float gi = __fmul_rn(g[i], grad_scale);
-  const float mi = __fadd_rn(m[i], __fmul_rn(__fsub_rn(gi, m[i]), 1.0f - beta1));
-  const float vi = __fadd_rn(__fmul_rn(v[i], beta2), __fmul_rn(__fmul_rn(gi, gi), 1.0f - beta2));
+  const float mi = __fadd_rn(m[i], __fmul_rn(__fsub_rn(gi, m[i]), c1));
+  const float vi = __fadd_rn(__fmul_rn(v[i], beta2), __fmul_rn(__fmul_rn(c2, gi), gi));
   m[i] = mi;
   v[i] = vi;
   const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), eps);
@@ -638,7 +641,7 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
 
 // All tensors of one optimiser group in ONE launch (24 launches of ~7 us otherwise): block -> tensor by a scan of the
 // per-tensor block counts carried in the kernel parameters.
-__global__ void adam_multi_kernel(const AdamMulti t, float beta1, float beta2, float eps, float step_size,
+__global__ void adam_multi_kernel(const AdamMulti t, float c1, float beta2, float c2, float eps, float step_size,
                                   float bc2_sqrt, float grad_scale) {
   int b = blockIdx.x, k = 0;
   while (k + 1 < t.count && b >= t.blocks[k]) b -= t.blocks[k++];
@@ -648,29 +651,30 @@ __global__ void adam_multi_kernel(const AdamMulti t, float beta1, float beta2, f
   float* __restrict__ m = t.m[k];
   float* __restrict__ v = t.v[k];
   const float gi = __fmul_rn(t.g[k][i], grad_scale);
-  const float mi = __fadd_rn(m[i], __fmul_rn(__fsub_rn(gi, m[i]), 1.0f - beta1));
-  const float vi = __fadd_rn(__fmul_rn(v[i], beta2), __fmul_rn(__fmul_rn(gi, gi), 1.0f - beta2));
+  const float mi = __fadd_rn(m[i], __fmul_rn(__fsub_rn(gi, m[i]), c1));
+  const float vi = __fadd_rn(__fmul_rn(v[i], beta2), __fmul_rn(__fmul_rn(c2, gi), gi));
   m[i] = mi;
   v[i] = vi;
   const float denom = __fadd_rn(__fdiv_rn(sqrtf(vi), bc2_sqrt), eps);
   p[i] = __fadd_rn(p[i], __fmul_rn(-step_size, __fdiv_rn(mi, denom)));
 }
 
-cudaError_t launch_adam_multi(const AdamMulti& t, float beta1, float beta2, float eps, float step_size, float bc2_sqrt,
-                              float grad_scale, cudaStream_t st) {
+cudaError_t launch_adam_multi(const AdamMulti& t, float c1, float beta2, float c2, float eps, float step_size,
+                              float bc2_sqrt, float grad_scale, cudaStream_t st) {
   int total = 0;
   for (int k = 0; k < t.count; ++k) total += t.blocks[k];
   if (total == 0) return cudaSuccess;
   LaunchScope scope(kKernAdam, st);
-  adam_multi_kernel<<<total, 256, 0, st>>>(t, beta1, beta2, eps, step_size, bc2_sqrt, grad_scale);
+  adam_multi_kernel<<<total, 256, 0, st>>>(t, c1, beta2, c2, eps, step_size, bc2_sqrt, grad_scale);
   return cudaGetLastError();
 }
 
-cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, float beta1, float beta2,
+cudaError_t launch_adam(float* p, const float* g, float* m, float* v, int64_t n, float c1, float beta2, float c2,
                         float eps, float step_size, float bc2_sqrt, float grad_scale, cudaStream_t st) {
   if (n == 0) return cudaSuccess;
   LaunchScope scope(kKernAdam, st);
-  adam_kernel<<<blocks_of(n, 256), 256, 0, st>>>(p, g, m, v, n, beta1, beta2, eps, step_size, bc2_sqrt, grad_scale);
+  adam_kernel<<<blocks_of(n, 256), 256, 0, st>>>(p, g, m, v, n, c1, beta2, c2, eps, step_size, bc2_sqrt,
+                                                 grad_scale);
   return cudaGetLastError();
 }
 

@@ -237,6 +237,11 @@ class DeviceRayBank:
             raise RuntimeError("DeviceRayBank keeps the scene in HBM; use Blender / Multicam for host rays")
         self.device = dev
         n = len(scene)
+        if n == 0:
+            raise ValueError("DeviceRayBank: the scene has no images")
+        # the kernel clamps pixel ids to [0, P): with P = 0 that is row -1, before the atlas
+        if not np.any(scene.heights.astype(np.int64) * scene.widths.astype(np.int64)):
+            raise ValueError("DeviceRayBank: the scene's images have no pixels")
         table = np.concatenate([scene.pix2cam.reshape(n, 9), scene.cam2world.reshape(n, 12), scene.lossmult[:, None],
                                 scene.near[:, None], scene.far[:, None]], axis=1).astype(np.float32)
         sizes = scene.heights.astype(np.int64) * scene.widths.astype(np.int64)
