@@ -470,6 +470,42 @@ int mipnerf_b200_isosurface_emit(const float* grid, int nx, int ny, int nz, cons
 int mipnerf_b200_isosurface_normals(const float* grid, int nx, int ny, int nz, const float* lo_host,
                                     const float* hi_host, float iso, const void* scratch, float* normals, void* stream);
 
+/* ---- baked grids (mipnerf_pl_b200/baked.py): density and raw SH colour on nested lattices, rendered by ray marching */
+#define MIPNERF_B200_GRID_MAX_LEVELS 4
+
+/* One level of a baked grid: a lattice of nx * ny * nz points spanning the grid's bounds (point (i, j, k) at
+ * lo + (i, j, k) * (hi - lo) / (n - 1)), x fastest. */
+typedef struct mipnerf_b200_grid_level {
+  const int32_t* cells; /* [nz, ny, nx, 2] per point: fp32 density (bit pattern), then the row of its SH coefficients
+                           in `sh` (-1: not kept, coefficients 0) */
+  const float* sh;      /* [M, (degree + 1)^2, 3] fp32 raw-colour SH coefficients of the kept points */
+  int32_t nx, ny, nz;
+} mipnerf_b200_grid_level;
+
+/* Levels nest: level l has (n_0 - 1) / 2^l + 1 points per axis.  `occupancy` [oz, oy, ox] uint8 (o = ceil((n_0 - 1) /
+ * block) per axis) marks the macro cells of block^3 finest cells where some level may interpolate to non-zero density;
+ * a 0 cell is skipped.  lo / hi: the bounds; rgb_padding: colour = sigmoid(raw) (1 + 2 rgb_padding) - rgb_padding. */
+typedef struct mipnerf_b200_grid {
+  mipnerf_b200_grid_level levels[MIPNERF_B200_GRID_MAX_LEVELS];
+  int32_t num_levels; /* 1..4 */
+  int32_t degree;     /* 0..3, the field.sh_basis convention */
+  float lo[3], hi[3];
+  float rgb_padding;
+  const uint8_t* occupancy;
+  int32_t block; /* macro cell edge in finest cells, a multiple of 2^(num_levels - 1) */
+} mipnerf_b200_grid;
+
+/* Render rays through a baked grid (rays->viewdirs required): K = max(1, ceil((far - near) |d| / step)) intervals of
+ * dt = (far - near) / K, samples at t_k = near + (k + 1/2) dt (K, dt, t_k in fp32), delta = dt |d|.  A sample at
+ * x = o + t_k d (fp32) outside [lo, hi] has density 0; inside, level lambda = clamp(log2(sqrt(3) radii t_k / s_0), 0,
+ * L - 1) (s_0: the finest level's largest voxel edge) blends the trilinear density and SH coefficients of levels
+ * floor(lambda) and floor(lambda) + 1.  Compositing as mipnerf_b200_volumetric_rendering (distance not divided by acc,
+ * clamped to [near, far]), stopping after the first sample that leaves the transmittance below 1e-4.  Empty macro cells
+ * are skipped without moving the samples, so the result equals marching every sample bit for bit.  rgb [B,3], distance
+ * [B], acc [B].  No allocation, no synchronisation. */
+int mipnerf_b200_grid_render(const mipnerf_b200_grid* grid, const mipnerf_b200_rays* rays, float step, int white_bkgd,
+                             float* rgb, float* distance, float* acc, void* stream);
+
 /* Hardware self-test of the wgmma building blocks (descriptor / swizzle / accumulator-fragment conventions):
  * d[128,n] = a[128,k] . b[n,k]^T, 16-bit operands (precision BF16|FP16), fp32 accumulate; n in {128, 256}.
  * variant bit 0: B through a pre-swizzled image + cp.async.bulk (needs `scratch`); bit 1: A in registers (the RS form

@@ -80,6 +80,19 @@ class QueryCotangent(C.Structure):
                 ("d_density", C.c_void_p)]
 
 
+class GridLevel(C.Structure):
+    _fields_ = [("cells", C.c_void_p), ("sh", C.c_void_p), ("nx", C.c_int32), ("ny", C.c_int32), ("nz", C.c_int32)]
+
+
+GRID_MAX_LEVELS = 4
+
+
+class Grid(C.Structure):
+    _fields_ = [("levels", GridLevel * GRID_MAX_LEVELS), ("num_levels", C.c_int32), ("degree", C.c_int32),
+                ("lo", C.c_float * 3), ("hi", C.c_float * 3), ("rgb_padding", C.c_float), ("occupancy", C.c_void_p),
+                ("block", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/mipnerf_b200.h declares.
 _V = C.c_void_p
 _SIGNATURES = {
@@ -156,6 +169,8 @@ _SIGNATURES = {
     "mipnerf_b200_isosurface_count": (C.c_int, [_V, C.c_int, C.c_int, C.c_int, C.c_float, _V, C.c_size_t, _V, _V]),
     "mipnerf_b200_isosurface_emit": (C.c_int, [_V, C.c_int, C.c_int, C.c_int, _f32p, _f32p, C.c_float, _V, _V, _V,
                                                _V]),
+    "mipnerf_b200_grid_render": (C.c_int, [C.POINTER(Grid), C.POINTER(RaysStruct), C.c_float, C.c_int, _V, _V, _V,
+                                           _V]),
     "mipnerf_b200_selftest_umma": (C.c_int, [_V, _V, _V, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),
     "mipnerf_b200_profile_enable": (C.c_int, [C.c_int]),
     "mipnerf_b200_profile_num_kernels": (C.c_int, []),

@@ -1,0 +1,264 @@
+"""Baked grids: the field sampled once on a mip pyramid of lattices (density and raw spherical-harmonic colour), and
+frames rendered from it by a CUDA ray marcher instead of the MLP.
+
+* Level l of `levels` has n_l = (n_0 - 1) / 2^l + 1 points per axis over the same bounds, so the lattices nest.  Its
+  density is `field.density_grid` with the default voxel variance (step_l^2 / 12 per axis): the IPE integrates the
+  field over each voxel, so level l is the field pre-filtered at 2^l times the finest scale, not a subsampled copy.
+* A point is kept where the 3x3x3 dilation of `density > threshold` holds; elsewhere the baked density is 0 (a dropped
+  point's density is at most `threshold`).  The kept points' colour is `field.bake_sh(raw=True)` of their voxel
+  Gaussians, stored fp32 [M_l, (degree + 1)^2, 3]; the renderer applies the model's activation after the SH sum.
+* The occupancy grid marks macro cells of `block`^3 finest cells.  A cell is empty only if every level's baked
+  density is 0 on the cell's lattice points widened by one point of that level, so that every position in the cell
+  (and any position a rounding error outside it) interpolates to exactly 0 at every level: skipping empty cells
+  leaves the rendered result bit for bit unchanged.
+* Memory layout read by csrc/grid_render.cu, decided here and there only: per level one int32 [nz, ny, nx, 2] array of
+  (density bits, SH row or -1), x fastest, and the SH rows in the order of the kept points (x fastest).
+
+The renderer (`BakedGrid.render`, `render_baked_frame`) marches K = max(1, ceil((far - near) |d| / step)) samples at
+t_k = near + (k + 1/2) dt, blends two levels picked by the cone footprint (lambda = log2(sqrt(3) radii t / s_0)) and
+composites as `volumetric_rendering`, stopping once the transmittance drops below 1e-4 (include/mipnerf_b200.h).
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import List, Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+
+from . import _cabi
+from .field import DEFAULT_BOUNDS, Resolution, _resolution, bake_sh, density_grid, lattice_axes, voxel_variance
+from .ops import _dev, _f32, _rays_struct, _stream
+from .rays import BLENDER_CAMERA_ANGLE_X, Rays
+from .render import gather_rows, generate_rays, shard_rows
+
+MAX_LEVELS = _cabi.GRID_MAX_LEVELS
+DEFAULT_BLOCK = 8
+DEFAULT_THRESHOLD = 1e-2
+_FORMAT = 1
+
+
+def level_resolutions(resolution: Resolution, levels: int) -> List[Tuple[int, int, int]]:
+    """(nx, ny, nz) of every level: (n_0 - 1) / 2^l + 1 per axis."""
+    n0 = _resolution(resolution)
+    if not 1 <= int(levels) <= MAX_LEVELS:
+        raise ValueError(f"levels {levels}: need 1..{MAX_LEVELS}")
+    scale = 1 << (int(levels) - 1)
+    if any((n - 1) % scale for n in n0):
+        raise ValueError(f"resolution {n0}: n - 1 must be divisible by 2^(levels - 1) = {scale} on every axis")
+    return [tuple((n - 1) // (1 << lvl) + 1 for n in n0) for lvl in range(int(levels))]
+
+
+def _cell_matrix(n_cells: int, n_points: int, block: int, scale: int, device) -> torch.Tensor:
+    """[n_cells, n_points] 0/1: the level points (spacing `scale` finest cells) macro cell I depends on, the points
+    of finest cells [I block, (I + 1) block] widened by one point per side."""
+    cell = torch.arange(n_cells, device=device)[:, None]
+    p = torch.arange(n_points, device=device)[None, :]
+    first = torch.div(cell * block, scale, rounding_mode="floor") - 1
+    last = -torch.div(-(cell + 1) * block, scale, rounding_mode="floor") + 1
+    return ((p >= first) & (p <= last)).to(torch.float32)
+
+
+@torch.no_grad()
+def grid_structure(densities: Sequence[torch.Tensor], threshold: float, block: int = DEFAULT_BLOCK):
+    """The mask, index and occupancy construction from the density grids of every level (no model; any device) ->
+    (baked densities [nz, ny, nx] fp32, indices [nz, ny, nx] int32, occupancy [oz, oy, ox] uint8).  Level l keeps the
+    3x3x3 dilation of density > threshold; its baked density is the density where kept and 0 elsewhere; its index is
+    the row of a kept point among the level's kept points in x-fastest order and -1 elsewhere.  occupancy (o = ceil((n_0
+    - 1) / block) per axis) is 0 only for macro cells whose widened lattice points have baked density 0 at every level."""
+    if not 1 <= len(densities) <= MAX_LEVELS:
+        raise ValueError(f"{len(densities)} levels: need 1..{MAX_LEVELS}")
+    n0 = tuple(densities[0].shape)
+    scale_max = 1 << (len(densities) - 1)
+    if int(block) < 1 or int(block) % scale_max:
+        raise ValueError(f"block {block}: need a positive multiple of 2^(levels - 1) = {scale_max}")
+    if len(n0) != 3 or min(n0) < 2 or any((n - 1) % scale_max for n in n0):
+        raise ValueError(f"level 0: grid {n0}, need [nz, ny, nx], each >= 2 with n - 1 divisible by {scale_max}")
+    baked, indices = [], []
+    dev = densities[0].device
+    o = [-(-(n - 1) // block) for n in n0]  # (oz, oy, ox)
+    occ = torch.zeros(o, dtype=torch.float32, device=dev)
+    for lvl, dens in enumerate(densities):
+        want = tuple((n - 1) // (1 << lvl) + 1 for n in n0)
+        if tuple(dens.shape) != want:
+            raise ValueError(f"level {lvl}: grid {tuple(dens.shape)}, need {want} nested in level 0's {n0}")
+        d = dens.to(torch.float32)
+        keep = torch.nn.functional.max_pool3d((d > threshold).to(torch.float32)[None, None], 3, 1, 1)[0, 0] > 0
+        bd = torch.where(keep, d, torch.zeros((), device=dev))
+        idx = torch.full(bd.shape, -1, dtype=torch.int32, device=dev)
+        idx[keep] = torch.arange(int(keep.sum()), dtype=torch.int32, device=dev)
+        baked.append(bd.contiguous())
+        indices.append(idx)
+        nz = (bd != 0).to(torch.float32)
+        s = 1 << lvl
+        ax, ay, az = (_cell_matrix(o[2 - a], want[2 - a], block, s, dev) for a in range(3))
+        t = torch.einsum("kji,ai->kja", nz, ax)
+        t = torch.einsum("kja,bj->kba", t, ay)
+        occ += torch.einsum("kba,ck->cba", t, az)
+    return baked, indices, (occ > 0).to(torch.uint8)
+
+
+class BakedGrid:
+    """A baked field: per level the density and SH index lattices and the SH rows, the bounds, the SH degree, the
+    model's rgb_padding and the macro-cell occupancy.  `render` marches rays through it on the GPU; `save` / `load`
+    keep it in one .npz."""
+
+    def __init__(self, densities: Sequence[torch.Tensor], indices: Sequence[torch.Tensor], sh: Sequence[torch.Tensor],
+                 occupancy: torch.Tensor, bounds=DEFAULT_BOUNDS, degree: int = 2, rgb_padding: float = 0.001,
+                 block: int = DEFAULT_BLOCK):
+        if not 0 <= int(degree) <= 3:
+            raise ValueError(f"degree {degree}: need 0..3")
+        if not (len(densities) == len(indices) == len(sh)) or not 1 <= len(densities) <= MAX_LEVELS:
+            raise ValueError(f"{len(densities)} / {len(indices)} / {len(sh)} levels: need the same count, 1..{MAX_LEVELS}")
+        self.degree = int(degree)
+        self.rgb_padding = float(rgb_padding)
+        self.block = int(block)
+        self.bounds = (tuple(float(v) for v in bounds[0]), tuple(float(v) for v in bounds[1]))
+        nc = (self.degree + 1) ** 2
+        self.cells, self.sh = [], []
+        for lvl, (d, i, c) in enumerate(zip(densities, indices, sh)):
+            if d.shape != i.shape or d.dim() != 3 or c.dim() != 3 or tuple(c.shape[1:]) != (nc, 3):
+                raise ValueError(f"level {lvl}: density {tuple(d.shape)}, index {tuple(i.shape)}, sh {tuple(c.shape)}")
+            # (density bits, row) per lattice point: the kernel reads one 8-byte word per corner
+            self.cells.append(torch.stack([_f32(d).view(torch.int32), i.to(torch.int32)], dim=-1).contiguous())
+            self.sh.append(_f32(c))
+        self.occupancy = occupancy.to(torch.uint8).contiguous()
+        n0 = tuple(self.cells[0].shape[:3])
+        want = tuple(-(-(n - 1) // self.block) for n in n0)
+        if tuple(self.occupancy.shape) != want:
+            raise ValueError(f"occupancy {tuple(self.occupancy.shape)}: need {want} for block {self.block}")
+
+    @property
+    def levels(self) -> int:
+        return len(self.cells)
+
+    @property
+    def device(self) -> torch.device:
+        return self.cells[0].device
+
+    @property
+    def resolutions(self) -> List[Tuple[int, int, int]]:
+        """(nx, ny, nz) per level."""
+        return [tuple(c.shape[2::-1]) for c in self.cells]
+
+    def density(self, level: int = 0) -> torch.Tensor:
+        """The baked density [nz, ny, nx] of a level (a view)."""
+        return self.cells[level][..., 0].view(torch.float32)
+
+    def index(self, level: int = 0) -> torch.Tensor:
+        """The SH row of each lattice point [nz, ny, nx] int32, -1 where not kept (a view)."""
+        return self.cells[level][..., 1]
+
+    @property
+    def kept(self) -> List[int]:
+        return [int(s.shape[0]) for s in self.sh]
+
+    @property
+    def nbytes(self) -> int:
+        return sum(t.numel() * t.element_size() for t in self.cells + self.sh) + self.occupancy.numel()
+
+    def default_step(self) -> float:
+        """Half the finest level's smallest voxel edge."""
+        _, step = lattice_axes(self.resolutions[0], self.bounds, "cpu")
+        return float(np.float32(0.5) * step.min())
+
+    def _struct(self) -> "_cabi.Grid":
+        g = _cabi.Grid()
+        for lvl, (c, s) in enumerate(zip(self.cells, self.sh)):
+            nz, ny, nx = c.shape[:3]
+            g.levels[lvl] = _cabi.GridLevel(c.data_ptr(), s.data_ptr() if s.numel() else None, nx, ny, nz)
+        g.num_levels, g.degree = self.levels, self.degree
+        g.lo = (C.c_float * 3)(*self.bounds[0])
+        g.hi = (C.c_float * 3)(*self.bounds[1])
+        g.rgb_padding, g.occupancy, g.block = self.rgb_padding, self.occupancy.data_ptr(), self.block
+        return g
+
+    @torch.no_grad()
+    def render(self, rays: Rays, white_bkgd: bool = True, step: Optional[float] = None):
+        """(rgb [B,3], distance [B], acc [B]) of flat rays on the grid's device, marched every `step` along |d| (default
+        `default_step()`)."""
+        dev = _dev(self.cells[0])
+        o = rays.origins.reshape(-1, 3)
+        if o.device != dev:
+            raise ValueError(f"rays on {o.device}, grid on {dev}")
+        n = o.shape[0]
+        rs, keep = _rays_struct(o, rays.directions.reshape(-1, 3), rays.radii.reshape(-1), rays.near.reshape(-1),
+                                rays.far.reshape(-1), rays.viewdirs.reshape(-1, 3))
+        g = self._struct()
+        rgb = torch.empty(n, 3, device=dev)
+        dist = torch.empty(n, device=dev)
+        acc = torch.empty(n, device=dev)
+        st = self.default_step() if step is None else float(step)
+        with torch.cuda.device(dev):
+            _cabi.check(_cabi.lib().mipnerf_b200_grid_render(C.byref(g), C.byref(rs), st, int(bool(white_bkgd)),
+                                                             rgb.data_ptr(), dist.data_ptr(), acc.data_ptr(),
+                                                             _stream(dev)), "grid_render")
+        return rgb, dist, acc
+
+    def save(self, path: str) -> None:
+        """One .npz: per level density, index and sh, plus occupancy, bounds, degree, rgb_padding and block."""
+        arrays = {"format": np.int32(_FORMAT), "levels": np.int32(self.levels), "degree": np.int32(self.degree),
+                  "rgb_padding": np.float32(self.rgb_padding), "block": np.int32(self.block),
+                  "bounds": np.asarray(self.bounds, dtype=np.float32), "occupancy": self.occupancy.cpu().numpy()}
+        for lvl in range(self.levels):
+            arrays[f"density_{lvl}"] = self.density(lvl).cpu().numpy()
+            arrays[f"index_{lvl}"] = self.index(lvl).cpu().numpy()
+            arrays[f"sh_{lvl}"] = self.sh[lvl].cpu().numpy()
+        np.savez(path, **arrays)
+
+    @classmethod
+    def load(cls, path: str, device="cuda") -> "BakedGrid":
+        with np.load(path) as z:
+            if int(z["format"]) != _FORMAT:
+                raise ValueError(f"{path}: baked-grid format {int(z['format'])}, this library reads {_FORMAT}")
+            levels = int(z["levels"])
+            t = lambda name: torch.from_numpy(np.ascontiguousarray(z[name])).to(device)  # noqa: E731
+            bounds = z["bounds"].astype(np.float64)
+            return cls([t(f"density_{lvl}") for lvl in range(levels)], [t(f"index_{lvl}") for lvl in range(levels)],
+                       [t(f"sh_{lvl}") for lvl in range(levels)], t("occupancy"),
+                       (tuple(bounds[0]), tuple(bounds[1])), int(z["degree"]), float(z["rgb_padding"]), int(z["block"]))
+
+
+@torch.no_grad()
+def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: float = DEFAULT_THRESHOLD,
+              degree: int = 2, n_theta: int = 8, bounds=DEFAULT_BOUNDS, block: int = DEFAULT_BLOCK,
+              slab_points: int = 1 << 20) -> BakedGrid:
+    """Bake `model` into a `levels`-level grid over `bounds` (level l: (n_0 - 1) / 2^l + 1 points per axis): the
+    density of `field.density_grid` at its default voxel variance, the keep mask, index and occupancy of
+    `grid_structure`, and the raw SH colour of the kept points' voxel Gaussians (`field.bake_sh(raw=True)`, degree
+    0..3, in slabs of `slab_points`), on the model's device."""
+    if not 0 <= int(degree) <= 3:
+        raise ValueError(f"degree {degree}: need 0..3")
+    res = level_resolutions(resolution, levels)
+    dens = [density_grid(model, r, bounds) for r in res]
+    baked, indices, occ = grid_structure(dens, threshold, block)
+    dev = dens[0].device
+    sh = []
+    for r, bd, idx in zip(res, baked, indices):
+        (xs, ys, zs), _ = lattice_axes(r, bounds, dev)
+        flat = (idx.reshape(-1) >= 0).nonzero().reshape(-1)
+        var = torch.tensor(voxel_variance(r, bounds), device=dev)
+        out = torch.empty(flat.numel(), (int(degree) + 1) ** 2, 3, device=dev)
+        nx, ny = r[0], r[1]
+        for s in range(0, flat.numel(), slab_points):
+            p = flat[s:s + slab_points]
+            means = torch.stack([xs[p % nx], ys[(p // nx) % ny], zs[p // (nx * ny)]], dim=-1)
+            out[s:s + len(p)] = bake_sh(model, means, var.expand(len(p), 3), degree, n_theta, raw=True)
+        sh.append(out)
+    return BakedGrid(baked, indices, sh, occ, bounds, degree, float(model.rgb_padding), block)
+
+
+@torch.no_grad()
+def render_baked_frame(grid: BakedGrid, c2w, height: int = 800, width: int = 800, white_bkgd: bool = True,
+                       camera_angle_x: float = BLENDER_CAMERA_ANGLE_X, near: float = 2.0, far: float = 6.0,
+                       world: int = 1, rank: int = 0, group=None, device=None, step: Optional[float] = None):
+    """One frame from a baked grid, with `render.render_frame`'s rays and row sharding: (rgb [H,W,3], distance [H,W],
+    acc [H,W]) on every rank."""
+    dev = device or grid.device
+    r0, r1 = shard_rows(height, world, rank)
+    rays = generate_rays(c2w, height, width, camera_angle_x, near, far, rows=(r0, r1), device=dev)
+    rgb, dist, acc = grid.render(rays, white_bkgd, step)
+    local = torch.cat([rgb, dist[:, None], acc[:, None]], dim=1)  # [rows*W, 5]
+    counts = [(shard_rows(height, world, r)[1] - shard_rows(height, world, r)[0]) * width for r in range(world)]
+    full = gather_rows(local, counts, group)
+    return full[:, 0:3].reshape(height, width, 3), full[:, 3].reshape(height, width), full[:, 4].reshape(height, width)

@@ -7,6 +7,9 @@
 
 #include "draws.h"
 
+struct mipnerf_b200_grid;  // include/mipnerf_b200.h
+struct mipnerf_b200_rays;
+
 namespace mipnerf {
 
 // ---- ray_kernels.cu ----
@@ -65,6 +68,10 @@ cudaError_t launch_isosurface_emit(const float* grid, int nx, int ny, int nz, co
 // after launch_isosurface_emit on the same scratch: the unit normal of every vertex (step: HOST float[3])
 cudaError_t launch_isosurface_normals(const float* grid, int nx, int ny, int nz, const float* step, float iso,
                                       const void* scratch, float* normals, cudaStream_t st);
+
+// ---- grid_render.cu (ray marching through a baked grid; arguments checked by the caller) ----
+cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
+                               int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st);
 
 // ---- metrics.cu ----
 size_t image_metrics_scratch_bytes(int height, int width, int channels);

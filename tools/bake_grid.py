@@ -1,0 +1,66 @@
+"""Bake a trained MipNeRFSystem checkpoint into a mip-mapped grid of density and SH colour (one .npz), and optionally
+render the spheric video path from the grid.
+
+    python tools/bake_grid.py --ckpt last.ckpt --out GRID.npz [--resolution 257] [--levels 1] [--threshold 0.01]
+        [--degree 2] [--bounds -1.5 -1.5 -1.5 1.5 1.5 1.5] [--precision bf16] [--frames DIR] [--size 800]
+
+Level l has (n - 1) / 2^l + 1 points per axis (n - 1 divisible by 2^(levels - 1)).  Lattice points farther than one
+point from any point of density > threshold are dropped (density 0).  With --frames, the 120 poses of
+`metrics.spheric_path()` are rendered from the grid with `render_baked_frame` and written with `save_images`
+(<idx>_rgb.png, _dist.png, _acc.png).  A saved grid renders without the checkpoint: `mp.BakedGrid.load(path)`.
+"""
+import argparse
+import os
+import sys
+import time
+
+ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+import torch  # noqa: E402
+
+import mipnerf_pl_b200 as mp  # noqa: E402
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--ckpt", required=True, help="MipNeRFSystem checkpoint (PL layout: state_dict + hyper_parameters)")
+    ap.add_argument("--out", required=True, help="the baked grid, .npz")
+    ap.add_argument("--resolution", type=int, nargs="+", default=[257], help="n, or nx ny nz (finest level)")
+    ap.add_argument("--levels", type=int, default=1, help="mip levels, 1..4")
+    ap.add_argument("--threshold", type=float, default=mp.baked.DEFAULT_THRESHOLD)
+    ap.add_argument("--degree", type=int, default=2, help="SH degree, 0..3")
+    ap.add_argument("--bounds", type=float, nargs=6, default=[-1.5, -1.5, -1.5, 1.5, 1.5, 1.5],
+                    metavar=("X0", "Y0", "Z0", "X1", "Y1", "Z1"))
+    ap.add_argument("--precision", default="bf16", choices=sorted(mp._cabi.PRECISIONS))
+    ap.add_argument("--frames", default=None, metavar="DIR", help="render the spheric path from the grid into DIR")
+    ap.add_argument("--size", type=int, default=800, help="frame height and width for --frames")
+    ap.add_argument("--device", default="cuda:0")
+    args = ap.parse_args(argv)
+    system = mp.MipNeRFSystem.load_from_checkpoint(args.ckpt, map_location="cpu", precision=args.precision)
+    model = system.mip_nerf.to(args.device).eval()
+    res = args.resolution[0] if len(args.resolution) == 1 else tuple(args.resolution)
+    bounds = (tuple(args.bounds[:3]), tuple(args.bounds[3:]))
+    t0 = time.perf_counter()
+    grid = mp.bake_grid(model, res, levels=args.levels, threshold=args.threshold, degree=args.degree, bounds=bounds)
+    torch.cuda.synchronize()
+    t1 = time.perf_counter()
+    grid.save(args.out)
+    print(f"{args.out}: levels {grid.resolutions}, kept points {grid.kept}, occupied macro cells "
+          f"{int(grid.occupancy.sum())}/{grid.occupancy.numel()}, {grid.nbytes / 2 ** 20:.1f} MiB, "
+          f"baked in {t1 - t0:.2f} s")
+    if args.frames:
+        times = []
+        for idx, c2w in enumerate(mp.spheric_path()):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            rgb, dist, acc = mp.render_baked_frame(grid, c2w, args.size, args.size)
+            e1.record()
+            mp.save_images(rgb, dist, acc, args.frames, idx)
+            times.append(e0.elapsed_time(e1))
+        print(f"{args.frames}: {len(times)} frames, median {sorted(times)[len(times) // 2]:.2f} ms per frame")
+
+
+if __name__ == "__main__":
+    main()
