@@ -182,8 +182,8 @@ class BakedGrid:
         if o.device != dev:
             raise ValueError(f"rays on {o.device}, grid on {dev}")
         n = o.shape[0]
-        rs, keep = _rays_struct(o, rays.directions.reshape(-1, 3), rays.radii.reshape(-1), rays.near.reshape(-1),
-                                rays.far.reshape(-1), rays.viewdirs.reshape(-1, 3))
+        rs, keep = _rays_struct(o, rays.directions.reshape(-1, 3), rays.viewdirs.reshape(-1, 3), rays.radii.reshape(-1),
+                                rays.near.reshape(-1), rays.far.reshape(-1))
         g = self._struct()
         rgb = torch.empty(n, 3, device=dev)
         dist = torch.empty(n, device=dev)

@@ -498,18 +498,6 @@ bool train_fused_supported(const mipnerf_b200_config* c, int precision) {
          c->num_levels <= 2 && c->net_depth == 8;
 }
 
-// Tensor-core GEMMs of the training step exist for the default widths only (linear_tc.cu).
-bool train_tc_supported(const mipnerf_b200_config* c, const Dims& d) {
-  if (!(c->net_width == 256 && c->net_width_condition == 128 && d.xyz_dim == 96 && d.view_dim == 27 &&
-        c->net_depth <= kMaxTrainDepth))
-    return false;
-  // packed-operand slots the step needs (forward + skip + transposed dgrad images + bottleneck / view layer x 2):
-  // must fit the kTrainImages slots carved from the workspace
-  int slots = 4;
-  for (int i = 0; i < c->net_depth; ++i) slots += 1 + (i > 1 && (i - 1) % c->skip_index == 0 ? 1 : 0) + (i > 0 ? 1 : 0);
-  return slots <= kTrainImages;
-}
-
 int check_train_config(const mipnerf_b200_config* c) {
   if (!c->use_viewdirs || c->net_depth_condition != 1)
     return fail(MIPNERF_B200_EUNSUPPORTED, "training: use_viewdirs=True with one view layer only");
@@ -522,34 +510,116 @@ inline bool takes_skip(const mipnerf_b200_config* c, int layer) {  // models/mip
   return layer > 1 && (layer - 1) % c->skip_index == 0;
 }
 
-// B operands of the per-layer tensor-core GEMMs, packed once per call (the weights change every optimiser step) into
-// kTrainImageBytes slots at `base`.  fwd[i] = W_i[:, :k_main], skip[i] = W_i[:, 256:352], bwd[i] = W_i[:, :256]^T;
-// slots depth / depth+1 hold the bottleneck and the view layer.
+// B operands of the training GEMMs, packed once per call (the weights change every optimiser step) into
+// kTrainImageBytes slots at `base`; a null base only counts the slots.  bwd[i] = W_i[:, :256]^T for i = 1 .. depth + 1
+// (depth / depth + 1: the bottleneck and the view layer), in bf16x3 with its lo image bwd_lo[i] kMaxTrainDepth + 2
+// slots further on.  The per-layer path (`fwd`) also takes fwd[i] = W_i[:, :k_main] and skip[i] = W_i[:, 256:352]
+// (fwd[depth] / fwd[depth + 1]: the bottleneck, the view layer's bottleneck columns).
 struct LayerImages {
-  const uint8_t *fwd[kMaxTrainDepth + 2], *skip[kMaxTrainDepth], *bwd[kMaxTrainDepth + 2];
+  const uint8_t *fwd[kMaxTrainDepth + 2], *skip[kMaxTrainDepth], *bwd[kMaxTrainDepth + 2], *bwd_lo[kMaxTrainDepth + 2];
+  int slots;  // slots taken, lo images not counted
 };
 
 cudaError_t pack_layer_images(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w, int precision,
-                              uint8_t* base, LayerImages* im, cudaStream_t st) {
+                              bool fwd, uint8_t* base, LayerImages* im, cudaStream_t st) {
   const int depth = c->net_depth, W = c->net_width, Wc = c->net_width_condition;
+  const int fmt = mipnerf::fmt_of(precision);
+  const bool x3 = mipnerf::is_x3(precision);
   *im = LayerImages{};
-  int slot = 0;
-  auto pack = [&](const mipnerf_b200_linear& l, int off, int transposed, int nn, int kk, const uint8_t** out) {
-    uint8_t* dst = base + (size_t)(slot++) * kTrainImageBytes;
+  // columns [off, off + kk) of linear li as an nn x kk image (transposed: B[k][n] = W[n][k]) into the next slot
+  auto pack = [&](int li, int off, int transposed, int nn, int kk, const uint8_t** out,
+                  const uint8_t** out_lo = nullptr) {
+    const size_t slot = im->slots++;
+    if (!base) return cudaSuccess;
+    const mipnerf_b200_linear& l = w->linears[li];
+    uint8_t* dst = base + slot * kTrainImageBytes;
     *out = dst;
-    return mipnerf::launch_pack_linear_image(l.weight, l.in_features, off, transposed, dst, nn, kk, precision, st);
+    if (out_lo) {
+      uint8_t* lo = base + (slot + kMaxTrainDepth + 2) * kTrainImageBytes;
+      *out_lo = lo;
+      cudaError_t e = mipnerf::launch_pack_linear_image(l.weight, l.in_features, off, transposed, lo, nn, kk, fmt, st, 1);
+      if (e != cudaSuccess) return e;
+    }
+    return mipnerf::launch_pack_linear_image(l.weight, l.in_features, off, transposed, dst, nn, kk, fmt, st);
   };
+  auto bwd = [&](int li, int i, int kk) { return pack(li, 0, 1, W, kk, &im->bwd[i], x3 ? &im->bwd_lo[i] : nullptr); };
   cudaError_t e;
   for (int i = 0; i < depth; ++i) {
-    const mipnerf_b200_linear& l = w->linears[i];
-    if ((e = pack(l, 0, 0, W, i == 0 ? d.xyz_dim : W, &im->fwd[i]))) return e;
-    if (takes_skip(c, i) && (e = pack(l, W, 0, W, d.xyz_dim, &im->skip[i]))) return e;
-    if (i > 0 && (e = pack(l, 0, 1, W, W, &im->bwd[i]))) return e;  // B[k_out][n] = W_i[n][k_out]
+    if (fwd && (e = pack(i, 0, 0, W, i == 0 ? d.xyz_dim : W, &im->fwd[i]))) return e;
+    if (fwd && takes_skip(c, i) && (e = pack(i, W, 0, W, d.xyz_dim, &im->skip[i]))) return e;
+    if (i > 0 && (e = bwd(i, i, W))) return e;
   }
-  if ((e = pack(w->linears[depth + 1], 0, 0, W, W, &im->fwd[depth]))) return e;  // bottleneck
-  if ((e = pack(w->linears[depth + 1], 0, 1, W, W, &im->bwd[depth]))) return e;
-  if ((e = pack(w->linears[depth + 2], 0, 0, Wc, W, &im->fwd[depth + 1]))) return e;  // view layer, bottleneck columns
-  return pack(w->linears[depth + 2], 0, 1, W, Wc, &im->bwd[depth + 1]);
+  if (fwd && (e = pack(depth + 1, 0, 0, W, W, &im->fwd[depth]))) return e;  // bottleneck
+  if ((e = bwd(depth + 1, depth, W))) return e;
+  if (fwd && (e = pack(depth + 2, 0, 0, Wc, W, &im->fwd[depth + 1]))) return e;  // view layer, bottleneck columns
+  return bwd(depth + 2, depth + 1, Wc);
+}
+
+// Tensor-core GEMMs of the training step exist for the default widths only (linear_tc.cu), and the per-layer step's
+// images must fit the kTrainImages slots carved from the workspace.
+bool train_tc_supported(const mipnerf_b200_config* c, const Dims& d) {
+  if (!(c->net_width == 256 && c->net_width_condition == 128 && d.xyz_dim == 96 && d.view_dim == 27 &&
+        c->net_depth <= kMaxTrainDepth))
+    return false;
+  LayerImages im;
+  pack_layer_images(c, d, nullptr, MIPNERF_B200_BF16, true, nullptr, &im, nullptr);
+  return im.slots <= kTrainImages;
+}
+
+// The gradient outputs of a backward pass: touched[i] (grads[i] already holds a sum to add to) starts at `accumulate`,
+// the backward chains set it for every linear they reach, and every gradient still untouched after them (no rays or
+// points, or the heads a density query does not reach) is written as exact zeros.
+int zero_untouched(const Dims& d, const mipnerf_b200_weights* w, const mipnerf_b200_linear_grad* grads,
+                   const bool* touched, cudaStream_t st) {
+  for (int i = 0; i < d.n_lin; ++i)
+    if (!touched[i]) {
+      const mipnerf_b200_linear& l = w->linears[i];
+      CUDA_TRY(cudaMemsetAsync(grads[i].weight_grad, 0, sizeof(float) * l.in_features * l.out_features, st));
+      CUDA_TRY(cudaMemsetAsync(grads[i].bias_grad, 0, sizeof(float) * l.out_features, st));
+    }
+  return MIPNERF_B200_OK;
+}
+
+int check_grads(const Dims& d, const mipnerf_b200_linear_grad* grads, int num_grads) {
+  if (num_grads != d.n_lin) return fail(MIPNERF_B200_EINVAL, "expected %d gradient pairs, got %d", d.n_lin, num_grads);
+  for (int i = 0; i < d.n_lin; ++i)
+    if (!grads[i].weight_grad || !grads[i].bias_grad) return fail(MIPNERF_B200_EINVAL, "grads[%d] has a NULL tensor", i);
+  return MIPNERF_B200_OK;
+}
+
+// The precisions a backward pass from arbitrary cotangents takes: FP32 and BF16.  `what` names the entry point.
+int check_cotangent_precision(int precision, const char* what) {
+  if (precision == MIPNERF_B200_FP16)
+    return fail(MIPNERF_B200_EUNSUPPORTED,
+                "%s: FP16's fixed gradient scale is sized for the training loss and arbitrary cotangents can overflow "
+                "or underflow it; use BF16 (fp32 range) or FP32", what);
+  if (mipnerf::is_x3(precision))
+    return fail(MIPNERF_B200_EUNSUPPORTED, "%s: the split-operand precisions are forward-only; use FP32 or BF16", what);
+  return MIPNERF_B200_OK;
+}
+
+// The factor the training loss's gradient is emitted with.  fp16 gradients underflow: d loss / d activation is ~1e-7 ..
+// 1e-4 per sample (the loss is a mean over the batch), below fp16's 6e-5 normal range.  The backward pass is linear in
+// d loss / d raw, so render_backward emits it scaled by 2^10 (it is bounded by 2/3 per sample: no overflow), every
+// 16-bit gradient operand carries that factor, and the fixed-order reduction of the wgrad partials takes it out again
+// (without it, measured at depth 16, the per-layer step lost 62 % of layers.0's gradient against the fp32 step).  bf16
+// has fp32's range: scale 1.
+float grad_scale_of(int precision) { return precision == MIPNERF_B200_FP16 ? 1024.f : 1.f; }
+
+// Where level l of the chunk [off, off + cnt) of a training step writes: its fenceposts and weights to the caller's
+// outs[l] or the scratch t / w, its pixels to outs[l] or, with given fenceposts (whose recomputed pixels nobody reads),
+// into the unused fencepost scratch t; inds and density_normal from the chunk's first ray.
+mipnerf_b200_level_out chunk_level_out(const mipnerf_b200_level_out& o, int64_t off, int64_t cnt, int n, bool given_t,
+                                       float* t, float* w) {
+  mipnerf_b200_level_out r;
+  r.comp_rgb = given_t ? t : o.comp_rgb + off * 3;
+  r.distance = given_t ? t + 3 * cnt : o.distance + off;
+  r.acc = given_t ? t + 4 * cnt : o.acc + off;
+  r.weights = o.weights ? o.weights + off * n : w;
+  r.t_samples = o.t_samples ? o.t_samples + off * (n + 1) : t;
+  r.inds = o.inds ? o.inds + off * (n + 1) : nullptr;
+  r.density_normal = o.density_normal ? o.density_normal + off * n : nullptr;
+  return r;
 }
 
 // MLP.forward of m rows with every activation the backward needs kept in `s` (models/mip_nerf.py:75-111): the trunk
@@ -754,17 +824,16 @@ struct TileChainOps {
 
 // The per-level backward chain of the fused training step, on 16-bit tile images: colour head, view layer, bottleneck
 // + density head, trunk, into `grads` (touched[i]: grads[i] already holds a sum to add to; inv_gscale takes the fp16
-// step's gradient scale out again).  img_bwd[i] = W_i[:, :256]^T (slots depth / depth + 1: bottleneck, view layer),
-// img_bwd_lo their lo images in bf16x3.  density_only (a density query): the chain starts at the density head; d h_7
+// step's gradient scale out again), on the images im.bwd (im.bwd_lo in bf16x3).  density_only (a density query): the
+// chain starts at the density head; d h_7
 // is then the rank-1 term d_raw_density . W_density, masked by h_7 > 0, which the bottleneck's dgrad computes on an
 // all-zero d_a with the mask read from the h_7 tile (there is no bottleneck wgrad to leave its sign bits behind).
 int tile_backward_chain(const mipnerf_b200_config* cfg, const Dims& d, const mipnerf_b200_weights* w, int precision,
-                        const uint8_t* const* img_bwd, const uint8_t* const* img_bwd_lo, const TileChainOps& o,
-                        bool density_only, float inv_gscale, const mipnerf_b200_linear_grad* grads, bool* touched,
-                        cudaStream_t st) {
+                        const LayerImages& im, const TileChainOps& o, bool density_only, float inv_gscale,
+                        const mipnerf_b200_linear_grad* grads, bool* touched, cudaStream_t st) {
   const int depth = cfg->net_depth, W = cfg->net_width, Wc = cfg->net_width_condition;
-  const bool x3 = precision == MIPNERF_B200_BF16X3;
-  const int fmt = x3 ? MIPNERF_B200_BF16 : precision;
+  const bool x3 = mipnerf::is_x3(precision);
+  const int fmt = mipnerf::fmt_of(precision);
   const int64_t m = o.tiles * 128;
   const mipnerf_b200_linear& dl = w->linears[depth];
   const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
@@ -799,9 +868,9 @@ int tile_backward_chain(const mipnerf_b200_config* cfg, const Dims& d, const mip
     const void* mask = act_in && !bits_ok ? act_in : nullptr;
     const void* bits = act_in && bits_ok ? o.relu_bits : nullptr;
     if (x3)
-      return mipnerf::launch_linear_t16_x3(xi, lo_img(xi, (size_t)kk * 256), img_bwd[slot], img_bwd_lo[slot], y,
+      return mipnerf::launch_linear_t16_x3(xi, lo_img(xi, (size_t)kk * 256), im.bwd[slot], im.bwd_lo[slot], y,
                                            lo_img(y, (size_t)nn * 256), m, nn, kk, r1, r1w, mask, st, bits);
-    return mipnerf::launch_linear_t16(xi, img_bwd[slot], y, m, nn, kk, r1, r1w, mask, fmt, st, bits);
+    return mipnerf::launch_linear_t16(xi, im.bwd[slot], y, m, nn, kk, r1, r1w, mask, fmt, st, bits);
   };
   auto h16 = [&](int i) { return o.act + (size_t)i * o.tiles * 65536; };  // h_0..h_7, 8 = bottleneck
   auto h16_lo = [&](int i) { return x3 ? h16(9 + i) : nullptr; };
@@ -851,34 +920,6 @@ int tile_backward_chain(const mipnerf_b200_config* cfg, const Dims& d, const mip
   return MIPNERF_B200_OK;
 }
 
-// The B operands of the tile-image dgrad chain, packed once per call (the weights change every optimiser step) into
-// kTrainImageBytes slots at `base`: bwd[i] = W_i[:, :256]^T (slots depth / depth + 1: bottleneck, view layer); bf16x3
-// also their lo images, kMaxTrainDepth + 2 slots further on.
-cudaError_t pack_bwd_images(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, int precision, uint8_t* base,
-                            const uint8_t** img_bwd, const uint8_t** img_bwd_lo, cudaStream_t st) {
-  const int depth = cfg->net_depth, W = cfg->net_width, Wc = cfg->net_width_condition;
-  const bool x3 = precision == MIPNERF_B200_BF16X3;
-  const int fmt = x3 ? MIPNERF_B200_BF16 : precision;
-  int slot = 0;
-  auto pack = [&](const mipnerf_b200_linear& l, int nn, int kk, const uint8_t** out) {
-    uint8_t* dst = base + (size_t)slot * kTrainImageBytes;
-    *out = dst;
-    if (x3) {
-      uint8_t* lo = base + (size_t)(slot + kMaxTrainDepth + 2) * kTrainImageBytes;
-      img_bwd_lo[out - img_bwd] = lo;
-      cudaError_t e = mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, lo, nn, kk, fmt, st, 1);
-      if (e != cudaSuccess) return e;
-    }
-    ++slot;
-    return mipnerf::launch_pack_linear_image(l.weight, l.in_features, 0, 1, dst, nn, kk, fmt, st);
-  };
-  cudaError_t e;
-  for (int i = 1; i < depth; ++i)
-    if ((e = pack(w->linears[i], W, W, &img_bwd[i]))) return e;
-  if ((e = pack(w->linears[depth + 1], W, W, &img_bwd[depth]))) return e;
-  return pack(w->linears[depth + 2], W, Wc, &img_bwd[depth + 1]);
-}
-
 static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d, const mipnerf_b200_weights* w,
                                   const mipnerf_b200_rays* rays, int randomized, const float* t_rand,
                                   const float* u_jitter, const mipnerf_b200_rng* rng, int white_bkgd, int precision,
@@ -890,23 +931,18 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
   const int64_t B = rays->num_rays;
   // bf16x3: every operand of the backward is a pair of bf16 tile images, hi and lo (the 16-bit launchers' format
   // argument is then bf16, and the *_lo arguments select their split kernels)
-  const bool x3 = precision == MIPNERF_B200_BF16X3;
-  const int fmt = x3 ? MIPNERF_B200_BF16 : precision;
+  const bool x3 = mipnerf::is_x3(precision);
+  const int fmt = mipnerf::fmt_of(precision);
   const int64_t chunk = x3 ? kChunkRaysX3 : kChunkRaysFp32;
   const FusedScratch s0 = carve_fused(cfg, d, B < chunk ? B : chunk, precision, workspace);
   // ---- once per call (the weights change every optimiser step): the level kernels' packed image, and the
-  //      transposed B operands of the dgrad chain  bwd[i] = W_i[:, :256]^T  (slots depth / depth+1: bottleneck, view)
+  //      transposed B operands of the dgrad chain
   mipnerf_b200_weights wl = *w;
   wl.packed = s0.packed;
   CUDA_TRY(mipnerf::tc_pack_weights(cfg, w, precision, s0.packed, st));
-  const uint8_t* img_bwd[kMaxTrainDepth + 2] = {nullptr};
-  const uint8_t* img_bwd_lo[kMaxTrainDepth + 2] = {nullptr};  // bf16x3: slot + kMaxTrainDepth + 2
-  CUDA_TRY(pack_bwd_images(cfg, w, precision, s0.images, img_bwd, img_bwd_lo, st));
-  // fp16 gradients underflow: d loss / d activation is ~1e-7 .. 1e-4 per sample (the loss is a mean over the batch),
-  // below fp16's 6e-5 normal range.  The backward pass is linear in d loss / d raw, so render_backward emits it
-  // scaled by 2^10 (it is bounded by 2/3 per sample: no overflow), every gradient tile image carries that factor, and
-  // the fixed-order reduction of the wgrad partials takes it out again.  bf16 has fp32's range: scale 1.
-  const float gscale = precision == MIPNERF_B200_FP16 ? 1024.f : 1.f, inv_gscale = 1.f / gscale;
+  LayerImages im;
+  CUDA_TRY(pack_layer_images(cfg, d, w, precision, false, s0.images, &im, st));
+  const float gscale = grad_scale_of(precision), inv_gscale = 1.f / gscale;
   for (int64_t off = 0; off < B; off += chunk) {
     const int64_t cnt = (B - off) < chunk ? (B - off) : chunk;
     const mipnerf_b200_rays rc_ = offset_rays(*rays, off, cnt);
@@ -920,16 +956,7 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
     mipnerf_b200_level_out lo[2];
     mipnerf::TcTrainDump dump{};
     for (int l = 0; l < cfg->num_levels; ++l) {
-      lo[l] = outs[l];
-      if (given_t) {  // the recompute's pixels are not needed: they go to the (unused) fencepost scratch
-        lo[l].comp_rgb = s.t[l], lo[l].distance = s.t[l] + 3 * cnt, lo[l].acc = s.t[l] + 4 * cnt;
-      } else {
-        lo[l].comp_rgb = outs[l].comp_rgb + off * 3, lo[l].distance = outs[l].distance + off, lo[l].acc = outs[l].acc + off;
-      }
-      lo[l].t_samples = outs[l].t_samples ? outs[l].t_samples + off * (n + 1) : s.t[l];
-      lo[l].weights = outs[l].weights ? outs[l].weights + off * n : s.w[l];
-      lo[l].inds = outs[l].inds ? outs[l].inds + off * (n + 1) : nullptr;
-      lo[l].density_normal = outs[l].density_normal ? outs[l].density_normal + off * n : nullptr;
+      lo[l] = chunk_level_out(outs[l], off, cnt, n, given_t, s.t[l], s.w[l]);
       dump.act[l] = s.act[l], dump.v[l] = s.v[l], dump.raw_rgb[l] = s.raw_rgb[l], dump.raw_density[l] = s.raw_density[l];
     }
     CUDA_TRY(mipnerf::tc_forward(cfg, &wl, &rc_, randomized, t_rand ? t_rand + off * (n + 1) : nullptr,
@@ -946,9 +973,7 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
       const TileChainOps ops{s.act[l], s.v[l], s.enc16, s.venc, n, s.d_raw_rgb, s.d_raw_density,
                              s.d_v, s.d_a, s.d_b, s.relu_bits, s.part, cnt};
       int rc;
-      if ((rc = tile_backward_chain(cfg, d, w, precision, img_bwd, img_bwd_lo, ops, false, inv_gscale, grads, touched,
-                                    st)))
-        return rc;
+      if ((rc = tile_backward_chain(cfg, d, w, precision, im, ops, false, inv_gscale, grads, touched, st))) return rc;
     }
   }
   return MIPNERF_B200_OK;
@@ -969,9 +994,9 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   if ((rc = check_train_config(cfg))) return rc;
   if ((rc = check_weights(cfg, d, w))) return rc;
   if ((rc = check_rays(rays))) return rc;
-  const bool x3 = precision == MIPNERF_B200_BF16X3;
+  const bool x3 = mipnerf::is_x3(precision);
   const bool tc = precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_FP16 || x3;
-  if (precision == MIPNERF_B200_FP16X3 || (x3 && (src.cots || !train_fused_supported(cfg, precision))))
+  if (x3 && (src.cots || !train_fused_supported(cfg, precision)))
     return fail(MIPNERF_B200_EUNSUPPORTED,
                 "training: BF16X3 is the one split-operand training precision, for the fused training-loss step only "
                 "(8x256 / 1x128 MLP, default encodings, 128 samples, at most two levels; no backward from cotangents); "
@@ -981,13 +1006,8 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
     return fail(MIPNERF_B200_EUNSUPPORTED,
                 "tensor-core training GEMMs: 8x256 trunk / 128 view layer / 96-d IPE only; use MIPNERF_B200_FP32");
   if (!outs || !(src.loss || src.cots) || !grads) return fail(MIPNERF_B200_EINVAL, "outs / loss / grads is NULL");
-  if (src.cots && precision == MIPNERF_B200_FP16)
-    return fail(MIPNERF_B200_EUNSUPPORTED,
-                "backward from arbitrary cotangents: FP16's fixed gradient scale is sized for the training loss; use "
-                "BF16 (same tensor-core path, fp32 range) or FP32");
-  if (num_grads != d.n_lin) return fail(MIPNERF_B200_EINVAL, "expected %d gradient pairs, got %d", d.n_lin, num_grads);
-  for (int i = 0; i < d.n_lin; ++i)
-    if (!grads[i].weight_grad || !grads[i].bias_grad) return fail(MIPNERF_B200_EINVAL, "grads[%d] has a NULL tensor", i);
+  if (src.cots && (rc = check_cotangent_precision(precision, "backward from arbitrary cotangents"))) return rc;
+  if ((rc = check_grads(d, grads, num_grads))) return rc;
   if (src.loss && (!src.loss->level_mse_mult || !src.loss->level_dist_mult))
     return fail(MIPNERF_B200_EINVAL, "loss multipliers are NULL");
   if (src.loss && rays->num_rays > 0 && (!src.loss->target_rgb || !src.loss->mask_sum || !rays->viewdirs))
@@ -1002,10 +1022,7 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
     if (given_t && rays->num_rays > 0 && !outs[l].t_samples)
       return fail(MIPNERF_B200_EINVAL, "t_samples[%d] is NULL", l);
   }
-  {
-    const int rcn = check_density_normals(cfg, randomized, rng, outs, rays->num_rays);
-    if (rcn) return rcn;
-  }
+  if ((rc = check_density_normals(cfg, randomized, rng, outs, rays->num_rays))) return rc;
   const size_t need = x3 ? mipnerf_b200_train_workspace_bytes_for(cfg, rays->num_rays, precision)
                         : mipnerf_b200_train_workspace_bytes(cfg, rays->num_rays);
   if (rays->num_rays > 0 && (!workspace || workspace_bytes < need))
@@ -1014,27 +1031,21 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   const int n = cfg->num_samples, depth = cfg->net_depth;
   const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   const int64_t B = rays->num_rays;
-  // the per-layer fp16 GEMMs carry the fused step's gradient scale (forward_backward_fused says why): without it the
-  // gradient operands of deep trunks fall below fp16's normal range (measured at depth 16: 62 % of layers.0's gradient
-  // lost against the fp32 step)
-  const float gscale = precision == MIPNERF_B200_FP16 ? 1024.f : 1.f;
+  const float gscale = grad_scale_of(precision);
+  // with rays, the chains reach every linear (check_train_config: one view layer)
   bool touched[kMaxTrainDepth + 8];
-  for (int i = 0; i < d.n_lin; ++i) touched[i] = accumulate != 0;
-  if (B == 0 && !accumulate)
-    for (int i = 0; i < d.n_lin; ++i) {
-      const mipnerf_b200_linear& l = w->linears[i];
-      CUDA_TRY(cudaMemsetAsync(grads[i].weight_grad, 0, sizeof(float) * l.in_features * l.out_features, st));
-      CUDA_TRY(cudaMemsetAsync(grads[i].bias_grad, 0, sizeof(float) * l.out_features, st));
-    }
-
-  if (tc && B > 0 && train_fused_supported(cfg, precision))
-    return forward_backward_fused(cfg, d, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision, src,
-                                  given_t, outs, grads, touched, workspace, st);
+  std::fill_n(touched, d.n_lin, accumulate != 0);
+  if (tc && B > 0 && train_fused_supported(cfg, precision)) {
+    if ((rc = forward_backward_fused(cfg, d, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision, src,
+                                     given_t, outs, grads, touched, workspace, st)))
+      return rc;
+    return zero_untouched(d, w, grads, touched, st);
+  }
   // ---- tensor-core mode: B operands of every forward / dgrad GEMM, packed once per call
   LayerImages im{};
   if (tc && B > 0)
-    CUDA_TRY(pack_layer_images(cfg, d, w, precision,
-                               carve_train(cfg, d, B < kChunkRaysFp32 ? B : kChunkRaysFp32, workspace).images, &im, st));
+    CUDA_TRY(pack_layer_images(cfg, d, w, precision, true,
+                               carve_train(cfg, d, std::min(B, kChunkRaysFp32), workspace).images, &im, st));
 
   for (int64_t off = 0; off < B; off += kChunkRaysFp32) {
     const int64_t cnt = (B - off) < kChunkRaysFp32 ? (B - off) : kChunkRaysFp32;
@@ -1048,43 +1059,37 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
     }
     const float *t_prev = nullptr, *w_prev = nullptr;
     for (int l = 0; l < cfg->num_levels; ++l) {
-      float* t_cur = outs[l].t_samples ? outs[l].t_samples + off * (n + 1) : s.t[l & 1];
-      float* w_cur = outs[l].weights ? outs[l].weights + off * n : s.w[l & 1];
-      // given fenceposts: the recomputed pixels go to the (unused) fencepost scratch
-      float* comp_cur = given_t ? s.t[l & 1] : outs[l].comp_rgb + off * 3;
-      float* dist_cur = given_t ? s.t[l & 1] + 3 * cnt : outs[l].distance + off;
-      float* acc_cur = given_t ? s.t[l & 1] + 4 * cnt : outs[l].acc + off;
+      const mipnerf_b200_level_out lo = chunk_level_out(outs[l], off, cnt, n, given_t, s.t[l & 1], s.w[l & 1]);
       // ---- forward of this level, every activation kept (models/mip_nerf.py:203-240)
       if (given_t) {
         // the caller's fenceposts: nothing to sample
       } else if (l == 0) {
         CUDA_TRY(mipnerf::launch_coarse_t(rc_.near, rc_.far, mipnerf::level_draws(randomized, t_rand, rng, off, 0, n + 1),
-                                          t_cur, cnt, n, randomized, cfg->disparity, st));
+                                          lo.t_samples, cnt, n, randomized, cfg->disparity, st));
       } else {
         CUDA_TRY(mipnerf::launch_resample(t_prev, w_prev, mipnerf::level_draws(randomized, u_jitter, rng, off, 1 + l, n + 1),
-                                          t_cur, outs[l].inds ? outs[l].inds + off * (n + 1) : nullptr, cnt, n, n + 1,
-                                          randomized, 1, cfg->resample_padding, st));
+                                          lo.t_samples, lo.inds, cnt, n, n + 1, randomized, 1, cfg->resample_padding, st));
       }
-      CUDA_TRY(mipnerf::launch_ipe_from_t(rc_.origins, rc_.directions, rc_.radii, t_cur, s.enc, cnt, n,
+      CUDA_TRY(mipnerf::launch_ipe_from_t(rc_.origins, rc_.directions, rc_.radii, lo.t_samples, s.enc, cnt, n,
                                           cfg->min_deg_point, cfg->max_deg_point, cfg->disable_integration, st));
       if ((rc = mlp_forward_kept(cfg, d, w, tc, precision, im, s, m, n, false, st))) return rc;
       // density noise (models/mip_nerf.py:232-233), in place: render_backward then takes softplus' at the noisy point
       CUDA_TRY(mipnerf::launch_add_density_noise(
           s.raw_density, mipnerf::density_noise_draws(cfg, randomized, outs[l].density_normal, rng, off, l, n), cnt, n, st));
-      CUDA_TRY(mipnerf::launch_composite(s.raw_rgb, s.raw_density, t_cur, rc_.directions, comp_cur, dist_cur, acc_cur,
-                                         w_cur, cnt, n, white_bkgd, 1, cfg->density_bias, rgb_scale, cfg->rgb_padding,
-                                         st));
+      CUDA_TRY(mipnerf::launch_composite(s.raw_rgb, s.raw_density, lo.t_samples, rc_.directions, lo.comp_rgb,
+                                         lo.distance, lo.acc, lo.weights, cnt, n, white_bkgd, 1, cfg->density_bias,
+                                         rgb_scale, cfg->rgb_padding, st));
 
       // ---- backward of this level (its fenceposts are constants, so levels are independent here)
-      CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb, s.raw_density, t_cur, rc_.directions, white_bkgd,
-                                  rgb_scale, gscale, s.d_raw_rgb, s.d_raw_density, st));
+      CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb, s.raw_density, lo.t_samples, rc_.directions,
+                                  white_bkgd, rgb_scale, gscale, s.d_raw_rgb, s.d_raw_density, st));
       if ((rc = mlp_backward_chain(cfg, d, w, tc, precision, im, s, m, n, false, grads, touched, st, 1.f / gscale)))
         return rc;
-      t_prev = t_cur;
-      w_prev = w_cur;
+      t_prev = lo.t_samples;
+      w_prev = lo.weights;
     }
   }
-  return MIPNERF_B200_OK;
+  return zero_untouched(d, w, grads, touched, st);
 }
 
 int mipnerf_b200_forward_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
@@ -1915,9 +1920,8 @@ int query_backward_bf16(const mipnerf_b200_config* cfg, const Dims& d, const mip
   mipnerf_b200_weights wl = *w;
   wl.packed = s0.packed, wl.packed_precision = prec, wl.packed_bytes = mipnerf::tc_packed_bytes(cfg, prec);
   CUDA_TRY(mipnerf::tc_pack_weights(cfg, w, prec, s0.packed, st));
-  const uint8_t* img_bwd[kMaxTrainDepth + 2] = {nullptr};
-  const uint8_t* img_bwd_lo[kMaxTrainDepth + 2] = {nullptr};
-  CUDA_TRY(pack_bwd_images(cfg, w, prec, s0.images, img_bwd, img_bwd_lo, st));
+  LayerImages im;
+  CUDA_TRY(pack_layer_images(cfg, d, w, prec, false, s0.images, &im, st));
   int rc;
   for (int64_t off = 0; off < num_points; off += chunk) {
     const int64_t m = std::min(num_points - off, chunk);
@@ -1946,8 +1950,7 @@ int query_backward_bf16(const mipnerf_b200_config* cfg, const Dims& d, const mip
     }
     const TileChainOps ops{s.act, s.v, s.enc16, s.venc, 1, s.d_raw_rgb, s.d_raw_density,
                            s.d_v, s.d_a, s.d_b, s.relu_bits, s0.part, tiles};
-    if ((rc = tile_backward_chain(cfg, d, w, prec, img_bwd, img_bwd_lo, ops, !radiance, 1.f, grads, touched, st)))
-      return rc;
+    if ((rc = tile_backward_chain(cfg, d, w, prec, im, ops, !radiance, 1.f, grads, touched, st))) return rc;
   }
   return MIPNERF_B200_OK;
 }
@@ -1970,15 +1973,8 @@ int mipnerf_b200_query_backward(const mipnerf_b200_config* cfg, const mipnerf_b2
   int rc;
   if ((rc = check_query(cfg, &d, w, num_points, means, precision))) return rc;
   if (!cot || !grads) return fail(MIPNERF_B200_EINVAL, "cot / grads is NULL");
-  if (num_grads != d.n_lin) return fail(MIPNERF_B200_EINVAL, "expected %d gradient pairs, got %d", d.n_lin, num_grads);
-  for (int i = 0; i < d.n_lin; ++i)
-    if (!grads[i].weight_grad || !grads[i].bias_grad) return fail(MIPNERF_B200_EINVAL, "grads[%d] has a NULL tensor", i);
-  if (precision == MIPNERF_B200_FP16)
-    return fail(MIPNERF_B200_EUNSUPPORTED,
-                "query backward: FP16's fixed gradient scale is sized for the training loss and arbitrary cotangents "
-                "can overflow or underflow it; use BF16 (fp32 range) or FP32");
-  if (precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3)
-    return fail(MIPNERF_B200_EUNSUPPORTED, "query backward: the split-operand precisions are forward-only; use FP32 or BF16");
+  if ((rc = check_grads(d, grads, num_grads))) return rc;
+  if ((rc = check_cotangent_precision(precision, "query backward"))) return rc;
   if ((rc = check_train_config(cfg))) return rc;
   if (!query_grad_supported(cfg, d, precision))
     return fail(MIPNERF_B200_EUNSUPPORTED,
@@ -1989,20 +1985,12 @@ int mipnerf_b200_query_backward(const mipnerf_b200_config* cfg, const mipnerf_b2
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
   bool touched[kMaxTrainDepth + 8];
-  for (int i = 0; i < d.n_lin; ++i) touched[i] = accumulate != 0;
+  std::fill_n(touched, d.n_lin, accumulate != 0);
   if (num_points > 0) {
-    rc = precision == MIPNERF_B200_BF16
-             ? query_backward_bf16(cfg, d, w, means, covs, viewdirs, num_points, cot, grads, touched, workspace, st)
-             : query_backward_fp32(cfg, d, w, means, covs, viewdirs, num_points, cot, grads, touched, workspace, st);
-    if (rc) return rc;
+    auto* driver = precision == MIPNERF_B200_BF16 ? query_backward_bf16 : query_backward_fp32;
+    if ((rc = driver(cfg, d, w, means, covs, viewdirs, num_points, cot, grads, touched, workspace, st))) return rc;
   }
-  for (int i = 0; i < d.n_lin; ++i)  // no points, or the heads a density query does not reach: exact zeros
-    if (!touched[i]) {
-      const mipnerf_b200_linear& l = w->linears[i];
-      CUDA_TRY(cudaMemsetAsync(grads[i].weight_grad, 0, sizeof(float) * l.in_features * l.out_features, st));
-      CUDA_TRY(cudaMemsetAsync(grads[i].bias_grad, 0, sizeof(float) * l.out_features, st));
-    }
-  return MIPNERF_B200_OK;
+  return zero_untouched(d, w, grads, touched, st);
 }
 
 size_t mipnerf_b200_isosurface_scratch_bytes(int nx, int ny, int nz) {

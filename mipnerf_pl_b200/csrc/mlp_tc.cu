@@ -1735,10 +1735,6 @@ TcScratch carve_tc(int64_t rays, int n, void* base) {
 
 int g_num_sms = 0;
 
-// operand format (0 fp16, 1 bf16) and split flag of a tensor-core precision
-inline int fmt_of(int precision) { return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_BF16X3) ? 1 : 0; }
-inline bool is_x3(int precision) { return precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3; }
-
 int num_sms() {
   if (g_num_sms == 0) {
     int dev = 0;
@@ -1775,7 +1771,7 @@ cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
 template <int kMode, int kT = 1>
 cudaError_t launch_level(const LevelParams& p, int precision, cudaStream_t st) {
   if (p.num_rays <= 0) return cudaSuccess;
-  const bool bf = fmt_of(precision) == 1;
+  const bool bf = fmt_of(precision) == MIPNERF_B200_BF16;
   if constexpr (kMode == kModeDensity || kMode == kModeRadiance)
     if (p.act_dump)
       return bf ? launch_level_t<1, false, 1, kMode, false, true>(p, st)
@@ -1856,7 +1852,7 @@ cudaError_t tc_pack_weights(const mipnerf_b200_config* c, const mipnerf_b200_wei
                             void* packed_out, cudaStream_t st) {
   if (!tc_supported(c, precision)) return cudaErrorNotSupported;
   uint8_t* img = static_cast<uint8_t*>(packed_out);
-  const bool bf = fmt_of(precision) == 1;
+  const bool bf = fmt_of(precision) == MIPNERF_B200_BF16;
   const int parts = is_x3(precision) ? 2 : 1;  // hi image, then (split modes) the lo stage image
   cudaError_t e = cudaMemsetAsync(img, 0, kImageEnd, st);
   if (e != cudaSuccess) return e;
@@ -1991,7 +1987,8 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
       if (!outs[l].density_normal) p.dnoise.ray_base += ray_base;
       // the split precisions' training forward dumps the lo halves as well (kTrain); bf16x3 is the one that trains
       if (dump && is_x3(precision))
-        e = fmt_of(precision) ? launch_level_t<1, true, 1, kModeForward, true>(p, st) : cudaErrorNotSupported;
+        e = fmt_of(precision) == MIPNERF_B200_BF16 ? launch_level_t<1, true, 1, kModeForward, true>(p, st)
+                                                  : cudaErrorNotSupported;
       else
         e = n == 2 * kN ? launch_level<kModeForward, 2>(p, precision, st)
                         : launch_level<kModeForward>(p, precision, st);

@@ -12,6 +12,13 @@ namespace mipnerf {
 // 1 + 2 rgb_padding, the scale of the padded sigmoid colour activation (models/mip_nerf.py:236)
 inline float rgb_scale_of(const mipnerf_b200_config* c) { return (float)(1.0 + 2.0 * (double)c->rgb_padding); }
 
+// The 16-bit operand format of a tensor-core precision (MIPNERF_B200_BF16 or MIPNERF_B200_FP16) and whether the
+// precision is split, carrying every operand as a hi / lo pair of that format.
+inline int fmt_of(int precision) {
+  return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_BF16X3) ? MIPNERF_B200_BF16 : MIPNERF_B200_FP16;
+}
+inline bool is_x3(int precision) { return precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3; }
+
 inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 
 // The scratch layouts' bump allocator: 256-byte-aligned takes from `base` in call order; a null base only counts bytes.

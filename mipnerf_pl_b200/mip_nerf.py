@@ -27,7 +27,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _cabi
-from .ops import _dev, _f32, _ptr, _stream, draw_density_normal, draw_t_rand, draw_u_jitter
+from .ops import _dev, _f32, _grad_array, _ptr, _rays_struct, _stream, draw_density_normal, draw_t_rand, draw_u_jitter
 from .rays import Rays
 
 
@@ -256,6 +256,25 @@ class MipNerf(torch.nn.Module):
         self.rng_offset += 1
         return rng
 
+    def _noise(self, randomized: bool, b: int, dev, t_rand, u_jitter, density_normal):
+        """The noise of a call on b rays -> (rng, t_rand, u_jitter, normals).  randomized without any injected array:
+        the kernels draw in-kernel from `next_rng()`.  Otherwise the arrays not given are drawn with torch's generator,
+        and `normals` holds one [B,N] tensor per level when density_noise > 0 (models/mip_nerf.py:232-233)."""
+        levels, n = self.num_levels, self.num_samples
+        if not randomized:
+            return None, None, None, [None] * levels
+        if t_rand is None and u_jitter is None and density_normal is None:
+            return self.next_rng(), None, None, [None] * levels  # no torch.rand launch, no [B,N+1] arrays
+        t_rand = _f32(t_rand) if t_rand is not None else draw_t_rand(b, n, dev)
+        u_jitter = _f32(u_jitter) if u_jitter is not None else draw_u_jitter(b, n + 1, dev)
+        normals = list(density_normal) if density_normal is not None else [None] * levels
+        if len(normals) != levels:
+            raise ValueError(f"density_normal: expected {levels} tensors (one per level)")
+        if not self.density_noise > 0:
+            return None, t_rand, u_jitter, [None] * levels
+        return None, t_rand, u_jitter, [_f32(x).reshape(b, n) if x is not None else draw_density_normal(b, n, dev)
+                                        for x in normals]
+
     def _config(self) -> "_cabi.Config":
         return self.mlp._config(
             num_samples=self.num_samples, num_levels=self.num_levels, min_deg_point=self.min_deg_point,
@@ -449,26 +468,8 @@ class MipNerf(torch.nn.Module):
         n = self.num_samples
         prec = _cabi.PRECISIONS[self.precision]
         cfg = self._config()
-        keep = [_f32(rays.origins), _f32(rays.directions), _f32(rays.viewdirs), _f32(rays.radii).reshape(-1),
-                _f32(rays.near).reshape(-1), _f32(rays.far).reshape(-1)]
-        rs = _cabi.RaysStruct(keep[0].data_ptr(), keep[1].data_ptr(), keep[2].data_ptr(), keep[3].data_ptr(),
-                              keep[4].data_ptr(), keep[5].data_ptr(), b)
-        rng = None
-        noisy = bool(randomized) and self.density_noise > 0     # models/mip_nerf.py:232
-        if randomized and t_rand is None and u_jitter is None and density_normal is None:
-            rng = self.next_rng()                       # in-kernel Philox: no torch.rand launch, no [B,N+1] arrays
-            normals = [None] * self.num_levels
-        elif randomized:
-            t_rand = _f32(t_rand) if t_rand is not None else draw_t_rand(b, n, dev)
-            u_jitter = _f32(u_jitter) if u_jitter is not None else draw_u_jitter(b, n + 1, dev)
-            normals = list(density_normal) if density_normal is not None else [None] * self.num_levels
-            if len(normals) != self.num_levels:
-                raise ValueError(f"density_normal: expected {self.num_levels} tensors (one per level)")
-            normals = [(_f32(x).reshape(b, n) if x is not None else draw_density_normal(b, n, dev)) if noisy else None
-                       for x in normals]
-        else:
-            t_rand = u_jitter = None
-            normals = [None] * self.num_levels
+        rs, keep = _rays_struct(rays.origins, rays.directions, rays.viewdirs, rays.radii, rays.near, rays.far)
+        rng, t_rand, u_jitter, normals = self._noise(randomized, b, dev, t_rand, u_jitter, density_normal)
         ws, wkeep = self.mlp._weights_struct(cfg, prec, dev)
         outs = (_cabi.LevelOut * self.num_levels)()
         # One allocation for everything: the per-level pixel outputs (comp_rgb | distance | acc = 5 floats/ray) of
@@ -513,16 +514,20 @@ class MipNerf(torch.nn.Module):
         return ret, cfg, rng, normals, keep
 
 
-def _check_autograd(model: MipNerf, rays: Rays, b: int) -> None:
-    """Refuse, at forward time, what the backward pass cannot differentiate."""
+def _check_autograd_precision(model: MipNerf, what: str) -> None:
+    """The precisions a backward pass from arbitrary cotangents takes: fp32 and bf16."""
     if model.precision in ("fp16x3", "bf16x3"):
-        raise NotImplementedError(f"MipNerf(autograd=True): precision={model.precision!r} is forward-only; "
-                                  "use 'fp32' or 'bf16'")
+        raise NotImplementedError(f"{what}: precision={model.precision!r} is forward-only; use 'fp32' or 'bf16'")
     if model.precision == "fp16":
-        raise NotImplementedError("MipNerf(autograd=True): fp16's fixed gradient scale is sized for the reference loss "
-                                  "and arbitrary losses can overflow or underflow it; use precision='bf16'")
+        raise NotImplementedError(f"{what}: fp16's fixed gradient scale is sized for the reference loss and arbitrary "
+                                  "losses can overflow or underflow it; use precision='bf16'")
     if model.precision not in ("fp32", "bf16"):
         raise ValueError(f"precision={model.precision!r}")
+
+
+def _check_autograd(model: MipNerf, rays: Rays, b: int) -> None:
+    """Refuse, at forward time, what the backward pass cannot differentiate."""
+    _check_autograd_precision(model, "MipNerf(autograd=True)")
     if not model.stop_resample_grad:
         raise NotImplementedError("MipNerf(autograd=True): gradients through the resampled fenceposts "
                                   "(stop_resample_grad=False) are not implemented")
@@ -530,15 +535,13 @@ def _check_autograd(model: MipNerf, rays: Rays, b: int) -> None:
         raise NotImplementedError("MipNerf(autograd=True): gradients with respect to the rays are not implemented; "
                                   "pass ray tensors that do not require grad")
     cfg = model._config()
-    if _cabi.lib().mipnerf_b200_train_workspace_bytes(C.byref(cfg), max(b, 1)) == 0:
+    lib = _cabi.lib()
+    if lib.mipnerf_b200_train_workspace_bytes(C.byref(cfg), max(b, 1)) == 0:
         raise NotImplementedError(f"MipNerf(autograd=True): {_cabi.last_error() or 'no training kernels'}; the "
                                   "backward pass needs use_viewdirs=True with one view layer and net_depth <= 16")
-    if model.precision == "bf16":
-        m = model.mlp
-        # the 16-bit training GEMMs exist for the default widths and encodings only (api.cu train_tc_supported)
-        if not (m.net_width == 256 and m.net_width_condition == 128 and m.xyz_dim == 96 and m.view_dim == 27):
-            raise NotImplementedError("MipNerf(autograd=True, precision='bf16'): the tensor-core backward supports the "
-                                      "8x256 / 1x128 MLP with max_deg_point=16, deg_view=4; use precision='fp32'")
+    if model.precision == "bf16" and lib.mipnerf_b200_train_workspace_bytes_for(C.byref(cfg), max(b, 1), _cabi.BF16) == 0:
+        raise NotImplementedError("MipNerf(autograd=True, precision='bf16'): the tensor-core backward supports the "
+                                  "8x256 / 1x128 MLP with max_deg_point=16, deg_view=4; use precision='fp32'")
 
 
 def _forward_with_grad(model: MipNerf, rays: Rays, randomized, white_bkgd, t_rand, u_jitter, density_normal,
@@ -595,7 +598,7 @@ class _ForwardWithGrad(torch.autograd.Function):
         out_grads = [torch.empty_like(p) for p in params]
         if all(g is None for g in grads) or b == 0:
             return (None,) * 9 + tuple(g.zero_() for g in out_grads)
-        rs = _cabi.RaysStruct(*[k.data_ptr() for k in keep], b)
+        rs, _ = _rays_struct(*keep)
         cots = (_cabi.LevelCotangent * levels)()
         cot_keep = []
         for lvl in range(levels):
@@ -616,9 +619,7 @@ class _ForwardWithGrad(torch.autograd.Function):
                 normal_arr[i] = x.data_ptr()
         rng = _cabi.Rng(*ctx.rng) if ctx.rng is not None else None
         ws, wkeep = model.mlp._weights_struct(cfg, _cabi.FP32, dev)
-        garr = (_cabi.LinearGrad * (np_ // 2))()
-        for i in range(np_ // 2):
-            garr[i] = _cabi.LinearGrad(out_grads[2 * i].data_ptr(), out_grads[2 * i + 1].data_ptr())
+        garr = _grad_array(out_grads)
         lib = _cabi.lib()
         nbytes = lib.mipnerf_b200_train_workspace_bytes(C.byref(cfg), b)
         scratch = _Workspace.get(dev, nbytes)
@@ -626,22 +627,14 @@ class _ForwardWithGrad(torch.autograd.Function):
             _cabi.check(lib.mipnerf_b200_backward(
                 C.byref(cfg), C.byref(ws), C.byref(rs), t_arr, int(ctx.randomized),
                 C.byref(rng) if rng is not None else None, normal_arr, int(ctx.white_bkgd),
-                _cabi.PRECISIONS[ctx.precision], cots, garr, np_ // 2, 0, scratch.data_ptr(), scratch.numel(),
+                _cabi.PRECISIONS[ctx.precision], cots, garr, len(garr), 0, scratch.data_ptr(), scratch.numel(),
                 _stream(dev)), "MipNerf.backward")
         return (None,) * 9 + tuple(out_grads)
 
 
 def _check_query_autograd(model: MipNerf, tensors, radiance: bool) -> None:
     """Refuse, at query time, what the query backward cannot differentiate."""
-    if model.precision in ("fp16x3", "bf16x3"):
-        raise NotImplementedError(f"MipNerf(autograd=True) queries: precision={model.precision!r} is forward-only; "
-                                  "use 'fp32' or 'bf16'")
-    if model.precision == "fp16":
-        raise NotImplementedError("MipNerf(autograd=True) queries: fp16's fixed gradient scale is sized for the "
-                                  "reference loss and arbitrary losses can overflow or underflow it; use "
-                                  "precision='bf16'")
-    if model.precision not in ("fp32", "bf16"):
-        raise ValueError(f"precision={model.precision!r}")
+    _check_autograd_precision(model, "MipNerf(autograd=True) queries")
     if any(isinstance(x, torch.Tensor) and x.requires_grad for x in tensors):
         raise NotImplementedError("MipNerf(autograd=True) queries: gradients with respect to means, covs or viewdirs "
                                   "are not implemented; pass tensors that do not require grad")
@@ -681,7 +674,7 @@ class _QueryWithGrad(torch.autograd.Function):
         else:
             outs = (model._query_density(means, covs, raw),)
         ctx.model, ctx.cfg, ctx.raw, ctx.radiance = model, model._config(), raw, radiance
-        ctx.precision, ctx.num_params = model.precision, len(params)
+        ctx.precision = model.precision
         ctx.save_for_backward(means, covs, viewdirs, *params)
         ctx.set_materialize_grads(False)
         return outs
@@ -692,7 +685,6 @@ class _QueryWithGrad(torch.autograd.Function):
         saved = ctx.saved_tensors  # raises if a parameter was updated in place since the forward
         means, covs, viewdirs = saved[:3]
         params = saved[3:]
-        np_ = ctx.num_params
         dev = means.device
         p = means.shape[0]
         out_grads = [torch.empty_like(x) for x in params]
@@ -708,9 +700,7 @@ class _QueryWithGrad(torch.autograd.Function):
         model, cfg = ctx.model, ctx.cfg
         prec = _cabi.PRECISIONS[ctx.precision]
         ws, wkeep = model.mlp._weights_struct(cfg, _cabi.FP32, dev)
-        garr = (_cabi.LinearGrad * (np_ // 2))()
-        for i in range(np_ // 2):
-            garr[i] = _cabi.LinearGrad(out_grads[2 * i].data_ptr(), out_grads[2 * i + 1].data_ptr())
+        garr = _grad_array(out_grads)
         lib = _cabi.lib()
         nbytes = lib.mipnerf_b200_query_backward_workspace_bytes(C.byref(cfg), p, int(ctx.radiance), prec)
         # per call, not the per-stream _Workspace: up to one chunk's activations (GBs), which a forward-only process
@@ -719,5 +709,5 @@ class _QueryWithGrad(torch.autograd.Function):
         with torch.cuda.device(dev):
             _cabi.check(lib.mipnerf_b200_query_backward(
                 C.byref(cfg), C.byref(ws), means.data_ptr(), _ptr(covs), _ptr(viewdirs), p, prec, C.byref(cot), garr,
-                np_ // 2, 0, scratch.data_ptr(), scratch.numel(), _stream(dev)), "MipNerf.query backward")
+                len(garr), 0, scratch.data_ptr(), scratch.numel(), _stream(dev)), "MipNerf.query backward")
         return (None,) * 5 + tuple(out_grads)

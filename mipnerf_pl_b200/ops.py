@@ -42,16 +42,22 @@ def _stream(device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
 
 
-def _rays_struct(origins, directions, radii, near=None, far=None, viewdirs=None):
+def _rays_struct(origins, directions, viewdirs, radii, near=None, far=None):
+    """(RaysStruct, keep): `keep` holds the fp32 ray tensors the struct points at, in its field order; viewdirs may be
+    None (NULL), near / far default to zeros."""
     n = origins.shape[0]
-    keep = [_f32(origins), _f32(directions), _f32(radii).reshape(-1)]
-    near_t = _f32(near).reshape(-1) if near is not None else torch.zeros(n, device=origins.device)
-    far_t = _f32(far).reshape(-1) if far is not None else torch.zeros(n, device=origins.device)
-    vd = _f32(viewdirs) if viewdirs is not None else None
-    keep += [near_t, far_t, vd]
-    s = _cabi.RaysStruct(keep[0].data_ptr(), keep[1].data_ptr(), _ptr(vd), keep[2].data_ptr(),
-                         near_t.data_ptr(), far_t.data_ptr(), n)
-    return s, keep
+    zeros = lambda: torch.zeros(n, device=origins.device)  # noqa: E731
+    keep = [_f32(origins), _f32(directions), _f32(viewdirs) if viewdirs is not None else None, _f32(radii).reshape(-1),
+            _f32(near).reshape(-1) if near is not None else zeros(), _f32(far).reshape(-1) if far is not None else zeros()]
+    return _cabi.RaysStruct(*[_ptr(k) for k in keep], n), keep
+
+
+def _grad_array(grads):
+    """The LinearGrad array over (weight, bias) gradient tensors in `MLP.linears()` order."""
+    arr = (_cabi.LinearGrad * (len(grads) // 2))()
+    for i in range(len(arr)):
+        arr[i] = _cabi.LinearGrad(grads[2 * i].data_ptr(), grads[2 * i + 1].data_ptr())
+    return arr
 
 
 def draw_t_rand(batch: int, num_samples: int, device) -> torch.Tensor:
@@ -106,7 +112,7 @@ def cast_rays(t_samples, origins, directions, radii, ray_shape, diagonal=True):
     dev = _dev(t_samples)
     t = _f32(t_samples)
     b, n = t.shape[0], t.shape[1] - 1
-    rs, keep = _rays_struct(origins, directions, radii)
+    rs, keep = _rays_struct(origins, directions, None, radii)
     means = torch.empty(b, n, 3, device=dev)
     covs = torch.empty(b, n, 3, device=dev)
     with torch.cuda.device(dev):
@@ -123,7 +129,7 @@ def sample_along_rays(origins, directions, radii, num_samples, near, far, random
     assert ray_shape == "cone"
     dev = _dev(origins)
     b = origins.shape[0]
-    rs, keep = _rays_struct(origins, directions, radii, near, far)
+    rs, keep = _rays_struct(origins, directions, None, radii, near, far)
     if randomized and t_rand is None:
         t_rand = draw_t_rand(b, num_samples, dev)
     tr = _f32(t_rand) if randomized else None
@@ -168,7 +174,7 @@ def resample_along_rays(origins, directions, radii, t_samples, weights, randomiz
     dev = _dev(t_samples)
     t, w = _f32(t_samples), _f32(weights)
     b, n = w.shape
-    rs, keep = _rays_struct(origins, directions, radii)
+    rs, keep = _rays_struct(origins, directions, None, radii)
     if randomized and u_jitter is None:
         u_jitter = draw_u_jitter(b, n + 1, dev)
     uj = _f32(u_jitter) if randomized else None

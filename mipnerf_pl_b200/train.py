@@ -27,7 +27,7 @@ import torch
 
 from . import _cabi
 from .mip_nerf import MipNerf, _Workspace
-from .ops import _dev, _f32, _ptr, _stream, draw_density_normal, draw_t_rand, draw_u_jitter
+from .ops import _dev, _f32, _grad_array, _ptr, _rays_struct, _stream
 from .rays import Rays
 
 
@@ -197,24 +197,8 @@ def _run(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized: bool, white
     dev = _dev(rays.origins)
     b, n, levels = rays.origins.shape[0], model.num_samples, model.num_levels
     cfg = model._config()
-    keep = [_f32(rays.origins), _f32(rays.directions), _f32(rays.viewdirs), _f32(rays.radii).reshape(-1),
-            _f32(rays.near).reshape(-1), _f32(rays.far).reshape(-1)]
-    rs = _cabi.RaysStruct(*[k.data_ptr() for k in keep], b)
-    rng = None
-    noisy = bool(randomized) and model.density_noise > 0    # models/mip_nerf.py:232-233
-    normals = [None] * levels
-    if randomized and t_rand is None and u_jitter is None and density_normal is None:
-        rng = model.next_rng()          # uniforms / normals drawn inside the kernels (Philox), as every training step does
-    elif randomized:
-        t_rand = _f32(t_rand) if t_rand is not None else draw_t_rand(b, n, dev)
-        u_jitter = _f32(u_jitter) if u_jitter is not None else draw_u_jitter(b, n + 1, dev)
-        if noisy:
-            given = list(density_normal) if density_normal is not None else [None] * levels
-            if len(given) != levels:
-                raise ValueError(f"density_normal: expected {levels} tensors (one per level)")
-            normals = [_f32(x).reshape(b, n) if x is not None else draw_density_normal(b, n, dev) for x in given]
-    else:
-        t_rand = u_jitter = None
+    rs, keep = _rays_struct(rays.origins, rays.directions, rays.viewdirs, rays.radii, rays.near, rays.far)
+    rng, t_rand, u_jitter, normals = model._noise(randomized, b, dev, t_rand, u_jitter, density_normal)
     target = _f32(rgbs[..., :3]).reshape(b, 3)
     mask = None if disable_multiscale_loss else _f32(rays.lossmult).reshape(b)
     if mask_sum is None:
@@ -228,11 +212,7 @@ def _run(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized: bool, white
     loss = _cabi.Loss(target.data_ptr(), _ptr(mask), mask_sum.data_ptr(), 1.0 / max(global_rays, 1), mse_arr, dist_arr,
                       sqerr.data_ptr(), dl.data_ptr())
     ws, wkeep = model.mlp._weights_struct(cfg, _cabi.FP32, dev)
-    lins = model.mlp.linears()
-    assert len(grad_tensors) == 2 * len(lins)
-    garr = (_cabi.LinearGrad * len(lins))()
-    for i in range(len(lins)):
-        garr[i] = _cabi.LinearGrad(grad_tensors[2 * i].data_ptr(), grad_tensors[2 * i + 1].data_ptr())
+    garr = _grad_array(grad_tensors)
     outs = (_cabi.LevelOut * levels)()
     ret = []
     for lvl in range(levels):
@@ -245,7 +225,7 @@ def _run(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized: bool, white
     nbytes = (lib.mipnerf_b200_train_workspace_bytes_for(C.byref(cfg), b, prec) if prec == _cabi.BF16X3
               else lib.mipnerf_b200_train_workspace_bytes(C.byref(cfg), b))
     scratch = _Workspace.get(dev, nbytes)
-    tail = (int(bool(white_bkgd)), prec, C.byref(loss), outs, garr, len(lins), int(bool(accumulate)),
+    tail = (int(bool(white_bkgd)), prec, C.byref(loss), outs, garr, len(garr), int(bool(accumulate)),
             scratch.data_ptr() if nbytes else None, scratch.numel() if nbytes else 0, _stream(dev))
     with torch.cuda.device(dev):
         if rng is not None:

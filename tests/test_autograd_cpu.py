@@ -29,3 +29,16 @@ def test_autograd_forward_on_cpu_tensors_raises():
     assert torch.is_grad_enabled() and all(p.requires_grad for p in model.parameters())
     with pytest.raises(RuntimeError):
         model(rays, False, True)
+
+
+def test_bf16_autograd_refuses_at_forward_time_what_the_backward_refuses():
+    """Depth 16 with skip index 2 has the default widths, but the per-layer tensor-core step cannot hold its weight
+    images, so the bf16 backward would refuse it: the forward's precondition asks the library and refuses it first."""
+    from mipnerf_pl_b200 import mip_nerf
+    model = mp.MipNerf(mlp_net_depth=16, mlp_skip_index=2, precision="bf16", autograd=True)
+    rays = mp.random_ray_batch(8, seed=1, multiscale=True)
+    cfg = model._config()
+    assert _cabi.lib().mipnerf_b200_train_workspace_bytes_for(C.byref(cfg), 8, _cabi.FP32) > 0
+    assert _cabi.lib().mipnerf_b200_train_workspace_bytes_for(C.byref(cfg), 8, _cabi.BF16) == 0
+    with pytest.raises(NotImplementedError, match="tensor-core backward"):
+        mip_nerf._check_autograd(model, rays, 8)

@@ -243,6 +243,9 @@ def test_training_rejects_bad_arguments():
         ws, _ = model.mlp._weights_struct(cfg, _cabi.FP32, torch.device(DEV))
         _cabi.check(_cabi.lib().mipnerf_b200_forward_backward(C.byref(cfg), C.byref(ws), None, 1, None, None, 1, 0,
                                                               None, None, None, 0, 0, None, 0, None), "fb")
+    with pytest.raises(ValueError, match="density_normal"):          # one normal per level, noise or not
+        mp.forward_backward(model, rays, torch.rand(8, 3, device=DEV), True, True,
+                            density_normal=[torch.randn(8, 128, device=DEV)])
     small = mp.MipNerf(num_samples=64, num_levels=1).to(DEV)          # other shapes train too (fp32 path)
     out = mp.forward_backward(small, rays, torch.rand(8, 3, device=DEV), False, True)
     assert torch.isfinite(out["loss"]) and all(torch.isfinite(p.grad).all() for p in small.parameters())
