@@ -685,8 +685,9 @@ int mlp_backward_chain(const mipnerf_b200_config* c, const Dims& d, const mipner
     const mipnerf_b200_linear& l = w->linears[idx];
     if (tc && mipnerf::wgrad_tc_shape_ok(l.out_features)) {  // tensor-core partials + same reduction
       int slices = 0;
-      cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy, 0, l.out_features, x1, 0, k1, k1, x2, 0, k2, k2, div,
-                                                         s.part, m, mipnerf::kWgradMaxSlices, precision, &slices, st);
+      cudaError_t e2 = mipnerf::launch_wgrad_mn_partials({dy, l.out_features}, l.out_features, {x1, k1}, k1, {x2, k2},
+                                                         k2, div, s.part, m, mipnerf::kWgradMaxSlices, precision,
+                                                         &slices, st);
       if (e2 != cudaSuccess) return e2;
       e2 = mipnerf::launch_wgrad_reduce(s.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
                                         grads[idx].bias_grad, touched[idx] ? 1 : 0, st, inv_gscale);
@@ -837,84 +838,72 @@ int tile_backward_chain(const mipnerf_b200_config* cfg, const Dims& d, const mip
   const int64_t m = o.tiles * 128;
   const mipnerf_b200_linear& dl = w->linears[depth];
   const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
-  // bf16x3: the lo image behind a hi image of `bytes_per_tile` bytes per tile (null in the 16-bit step)
-  auto lo_img = [&](const uint8_t* hi, size_t bytes_per_tile) {
-    return x3 ? const_cast<uint8_t*>(hi) + (size_t)o.tiles * bytes_per_tile : nullptr;
-  };
   // MIPNERF_B200_TRAIN_MASKBITS=0: the dgrad GEMMs read the ReLU mask from the activation tile images again (A/B)
   const char* bits_env = getenv("MIPNERF_B200_TRAIN_MASKBITS");
   const bool use_bits = !(bits_env && bits_env[0] == '0');
-  // dy16_lo / x1_lo / x2_lo: bf16x3's lo images (null otherwise)
-  auto wgrad = [&](int idx, const void* dy16, const void* x1, int k1, const void* x2, int x2_t16, int k2, int div,
-                   bool emit_mask, const void* dy16_lo, const void* x1_lo, const void* x2_lo) {
+  auto wgrad = [&](int idx, mipnerf::T16 dy, mipnerf::T16 x1, int k1, const mipnerf::WgradOperand& x2, int k2, int div,
+                   bool emit_mask) {
     const mipnerf_b200_linear& l = w->linears[idx];
     int slices = 0;
-    cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy16, 1, l.out_features, x1, 1, k1, k1, x2, x2_t16, k2, k2, div,
-                                                       o.part, m, mipnerf::kWgradMaxSlices, fmt, &slices, st,
-                                                       emit_mask && use_bits ? o.relu_bits : nullptr, dy16_lo, x1_lo,
-                                                       x2_lo);
+    cudaError_t e2 = mipnerf::launch_wgrad_mn_partials(dy, l.out_features, x1, k1, x2, k2, div, o.part, m,
+                                                       mipnerf::kWgradMaxSlices, fmt, &slices, st,
+                                                       emit_mask && use_bits ? o.relu_bits : nullptr);
     if (e2 != cudaSuccess) return e2;
     e2 = mipnerf::launch_wgrad_reduce(o.part, slices, l.out_features, k1 + k2, grads[idx].weight_grad,
                                       grads[idx].bias_grad, touched[idx] ? 1 : 0, st, inv_gscale);
     touched[idx] = true;
     return e2;
   };
-  // y = [mask] (x . B^T + r1 r1w) on tile images, in bf16x3 on the hi / lo pairs
+  // y = [mask] (x . B^T + r1 r1w) on tile images
   // (act: the layer input whose ReLU masks the output, read as the sign bits the preceding wgrad left behind, or
   // null for no mask; image_mask: read it from the activation tile itself)
-  auto dgrad = [&](const uint8_t* xi, int slot, uint8_t* y, int nn, int kk, const float* r1, const float* r1w,
+  auto dgrad = [&](mipnerf::T16 x, int slot, mipnerf::T16Out y, int nn, int kk, const float* r1, const float* r1w,
                    const uint8_t* act_in, bool image_mask = false) {
     const bool bits_ok = use_bits && !image_mask;
     const void* mask = act_in && !bits_ok ? act_in : nullptr;
     const void* bits = act_in && bits_ok ? o.relu_bits : nullptr;
-    if (x3)
-      return mipnerf::launch_linear_t16_x3(xi, lo_img(xi, (size_t)kk * 256), im.bwd[slot], im.bwd_lo[slot], y,
-                                           lo_img(y, (size_t)nn * 256), m, nn, kk, r1, r1w, mask, st, bits);
-    return mipnerf::launch_linear_t16(xi, im.bwd[slot], y, m, nn, kk, r1, r1w, mask, fmt, st, bits);
+    return mipnerf::launch_linear_t16(x, {im.bwd[slot], im.bwd_lo[slot]}, y, m, nn, kk, r1, r1w, mask, fmt, st, bits);
   };
-  auto h16 = [&](int i) { return o.act + (size_t)i * o.tiles * 65536; };  // h_0..h_7, 8 = bottleneck
-  auto h16_lo = [&](int i) { return x3 ? h16(9 + i) : nullptr; };
-  const uint8_t* enc16_lo = lo_img(o.enc16, 32768);
+  // h_0..h_7, 8 = bottleneck: the dump is one carve of 9 layers of tiles, in bf16x3 followed by their lo images
+  auto h16 = [&](int i) { return mipnerf::tile_pair(o.act + (size_t)i * o.tiles * 65536, 9 * o.tiles, 256, x3); };
+  const mipnerf::T16 enc16 = mipnerf::tile_pair(o.enc16, o.tiles, 128, x3);
+  const mipnerf::T16 v = mipnerf::tile_pair(o.v, o.tiles, 128, x3);
+  const mipnerf::T16Out d_v = mipnerf::tile_pair(o.d_v, o.tiles, 128, x3);
+  const mipnerf::T16Out d_a = mipnerf::tile_pair(o.d_a, o.tiles, 256, x3);
+  const mipnerf::T16Out d_b = mipnerf::tile_pair(o.d_b, o.tiles, 256, x3);
   if (density_only) {
     CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(o.d_raw_density, 1, h16(depth - 1), W, o.part, grads[depth].weight_grad,
-                                               grads[depth].bias_grad, touched[depth] ? 1 : 0, m, fmt, st, inv_gscale,
-                                               h16_lo(depth - 1)));
+                                               grads[depth].bias_grad, touched[depth] ? 1 : 0, m, fmt, st, inv_gscale));
     touched[depth] = true;
     CUDA_TRY(cudaMemsetAsync(o.d_a, 0, (size_t)o.tiles * 65536 * (x3 ? 2 : 1), st));
-    CUDA_TRY(dgrad(o.d_a, depth, o.d_b, W, W, o.d_raw_density, dl.weight, h16(depth - 1), /*image_mask=*/true));
+    CUDA_TRY(dgrad(d_a, depth, d_b, W, W, o.d_raw_density, dl.weight, h16(depth - 1).hi, /*image_mask=*/true));
   } else {
     // colour head, view layer                                          (models/mip_nerf.py:106-110)
-    CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(o.d_raw_rgb, 3, o.v, Wc, o.part, grads[d.n_lin - 1].weight_grad,
+    CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(o.d_raw_rgb, 3, v, Wc, o.part, grads[d.n_lin - 1].weight_grad,
                                                grads[d.n_lin - 1].bias_grad, touched[d.n_lin - 1] ? 1 : 0, m, fmt, st,
-                                               inv_gscale, lo_img(o.v, 32768)));
+                                               inv_gscale));
     touched[d.n_lin - 1] = true;
-    CUDA_TRY(mipnerf::launch_color_dgrad_t16(o.d_raw_rgb, cl.weight, o.v, o.d_v, m, Wc, fmt, st, lo_img(o.d_v, 32768)));
-    CUDA_TRY(wgrad(depth + 2, o.d_v, h16(8), W, o.venc, 0, d.view_dim, o.view_div, false, lo_img(o.d_v, 32768),
-                   h16_lo(8), nullptr));
-    CUDA_TRY(dgrad(o.d_v, depth + 1, o.d_a, W, Wc, nullptr, nullptr, nullptr));
+    CUDA_TRY(mipnerf::launch_color_dgrad_t16(o.d_raw_rgb, cl.weight, o.v, d_v, m, Wc, fmt, st));
+    CUDA_TRY(wgrad(depth + 2, d_v, h16(8), W, {o.venc, d.view_dim}, d.view_dim, o.view_div, false));
+    CUDA_TRY(dgrad(d_v, depth + 1, d_a, W, Wc, nullptr, nullptr, nullptr));
     // bottleneck + density head share h_7                              (models/mip_nerf.py:98-101)
-    CUDA_TRY(wgrad(depth + 1, o.d_a, h16(depth - 1), W, nullptr, 0, 0, 1, /*emit_mask=*/true, lo_img(o.d_a, 65536),
-                   h16_lo(depth - 1), nullptr));  // sign mask of h_7
+    CUDA_TRY(wgrad(depth + 1, d_a, h16(depth - 1), W, {}, 0, 1, /*emit_mask=*/true));  // sign mask of h_7
     CUDA_TRY(mipnerf::launch_wgrad_small_n_t16(o.d_raw_density, 1, h16(depth - 1), W, o.part, grads[depth].weight_grad,
-                                               grads[depth].bias_grad, touched[depth] ? 1 : 0, m, fmt, st, inv_gscale,
-                                               h16_lo(depth - 1)));
+                                               grads[depth].bias_grad, touched[depth] ? 1 : 0, m, fmt, st, inv_gscale));
     touched[depth] = true;
-    CUDA_TRY(dgrad(o.d_a, depth, o.d_b, W, W, o.d_raw_density, dl.weight, h16(depth - 1)));
+    CUDA_TRY(dgrad(d_a, depth, d_b, W, W, o.d_raw_density, dl.weight, h16(depth - 1).hi));
   }
   // trunk                                                            (models/mip_nerf.py:93-97)
-  uint8_t *cur = o.d_b, *other = o.d_a;
+  mipnerf::T16Out cur = d_b, other = d_a;
   for (int i = depth - 1; i >= 0; --i) {
     const bool skip = takes_skip(cfg, i);
     if (i == 0)
-      CUDA_TRY(wgrad(0, cur, o.enc16, d.xyz_dim, nullptr, 0, 0, 1, false, lo_img(cur, 65536), enc16_lo, nullptr));
+      CUDA_TRY(wgrad(0, cur, enc16, d.xyz_dim, {}, 0, 1, false));
     else
-      CUDA_TRY(wgrad(i, cur, h16(i - 1), W, skip ? o.enc16 : nullptr, 1, skip ? d.xyz_dim : 0, 1, true,
-                     lo_img(cur, 65536), h16_lo(i - 1), skip ? enc16_lo : nullptr));
+      CUDA_TRY(wgrad(i, cur, h16(i - 1), W, skip ? enc16 : mipnerf::T16{}, skip ? d.xyz_dim : 0, 1, true));
     if (i > 0) {  // the wgrad just streamed h_{i-1} and left its sign mask behind: 32 B per row instead of 512
-      CUDA_TRY(dgrad(cur, i, other, W, W, nullptr, nullptr, h16(i - 1)));
-      uint8_t* tmp = cur;
-      cur = other;
-      other = tmp;
+      CUDA_TRY(dgrad(cur, i, other, W, W, nullptr, nullptr, h16(i - 1).hi));
+      std::swap(cur, other);
     }
   }
   return MIPNERF_B200_OK;
@@ -947,10 +936,6 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
     const int64_t cnt = (B - off) < chunk ? (B - off) : chunk;
     const mipnerf_b200_rays rc_ = offset_rays(*rays, off, cnt);
     const FusedScratch s = carve_fused(cfg, d, cnt, precision, workspace);
-    // bf16x3: the lo image behind a hi image of `bytes_per_ray` bytes per ray (null in the 16-bit step)
-    auto lo_img = [&](const uint8_t* hi, size_t bytes_per_ray) {
-      return x3 ? const_cast<uint8_t*>(hi) + (size_t)cnt * bytes_per_ray : nullptr;
-    };
     CUDA_TRY(mipnerf::launch_pos_enc(rc_.viewdirs, s.venc, cnt, 0, cfg->deg_view, 1, st));
     // ---- forward of all levels: two launches, everything the backward needs is left behind as tile images
     mipnerf_b200_level_out lo[2];
@@ -966,8 +951,9 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
       const float* t_cur = lo[l].t_samples;
       // the IPE features again (operand of two wgrads; the level kernel keeps its own 16-bit copy on chip), written
       // straight into a tile image so that those wgrads stage them by bulk copy like every other operand
-      CUDA_TRY(mipnerf::launch_ipe_t16(rc_.origins, rc_.directions, rc_.radii, t_cur, s.enc16, cnt, n,
-                                       cfg->disable_integration, fmt, st, lo_img(s.enc16, 32768)));
+      CUDA_TRY(mipnerf::launch_ipe_t16(rc_.origins, rc_.directions, rc_.radii, t_cur,
+                                       mipnerf::tile_pair(s.enc16, cnt, 128, x3), cnt, n, cfg->disable_integration,
+                                       fmt, st));
       CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb[l], s.raw_density[l], t_cur, rc_.directions,
                                   white_bkgd, rgb_scale, gscale, s.d_raw_rgb, s.d_raw_density, st));
       const TileChainOps ops{s.act[l], s.v[l], s.enc16, s.venc, n, s.d_raw_rgb, s.d_raw_density,
@@ -1171,7 +1157,7 @@ int mipnerf_b200_wgrad_tc(const float* dy, int n, const float* x1, int k1, const
   if (!scratch || scratch_bytes < need) return fail(MIPNERF_B200_EWORKSPACE, "scratch %zu < %zu bytes", scratch_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
   int slices = 0;
-  CUDA_TRY(mipnerf::launch_wgrad_mn_partials(dy, 0, n, x1, 0, k1, k1, k2 > 0 ? x2 : nullptr, 0, k2, k2, x2_row_div,
+  CUDA_TRY(mipnerf::launch_wgrad_mn_partials({dy, n}, n, {x1, k1}, k1, {k2 > 0 ? x2 : nullptr, k2}, k2, x2_row_div,
                                              static_cast<float*>(scratch), m, mipnerf::kWgradMaxSlices, precision,
                                              &slices, st));
   CUDA_TRY(mipnerf::launch_wgrad_reduce(static_cast<float*>(scratch), slices, n, k1 + k2, dw, db, 0, st));
@@ -1197,21 +1183,21 @@ int mipnerf_b200_linear_x3(const float* x, const float* weight, const float* r1,
   if (!scratch || scratch_bytes < need) return fail(MIPNERF_B200_EWORKSPACE, "scratch %zu < %zu bytes", scratch_bytes, need);
   if (m == 0) return MIPNERF_B200_OK;
   cudaStream_t st = (cudaStream_t)stream;
+  const int64_t tiles = (m + 127) / 128, mp = tiles * 128;  // the images are whole 128-row tiles (zero rows past m)
   uint8_t* base = static_cast<uint8_t*>(scratch);
-  const size_t xi = mipnerf::t16_image_bytes(m, k), yi = mipnerf::t16_image_bytes(m, n);
-  uint8_t *xh = base, *yh = base + t16_pair(m, k), *mk = yh + t16_pair(m, n);
-  uint8_t* img = mk + align_up(yi);
+  const mipnerf::T16Out xh = mipnerf::tile_pair(base, tiles, k, true);
+  const mipnerf::T16Out yh = mipnerf::tile_pair(base + t16_pair(m, k), tiles, n, true);
+  uint8_t* mk = yh.hi + t16_pair(m, n);
+  uint8_t* img = mk + align_up(mipnerf::t16_image_bytes(m, n));
   const size_t ib = mipnerf::linear_tc_image_bytes(n, k);
-  const int64_t mp = (m + 127) / 128 * 128;  // the images are whole 128-row tiles (zero rows past m)
-  CUDA_TRY(mipnerf::launch_t16_pack(x, k, k, m, xh, MIPNERF_B200_BF16, st, xh + xi));
+  CUDA_TRY(mipnerf::launch_t16_pack(x, k, k, m, xh, MIPNERF_B200_BF16, st));
   if (mask) CUDA_TRY(mipnerf::launch_t16_pack(mask, n, n, m, mk, MIPNERF_B200_BF16, st));
   CUDA_TRY(mipnerf::launch_pack_linear_image(weight, k, 0, 0, img, n, k, MIPNERF_B200_BF16, st));
   CUDA_TRY(mipnerf::launch_pack_linear_image(weight, k, 0, 0, img + ib, n, k, MIPNERF_B200_BF16, st, 1));
-  const float* r1p = r1;
   if (r1 && mp != m) return fail(MIPNERF_B200_EINVAL, "linear_x3: r1 needs m a multiple of 128");
-  CUDA_TRY(mipnerf::launch_linear_t16_x3(xh, xh + xi, img, img + ib, yh, yh + yi, mp, n, k, r1p, r1w,
-                                         mask ? mk : nullptr, st));
-  CUDA_TRY(mipnerf::launch_t16_unpack(yh, n, y, n, m, MIPNERF_B200_BF16, st, yh + yi));
+  CUDA_TRY(mipnerf::launch_linear_t16(xh, {img, img + ib}, yh, mp, n, k, r1, r1w, mask ? mk : nullptr,
+                                      MIPNERF_B200_BF16, st));
+  CUDA_TRY(mipnerf::launch_t16_unpack(yh, n, y, n, m, MIPNERF_B200_BF16, st));
   return MIPNERF_B200_OK;
 }
 
@@ -1232,25 +1218,24 @@ int mipnerf_b200_wgrad_x3(const float* dy, int n, const float* x1, int k1, const
   const size_t need = mipnerf_b200_wgrad_x3_scratch_bytes(m, n, k1, k2, x2_row_div);
   if (!scratch || scratch_bytes < need) return fail(MIPNERF_B200_EWORKSPACE, "scratch %zu < %zu bytes", scratch_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
+  const int64_t tiles = (m + 127) / 128, mp = tiles * 128;  // zero rows past m add nothing
   uint8_t* base = static_cast<uint8_t*>(scratch);
   float* part = reinterpret_cast<float*>(base);
-  uint8_t* dyh = base + align_up(mipnerf_b200_wgrad_tc_scratch_bytes(n, k1 + k2));
-  uint8_t* x1h = dyh + t16_pair(m, n);
-  uint8_t* x2h = x1h + t16_pair(m, k1);
-  const int64_t mp = (m + 127) / 128 * 128;  // zero rows past m add nothing
+  const mipnerf::T16Out dyh =
+      mipnerf::tile_pair(base + align_up(mipnerf_b200_wgrad_tc_scratch_bytes(n, k1 + k2)), tiles, n, true);
+  const mipnerf::T16Out x1h = mipnerf::tile_pair(dyh.hi + t16_pair(m, n), tiles, k1, true);
+  const mipnerf::T16Out x2h = mipnerf::tile_pair(x1h.hi + t16_pair(m, k1), tiles, k2, true);
   const bool x2_img = k2 > 0 && x2_row_div == 1;
   if (x2_row_div > 1 && mp != m) return fail(MIPNERF_B200_EINVAL, "wgrad_x3: x2_row_div > 1 needs m a multiple of 128");
-  CUDA_TRY(mipnerf::launch_t16_pack(dy, n, n, m, dyh, MIPNERF_B200_BF16, st, dyh + mipnerf::t16_image_bytes(m, n)));
-  CUDA_TRY(mipnerf::launch_t16_pack(x1, k1, k1, m, x1h, MIPNERF_B200_BF16, st, x1h + mipnerf::t16_image_bytes(m, k1)));
-  if (x2_img)
-    CUDA_TRY(mipnerf::launch_t16_pack(x2, k2, k2, m, x2h, MIPNERF_B200_BF16, st, x2h + mipnerf::t16_image_bytes(m, k2)));
+  CUDA_TRY(mipnerf::launch_t16_pack(dy, n, n, m, dyh, MIPNERF_B200_BF16, st));
+  CUDA_TRY(mipnerf::launch_t16_pack(x1, k1, k1, m, x1h, MIPNERF_B200_BF16, st));
+  if (x2_img) CUDA_TRY(mipnerf::launch_t16_pack(x2, k2, k2, m, x2h, MIPNERF_B200_BF16, st));
   int slices = 0;
   if (mp > 0) {
-    CUDA_TRY(mipnerf::launch_wgrad_mn_partials(
-        dyh, 1, n, x1h, 1, k1, k1, k2 > 0 ? (x2_img ? (const void*)x2h : (const void*)x2) : nullptr, x2_img ? 1 : 0, k2,
-        k2, x2_row_div, part, mp, mipnerf::kWgradMaxSlices, MIPNERF_B200_BF16, &slices, st, nullptr,
-        dyh + mipnerf::t16_image_bytes(m, n), x1h + mipnerf::t16_image_bytes(m, k1),
-        x2_img ? x2h + mipnerf::t16_image_bytes(m, k2) : nullptr));
+    const mipnerf::WgradOperand x2op = x2_img ? mipnerf::WgradOperand(x2h) : mipnerf::WgradOperand(x2, k2);
+    CUDA_TRY(mipnerf::launch_wgrad_mn_partials(dyh, n, x1h, k1, k2 > 0 ? x2op : mipnerf::WgradOperand(), k2,
+                                               x2_row_div, part, mp, mipnerf::kWgradMaxSlices, MIPNERF_B200_BF16,
+                                               &slices, st));
     CUDA_TRY(mipnerf::launch_wgrad_reduce(part, slices, n, k1 + k2, dw, db, 0, st));
   } else {
     CUDA_TRY(cudaMemsetAsync(dw, 0, sizeof(float) * n * (k1 + k2), st));

@@ -86,7 +86,7 @@ cudaError_t launch_linear_f32(const float* x1, int ld1, int k1, const float* x2,
 
 // ---- train_kernels.cu (fp32 training step: backward + Adam) ----
 constexpr int kWgradMaxSlices = 160;
-int wgrad_num_slices(int64_t m, int tiles);
+int wgrad_num_slices(int64_t m, int tiles, int sms);
 cudaError_t launch_render_backward(const float* raw_rgb, const float* raw_dens, const float* t, const float* dirs,
                                    const float* target, const float* lossmult, const float* mask_sum,
                                    float mse_mult, float dist_mult, int white_bkgd, float density_bias,
@@ -137,6 +137,25 @@ struct AdamMulti {  // passed by value in the kernel parameters
 cudaError_t launch_adam_multi(const AdamMulti& t, float c1, float beta2, float c2, float eps, float step_size,
                               float bc2_sqrt, float grad_scale, cudaStream_t st);
 
+// A 16-bit tile image (train_t16.cu's layout below) and, in bf16x3, its lo image of the same shape; lo null: a plain
+// 16-bit image.  Byte is const uint8_t for an operand (T16) and uint8_t for an output (T16Out), which converts to T16.
+template <typename Byte>
+struct TileImage {
+  Byte* hi = nullptr;
+  Byte* lo = nullptr;
+  TileImage(Byte* hi = nullptr, Byte* lo = nullptr) : hi(hi), lo(lo) {}
+  template <typename B>
+  TileImage(const TileImage<B>& o) : hi(o.hi), lo(o.lo) {}
+};
+using T16 = TileImage<const uint8_t>;
+using T16Out = TileImage<uint8_t>;
+// The pair of a carve of `tiles` tiles of `cols` columns at hi, laid out as hi, then lo `tiles` tiles further on
+// (split false: the plain image at hi).
+template <typename Byte>
+TileImage<Byte> tile_pair(Byte* hi, int64_t tiles, int cols, bool split) {
+  return {hi, split ? hi + (size_t)tiles * ((cols + 63) / 64) * 16384 : nullptr};
+}
+
 // ---- linear_tc.cu (wgmma linear layer for the training step's forward / dgrad GEMMs) ----
 size_t linear_tc_image_bytes(int n, int k);
 bool linear_tc_shape_ok(int n, int k);
@@ -151,44 +170,55 @@ cudaError_t launch_linear_tc(const float* x, int ldx, const void* image, float* 
                              cudaStream_t st);
 
 bool wgrad_tc_shape_ok(int n_dim);
-cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, const void* x1, int x1_t16, int ld1, int k1,
-                                     const void* x2, int x2_t16, int ld2, int k2, int x2_row_div, float* part,
-                                     int64_t m, int max_slices, int precision, int* slices_out, cudaStream_t st,
-                                     void* mask_out = nullptr, const void* dy_lo = nullptr,
-                                     const void* x1_lo = nullptr, const void* x2_lo = nullptr);
+// One operand of launch_wgrad_mn_partials: an fp32 row-major matrix with leading dimension ld, or a tile image (pair)
+// whose rows are its k columns.  The default operand is absent.
+struct WgradOperand {
+  const float* f32 = nullptr;
+  int ld = 0;
+  T16 image;
+  WgradOperand() = default;
+  WgradOperand(const float* p, int ld) : f32(p), ld(ld) {}
+  template <typename Byte>
+  WgradOperand(TileImage<Byte> image) : image(image) {}
+  bool is_image() const { return image.hi != nullptr; }
+  bool absent() const { return !f32 && !is_image(); }
+};
+// Wgrad partials only; the caller runs the fixed-order reduction (launch_wgrad_reduce) afterwards with the slice count
+// returned in *slices_out.  dy (an fp32 dy: ld == n_dim, 16-byte aligned) and x1 are required, x2 (k2 columns) may be
+// absent.  Tile-image operands need m a multiple of 128, and x2 as an image x2_row_div == 1.  No k tile may straddle
+// x1 and x2: k2 > 0 needs k1 % 256 == 0.  bf16x3: dy and x1 are pairs, and so is x2 if it is an image.
+cudaError_t launch_wgrad_mn_partials(const WgradOperand& dy, int n_dim, const WgradOperand& x1, int k1,
+                                     const WgradOperand& x2, int k2, int x2_row_div, float* part, int64_t m,
+                                     int max_slices, int precision, int* slices_out, cudaStream_t st,
+                                     void* mask_out = nullptr);
 // fixed-order reduction of [slices, n_dim, k_dim + 1] partials into dW / db (train_kernels.cu)
 cudaError_t launch_wgrad_reduce(const float* part, int slices, int n_dim, int k_dim, float* dw, float* db,
                                 int accumulate, cudaStream_t st, float scale = 1.f);
 
 // ---- train_t16.cu (backward pass on 16-bit tile images: [tile = 128 rows][64-column slab][128 rows x 128 B, SW128]) ----
-// The split (bf16x3) backward carries every operand as two such images, hi = fl16(x) and lo = fl16(x - hi): the `*_lo`
-// arguments below (null: the 16-bit path; non-null: bf16x3, precision must be 1 = bf16).
+// The split (bf16x3) backward carries every operand as two such images, hi = fl16(x) and lo = fl16(x - hi): the
+// TileImage pairs below (lo null: the 16-bit path; lo given: bf16x3, and precision must be bf16).
 size_t t16_image_bytes(int64_t rows, int cols);
-cudaError_t launch_t16_pack(const float* src, int ld, int cols, int64_t m, void* image, int precision, cudaStream_t st,
-                            void* image_lo = nullptr);
-cudaError_t launch_ipe_t16(const float* origins, const float* directions, const float* radii, const float* t, void* image,
-                           int64_t num_rays, int n, int disable_integration, int precision, cudaStream_t st,
-                           void* image_lo = nullptr);
+cudaError_t launch_t16_pack(const float* src, int ld, int cols, int64_t m, T16Out image, int precision,
+                            cudaStream_t st);
+cudaError_t launch_ipe_t16(const float* origins, const float* directions, const float* radii, const float* t,
+                           T16Out image, int64_t num_rays, int n, int disable_integration, int precision,
+                           cudaStream_t st);
 // the IPE of query points [num_points, 3] (covs null: zero) as a tile image, whole tiles (rows past num_points: the IPE
 // of a zero Gaussian), with the query modes' ipe_pair<false>
 cudaError_t launch_ipe_points_t16(const float* means, const float* covs, void* image, int64_t num_points,
                                   int disable_integration, int precision, cudaStream_t st);
-// image_lo: dst = hi + lo
-cudaError_t launch_t16_unpack(const void* image, int cols, float* dst, int ld, int64_t m, int precision,
-                              cudaStream_t st, const void* image_lo = nullptr);
-// mask: a tile image like y (zero where mask <= 0), or mask_bits: [m][32 B] sign bits of a 256-column image
-// (wgrad_mn_kernel's by-product); at most one of them
-cudaError_t launch_linear_t16(const void* x, const void* image, void* y, int64_t m, int n, int k, const float* r1,
-                              const float* r1w, const void* mask, int precision, cudaStream_t st,
-                              const void* mask_bits = nullptr);
-cudaError_t launch_linear_t16_x3(const void* x, const void* x_lo, const void* image, const void* image_lo, void* y,
-                                 void* y_lo, int64_t m, int n, int k, const float* r1, const float* r1w,
-                                 const void* mask, cudaStream_t st, const void* mask_bits = nullptr);
-cudaError_t launch_color_dgrad_t16(const float* d_rgb, const float* wc, const void* v, void* d_v, int64_t m, int k_dim,
-                                   int precision, cudaStream_t st, void* d_v_lo = nullptr);
-cudaError_t launch_wgrad_small_n_t16(const float* dy, int n_dim, const void* x, int k_dim, float* part, float* dw,
-                                     float* db, int accumulate, int64_t m, int precision, cudaStream_t st,
-                                     float scale = 1.f, const void* x_lo = nullptr);
+// a pair: dst = hi + lo
+cudaError_t launch_t16_unpack(T16 image, int cols, float* dst, int ld, int64_t m, int precision, cudaStream_t st);
+// y = [mask > 0] * (x . B^T + r1 * r1w), B the weight image (launch_pack_linear_image).  mask: a tile image like y
+// (zero where mask <= 0), or mask_bits: [m][32 B] sign bits of a 256-column image (wgrad_mn_kernel's by-product); at
+// most one of them.  bf16x3 (x.lo given): x, the weight image and y are pairs.
+cudaError_t launch_linear_t16(T16 x, T16 image, T16Out y, int64_t m, int n, int k, const float* r1, const float* r1w,
+                              const void* mask, int precision, cudaStream_t st, const void* mask_bits = nullptr);
+cudaError_t launch_color_dgrad_t16(const float* d_rgb, const float* wc, const void* v, T16Out d_v, int64_t m, int k_dim,
+                                   int precision, cudaStream_t st);
+cudaError_t launch_wgrad_small_n_t16(const float* dy, int n_dim, T16 x, int k_dim, float* part, float* dw, float* db,
+                                     int accumulate, int64_t m, int precision, cudaStream_t st, float scale = 1.f);
 
 // ---- mlp_tc.cu ----
 // out[ray][n] = b[n] + W[n, in_main : in_main + view_dim] . venc[ray]   (view-direction part of the view layer)

@@ -12,6 +12,7 @@
 //     register accumulators straight to global memory:  + bias[col]  + row_bias[row / row_div][col]  + prev[row][col]
 //     + r1[row]*r1w[col], ReLU, ReLU-mask by another activation (dgrad).
 #include "kernels.h"
+#include "mlp_tc.h"
 #include "profile.h"
 #include "tc_common.cuh"
 
@@ -506,9 +507,6 @@ __global__ void __launch_bounds__(288, 1) wgrad_mn_kernel(const WgradTcParams p)
   }
 }
 
-int g_sms = 0;
-bool g_attr[2] = {false, false};
-
 }  // namespace
 
 size_t linear_tc_image_bytes(int n, int k) { return (size_t)((k + 63) / 64) * n * 128; }
@@ -519,76 +517,63 @@ cudaError_t launch_pack_linear_image(const float* w, int ldw, int off, int trans
                                      int precision, cudaStream_t st, int lo) {
   const int total = n * ((k + 63) / 64) * 64;
   LaunchScope scope(kKernPackWeights, st);
-  if (precision == 1)
-    pack_linear_image_kernel<1><<<(total + 255) / 256, 256, 0, st>>>(w, ldw, off, transposed, (uint8_t*)image, n, k, lo);
-  else
-    pack_linear_image_kernel<0><<<(total + 255) / 256, 256, 0, st>>>(w, ldw, off, transposed, (uint8_t*)image, n, k, lo);
-  return cudaGetLastError();
+  return with_fmt(precision, false, [&](auto fmt, auto) {
+    pack_linear_image_kernel<fmt><<<(total + 255) / 256, 256, 0, st>>>(w, ldw, off, transposed, (uint8_t*)image, n, k,
+                                                                       lo);
+    return cudaGetLastError();
+  });
 }
 
-// precision: 1 = bf16, 2 = fp16 (MIPNERF_B200_BF16 / _FP16)
+// precision: MIPNERF_B200_BF16 / _FP16
 cudaError_t launch_linear_tc(const float* x, int ldx, const void* image, float* y, int ldy, int64_t m, int n, int k,
                              const float* bias, const float* row_bias, int row_div, const float* prev,
                              const float* r1, const float* r1w, const float* mask, int relu, int precision,
                              cudaStream_t st) {
   if (m == 0) return cudaSuccess;
   if (!linear_tc_shape_ok(n, k) || ldx % 4 != 0 || ldy % 4 != 0) return cudaErrorInvalidValue;
+  int sms = 0;
+  cudaError_t e = num_sms(&sms);
+  if (e != cudaSuccess) return e;
   const int slabs = (k + 63) / 64;
   const size_t smem = 1024 + (size_t)slabs * 16384 + linear_tc_image_bytes(n, k) + 64;
-  const int fmt = precision == 1 ? 1 : 0;
-  if (!g_attr[fmt]) {
-    cudaError_t e = fmt ? cudaFuncSetAttribute(linear_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               200 * 1024)
-                        : cudaFuncSetAttribute(linear_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               200 * 1024);
-    if (e != cudaSuccess) return e;
-    g_attr[fmt] = true;
-  }
-  if (g_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
   LinearTcParams p{};
   p.x = x, p.ldx = ldx, p.image = static_cast<const uint8_t*>(image), p.y = y, p.ldy = ldy, p.m = m, p.n = n, p.k = k;
   p.bias = bias, p.row_bias = row_bias, p.row_div = row_div < 1 ? 1 : row_div, p.prev = prev;
   p.r1 = r1, p.r1w = r1w, p.mask = mask, p.relu = relu;
   const int64_t tiles = (m + 127) / 128;
-  const int grid = (int)(tiles < g_sms ? tiles : g_sms);
-  LaunchScope scope(kKernLinearTc, st);
-  if (fmt) linear_tc_kernel<1><<<grid, 256, smem, st>>>(p);
-  else linear_tc_kernel<0><<<grid, 256, smem, st>>>(p);
-  return cudaGetLastError();
+  const int grid = (int)(tiles < sms ? tiles : sms);
+  return with_fmt(precision, false, [&](auto fmt, auto) {
+    cudaError_t e = allow_smem<linear_tc_kernel<fmt>>(200 * 1024);
+    if (e != cudaSuccess) return e;
+    LaunchScope scope(kKernLinearTc, st);
+    linear_tc_kernel<fmt><<<grid, 256, smem, st>>>(p);
+    return cudaGetLastError();
+  });
 }
 
 bool wgrad_tc_shape_ok(int n_dim) { return n_dim == 128 || n_dim == 256; }
 
-// Wgrad partials only; the caller runs the fixed-order reduction (train_kernels.cu) afterwards with the slice count
-// returned in *slices_out.  dy / x1 / x2 are fp32 row-major matrices (an fp32 dy 16-byte aligned), or (*_t16 != 0)
-// 16-bit tile images (then m must be a multiple of 128 and x1 has k1 / 64 slabs per tile).  No k tile may straddle
-// x1 and x2: k2 > 0 needs k1 % 256 == 0.
-cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, const void* x1, int x1_t16, int ld1, int k1,
-                                     const void* x2, int x2_t16, int ld2, int k2, int x2_row_div, float* part,
-                                     int64_t m, int max_slices, int precision, int* slices_out, cudaStream_t st,
-                                     void* mask_out, const void* dy_lo, const void* x1_lo, const void* x2_lo) {
-  // bf16x3 (dy_lo given): dy and x1 are tile images with their lo images, x2 an image with its lo image or fp32
-  const bool x3 = dy_lo != nullptr;
-  if (x3 && (precision != 1 || !dy_t16 || !x1_t16 || !x1_lo || (x2 && x2_t16 && k2 > 0 && !x2_lo)))
-    return cudaErrorInvalidValue;
-  if (!x2) x2 = x1, x2_t16 = x1_t16, ld2 = ld1, k2 = 0, x2_lo = x1_lo;
+cudaError_t launch_wgrad_mn_partials(const WgradOperand& dy, int n_dim, const WgradOperand& x1, int k1,
+                                     const WgradOperand& x2_in, int k2, int x2_row_div, float* part, int64_t m,
+                                     int max_slices, int precision, int* slices_out, cudaStream_t st,
+                                     void* mask_out) {
+  const WgradOperand& x2 = x2_in.absent() ? x1 : x2_in;  // no x2: x1 again, with no columns
+  if (x2_in.absent()) k2 = 0;
+  // bf16x3 when dy is a pair; then x1 and an image x2 are pairs too, and otherwise no operand has a lo image
+  auto paired = [](const WgradOperand& o) { return o.is_image() && o.image.lo != nullptr; };
+  const bool x3 = paired(dy);
+  if (paired(x1) != x3 || (x2.is_image() && k2 > 0 && paired(x2) != x3)) return cudaErrorInvalidValue;
   if (x2_row_div < 1) x2_row_div = 1;
   const int K = k1 + k2;
   if (!(k2 == 0 || k1 % 256 == 0) || !(n_dim == 128 || n_dim == 256)) return cudaErrorInvalidValue;
-  if ((dy_t16 || x1_t16 || x2_t16) && m % 128 != 0) return cudaErrorInvalidValue;
-  if (x2_t16 && k2 > 0 && x2_row_div != 1) return cudaErrorInvalidValue;
-  if (g_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  const int fmt = precision == 1 ? 1 : 0;
+  if (dy.f32 && dy.ld != n_dim) return cudaErrorInvalidValue;
+  if ((dy.is_image() || x1.is_image() || x2.is_image()) && m % 128 != 0) return cudaErrorInvalidValue;
+  if (x2.is_image() && k2 > 0 && x2_row_div != 1) return cudaErrorInvalidValue;
+  int sms = 0;
+  cudaError_t e = num_sms(&sms);
+  if (e != cudaSuccess) return e;
   const int k_tiles = (K + kWgK - 1) / kWgK;
-  int64_t slices = g_sms / k_tiles;  // one CTA per SM, one wave
+  int64_t slices = sms / k_tiles;  // one CTA per SM, one wave
   const int slab = x3 ? kWgSlabX3 : kWgSlab;
   const int64_t by_rows = (m + slab - 1) / slab;
   if (slices > by_rows) slices = by_rows;
@@ -596,30 +581,23 @@ cudaError_t launch_wgrad_mn_partials(const void* dy, int dy_t16, int n_dim, cons
   if (slices < 1) slices = 1;
   int64_t slice_rows = (m + slices - 1) / slices;
   slice_rows = (slice_rows + slab - 1) / slab * slab;
-  static bool attr[3] = {false, false, false};
   const size_t smem = 1024 + (size_t)kWgStages * kWgStage + 8 * 256 * sizeof(float) + 128;
-  const int variant = x3 ? 2 : fmt;
-  if (!attr[variant]) {
-    cudaError_t e = x3    ? cudaFuncSetAttribute(wgrad_mn_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                    : fmt ? cudaFuncSetAttribute(wgrad_mn_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                          : cudaFuncSetAttribute(wgrad_mn_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    attr[variant] = true;
-  }
+  auto data = [](const WgradOperand& o) { return o.is_image() ? reinterpret_cast<const float*>(o.image.hi) : o.f32; };
   WgradTcParams p{};
-  p.dy = static_cast<const float*>(dy), p.n_dim = n_dim, p.x1 = static_cast<const float*>(x1), p.ld1 = ld1, p.k1 = k1;
-  p.x2 = static_cast<const float*>(x2), p.ld2 = ld2, p.k2 = k2, p.x2_row_div = x2_row_div, p.part = part, p.m = m;
-  p.slice_rows = slice_rows, p.dy_t16 = dy_t16, p.x1_t16 = x1_t16, p.x2_t16 = x2_t16;
-  p.mask_out = (x1_t16 && k1 == 256) ? static_cast<uint8_t*>(mask_out) : nullptr;
-  p.dy_lo = static_cast<const uint8_t*>(dy_lo), p.x1_lo = static_cast<const uint8_t*>(x1_lo);
-  p.x2_lo = static_cast<const uint8_t*>(x2_lo);
-  dim3 grid((unsigned)slices, (unsigned)k_tiles);
-  LaunchScope scope(kKernWgradTc, st);
-  if (x3) wgrad_mn_kernel<1, true><<<grid, 288, smem, st>>>(p);
-  else if (fmt) wgrad_mn_kernel<1><<<grid, 288, smem, st>>>(p);
-  else wgrad_mn_kernel<0><<<grid, 288, smem, st>>>(p);
+  p.dy = data(dy), p.n_dim = n_dim, p.x1 = data(x1), p.ld1 = x1.ld, p.k1 = k1;
+  p.x2 = data(x2), p.ld2 = x2.ld, p.k2 = k2, p.x2_row_div = x2_row_div, p.part = part, p.m = m;
+  p.slice_rows = slice_rows, p.dy_t16 = dy.is_image(), p.x1_t16 = x1.is_image(), p.x2_t16 = x2.is_image();
+  p.mask_out = (x1.is_image() && k1 == 256) ? static_cast<uint8_t*>(mask_out) : nullptr;
+  p.dy_lo = dy.image.lo, p.x1_lo = x1.image.lo, p.x2_lo = x2.image.lo;
+  const dim3 grid((unsigned)slices, (unsigned)k_tiles);
   *slices_out = (int)slices;
-  return cudaGetLastError();
+  return with_fmt(precision, x3, [&](auto fmt, auto split) {
+    cudaError_t e = allow_smem<wgrad_mn_kernel<fmt, split>>((int)smem);
+    if (e != cudaSuccess) return e;
+    LaunchScope scope(kKernWgradTc, st);
+    wgrad_mn_kernel<fmt, split><<<grid, 288, smem, st>>>(p);
+    return cudaGetLastError();
+  });
 }
 
 }  // namespace mipnerf

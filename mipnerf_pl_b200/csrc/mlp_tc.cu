@@ -1670,7 +1670,6 @@ __global__ void pack_view_dir_kernel(const float* __restrict__ w, const float* _
 // stream wait for the previous user's kernels (on another stream) before overwriting the bank, and records an event
 // after this call's launches.  Same-stream callers (the normal case) pay one event record.  During stream capture the
 // cross-stream wait is skipped (a capture is single-stream by construction and the event lives outside the graph).
-constexpr int kMaxDevices = 64;
 struct SmallBankState {
   cudaEvent_t done = nullptr;
   cudaStream_t last = nullptr;
@@ -1733,34 +1732,20 @@ TcScratch carve_tc(int64_t rays, int n, void* base) {
   return s;
 }
 
-int g_num_sms = 0;
-
-int num_sms() {
-  if (g_num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return g_num_sms;
-}
-
 template <int kFmt, bool kX3, int kT, int kMode = kModeForward, bool kTrain = false, bool kQueryDump = false>
 cudaError_t launch_level_t(const LevelParams& p, cudaStream_t st) {
-  auto kern = mlp_level_kernel<kFmt, kX3, kT, kMode, kTrain, kQueryDump>;
+  constexpr auto kern = mlp_level_kernel<kFmt, kX3, kT, kMode, kTrain, kQueryDump>;
   constexpr uint32_t smem = LevelLayout<kX3, kT>::kTotal;
-  static bool attr_set = false;  // one flag per instantiation
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  num_sms();
+  cudaError_t e = allow_smem<kern>((int)smem);
+  if (e != cudaSuccess) return e;
+  int sms = 0;
+  if ((e = num_sms(&sms)) != cudaSuccess) return e;
   LaunchScope scope(kMode == kModeDensity    ? kKernDensityTc
                     : kMode == kModeRadiance ? kKernRadianceTc
                     : kMode == kModeViewAcc  ? kKernRadianceDirsTc
                                              : (p.feat_in ? kKernMlpTc : kKernMlpLevelTc),
                     st);
-  const int grid = (int)(p.num_rays < g_num_sms ? p.num_rays : g_num_sms);
+  const int grid = (int)(p.num_rays < sms ? p.num_rays : sms);
   kern<<<grid, kThreads, smem, st>>>(p);
   return cudaGetLastError();
 }
@@ -1800,11 +1785,14 @@ LevelParams query_params(const mipnerf_b200_config* c, const uint8_t* img, const
 }
 
 // radiance mode: the view-direction slots [ctas][2][128][128] fp32, one pair per CTA of a launch of min(tiles, SMs)
+// (0 without a device)
 constexpr size_t kRadianceSlotBytes = 2 * (size_t)kN * kCond * sizeof(float);
 int64_t radiance_ctas(int64_t num_points) {
   const int64_t tiles = (num_points + kN - 1) / kN, chunk = kDensityChunkPoints / kN;
   const int64_t t = tiles < chunk ? tiles : chunk;
-  return t < num_sms() ? t : num_sms();
+  int sms = 0;
+  num_sms(&sms);
+  return t < sms ? t : sms;
 }
 
 }  // namespace

@@ -4,6 +4,9 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <atomic>
+#include <type_traits>
+
 #include "../../include/mipnerf_b200.h"
 #include "draws.h"
 
@@ -18,6 +21,46 @@ inline int fmt_of(int precision) {
   return (precision == MIPNERF_B200_BF16 || precision == MIPNERF_B200_BF16X3) ? MIPNERF_B200_BF16 : MIPNERF_B200_FP16;
 }
 inline bool is_x3(int precision) { return precision == MIPNERF_B200_FP16X3 || precision == MIPNERF_B200_BF16X3; }
+
+// Calls f(fmt, split) with the kernels' template arguments kFmt (1: bf16, 0: fp16, the format fmt_of(precision)) and
+// kX3 = split as std::integral_constants, and returns what f returns.  The split (x3) variants of the launchers'
+// kernels exist in bf16 only: split with fp16 is refused before f runs.
+template <typename F>
+cudaError_t with_fmt(int precision, bool split, F&& f) {
+  using Bf16 = std::integral_constant<int, 1>;
+  if (fmt_of(precision) == MIPNERF_B200_BF16) return split ? f(Bf16{}, std::true_type{}) : f(Bf16{}, std::false_type{});
+  return split ? cudaErrorInvalidValue : f(std::integral_constant<int, 0>{}, std::false_type{});
+}
+
+// Devices with host state of their own (the caches below query a device past them every time).
+constexpr int kMaxDevices = 64;
+
+// The current device's SM count, queried once per device; *sms = 0 if the query fails.
+inline cudaError_t num_sms(int* sms) {
+  static std::atomic<int> cache[kMaxDevices];
+  int dev = 0, n = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess && dev < kMaxDevices) n = cache[dev].load(std::memory_order_relaxed);
+  if (e == cudaSuccess && n == 0) e = cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  if (e != cudaSuccess) n = 0;
+  else if (dev < kMaxDevices) cache[dev].store(n, std::memory_order_relaxed);
+  *sms = n;
+  return e;
+}
+
+// Lets kKernel (one kernel instantiation) take `bytes` of dynamic shared memory on the current device, once per
+// device.  Two threads racing here both set the same attribute, which is harmless.
+template <auto kKernel>
+cudaError_t allow_smem(int bytes) {
+  static std::atomic<bool> done[kMaxDevices];
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < kMaxDevices && done[dev].load(std::memory_order_relaxed)) return cudaSuccess;
+  e = cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess && dev < kMaxDevices) done[dev].store(true, std::memory_order_relaxed);
+  return e;
+}
 
 inline size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
 

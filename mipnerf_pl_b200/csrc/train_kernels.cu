@@ -17,6 +17,7 @@
 //   wgrad_reduce_kernel      fixed-order sum of the partials into dW / db (deterministic, optional accumulate)
 //   adam_kernel              torch.optim.Adam single-tensor update, one thread per element
 #include "kernels.h"
+#include "mlp_tc.h"
 #include "profile.h"
 #include "ray_math.cuh"
 #include "sgemm_tile.cuh"
@@ -544,20 +545,14 @@ wgrad_reduce_kernel(const float* __restrict__ part, int slices, int n_dim, int k
   }
 }
 
-// Number of M-slices for a wgrad with `tiles` output tiles.  Small problems: one slice per 4096 rows.  Large ones:
-// fill whole waves of the grid (2 CTAs per SM resident) so the last wave is not mostly empty — 4 tiles x 74 slices
-// is exactly one wave of 296 CTAs on 148 SMs, where the old fixed 128 slices left the second wave 27 % full.
-int wgrad_num_slices(int64_t m, int tiles) {
+// Number of M-slices for a wgrad with `tiles` output tiles on `sms` SMs.  Small problems: one slice per 4096 rows.
+// Large ones: fill whole waves of the grid (2 CTAs per SM resident) so the last wave is not mostly empty — 4 tiles x
+// 66 slices is exactly one wave of 264 CTAs on the H100's 132 SMs.
+int wgrad_num_slices(int64_t m, int tiles, int sms) {
   int64_t s = (m + 4095) / 4096;
   if (s < 1) s = 1;
   if (s > kWgradMaxSlices) s = kWgradMaxSlices;
-  static int resident = 0;
-  if (resident == 0) {
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    resident = 2 * sms;
-  }
+  const int resident = 2 * sms;
   if (tiles < 1) tiles = 1;
   if (s * tiles > resident) {  // more than one wave anyway: round the slice count to whole waves
     const int64_t waves = (s * tiles + resident - 1) / resident;
@@ -601,8 +596,11 @@ cudaError_t launch_wgrad_f32(const float* dy, int n_dim, const float* x1, int ld
                                                                                  accumulate, scale);
     return cudaGetLastError();
   }
+  int sms = 0;
+  cudaError_t e = num_sms(&sms);
+  if (e != cudaSuccess) return e;
   const int tiles = ((n_dim + 127) / 128) * ((K + 127) / 128);
-  const int slices = wgrad_num_slices(m, tiles);
+  const int slices = wgrad_num_slices(m, tiles, sms);
   int64_t slice_rows = (m + slices - 1) / slices;
   slice_rows = (slice_rows + 15) / 16 * 16;
   LaunchScope scope(kKernWgrad, st);
@@ -611,7 +609,7 @@ cudaError_t launch_wgrad_f32(const float* dy, int n_dim, const float* x1, int ld
   const int vec_b = aligned16(x1) && ld1 % 4 == 0;
   wgrad_f32_kernel<<<grid, kTileThreads, 0, st>>>(dy, n_dim, x1, ld1, k1, x2, ld2, k2, x2_row_div, part, m, slice_rows,
                                                   vec_a, vec_b);
-  cudaError_t e = cudaGetLastError();
+  e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   wgrad_reduce_kernel<<<blocks_of((int64_t)n_dim * (K + 1), 64), 256, 0, st>>>(part, slices, n_dim, K, dw, db,
                                                                                accumulate, scale);

@@ -10,6 +10,7 @@
 //   t16_pack / t16_unpack fp32 row-major <-> tile image (tests, stand-alone entry points)
 // The wgrad GEMMs on tile images are in linear_tc.cu (wgrad_mn_kernel: a row-major tile IS an MN-major operand).
 #include "kernels.h"
+#include "mlp_tc.h"
 #include "profile.h"
 #include "ray_math.cuh"
 #include "tc_common.cuh"
@@ -552,7 +553,6 @@ __global__ void t16_unpack_kernel(const uint8_t* __restrict__ src, int img_cols,
   dst[row * ld + col] = v;
 }
 
-int g_sms_t16 = 0;
 inline unsigned blocks_of(int64_t n, int per_block) { return (unsigned)((n + per_block - 1) / per_block); }
 
 }  // namespace
@@ -561,40 +561,34 @@ size_t t16_image_bytes(int64_t rows, int cols) {
   return (size_t)((rows + 127) / 128) * (size_t)((cols + 63) / 64) * kSlab;
 }
 
-cudaError_t launch_t16_pack(const float* src, int ld, int cols, int64_t m, void* image, int precision,
-                            cudaStream_t st, void* image_lo) {
+cudaError_t launch_t16_pack(const float* src, int ld, int cols, int64_t m, T16Out image, int precision,
+                            cudaStream_t st) {
   const int img_cols = (cols + 63) / 64 * 64;
   const int64_t padded = (m + 127) / 128 * 128;
   if (padded == 0) return cudaSuccess;
   LaunchScope scope(kKernIpe, st);  // accounted with the feature kernels (its use in the training step)
   const int vec = (ld & 3) == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
   const int64_t total = padded * (img_cols / 8);
-  uint8_t* lo = static_cast<uint8_t*>(image_lo);
-  if (precision == 1)
-    t16_pack_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(src, ld, cols, m, (uint8_t*)image, img_cols, padded, vec, lo);
-  else
-    t16_pack_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(src, ld, cols, m, (uint8_t*)image, img_cols, padded, vec, lo);
-  return cudaGetLastError();
+  return with_fmt(precision, false, [&](auto fmt, auto) {
+    t16_pack_kernel<fmt><<<blocks_of(total, 256), 256, 0, st>>>(src, ld, cols, m, image.hi, img_cols, padded, vec,
+                                                                 image.lo);
+    return cudaGetLastError();
+  });
 }
 
 // min_deg = 0, max_deg = 16 (96 features), n = 128 samples per ray: the level kernels' shape
-cudaError_t launch_ipe_t16(const float* origins, const float* directions, const float* radii, const float* t, void* image,
-                           int64_t num_rays, int n, int disable_integration, int precision, cudaStream_t st,
-                           void* image_lo) {
+cudaError_t launch_ipe_t16(const float* origins, const float* directions, const float* radii, const float* t,
+                           T16Out image, int64_t num_rays, int n, int disable_integration, int precision,
+                           cudaStream_t st) {
   if (num_rays == 0) return cudaSuccess;
-  if (n != 128 || (image_lo && precision != 1)) return cudaErrorInvalidValue;
-  LaunchScope scope(kKernIpe, st);
+  if (n != 128) return cudaErrorInvalidValue;
   const int64_t total = num_rays * n * 8;
-  if (image_lo)
-    ipe_t16_kernel<1, true><<<blocks_of(total, 256), 256, 0, st>>>(origins, directions, radii, t, (uint8_t*)image,
-                                                                    num_rays, n, disable_integration, (uint8_t*)image_lo);
-  else if (precision == 1)
-    ipe_t16_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(origins, directions, radii, t, (uint8_t*)image, num_rays, n,
-                                                              disable_integration);
-  else
-    ipe_t16_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(origins, directions, radii, t, (uint8_t*)image, num_rays, n,
-                                                              disable_integration);
-  return cudaGetLastError();
+  return with_fmt(precision, image.lo != nullptr, [&](auto fmt, auto split) {
+    LaunchScope scope(kKernIpe, st);
+    ipe_t16_kernel<fmt, split><<<blocks_of(total, 256), 256, 0, st>>>(origins, directions, radii, t, image.hi, num_rays,
+                                                                       n, disable_integration, image.lo);
+    return cudaGetLastError();
+  });
 }
 
 cudaError_t launch_ipe_points_t16(const float* means, const float* covs, void* image, int64_t num_points,
@@ -603,143 +597,98 @@ cudaError_t launch_ipe_points_t16(const float* means, const float* covs, void* i
   if (padded == 0) return cudaSuccess;
   LaunchScope scope(kKernIpe, st);
   const int64_t total = padded * 8;
-  if (precision == 1)
-    ipe_points_t16_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(means, covs, (uint8_t*)image, num_points, padded,
-                                                                     disable_integration);
-  else
-    ipe_points_t16_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(means, covs, (uint8_t*)image, num_points, padded,
-                                                                     disable_integration);
-  return cudaGetLastError();
+  return with_fmt(precision, false, [&](auto fmt, auto) {
+    ipe_points_t16_kernel<fmt><<<blocks_of(total, 256), 256, 0, st>>>(means, covs, (uint8_t*)image, num_points, padded,
+                                                                       disable_integration);
+    return cudaGetLastError();
+  });
 }
 
-cudaError_t launch_t16_unpack(const void* image, int cols, float* dst, int ld, int64_t m, int precision,
-                              cudaStream_t st, const void* image_lo) {
+cudaError_t launch_t16_unpack(T16 image, int cols, float* dst, int ld, int64_t m, int precision, cudaStream_t st) {
   const int img_cols = (cols + 63) / 64 * 64;
   if (m == 0) return cudaSuccess;
-  const uint8_t* lo = static_cast<const uint8_t*>(image_lo);
-  if (precision == 1)
-    t16_unpack_kernel<1><<<blocks_of(m * cols, 256), 256, 0, st>>>((const uint8_t*)image, img_cols, dst, ld, cols, m, lo);
-  else
-    t16_unpack_kernel<0><<<blocks_of(m * cols, 256), 256, 0, st>>>((const uint8_t*)image, img_cols, dst, ld, cols, m, lo);
-  return cudaGetLastError();
+  return with_fmt(precision, false, [&](auto fmt, auto) {
+    t16_unpack_kernel<fmt><<<blocks_of(m * cols, 256), 256, 0, st>>>(image.hi, img_cols, dst, ld, cols, m, image.lo);
+    return cudaGetLastError();
+  });
 }
 
-// y = [mask > 0] * (x . B^T + r1 * r1w) on tile images; m rows (a multiple of 128), n in {128, 256}, k in {128, 256}
-cudaError_t launch_linear_t16(const void* x, const void* image, void* y, int64_t m, int n, int k, const float* r1,
-                              const float* r1w, const void* mask, int precision, cudaStream_t st,
-                              const void* mask_bits) {
+// m rows (a multiple of 128), n in {128, 256}, k in {128, 256}
+cudaError_t launch_linear_t16(T16 x, T16 image, T16Out y, int64_t m, int n, int k, const float* r1, const float* r1w,
+                              const void* mask, int precision, cudaStream_t st, const void* mask_bits) {
   if (m == 0) return cudaSuccess;
   if (m % 128 != 0 || !(n == 128 || n == 256) || !(k == 128 || k == 256)) return cudaErrorInvalidValue;
   if (mask_bits && (mask || n != 256)) return cudaErrorInvalidValue;
-  const int slabs = k / 64;
-  const size_t smem = 1024 + (size_t)slabs * kSlab + linear_tc_image_bytes(n, k) + 128;
-  const int fmt = precision == 1 ? 1 : 0;
-  static bool attr[2] = {false, false};
-  if (!attr[fmt]) {
-    cudaError_t e = fmt ? cudaFuncSetAttribute(linear_t16_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)
-                        : cudaFuncSetAttribute(linear_t16_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e != cudaSuccess) return e;
-    attr[fmt] = true;
-  }
-  if (g_sms_t16 == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sms_t16, cudaDevAttrMultiProcessorCount, dev);
-  }
-  LinearT16Params p{};
-  p.x = static_cast<const uint8_t*>(x), p.image = static_cast<const uint8_t*>(image), p.y = static_cast<uint8_t*>(y);
-  p.mask_bits = static_cast<const uint8_t*>(mask_bits);
-  p.mask = static_cast<const uint8_t*>(mask), p.r1 = r1, p.r1w = r1w, p.tiles = m / 128, p.n = n, p.k = k;
-  const int grid = (int)(p.tiles < g_sms_t16 ? p.tiles : g_sms_t16);
-  LaunchScope scope(kKernLinearTc, st);
-  if (fmt) linear_t16_kernel<1><<<grid, 256, smem, st>>>(p);
-  else linear_t16_kernel<0><<<grid, 256, smem, st>>>(p);
-  return cudaGetLastError();
-}
-
-// the same in bf16x3: x, B and y as hi and lo images (linear_t16_x3_kernel)
-cudaError_t launch_linear_t16_x3(const void* x, const void* x_lo, const void* image, const void* image_lo, void* y,
-                                 void* y_lo, int64_t m, int n, int k, const float* r1, const float* r1w,
-                                 const void* mask, cudaStream_t st, const void* mask_bits) {
-  if (m == 0) return cudaSuccess;
-  if (m % 128 != 0 || !(n == 128 || n == 256) || !(k == 128 || k == 256)) return cudaErrorInvalidValue;
-  if (mask_bits && (mask || n != 256)) return cudaErrorInvalidValue;
+  if (!x.lo != !image.lo || !x.lo != !y.lo) return cudaErrorInvalidValue;  // bf16x3: all three are pairs
+  int sms = 0;
+  cudaError_t e = num_sms(&sms);
+  if (e != cudaSuccess) return e;
   const int slabs = k / 64, halves = n / 128;
-  const size_t smem = 1024 + (size_t)(2 * slabs + 4) * kSlab + 64;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(linear_t16_x3_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)(1024 + (size_t)(2 * 4 + 4) * kSlab + 64));
-    if (e != cudaSuccess) return e;
-    attr = true;
-  }
-  if (g_sms_t16 == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sms_t16, cudaDevAttrMultiProcessorCount, dev);
-  }
-  LinearT16X3Params q{};
-  LinearT16Params& p = q.hi;
-  p.x = static_cast<const uint8_t*>(x), p.image = static_cast<const uint8_t*>(image), p.y = static_cast<uint8_t*>(y);
+  LinearT16Params p{};
+  p.x = x.hi, p.image = image.hi, p.y = y.hi;
   p.mask_bits = static_cast<const uint8_t*>(mask_bits);
   p.mask = static_cast<const uint8_t*>(mask), p.r1 = r1, p.r1w = r1w, p.tiles = m / 128, p.n = n, p.k = k;
-  q.x_lo = static_cast<const uint8_t*>(x_lo), q.image_lo = static_cast<const uint8_t*>(image_lo);
-  q.y_lo = static_cast<uint8_t*>(y_lo);
-  // a CTA keeps one N-half for good: the grid is a whole number of CTAs per half
-  const int64_t per_half = p.tiles < g_sms_t16 / halves ? p.tiles : g_sms_t16 / halves;
-  LaunchScope scope(kKernLinearTc, st);
-  linear_t16_x3_kernel<1><<<(unsigned)(per_half * halves), 288, smem, st>>>(q);
-  return cudaGetLastError();
+  if (!x.lo)
+    return with_fmt(precision, false, [&](auto fmt, auto) {
+      const size_t smem = 1024 + (size_t)slabs * kSlab + linear_tc_image_bytes(n, k) + 128;
+      cudaError_t e = allow_smem<linear_t16_kernel<fmt>>(200 * 1024);
+      if (e != cudaSuccess) return e;
+      const int grid = (int)(p.tiles < sms ? p.tiles : sms);
+      LaunchScope scope(kKernLinearTc, st);
+      linear_t16_kernel<fmt><<<grid, 256, smem, st>>>(p);
+      return cudaGetLastError();
+    });
+  return with_fmt(precision, true, [&](auto fmt, auto split) {  // bf16x3: linear_t16_x3_kernel
+    if constexpr (split) {
+      const size_t smem = 1024 + (size_t)(2 * slabs + 4) * kSlab + 64;
+      cudaError_t e = allow_smem<linear_t16_x3_kernel<fmt>>((int)(1024 + (size_t)(2 * 4 + 4) * kSlab + 64));
+      if (e != cudaSuccess) return e;
+      const LinearT16X3Params q{p, x.lo, image.lo, y.lo};
+      // a CTA keeps one N-half for good: the grid is a whole number of CTAs per half
+      const int64_t per_half = p.tiles < sms / halves ? p.tiles : sms / halves;
+      LaunchScope scope(kKernLinearTc, st);
+      linear_t16_x3_kernel<fmt><<<(unsigned)(per_half * halves), 288, smem, st>>>(q);
+    }
+    return cudaGetLastError();
+  });
 }
 
-cudaError_t launch_color_dgrad_t16(const float* d_rgb, const float* wc, const void* v, void* d_v, int64_t m, int k_dim,
-                                   int precision, cudaStream_t st, void* d_v_lo) {
+cudaError_t launch_color_dgrad_t16(const float* d_rgb, const float* wc, const void* v, T16Out d_v, int64_t m, int k_dim,
+                                   int precision, cudaStream_t st) {
   if (m == 0) return cudaSuccess;
-  if (k_dim % 64 != 0 || (d_v_lo && precision != 1)) return cudaErrorInvalidValue;
-  LaunchScope scope(kKernDgrad, st);
+  if (k_dim % 64 != 0) return cudaErrorInvalidValue;
   const int64_t total = m * (k_dim / 8);
-  if (d_v_lo)
-    color_dgrad_t16_kernel<1, true><<<blocks_of(total, 256), 256, 0, st>>>(d_rgb, wc, (const uint8_t*)v, (uint8_t*)d_v, m,
-                                                                          k_dim, (uint8_t*)d_v_lo);
-  else if (precision == 1)
-    color_dgrad_t16_kernel<1><<<blocks_of(total, 256), 256, 0, st>>>(d_rgb, wc, (const uint8_t*)v, (uint8_t*)d_v, m, k_dim);
-  else
-    color_dgrad_t16_kernel<0><<<blocks_of(total, 256), 256, 0, st>>>(d_rgb, wc, (const uint8_t*)v, (uint8_t*)d_v, m, k_dim);
-  return cudaGetLastError();
+  return with_fmt(precision, d_v.lo != nullptr, [&](auto fmt, auto split) {
+    LaunchScope scope(kKernDgrad, st);
+    color_dgrad_t16_kernel<fmt, split><<<blocks_of(total, 256), 256, 0, st>>>(d_rgb, wc, (const uint8_t*)v, d_v.hi, m,
+                                                                               k_dim, d_v.lo);
+    return cudaGetLastError();
+  });
 }
 
 // narrow heads: dW[n_dim, k_dim] and db from dy (fp32 [m, n_dim], n_dim = 1 or 3) and a tile-image X; partials +
 // fixed-order sum
-cudaError_t launch_wgrad_small_n_t16(const float* dy, int n_dim, const void* x, int k_dim, float* part, float* dw,
-                                     float* db, int accumulate, int64_t m, int precision, cudaStream_t st,
-                                     float scale, const void* x_lo) {
+cudaError_t launch_wgrad_small_n_t16(const float* dy, int n_dim, T16 x, int k_dim, float* part, float* dw, float* db,
+                                     int accumulate, int64_t m, int precision, cudaStream_t st, float scale) {
   if (m == 0 || n_dim == 0) return cudaSuccess;
   if (!(n_dim == 1 || n_dim == 3) || !(k_dim == 128 || k_dim == 256)) return cudaErrorInvalidValue;
-  if (x_lo && precision != 1) return cudaErrorInvalidValue;
-  if (g_sms_t16 == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_sms_t16, cudaDevAttrMultiProcessorCount, dev);
-  }
-  int64_t want = 4 * (int64_t)g_sms_t16;  // four resident blocks per SM, one wave
+  int sms = 0;
+  cudaError_t e = num_sms(&sms);
+  if (e != cudaSuccess) return e;
+  int64_t want = 4 * (int64_t)sms;  // four resident blocks per SM, one wave
   if (want > (m + 63) / 64) want = (m + 63) / 64;
   if (want < 1) want = 1;
   const int slices = (int)want;
   const int64_t rows = (m + slices - 1) / slices;
-  const uint8_t* x8 = static_cast<const uint8_t*>(x);
-  {
+  e = with_fmt(precision, x.lo != nullptr, [&](auto fmt, auto split) {
     LaunchScope scope(kKernWgrad, st);
-    const int fmt = precision == 1 ? 1 : 0;
-    const uint8_t* xl = static_cast<const uint8_t*>(x_lo);
-    if (xl && n_dim == 1) wgrad_small_n_t16_kernel<1, 1, true><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows, xl);
-    else if (xl) wgrad_small_n_t16_kernel<1, 3, true><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows, xl);
-    else if (fmt && n_dim == 1) wgrad_small_n_t16_kernel<1, 1><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);
-    else if (fmt) wgrad_small_n_t16_kernel<1, 3><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);
-    else if (n_dim == 1) wgrad_small_n_t16_kernel<0, 1><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);
-    else wgrad_small_n_t16_kernel<0, 3><<<slices, 256, 0, st>>>(dy, x8, k_dim, part, m, rows);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-  }
+    if (n_dim == 1)
+      wgrad_small_n_t16_kernel<fmt, 1, split><<<slices, 256, 0, st>>>(dy, x.hi, k_dim, part, m, rows, x.lo);
+    else
+      wgrad_small_n_t16_kernel<fmt, 3, split><<<slices, 256, 0, st>>>(dy, x.hi, k_dim, part, m, rows, x.lo);
+    return cudaGetLastError();
+  });
+  if (e != cudaSuccess) return e;
   return launch_wgrad_reduce(part, slices, n_dim, k_dim, dw, db, accumulate, st, scale);
 }
 
