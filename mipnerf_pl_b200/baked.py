@@ -28,7 +28,7 @@ import torch
 
 from . import _cabi
 from .field import DEFAULT_BOUNDS, Resolution, _resolution, bake_sh, density_grid, lattice_axes, voxel_variance
-from .ops import _dev, _f32, _rays_struct, _stream
+from .ops import _call, _dev, _f32, _rays_struct
 from .rays import BLENDER_CAMERA_ANGLE_X, Rays
 from .render import gather_rows, generate_rays, shard_rows
 
@@ -189,10 +189,8 @@ class BakedGrid:
         dist = torch.empty(n, device=dev)
         acc = torch.empty(n, device=dev)
         st = self.default_step() if step is None else float(step)
-        with torch.cuda.device(dev):
-            _cabi.check(_cabi.lib().mipnerf_b200_grid_render(C.byref(g), C.byref(rs), st, int(bool(white_bkgd)),
-                                                             rgb.data_ptr(), dist.data_ptr(), acc.data_ptr(),
-                                                             _stream(dev)), "grid_render")
+        _call(dev, "grid_render", _cabi.lib().mipnerf_b200_grid_render, C.byref(g), C.byref(rs), st,
+              int(bool(white_bkgd)), rgb.data_ptr(), dist.data_ptr(), acc.data_ptr())
         return rgb, dist, acc
 
     def save(self, path: str) -> None:

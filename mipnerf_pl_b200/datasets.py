@@ -256,16 +256,15 @@ class DeviceRayBank:
     def rays(self, pixel_ids: torch.Tensor) -> Tuple[Rays, torch.Tensor]:
         """pixel_ids: int64 [B] atlas rows (image-major, then row-major pixels) -> (Rays [B,*], rgb [B,3])."""
         from . import _cabi
-        from .ops import _stream
+        from .ops import _call
         ids = pixel_ids.to(device=self.device, dtype=torch.int64).contiguous()
         b = ids.numel()
         mk = lambda c: torch.empty(b, c, device=self.device)  # noqa: E731
         o, d, v, rad, lm, nr, fr, rgb = mk(3), mk(3), mk(3), mk(1), mk(1), mk(1), mk(1), mk(3)
-        with torch.cuda.device(self.device):
-            _cabi.check(_cabi.lib().mipnerf_b200_rays_from_pixels(
-                self.cam_table.data_ptr(), self.offsets.data_ptr(), self.widths.data_ptr(), self.num_images,
-                ids.data_ptr(), b, self.atlas.data_ptr(), o.data_ptr(), d.data_ptr(), v.data_ptr(), rad.data_ptr(),
-                lm.data_ptr(), nr.data_ptr(), fr.data_ptr(), rgb.data_ptr(), _stream(self.device)), "rays_from_pixels")
+        _call(self.device, "rays_from_pixels", _cabi.lib().mipnerf_b200_rays_from_pixels, self.cam_table.data_ptr(),
+              self.offsets.data_ptr(), self.widths.data_ptr(), self.num_images, ids.data_ptr(), b,
+              self.atlas.data_ptr(), o.data_ptr(), d.data_ptr(), v.data_ptr(), rad.data_ptr(), lm.data_ptr(),
+              nr.data_ptr(), fr.data_ptr(), rgb.data_ptr())
         return Rays(o, d, v, rad, lm, nr, fr), rgb
 
     def sample(self, batch_size: int, generator: Optional[torch.Generator] = None) -> Tuple[Rays, torch.Tensor]:

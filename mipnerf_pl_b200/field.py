@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .ops import _dev, _f32, _stream
+from .ops import _call, _dev, _f32
 
 DEFAULT_BOUNDS = ((-1.5, -1.5, -1.5), (1.5, 1.5, 1.5))
 Resolution = Union[int, Sequence[int]]
@@ -93,22 +93,18 @@ def isosurface(grid: torch.Tensor, iso: float, bounds=DEFAULT_BOUNDS, normals: b
     counts = torch.empty(2, dtype=torch.int64, device=dev)
     lo = (C.c_float * 3)(*[float(v) for v in bounds[0]])
     hi = (C.c_float * 3)(*[float(v) for v in bounds[1]])
-    with torch.cuda.device(dev):
-        st = _stream(dev)
-        _cabi.check(lib.mipnerf_b200_isosurface_count(g.data_ptr(), nx, ny, nz, float(iso), scratch.data_ptr(), nbytes,
-                                                      counts.data_ptr(), st), "isosurface")
-        nv, nf = (int(v) for v in counts.tolist())
-        verts = torch.empty(nv, 3, device=dev)
-        faces = torch.empty(nf, 3, dtype=torch.int32, device=dev)
-        _cabi.check(lib.mipnerf_b200_isosurface_emit(g.data_ptr(), nx, ny, nz, lo, hi, float(iso), scratch.data_ptr(),
-                                                     verts.data_ptr() if nv else None,
-                                                     faces.data_ptr() if nf else None, st), "isosurface")
-        if not normals:
-            return verts, faces
-        nrm = torch.empty(nv, 3, device=dev)
-        _cabi.check(lib.mipnerf_b200_isosurface_normals(g.data_ptr(), nx, ny, nz, lo, hi, float(iso),
-                                                        scratch.data_ptr(), nrm.data_ptr() if nv else None, st),
-                    "isosurface")
+    _call(dev, "isosurface", lib.mipnerf_b200_isosurface_count, g.data_ptr(), nx, ny, nz, float(iso),
+          scratch.data_ptr(), nbytes, counts.data_ptr())
+    nv, nf = (int(v) for v in counts.tolist())
+    verts = torch.empty(nv, 3, device=dev)
+    faces = torch.empty(nf, 3, dtype=torch.int32, device=dev)
+    _call(dev, "isosurface", lib.mipnerf_b200_isosurface_emit, g.data_ptr(), nx, ny, nz, lo, hi, float(iso),
+          scratch.data_ptr(), verts.data_ptr() if nv else None, faces.data_ptr() if nf else None)
+    if not normals:
+        return verts, faces
+    nrm = torch.empty(nv, 3, device=dev)
+    _call(dev, "isosurface", lib.mipnerf_b200_isosurface_normals, g.data_ptr(), nx, ny, nz, lo, hi, float(iso),
+          scratch.data_ptr(), nrm.data_ptr() if nv else None)
     return verts, faces, nrm
 
 

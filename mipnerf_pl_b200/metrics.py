@@ -18,7 +18,7 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .ops import _dev, _f32, _stream
+from .ops import _call, _dev, _f32
 from .rays import spheric_pose
 
 
@@ -37,9 +37,8 @@ def eval_errors(pred_color: torch.Tensor, batch_pixels: torch.Tensor):
     nbytes = lib.mipnerf_b200_image_metrics_scratch_bytes(h, w, c)
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     out = torch.empty(3, device=dev)
-    with torch.cuda.device(dev):
-        _cabi.check(lib.mipnerf_b200_image_metrics(p.data_ptr(), t.data_ptr(), h, w, c, scratch.data_ptr(), nbytes,
-                                                   out.data_ptr(), _stream(dev)), "eval_errors")
+    _call(dev, "eval_errors", lib.mipnerf_b200_image_metrics, p.data_ptr(), t.data_ptr(), h, w, c, scratch.data_ptr(),
+          nbytes, out.data_ptr())
     return out[0], out[1]
 
 

@@ -27,7 +27,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _cabi
-from .ops import _dev, _f32, _grad_array, _ptr, _rays_struct, _stream, draw_density_normal, draw_t_rand, draw_u_jitter
+from .ops import _call, _dev, _f32, _grad_array, _ptr, _rays_struct, draw_density_normal, draw_t_rand, draw_u_jitter
 from .rays import Rays
 
 
@@ -91,13 +91,11 @@ class MLP(torch.nn.Module):
             layers.append(torch.nn.Sequential(linear, torch.nn.ReLU(True)))
         self.view_layers = torch.nn.Sequential(*layers)
         self.color_layer = torch.nn.Linear(net_width_condition, num_rgb_channels)
-        self._packed = {}  # precision -> (versions, tensor)
 
     def __getstate__(self):  # ctypes marshalling caches are per-process
         d = self.__dict__.copy()
         d.pop("_ws_cache", None)
         d.pop("_lin_cache", None)
-        d["_packed"] = {}
         return d
 
     # ---- marshalling --------------------------------------------------------------------------
@@ -110,40 +108,43 @@ class MLP(torch.nn.Module):
             self.__dict__["_lin_cache"] = lins
         return lins
 
+    def params(self) -> List[torch.nn.Parameter]:
+        """weight, bias of every layer in `linears()` order: the order of the library's gradient arrays."""
+        return [p for lin in self.linears() for p in (lin.weight, lin.bias)]
+
     def _weights_struct(self, cfg: "_cabi.Config", precision: int, device):
-        """(struct, keep-alive list), cached until a parameter is modified / moved / re-typed."""
+        """(struct, keep-alive list) for `precision` on `device`.  Cached per (precision, device) until a parameter is
+        modified, moved or re-typed; every precision's struct points at the same fp32 parameter tensors, and a
+        tensor-core precision adds its packed weight image."""
         lins = self.linears()
-        key = (precision, str(device), tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version,
-                                               l.weight.dtype) for l in lins))
-        hit = self.__dict__.get("_ws_cache")
-        if hit is not None and hit[0] == key:
-            return hit[1], hit[2]
-        ws, keep = self._weights_struct_uncached(cfg, precision, device, lins)
-        self.__dict__["_ws_cache"] = (key, ws, keep)
-        return ws, keep
+        state = tuple((l.weight.data_ptr(), l.weight._version, l.bias.data_ptr(), l.bias._version, l.weight.dtype)
+                      for l in lins)
+        cache = self.__dict__.get("_ws_cache")
+        if cache is None or cache[0] != state:
+            cache = self.__dict__["_ws_cache"] = (state, {})
+        key = (precision, str(device))
+        hit = cache[1].get(key)
+        if hit is not None:
+            return hit
+        if precision == _cabi.FP32:
+            arr = (_cabi.Linear * len(lins))()
+            keep = []
+            for i, l in enumerate(lins):
+                w, b = _f32(l.weight), _f32(l.bias)
+                if w.device != device:
+                    raise RuntimeError(f"MLP parameters live on {w.device}, rays on {device}")
+                keep += [w, b]
+                arr[i] = _cabi.Linear(w.data_ptr(), b.data_ptr(), l.in_features, l.out_features)
+            hit = (_cabi.Weights(arr, len(lins), -1, None, 0), keep + [arr])
+        else:
+            ws, keep = self._weights_struct(cfg, _cabi.FP32, device)
+            hit = self._packed_image(cfg, ws, precision, device, keep)
+        cache[1][key] = hit
+        return hit
 
-    def _weights_struct_uncached(self, cfg, precision, device, lins):
-        arr = (_cabi.Linear * len(lins))()
-        keep = []
-        for i, l in enumerate(lins):
-            w, b = _f32(l.weight), _f32(l.bias)
-            if w.device != device:
-                raise RuntimeError(f"MLP parameters live on {w.device}, rays on {device}")
-            keep += [w, b]
-            arr[i] = _cabi.Linear(w.data_ptr(), b.data_ptr(), l.in_features, l.out_features)
-        ws = _cabi.Weights(arr, len(lins), -1, None, 0)
-        if precision != _cabi.FP32:
-            packed = self._packed_image(cfg, ws, precision, device, lins)
-            ws.packed, ws.packed_bytes, ws.packed_precision = packed.data_ptr(), packed.numel(), precision
-            keep.append(packed)
-        keep.append(arr)
-        return ws, keep
-
-    def _packed_image(self, cfg, ws, precision, device, lins):
-        versions = tuple((p.data_ptr(), p._version) for l in lins for p in (l.weight, l.bias))
-        hit = self._packed.get((precision, str(device)))
-        if hit is not None and hit[0] == versions:
-            return hit[1]
+    def _packed_image(self, cfg, ws, precision, device, keep):
+        """(struct, keep-alive list) of a tensor-core precision: the fp32 struct `ws` (whose tensors `keep` holds) plus
+        its weight image, packed on `device`."""
         lib = _cabi.lib()
         nbytes = lib.mipnerf_b200_packed_weights_bytes(C.byref(cfg), precision)
         if nbytes == 0:
@@ -151,11 +152,10 @@ class MLP(torch.nn.Module):
                                       "min_deg_point=0, max_deg_point 1..16 and deg_view 1..4 is implemented; "
                                       "use precision='fp32'")
         packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        with torch.cuda.device(device):
-            _cabi.check(lib.mipnerf_b200_pack_weights(C.byref(cfg), C.byref(ws), precision, packed.data_ptr(),
-                                                      nbytes, _stream(device)), "pack_weights")
-        self._packed[(precision, str(device))] = (versions, packed)
-        return packed
+        _call(device, "pack_weights", lib.mipnerf_b200_pack_weights, C.byref(cfg), C.byref(ws), precision,
+              packed.data_ptr(), nbytes)
+        return (_cabi.Weights(ws.linears, ws.num_linears, precision, packed.data_ptr(), packed.numel()),
+                keep + [packed])
 
     def _config(self, num_samples=128, **over) -> "_cabi.Config":
         deg_pts = self.xyz_dim // 6
@@ -184,10 +184,8 @@ class MLP(torch.nn.Module):
         raw_density = torch.empty(b, n, 1, device=dev)
         nbytes = lib.mipnerf_b200_mlp_workspace_bytes(C.byref(cfg), b, n, prec)
         scratch = _Workspace.get(dev, nbytes)
-        with torch.cuda.device(dev):
-            _cabi.check(lib.mipnerf_b200_mlp_forward(
-                C.byref(cfg), C.byref(ws), xx.data_ptr(), _ptr(vd), b, n, prec, raw_rgb.data_ptr(),
-                raw_density.data_ptr(), scratch.data_ptr(), scratch.numel(), _stream(dev)), "MLP.forward")
+        _call(dev, "MLP.forward", lib.mipnerf_b200_mlp_forward, C.byref(cfg), C.byref(ws), xx.data_ptr(), _ptr(vd), b,
+              n, prec, raw_rgb.data_ptr(), raw_density.data_ptr(), scratch.data_ptr(), scratch.numel())
         return raw_rgb, raw_density
 
 
@@ -196,6 +194,51 @@ class LevelOutputs(list):
     `.pixels` — comp_rgb | distance | acc of every level as one contiguous [levels, 5*B] tensor (a view of the same
     memory), for reading rendered pixels back to the host with a single copy."""
     pixels: Optional[torch.Tensor] = None
+
+
+def _level_outputs(b: int, n: int, levels: int, dev, normals, return_inds: bool):
+    """(LevelOutputs, LevelOut array) of a call on b rays with n samples per level, in one allocation: the pixel outputs
+    (comp_rgb | distance | acc = 5 floats per ray) of all levels first, so that a caller that only wants pixels reads
+    them back with ONE contiguous copy (`.pixels`, [levels, 5*B]); then weights / fenceposts per level.  `normals`: the
+    density normals handed to the library, one tensor or None per level."""
+    flat = torch.empty(levels * b * (5 + n + n + 1), device=dev)
+    ret = LevelOutputs()
+    ret.pixels = flat[:levels * 5 * b].view(levels, 5 * b) if b > 0 else flat[:0].view(levels, 0)
+    outs = (_cabi.LevelOut * levels)()
+    tail = levels * 5 * b
+    for lvl in range(levels):
+        o = lvl * 5 * b
+        comp = flat[o:o + 3 * b].view(b, 3)
+        dist = flat[o + 3 * b:o + 4 * b]
+        acc = flat[o + 4 * b:o + 5 * b]
+        q = tail + lvl * (2 * n + 1) * b
+        w = flat[q:q + n * b].view(b, n)
+        t = flat[q + n * b:q + (2 * n + 1) * b].view(b, n + 1)
+        inds = torch.empty(b, n + 1, device=dev, dtype=torch.int64) if (return_inds and lvl > 0) else None
+        outs[lvl] = _cabi.LevelOut(comp.data_ptr(), dist.data_ptr(), acc.data_ptr(), w.data_ptr(), t.data_ptr(),
+                                   _ptr(inds), _ptr(normals[lvl]))
+        ret.append((comp, dist, acc, w, t, inds) if return_inds else (comp, dist, acc, w, t))
+    return ret, outs
+
+
+def _shape(x: Optional[torch.Tensor]):
+    return None if x is None else tuple(x.shape)
+
+
+def _query_points(what: str, means: torch.Tensor, covs: Optional[torch.Tensor], viewdirs: Optional[torch.Tensor] = None,
+                  dirs: Optional[torch.Tensor] = None, table: Optional[torch.Tensor] = None):
+    """Check the arguments of a field query -> (leading shape, means, covs, viewdirs, dirs, table): means / covs /
+    viewdirs flattened to fp32 [P, 3], dirs [D, 3] and table [D, K] fp32 on means' device; None stays None.  Only
+    shapes are checked: a CPU tensor is refused where it is handed to the library."""
+    if means.shape[-1] != 3 or any(x is not None and x.shape != means.shape for x in (covs, viewdirs)):
+        raise ValueError(f"{what}: means {_shape(means)} / covs {_shape(covs)} / viewdirs {_shape(viewdirs)}: need "
+                         "[..., 3] of the same shape")
+    if dirs is not None and (dirs.dim() != 2 or dirs.shape[1] != 3 or dirs.shape[0] < 1):
+        raise ValueError(f"{what}: dirs {_shape(dirs)}: need [D, 3] with D >= 1")
+    if table is not None and (table.dim() != 2 or table.shape[0] != dirs.shape[0] or not 1 <= table.shape[1] <= 16):
+        raise ValueError(f"{what}: table {_shape(table)}: need [D = {dirs.shape[0]}, K] with 1 <= K <= 16")
+    return (means.shape[:-1], *[None if x is None else _f32(x).reshape(-1, 3) for x in (means, covs, viewdirs)],
+            *[None if x is None else _f32(x).to(means.device) for x in (dirs, table)])
 
 
 class MipNerf(torch.nn.Module):
@@ -312,35 +355,29 @@ class MipNerf(torch.nn.Module):
         With `autograd=True`, grad mode on and a parameter that requires grad, the result carries a `grad_fn` over the
         24 MLP tensors (same values: the same launches run); its backward is `mipnerf_b200_query_backward`.  fp32 and
         bf16 (default encodings) only; means / covs that require grad are refused.  Otherwise no grad_fn."""
-        if means.shape[-1] != 3 or (covs is not None and covs.shape != means.shape):
-            raise ValueError(f"means {tuple(means.shape)} / covs {None if covs is None else tuple(covs.shape)}: "
-                             "need [..., 3] of the same shape")
+        shape, m, c = _query_points("query_density", means, covs)[:3]
         if self._builds_graph():
-            return _query_with_grad(self, means, covs, None, raw)
+            return _query_with_grad(self, (means, covs), shape, m, c, None, raw)
         with torch.no_grad():
-            return self._query_density(means, covs, raw)
+            return self._query_density(m, c, raw).reshape(shape)
 
-    def _query_density(self, means: torch.Tensor, covs: Optional[torch.Tensor], raw: bool):
-        dev = _dev(means)
-        shape = means.shape[:-1]
-        m = _f32(means).reshape(-1, 3)
-        c = _f32(covs).reshape(-1, 3) if covs is not None else None
+    def _query_density(self, m: torch.Tensor, c: Optional[torch.Tensor], raw: bool):
+        """The density [P] at the flat fp32 points of `_query_points`."""
+        dev = _dev(m)
         p = m.shape[0]
         prec = _cabi.PRECISIONS[self.precision]
         cfg = self._config()
         ws, keep = self.mlp._weights_struct(cfg, prec, dev)
         out = torch.empty(p, device=dev)
         if p == 0:
-            return out.reshape(shape)
+            return out
         lib = _cabi.lib()
         nbytes = lib.mipnerf_b200_density_workspace_bytes(C.byref(cfg), p, prec)
         scratch = _Workspace.get(dev, nbytes)
-        with torch.cuda.device(dev):
-            _cabi.check(lib.mipnerf_b200_query_density(
-                C.byref(cfg), C.byref(ws), m.data_ptr(), _ptr(c), p, prec,
-                out.data_ptr() if raw else None, None if raw else out.data_ptr(), scratch.data_ptr(), scratch.numel(),
-                _stream(dev)), "MipNerf.query_density")
-        return out.reshape(shape)
+        _call(dev, "MipNerf.query_density", lib.mipnerf_b200_query_density, C.byref(cfg), C.byref(ws), m.data_ptr(),
+              _ptr(c), p, prec, out.data_ptr() if raw else None, None if raw else out.data_ptr(), scratch.data_ptr(),
+              scratch.numel())
+        return out
 
     def query_radiance(self, means: torch.Tensor, covs: Optional[torch.Tensor] = None,
                        viewdirs: Optional[torch.Tensor] = None, *, raw: bool = False):
@@ -351,25 +388,18 @@ class MipNerf(torch.nn.Module):
         unit directions.  They may be None only for a model with use_viewdirs=False (fp32: the colour head then reads
         the trunk).  The tensor-core precisions take the configs `forward` takes on the tensor cores (the radiance mode
         of the level kernel); fp32 any.  Gradients with respect to the MLP tensors as for `query_density`."""
-        if (means.shape[-1] != 3 or (covs is not None and covs.shape != means.shape) or
-                (viewdirs is not None and viewdirs.shape != means.shape)):
-            raise ValueError(f"means {tuple(means.shape)} / covs {None if covs is None else tuple(covs.shape)} / "
-                             f"viewdirs {None if viewdirs is None else tuple(viewdirs.shape)}: need [..., 3] of the "
-                             "same shape")
+        shape, m, c, v = _query_points("query_radiance", means, covs, viewdirs)[:4]
         if viewdirs is None and self.use_viewdirs:
             raise ValueError("query_radiance: viewdirs are required when use_viewdirs=True")
         if self._builds_graph():
-            return _query_with_grad(self, means, covs, viewdirs, raw)
+            return _query_with_grad(self, (means, covs, viewdirs), shape, m, c, v, raw)
         with torch.no_grad():
-            return self._query_radiance(means, covs, viewdirs, raw)
+            rgb, dens = self._query_radiance(m, c, v, raw)
+        return rgb.reshape(*shape, 3), dens.reshape(shape)
 
-    def _query_radiance(self, means: torch.Tensor, covs: Optional[torch.Tensor], viewdirs: Optional[torch.Tensor],
-                        raw: bool):
-        dev = _dev(means)
-        shape = means.shape[:-1]
-        m = _f32(means).reshape(-1, 3)
-        c = _f32(covs).reshape(-1, 3) if covs is not None else None
-        v = _f32(viewdirs).reshape(-1, 3) if viewdirs is not None else None
+    def _query_radiance(self, m: torch.Tensor, c: Optional[torch.Tensor], v: Optional[torch.Tensor], raw: bool):
+        """(rgb [P, 3], density [P]) at the flat fp32 points and view directions of `_query_points`."""
+        dev = _dev(m)
         p = m.shape[0]
         prec = _cabi.PRECISIONS[self.precision]
         cfg = self._config()
@@ -382,11 +412,9 @@ class MipNerf(torch.nn.Module):
             scratch = _Workspace.get(dev, nbytes)
             rgb_ptrs = (out_rgb.data_ptr(), out_dens.data_ptr(), None, None) if raw else \
                 (None, None, out_rgb.data_ptr(), out_dens.data_ptr())
-            with torch.cuda.device(dev):
-                _cabi.check(lib.mipnerf_b200_query_radiance(
-                    C.byref(cfg), C.byref(ws), m.data_ptr(), _ptr(c), _ptr(v), p, prec, *rgb_ptrs,
-                    scratch.data_ptr(), scratch.numel(), _stream(dev)), "MipNerf.query_radiance")
-        return out_rgb.reshape(*shape, 3), out_dens.reshape(shape)
+            _call(dev, "MipNerf.query_radiance", lib.mipnerf_b200_query_radiance, C.byref(cfg), C.byref(ws),
+                  m.data_ptr(), _ptr(c), _ptr(v), p, prec, *rgb_ptrs, scratch.data_ptr(), scratch.numel())
+        return out_rgb, out_dens
 
     def query_radiance_dirs(self, means: torch.Tensor, covs: Optional[torch.Tensor], dirs: torch.Tensor, *,
                             raw: bool = False):
@@ -410,25 +438,14 @@ class MipNerf(torch.nn.Module):
 
     def _query_radiance_dirs(self, means, covs, dirs, table, raw: bool, colors: bool):
         name = "query_radiance_dirs" if colors else "query_radiance_proj"
-        if means.shape[-1] != 3 or (covs is not None and covs.shape != means.shape):
-            raise ValueError(f"{name}: means {tuple(means.shape)} / covs "
-                             f"{None if covs is None else tuple(covs.shape)}: need [..., 3] of the same shape")
-        if dirs.dim() != 2 or dirs.shape[1] != 3 or dirs.shape[0] < 1:
-            raise ValueError(f"{name}: dirs {tuple(dirs.shape)}: need [D, 3] with D >= 1")
-        if table is not None and (table.dim() != 2 or table.shape[0] != dirs.shape[0] or not 1 <= table.shape[1] <= 16):
-            raise ValueError(f"{name}: table {tuple(table.shape)}: need [D = {dirs.shape[0]}, K] with 1 <= K <= 16")
+        shape, m, c, _, dd, tab = _query_points(name, means, covs, None, dirs, table)
         if not self.use_viewdirs:
             raise NotImplementedError(f"{name}: the model has use_viewdirs=False (its colour does not depend on the "
                                       "direction; use query_radiance)")
         if self._builds_graph():
             raise NotImplementedError(f"{name}: no gradients; call it under torch.no_grad() on an autograd model")
         with torch.no_grad():
-            dev = _dev(means)
-            shape = means.shape[:-1]
-            m = _f32(means).reshape(-1, 3)
-            c = _f32(covs).reshape(-1, 3) if covs is not None else None
-            dd = _f32(dirs).to(dev)
-            tab = _f32(table).to(dev) if table is not None else None
+            dev = _dev(m)
             p, nd = m.shape[0], dd.shape[0]
             k = tab.shape[1] if tab is not None else 0
             prec = _cabi.PRECISIONS[self.precision]
@@ -444,12 +461,11 @@ class MipNerf(torch.nn.Module):
                     raise NotImplementedError(f"{name}: precision {self.precision!r} does not take this model")
                 scratch = _Workspace.get(dev, nbytes)
                 rgb_ptr = _ptr(out_rgb)
-                with torch.cuda.device(dev):
-                    _cabi.check(lib.mipnerf_b200_query_radiance_dirs(
-                        C.byref(cfg), C.byref(ws), m.data_ptr(), _ptr(c), p, dd.data_ptr(), nd, prec,
-                        rgb_ptr if raw else None, None if raw else rgb_ptr, out_dens.data_ptr() if raw else None,
-                        None if raw else out_dens.data_ptr(), _ptr(tab), k, int(raw), _ptr(proj),
-                        scratch.data_ptr(), scratch.numel(), _stream(dev)), f"MipNerf.{name}")
+                _call(dev, f"MipNerf.{name}", lib.mipnerf_b200_query_radiance_dirs, C.byref(cfg), C.byref(ws),
+                      m.data_ptr(), _ptr(c), p, dd.data_ptr(), nd, prec, rgb_ptr if raw else None,
+                      None if raw else rgb_ptr, out_dens.data_ptr() if raw else None,
+                      None if raw else out_dens.data_ptr(), _ptr(tab), k, int(raw), _ptr(proj), scratch.data_ptr(),
+                      scratch.numel())
         return (out_rgb.reshape(*shape, nd, 3) if colors else None, out_dens.reshape(shape),
                 proj.reshape(*shape, k, 3) if proj is not None else None)
 
@@ -465,52 +481,22 @@ class MipNerf(torch.nn.Module):
                                "(same failure as the reference)")
         dev = _dev(rays.origins)
         b = rays.origins.shape[0]
-        n = self.num_samples
         prec = _cabi.PRECISIONS[self.precision]
         cfg = self._config()
         rs, keep = _rays_struct(rays.origins, rays.directions, rays.viewdirs, rays.radii, rays.near, rays.far)
         rng, t_rand, u_jitter, normals = self._noise(randomized, b, dev, t_rand, u_jitter, density_normal)
         ws, wkeep = self.mlp._weights_struct(cfg, prec, dev)
-        outs = (_cabi.LevelOut * self.num_levels)()
-        # One allocation for everything: the per-level pixel outputs (comp_rgb | distance | acc = 5 floats/ray) of
-        # all levels first, so that a caller that only wants pixels reads them back with ONE contiguous copy
-        # (`ret.pixels`, [levels, 5*B]); then weights / fenceposts per level.
-        levels = self.num_levels
-        flat = torch.empty(levels * b * (5 + n + n + 1), device=dev)
-        ret = LevelOutputs()
-        ret.pixels = flat[:levels * 5 * b].view(levels, 5 * b) if b > 0 else flat[:0].view(levels, 0)
-        tail = levels * 5 * b
-        for lvl in range(levels):
-            o = lvl * 5 * b
-            comp = flat[o:o + 3 * b].view(b, 3)
-            dist = flat[o + 3 * b:o + 4 * b]
-            acc = flat[o + 4 * b:o + 5 * b]
-            q = tail + lvl * (2 * n + 1) * b
-            w = flat[q:q + n * b].view(b, n)
-            t = flat[q + n * b:q + (2 * n + 1) * b].view(b, n + 1)
-            inds = torch.empty(b, n + 1, device=dev, dtype=torch.int64) if (return_inds and lvl > 0) else None
-            outs[lvl] = _cabi.LevelOut(comp.data_ptr(), dist.data_ptr(), acc.data_ptr(), w.data_ptr(),
-                                       t.data_ptr(), _ptr(inds), _ptr(normals[lvl]))
-            ret.append((comp, dist, acc, w, t, inds) if return_inds else (comp, dist, acc, w, t))
+        ret, outs = _level_outputs(b, self.num_samples, self.num_levels, dev, normals, return_inds)
         lib = _cabi.lib()
-        nbytes = lib.mipnerf_b200_workspace_bytes(C.byref(cfg), b, prec)
-        if nbytes == 0 and b > 0:
-            _cabi.check(lib.mipnerf_b200_forward(C.byref(cfg), C.byref(ws), C.byref(rs), 0, None, None, 0, prec,
-                                                 outs, None, 0, None), "MipNerf.forward")
-        scratch = _Workspace.get(dev, nbytes)
+        # a config the library refuses sizes no workspace; the call below then raises the refusal
+        scratch = _Workspace.get(dev, lib.mipnerf_b200_workspace_bytes(C.byref(cfg), b, prec))
         if rng is not None:
-            fn = lib.mipnerf_b200_forward_rng
-            args = (C.byref(cfg), C.byref(ws), C.byref(rs), C.byref(rng), int(bool(white_bkgd)), prec, outs,
-                    scratch.data_ptr(), scratch.numel(), _stream(dev))
+            _call(dev, "MipNerf.forward", lib.mipnerf_b200_forward_rng, C.byref(cfg), C.byref(ws), C.byref(rs),
+                  C.byref(rng), int(bool(white_bkgd)), prec, outs, scratch.data_ptr(), scratch.numel())
         else:
-            fn = lib.mipnerf_b200_forward
-            args = (C.byref(cfg), C.byref(ws), C.byref(rs), int(bool(randomized)), _ptr(t_rand), _ptr(u_jitter),
-                    int(bool(white_bkgd)), prec, outs, scratch.data_ptr(), scratch.numel(), _stream(dev))
-        if dev.index is None or dev.index == torch.cuda.current_device():
-            _cabi.check(fn(*args), "MipNerf.forward")
-        else:
-            with torch.cuda.device(dev):
-                _cabi.check(fn(*args), "MipNerf.forward")
+            _call(dev, "MipNerf.forward", lib.mipnerf_b200_forward, C.byref(cfg), C.byref(ws), C.byref(rs),
+                  int(bool(randomized)), _ptr(t_rand), _ptr(u_jitter), int(bool(white_bkgd)), prec, outs,
+                  scratch.data_ptr(), scratch.numel())
         return ret, cfg, rng, normals, keep
 
 
@@ -549,9 +535,8 @@ def _forward_with_grad(model: MipNerf, rays: Rays, randomized, white_bkgd, t_ran
     _dev(rays.origins)
     _check_autograd(model, rays, rays.origins.shape[0])
     holder = {}
-    params = [p for lin in model.mlp.linears() for p in (lin.weight, lin.bias)]
     flat = _ForwardWithGrad.apply(model, rays, randomized, white_bkgd, t_rand, u_jitter, density_normal,
-                                  return_inds, holder, *params)
+                                  return_inds, holder, *model.mlp.params())
     per = 6 if return_inds else 5
     ret = LevelOutputs(tuple(flat[i:i + per]) for i in range(0, len(flat), per))
     ret.pixels = holder["pixels"]
@@ -623,12 +608,9 @@ class _ForwardWithGrad(torch.autograd.Function):
         lib = _cabi.lib()
         nbytes = lib.mipnerf_b200_train_workspace_bytes(C.byref(cfg), b)
         scratch = _Workspace.get(dev, nbytes)
-        with torch.cuda.device(dev):
-            _cabi.check(lib.mipnerf_b200_backward(
-                C.byref(cfg), C.byref(ws), C.byref(rs), t_arr, int(ctx.randomized),
-                C.byref(rng) if rng is not None else None, normal_arr, int(ctx.white_bkgd),
-                _cabi.PRECISIONS[ctx.precision], cots, garr, len(garr), 0, scratch.data_ptr(), scratch.numel(),
-                _stream(dev)), "MipNerf.backward")
+        _call(dev, "MipNerf.backward", lib.mipnerf_b200_backward, C.byref(cfg), C.byref(ws), C.byref(rs), t_arr,
+              int(ctx.randomized), C.byref(rng) if rng is not None else None, normal_arr, int(ctx.white_bkgd),
+              _cabi.PRECISIONS[ctx.precision], cots, garr, len(garr), 0, scratch.data_ptr(), scratch.numel())
         return (None,) * 9 + tuple(out_grads)
 
 
@@ -647,15 +629,11 @@ def _check_query_autograd(model: MipNerf, tensors, radiance: bool) -> None:
                                   "deg_view=4; use precision='fp32' or autograd=False")
 
 
-def _query_with_grad(model: MipNerf, means, covs, viewdirs, raw: bool):
-    radiance = viewdirs is not None
-    _check_query_autograd(model, (means, covs, viewdirs), radiance)
-    shape = means.shape[:-1]
-    m = _f32(means).reshape(-1, 3)
-    c = _f32(covs).reshape(-1, 3) if covs is not None else None
-    v = _f32(viewdirs).reshape(-1, 3) if viewdirs is not None else None
-    params = [p for lin in model.mlp.linears() for p in (lin.weight, lin.bias)]
-    outs = _QueryWithGrad.apply(model, m, c, v, bool(raw), *params)
+def _query_with_grad(model: MipNerf, given, shape, m, c, v, raw: bool):
+    """A query with a grad_fn, on the output of `_query_points`; `given` are the caller's tensors."""
+    radiance = v is not None
+    _check_query_autograd(model, given, radiance)
+    outs = _QueryWithGrad.apply(model, m, c, v, bool(raw), *model.mlp.params())
     if not radiance:
         return outs[0].reshape(shape)
     return outs[0].reshape(*shape, 3), outs[1].reshape(shape)
@@ -706,8 +684,7 @@ class _QueryWithGrad(torch.autograd.Function):
         # per call, not the per-stream _Workspace: up to one chunk's activations (GBs), which a forward-only process
         # that ran one query backward should not keep reserved for small forwards
         scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            _cabi.check(lib.mipnerf_b200_query_backward(
-                C.byref(cfg), C.byref(ws), means.data_ptr(), _ptr(covs), _ptr(viewdirs), p, prec, C.byref(cot), garr,
-                len(garr), 0, scratch.data_ptr(), scratch.numel(), _stream(dev)), "MipNerf.query backward")
+        _call(dev, "MipNerf.query backward", lib.mipnerf_b200_query_backward, C.byref(cfg), C.byref(ws),
+              means.data_ptr(), _ptr(covs), _ptr(viewdirs), p, prec, C.byref(cot), garr, len(garr), 0,
+              scratch.data_ptr(), scratch.numel())
         return (None,) * 5 + tuple(out_grads)

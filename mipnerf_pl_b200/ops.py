@@ -42,6 +42,16 @@ def _stream(device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
 
 
+def _call(dev: torch.device, what: str, fn, *args) -> None:
+    """Launch the library entry point `fn(*args, stream)` on `dev`'s current stream, the last argument of every entry
+    point that launches, and raise its error as `_cabi.check` does.  The device is made current only when it is not
+    already: the guard costs host time on every call."""
+    if dev.index is not None and dev.index != torch.cuda.current_device():
+        with torch.cuda.device(dev):
+            return _call(dev, what, fn, *args)
+    _cabi.check(fn(*args, _stream(dev)), what)
+
+
 def _rays_struct(origins, directions, viewdirs, radii, near=None, far=None):
     """(RaysStruct, keep): `keep` holds the fp32 ray tensors the struct points at, in its field order; viewdirs may be
     None (NULL), near / far default to zeros."""
@@ -78,9 +88,8 @@ def philox_uniform(seed: int, offset: int, stream_id: int, batch: int, num_draws
     dev = torch.device(device)
     out = torch.empty(batch, num_draws, device=dev)
     rng = _cabi.Rng(seed & 0xFFFFFFFFFFFFFFFF, offset)
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_philox_uniform(C.byref(rng), stream_id, batch, num_draws, out.data_ptr(),
-                                                            _stream(dev)), "philox_uniform")
+    _call(dev, "philox_uniform", _cabi.lib().mipnerf_b200_philox_uniform, C.byref(rng), stream_id, batch, num_draws,
+          out.data_ptr())
     return out
 
 
@@ -96,9 +105,8 @@ def philox_normal(seed: int, offset: int, level: int, batch: int, num_samples: i
     dev = torch.device(device)
     out = torch.empty(batch, num_samples, device=dev)
     rng = _cabi.Rng(seed & 0xFFFFFFFFFFFFFFFF, offset)
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_philox_normal(C.byref(rng), level, batch, num_samples, out.data_ptr(),
-                                                           _stream(dev)), "philox_normal")
+    _call(dev, "philox_normal", _cabi.lib().mipnerf_b200_philox_normal, C.byref(rng), level, batch, num_samples,
+          out.data_ptr())
     return out
 
 
@@ -115,9 +123,8 @@ def cast_rays(t_samples, origins, directions, radii, ray_shape, diagonal=True):
     rs, keep = _rays_struct(origins, directions, None, radii)
     means = torch.empty(b, n, 3, device=dev)
     covs = torch.empty(b, n, 3, device=dev)
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_cast_rays(C.byref(rs), t.data_ptr(), n, means.data_ptr(),
-                                                       covs.data_ptr(), _stream(dev)), "cast_rays")
+    _call(dev, "cast_rays", _cabi.lib().mipnerf_b200_cast_rays, C.byref(rs), t.data_ptr(), n, means.data_ptr(),
+          covs.data_ptr())
     return means, covs
 
 
@@ -136,10 +143,8 @@ def sample_along_rays(origins, directions, radii, num_samples, near, far, random
     t = torch.empty(b, num_samples + 1, device=dev)
     means = torch.empty(b, num_samples, 3, device=dev)
     covs = torch.empty(b, num_samples, 3, device=dev)
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_sample_along_rays(
-            C.byref(rs), num_samples, int(bool(randomized)), int(bool(disparity)), _ptr(tr), t.data_ptr(),
-            means.data_ptr(), covs.data_ptr(), _stream(dev)), "sample_along_rays")
+    _call(dev, "sample_along_rays", _cabi.lib().mipnerf_b200_sample_along_rays, C.byref(rs), num_samples,
+          int(bool(randomized)), int(bool(disparity)), _ptr(tr), t.data_ptr(), means.data_ptr(), covs.data_ptr())
     return t, (means, covs)
 
 
@@ -156,10 +161,8 @@ def sorted_piecewise_constant_pdf(bins, weights, num_samples, randomized,
     uj = _f32(u_jitter) if randomized else None
     out = torch.empty(b, num_samples, device=dev)
     inds = torch.empty(b, num_samples, device=dev, dtype=torch.int64) if return_inds else None
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_sorted_piecewise_constant_pdf(
-            bn.data_ptr(), w.data_ptr(), b, nb, num_samples, int(bool(randomized)), _ptr(uj), out.data_ptr(),
-            _ptr(inds), _stream(dev)), "sorted_piecewise_constant_pdf")
+    _call(dev, "sorted_piecewise_constant_pdf", _cabi.lib().mipnerf_b200_sorted_piecewise_constant_pdf, bn.data_ptr(),
+          w.data_ptr(), b, nb, num_samples, int(bool(randomized)), _ptr(uj), out.data_ptr(), _ptr(inds))
     return (out, inds) if return_inds else out
 
 
@@ -182,11 +185,9 @@ def resample_along_rays(origins, directions, radii, t_samples, weights, randomiz
     means = torch.empty(b, n, 3, device=dev)
     covs = torch.empty(b, n, 3, device=dev)
     inds = torch.empty(b, n + 1, device=dev, dtype=torch.int64) if return_inds else None
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_resample_along_rays(
-            C.byref(rs), t.data_ptr(), w.data_ptr(), n, int(bool(randomized)), _ptr(uj),
-            float(resample_padding), new_t.data_ptr(), means.data_ptr(), covs.data_ptr(), _ptr(inds),
-            _stream(dev)), "resample_along_rays")
+    _call(dev, "resample_along_rays", _cabi.lib().mipnerf_b200_resample_along_rays, C.byref(rs), t.data_ptr(),
+          w.data_ptr(), n, int(bool(randomized)), _ptr(uj), float(resample_padding), new_t.data_ptr(), means.data_ptr(),
+          covs.data_ptr(), _ptr(inds))
     return (new_t, (means, covs), inds) if return_inds else (new_t, (means, covs))
 
 
@@ -200,10 +201,8 @@ def integrated_pos_enc(means_covs, min_deg, max_deg, diagonal=True):
     lead = m.shape[:-1]
     npts = m.numel() // 3
     out = torch.empty(*lead, 6 * (max_deg - min_deg), device=dev)
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_integrated_pos_enc(
-            m.data_ptr(), c.data_ptr(), npts, int(min_deg), int(max_deg), out.data_ptr(), _stream(dev)),
-            "integrated_pos_enc")
+    _call(dev, "integrated_pos_enc", _cabi.lib().mipnerf_b200_integrated_pos_enc, m.data_ptr(), c.data_ptr(), npts,
+          int(min_deg), int(max_deg), out.data_ptr())
     return out
 
 
@@ -214,10 +213,8 @@ def pos_enc(x, min_deg, max_deg, append_identity=True):
     lead = xx.shape[:-1]
     width = 6 * (max_deg - min_deg) + (3 if append_identity else 0)
     out = torch.empty(*lead, width, device=dev)
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_pos_enc(
-            xx.data_ptr(), xx.numel() // 3, int(min_deg), int(max_deg), int(bool(append_identity)),
-            out.data_ptr(), _stream(dev)), "pos_enc")
+    _call(dev, "pos_enc", _cabi.lib().mipnerf_b200_pos_enc, xx.data_ptr(), xx.numel() // 3, int(min_deg),
+          int(max_deg), int(bool(append_identity)), out.data_ptr())
     return out
 
 
@@ -231,11 +228,9 @@ def volumetric_rendering(rgb, density, t_samples, dirs, white_bkgd):
     dist = torch.empty(b, device=dev)
     acc = torch.empty(b, device=dev)
     w = torch.empty(b, n, device=dev)
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_volumetric_rendering(
-            r.data_ptr(), d.data_ptr(), t.data_ptr(), dd.data_ptr(), b, n, int(bool(white_bkgd)),
-            comp.data_ptr(), dist.data_ptr(), acc.data_ptr(), w.data_ptr(), _stream(dev)),
-            "volumetric_rendering")
+    _call(dev, "volumetric_rendering", _cabi.lib().mipnerf_b200_volumetric_rendering, r.data_ptr(), d.data_ptr(),
+          t.data_ptr(), dd.data_ptr(), b, n, int(bool(white_bkgd)), comp.data_ptr(), dist.data_ptr(), acc.data_ptr(),
+          w.data_ptr())
     return comp, dist, acc, w
 
 
@@ -243,9 +238,7 @@ def _distloss_value(w: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
     dev = _dev(w)
     b, n = w.shape
     out = torch.empty(b, device=dev)
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_distloss(w.data_ptr(), t.data_ptr(), b, n, out.data_ptr(), _stream(dev)),
-                    "distloss")
+    _call(dev, "distloss", _cabi.lib().mipnerf_b200_distloss, w.data_ptr(), t.data_ptr(), b, n, out.data_ptr())
     return out.mean()
 
 
@@ -265,10 +258,8 @@ class _DistLoss(torch.autograd.Function):
         dev = w.device
         d_w = torch.empty_like(w)
         g = _f32(grad_out).reshape(1)
-        with torch.cuda.device(dev):
-            _cabi.check(_cabi.lib().mipnerf_b200_distloss_backward(w.data_ptr(), t.data_ptr(), b, n, g.data_ptr(),
-                                                                    1.0 / max(b, 1), d_w.data_ptr(), _stream(dev)),
-                        "distloss_backward")
+        _call(dev, "distloss_backward", _cabi.lib().mipnerf_b200_distloss_backward, w.data_ptr(), t.data_ptr(), b, n,
+              g.data_ptr(), 1.0 / max(b, 1), d_w.data_ptr())
         return d_w.to(ctx.weight_dtype), None
 
 

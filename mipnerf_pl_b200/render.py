@@ -36,7 +36,7 @@ def generate_rays(c2w, height: int = 800, width: int = 800, camera_angle_x: floa
                   device="cuda") -> Rays:
     """Rays of frame rows [rows[0], rows[1]) (default: all) as flat [R*W, C] CUDA tensors."""
     from . import _cabi
-    from .ops import _stream
+    from .ops import _call
     dev = torch.device(device)
     if dev.type != "cuda":
         raise RuntimeError("generate_rays writes rays straight into HBM; use rays.blender_rays() on the host")
@@ -46,11 +46,9 @@ def generate_rays(c2w, height: int = 800, width: int = 800, camera_angle_x: floa
     o, d, v, rad, nr, fr = mk(3), mk(3), mk(3), mk(1), mk(1), mk(1)
     pose = np.ascontiguousarray(np.asarray(c2w, dtype=np.float32)[:3, :4]).reshape(-1)
     focal = float(np.float32(0.5 * width / np.tan(0.5 * camera_angle_x)))
-    with torch.cuda.device(dev):
-        _cabi.check(_cabi.lib().mipnerf_b200_generate_rays(
-            pose.ctypes.data_as(C.POINTER(C.c_float)), height, width, focal, near, far, r0, r1 - r0,
-            o.data_ptr(), d.data_ptr(), v.data_ptr(), rad.data_ptr(), nr.data_ptr(), fr.data_ptr(), _stream(dev)),
-            "generate_rays")
+    _call(dev, "generate_rays", _cabi.lib().mipnerf_b200_generate_rays, pose.ctypes.data_as(C.POINTER(C.c_float)),
+          height, width, focal, near, far, r0, r1 - r0, o.data_ptr(), d.data_ptr(), v.data_ptr(), rad.data_ptr(),
+          nr.data_ptr(), fr.data_ptr())
     return Rays(o, d, v, rad, torch.ones_like(rad), nr, fr)
 
 

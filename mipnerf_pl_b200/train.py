@@ -21,13 +21,13 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Dict, Iterable, List, Optional, Sequence
+from typing import Dict, Iterable, Optional, Sequence
 
 import torch
 
 from . import _cabi
-from .mip_nerf import MipNerf, _Workspace
-from .ops import _dev, _f32, _grad_array, _ptr, _rays_struct, _stream
+from .mip_nerf import MipNerf, _level_outputs, _Workspace
+from .ops import _call, _dev, _f32, _grad_array, _ptr, _rays_struct
 from .rays import Rays
 
 
@@ -72,6 +72,15 @@ class FusedAdam(torch.optim.Optimizer):
         step = st["step"]
         return step if isinstance(step, int) else int(float(step))
 
+    def _state(self, p):
+        """p's Adam state, created at step 0 with zero moments on first use."""
+        st = self.state[p]
+        if not st:
+            st["step"] = 0
+            st["exp_avg"] = torch.zeros_like(p)
+            st["exp_avg_sq"] = torch.zeros_like(p)
+        return st
+
     def _step_group(self, lib, group, b1: float, b2: float, grad_scale: float) -> bool:
         """One launch for the whole group (`mipnerf_b200_adam_step_multi`) when its tensors sit on one CUDA device
         and share a step count — the normal case; otherwise the caller falls back to one launch per tensor."""
@@ -79,26 +88,16 @@ class FusedAdam(torch.optim.Optimizer):
         if not ps or any(p.dtype != torch.float32 or not p.is_contiguous() or not p.grad.is_contiguous() or
                          p.device != ps[0].device or not p.is_cuda for p in ps):
             return False
-        for p in ps:
-            st = self.state[p]
-            if not st:
-                st["step"] = 0
-                st["exp_avg"] = torch.zeros_like(p)
-                st["exp_avg_sq"] = torch.zeros_like(p)
-        steps = {self._step_count(self.state[p]) for p in ps}
+        steps = {self._step_count(self._state(p)) for p in ps}
         if len(steps) != 1:
             return False
         step = steps.pop() + 1
         n = len(ps)
         arr = C.c_void_p * n
-        dev = _dev(ps[0])
-        with torch.cuda.device(dev):
-            _cabi.check(lib.mipnerf_b200_adam_step_multi(
-                n, arr(*[p.data_ptr() for p in ps]), arr(*[p.grad.data_ptr() for p in ps]),
-                arr(*[self.state[p]["exp_avg"].data_ptr() for p in ps]),
-                arr(*[self.state[p]["exp_avg_sq"].data_ptr() for p in ps]),
-                (C.c_int64 * n)(*[p.numel() for p in ps]), float(group["lr"]), b1, b2, float(group["eps"]), step,
-                grad_scale, _stream(dev)), "FusedAdam.step")
+        _call(_dev(ps[0]), "FusedAdam.step", lib.mipnerf_b200_adam_step_multi, n, arr(*[p.data_ptr() for p in ps]),
+              arr(*[p.grad.data_ptr() for p in ps]), arr(*[self.state[p]["exp_avg"].data_ptr() for p in ps]),
+              arr(*[self.state[p]["exp_avg_sq"].data_ptr() for p in ps]), (C.c_int64 * n)(*[p.numel() for p in ps]),
+              float(group["lr"]), b1, b2, float(group["eps"]), step, grad_scale)
         for p in ps:
             self.state[p]["step"] = step
             torch.autograd.graph.increment_version(p)  # written in place by the library: keep the packed-weight
@@ -123,17 +122,11 @@ class FusedAdam(torch.optim.Optimizer):
                 dev = _dev(p)
                 if p.dtype != torch.float32 or not p.is_contiguous() or not p.grad.is_contiguous():
                     raise RuntimeError("FusedAdam: contiguous fp32 parameters only")
-                st = self.state[p]
-                if not st:
-                    st["step"] = 0
-                    st["exp_avg"] = torch.zeros_like(p)
-                    st["exp_avg_sq"] = torch.zeros_like(p)
+                st = self._state(p)
                 st["step"] = self._step_count(st) + 1
-                with torch.cuda.device(dev):
-                    _cabi.check(lib.mipnerf_b200_adam_step(
-                        p.data_ptr(), p.grad.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(),
-                        p.numel(), float(group["lr"]), float(b1), float(b2), float(group["eps"]), st["step"],
-                        grad_scale, _stream(dev)), "FusedAdam.step")
+                _call(dev, "FusedAdam.step", lib.mipnerf_b200_adam_step, p.data_ptr(), p.grad.data_ptr(),
+                      st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(), p.numel(), float(group["lr"]), float(b1),
+                      float(b2), float(group["eps"]), st["step"], grad_scale)
                 torch.autograd.graph.increment_version(p)  # written in place by the library: keep the
                 #                                            packed-weight caches (keyed on _version) honest
         return loss
@@ -213,35 +206,23 @@ def _run(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized: bool, white
                       sqerr.data_ptr(), dl.data_ptr())
     ws, wkeep = model.mlp._weights_struct(cfg, _cabi.FP32, dev)
     garr = _grad_array(grad_tensors)
-    outs = (_cabi.LevelOut * levels)()
-    ret = []
-    for lvl in range(levels):
-        comp, dist, acc = torch.empty(b, 3, device=dev), torch.empty(b, device=dev), torch.empty(b, device=dev)
-        w, t = torch.empty(b, n, device=dev), torch.empty(b, n + 1, device=dev)
-        outs[lvl] = _cabi.LevelOut(comp.data_ptr(), dist.data_ptr(), acc.data_ptr(), w.data_ptr(), t.data_ptr(), None,
-                                   _ptr(normals[lvl]))
-        ret.append((comp, dist, acc, w, t))
+    ret, outs = _level_outputs(b, n, levels, dev, normals, False)
     lib = _cabi.lib()
     nbytes = (lib.mipnerf_b200_train_workspace_bytes_for(C.byref(cfg), b, prec) if prec == _cabi.BF16X3
               else lib.mipnerf_b200_train_workspace_bytes(C.byref(cfg), b))
     scratch = _Workspace.get(dev, nbytes)
     tail = (int(bool(white_bkgd)), prec, C.byref(loss), outs, garr, len(garr), int(bool(accumulate)),
-            scratch.data_ptr() if nbytes else None, scratch.numel() if nbytes else 0, _stream(dev))
-    with torch.cuda.device(dev):
-        if rng is not None:
-            rc = lib.mipnerf_b200_forward_backward_rng(C.byref(cfg), C.byref(ws), C.byref(rs), C.byref(rng), *tail)
-        else:
-            rc = lib.mipnerf_b200_forward_backward(C.byref(cfg), C.byref(ws), C.byref(rs), int(bool(randomized)),
-                                                   _ptr(t_rand), _ptr(u_jitter), *tail)
-        _cabi.check(rc, "forward_backward")
+            scratch.data_ptr() if nbytes else None, scratch.numel() if nbytes else 0)
+    if rng is not None:
+        _call(dev, "forward_backward", lib.mipnerf_b200_forward_backward_rng, C.byref(cfg), C.byref(ws), C.byref(rs),
+              C.byref(rng), *tail)
+    else:
+        _call(dev, "forward_backward", lib.mipnerf_b200_forward_backward, C.byref(cfg), C.byref(ws), C.byref(rs),
+              int(bool(randomized)), _ptr(t_rand), _ptr(u_jitter), *tail)
     mse = sqerr.sum(dim=1) / mask_sum                      # [levels]   (models/nerf_system.py:104-105)
     distl = dl.sum(dim=1) / max(global_rays, 1)            # [levels]   (:106)
     total = (mse * torch.tensor(mse_m, device=dev) + distl * torch.tensor(dist_m, device=dev)).sum()
     return {"loss": total, "mse": mse, "distloss": distl, "ret": ret}
-
-
-def _param_list(model: MipNerf) -> List[torch.nn.Parameter]:
-    return [p for lin in model.mlp.linears() for p in (lin.weight, lin.bias)]
 
 
 def forward_backward(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized: bool, white_bkgd: bool, *,
@@ -251,7 +232,7 @@ def forward_backward(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized:
     """Forward + backward of the training loss; gradients are written (or added, with `accumulate`)
     into `param.grad`.  For a ray shard of a larger batch pass the GLOBAL `mask_sum` / `global_rays`;
     shard gradients then sum to the full-batch gradient."""
-    params = _param_list(model)
+    params = model.mlp.params()
     if all(p.grad is None for p in params) and len({(p.device, p.dtype) for p in params}) == 1:
         # first step: carve every .grad out of ONE flat buffer, so that the data-parallel all-reduce
         # (`allreduce_grads`) is a single NCCL call on it with no concatenate / scatter copies
@@ -293,5 +274,5 @@ def fused_loss(model: MipNerf, rays: Rays, rgbs: torch.Tensor, randomized: bool,
     holder: Dict[str, object] = {}
     kwargs = dict(coarse_loss_mult=coarse_loss_mult, dist_mult=dist_mult,
                   disable_multiscale_loss=disable_multiscale_loss, **kw)
-    loss = _FusedLoss.apply(model, rays, rgbs, randomized, white_bkgd, kwargs, holder, *_param_list(model))
+    loss = _FusedLoss.apply(model, rays, rgbs, randomized, white_bkgd, kwargs, holder, *model.mlp.params())
     return loss, holder
