@@ -609,10 +609,11 @@ __device__ __forceinline__ void level_epilogue_chunk_rs(const float (&acc)[64], 
       ffma2(d0, d1, fmaxf(a0, 0.f), fmaxf(a2, 0.f), wd.x, wd.x);
       ffma2(d0, d1, fmaxf(a1, 0.f), fmaxf(a3, 0.f), wd.y, wd.y);
     }
-    if (relu) a0 = fmaxf(a0, 0.f), a1 = fmaxf(a1, 0.f), a2 = fmaxf(a2, 0.f), a3 = fmaxf(a3, 0.f);
+    // ReLU in the conversion (F2FP.RELU): rounding keeps the sign, so clamping after it gives max(x, 0) rounded, the
+    // same bits as fmaxf then pack2 for every x but NaN (which fmaxf would turn into 0)
     const int jg = (c_base >> 3) + j;
-    x[2 * jg] = pack2<kFmt>(a0, a1);
-    x[2 * jg + 1] = pack2<kFmt>(a2, a3);
+    x[2 * jg] = relu ? pack2_relu<kFmt>(a0, a1) : pack2<kFmt>(a0, a1);
+    x[2 * jg + 1] = relu ? pack2_relu<kFmt>(a2, a3) : pack2<kFmt>(a2, a3);
   }
   if (dump) {
     // The four threads of a quad hold the four 4-byte quarters of the chunk's four 16-byte column groups (per row): a
