@@ -506,6 +506,30 @@ typedef struct mipnerf_b200_grid {
 int mipnerf_b200_grid_render(const mipnerf_b200_grid* grid, const mipnerf_b200_rays* rays, float step, int white_bkgd,
                              float* rgb, float* distance, float* acc, void* stream);
 
+/* Per-level gradient buffers of a baked grid's parameters: density[l] [M_l] is indexed by SH row (the density of the
+ * kept point whose row is r), sh[l] [M_l, (degree + 1)^2, 3] has the layout of levels[l].sh.  Dropped points (row -1)
+ * are not parameters. */
+typedef struct mipnerf_b200_grid_grads {
+  float* density[MIPNERF_B200_GRID_MAX_LEVELS];
+  float* sh[MIPNERF_B200_GRID_MAX_LEVELS];
+} mipnerf_b200_grid_grads;
+
+/* The derivative of mipnerf_b200_grid_render's outputs (same grid, rays, step and white_bkgd) under the cotangents
+ * d_rgb [B,3], d_distance [B], d_acc [B] (each may be NULL: zero) with respect to the kept points' densities and SH
+ * coefficients, ADDED into `grads` (the caller zeroes it; density[l] and sh[l] are required for every level whose
+ * levels[l].sh is non-NULL).  It differentiates the marcher as it runs: the same fp32 sample lattice, inside test,
+ * level choice and blend, trilinear corner weights, the sigmoid with rgb_padding, white_bkgd, and the distance clamp
+ * (the gradient passes where near <= distance <= far).  Samples outside the bounds, in empty macro cells, or after the
+ * one that stops the ray contribute nothing.  A sample of an occupied cell whose density interpolates to exactly 0
+ * does contribute to the density of its kept corners.  On a grid straight from the baker, every corner a sample in an
+ * empty cell reads is a dropped point, so skipping empty cells loses no gradient up to rounding at cell faces; once
+ * kept densities have been set to 0 (and the occupancy rebuilt from them) the skip can drop the gradient that would
+ * let those densities grow back.  The scatter is fp32 atomic adds: reproducible to round-off, not bit for bit.  No
+ * allocation, no synchronisation. */
+int mipnerf_b200_grid_render_backward(const mipnerf_b200_grid* grid, const mipnerf_b200_rays* rays, float step,
+                                      int white_bkgd, const float* d_rgb, const float* d_distance, const float* d_acc,
+                                      const mipnerf_b200_grid_grads* grads, void* stream);
+
 /* Hardware self-test of the wgmma building blocks (descriptor / swizzle / accumulator-fragment conventions):
  * d[128,n] = a[128,k] . b[n,k]^T, 16-bit operands (precision BF16|FP16), fp32 accumulate; n in {128, 256}.
  * variant bit 0: B through a pre-swizzled image + cp.async.bulk (needs `scratch`); bit 1: A in registers (the RS form

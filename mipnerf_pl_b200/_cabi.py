@@ -93,6 +93,10 @@ class Grid(C.Structure):
                 ("block", C.c_int32)]
 
 
+class GridGrads(C.Structure):
+    _fields_ = [("density", C.c_void_p * GRID_MAX_LEVELS), ("sh", C.c_void_p * GRID_MAX_LEVELS)]
+
+
 # name -> (restype, argtypes); every symbol include/mipnerf_b200.h declares.
 _V = C.c_void_p
 _SIGNATURES = {
@@ -171,6 +175,8 @@ _SIGNATURES = {
                                                _V]),
     "mipnerf_b200_grid_render": (C.c_int, [C.POINTER(Grid), C.POINTER(RaysStruct), C.c_float, C.c_int, _V, _V, _V,
                                            _V]),
+    "mipnerf_b200_grid_render_backward": (C.c_int, [C.POINTER(Grid), C.POINTER(RaysStruct), C.c_float, C.c_int, _V,
+                                                    _V, _V, C.POINTER(GridGrads), _V]),
     "mipnerf_b200_selftest_umma": (C.c_int, [_V, _V, _V, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),
     "mipnerf_b200_profile_enable": (C.c_int, [C.c_int]),
     "mipnerf_b200_profile_num_kernels": (C.c_int, []),

@@ -35,6 +35,9 @@ from .render import gather_rows, generate_rays, shard_rows
 MAX_LEVELS = _cabi.GRID_MAX_LEVELS
 DEFAULT_BLOCK = 8
 DEFAULT_THRESHOLD = 1e-2
+# finetune_grid's Adam learning rates (README, "Fine-tuning a baked grid")
+FINETUNE_LR_DENSITY = 0.1
+FINETUNE_LR_SH = 0.01
 _FORMAT = 1
 
 
@@ -76,8 +79,6 @@ def grid_structure(densities: Sequence[torch.Tensor], threshold: float, block: i
         raise ValueError(f"level 0: grid {n0}, need [nz, ny, nx], each >= 2 with n - 1 divisible by {scale_max}")
     baked, indices = [], []
     dev = densities[0].device
-    o = [-(-(n - 1) // block) for n in n0]  # (oz, oy, ox)
-    occ = torch.zeros(o, dtype=torch.float32, device=dev)
     for lvl, dens in enumerate(densities):
         want = tuple((n - 1) // (1 << lvl) + 1 for n in n0)
         if tuple(dens.shape) != want:
@@ -89,13 +90,27 @@ def grid_structure(densities: Sequence[torch.Tensor], threshold: float, block: i
         idx[keep] = torch.arange(int(keep.sum()), dtype=torch.int32, device=dev)
         baked.append(bd.contiguous())
         indices.append(idx)
+    return baked, indices, grid_occupancy(baked, block)
+
+
+@torch.no_grad()
+def grid_occupancy(baked_densities: Sequence[torch.Tensor], block: int = DEFAULT_BLOCK) -> torch.Tensor:
+    """The occupancy [oz, oy, ox] uint8 (o = ceil((n_0 - 1) / block) per axis) of nested baked density grids [nz, ny,
+    nx] (level l: (n_0 - 1) / 2^l + 1 points per axis): 0 only for macro cells of `block`^3 finest cells whose lattice
+    points, widened by one point of each level, have baked density 0 at every level."""
+    n0 = tuple(baked_densities[0].shape)
+    dev = baked_densities[0].device
+    o = [-(-(n - 1) // block) for n in n0]  # (oz, oy, ox)
+    occ = torch.zeros(o, dtype=torch.float32, device=dev)
+    for lvl, bd in enumerate(baked_densities):
+        want = tuple(bd.shape)
         nz = (bd != 0).to(torch.float32)
         s = 1 << lvl
         ax, ay, az = (_cell_matrix(o[2 - a], want[2 - a], block, s, dev) for a in range(3))
         t = torch.einsum("kji,ai->kja", nz, ax)
         t = torch.einsum("kja,bj->kba", t, ay)
         occ += torch.einsum("kba,ck->cba", t, az)
-    return baked, indices, (occ > 0).to(torch.uint8)
+    return (occ > 0).to(torch.uint8)
 
 
 class BakedGrid:
@@ -127,6 +142,60 @@ class BakedGrid:
         want = tuple(-(-(n - 1) // self.block) for n in n0)
         if tuple(self.occupancy.shape) != want:
             raise ValueError(f"occupancy {tuple(self.occupancy.shape)}: need {want} for block {self.block}")
+        self.kept_density: Optional[List[torch.Tensor]] = None  # trainable: per level [M_l] in row order
+        self._kept_pos: List[torch.Tensor] = []
+        self._synced: List[int] = []
+
+    # ---- fine-tuning: the kept points' densities and SH rows as parameters -----------------------------------------
+
+    def requires_grad_(self, requires_grad: bool = True) -> "BakedGrid":
+        """Make the grid trainable: per level a contiguous fp32 leaf `kept_density[l]` [M_l] (the kept points'
+        densities in SH-row order) and `sh[l]` requiring grad.  The cells follow `kept_density` on the next read
+        (`_struct`, `density`, `save`): projected onto >= 0, scattered into the kept points, occupancy rebuilt.  The
+        kept set and the rows never change.  False syncs and turns the parameters back into plain tensors."""
+        if not requires_grad:
+            if self.kept_density is not None:
+                self._sync()
+                self.kept_density, self._kept_pos, self._synced = None, [], []
+            for c in self.sh:
+                c.requires_grad_(False)
+            return self
+        if self.kept_density is not None:
+            return self
+        kd, pos = [], []
+        for lvl in range(self.levels):
+            idx = self.cells[lvl][..., 1].reshape(-1)
+            flat = (idx >= 0).nonzero().reshape(-1)
+            p = torch.empty_like(flat)
+            p[idx[flat].long()] = flat  # the lattice position of row r
+            pos.append(p)
+            kd.append(self.cells[lvl].view(-1, 2)[p, 0].view(torch.float32).requires_grad_(True))
+            self.sh[lvl].requires_grad_(True)
+        self.kept_density, self._kept_pos = kd, pos
+        self._synced = [t._version for t in kd]
+        return self
+
+    @property
+    def trainable(self) -> bool:
+        return self.kept_density is not None
+
+    def parameters(self) -> List[torch.Tensor]:
+        """[kept_density_0, sh_0, kept_density_1, sh_1, ...] of a trainable grid."""
+        if self.kept_density is None:
+            raise RuntimeError("BakedGrid.parameters: call requires_grad_() first")
+        return [t for pair in zip(self.kept_density, self.sh) for t in pair]
+
+    @torch.no_grad()
+    def _sync(self) -> None:
+        """Bring the cells and occupancy up to `kept_density` if it changed since the last sync."""
+        if self.kept_density is None or [t._version for t in self.kept_density] == self._synced:
+            return
+        for lvl, (kd, p) in enumerate(zip(self.kept_density, self._kept_pos)):
+            kd.clamp_(min=0)
+            self.cells[lvl].view(-1, 2)[p, 0] = kd.view(torch.int32)
+        self.occupancy = grid_occupancy([self.cells[lvl][..., 0].view(torch.float32) for lvl in range(self.levels)],
+                                        self.block)
+        self._synced = [t._version for t in self.kept_density]
 
     @property
     def levels(self) -> int:
@@ -143,6 +212,7 @@ class BakedGrid:
 
     def density(self, level: int = 0) -> torch.Tensor:
         """The baked density [nz, ny, nx] of a level (a view)."""
+        self._sync()
         return self.cells[level][..., 0].view(torch.float32)
 
     def index(self, level: int = 0) -> torch.Tensor:
@@ -163,6 +233,7 @@ class BakedGrid:
         return float(np.float32(0.5) * step.min())
 
     def _struct(self) -> "_cabi.Grid":
+        self._sync()
         g = _cabi.Grid()
         for lvl, (c, s) in enumerate(zip(self.cells, self.sh)):
             nz, ny, nx = c.shape[:3]
@@ -173,10 +244,20 @@ class BakedGrid:
         g.rgb_padding, g.occupancy, g.block = self.rgb_padding, self.occupancy.data_ptr(), self.block
         return g
 
-    @torch.no_grad()
     def render(self, rays: Rays, white_bkgd: bool = True, step: Optional[float] = None):
         """(rgb [B,3], distance [B], acc [B]) of flat rays on the grid's device, marched every `step` along |d| (default
-        `default_step()`)."""
+        `default_step()`).  Differentiable in `parameters()` when the grid is trainable and grad mode is on (rays that
+        require grad are refused: there is no ray gradient)."""
+        if self.kept_density is None or not torch.is_grad_enabled():
+            with torch.no_grad():
+                return self._render(rays, white_bkgd, step)[0]
+        if any(isinstance(f, torch.Tensor) and f.requires_grad for f in rays):
+            raise ValueError("BakedGrid.render: rays that require grad; the grid has no gradient for rays")
+        self._sync()
+        return _GridRender.apply(self, rays, bool(white_bkgd), step, *self.parameters())
+
+    def _render(self, rays: Rays, white_bkgd: bool, step: Optional[float]):
+        """((rgb, distance, acc), the fp32 ray fields the launch read, the step it used)."""
         dev = _dev(self.cells[0])
         o = rays.origins.reshape(-1, 3)
         if o.device != dev:
@@ -191,17 +272,18 @@ class BakedGrid:
         st = self.default_step() if step is None else float(step)
         _call(dev, "grid_render", _cabi.lib().mipnerf_b200_grid_render, C.byref(g), C.byref(rs), st,
               int(bool(white_bkgd)), rgb.data_ptr(), dist.data_ptr(), acc.data_ptr())
-        return rgb, dist, acc
+        return (rgb, dist, acc), keep, st
 
     def save(self, path: str) -> None:
         """One .npz: per level density, index and sh, plus occupancy, bounds, degree, rgb_padding and block."""
+        self._sync()
         arrays = {"format": np.int32(_FORMAT), "levels": np.int32(self.levels), "degree": np.int32(self.degree),
                   "rgb_padding": np.float32(self.rgb_padding), "block": np.int32(self.block),
                   "bounds": np.asarray(self.bounds, dtype=np.float32), "occupancy": self.occupancy.cpu().numpy()}
         for lvl in range(self.levels):
             arrays[f"density_{lvl}"] = self.density(lvl).cpu().numpy()
             arrays[f"index_{lvl}"] = self.index(lvl).cpu().numpy()
-            arrays[f"sh_{lvl}"] = self.sh[lvl].cpu().numpy()
+            arrays[f"sh_{lvl}"] = self.sh[lvl].detach().cpu().numpy()
         np.savez(path, **arrays)
 
     @classmethod
@@ -215,6 +297,40 @@ class BakedGrid:
             return cls([t(f"density_{lvl}") for lvl in range(levels)], [t(f"index_{lvl}") for lvl in range(levels)],
                        [t(f"sh_{lvl}") for lvl in range(levels)], t("occupancy"),
                        (tuple(bounds[0]), tuple(bounds[1])), int(z["degree"]), float(z["rgb_padding"]), int(z["block"]))
+
+
+class _GridRender(torch.autograd.Function):
+    """BakedGrid.render of a trainable grid: the forward is the no-grad launch; the backward zeroes one gradient per
+    parameter and adds mipnerf_b200_grid_render_backward into them."""
+
+    @staticmethod
+    def forward(ctx, grid, rays, white_bkgd, step, *params):
+        ctx.set_materialize_grads(False)  # an unused output's cotangent stays None: NULL to the kernel
+        out, rays_keep, ctx.step = grid._render(rays, white_bkgd, step)
+        ctx.grid, ctx.white_bkgd, ctx.num_rays = grid, white_bkgd, out[0].shape[0]
+        # the parameters and the ray fields the kernel reads (aliases of the caller's rays when those are contiguous
+        # fp32): an in-place update of either before the backward raises autograd's version error
+        ctx.save_for_backward(*params, *rays_keep)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_rgb, d_dist, d_acc):
+        saved = ctx.saved_tensors
+        params, rays_keep = saved[:-6], saved[-6:]
+        grid = ctx.grid
+        dev = _dev(grid.cells[0])
+        grads = [torch.zeros_like(p, memory_format=torch.contiguous_format) for p in params]
+        gg = _cabi.GridGrads()
+        for lvl in range(grid.levels):
+            if grads[2 * lvl + 1].numel():
+                gg.density[lvl], gg.sh[lvl] = grads[2 * lvl].data_ptr(), grads[2 * lvl + 1].data_ptr()
+        cot = [None if t is None else _f32(t) for t in (d_rgb, d_dist, d_acc)]
+        rs = _cabi.RaysStruct(*[t.data_ptr() for t in rays_keep], ctx.num_rays)
+        _call(dev, "grid_render_backward", _cabi.lib().mipnerf_b200_grid_render_backward, C.byref(grid._struct()),
+              C.byref(rs), ctx.step, int(ctx.white_bkgd), *[None if t is None else t.data_ptr() for t in cot],
+              C.byref(gg))
+        return (None, None, None, None, *grads)
 
 
 @torch.no_grad()
@@ -260,3 +376,28 @@ def render_baked_frame(grid: BakedGrid, c2w, height: int = 800, width: int = 800
     counts = [(shard_rows(height, world, r)[1] - shard_rows(height, world, r)[0]) * width for r in range(world)]
     full = gather_rows(local, counts, group)
     return full[:, 0:3].reshape(height, width, 3), full[:, 3].reshape(height, width), full[:, 4].reshape(height, width)
+
+
+def finetune_grid(grid: BakedGrid, bank, steps: int, batch_size: int = 8192, lr_density: float = FINETUNE_LR_DENSITY,
+                  lr_sh: float = FINETUNE_LR_SH, white_bkgd: bool = True, step: Optional[float] = None,
+                  generator: Optional[torch.Generator] = None) -> List[float]:
+    """Fine-tune a baked grid's kept densities and SH rows against a `DeviceRayBank`'s pixels (PlenOctrees / SNeRG
+    style): per step a random batch, `grid.render`, the MSE against the targets, its backward through the grid ray
+    marcher, and one `FusedAdam` step (`lr_density` for the densities, `lr_sh` for the SH rows).  Makes the grid
+    trainable if it is not; returns the per-step losses."""
+    from .train import FusedAdam
+    grid.requires_grad_(True)
+    params = [p for p in grid.parameters() if p.numel()]  # a level without kept points has nothing to train
+    opt = FusedAdam([{"params": [p for p in params if p.dim() == 1], "lr": float(lr_density)},
+                     {"params": [p for p in params if p.dim() == 3], "lr": float(lr_sh)}])
+    losses = []
+    for _ in range(int(steps)):
+        rays, target = bank.sample(batch_size, generator)
+        rgb, _, _ = grid.render(rays, white_bkgd, step)
+        loss = torch.mean((rgb - target) ** 2)
+        for p in params:
+            p.grad = None
+        loss.backward()
+        opt.step()
+        losses.append(loss.detach())
+    return torch.stack(losses).tolist() if losses else []

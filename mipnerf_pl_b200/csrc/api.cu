@@ -145,6 +145,32 @@ int check_rays(const mipnerf_b200_rays* r) {
   return MIPNERF_B200_OK;
 }
 
+// The grid description of mipnerf_b200_grid_render and its backward (`g` checked non-NULL by the caller).
+int check_grid(const mipnerf_b200_grid* g) {
+  if (g->num_levels < 1 || g->num_levels > MIPNERF_B200_GRID_MAX_LEVELS)
+    return fail(MIPNERF_B200_EINVAL, "num_levels=%d: need 1..%d", g->num_levels, MIPNERF_B200_GRID_MAX_LEVELS);
+  if (g->degree < 0 || g->degree > 3) return fail(MIPNERF_B200_EINVAL, "degree=%d: need 0..3", g->degree);
+  const int scale = 1 << (g->num_levels - 1);
+  if (g->block < 1 || g->block % scale != 0)
+    return fail(MIPNERF_B200_EINVAL, "block=%d: need a positive multiple of 2^(num_levels - 1) = %d", g->block, scale);
+  if (!g->occupancy) return fail(MIPNERF_B200_EINVAL, "occupancy is NULL");
+  if (!std::isfinite(g->rgb_padding)) return fail(MIPNERF_B200_EINVAL, "rgb_padding=%g", g->rgb_padding);
+  for (int a = 0; a < 3; ++a)
+    if (!(g->hi[a] > g->lo[a]) || !std::isfinite(g->lo[a]) || !std::isfinite(g->hi[a]))
+      return fail(MIPNERF_B200_EINVAL, "bounds axis %d: [%g, %g], need lo < hi, finite", a, g->lo[a], g->hi[a]);
+  const int32_t* n0 = &g->levels[0].nx;
+  for (int l = 0; l < g->num_levels; ++l) {
+    const mipnerf_b200_grid_level& lv = g->levels[l];
+    if (!lv.cells) return fail(MIPNERF_B200_EINVAL, "level %d: cells is NULL", l);
+    const int32_t n[3] = {lv.nx, lv.ny, lv.nz};
+    for (int a = 0; a < 3; ++a)
+      if (n[a] < 2 || (int64_t)(n[a] - 1) << l != (int64_t)n0[a] - 1)
+        return fail(MIPNERF_B200_EINVAL, "level %d: %d x %d x %d points, need >= 2 per axis and (n_0 - 1) / 2^%d + 1",
+                    l, lv.nx, lv.ny, lv.nz, l);
+  }
+  return MIPNERF_B200_OK;
+}
+
 mipnerf_b200_rays offset_rays(const mipnerf_b200_rays& r, int64_t off, int64_t count) {
   mipnerf_b200_rays o = r;
   o.origins = r.origins + off * 3;
@@ -2038,28 +2064,26 @@ int mipnerf_b200_grid_render(const mipnerf_b200_grid* g, const mipnerf_b200_rays
   if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
   if (rays->num_rays > 0 && (!rgb || !distance || !acc)) return fail(MIPNERF_B200_EINVAL, "rgb / distance / acc is NULL");
   if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
-  if (g->num_levels < 1 || g->num_levels > MIPNERF_B200_GRID_MAX_LEVELS)
-    return fail(MIPNERF_B200_EINVAL, "num_levels=%d: need 1..%d", g->num_levels, MIPNERF_B200_GRID_MAX_LEVELS);
-  if (g->degree < 0 || g->degree > 3) return fail(MIPNERF_B200_EINVAL, "degree=%d: need 0..3", g->degree);
-  const int scale = 1 << (g->num_levels - 1);
-  if (g->block < 1 || g->block % scale != 0)
-    return fail(MIPNERF_B200_EINVAL, "block=%d: need a positive multiple of 2^(num_levels - 1) = %d", g->block, scale);
-  if (!g->occupancy) return fail(MIPNERF_B200_EINVAL, "occupancy is NULL");
-  if (!std::isfinite(g->rgb_padding)) return fail(MIPNERF_B200_EINVAL, "rgb_padding=%g", g->rgb_padding);
-  for (int a = 0; a < 3; ++a)
-    if (!(g->hi[a] > g->lo[a]) || !std::isfinite(g->lo[a]) || !std::isfinite(g->hi[a]))
-      return fail(MIPNERF_B200_EINVAL, "bounds axis %d: [%g, %g], need lo < hi, finite", a, g->lo[a], g->hi[a]);
-  const int32_t* n0 = &g->levels[0].nx;
-  for (int l = 0; l < g->num_levels; ++l) {
-    const mipnerf_b200_grid_level& lv = g->levels[l];
-    if (!lv.cells) return fail(MIPNERF_B200_EINVAL, "level %d: cells is NULL", l);
-    const int32_t n[3] = {lv.nx, lv.ny, lv.nz};
-    for (int a = 0; a < 3; ++a)
-      if (n[a] < 2 || (int64_t)(n[a] - 1) << l != (int64_t)n0[a] - 1)
-        return fail(MIPNERF_B200_EINVAL, "level %d: %d x %d x %d points, need >= 2 per axis and (n_0 - 1) / 2^%d + 1",
-                    l, lv.nx, lv.ny, lv.nz, l);
-  }
+  if ((rc = check_grid(g))) return rc;
   CUDA_TRY(mipnerf::launch_grid_render(*g, *rays, step, white_bkgd, rgb, distance, acc, (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_grid_render_backward(const mipnerf_b200_grid* g, const mipnerf_b200_rays* rays, float step,
+                                      int white_bkgd, const float* d_rgb, const float* d_distance, const float* d_acc,
+                                      const mipnerf_b200_grid_grads* grads, void* stream) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_rays(rays))) return rc;
+  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
+  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
+  if ((rc = check_grid(g))) return rc;
+  if (!grads) return fail(MIPNERF_B200_EINVAL, "grads is NULL");
+  for (int l = 0; l < g->num_levels; ++l)
+    if (g->levels[l].sh && (!grads->density[l] || !grads->sh[l]))
+      return fail(MIPNERF_B200_EINVAL, "level %d has kept points: grads->density[%d] / grads->sh[%d] is NULL", l, l, l);
+  CUDA_TRY(mipnerf::launch_grid_render_backward(*g, *rays, step, white_bkgd, d_rgb, d_distance, d_acc, *grads,
+                                                (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

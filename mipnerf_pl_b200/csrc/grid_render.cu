@@ -131,18 +131,23 @@ __device__ __forceinline__ void sh_basis(float x, float y, float z, float (&b)[1
   b[15] = -0.5900435899266435f * x * (xx - 3.f * yy);
 }
 
-template <int NC>
-__global__ void __launch_bounds__(kGridThreads)
-    grid_render_kernel(const GParams g, const mipnerf_b200_rays rays, float step, int white_bkgd,
-                       float* __restrict__ rgb_out, float* __restrict__ dist_out, float* __restrict__ acc_out) {
-  const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
-  if (r >= rays.num_rays) return;
+// One ray's sample lattice, clipped to the samples inside the bounds grown by a margin.
+struct RayMarch {
   float o[3], d[3];
+  float radius, near, far;
+  float dt, delta;
+  int64_t k0, k1;
+};
+
+__device__ __forceinline__ void ray_setup(const GParams& g, const mipnerf_b200_rays& rays, int64_t r, float step,
+                                          RayMarch& m, float (&y)[16]) {
 #pragma unroll
-  for (int a = 0; a < 3; ++a) o[a] = __ldg(rays.origins + 3 * r + a), d[a] = __ldg(rays.directions + 3 * r + a);
-  const float radius = __ldg(rays.radii + r), near = __ldg(rays.near + r), far = __ldg(rays.far + r);
-  float y[16];
+  for (int a = 0; a < 3; ++a) m.o[a] = __ldg(rays.origins + 3 * r + a), m.d[a] = __ldg(rays.directions + 3 * r + a);
+  m.radius = __ldg(rays.radii + r), m.near = __ldg(rays.near + r), m.far = __ldg(rays.far + r);
   sh_basis(__ldg(rays.viewdirs + 3 * r), __ldg(rays.viewdirs + 3 * r + 1), __ldg(rays.viewdirs + 3 * r + 2), y);
+  const float(&o)[3] = m.o;
+  const float(&d)[3] = m.d;
+  const float near = m.near, far = m.far;
 
   // the sample lattice, every operation rounded as the contract states
   const float dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
@@ -150,7 +155,8 @@ __global__ void __launch_bounds__(kGridThreads)
   const float kf = ceilf(__fdiv_rn(__fmul_rn(span, dn), step));
   const int64_t K = kf >= 1.f ? (int64_t)fminf(kf, 4e18f) : 1;
   const float dt = __fdiv_rn(span, (float)K);
-  const float delta = __fmul_rn(dt, dn);
+  m.dt = dt;
+  m.delta = __fmul_rn(dt, dn);
 
   // clip [0, K) to the samples inside the bounds grown by a margin: t_k increases with k only for dt > 0
   int64_t k0 = 0, k1 = K;
@@ -178,79 +184,224 @@ __global__ void __launch_bounds__(kGridThreads)
       k1 = first_past(t1, near, dt, k0, K);
     }
   }
+  m.k0 = k0, m.k1 = k1;
+}
 
-  const GLevel& l0 = g.lv[0];
-  float T = 1.f, acc = 0.f, dist = 0.f, cr = 0.f, cg = 0.f, cb = 0.f;
-  for (int64_t k = k0; k < k1;) {
-    const float t = sample_t(near, dt, k);
-    float x[3];
-    bool inside = true;
+// Sample k's t and position; whether the position is inside the bounds.
+__device__ __forceinline__ bool sample_at(const GParams& g, const RayMarch& m, int64_t k, float& t, float (&x)[3]) {
+  t = sample_t(m.near, m.dt, k);
+  bool inside = true;
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      x[a] = __fadd_rn(o[a], __fmul_rn(t, d[a]));
-      inside = inside && x[a] >= g.lo[a] && x[a] <= g.hi[a];
-    }
-    if (!inside) {
+  for (int a = 0; a < 3; ++a) {
+    x[a] = __fadd_rn(m.o[a], __fmul_rn(t, m.d[a]));
+    inside = inside && x[a] >= g.lo[a] && x[a] <= g.hi[a];
+  }
+  return inside;
+}
+
+// For dt > 0: if x lies in an empty macro cell, move k to the first sample past the cell's exit t (at least k + 1) and
+// return true.
+__device__ __forceinline__ bool skip_empty(const GParams& g, const RayMarch& m, const float (&x)[3], int64_t& k) {
+  const GLevel& l0 = g.lv[0];
+  int c[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const int i = (int)fminf(fmaxf((x[a] - g.lo[a]) * l0.inv_s[a], 0.f), (float)(l0.n[a] - 2));
+    c[a] = i / g.block;
+  }
+  if (__ldg(g.occ + ((int64_t)c[2] * g.on[1] + c[1]) * g.on[0] + c[0])) return false;
+  float t_exit = INFINITY;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    if (m.d[a] == 0.f) continue;
+    const int p = m.d[a] > 0.f ? min((c[a] + 1) * g.block, l0.n[a] - 1) : c[a] * g.block;
+    t_exit = fminf(t_exit, (g.lo[a] + (float)p * g.s0[a] - m.o[a]) / m.d[a]);
+  }
+  const int64_t next = first_past(t_exit, m.near, m.dt, k, m.k1);
+  k = next > k ? next : k + 1;
+  return true;
+}
+
+// The level(s) the cone footprint picks at a sample, with both levels' corner rows and weights.
+struct Blend {
+  int la;
+  float f;  // weight of level la + 1; level la has 1 - f (1 when f == 0, and level la + 1 is not read)
+  int row_a[8], row_b[8];
+  float w_a[8], w_b[8];
+};
+
+__device__ __forceinline__ float blend_density(const GParams& g, float radius, float t, const float (&x)[3], Blend& b) {
+  float lam = log2f(kSqrt3 * radius * t / g.s0_max);
+  lam = fminf(fmaxf(lam, 0.f), (float)(g.num_levels - 1));  // NaN -> 0
+  b.la = min((int)lam, g.num_levels - 1);
+  b.f = b.la == g.num_levels - 1 ? 0.f : lam - (float)b.la;
+  float sigma = level_density(g.lv[b.la], g.lo, x, b.row_a, b.w_a);
+  if (b.f > 0.f) sigma = (1.f - b.f) * sigma + b.f * level_density(g.lv[b.la + 1], g.lo, x, b.row_b, b.w_b);
+  return sigma;
+}
+
+// The blended raw colour Y . c of a sample.
+template <int NC>
+__device__ __forceinline__ void blend_raw(const GParams& g, const Blend& b, const float (&y)[16], float (&raw)[3]) {
+  raw[0] = raw[1] = raw[2] = 0.f;
+  level_color<NC>(g.lv[b.la].sh, b.row_a, b.w_a, y, b.f > 0.f ? 1.f - b.f : 1.f, raw);
+  if (b.f > 0.f) level_color<NC>(g.lv[b.la + 1].sh, b.row_b, b.w_b, y, b.f, raw);
+}
+
+// Front-to-back compositing state: transmittance and the running sums of the outputs.
+struct Composite {
+  float T = 1.f, acc = 0.f, dist = 0.f, c[3] = {0.f, 0.f, 0.f};
+};
+
+__device__ __forceinline__ void composite(Composite& s, float alpha, const float (&c)[3], float t) {
+  const float w = s.T * alpha;
+  s.c[0] += w * c[0], s.c[1] += w * c[1], s.c[2] += w * c[2];
+  s.acc += w;
+  s.dist += w * t;
+  s.T *= 1.f - alpha;
+}
+
+// The forward march of one ray: every sample with non-zero density composited, up to the one that leaves T < 1e-4.
+template <int NC>
+__device__ __forceinline__ void march(const GParams& g, const RayMarch& m, const float (&y)[16], Composite& s) {
+  for (int64_t k = m.k0; k < m.k1;) {
+    float t, x[3];
+    if (!sample_at(g, m, k, t, x)) {
       ++k;
       continue;
     }
-    if (dt > 0.f) {
-      int c[3];
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        const int i = (int)fminf(fmaxf((x[a] - g.lo[a]) * l0.inv_s[a], 0.f), (float)(l0.n[a] - 2));
-        c[a] = i / g.block;
-      }
-      if (!__ldg(g.occ + ((int64_t)c[2] * g.on[1] + c[1]) * g.on[0] + c[0])) {
-        float t_exit = INFINITY;
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-          if (d[a] == 0.f) continue;
-          const int p = d[a] > 0.f ? min((c[a] + 1) * g.block, l0.n[a] - 1) : c[a] * g.block;
-          t_exit = fminf(t_exit, (g.lo[a] + (float)p * g.s0[a] - o[a]) / d[a]);
-        }
-        const int64_t next = first_past(t_exit, near, dt, k, k1);
-        k = next > k ? next : k + 1;
-        continue;
-      }
-    }
-    float lam = log2f(kSqrt3 * radius * t / g.s0_max);
-    lam = fminf(fmaxf(lam, 0.f), (float)(g.num_levels - 1));  // NaN -> 0
-    const int la = min((int)lam, g.num_levels - 1);
-    const float f = la == g.num_levels - 1 ? 0.f : lam - (float)la;
-    int row_a[8], row_b[8];
-    float w_a[8], w_b[8];
-    float sigma = level_density(g.lv[la], g.lo, x, row_a, w_a);
-    if (f > 0.f) sigma = (1.f - f) * sigma + f * level_density(g.lv[la + 1], g.lo, x, row_b, w_b);
+    if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
+    Blend b;
+    const float sigma = blend_density(g, m.radius, t, x, b);
     ++k;
     if (!(sigma != 0.f)) continue;
-    const float alpha = 1.f - expf(-sigma * delta);
-    const float w = T * alpha;
-    float raw[3] = {0.f, 0.f, 0.f};
-    level_color<NC>(g.lv[la].sh, row_a, w_a, y, f > 0.f ? 1.f - f : 1.f, raw);
-    if (f > 0.f) level_color<NC>(g.lv[la + 1].sh, row_b, w_b, y, f, raw);
-    const float c0 = g.rgb_scale / (1.f + expf(-raw[0])) - g.rgb_padding;
-    const float c1 = g.rgb_scale / (1.f + expf(-raw[1])) - g.rgb_padding;
-    const float c2 = g.rgb_scale / (1.f + expf(-raw[2])) - g.rgb_padding;
-    cr += w * c0, cg += w * c1, cb += w * c2;
-    acc += w;
-    dist += w * t;
-    T *= 1.f - alpha;
-    if (T < kStopTransmittance) break;
+    const float alpha = 1.f - expf(-sigma * m.delta);
+    float raw[3], c[3];
+    blend_raw<NC>(g, b, y, raw);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) c[ch] = g.rgb_scale / (1.f + expf(-raw[ch])) - g.rgb_padding;
+    composite(s, alpha, c, t);
+    if (s.T < kStopTransmittance) break;
   }
-  const float bg = white_bkgd ? 1.f - acc : 0.f;
-  rgb_out[3 * r] = cr + bg;
-  rgb_out[3 * r + 1] = cg + bg;
-  rgb_out[3 * r + 2] = cb + bg;
-  acc_out[r] = acc;
-  dist_out[r] = fminf(fmaxf(dist, near), far);
 }
 
-}  // namespace
+template <int NC>
+__global__ void __launch_bounds__(kGridThreads)
+    grid_render_kernel(const GParams g, const mipnerf_b200_rays rays, float step, int white_bkgd,
+                       float* __restrict__ rgb_out, float* __restrict__ dist_out, float* __restrict__ acc_out) {
+  const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
+  if (r >= rays.num_rays) return;
+  RayMarch m;
+  float y[16];
+  ray_setup(g, rays, r, step, m, y);
+  Composite s;
+  march<NC>(g, m, y, s);
+  const float bg = white_bkgd ? 1.f - s.acc : 0.f;
+  rgb_out[3 * r] = s.c[0] + bg;
+  rgb_out[3 * r + 1] = s.c[1] + bg;
+  rgb_out[3 * r + 2] = s.c[2] + bg;
+  acc_out[r] = s.acc;
+  dist_out[r] = fminf(fmaxf(s.dist, m.near), m.far);
+}
 
-cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
-                               int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st) {
-  if (rays.num_rays == 0) return cudaSuccess;
+// Add one level's share of a sample's gradients into the kept corners: density with weight lw * wc, each SH
+// coefficient with lw * wc * Y_k (only when the colour has a gradient).
+template <int NC>
+__device__ __forceinline__ void level_scatter(float* __restrict__ gd, float* __restrict__ gsh, const int (&row)[8],
+                                              const float (&wc)[8], float lw, const float (&y)[16], float d_sigma,
+                                              const float (&d_raw)[3], bool color) {
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    if (row[c] < 0) continue;
+    const float w = lw * wc[c];
+    atomicAdd(gd + row[c], w * d_sigma);
+    if (!color) continue;
+    float* p = gsh + (int64_t)row[c] * (NC * 3);
+    const float a0 = w * d_raw[0], a1 = w * d_raw[1], a2 = w * d_raw[2];
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      atomicAdd(p + 3 * k, y[k] * a0);
+      atomicAdd(p + 3 * k + 1, y[k] * a1);
+      atomicAdd(p + 3 * k + 2, y[k] * a2);
+    }
+  }
+}
+
+__device__ __forceinline__ bool any_kept(const int (&row)[8]) {
+  bool any = false;
+#pragma unroll
+  for (int c = 0; c < 8; ++c) any = any || row[c] >= 0;
+  return any;
+}
+
+// The gradient of grid_render_kernel's outputs, one thread per ray.  Pass 1 is the forward march (its totals: the
+// foreground rgb, acc and the unclamped distance).  Pass 2 walks the same samples front to back with the same
+// compositing arithmetic, so the prefix sums it forms equal the totals bit for bit at the last composited sample.  With
+// e_k = g_rgb . c_k + g_acc' + g_dist t_k (g_acc' = g_acc - sum g_rgb under a white background) and w_k = T_k alpha_k,
+// dL/dsigma_k = delta (T_{k+1} e_k - sum_{j > k} w_j e_j), the suffix being total - prefix, and dL/draw_k = w_k g_rgb
+// (1 + 2 rgb_padding) s (1 - s) for s the sigmoid of the raw colour.
+template <int NC>
+__global__ void __launch_bounds__(kGridThreads)
+    grid_render_backward_kernel(const GParams g, const mipnerf_b200_rays rays, float step, int white_bkgd,
+                                const float* __restrict__ d_rgb, const float* __restrict__ d_dist,
+                                const float* __restrict__ d_acc,
+                                const __grid_constant__ mipnerf_b200_grid_grads grads) {
+  const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
+  if (r >= rays.num_rays) return;
+  float g_rgb[3] = {0.f, 0.f, 0.f};
+  if (d_rgb) g_rgb[0] = d_rgb[3 * r], g_rgb[1] = d_rgb[3 * r + 1], g_rgb[2] = d_rgb[3 * r + 2];
+  float g_acc = d_acc ? d_acc[r] : 0.f, g_dist = d_dist ? d_dist[r] : 0.f;
+  if (white_bkgd) g_acc -= g_rgb[0] + g_rgb[1] + g_rgb[2];
+  if (g_rgb[0] == 0.f && g_rgb[1] == 0.f && g_rgb[2] == 0.f && g_acc == 0.f && g_dist == 0.f) return;
+  RayMarch m;
+  float y[16];
+  ray_setup(g, rays, r, step, m, y);
+  Composite total;
+  march<NC>(g, m, y, total);
+  if (!(total.dist >= m.near && total.dist <= m.far)) g_dist = 0.f;  // the clamp passes the gradient inside, inclusive
+
+  Composite s;
+  for (int64_t k = m.k0; k < m.k1;) {
+    float t, x[3];
+    if (!sample_at(g, m, k, t, x)) {
+      ++k;
+      continue;
+    }
+    if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
+    Blend b;
+    const float sigma = blend_density(g, m.radius, t, x, b);
+    ++k;
+    // a zero density still has a gradient; it reaches parameters only through kept corners
+    const bool zero = !(sigma != 0.f);
+    if (zero && !any_kept(b.row_a) && !(b.f > 0.f && any_kept(b.row_b))) continue;
+    const float alpha = 1.f - expf(-sigma * m.delta);
+    float raw[3], c[3], sg[3];
+    blend_raw<NC>(g, b, y, raw);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+      sg[ch] = 1.f / (1.f + expf(-raw[ch]));
+      c[ch] = g.rgb_scale / (1.f + expf(-raw[ch])) - g.rgb_padding;
+    }
+    const float w = s.T * alpha;
+    if (!zero) composite(s, alpha, c, t);  // s.T is now T_{k+1}, the prefix sums include this sample
+    const float suffix = g_rgb[0] * (total.c[0] - s.c[0]) + g_rgb[1] * (total.c[1] - s.c[1]) +
+                         g_rgb[2] * (total.c[2] - s.c[2]) + g_acc * (total.acc - s.acc) +
+                         g_dist * (total.dist - s.dist);
+    const float e = g_rgb[0] * c[0] + g_rgb[1] * c[1] + g_rgb[2] * c[2] + g_acc + g_dist * t;
+    const float d_sigma = m.delta * (s.T * e - suffix);
+    float d_raw[3];
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) d_raw[ch] = w * g_rgb[ch] * g.rgb_scale * sg[ch] * (1.f - sg[ch]);
+    const bool color = !zero;  // w == 0 at a zero density
+    level_scatter<NC>(grads.density[b.la], grads.sh[b.la], b.row_a, b.w_a, b.f > 0.f ? 1.f - b.f : 1.f, y, d_sigma,
+                      d_raw, color);
+    if (b.f > 0.f)
+      level_scatter<NC>(grads.density[b.la + 1], grads.sh[b.la + 1], b.row_b, b.w_b, b.f, y, d_sigma, d_raw, color);
+    if (s.T < kStopTransmittance) break;
+  }
+}
+
+GParams make_params(const mipnerf_b200_grid& grid) {
   GParams g{};
   g.num_levels = grid.num_levels;
   g.nc = (grid.degree + 1) * (grid.degree + 1);
@@ -278,6 +429,15 @@ cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200
   g.rgb_padding = grid.rgb_padding;
   g.occ = grid.occupancy;
   g.block = grid.block;
+  return g;
+}
+
+}  // namespace
+
+cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
+                               int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st) {
+  if (rays.num_rays == 0) return cudaSuccess;
+  const GParams g = make_params(grid);
   const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
   LaunchScope scope(kKernGridRender, st);
   switch (grid.degree) {
@@ -286,6 +446,25 @@ cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200
     case 2: grid_render_kernel<9><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc); break;
     default: grid_render_kernel<16><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc);
   }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
+                                        int white_bkgd, const float* d_rgb, const float* d_distance,
+                                        const float* d_acc, const mipnerf_b200_grid_grads& grads, cudaStream_t st) {
+  if (rays.num_rays == 0 || (!d_rgb && !d_distance && !d_acc)) return cudaSuccess;
+  const GParams g = make_params(grid);
+  const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
+  LaunchScope scope(kKernGridRenderBackward, st);
+#define MIPNERF_GRID_BWD(NC) \
+  grid_render_backward_kernel<NC><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, d_rgb, d_distance, d_acc, grads)
+  switch (grid.degree) {
+    case 0: MIPNERF_GRID_BWD(1); break;
+    case 1: MIPNERF_GRID_BWD(4); break;
+    case 2: MIPNERF_GRID_BWD(9); break;
+    default: MIPNERF_GRID_BWD(16);
+  }
+#undef MIPNERF_GRID_BWD
   return cudaGetLastError();
 }
 

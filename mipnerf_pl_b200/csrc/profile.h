@@ -33,6 +33,7 @@ enum KernelId : int {
   kKernRadianceTc,   // radiance mode of the wgmma level kernel (IPE + per-point view term + the whole MLP)
   kKernRadianceDirsTc,  // view-accumulator mode of the wgmma level kernel (IPE + the MLP up to the view layer's GEMM)
   kKernRadiancePairs,   // per-(point, direction) view layer + colour head (+ projection) of a shared direction set
+  kKernGridRenderBackward,  // gradient of the baked-grid ray marcher with respect to the densities and SH rows
   kKernGridRender,      // ray marching through a baked density + SH grid
   kKernCount
 };
