@@ -438,45 +438,98 @@ struct TrainScratch {
 constexpr int kTrainImages = 2 * kMaxTrainDepth + 8;
 constexpr size_t kTrainImageBytes = 131072;  // 256 x 256 x 16 bit
 
-TrainScratch carve_train(const mipnerf_b200_config* c, const Dims& d, int64_t rays, void* base) {
+// Per-layer scratch of m rows: a training chunk of `rays` rays, or (rays = 0) the fp32 query backward's points, one view
+// encoding each.  The images come last: they are packed once per call into the first chunk's carve.
+TrainScratch carve_train(const mipnerf_b200_config* c, const Dims& d, size_t m, int64_t rays, bool radiance, void* base) {
   TrainScratch s{};
-  const size_t m = (size_t)rays * c->num_samples;
   Carver cv{base};
   s.enc = cv.floats(m * d.xyz_dim);
-  s.venc = cv.floats((size_t)rays * d.view_dim);
   for (int i = 0; i < c->net_depth; ++i) s.h[i] = cv.floats(m * c->net_width);
-  s.bott = cv.floats(m * c->net_width);
-  s.v = cv.floats(m * c->net_width_condition);
-  s.raw_rgb = cv.floats(m * 3);
   s.raw_density = cv.floats(m);
   s.d_a = cv.floats(m * c->net_width);
   s.d_b = cv.floats(m * c->net_width);
-  s.d_v = cv.floats(m * c->net_width_condition);
-  s.d_raw_rgb = cv.floats(m * 3);
   s.d_raw_density = cv.floats(m);
   s.part = cv.floats(wgrad_part_floats(c, d));
-  for (int i = 0; i < 2; ++i) {
-    s.t[i] = cv.floats((size_t)rays * (c->num_samples + 1));
-    s.w[i] = cv.floats(m);
+  if (radiance) {
+    s.venc = cv.floats((rays ? rays : m) * d.view_dim);
+    s.bott = cv.floats(m * c->net_width);
+    s.v = cv.floats(m * c->net_width_condition);
+    s.raw_rgb = cv.floats(m * 3);
+    s.d_v = cv.floats(m * c->net_width_condition);
+    s.d_raw_rgb = cv.floats(m * 3);
   }
-  s.vrow = cv.floats((size_t)rays * c->net_width_condition);
-  s.images = cv.bytes(kTrainImages * kTrainImageBytes);
+  if (rays) {
+    for (int i = 0; i < 2; ++i) {
+      s.t[i] = cv.floats((size_t)rays * (c->num_samples + 1));
+      s.w[i] = cv.floats(m);
+    }
+    s.vrow = cv.floats((size_t)rays * c->net_width_condition);
+    s.images = cv.bytes(kTrainImages * kTrainImageBytes);
+  }
   s.bytes = cv.off;
   return s;
 }
 
+// The chunk-invariant head of the fused backward drivers' workspace: the wgrad partials, `image_slots` slots for the
+// dgrad chain's B images and the level kernels' packed weights.  Carved first: the weights are packed once per call
+// into the first chunk's carve and read by every chunk, so no buffer of a shorter last chunk may move onto them.
+struct FusedHead {
+  float* part;
+  uint8_t *images, *packed;
+};
+
+FusedHead carve_fused_head(Carver& cv, const mipnerf_b200_config* c, const Dims& d, int precision, int image_slots) {
+  FusedHead h;
+  h.part = cv.floats(wgrad_part_floats(c, d));
+  h.images = cv.bytes((size_t)image_slots * kTrainImageBytes);
+  h.packed = cv.bytes(mipnerf::tc_packed_bytes(c, precision));
+  return h;
+}
+
+// Operands of the tile-image backward chain for `rows` rows in whole 128-row tiles: the level kernel's dump (act
+// [9][tiles][64 KB]: h_0..h_7, bottleneck; v [tiles][32 KB]: view-layer output) and the head's wgrad partials, set by
+// the caller; the IPE features enc16 [tiles][32 KB], the fp32 view encoding (one row per view_div rows), d raw_rgb /
+// d raw_density, the ReLU sign mask relu_bits [tiles * 128][32 B] and the gradient images.  bf16x3: each image, its lo.
+struct TileChainOps {
+  uint8_t *act, *v;
+  float* part;
+  uint8_t* enc16;
+  float* venc;
+  int view_div;
+  float *d_raw_rgb, *d_raw_density;
+  uint8_t *d_v, *d_a, *d_b, *relu_bits;
+  int64_t rows, tiles;
+};
+
+// The chain's own operands for `rows` rows; without `radiance` (a density query) no view encoding, d raw_rgb or d_v.
+TileChainOps carve_tile_chain(Carver& cv, const Dims& d, int precision, int64_t rows, int view_div, bool radiance) {
+  TileChainOps o{};
+  o.rows = rows;
+  o.tiles = (rows + 127) / 128;
+  o.view_div = view_div;
+  const size_t x = mipnerf::is_x3(precision) ? 2 : 1, m = o.tiles * 128;  // tile images per operand: hi (, lo)
+  if (radiance) {
+    o.venc = cv.floats(m / view_div * d.view_dim);
+    o.d_raw_rgb = cv.floats(m * 3);
+    o.d_v = cv.bytes(x * o.tiles * 32768);
+  }
+  o.d_raw_density = cv.floats(m);
+  o.enc16 = cv.bytes(x * o.tiles * 32768);
+  o.relu_bits = cv.bytes(m * 32);
+  o.d_a = cv.bytes(x * o.tiles * 65536);
+  o.d_b = cv.bytes(x * o.tiles * 65536);
+  return o;
+}
+
 // Scratch of the fused tensor-core training step (forward = the level kernels with the activation dump, backward on
-// 16-bit tile images, train_t16.cu).  Overlays the same workspace as TrainScratch.
+// 16-bit tile images, train_t16.cu), one tile per ray.  Overlays the same workspace as TrainScratch.
 struct FusedScratch {
-  // bf16x3: every tile image below is followed by its lo image of the same size (act: [2][9][rays][64 KB]), and the
-  // images carve holds the lo images of the dgrad B operands as well
-  uint8_t *act[2], *v[2];                // forward dump per level: [9][rays][64 KB], [rays][32 KB]
-  float *raw_rgb[2], *raw_density[2];    // raw heads per level
-  float *enc, *venc, *d_raw_rgb, *d_raw_density, *part, *t[2], *w[2];
-  uint8_t *enc16;                        // the IPE features as a tile image [rays][2 slabs] (96 columns + zero padding)
-  uint8_t *relu_bits;                    // [m][32 B]: sign mask of the layer input the current wgrad streams
-  uint8_t *d_v, *d_a, *d_b;              // gradient tile images: [rays][32 KB], [rays][64 KB] x 2
-  uint8_t *images, *packed, *tcws;
+  FusedHead head;
+  // bf16x3: every tile image below is followed by its lo image of the same size (act: [2][9][rays][64 KB])
+  uint8_t *act[2], *v[2];              // forward dump per level: [9][rays][64 KB], [rays][32 KB]
+  float *raw_rgb[2], *raw_density[2], *t[2], *w[2];  // raw heads, fenceposts and weights per level
+  TileChainOps chain;
+  uint8_t* tcws;
   size_t tcws_bytes, bytes;
 };
 
@@ -485,11 +538,8 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
   const size_t m = (size_t)rays * c->num_samples;
   Carver cv{base};
   const size_t x = precision == MIPNERF_B200_BF16X3 ? 2 : 1;  // tile images per operand: hi (, lo)
-  // chunk-invariant buffers first: the weight images are packed once per call into the first chunk's carve and read
-  // by every chunk, so no per-ray buffer of a shorter last chunk may move onto them
-  s.part = cv.floats(wgrad_part_floats(c, d));
-  s.images = cv.bytes((size_t)kTrainImages * kTrainImageBytes);
-  s.packed = cv.bytes(mipnerf::tc_packed_bytes(c, precision));
+  // bf16x3: the image slots hold the lo images of the dgrad B operands as well
+  s.head = carve_fused_head(cv, c, d, precision, kTrainImages);
   for (int l = 0; l < 2; ++l) {
     s.act[l] = cv.bytes(x * 9 * rays * 65536);
     s.v[l] = cv.bytes(x * rays * 32768);
@@ -498,15 +548,9 @@ FusedScratch carve_fused(const mipnerf_b200_config* c, const Dims& d, int64_t ra
     s.t[l] = cv.floats((size_t)rays * (c->num_samples + 1));
     s.w[l] = cv.floats(m);
   }
-  s.enc = cv.floats(m * d.xyz_dim);
-  s.venc = cv.floats((size_t)rays * d.view_dim);
-  s.d_raw_rgb = cv.floats(m * 3);
-  s.d_raw_density = cv.floats(m);
-  s.enc16 = cv.bytes(x * rays * 32768);
-  s.relu_bits = cv.bytes(m * 32);
-  s.d_v = cv.bytes(x * rays * 32768);
-  s.d_a = cv.bytes(x * rays * 65536);
-  s.d_b = cv.bytes(x * rays * 65536);
+  cv.floats(m * d.xyz_dim);  // unread; keeps the size mipnerf_b200_train_workspace_bytes_for has always returned
+  s.chain = carve_tile_chain(cv, d, precision, m, c->num_samples, true);
+  s.chain.part = s.head.part;
   s.tcws_bytes = mipnerf::tc_workspace_bytes(c, rays, precision);
   s.tcws = cv.bytes(s.tcws_bytes);
   s.bytes = cv.off;
@@ -590,6 +634,17 @@ bool train_tc_supported(const mipnerf_b200_config* c, const Dims& d) {
   LayerImages im;
   pack_layer_images(c, d, nullptr, MIPNERF_B200_BF16, true, nullptr, &im, nullptr);
   return im.slots <= kTrainImages;
+}
+
+// The fused drivers' prologue, once per call (the weights change every optimiser step): the level kernels' image and
+// the dgrad chain's transposed B operands (*im) packed into the head `h`; *wl: the weights with that packed image.
+int pack_fused_weights(const mipnerf_b200_config* c, const Dims& d, const mipnerf_b200_weights* w, int precision,
+                       const FusedHead& h, mipnerf_b200_weights* wl, LayerImages* im, cudaStream_t st) {
+  *wl = *w;
+  wl->packed = h.packed, wl->packed_precision = precision, wl->packed_bytes = mipnerf::tc_packed_bytes(c, precision);
+  CUDA_TRY(mipnerf::tc_pack_weights(c, w, precision, h.packed, st));
+  CUDA_TRY(pack_layer_images(c, d, w, precision, false, h.images, im, st));
+  return MIPNERF_B200_OK;
 }
 
 // The gradient outputs of a backward pass: touched[i] (grads[i] already holds a sum to add to) starts at `accumulate`,
@@ -819,7 +874,7 @@ size_t mipnerf_b200_train_workspace_bytes_for(const mipnerf_b200_config* cfg, in
   if (precision != MIPNERF_B200_FP32 && precision != MIPNERF_B200_BF16 && precision != MIPNERF_B200_FP16) return 0;
   if (precision != MIPNERF_B200_FP32 && !train_tc_supported(cfg, d)) return 0;  // forward_backward refuses it
   const int64_t r = std::clamp<int64_t>(num_rays, 1, kChunkRaysFp32);
-  size_t bytes = carve_train(cfg, d, r, nullptr).bytes;
+  size_t bytes = carve_train(cfg, d, r * cfg->num_samples, r, true, nullptr).bytes;
   if (train_fused_supported(cfg, precision))  // the fused tensor-core step overlays the same buffer
     bytes = std::max(bytes, carve_fused(cfg, d, r, precision, nullptr).bytes);
   return bytes;
@@ -834,20 +889,6 @@ size_t mipnerf_b200_train_workspace_bytes(const mipnerf_b200_config* cfg, int64_
   }
   return bytes;
 }
-
-// Operands of the tile-image backward chain for one chunk of `tiles` 128-row tiles: the forward's dump of the level
-// kernel (act [9][tiles][64 KB]: h_0..h_7, bottleneck; v [tiles][32 KB]: view-layer output), the IPE features enc16
-// [tiles][32 KB], the fp32 view encoding (one row per view_div rows), d raw_rgb / d raw_density [tiles * 128] and the
-// gradient tile images.  bf16x3: every image is followed by its lo image, `tiles` images further on.
-struct TileChainOps {
-  const uint8_t *act, *v, *enc16;
-  const float* venc;
-  int view_div;
-  const float *d_raw_rgb, *d_raw_density;
-  uint8_t *d_v, *d_a, *d_b, *relu_bits;
-  float* part;
-  int64_t tiles;
-};
 
 // The per-level backward chain of the fused training step, on 16-bit tile images: colour head, view layer, bottleneck
 // + density head, trunk, into `grads` (touched[i]: grads[i] already holds a sum to add to; inv_gscale takes the fp16
@@ -864,6 +905,14 @@ int tile_backward_chain(const mipnerf_b200_config* cfg, const Dims& d, const mip
   const int64_t m = o.tiles * 128;
   const mipnerf_b200_linear& dl = w->linears[depth];
   const mipnerf_b200_linear& cl = w->linears[d.n_lin - 1];
+  // the rows of a query's last tile past its last point (view_div 1) take no cotangent and a zero view encoding
+  if (o.rows < m) {
+    CUDA_TRY(cudaMemsetAsync(o.d_raw_density + o.rows, 0, (size_t)(m - o.rows) * 4, st));
+    if (!density_only) {
+      CUDA_TRY(cudaMemsetAsync(o.d_raw_rgb + o.rows * 3, 0, (size_t)(m - o.rows) * 12, st));
+      CUDA_TRY(cudaMemsetAsync(o.venc + o.rows * d.view_dim, 0, (size_t)(m - o.rows) * d.view_dim * 4, st));
+    }
+  }
   // MIPNERF_B200_TRAIN_MASKBITS=0: the dgrad GEMMs read the ReLU mask from the activation tile images again (A/B)
   const char* bits_env = getenv("MIPNERF_B200_TRAIN_MASKBITS");
   const bool use_bits = !(bits_env && bits_env[0] == '0');
@@ -949,20 +998,19 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
   const bool x3 = mipnerf::is_x3(precision);
   const int fmt = mipnerf::fmt_of(precision);
   const int64_t chunk = x3 ? kChunkRaysX3 : kChunkRaysFp32;
-  const FusedScratch s0 = carve_fused(cfg, d, B < chunk ? B : chunk, precision, workspace);
-  // ---- once per call (the weights change every optimiser step): the level kernels' packed image, and the
-  //      transposed B operands of the dgrad chain
-  mipnerf_b200_weights wl = *w;
-  wl.packed = s0.packed;
-  CUDA_TRY(mipnerf::tc_pack_weights(cfg, w, precision, s0.packed, st));
+  mipnerf_b200_weights wl;
   LayerImages im;
-  CUDA_TRY(pack_layer_images(cfg, d, w, precision, false, s0.images, &im, st));
+  int rc;
+  if ((rc = pack_fused_weights(cfg, d, w, precision, carve_fused(cfg, d, std::min(B, chunk), precision, workspace).head,
+                               &wl, &im, st)))
+    return rc;
   const float gscale = grad_scale_of(precision), inv_gscale = 1.f / gscale;
   for (int64_t off = 0; off < B; off += chunk) {
     const int64_t cnt = (B - off) < chunk ? (B - off) : chunk;
     const mipnerf_b200_rays rc_ = offset_rays(*rays, off, cnt);
     const FusedScratch s = carve_fused(cfg, d, cnt, precision, workspace);
-    CUDA_TRY(mipnerf::launch_pos_enc(rc_.viewdirs, s.venc, cnt, 0, cfg->deg_view, 1, st));
+    TileChainOps ops = s.chain;
+    CUDA_TRY(mipnerf::launch_pos_enc(rc_.viewdirs, ops.venc, cnt, 0, cfg->deg_view, 1, st));
     // ---- forward of all levels: two launches, everything the backward needs is left behind as tile images
     mipnerf_b200_level_out lo[2];
     mipnerf::TcTrainDump dump{};
@@ -978,13 +1026,11 @@ static int forward_backward_fused(const mipnerf_b200_config* cfg, const Dims& d,
       // the IPE features again (operand of two wgrads; the level kernel keeps its own 16-bit copy on chip), written
       // straight into a tile image so that those wgrads stage them by bulk copy like every other operand
       CUDA_TRY(mipnerf::launch_ipe_t16(rc_.origins, rc_.directions, rc_.radii, t_cur,
-                                       mipnerf::tile_pair(s.enc16, cnt, 128, x3), cnt, n, cfg->disable_integration,
+                                       mipnerf::tile_pair(ops.enc16, cnt, 128, x3), cnt, n, cfg->disable_integration,
                                        fmt, st));
       CUDA_TRY(launch_grad_source(src, cfg, l, off, B, cnt, s.raw_rgb[l], s.raw_density[l], t_cur, rc_.directions,
-                                  white_bkgd, rgb_scale, gscale, s.d_raw_rgb, s.d_raw_density, st));
-      const TileChainOps ops{s.act[l], s.v[l], s.enc16, s.venc, n, s.d_raw_rgb, s.d_raw_density,
-                             s.d_v, s.d_a, s.d_b, s.relu_bits, s.part, cnt};
-      int rc;
+                                  white_bkgd, rgb_scale, gscale, ops.d_raw_rgb, ops.d_raw_density, st));
+      ops.act = s.act[l], ops.v = s.v[l];
       if ((rc = tile_backward_chain(cfg, d, w, precision, im, ops, false, inv_gscale, grads, touched, st))) return rc;
     }
   }
@@ -1055,15 +1101,17 @@ static int forward_backward_impl(const mipnerf_b200_config* cfg, const mipnerf_b
   }
   // ---- tensor-core mode: B operands of every forward / dgrad GEMM, packed once per call
   LayerImages im{};
-  if (tc && B > 0)
-    CUDA_TRY(pack_layer_images(cfg, d, w, precision, true,
-                               carve_train(cfg, d, std::min(B, kChunkRaysFp32), workspace).images, &im, st));
+  if (tc && B > 0) {
+    const int64_t r = std::min(B, kChunkRaysFp32);
+    CUDA_TRY(pack_layer_images(cfg, d, w, precision, true, carve_train(cfg, d, r * n, r, true, workspace).images, &im,
+                               st));
+  }
 
   for (int64_t off = 0; off < B; off += kChunkRaysFp32) {
     const int64_t cnt = (B - off) < kChunkRaysFp32 ? (B - off) : kChunkRaysFp32;
     const int64_t m = cnt * n;
     const mipnerf_b200_rays rc_ = offset_rays(*rays, off, cnt);
-    const TrainScratch s = carve_train(cfg, d, cnt, workspace);
+    const TrainScratch s = carve_train(cfg, d, m, cnt, true, workspace);
     CUDA_TRY(mipnerf::launch_pos_enc(rc_.viewdirs, s.venc, cnt, 0, cfg->deg_view, 1, st));
     if (tc) {
       const mipnerf_b200_linear& vl0 = w->linears[depth + 2];
@@ -1807,68 +1855,29 @@ int mipnerf_b200_query_radiance_dirs(const mipnerf_b200_config* cfg, const mipne
 }
 
 namespace {
-// Scratch of the fp32 query backward for one chunk of m points: the training step's activation layout (TrainScratch
-// with one row per point, view encoding included) without its per-ray buffers, and the zero covariances.
-struct QueryGradScratch {
-  TrainScratch t;
-  float* zero_covs;
-  size_t bytes;
-};
-QueryGradScratch carve_query_grad(const mipnerf_b200_config* c, const Dims& d, int64_t m, bool radiance, void* base) {
-  QueryGradScratch s{};
-  Carver cv{base};
-  s.t.part = cv.floats(wgrad_part_floats(c, d));
-  s.zero_covs = cv.floats((size_t)m * 3);
-  s.t.enc = cv.floats((size_t)m * d.xyz_dim);
-  for (int i = 0; i < c->net_depth; ++i) s.t.h[i] = cv.floats((size_t)m * c->net_width);
-  s.t.raw_density = cv.floats((size_t)m);
-  s.t.d_raw_density = cv.floats((size_t)m);
-  s.t.d_a = cv.floats((size_t)m * c->net_width);
-  s.t.d_b = cv.floats((size_t)m * c->net_width);
-  if (radiance) {
-    s.t.venc = cv.floats((size_t)m * d.view_dim);
-    s.t.bott = cv.floats((size_t)m * c->net_width);
-    s.t.v = cv.floats((size_t)m * c->net_width_condition);
-    s.t.raw_rgb = cv.floats((size_t)m * 3);
-    s.t.d_v = cv.floats((size_t)m * c->net_width_condition);
-    s.t.d_raw_rgb = cv.floats((size_t)m * 3);
-  }
-  s.bytes = cv.off;
-  return s;
-}
-
-// Scratch of the bf16 query backward for one chunk of m points, T = ceil(m / 128) tiles: the level kernel's query dump
-// (act: h_0..h_7 and, radiance, the bottleneck; v), the raw heads, the IPE tile image, the fp32 view encoding and the
-// gradient tile images of the fused step's chain, all over whole tiles (rows past m: zero cotangents).
+// Scratch of the bf16 query backward for one chunk of m points: the fused step's chain over whole tiles, its act / v
+// the level kernel's query dump (h_0..h_7 and, radiance, the bottleneck; the view layer), and the raw heads.
 struct QueryFusedScratch {
-  uint8_t *images, *packed, *act, *v, *enc16, *relu_bits, *d_v, *d_a, *d_b;
-  float *part, *slots, *raw_rgb, *raw_density, *venc, *d_raw_rgb, *d_raw_density;
+  FusedHead head;
+  float* slots;  // radiance mode's view-direction terms, chunk-invariant too
+  float *raw_rgb, *raw_density;
+  TileChainOps chain;
   size_t slots_bytes, bytes;
 };
 QueryFusedScratch carve_query_fused(const mipnerf_b200_config* c, const Dims& d, int64_t m, bool radiance,
                                     void* base) {
   QueryFusedScratch s{};
   Carver cv{base};
-  const int64_t tiles = (m + 127) / 128, rows = tiles * 128;
-  // chunk-invariant buffers first: the weight images are packed once per call into the first chunk's carve
-  s.part = cv.floats(wgrad_part_floats(c, d));
-  s.images = cv.bytes((size_t)(kMaxTrainDepth + 2) * kTrainImageBytes);
-  s.packed = cv.bytes(mipnerf::tc_packed_bytes(c, MIPNERF_B200_BF16));
+  s.head = carve_fused_head(cv, c, d, MIPNERF_B200_BF16, kMaxTrainDepth + 2);
   s.slots_bytes = radiance ? mipnerf::tc_radiance_workspace_bytes(mipnerf::kDensityChunkPoints) : 0;
   s.slots = reinterpret_cast<float*>(cv.bytes(s.slots_bytes));
-  s.act = cv.bytes((size_t)(radiance ? 9 : 8) * tiles * 65536);
-  s.raw_density = cv.floats((size_t)rows);
-  s.d_raw_density = cv.floats((size_t)rows);
-  s.enc16 = cv.bytes((size_t)tiles * 32768);
-  s.relu_bits = cv.bytes((size_t)rows * 32);
-  s.d_a = cv.bytes((size_t)tiles * 65536);
-  s.d_b = cv.bytes((size_t)tiles * 65536);
+  s.chain = carve_tile_chain(cv, d, MIPNERF_B200_BF16, m, 1, radiance);
+  s.chain.part = s.head.part;
+  s.chain.act = cv.bytes((size_t)(radiance ? 9 : 8) * s.chain.tiles * 65536);
+  s.raw_density = cv.floats((size_t)s.chain.tiles * 128);
   if (radiance) {
-    s.v = cv.bytes((size_t)tiles * 32768);
-    s.raw_rgb = cv.floats((size_t)rows * 3);
-    s.d_raw_rgb = cv.floats((size_t)rows * 3);
-    s.venc = cv.floats((size_t)rows * d.view_dim);
-    s.d_v = cv.bytes((size_t)tiles * 32768);
+    s.chain.v = cv.bytes((size_t)s.chain.tiles * 32768);
+    s.raw_rgb = cv.floats((size_t)s.chain.tiles * 128 * 3);
   }
   s.bytes = cv.off;
   return s;
@@ -1902,16 +1911,16 @@ int query_backward_fp32(const mipnerf_b200_config* cfg, const Dims& d, const mip
   int rc;
   for (int64_t off = 0; off < num_points; off += kChunkPointsFp32) {
     const int64_t m = std::min(num_points - off, kChunkPointsFp32);
-    const QueryGradScratch s = carve_query_grad(cfg, d, m, radiance, workspace);
+    const TrainScratch s = carve_train(cfg, d, m, 0, radiance, workspace);
+    float* zero_covs = Carver{workspace, s.bytes}.floats((size_t)m * 3);
     // the forward of the query (models/mip.py:322-363, models/mip_nerf.py:75-111), every activation kept
-    if ((rc = query_ipe_fp32(cfg, means, covs, off, m, s.zero_covs, s.t.enc, st))) return rc;
-    if (radiance) CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, s.t.venc, m, 0, cfg->deg_view, 1, st));
-    if ((rc = mlp_forward_kept(cfg, d, w, false, MIPNERF_B200_FP32, im, s.t, m, 1, !radiance, st))) return rc;
+    if ((rc = query_ipe_fp32(cfg, means, covs, off, m, zero_covs, s.enc, st))) return rc;
+    if (radiance) CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, s.venc, m, 0, cfg->deg_view, 1, st));
+    if ((rc = mlp_forward_kept(cfg, d, w, false, MIPNERF_B200_FP32, im, s, m, 1, !radiance, st))) return rc;
     // the activations' VJP, then the training step's per-layer chain
-    CUDA_TRY(mipnerf::launch_query_activation_vjp(s.t.raw_rgb, s.t.raw_density, chunk_cot(cot, off, radiance),
-                                                  cfg->density_bias, rgb_scale, radiance ? s.t.d_raw_rgb : nullptr,
-                                                  s.t.d_raw_density, m, st));
-    if ((rc = mlp_backward_chain(cfg, d, w, false, MIPNERF_B200_FP32, im, s.t, m, 1, !radiance, grads, touched, st)))
+    CUDA_TRY(mipnerf::launch_query_activation_vjp(s.raw_rgb, s.raw_density, chunk_cot(cot, off, radiance),
+                                                  cfg->density_bias, rgb_scale, s.d_raw_rgb, s.d_raw_density, m, st));
+    if ((rc = mlp_backward_chain(cfg, d, w, false, MIPNERF_B200_FP32, im, s, m, 1, !radiance, grads, touched, st)))
       return rc;
   }
   return MIPNERF_B200_OK;
@@ -1927,41 +1936,30 @@ int query_backward_bf16(const mipnerf_b200_config* cfg, const Dims& d, const mip
   const int prec = MIPNERF_B200_BF16;
   const float rgb_scale = mipnerf::rgb_scale_of(cfg);
   const int64_t chunk = mipnerf::kDensityChunkPoints;
-  const QueryFusedScratch s0 = carve_query_fused(cfg, d, std::min(num_points, chunk), radiance, workspace);
-  mipnerf_b200_weights wl = *w;
-  wl.packed = s0.packed, wl.packed_precision = prec, wl.packed_bytes = mipnerf::tc_packed_bytes(cfg, prec);
-  CUDA_TRY(mipnerf::tc_pack_weights(cfg, w, prec, s0.packed, st));
+  mipnerf_b200_weights wl;
   LayerImages im;
-  CUDA_TRY(pack_layer_images(cfg, d, w, prec, false, s0.images, &im, st));
   int rc;
+  if ((rc = pack_fused_weights(cfg, d, w, prec,
+                               carve_query_fused(cfg, d, std::min(num_points, chunk), radiance, workspace).head, &wl,
+                               &im, st)))
+    return rc;
   for (int64_t off = 0; off < num_points; off += chunk) {
     const int64_t m = std::min(num_points - off, chunk);
-    const int64_t tiles = (m + 127) / 128, rows = tiles * 128;
     const QueryFusedScratch s = carve_query_fused(cfg, d, m, radiance, workspace);
+    const TileChainOps& o = s.chain;
     const float* mp = means + off * 3;
     const float* cv = covs ? covs + off * 3 : nullptr;
-    const mipnerf::TcQueryDump dump{s.act, s.v};
+    const mipnerf::TcQueryDump dump{o.act, o.v};
     cudaError_t e = radiance ? mipnerf::tc_query_radiance(cfg, &wl, mp, cv, viewdirs + off * 3, m, prec, s.raw_rgb,
-                                                          s.raw_density, nullptr, nullptr, s0.slots, s0.slots_bytes, st,
+                                                          s.raw_density, nullptr, nullptr, s.slots, s.slots_bytes, st,
                                                           &dump)
                              : mipnerf::tc_query_density(cfg, &wl, mp, cv, m, prec, s.raw_density, nullptr, st, &dump);
     if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "query backward, forward: %s", cudaGetErrorString(e));
-    CUDA_TRY(mipnerf::launch_ipe_points_t16(mp, cv, s.enc16, m, cfg->disable_integration, prec, st));
-    if (radiance) {
-      CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, s.venc, m, 0, cfg->deg_view, 1, st));
-      if (rows > m) CUDA_TRY(cudaMemsetAsync(s.venc + m * d.view_dim, 0, (size_t)(rows - m) * d.view_dim * 4, st));
-    }
-    // the activations' VJP; the rows of the last tile past the last point take no cotangent
+    CUDA_TRY(mipnerf::launch_ipe_points_t16(mp, cv, o.enc16, m, cfg->disable_integration, prec, st));
+    if (radiance) CUDA_TRY(mipnerf::launch_pos_enc(viewdirs + off * 3, o.venc, m, 0, cfg->deg_view, 1, st));
     CUDA_TRY(mipnerf::launch_query_activation_vjp(s.raw_rgb, s.raw_density, chunk_cot(cot, off, radiance),
-                                                  cfg->density_bias, rgb_scale, radiance ? s.d_raw_rgb : nullptr,
-                                                  s.d_raw_density, m, st));
-    if (rows > m) {
-      CUDA_TRY(cudaMemsetAsync(s.d_raw_density + m, 0, (size_t)(rows - m) * 4, st));
-      if (radiance) CUDA_TRY(cudaMemsetAsync(s.d_raw_rgb + m * 3, 0, (size_t)(rows - m) * 12, st));
-    }
-    const TileChainOps ops{s.act, s.v, s.enc16, s.venc, 1, s.d_raw_rgb, s.d_raw_density,
-                           s.d_v, s.d_a, s.d_b, s.relu_bits, s0.part, tiles};
-    if ((rc = tile_backward_chain(cfg, d, w, prec, im, ops, !radiance, 1.f, grads, touched, st))) return rc;
+                                                  cfg->density_bias, rgb_scale, o.d_raw_rgb, o.d_raw_density, m, st));
+    if ((rc = tile_backward_chain(cfg, d, w, prec, im, o, !radiance, 1.f, grads, touched, st))) return rc;
   }
   return MIPNERF_B200_OK;
 }
@@ -1973,7 +1971,7 @@ size_t mipnerf_b200_query_backward_workspace_bytes(const mipnerf_b200_config* cf
   if (check_config(cfg, &d) != MIPNERF_B200_OK || num_points < 0 || !query_grad_supported(cfg, d, precision)) return 0;
   const int64_t m = std::clamp<int64_t>(num_points, 1, kChunkPointsFp32);
   if (precision == MIPNERF_B200_BF16) return carve_query_fused(cfg, d, m, radiance != 0, nullptr).bytes;
-  return carve_query_grad(cfg, d, m, radiance != 0, nullptr).bytes;
+  return carve_train(cfg, d, m, 0, radiance != 0, nullptr).bytes + align_up((size_t)m * 3 * sizeof(float));
 }
 
 int mipnerf_b200_query_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w, const float* means,
