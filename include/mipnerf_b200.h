@@ -530,6 +530,22 @@ int mipnerf_b200_grid_render_backward(const mipnerf_b200_grid* grid, const mipne
                                       int white_bkgd, const float* d_rgb, const float* d_distance, const float* d_acc,
                                       const mipnerf_b200_grid_grads* grads, void* stream);
 
+/* The visibility of a baked grid's kept points over a batch of rays, for pruning (PlenOctrees): per kept point the
+ * largest score it receives from any composited sample.  The march is mipnerf_b200_grid_render's for density only
+ * (same samples, skipping, level blend and trilinear weights, same stop after the sample that leaves the transmittance
+ * below 1e-4).  At a composited sample of blending weight w_k = T_k alpha_k (formed as the renderer forms it), a kept
+ * corner c of level l scores w_k * (lw * wc_c): wc_c is its trilinear weight and lw the level weight (1 - f for level
+ * floor(lambda), 1 when f == 0, f for level floor(lambda) + 1), so lw * wc_c is the coefficient the renderer gives the
+ * corner's colour.  max_weight holds num_levels pointers; entry l has M_l floats in SH-row order (required for every
+ * level whose levels[l].sh is non-NULL).  The call RAISES each entry to the maximum of its current value and every
+ * score from these rays: the caller initialises the entries to 0, and calls over batches of rays accumulate.  The
+ * maximum is an integer atomicMax on the float bits (valid as scores are >= 0; a negative score from a negative
+ * density never raises an entry from 0), so the result is bit-reproducible: across runs, across any split of the rays
+ * into calls and under any permutation of the rays.  A prune holds for renders at the step it was computed with.  No
+ * allocation, no synchronisation. */
+int mipnerf_b200_grid_visibility(const mipnerf_b200_grid* grid, const mipnerf_b200_rays* rays, float step,
+                                 float* const* max_weight, void* stream);
+
 /* Hardware self-test of the wgmma building blocks (descriptor / swizzle / accumulator-fragment conventions):
  * d[128,n] = a[128,k] . b[n,k]^T, 16-bit operands (precision BF16|FP16), fp32 accumulate; n in {128, 256}.
  * variant bit 0: B through a pre-swizzled image + cp.async.bulk (needs `scratch`); bit 1: A in registers (the RS form

@@ -19,7 +19,8 @@ from .graph import GraphedForward
 from .metrics import eval_errors, ssim, evaluate, render_path, spheric_path, save_images
 from .field import (density_grid, isosurface, extract_mesh, mesh_colors, voxel_variance, write_ply, sh_basis,
                     sphere_quadrature, bake_sh, eval_sh, mesh_sh)
-from .baked import BakedGrid, bake_grid, finetune_grid, grid_occupancy, grid_structure, render_baked_frame
+from .baked import (BakedGrid, bake_grid, finetune_grid, grid_occupancy, grid_structure, prune_grid,
+                    render_baked_frame)
 
 __all__ = [
     "Rays", "Rays_keys", "namedtuple_map", "rearrange_render_image", "blender_rays", "spheric_pose",
@@ -32,5 +33,5 @@ __all__ = [
     "write_synthetic_blender_scene", "GraphedForward", "philox_uniform", "philox_normal", "eval_errors", "ssim", "evaluate",
     "render_path", "spheric_path", "save_images", "density_grid", "isosurface", "extract_mesh", "write_ply",
     "mesh_colors", "voxel_variance", "sh_basis", "sphere_quadrature", "bake_sh", "eval_sh", "mesh_sh",
-    "BakedGrid", "bake_grid", "finetune_grid", "grid_occupancy", "grid_structure", "render_baked_frame",
+    "BakedGrid", "bake_grid", "finetune_grid", "grid_occupancy", "grid_structure", "prune_grid", "render_baked_frame",
 ]

@@ -17,6 +17,10 @@ frames rendered from it by a CUDA ray marcher instead of the MLP.
 The renderer (`BakedGrid.render`, `render_baked_frame`) marches K = max(1, ceil((far - near) |d| / step)) samples at
 t_k = near + (k + 1/2) dt, blends two levels picked by the cone footprint (lambda = log2(sqrt(3) radii t / s_0)) and
 composites as `volumetric_rendering`, stopping once the transmittance drops below 1e-4 (include/mipnerf_b200.h).
+
+Pruning (`BakedGrid.visibility`, `BakedGrid.prune`, `prune_grid`) drops the kept points that no training ray sees: per
+kept point the largest blending weight T_k alpha_k, times the coefficient the renderer gives its colour, over every
+training ray (PlenOctrees), and a threshold on it.
 """
 from __future__ import annotations
 
@@ -38,6 +42,8 @@ DEFAULT_THRESHOLD = 1e-2
 # finetune_grid's Adam learning rates (README, "Fine-tuning a baked grid")
 FINETUNE_LR_DENSITY = 0.1
 FINETUNE_LR_SH = 0.01
+# prune_grid's visibility threshold (README, "Pruning a baked grid by visibility")
+DEFAULT_WEIGHT_THRESHOLD = 1e-5
 _FORMAT = 1
 
 
@@ -274,6 +280,61 @@ class BakedGrid:
               int(bool(white_bkgd)), rgb.data_ptr(), dist.data_ptr(), acc.data_ptr())
         return (rgb, dist, acc), keep, st
 
+    def visibility(self, rays: Rays, step: Optional[float] = None,
+                   out: Optional[Sequence[torch.Tensor]] = None) -> List[torch.Tensor]:
+        """Per level an fp32 [M_l] tensor (SH-row order) of each kept point's largest score over `rays`: at every
+        composited sample of `render`'s march, blending weight T_k alpha_k times the coefficient the renderer gives the
+        point's colour (level weight times trilinear weight).  With `out` (such tensors, e.g. from an earlier call),
+        the scores are raised into it in place and it is returned, so calls over batches of rays accumulate.  The
+        result is bit-reproducible under any order or split of the rays.  `step` defaults to `default_step()` as in
+        `render`; a prune by these scores only holds for renders at the same step."""
+        dev = _dev(self.cells[0])
+        o = rays.origins.reshape(-1, 3)
+        if o.device != dev:
+            raise ValueError(f"rays on {o.device}, grid on {dev}")
+        if out is None:
+            out = [torch.zeros(m, device=dev) for m in self.kept]
+        else:
+            out = list(out)
+            if len(out) != self.levels or any(
+                    t.dtype != torch.float32 or t.device != dev or tuple(t.shape) != (m,) or not t.is_contiguous()
+                    for t, m in zip(out, self.kept)):
+                raise ValueError(f"out: need {self.levels} contiguous fp32 tensors of shapes {self.kept} on {dev}")
+        rs, _ = _rays_struct(o, rays.directions.reshape(-1, 3), rays.viewdirs.reshape(-1, 3), rays.radii.reshape(-1),
+                             rays.near.reshape(-1), rays.far.reshape(-1))
+        g = self._struct()
+        ptrs = (C.c_void_p * self.levels)(*[t.data_ptr() if t.numel() else None for t in out])
+        st = self.default_step() if step is None else float(step)
+        _call(dev, "grid_visibility", _cabi.lib().mipnerf_b200_grid_visibility, C.byref(g), C.byref(rs), st, ptrs)
+        return out
+
+    @torch.no_grad()
+    def prune(self, max_weight: Sequence[torch.Tensor], weight_threshold: float) -> "BakedGrid":
+        """A new, non-trainable grid that keeps the points kept here whose score in `max_weight` (per level [M_l] in
+        SH-row order, as `visibility` returns) is > `weight_threshold`; `self` is left as it is.  A point pruned away
+        gets density 0 and index -1; the kept points' rows are renumbered in x-fastest order and their SH rows carried
+        over bit for bit; the occupancy is rebuilt by `grid_occupancy`; bounds, degree, rgb_padding and block are
+        copied.  Plain torch on the grid's device (CPU tensors too)."""
+        self._sync()
+        if len(max_weight) != self.levels:
+            raise ValueError(f"max_weight: {len(max_weight)} levels, the grid has {self.levels}")
+        dens, indices, sh = [], [], []
+        for lvl, (mw, m) in enumerate(zip(max_weight, self.kept)):
+            if tuple(mw.shape) != (m,):
+                raise ValueError(f"max_weight[{lvl}]: shape {tuple(mw.shape)}, need ({m},)")
+            old = self.index(lvl)
+            d = self.density(lvl)
+            kept = old >= 0
+            keep = kept.clone()
+            keep[kept] = mw.to(d.device)[old[kept].long()] > float(weight_threshold)
+            idx = torch.full_like(old, -1)
+            idx[keep] = torch.arange(int(keep.sum()), dtype=old.dtype, device=old.device)
+            dens.append(torch.where(kept & ~keep, torch.zeros((), device=d.device), d))
+            indices.append(idx)
+            sh.append(self.sh[lvl].detach()[old[keep].long()])  # x-fastest order of the kept points
+        return BakedGrid(dens, indices, sh, grid_occupancy(dens, self.block), self.bounds, self.degree,
+                         self.rgb_padding, self.block)
+
     def save(self, path: str) -> None:
         """One .npz: per level density, index and sh, plus occupancy, bounds, degree, rgb_padding and block."""
         self._sync()
@@ -376,6 +437,20 @@ def render_baked_frame(grid: BakedGrid, c2w, height: int = 800, width: int = 800
     counts = [(shard_rows(height, world, r)[1] - shard_rows(height, world, r)[0]) * width for r in range(world)]
     full = gather_rows(local, counts, group)
     return full[:, 0:3].reshape(height, width, 3), full[:, 3].reshape(height, width), full[:, 4].reshape(height, width)
+
+
+def prune_grid(grid: BakedGrid, bank, weight_threshold: float = DEFAULT_WEIGHT_THRESHOLD, step: Optional[float] = None,
+               batch_size: int = 1 << 20) -> BakedGrid:
+    """Prune the points no training ray sees (PlenOctrees): `grid.visibility` over every pixel of a `DeviceRayBank`,
+    in id order and batches of `batch_size`, then `grid.prune(scores, weight_threshold)`.  Returns the new grid; the
+    intended pipeline is `bake_grid` -> `prune_grid` -> `finetune_grid`, at one `step`."""
+    if int(batch_size) < 1:
+        raise ValueError(f"batch_size {batch_size}: need >= 1")
+    scores = [torch.zeros(m, device=grid.device) for m in grid.kept]
+    for s in range(0, bank.num_pixels, int(batch_size)):
+        rays, _ = bank.rays(torch.arange(s, min(s + int(batch_size), bank.num_pixels), device=bank.device))
+        grid.visibility(rays, step, scores)
+    return grid.prune(scores, weight_threshold)
 
 
 def finetune_grid(grid: BakedGrid, bank, steps: int, batch_size: int = 8192, lr_density: float = FINETUNE_LR_DENSITY,

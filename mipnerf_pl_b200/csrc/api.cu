@@ -145,7 +145,8 @@ int check_rays(const mipnerf_b200_rays* r) {
   return MIPNERF_B200_OK;
 }
 
-// The grid description of mipnerf_b200_grid_render and its backward (`g` checked non-NULL by the caller).
+// The grid description of mipnerf_b200_grid_render, its backward and mipnerf_b200_grid_visibility (`g` checked
+// non-NULL by the caller).
 int check_grid(const mipnerf_b200_grid* g) {
   if (g->num_levels < 1 || g->num_levels > MIPNERF_B200_GRID_MAX_LEVELS)
     return fail(MIPNERF_B200_EINVAL, "num_levels=%d: need 1..%d", g->num_levels, MIPNERF_B200_GRID_MAX_LEVELS);
@@ -2082,6 +2083,22 @@ int mipnerf_b200_grid_render_backward(const mipnerf_b200_grid* g, const mipnerf_
       return fail(MIPNERF_B200_EINVAL, "level %d has kept points: grads->density[%d] / grads->sh[%d] is NULL", l, l, l);
   CUDA_TRY(mipnerf::launch_grid_render_backward(*g, *rays, step, white_bkgd, d_rgb, d_distance, d_acc, *grads,
                                                 (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_grid_visibility(const mipnerf_b200_grid* g, const mipnerf_b200_rays* rays, float step,
+                                 float* const* max_weight, void* stream) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_rays(rays))) return rc;
+  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
+  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
+  if ((rc = check_grid(g))) return rc;
+  if (!max_weight) return fail(MIPNERF_B200_EINVAL, "max_weight is NULL");
+  for (int l = 0; l < g->num_levels; ++l)
+    if (g->levels[l].sh && !max_weight[l])
+      return fail(MIPNERF_B200_EINVAL, "level %d has kept points: max_weight[%d] is NULL", l, l);
+  CUDA_TRY(mipnerf::launch_grid_visibility(*g, *rays, step, max_weight, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

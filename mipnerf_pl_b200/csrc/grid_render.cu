@@ -36,6 +36,11 @@ struct GLevel {
   float inv_s[3];  // (n - 1) / (hi - lo): lattice coordinate per unit length
 };
 
+// Per level the maxima of mipnerf_b200_grid_visibility, indexed by SH row (NULL for a level without kept points).
+struct GMaxWeight {
+  float* w[MIPNERF_B200_GRID_MAX_LEVELS];
+};
+
 struct GParams {
   GLevel lv[MIPNERF_B200_GRID_MAX_LEVELS];
   int num_levels, nc;  // nc = (degree + 1)^2
@@ -401,6 +406,56 @@ __global__ void __launch_bounds__(kGridThreads)
   }
 }
 
+// Raise one level's kept corners to their scores at a composited sample of blending weight w: corner c's score is
+// w * (lw * wc[c]), w times the coefficient level_color gives the corner's colour.  The maximum is an integer atomicMax
+// on the float's bits, which orders non-negative floats as the floats; a negative score (from a negative density)
+// never raises an entry the caller started at 0.  The plain load in front skips the atomic when the entry already
+// holds at least the score: entries only grow, so a stale read costs one unneeded atomic and never loses a maximum.
+__device__ __forceinline__ void level_visibility(float* __restrict__ max_weight, const int (&row)[8],
+                                                 const float (&wc)[8], float lw, float w) {
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    if (row[c] < 0) continue;
+    const int s = __float_as_int(w * (lw * wc[c]));
+    int* p = reinterpret_cast<int*>(max_weight) + row[c];
+    if (s > *p) atomicMax(p, s);
+  }
+}
+
+// Per kept corner, the largest score over these rays (mipnerf_b200_grid_visibility), one thread per ray.  The march
+// is the forward's for density only: the same samples, skipping, level blend and trilinear weights, the same
+// compositing arithmetic on T (w_k = T_k alpha_k exactly as `composite` forms it) and the same stop after the sample
+// that leaves T < 1e-4; no colour is evaluated.  A maximum does not depend on the order of its updates, so the result
+// is bit for bit the same across runs, across any split of the rays into calls, and under any permutation of the rays.
+__global__ void __launch_bounds__(kGridThreads)
+    grid_visibility_kernel(const GParams g, const mipnerf_b200_rays rays, float step,
+                           const __grid_constant__ GMaxWeight max_weight) {
+  const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
+  if (r >= rays.num_rays) return;
+  RayMarch m;
+  float y[16];
+  ray_setup(g, rays, r, step, m, y);
+  float T = 1.f;
+  for (int64_t k = m.k0; k < m.k1;) {
+    float t, x[3];
+    if (!sample_at(g, m, k, t, x)) {
+      ++k;
+      continue;
+    }
+    if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
+    Blend b;
+    const float sigma = blend_density(g, m.radius, t, x, b);
+    ++k;
+    if (!(sigma != 0.f)) continue;
+    const float alpha = 1.f - expf(-sigma * m.delta);
+    const float w = T * alpha;
+    level_visibility(max_weight.w[b.la], b.row_a, b.w_a, b.f > 0.f ? 1.f - b.f : 1.f, w);
+    if (b.f > 0.f) level_visibility(max_weight.w[b.la + 1], b.row_b, b.w_b, b.f, w);
+    T *= 1.f - alpha;
+    if (T < kStopTransmittance) break;
+  }
+}
+
 GParams make_params(const mipnerf_b200_grid& grid) {
   GParams g{};
   g.num_levels = grid.num_levels;
@@ -465,6 +520,18 @@ cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mip
     default: MIPNERF_GRID_BWD(16);
   }
 #undef MIPNERF_GRID_BWD
+  return cudaGetLastError();
+}
+
+cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
+                                   float* const* max_weight, cudaStream_t st) {
+  if (rays.num_rays == 0) return cudaSuccess;
+  const GParams g = make_params(grid);
+  GMaxWeight mw{};
+  for (int l = 0; l < grid.num_levels; ++l) mw.w[l] = max_weight[l];
+  const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
+  LaunchScope scope(kKernGridVisibility, st);
+  grid_visibility_kernel<<<blocks, kGridThreads, 0, st>>>(g, rays, step, mw);
   return cudaGetLastError();
 }
 

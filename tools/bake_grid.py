@@ -2,10 +2,13 @@
 render the spheric video path from the grid.
 
     python tools/bake_grid.py --ckpt last.ckpt --out GRID.npz [--resolution 257] [--levels 1] [--threshold 0.01]
-        [--degree 2] [--bounds -1.5 -1.5 -1.5 1.5 1.5 1.5] [--precision bf16] [--frames DIR] [--size 800]
+        [--degree 2] [--bounds -1.5 -1.5 -1.5 1.5 1.5 1.5] [--precision bf16] [--prune DATA_DIR]
+        [--weight-threshold 1e-5] [--frames DIR] [--size 800]
 
 Level l has (n - 1) / 2^l + 1 points per axis (n - 1 divisible by 2^(levels - 1)).  Lattice points farther than one
-point from any point of density > threshold are dropped (density 0).  With --frames, the 120 poses of
+point from any point of density > threshold are dropped (density 0).  With --prune, the kept points that no pixel of
+the Blender scene's train split sees (largest blending weight times colour coefficient <= --weight-threshold over
+every training ray, `mp.prune_grid`) are dropped as well, before the grid is saved.  With --frames, the 120 poses of
 `metrics.spheric_path()` are rendered from the grid with `render_baked_frame` and written with `save_images`
 (<idx>_rgb.png, _dist.png, _acc.png).  A saved grid renders without the checkpoint: `mp.BakedGrid.load(path)`.
 """
@@ -34,6 +37,9 @@ def main(argv=None):
     ap.add_argument("--bounds", type=float, nargs=6, default=[-1.5, -1.5, -1.5, 1.5, 1.5, 1.5],
                     metavar=("X0", "Y0", "Z0", "X1", "Y1", "Z1"))
     ap.add_argument("--precision", default="bf16", choices=sorted(mp._cabi.PRECISIONS))
+    ap.add_argument("--prune", default=None, metavar="DATA_DIR",
+                    help="prune by visibility from the train split of this Blender scene")
+    ap.add_argument("--weight-threshold", type=float, default=mp.baked.DEFAULT_WEIGHT_THRESHOLD)
     ap.add_argument("--frames", default=None, metavar="DIR", help="render the spheric path from the grid into DIR")
     ap.add_argument("--size", type=int, default=800, help="frame height and width for --frames")
     ap.add_argument("--device", default="cuda:0")
@@ -46,10 +52,18 @@ def main(argv=None):
     grid = mp.bake_grid(model, res, levels=args.levels, threshold=args.threshold, degree=args.degree, bounds=bounds)
     torch.cuda.synchronize()
     t1 = time.perf_counter()
+    summary = lambda g: (f"kept points {g.kept}, occupied macro cells {int(g.occupancy.sum())}/"  # noqa: E731
+                         f"{g.occupancy.numel()}, {g.nbytes / 2 ** 20:.1f} MiB")
+    print(f"baked: levels {grid.resolutions}, {summary(grid)}, in {t1 - t0:.2f} s")
+    if args.prune:
+        bank = mp.DeviceRayBank(mp.load_blender_scene(args.prune, "train", white_bkgd=True), args.device)
+        t0 = time.perf_counter()
+        grid = mp.prune_grid(grid, bank, args.weight_threshold)
+        torch.cuda.synchronize()
+        print(f"pruned over {bank.num_pixels} training rays at weight threshold {args.weight_threshold:g}: "
+              f"{summary(grid)}, in {time.perf_counter() - t0:.2f} s")
     grid.save(args.out)
-    print(f"{args.out}: levels {grid.resolutions}, kept points {grid.kept}, occupied macro cells "
-          f"{int(grid.occupancy.sum())}/{grid.occupancy.numel()}, {grid.nbytes / 2 ** 20:.1f} MiB, "
-          f"baked in {t1 - t0:.2f} s")
+    print(f"{args.out}: written")
     if args.frames:
         times = []
         for idx, c2w in enumerate(mp.spheric_path()):
