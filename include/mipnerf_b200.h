@@ -506,6 +506,29 @@ typedef struct mipnerf_b200_grid {
 int mipnerf_b200_grid_render(const mipnerf_b200_grid* grid, const mipnerf_b200_rays* rays, float step, int white_bkgd,
                              float* rgb, float* distance, float* acc, void* stream);
 
+/* The SH rows of a baked grid quantized to 8 bits (mipnerf_pl_b200/baked.py, BakedGrid.quantize): per level and per
+ * (coefficient k, channel), an affine code with offset = the column's minimum and scale = (max - min) / 255, so
+ * rows[l][r, k, ch] = clamp(round((c - offset) / scale), 0, 255) (0 for a constant column, scale 0).  Coefficient k,
+ * channel ch of a row reads as deq(q) = fl32(fl32(float(q) * scale[l][k][ch]) + offset[l][k][ch]): two explicitly
+ * rounded fp32 operations, no fused multiply-add.  scale and offset are values in the struct, not device pointers;
+ * entries past (degree + 1)^2 and num_levels are not read. */
+typedef struct mipnerf_b200_grid_sh_u8 {
+  const uint8_t* rows[MIPNERF_B200_GRID_MAX_LEVELS]; /* [M_l, (degree + 1)^2, 3] uint8; NULL: no kept points */
+  float scale[MIPNERF_B200_GRID_MAX_LEVELS][16][3];  /* [level][k][channel], k < (degree + 1)^2 */
+  float offset[MIPNERF_B200_GRID_MAX_LEVELS][16][3];
+} mipnerf_b200_grid_sh_u8;
+
+/* mipnerf_b200_grid_render on a grid whose SH rows are `sh`'s uint8 rows: the same march, skipping, level blend and
+ * compositing, with every SH coefficient read as deq(q) above, in the same order and accumulation as the fp32 rows.
+ * So rgb, distance and acc equal, bit for bit, mipnerf_b200_grid_render's on the grid whose levels[l].sh are the
+ * dequantized rows; distance and acc equal the unquantized grid's, since the density path does not read the rows.
+ * Every levels[l].sh must be NULL (the rows read are sh->rows[l]), and scale / offset must be finite for every level and
+ * coefficient in use.  The scale / offset tables are passed to the kernel by value: no allocation, no copy, no
+ * synchronisation. */
+int mipnerf_b200_grid_render_u8(const mipnerf_b200_grid* grid, const mipnerf_b200_grid_sh_u8* sh,
+                                const mipnerf_b200_rays* rays, float step, int white_bkgd, float* rgb, float* distance,
+                                float* acc, void* stream);
+
 /* Per-level gradient buffers of a baked grid's parameters: density[l] [M_l] is indexed by SH row (the density of the
  * kept point whose row is r), sh[l] [M_l, (degree + 1)^2, 3] has the layout of levels[l].sh.  Dropped points (row -1)
  * are not parameters. */

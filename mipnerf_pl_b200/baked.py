@@ -21,6 +21,13 @@ composites as `volumetric_rendering`, stopping once the transmittance drops belo
 Pruning (`BakedGrid.visibility`, `BakedGrid.prune`, `prune_grid`) drops the kept points that no training ray sees: per
 kept point the largest blending weight T_k alpha_k, times the coefficient the renderer gives its colour, over every
 training ray (PlenOctrees), and a threshold on it.
+
+Quantization (`BakedGrid.quantize`, SNeRG's 8-bit storage) stores the SH rows as uint8 with an affine code per level,
+coefficient and channel: offset = the column's minimum, scale = (max - min) / 255 in fp32, q = clamp(round((c - offset) /
+scale), 0, 255) (0 for a constant column).  A coefficient reads as deq(q) = fl32(fl32(q * scale) + offset), two
+explicitly rounded fp32 operations, in `dequantize` and in the renderer's kernel alike
+(mipnerf_b200_grid_render_u8), so a quantized grid renders bit for bit as its `dequantize()` does.  The intended
+pipeline is bake -> prune -> fine-tune -> quantize: a quantized grid is not pruned or trained.
 """
 from __future__ import annotations
 
@@ -45,6 +52,7 @@ FINETUNE_LR_SH = 0.01
 # prune_grid's visibility threshold (README, "Pruning a baked grid by visibility")
 DEFAULT_WEIGHT_THRESHOLD = 1e-5
 _FORMAT = 1
+_FORMAT_U8 = 2  # a quantized grid: uint8 SH rows plus per-level scale / offset
 
 
 def level_resolutions(resolution: Resolution, levels: int) -> List[Tuple[int, int, int]]:
@@ -122,11 +130,13 @@ def grid_occupancy(baked_densities: Sequence[torch.Tensor], block: int = DEFAULT
 class BakedGrid:
     """A baked field: per level the density and SH index lattices and the SH rows, the bounds, the SH degree, the
     model's rgb_padding and the macro-cell occupancy.  `render` marches rays through it on the GPU; `save` / `load`
-    keep it in one .npz."""
+    keep it in one .npz.  With `sh_scale` and `sh_offset` (per level fp32 [(degree + 1)^2, 3]) the grid is quantized:
+    `sh` holds uint8 rows read as fl(fl(q * scale) + offset) (`quantize`)."""
 
     def __init__(self, densities: Sequence[torch.Tensor], indices: Sequence[torch.Tensor], sh: Sequence[torch.Tensor],
                  occupancy: torch.Tensor, bounds=DEFAULT_BOUNDS, degree: int = 2, rgb_padding: float = 0.001,
-                 block: int = DEFAULT_BLOCK):
+                 block: int = DEFAULT_BLOCK, sh_scale: Optional[Sequence[torch.Tensor]] = None,
+                 sh_offset: Optional[Sequence[torch.Tensor]] = None):
         if not 0 <= int(degree) <= 3:
             raise ValueError(f"degree {degree}: need 0..3")
         if not (len(densities) == len(indices) == len(sh)) or not 1 <= len(densities) <= MAX_LEVELS:
@@ -136,13 +146,39 @@ class BakedGrid:
         self.block = int(block)
         self.bounds = (tuple(float(v) for v in bounds[0]), tuple(float(v) for v in bounds[1]))
         nc = (self.degree + 1) ** 2
+        if (sh_scale is None) != (sh_offset is None):
+            raise ValueError("sh_scale and sh_offset: give both (a quantized grid) or neither")
+        quantized = sh_scale is not None
+        if quantized and not (len(sh_scale) == len(sh_offset) == len(sh)):
+            raise ValueError(f"{len(sh_scale)} / {len(sh_offset)} levels of sh_scale / sh_offset, {len(sh)} of sh")
         self.cells, self.sh = [], []
         for lvl, (d, i, c) in enumerate(zip(densities, indices, sh)):
             if d.shape != i.shape or d.dim() != 3 or c.dim() != 3 or tuple(c.shape[1:]) != (nc, 3):
                 raise ValueError(f"level {lvl}: density {tuple(d.shape)}, index {tuple(i.shape)}, sh {tuple(c.shape)}")
+            if quantized and c.dtype != torch.uint8:
+                raise ValueError(f"level {lvl}: sh of a quantized grid must be uint8, got {c.dtype}")
             # (density bits, row) per lattice point: the kernel reads one 8-byte word per corner
             self.cells.append(torch.stack([_f32(d).view(torch.int32), i.to(torch.int32)], dim=-1).contiguous())
-            self.sh.append(_f32(c))
+            self.sh.append(c.detach().contiguous() if quantized else _f32(c))
+        self.sh_scale: Optional[List[torch.Tensor]] = None  # quantized: per level fp32 [nc, 3]
+        self.sh_offset: Optional[List[torch.Tensor]] = None
+        if quantized:
+            self.sh_scale, self.sh_offset = [], []
+            for lvl, (s, o) in enumerate(zip(sh_scale, sh_offset)):
+                s, o = _f32(s).to(self.cells[0].device), _f32(o).to(self.cells[0].device)
+                if tuple(s.shape) != (nc, 3) or tuple(o.shape) != (nc, 3):
+                    raise ValueError(f"level {lvl}: sh_scale {tuple(s.shape)}, sh_offset {tuple(o.shape)}, need {(nc, 3)}")
+                if not bool(torch.isfinite(s).all() and torch.isfinite(o).all()):
+                    raise ValueError(f"level {lvl}: sh_scale / sh_offset is not finite")
+                self.sh_scale.append(s)
+                self.sh_offset.append(o)
+            # the tables as the kernel takes them by value ([MAX_LEVELS][16][3] fp32), copied to the host once
+            self._deq_host = []
+            for tabs in (self.sh_scale, self.sh_offset):
+                pad = np.zeros((MAX_LEVELS, 16, 3), dtype=np.float32)
+                for lvl, tab in enumerate(tabs):
+                    pad[lvl, :nc] = tab.cpu().numpy()
+                self._deq_host.append(pad)
         self.occupancy = occupancy.to(torch.uint8).contiguous()
         n0 = tuple(self.cells[0].shape[:3])
         want = tuple(-(-(n - 1) // self.block) for n in n0)
@@ -158,7 +194,11 @@ class BakedGrid:
         """Make the grid trainable: per level a contiguous fp32 leaf `kept_density[l]` [M_l] (the kept points'
         densities in SH-row order) and `sh[l]` requiring grad.  The cells follow `kept_density` on the next read
         (`_struct`, `density`, `save`): projected onto >= 0, scattered into the kept points, occupancy rebuilt.  The
-        kept set and the rows never change.  False syncs and turns the parameters back into plain tensors."""
+        kept set and the rows never change.  False syncs and turns the parameters back into plain tensors.  A quantized
+        grid is not trainable: fine-tune before `quantize`, or train `dequantize()`."""
+        if requires_grad and self.quantized:
+            raise ValueError("BakedGrid.requires_grad_: a quantized grid is not trainable; the order is bake -> prune -> "
+                             "fine-tune -> quantize, or fine-tune dequantize()")
         if not requires_grad:
             if self.kept_density is not None:
                 self._sync()
@@ -184,6 +224,11 @@ class BakedGrid:
     @property
     def trainable(self) -> bool:
         return self.kept_density is not None
+
+    @property
+    def quantized(self) -> bool:
+        """Whether the SH rows are uint8 (`quantize`)."""
+        return self.sh_scale is not None
 
     def parameters(self) -> List[torch.Tensor]:
         """[kept_density_0, sh_0, kept_density_1, sh_1, ...] of a trainable grid."""
@@ -231,7 +276,8 @@ class BakedGrid:
 
     @property
     def nbytes(self) -> int:
-        return sum(t.numel() * t.element_size() for t in self.cells + self.sh) + self.occupancy.numel()
+        tables = self.sh_scale + self.sh_offset if self.quantized else []
+        return sum(t.numel() * t.element_size() for t in self.cells + self.sh + tables) + self.occupancy.numel()
 
     def default_step(self) -> float:
         """Half the finest level's smallest voxel edge."""
@@ -243,17 +289,29 @@ class BakedGrid:
         g = _cabi.Grid()
         for lvl, (c, s) in enumerate(zip(self.cells, self.sh)):
             nz, ny, nx = c.shape[:3]
-            g.levels[lvl] = _cabi.GridLevel(c.data_ptr(), s.data_ptr() if s.numel() else None, nx, ny, nz)
+            fp32_rows = s.data_ptr() if s.numel() and not self.quantized else None  # a quantized grid's are in _sh_u8
+            g.levels[lvl] = _cabi.GridLevel(c.data_ptr(), fp32_rows, nx, ny, nz)
         g.num_levels, g.degree = self.levels, self.degree
         g.lo = (C.c_float * 3)(*self.bounds[0])
         g.hi = (C.c_float * 3)(*self.bounds[1])
         g.rgb_padding, g.occupancy, g.block = self.rgb_padding, self.occupancy.data_ptr(), self.block
         return g
 
+    def _sh_u8(self) -> "_cabi.GridShU8":
+        """The uint8 rows and the scale / offset values of a quantized grid, as mipnerf_b200_grid_render_u8 takes them."""
+        t = _cabi.GridShU8()
+        for lvl, s in enumerate(self.sh):
+            t.rows[lvl] = s.data_ptr() if s.numel() else None
+        scale, offset = self._deq_host
+        C.memmove(C.addressof(t.scale), scale.ctypes.data, scale.nbytes)
+        C.memmove(C.addressof(t.offset), offset.ctypes.data, offset.nbytes)
+        return t
+
     def render(self, rays: Rays, white_bkgd: bool = True, step: Optional[float] = None):
         """(rgb [B,3], distance [B], acc [B]) of flat rays on the grid's device, marched every `step` along |d| (default
         `default_step()`).  Differentiable in `parameters()` when the grid is trainable and grad mode is on (rays that
-        require grad are refused: there is no ray gradient)."""
+        require grad are refused: there is no ray gradient).  A quantized grid renders on
+        mipnerf_b200_grid_render_u8, bit for bit as its `dequantize()` renders."""
         if self.kept_density is None or not torch.is_grad_enabled():
             with torch.no_grad():
                 return self._render(rays, white_bkgd, step)[0]
@@ -276,8 +334,12 @@ class BakedGrid:
         dist = torch.empty(n, device=dev)
         acc = torch.empty(n, device=dev)
         st = self.default_step() if step is None else float(step)
-        _call(dev, "grid_render", _cabi.lib().mipnerf_b200_grid_render, C.byref(g), C.byref(rs), st,
-              int(bool(white_bkgd)), rgb.data_ptr(), dist.data_ptr(), acc.data_ptr())
+        out = (int(bool(white_bkgd)), rgb.data_ptr(), dist.data_ptr(), acc.data_ptr())
+        if self.quantized:
+            _call(dev, "grid_render_u8", _cabi.lib().mipnerf_b200_grid_render_u8, C.byref(g), C.byref(self._sh_u8()),
+                  C.byref(rs), st, *out)
+        else:
+            _call(dev, "grid_render", _cabi.lib().mipnerf_b200_grid_render, C.byref(g), C.byref(rs), st, *out)
         return (rgb, dist, acc), keep, st
 
     def visibility(self, rays: Rays, step: Optional[float] = None,
@@ -287,7 +349,9 @@ class BakedGrid:
         point's colour (level weight times trilinear weight).  With `out` (such tensors, e.g. from an earlier call),
         the scores are raised into it in place and it is returned, so calls over batches of rays accumulate.  The
         result is bit-reproducible under any order or split of the rays.  `step` defaults to `default_step()` as in
-        `render`; a prune by these scores only holds for renders at the same step."""
+        `render`; a prune by these scores only holds for renders at the same step.  Not on a quantized grid: prune
+        before `quantize`."""
+        self._refuse_quantized("visibility")
         dev = _dev(self.cells[0])
         o = rays.origins.reshape(-1, 3)
         if o.device != dev:
@@ -314,7 +378,9 @@ class BakedGrid:
         SH-row order, as `visibility` returns) is > `weight_threshold`; `self` is left as it is.  A point pruned away
         gets density 0 and index -1; the kept points' rows are renumbered in x-fastest order and their SH rows carried
         over bit for bit; the occupancy is rebuilt by `grid_occupancy`; bounds, degree, rgb_padding and block are
-        copied.  Plain torch on the grid's device (CPU tensors too)."""
+        copied.  Plain torch on the grid's device (CPU tensors too).  Not on a quantized grid: prune before
+        `quantize`."""
+        self._refuse_quantized("prune")
         self._sync()
         if len(max_weight) != self.levels:
             raise ValueError(f"max_weight: {len(max_weight)} levels, the grid has {self.levels}")
@@ -335,29 +401,95 @@ class BakedGrid:
         return BakedGrid(dens, indices, sh, grid_occupancy(dens, self.block), self.bounds, self.degree,
                          self.rgb_padding, self.block)
 
-    def save(self, path: str) -> None:
-        """One .npz: per level density, index and sh, plus occupancy, bounds, degree, rgb_padding and block."""
+    def _refuse_quantized(self, what: str) -> None:
+        if self.quantized:
+            raise ValueError(f"BakedGrid.{what}: the grid is quantized; the order is bake -> prune -> fine-tune -> "
+                             f"quantize, or use dequantize()")
+
+    @torch.no_grad()
+    def quantize(self) -> "BakedGrid":
+        """A new, non-trainable grid whose SH rows are uint8, with per level, coefficient and channel offset = the
+        column's minimum over the kept rows and scale = (max - min) / 255 (fp32), and q = clamp(round((c - offset) /
+        scale), 0, 255), 0 where scale == 0; a level without kept rows gets scale = offset = 0.  Each coefficient then
+        reads as fl(fl(q * scale) + offset), within scale / 2 (plus a few ulp of the column's magnitude) of c.  A
+        trainable grid is synced first and its detached values are used; `self` is left as it is.  The cells,
+        indices, occupancy, bounds, degree, rgb_padding and block are copied.  Plain, deterministic torch on the
+        grid's device (CPU tensors too).  Non-finite rows are refused."""
+        if self.quantized:
+            raise ValueError("BakedGrid.quantize: the grid is already quantized")
         self._sync()
-        arrays = {"format": np.int32(_FORMAT), "levels": np.int32(self.levels), "degree": np.int32(self.degree),
+        nc = (self.degree + 1) ** 2
+        rows, scales, offsets = [], [], []
+        for lvl, c in enumerate(self.sh):
+            c = c.detach()
+            if not bool(torch.isfinite(c).all()):
+                raise ValueError(f"BakedGrid.quantize: level {lvl} has non-finite SH coefficients")
+            if c.shape[0] == 0:
+                scale = offset = torch.zeros(nc, 3, device=c.device)
+                q = torch.empty(0, nc, 3, dtype=torch.uint8, device=c.device)
+            else:
+                offset, hi = c.amin(dim=0), c.amax(dim=0)
+                # a tensor divisor: CUDA torch turns a Python-scalar divisor into a multiply by its reciprocal, which
+                # is not the correctly rounded quotient the CPU gives
+                scale = (hi - offset) / torch.full_like(hi, 255.0)
+                if not bool(torch.isfinite(scale).all()):
+                    raise ValueError(f"BakedGrid.quantize: level {lvl}: a column's range overflows fp32")
+                live = scale > 0
+                code = torch.round((c - offset) / torch.where(live, scale, torch.ones((), device=c.device)))
+                q = torch.where(live, code.clamp(0, 255), torch.zeros((), device=c.device)).to(torch.uint8)
+            rows.append(q)
+            scales.append(scale)
+            offsets.append(offset)
+        return BakedGrid([self.density(lvl) for lvl in range(self.levels)],
+                         [self.index(lvl) for lvl in range(self.levels)], rows, self.occupancy.clone(), self.bounds,
+                         self.degree, self.rgb_padding, self.block, scales, offsets)
+
+    @torch.no_grad()
+    def dequantize(self) -> "BakedGrid":
+        """The fp32 grid of a quantized one: SH rows fl(fl(q * scale) + offset) (eager torch: one rounded multiply,
+        then one rounded add), everything else copied.  It renders bit for bit as the quantized grid does."""
+        if not self.quantized:
+            raise ValueError("BakedGrid.dequantize: the grid is not quantized (fp32 rows)")
+        rows = [q.to(torch.float32) * s + o for q, s, o in zip(self.sh, self.sh_scale, self.sh_offset)]
+        return BakedGrid([self.density(lvl) for lvl in range(self.levels)],
+                         [self.index(lvl) for lvl in range(self.levels)], rows, self.occupancy.clone(), self.bounds,
+                         self.degree, self.rgb_padding, self.block)
+
+    def save(self, path: str) -> None:
+        """One .npz: per level density, index and sh, plus occupancy, bounds, degree, rgb_padding and block (format
+        1).  A quantized grid writes format 2: sh_{l} is its uint8 rows, plus sh_scale_{l} and sh_offset_{l} fp32
+        [(degree + 1)^2, 3]."""
+        self._sync()
+        fmt = _FORMAT_U8 if self.quantized else _FORMAT
+        arrays = {"format": np.int32(fmt), "levels": np.int32(self.levels), "degree": np.int32(self.degree),
                   "rgb_padding": np.float32(self.rgb_padding), "block": np.int32(self.block),
                   "bounds": np.asarray(self.bounds, dtype=np.float32), "occupancy": self.occupancy.cpu().numpy()}
         for lvl in range(self.levels):
             arrays[f"density_{lvl}"] = self.density(lvl).cpu().numpy()
             arrays[f"index_{lvl}"] = self.index(lvl).cpu().numpy()
             arrays[f"sh_{lvl}"] = self.sh[lvl].detach().cpu().numpy()
+            if self.quantized:
+                arrays[f"sh_scale_{lvl}"] = self.sh_scale[lvl].cpu().numpy()
+                arrays[f"sh_offset_{lvl}"] = self.sh_offset[lvl].cpu().numpy()
         np.savez(path, **arrays)
 
     @classmethod
     def load(cls, path: str, device="cuda") -> "BakedGrid":
         with np.load(path) as z:
-            if int(z["format"]) != _FORMAT:
-                raise ValueError(f"{path}: baked-grid format {int(z['format'])}, this library reads {_FORMAT}")
+            fmt = int(z["format"])
+            if fmt not in (_FORMAT, _FORMAT_U8):
+                raise ValueError(f"{path}: baked-grid format {fmt}, this library reads {_FORMAT} and {_FORMAT_U8}")
             levels = int(z["levels"])
             t = lambda name: torch.from_numpy(np.ascontiguousarray(z[name])).to(device)  # noqa: E731
             bounds = z["bounds"].astype(np.float64)
+            tables = {}
+            if fmt == _FORMAT_U8:
+                tables = {"sh_scale": [t(f"sh_scale_{lvl}") for lvl in range(levels)],
+                          "sh_offset": [t(f"sh_offset_{lvl}") for lvl in range(levels)]}
             return cls([t(f"density_{lvl}") for lvl in range(levels)], [t(f"index_{lvl}") for lvl in range(levels)],
                        [t(f"sh_{lvl}") for lvl in range(levels)], t("occupancy"),
-                       (tuple(bounds[0]), tuple(bounds[1])), int(z["degree"]), float(z["rgb_padding"]), int(z["block"]))
+                       (tuple(bounds[0]), tuple(bounds[1])), int(z["degree"]), float(z["rgb_padding"]), int(z["block"]),
+                       **tables)
 
 
 class _GridRender(torch.autograd.Function):

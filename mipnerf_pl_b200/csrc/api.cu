@@ -2068,6 +2068,31 @@ int mipnerf_b200_grid_render(const mipnerf_b200_grid* g, const mipnerf_b200_rays
   return MIPNERF_B200_OK;
 }
 
+int mipnerf_b200_grid_render_u8(const mipnerf_b200_grid* g, const mipnerf_b200_grid_sh_u8* sh,
+                                const mipnerf_b200_rays* rays, float step, int white_bkgd, float* rgb, float* distance,
+                                float* acc, void* stream) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_rays(rays))) return rc;
+  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
+  if (rays->num_rays > 0 && (!rgb || !distance || !acc)) return fail(MIPNERF_B200_EINVAL, "rgb / distance / acc is NULL");
+  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
+  if ((rc = check_grid(g))) return rc;
+  if (!sh) return fail(MIPNERF_B200_EINVAL, "sh is NULL");
+  const int nc = (g->degree + 1) * (g->degree + 1);
+  for (int l = 0; l < g->num_levels; ++l) {
+    if (g->levels[l].sh)
+      return fail(MIPNERF_B200_EINVAL, "level %d: levels[%d].sh is set; the uint8 rows are read from sh->rows", l, l);
+    for (int k = 0; k < nc; ++k)
+      for (int ch = 0; ch < 3; ++ch)
+        if (!std::isfinite(sh->scale[l][k][ch]) || !std::isfinite(sh->offset[l][k][ch]))
+          return fail(MIPNERF_B200_EINVAL, "level %d coefficient %d channel %d: scale=%g offset=%g, need finite", l, k,
+                      ch, sh->scale[l][k][ch], sh->offset[l][k][ch]);
+  }
+  CUDA_TRY(mipnerf::launch_grid_render_u8(*g, *sh, *rays, step, white_bkgd, rgb, distance, acc, (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
 int mipnerf_b200_grid_render_backward(const mipnerf_b200_grid* g, const mipnerf_b200_rays* rays, float step,
                                       int white_bkgd, const float* d_rgb, const float* d_distance, const float* d_acc,
                                       const mipnerf_b200_grid_grads* grads, void* stream) {

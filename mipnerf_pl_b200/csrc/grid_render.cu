@@ -95,20 +95,60 @@ __device__ __forceinline__ float level_density(const GLevel& l, const float (&lo
   return sigma;
 }
 
+// Row readers: how level_color reads the SH coefficients of one level.  `rows.level(g, l)` is level l's reader, and
+// `.row<NC>(r)(k, ch)` coefficient k, channel ch of its SH row r.  F32Rows reads GLevel::sh as stored.  U8Rows reads
+// the uint8 rows of mipnerf_b200_grid_render_u8 and dequantizes each coefficient as fl(fl(q * scale) + offset), two
+// explicitly rounded fp32 operations (never an FMA), so a u8 render equals the fp32 render of the dequantized rows bit
+// for bit.  Both run the one march below: same coefficient order, same accumulation.
+struct F32Rows {
+  struct Row {
+    const float* __restrict__ p;
+    __device__ __forceinline__ float operator()(int k, int ch) const { return __ldg(p + 3 * k + ch); }
+  };
+  struct Level {
+    const float* __restrict__ sh;
+    template <int NC>
+    __device__ __forceinline__ Row row(int r) const { return {sh + (int64_t)r * (NC * 3)}; }
+  };
+  __device__ __forceinline__ Level level(const GParams& g, int l) const { return {g.lv[l].sh}; }
+};
+
+// The kernel takes this by value as a __grid_constant__ parameter: the scale / offset tables are read from the
+// parameter space in place, with no copy to a stack frame.
+struct U8Rows {
+  mipnerf_b200_grid_sh_u8 t;
+  struct Row {
+    const uint8_t* p;
+    const float (*scale)[3];
+    const float (*offset)[3];
+    __device__ __forceinline__ float operator()(int k, int ch) const {
+      return __fadd_rn(__fmul_rn((float)__ldg(p + 3 * k + ch), scale[k][ch]), offset[k][ch]);
+    }
+  };
+  struct Level {
+    const uint8_t* rows;
+    const float (*scale)[3];
+    const float (*offset)[3];
+    template <int NC>
+    __device__ __forceinline__ Row row(int r) const { return {rows + (int64_t)r * (NC * 3), scale, offset}; }
+  };
+  __device__ __forceinline__ Level level(const GParams&, int l) const { return {t.rows[l], t.scale[l], t.offset[l]}; }
+};
+
 // sum over kept corners of weight * Y . c (raw colour, 3 channels)
-template <int NC>
-__device__ __forceinline__ void level_color(const float* __restrict__ sh, const int (&row)[8], const float (&wc)[8],
+template <int NC, class Level>
+__device__ __forceinline__ void level_color(const Level sh, const int (&row)[8], const float (&wc)[8],
                                             const float (&y)[16], float scale, float (&raw)[3]) {
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
     if (row[c] < 0) continue;
-    const float* p = sh + (int64_t)row[c] * (NC * 3);
+    const auto p = sh.template row<NC>(row[c]);
     float s0 = 0.f, s1 = 0.f, s2 = 0.f;
 #pragma unroll
     for (int k = 0; k < NC; ++k) {
-      s0 += y[k] * __ldg(p + 3 * k);
-      s1 += y[k] * __ldg(p + 3 * k + 1);
-      s2 += y[k] * __ldg(p + 3 * k + 2);
+      s0 += y[k] * p(k, 0);
+      s1 += y[k] * p(k, 1);
+      s2 += y[k] * p(k, 2);
     }
     const float w = scale * wc[c];
     raw[0] += w * s0, raw[1] += w * s1, raw[2] += w * s2;
@@ -246,11 +286,12 @@ __device__ __forceinline__ float blend_density(const GParams& g, float radius, f
 }
 
 // The blended raw colour Y . c of a sample.
-template <int NC>
-__device__ __forceinline__ void blend_raw(const GParams& g, const Blend& b, const float (&y)[16], float (&raw)[3]) {
+template <int NC, class Rows>
+__device__ __forceinline__ void blend_raw(const GParams& g, const Rows& rows, const Blend& b, const float (&y)[16],
+                                          float (&raw)[3]) {
   raw[0] = raw[1] = raw[2] = 0.f;
-  level_color<NC>(g.lv[b.la].sh, b.row_a, b.w_a, y, b.f > 0.f ? 1.f - b.f : 1.f, raw);
-  if (b.f > 0.f) level_color<NC>(g.lv[b.la + 1].sh, b.row_b, b.w_b, y, b.f, raw);
+  level_color<NC>(rows.level(g, b.la), b.row_a, b.w_a, y, b.f > 0.f ? 1.f - b.f : 1.f, raw);
+  if (b.f > 0.f) level_color<NC>(rows.level(g, b.la + 1), b.row_b, b.w_b, y, b.f, raw);
 }
 
 // Front-to-back compositing state: transmittance and the running sums of the outputs.
@@ -267,8 +308,9 @@ __device__ __forceinline__ void composite(Composite& s, float alpha, const float
 }
 
 // The forward march of one ray: every sample with non-zero density composited, up to the one that leaves T < 1e-4.
-template <int NC>
-__device__ __forceinline__ void march(const GParams& g, const RayMarch& m, const float (&y)[16], Composite& s) {
+template <int NC, class Rows>
+__device__ __forceinline__ void march(const GParams& g, const Rows& rows, const RayMarch& m, const float (&y)[16],
+                                      Composite& s) {
   for (int64_t k = m.k0; k < m.k1;) {
     float t, x[3];
     if (!sample_at(g, m, k, t, x)) {
@@ -282,7 +324,7 @@ __device__ __forceinline__ void march(const GParams& g, const RayMarch& m, const
     if (!(sigma != 0.f)) continue;
     const float alpha = 1.f - expf(-sigma * m.delta);
     float raw[3], c[3];
-    blend_raw<NC>(g, b, y, raw);
+    blend_raw<NC>(g, rows, b, y, raw);
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) c[ch] = g.rgb_scale / (1.f + expf(-raw[ch])) - g.rgb_padding;
     composite(s, alpha, c, t);
@@ -290,17 +332,18 @@ __device__ __forceinline__ void march(const GParams& g, const RayMarch& m, const
   }
 }
 
-template <int NC>
+template <int NC, class Rows>
 __global__ void __launch_bounds__(kGridThreads)
     grid_render_kernel(const GParams g, const mipnerf_b200_rays rays, float step, int white_bkgd,
-                       float* __restrict__ rgb_out, float* __restrict__ dist_out, float* __restrict__ acc_out) {
+                       float* __restrict__ rgb_out, float* __restrict__ dist_out, float* __restrict__ acc_out,
+                       const __grid_constant__ Rows rows) {
   const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
   if (r >= rays.num_rays) return;
   RayMarch m;
   float y[16];
   ray_setup(g, rays, r, step, m, y);
   Composite s;
-  march<NC>(g, m, y, s);
+  march<NC>(g, rows, m, y, s);
   const float bg = white_bkgd ? 1.f - s.acc : 0.f;
   rgb_out[3 * r] = s.c[0] + bg;
   rgb_out[3 * r + 1] = s.c[1] + bg;
@@ -362,7 +405,7 @@ __global__ void __launch_bounds__(kGridThreads)
   float y[16];
   ray_setup(g, rays, r, step, m, y);
   Composite total;
-  march<NC>(g, m, y, total);
+  march<NC>(g, F32Rows{}, m, y, total);
   if (!(total.dist >= m.near && total.dist <= m.far)) g_dist = 0.f;  // the clamp passes the gradient inside, inclusive
 
   Composite s;
@@ -381,7 +424,7 @@ __global__ void __launch_bounds__(kGridThreads)
     if (zero && !any_kept(b.row_a) && !(b.f > 0.f && any_kept(b.row_b))) continue;
     const float alpha = 1.f - expf(-sigma * m.delta);
     float raw[3], c[3], sg[3];
-    blend_raw<NC>(g, b, y, raw);
+    blend_raw<NC>(g, F32Rows{}, b, y, raw);
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
       sg[ch] = 1.f / (1.f + expf(-raw[ch]));
@@ -489,19 +532,38 @@ GParams make_params(const mipnerf_b200_grid& grid) {
 
 }  // namespace
 
-cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
-                               int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st) {
+namespace {
+
+template <class Rows>
+cudaError_t launch_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step, int white_bkgd,
+                          float* rgb, float* distance, float* acc, const Rows& rows, KernelId id, cudaStream_t st) {
   if (rays.num_rays == 0) return cudaSuccess;
   const GParams g = make_params(grid);
   const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
-  LaunchScope scope(kKernGridRender, st);
+  LaunchScope scope(id, st);
+#define MIPNERF_GRID_FWD(NC) \
+  grid_render_kernel<NC, Rows><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc, rows)
   switch (grid.degree) {
-    case 0: grid_render_kernel<1><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc); break;
-    case 1: grid_render_kernel<4><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc); break;
-    case 2: grid_render_kernel<9><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc); break;
-    default: grid_render_kernel<16><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc);
+    case 0: MIPNERF_GRID_FWD(1); break;
+    case 1: MIPNERF_GRID_FWD(4); break;
+    case 2: MIPNERF_GRID_FWD(9); break;
+    default: MIPNERF_GRID_FWD(16);
   }
+#undef MIPNERF_GRID_FWD
   return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
+                               int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st) {
+  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, F32Rows{}, kKernGridRender, st);
+}
+
+cudaError_t launch_grid_render_u8(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_sh_u8& sh,
+                                  const mipnerf_b200_rays& rays, float step, int white_bkgd, float* rgb,
+                                  float* distance, float* acc, cudaStream_t st) {
+  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, U8Rows{sh}, kKernGridRenderU8, st);
 }
 
 cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,

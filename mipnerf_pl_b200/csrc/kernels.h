@@ -9,6 +9,7 @@
 
 struct mipnerf_b200_grid;  // include/mipnerf_b200.h
 struct mipnerf_b200_grid_grads;
+struct mipnerf_b200_grid_sh_u8;
 struct mipnerf_b200_rays;
 
 namespace mipnerf {
@@ -73,6 +74,9 @@ cudaError_t launch_isosurface_normals(const float* grid, int nx, int ny, int nz,
 // ---- grid_render.cu (ray marching through a baked grid; arguments checked by the caller) ----
 cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
                                int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st);
+cudaError_t launch_grid_render_u8(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_sh_u8& sh,
+                                  const mipnerf_b200_rays& rays, float step, int white_bkgd, float* rgb,
+                                  float* distance, float* acc, cudaStream_t st);
 cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
                                         int white_bkgd, const float* d_rgb, const float* d_distance,
                                         const float* d_acc, const mipnerf_b200_grid_grads& grads, cudaStream_t st);

@@ -34,6 +34,7 @@ enum KernelId : int {
   kKernRadianceDirsTc,  // view-accumulator mode of the wgmma level kernel (IPE + the MLP up to the view layer's GEMM)
   kKernRadiancePairs,   // per-(point, direction) view layer + colour head (+ projection) of a shared direction set
   kKernGridRenderBackward,  // gradient of the baked-grid ray marcher with respect to the densities and SH rows
+  kKernGridRenderU8,    // ray marching through a baked grid whose SH rows are uint8, dequantized in the kernel
   kKernGridVisibility,  // largest blending weight per kept baked-grid point over a batch of rays
   kKernGridRender,      // ray marching through a baked density + SH grid
   kKernCount

@@ -3,12 +3,14 @@ render the spheric video path from the grid.
 
     python tools/bake_grid.py --ckpt last.ckpt --out GRID.npz [--resolution 257] [--levels 1] [--threshold 0.01]
         [--degree 2] [--bounds -1.5 -1.5 -1.5 1.5 1.5 1.5] [--precision bf16] [--prune DATA_DIR]
-        [--weight-threshold 1e-5] [--frames DIR] [--size 800]
+        [--weight-threshold 1e-5] [--quantize] [--frames DIR] [--size 800]
 
 Level l has (n - 1) / 2^l + 1 points per axis (n - 1 divisible by 2^(levels - 1)).  Lattice points farther than one
 point from any point of density > threshold are dropped (density 0).  With --prune, the kept points that no pixel of
 the Blender scene's train split sees (largest blending weight times colour coefficient <= --weight-threshold over
-every training ray, `mp.prune_grid`) are dropped as well, before the grid is saved.  With --frames, the 120 poses of
+every training ray, `mp.prune_grid`) are dropped as well, before the grid is saved.  With --quantize, the SH rows are
+stored as uint8 with a per-level, per-coefficient affine code (`BakedGrid.quantize`, after any pruning; the .npz is
+then format 2).  With --frames, the 120 poses of
 `metrics.spheric_path()` are rendered from the grid with `render_baked_frame` and written with `save_images`
 (<idx>_rgb.png, _dist.png, _acc.png).  A saved grid renders without the checkpoint: `mp.BakedGrid.load(path)`.
 """
@@ -40,6 +42,7 @@ def main(argv=None):
     ap.add_argument("--prune", default=None, metavar="DATA_DIR",
                     help="prune by visibility from the train split of this Blender scene")
     ap.add_argument("--weight-threshold", type=float, default=mp.baked.DEFAULT_WEIGHT_THRESHOLD)
+    ap.add_argument("--quantize", action="store_true", help="store the SH rows in 8 bits (after --prune)")
     ap.add_argument("--frames", default=None, metavar="DIR", help="render the spheric path from the grid into DIR")
     ap.add_argument("--size", type=int, default=800, help="frame height and width for --frames")
     ap.add_argument("--device", default="cuda:0")
@@ -62,6 +65,11 @@ def main(argv=None):
         torch.cuda.synchronize()
         print(f"pruned over {bank.num_pixels} training rays at weight threshold {args.weight_threshold:g}: "
               f"{summary(grid)}, in {time.perf_counter() - t0:.2f} s")
+    if args.quantize:
+        t0 = time.perf_counter()
+        grid = grid.quantize()
+        torch.cuda.synchronize()
+        print(f"quantized the SH rows to 8 bits: {summary(grid)}, in {time.perf_counter() - t0:.2f} s")
     grid.save(args.out)
     print(f"{args.out}: written")
     if args.frames:
