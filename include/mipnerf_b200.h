@@ -529,6 +529,26 @@ int mipnerf_b200_grid_render_u8(const mipnerf_b200_grid* grid, const mipnerf_b20
                                 const mipnerf_b200_rays* rays, float step, int white_bkgd, float* rgb, float* distance,
                                 float* acc, void* stream);
 
+/* The cells of a baked grid stored as bricks of 8 x 8 x 8 lattice points (mipnerf_pl_b200/baked.py,
+ * BakedGrid.sparsify), in place of levels[l].cells.  Level l's table is [tz, ty, tx] int32 with t = ceil(n / 8) per
+ * axis of that level: brick (bi, bj, bk)'s id in the pool, or -1 for a brick not stored.  The pool is [num_bricks, 8,
+ * 8, 8, 2] int32: brick b's point (z, y, x), x fastest, holds the word levels[l].cells holds, (density bits, SH row).
+ * Lattice point (i, j, k) lives in brick (i >> 3, j >> 3, k >> 3) at (k & 7, j & 7, i & 7).  A brick not stored reads
+ * (+0.0 bits, -1) at every point, so a grid whose bricks holding any other word are all stored renders exactly as
+ * its dense cells.  The pool may be NULL for a level whose table holds only -1. */
+typedef struct mipnerf_b200_grid_bricks {
+  const int32_t* table[MIPNERF_B200_GRID_MAX_LEVELS];
+  const int32_t* pool[MIPNERF_B200_GRID_MAX_LEVELS];
+} mipnerf_b200_grid_bricks;
+
+/* mipnerf_b200_grid_render (sh_u8 NULL: fp32 rows in levels[l].sh) or mipnerf_b200_grid_render_u8 (sh_u8 non-NULL,
+ * every levels[l].sh NULL) on a grid whose cells are `bricks`: every levels[l].cells must be NULL and every
+ * bricks->table[l] non-NULL.  The same march, skipping, level blend, row reads and compositing, so rgb, distance and
+ * acc equal, bit for bit, the dense render of the cells the bricks encode.  No allocation, no synchronisation. */
+int mipnerf_b200_grid_render_bricks(const mipnerf_b200_grid* grid, const mipnerf_b200_grid_bricks* bricks,
+                                    const mipnerf_b200_grid_sh_u8* sh_u8, const mipnerf_b200_rays* rays, float step,
+                                    int white_bkgd, float* rgb, float* distance, float* acc, void* stream);
+
 /* Per-level gradient buffers of a baked grid's parameters: density[l] [M_l] is indexed by SH row (the density of the
  * kept point whose row is r), sh[l] [M_l, (degree + 1)^2, 3] has the layout of levels[l].sh.  Dropped points (row -1)
  * are not parameters. */

@@ -98,6 +98,10 @@ class GridShU8(C.Structure):
                 ("offset", (C.c_float * 3 * 16) * GRID_MAX_LEVELS)]
 
 
+class GridBricks(C.Structure):
+    _fields_ = [("table", C.c_void_p * GRID_MAX_LEVELS), ("pool", C.c_void_p * GRID_MAX_LEVELS)]
+
+
 class GridGrads(C.Structure):
     _fields_ = [("density", C.c_void_p * GRID_MAX_LEVELS), ("sh", C.c_void_p * GRID_MAX_LEVELS)]
 
@@ -182,6 +186,8 @@ _SIGNATURES = {
                                            _V]),
     "mipnerf_b200_grid_render_u8": (C.c_int, [C.POINTER(Grid), C.POINTER(GridShU8), C.POINTER(RaysStruct), C.c_float,
                                               C.c_int, _V, _V, _V, _V]),
+    "mipnerf_b200_grid_render_bricks": (C.c_int, [C.POINTER(Grid), C.POINTER(GridBricks), C.POINTER(GridShU8),
+                                                  C.POINTER(RaysStruct), C.c_float, C.c_int, _V, _V, _V, _V]),
     "mipnerf_b200_grid_render_backward": (C.c_int, [C.POINTER(Grid), C.POINTER(RaysStruct), C.c_float, C.c_int, _V,
                                                     _V, _V, C.POINTER(GridGrads), _V]),
     "mipnerf_b200_grid_visibility": (C.c_int, [C.POINTER(Grid), C.POINTER(RaysStruct), C.c_float, C.POINTER(_V), _V]),

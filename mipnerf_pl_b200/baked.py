@@ -11,8 +11,16 @@ frames rendered from it by a CUDA ray marcher instead of the MLP.
   density is 0 on the cell's lattice points widened by one point of that level, so that every position in the cell
   (and any position a rounding error outside it) interpolates to exactly 0 at every level: skipping empty cells
   leaves the rendered result bit for bit unchanged.
-* Memory layout read by csrc/grid_render.cu, decided here and there only: per level one int32 [nz, ny, nx, 2] array of
-  (density bits, SH row or -1), x fastest, and the SH rows in the order of the kept points (x fastest).
+* Memory layout read by csrc/grid_render.cu, decided here and there only.  Each lattice point has one 8-byte word
+  (density bits, SH row or -1), and the SH rows are in the order of the kept points (x fastest).  A dense grid holds
+  the words of level l as one int32 [nz, ny, nx, 2] array, x fastest.  A sparse grid (`sparsify`) holds them in
+  bricks of 8^3 points: an int32 table [tz, ty, tx] (t = ceil(n / 8) per axis) of brick ids in raster order (x
+  fastest), -1 for a brick not stored, and an int32 pool [num_bricks, 8, 8, 8, 2]; point (i, j, k) is point (k & 7, j &
+  7, i & 7) of brick (k >> 3, j >> 3, i >> 3).  A brick is stored iff one of its points inside the lattice holds a word
+  other than (+0.0 bits, -1), and points past the lattice in an edge brick hold (0, -1), so an absent brick reads
+  what the dense array holds there: the encoding is lossless and renders bit for bit as the dense grid.  The rule
+  looks at rows as well as densities because a kept point may have density 0 (the keep mask is a dilation, and
+  fine-tuning projects onto >= 0) and the renderer still adds its colour wherever the blended density is non-zero.
 
 The renderer (`BakedGrid.render`, `render_baked_frame`) marches K = max(1, ceil((far - near) |d| / step)) samples at
 t_k = near + (k + 1/2) dt, blends two levels picked by the cone footprint (lambda = log2(sqrt(3) radii t / s_0)) and
@@ -28,6 +36,11 @@ scale), 0, 255) (0 for a constant column).  A coefficient reads as deq(q) = fl32
 explicitly rounded fp32 operations, in `dequantize` and in the renderer's kernel alike
 (mipnerf_b200_grid_render_u8), so a quantized grid renders bit for bit as its `dequantize()` does.  The intended
 pipeline is bake -> prune -> fine-tune -> quantize: a quantized grid is not pruned or trained.
+
+Sparse cells (`BakedGrid.sparsify`, the occupied blocks PlenOctrees and SNeRG store) keep only the non-empty bricks
+of each level, fp32 or quantized rows alike; `densify` restores the dense grid bit for bit.  A sparse grid is a
+viewer format, the last step of bake -> prune -> fine-tune -> quantize -> sparsify: it renders
+(mipnerf_b200_grid_render_bricks) and saves, and is not pruned, trained or (de)quantized.
 """
 from __future__ import annotations
 
@@ -53,6 +66,9 @@ FINETUNE_LR_SH = 0.01
 DEFAULT_WEIGHT_THRESHOLD = 1e-5
 _FORMAT = 1
 _FORMAT_U8 = 2  # a quantized grid: uint8 SH rows plus per-level scale / offset
+_FORMAT_BRICKS = 3  # a sparse grid: per-level brick table and pool, fp32 or uint8 rows
+BRICK = 8  # brick edge in lattice points, every level
+_SLAB_BYTES = 1 << 28  # sparsify / densify: bytes of dense cells handled at once
 
 
 def level_resolutions(resolution: Resolution, levels: int) -> List[Tuple[int, int, int]]:
@@ -141,6 +157,50 @@ class BakedGrid:
             raise ValueError(f"degree {degree}: need 0..3")
         if not (len(densities) == len(indices) == len(sh)) or not 1 <= len(densities) <= MAX_LEVELS:
             raise ValueError(f"{len(densities)} / {len(indices)} / {len(sh)} levels: need the same count, 1..{MAX_LEVELS}")
+        cells = []
+        for lvl, (d, i, c) in enumerate(zip(densities, indices, sh)):
+            if d.shape != i.shape or d.dim() != 3:
+                raise ValueError(f"level {lvl}: density {tuple(d.shape)}, index {tuple(i.shape)}, sh {tuple(c.shape)}")
+            # (density bits, row) per lattice point: the kernel reads one 8-byte word per corner
+            cells.append(torch.stack([_f32(d).view(torch.int32), i.to(torch.int32)], dim=-1).contiguous())
+        self._setup(cells, None, [tuple(c.shape[2::-1]) for c in cells], sh, occupancy, bounds, degree, rgb_padding,
+                    block, sh_scale, sh_offset)
+
+    @classmethod
+    def from_bricks(cls, tables: Sequence[torch.Tensor], pools: Sequence[torch.Tensor],
+                    resolutions: Sequence[Tuple[int, int, int]], sh: Sequence[torch.Tensor], occupancy: torch.Tensor,
+                    bounds=DEFAULT_BOUNDS, degree: int = 2, rgb_padding: float = 0.001, block: int = DEFAULT_BLOCK,
+                    sh_scale: Optional[Sequence[torch.Tensor]] = None,
+                    sh_offset: Optional[Sequence[torch.Tensor]] = None) -> "BakedGrid":
+        """A sparse grid from its bricks (the layout of `sparsify`): per level an int32 table [tz, ty, tx] (t = ceil(n
+        / 8) of `resolutions[l]` = (nx, ny, nz)) and an int32 pool [num_bricks, 8, 8, 8, 2]; the other arguments as
+        for the dense constructor.  Every table entry must be -1 or a brick id below num_bricks."""
+        if not 0 <= int(degree) <= 3:
+            raise ValueError(f"degree {degree}: need 0..3")
+        if not (len(tables) == len(pools) == len(resolutions) == len(sh)) or not 1 <= len(tables) <= MAX_LEVELS:
+            raise ValueError(f"{len(tables)} / {len(pools)} / {len(resolutions)} / {len(sh)} levels of tables / pools / "
+                             f"resolutions / sh: need the same count, 1..{MAX_LEVELS}")
+        bricks, res = [], []
+        for lvl, (t, p, r) in enumerate(zip(tables, pools, resolutions)):
+            r = tuple(int(n) for n in r)
+            want = tuple(-(-n // BRICK) for n in r[::-1])
+            if len(r) != 3 or min(r) < 2 or t.dtype != torch.int32 or tuple(t.shape) != want:
+                raise ValueError(f"level {lvl}: table {t.dtype} {tuple(t.shape)} for {r} points, need int32 {want}")
+            if p.dtype != torch.int32 or p.dim() != 5 or tuple(p.shape[1:]) != (BRICK, BRICK, BRICK, 2):
+                raise ValueError(f"level {lvl}: pool {p.dtype} {tuple(p.shape)}, need int32 [num_bricks, 8, 8, 8, 2]")
+            if t.numel() and not (int(t.min()) >= -1 and int(t.max()) < p.shape[0]):
+                raise ValueError(f"level {lvl}: table entries in [{int(t.min())}, {int(t.max())}], need -1 or a "
+                                 f"brick id below {p.shape[0]}")
+            bricks.append((t.contiguous(), p.contiguous()))
+            res.append(r)
+        grid = cls.__new__(cls)
+        grid._setup(None, bricks, res, sh, occupancy, bounds, degree, rgb_padding, block, sh_scale, sh_offset)
+        return grid
+
+    def _setup(self, cells, bricks, resolutions, sh, occupancy, bounds, degree, rgb_padding, block, sh_scale,
+               sh_offset) -> None:
+        """The constructors' shared part: `cells` (dense) or `bricks` (sparse, per level (table, pool)), one of them
+        None, with the (nx, ny, nz) of each level."""
         self.degree = int(degree)
         self.rgb_padding = float(rgb_padding)
         self.block = int(block)
@@ -151,21 +211,22 @@ class BakedGrid:
         quantized = sh_scale is not None
         if quantized and not (len(sh_scale) == len(sh_offset) == len(sh)):
             raise ValueError(f"{len(sh_scale)} / {len(sh_offset)} levels of sh_scale / sh_offset, {len(sh)} of sh")
-        self.cells, self.sh = [], []
-        for lvl, (d, i, c) in enumerate(zip(densities, indices, sh)):
-            if d.shape != i.shape or d.dim() != 3 or c.dim() != 3 or tuple(c.shape[1:]) != (nc, 3):
-                raise ValueError(f"level {lvl}: density {tuple(d.shape)}, index {tuple(i.shape)}, sh {tuple(c.shape)}")
+        self.cells: Optional[List[torch.Tensor]] = cells  # dense: per level [nz, ny, nx, 2] int32
+        self.bricks: Optional[List[Tuple[torch.Tensor, torch.Tensor]]] = bricks  # sparse: per level (table, pool)
+        self._resolutions = [tuple(r) for r in resolutions]
+        self.sh = []
+        for lvl, c in enumerate(sh):
+            if c.dim() != 3 or tuple(c.shape[1:]) != (nc, 3):
+                raise ValueError(f"level {lvl}: sh {tuple(c.shape)}, need [M, {nc}, 3]")
             if quantized and c.dtype != torch.uint8:
                 raise ValueError(f"level {lvl}: sh of a quantized grid must be uint8, got {c.dtype}")
-            # (density bits, row) per lattice point: the kernel reads one 8-byte word per corner
-            self.cells.append(torch.stack([_f32(d).view(torch.int32), i.to(torch.int32)], dim=-1).contiguous())
             self.sh.append(c.detach().contiguous() if quantized else _f32(c))
         self.sh_scale: Optional[List[torch.Tensor]] = None  # quantized: per level fp32 [nc, 3]
         self.sh_offset: Optional[List[torch.Tensor]] = None
         if quantized:
             self.sh_scale, self.sh_offset = [], []
             for lvl, (s, o) in enumerate(zip(sh_scale, sh_offset)):
-                s, o = _f32(s).to(self.cells[0].device), _f32(o).to(self.cells[0].device)
+                s, o = _f32(s).to(self.device), _f32(o).to(self.device)
                 if tuple(s.shape) != (nc, 3) or tuple(o.shape) != (nc, 3):
                     raise ValueError(f"level {lvl}: sh_scale {tuple(s.shape)}, sh_offset {tuple(o.shape)}, need {(nc, 3)}")
                 if not bool(torch.isfinite(s).all() and torch.isfinite(o).all()):
@@ -180,7 +241,7 @@ class BakedGrid:
                     pad[lvl, :nc] = tab.cpu().numpy()
                 self._deq_host.append(pad)
         self.occupancy = occupancy.to(torch.uint8).contiguous()
-        n0 = tuple(self.cells[0].shape[:3])
+        n0 = self._resolutions[0][::-1]
         want = tuple(-(-(n - 1) // self.block) for n in n0)
         if tuple(self.occupancy.shape) != want:
             raise ValueError(f"occupancy {tuple(self.occupancy.shape)}: need {want} for block {self.block}")
@@ -196,6 +257,8 @@ class BakedGrid:
         (`_struct`, `density`, `save`): projected onto >= 0, scattered into the kept points, occupancy rebuilt.  The
         kept set and the rows never change.  False syncs and turns the parameters back into plain tensors.  A quantized
         grid is not trainable: fine-tune before `quantize`, or train `dequantize()`."""
+        if requires_grad:
+            self._refuse_sparse("requires_grad_")
         if requires_grad and self.quantized:
             raise ValueError("BakedGrid.requires_grad_: a quantized grid is not trainable; the order is bake -> prune -> "
                              "fine-tune -> quantize, or fine-tune dequantize()")
@@ -230,6 +293,11 @@ class BakedGrid:
         """Whether the SH rows are uint8 (`quantize`)."""
         return self.sh_scale is not None
 
+    @property
+    def sparse(self) -> bool:
+        """Whether the cells are 8^3-point bricks (`sparsify`)."""
+        return self.bricks is not None
+
     def parameters(self) -> List[torch.Tensor]:
         """[kept_density_0, sh_0, kept_density_1, sh_1, ...] of a trainable grid."""
         if self.kept_density is None:
@@ -250,25 +318,49 @@ class BakedGrid:
 
     @property
     def levels(self) -> int:
-        return len(self.cells)
+        return len(self.sh)
 
     @property
     def device(self) -> torch.device:
-        return self.cells[0].device
+        return self.sh[0].device
 
     @property
     def resolutions(self) -> List[Tuple[int, int, int]]:
         """(nx, ny, nz) per level."""
-        return [tuple(c.shape[2::-1]) for c in self.cells]
+        return list(self._resolutions)
 
     def density(self, level: int = 0) -> torch.Tensor:
-        """The baked density [nz, ny, nx] of a level (a view)."""
+        """The baked density [nz, ny, nx] of a level: a view of a dense grid's cells, or on a sparse grid a copy
+        rebuilt from the bricks."""
+        if self.sparse:
+            return self._dense_cells(level)[..., 0].view(torch.float32)
         self._sync()
         return self.cells[level][..., 0].view(torch.float32)
 
     def index(self, level: int = 0) -> torch.Tensor:
-        """The SH row of each lattice point [nz, ny, nx] int32, -1 where not kept (a view)."""
+        """The SH row of each lattice point [nz, ny, nx] int32, -1 where not kept: a view of a dense grid's cells, or
+        on a sparse grid a copy rebuilt from the bricks."""
+        if self.sparse:
+            return self._dense_cells(level)[..., 1]
         return self.cells[level][..., 1]
+
+    def _dense_cells(self, level: int, slab_bytes: int = _SLAB_BYTES) -> torch.Tensor:
+        """Level `level`'s [nz, ny, nx, 2] cells rebuilt from a sparse grid's bricks, in slabs of brick layers."""
+        table, pool = self.bricks[level]
+        nz, ny, nx = self._resolutions[level][::-1]
+        tz, ty, tx = table.shape
+        cells = torch.empty(nz, ny, nx, 2, dtype=torch.int32, device=table.device)
+        step = _slab_layers(ty, tx, slab_bytes)
+        for z0 in range(0, tz, step):
+            z1 = min(z0 + step, tz)
+            tab = table[z0:z1]
+            b = _empty_words((z1 - z0, ty, tx, BRICK, BRICK, BRICK), table.device)
+            stored = tab >= 0
+            b[stored] = pool[tab[stored].long()]
+            dense = b.permute(0, 3, 1, 4, 2, 5, 6).reshape((z1 - z0) * BRICK, ty * BRICK, tx * BRICK, 2)
+            zn = min(z1 * BRICK, nz) - z0 * BRICK
+            cells[z0 * BRICK:z0 * BRICK + zn] = dense[:zn, :ny, :nx]
+        return cells
 
     @property
     def kept(self) -> List[int]:
@@ -276,8 +368,10 @@ class BakedGrid:
 
     @property
     def nbytes(self) -> int:
+        """Bytes held: cells (dense array, or brick pools and tables), SH rows, quantization tables and occupancy."""
         tables = self.sh_scale + self.sh_offset if self.quantized else []
-        return sum(t.numel() * t.element_size() for t in self.cells + self.sh + tables) + self.occupancy.numel()
+        cells = [t for pair in self.bricks for t in pair] if self.sparse else self.cells
+        return sum(t.numel() * t.element_size() for t in cells + self.sh + tables) + self.occupancy.numel()
 
     def default_step(self) -> float:
         """Half the finest level's smallest voxel edge."""
@@ -287,10 +381,10 @@ class BakedGrid:
     def _struct(self) -> "_cabi.Grid":
         self._sync()
         g = _cabi.Grid()
-        for lvl, (c, s) in enumerate(zip(self.cells, self.sh)):
-            nz, ny, nx = c.shape[:3]
+        for lvl, (s, (nx, ny, nz)) in enumerate(zip(self.sh, self._resolutions)):
             fp32_rows = s.data_ptr() if s.numel() and not self.quantized else None  # a quantized grid's are in _sh_u8
-            g.levels[lvl] = _cabi.GridLevel(c.data_ptr(), fp32_rows, nx, ny, nz)
+            cells = None if self.sparse else self.cells[lvl].data_ptr()  # a sparse grid's are in _bricks
+            g.levels[lvl] = _cabi.GridLevel(cells, fp32_rows, nx, ny, nz)
         g.num_levels, g.degree = self.levels, self.degree
         g.lo = (C.c_float * 3)(*self.bounds[0])
         g.hi = (C.c_float * 3)(*self.bounds[1])
@@ -307,11 +401,20 @@ class BakedGrid:
         C.memmove(C.addressof(t.offset), offset.ctypes.data, offset.nbytes)
         return t
 
+    def _bricks_struct(self) -> "_cabi.GridBricks":
+        """The brick tables and pools of a sparse grid, as mipnerf_b200_grid_render_bricks takes them."""
+        b = _cabi.GridBricks()
+        for lvl, (table, pool) in enumerate(self.bricks):
+            b.table[lvl] = table.data_ptr()
+            b.pool[lvl] = pool.data_ptr() if pool.numel() else None
+        return b
+
     def render(self, rays: Rays, white_bkgd: bool = True, step: Optional[float] = None):
         """(rgb [B,3], distance [B], acc [B]) of flat rays on the grid's device, marched every `step` along |d| (default
         `default_step()`).  Differentiable in `parameters()` when the grid is trainable and grad mode is on (rays that
         require grad are refused: there is no ray gradient).  A quantized grid renders on
-        mipnerf_b200_grid_render_u8, bit for bit as its `dequantize()` renders."""
+        mipnerf_b200_grid_render_u8, bit for bit as its `dequantize()` renders; a sparse grid on
+        mipnerf_b200_grid_render_bricks, bit for bit as its `densify()` renders."""
         if self.kept_density is None or not torch.is_grad_enabled():
             with torch.no_grad():
                 return self._render(rays, white_bkgd, step)[0]
@@ -322,7 +425,7 @@ class BakedGrid:
 
     def _render(self, rays: Rays, white_bkgd: bool, step: Optional[float]):
         """((rgb, distance, acc), the fp32 ray fields the launch read, the step it used)."""
-        dev = _dev(self.cells[0])
+        dev = _dev(self.sh[0])
         o = rays.origins.reshape(-1, 3)
         if o.device != dev:
             raise ValueError(f"rays on {o.device}, grid on {dev}")
@@ -335,7 +438,11 @@ class BakedGrid:
         acc = torch.empty(n, device=dev)
         st = self.default_step() if step is None else float(step)
         out = (int(bool(white_bkgd)), rgb.data_ptr(), dist.data_ptr(), acc.data_ptr())
-        if self.quantized:
+        if self.sparse:
+            _call(dev, "grid_render_bricks", _cabi.lib().mipnerf_b200_grid_render_bricks, C.byref(g),
+                  C.byref(self._bricks_struct()), C.byref(self._sh_u8()) if self.quantized else None, C.byref(rs), st,
+                  *out)
+        elif self.quantized:
             _call(dev, "grid_render_u8", _cabi.lib().mipnerf_b200_grid_render_u8, C.byref(g), C.byref(self._sh_u8()),
                   C.byref(rs), st, *out)
         else:
@@ -349,8 +456,9 @@ class BakedGrid:
         point's colour (level weight times trilinear weight).  With `out` (such tensors, e.g. from an earlier call),
         the scores are raised into it in place and it is returned, so calls over batches of rays accumulate.  The
         result is bit-reproducible under any order or split of the rays.  `step` defaults to `default_step()` as in
-        `render`; a prune by these scores only holds for renders at the same step.  Not on a quantized grid: prune
-        before `quantize`."""
+        `render`; a prune by these scores only holds for renders at the same step.  Not on a quantized or sparse grid:
+        prune before `quantize` and `sparsify`."""
+        self._refuse_sparse("visibility")
         self._refuse_quantized("visibility")
         dev = _dev(self.cells[0])
         o = rays.origins.reshape(-1, 3)
@@ -378,8 +486,9 @@ class BakedGrid:
         SH-row order, as `visibility` returns) is > `weight_threshold`; `self` is left as it is.  A point pruned away
         gets density 0 and index -1; the kept points' rows are renumbered in x-fastest order and their SH rows carried
         over bit for bit; the occupancy is rebuilt by `grid_occupancy`; bounds, degree, rgb_padding and block are
-        copied.  Plain torch on the grid's device (CPU tensors too).  Not on a quantized grid: prune before
-        `quantize`."""
+        copied.  Plain torch on the grid's device (CPU tensors too).  Not on a quantized or sparse grid: prune before
+        `quantize` and `sparsify`."""
+        self._refuse_sparse("prune")
         self._refuse_quantized("prune")
         self._sync()
         if len(max_weight) != self.levels:
@@ -401,6 +510,11 @@ class BakedGrid:
         return BakedGrid(dens, indices, sh, grid_occupancy(dens, self.block), self.bounds, self.degree,
                          self.rgb_padding, self.block)
 
+    def _refuse_sparse(self, what: str) -> None:
+        if self.sparse:
+            raise ValueError(f"BakedGrid.{what}: the grid is sparse (brick cells); the order is bake -> prune -> "
+                             f"fine-tune -> quantize -> sparsify, or use densify()")
+
     def _refuse_quantized(self, what: str) -> None:
         if self.quantized:
             raise ValueError(f"BakedGrid.{what}: the grid is quantized; the order is bake -> prune -> fine-tune -> "
@@ -414,7 +528,8 @@ class BakedGrid:
         reads as fl(fl(q * scale) + offset), within scale / 2 (plus a few ulp of the column's magnitude) of c.  A
         trainable grid is synced first and its detached values are used; `self` is left as it is.  The cells,
         indices, occupancy, bounds, degree, rgb_padding and block are copied.  Plain, deterministic torch on the
-        grid's device (CPU tensors too).  Non-finite rows are refused."""
+        grid's device (CPU tensors too).  Non-finite rows are refused.  Not on a sparse grid."""
+        self._refuse_sparse("quantize")
         if self.quantized:
             raise ValueError("BakedGrid.quantize: the grid is already quantized")
         self._sync()
@@ -447,7 +562,9 @@ class BakedGrid:
     @torch.no_grad()
     def dequantize(self) -> "BakedGrid":
         """The fp32 grid of a quantized one: SH rows fl(fl(q * scale) + offset) (eager torch: one rounded multiply,
-        then one rounded add), everything else copied.  It renders bit for bit as the quantized grid does."""
+        then one rounded add), everything else copied.  It renders bit for bit as the quantized grid does.  Not on a
+        sparse grid."""
+        self._refuse_sparse("dequantize")
         if not self.quantized:
             raise ValueError("BakedGrid.dequantize: the grid is not quantized (fp32 rows)")
         rows = [q.to(torch.float32) * s + o for q, s, o in zip(self.sh, self.sh_scale, self.sh_offset)]
@@ -455,18 +572,77 @@ class BakedGrid:
                          [self.index(lvl) for lvl in range(self.levels)], rows, self.occupancy.clone(), self.bounds,
                          self.degree, self.rgb_padding, self.block)
 
+    @torch.no_grad()
+    def sparsify(self, slab_bytes: int = _SLAB_BYTES) -> "BakedGrid":
+        """A new grid whose cells keep only each level's non-empty bricks of 8^3 lattice points (module docstring,
+        "Memory layout"); `self` is left as it is.  Lossless: it renders bit for bit as `self`, and `densify()` gives
+        back every array bit for bit.  The SH rows (fp32 or uint8), quantization tables, occupancy, bounds, degree,
+        rgb_padding and block are copied.  A trainable grid is synced first and its detached values are used.  Plain,
+        deterministic torch on the grid's device (CPU tensors too), in slabs of brick layers of about `slab_bytes`
+        bytes of dense cells each, so that its transient memory stays near the size of the result."""
+        if self.sparse:
+            raise ValueError("BakedGrid.sparsify: the grid is already sparse")
+        self._sync()
+        tables, pools = [], []
+        for c in self.cells:
+            nz, ny, nx = c.shape[:3]
+            t = (-(-nz // BRICK), -(-ny // BRICK), -(-nx // BRICK))
+            step = _slab_layers(t[1], t[2], slab_bytes)
+            table = torch.empty(t, dtype=torch.int32, device=c.device)
+            count = 0
+            for z0 in range(0, t[0], step):  # the table: stored bricks numbered in raster order
+                z1 = min(z0 + step, t[0])
+                b = _brick_slab(c, z0, z1, t)
+                stored = ((b[..., 0] != 0) | (b[..., 1] != -1)).flatten(3).any(-1)
+                ids = torch.cumsum(stored.reshape(-1), 0).view(stored.shape) - 1 + count
+                table[z0:z1] = torch.where(stored, ids, torch.full((), -1, device=c.device)).to(torch.int32)
+                count += int(stored.sum())
+            pool = torch.empty(count, BRICK, BRICK, BRICK, 2, dtype=torch.int32, device=c.device)
+            for z0 in range(0, t[0], step):  # the pool, filled slab by slab
+                z1 = min(z0 + step, t[0])
+                tab = table[z0:z1]
+                stored = tab >= 0
+                pool[tab[stored].long()] = _brick_slab(c, z0, z1, t)[stored]
+            tables.append(table)
+            pools.append(pool)
+        q = self.quantized
+        return BakedGrid.from_bricks(tables, pools, self.resolutions, [s.detach().clone() for s in self.sh],
+                                     self.occupancy.clone(), self.bounds, self.degree, self.rgb_padding, self.block,
+                                     [s.clone() for s in self.sh_scale] if q else None,
+                                     [o.clone() for o in self.sh_offset] if q else None)
+
+    @torch.no_grad()
+    def densify(self, slab_bytes: int = _SLAB_BYTES) -> "BakedGrid":
+        """The dense grid of a sparse one (`sparsify`'s inverse, bit for bit in every array), in slabs of brick
+        layers; `self` is left as it is."""
+        if not self.sparse:
+            raise ValueError("BakedGrid.densify: the grid is not sparse (dense cells)")
+        q = self.quantized
+        cells = [self._dense_cells(lvl, slab_bytes) for lvl in range(self.levels)]
+        return BakedGrid([c[..., 0].view(torch.float32) for c in cells], [c[..., 1] for c in cells],
+                         [s.clone() for s in self.sh], self.occupancy.clone(), self.bounds, self.degree,
+                         self.rgb_padding, self.block, [s.clone() for s in self.sh_scale] if q else None,
+                         [o.clone() for o in self.sh_offset] if q else None)
+
     def save(self, path: str) -> None:
         """One .npz: per level density, index and sh, plus occupancy, bounds, degree, rgb_padding and block (format
         1).  A quantized grid writes format 2: sh_{l} is its uint8 rows, plus sh_scale_{l} and sh_offset_{l} fp32
-        [(degree + 1)^2, 3]."""
+        [(degree + 1)^2, 3].  A sparse grid writes format 3: per level table_{l} and pool_{l} in place of density_{l}
+        and index_{l}, `resolutions` int32 [levels, 3] (nx, ny, nz), and its rows as format 1 or 2 does."""
         self._sync()
-        fmt = _FORMAT_U8 if self.quantized else _FORMAT
+        fmt = _FORMAT_BRICKS if self.sparse else _FORMAT_U8 if self.quantized else _FORMAT
         arrays = {"format": np.int32(fmt), "levels": np.int32(self.levels), "degree": np.int32(self.degree),
                   "rgb_padding": np.float32(self.rgb_padding), "block": np.int32(self.block),
                   "bounds": np.asarray(self.bounds, dtype=np.float32), "occupancy": self.occupancy.cpu().numpy()}
+        if self.sparse:
+            arrays["resolutions"] = np.asarray(self._resolutions, dtype=np.int32)
         for lvl in range(self.levels):
-            arrays[f"density_{lvl}"] = self.density(lvl).cpu().numpy()
-            arrays[f"index_{lvl}"] = self.index(lvl).cpu().numpy()
+            if self.sparse:
+                arrays[f"table_{lvl}"] = self.bricks[lvl][0].cpu().numpy()
+                arrays[f"pool_{lvl}"] = self.bricks[lvl][1].cpu().numpy()
+            else:
+                arrays[f"density_{lvl}"] = self.density(lvl).cpu().numpy()
+                arrays[f"index_{lvl}"] = self.index(lvl).cpu().numpy()
             arrays[f"sh_{lvl}"] = self.sh[lvl].detach().cpu().numpy()
             if self.quantized:
                 arrays[f"sh_scale_{lvl}"] = self.sh_scale[lvl].cpu().numpy()
@@ -477,19 +653,54 @@ class BakedGrid:
     def load(cls, path: str, device="cuda") -> "BakedGrid":
         with np.load(path) as z:
             fmt = int(z["format"])
-            if fmt not in (_FORMAT, _FORMAT_U8):
-                raise ValueError(f"{path}: baked-grid format {fmt}, this library reads {_FORMAT} and {_FORMAT_U8}")
+            if fmt not in (_FORMAT, _FORMAT_U8, _FORMAT_BRICKS):
+                raise ValueError(f"{path}: baked-grid format {fmt}, this library reads {_FORMAT}, {_FORMAT_U8} and "
+                                 f"{_FORMAT_BRICKS}")
             levels = int(z["levels"])
             t = lambda name: torch.from_numpy(np.ascontiguousarray(z[name])).to(device)  # noqa: E731
             bounds = z["bounds"].astype(np.float64)
             tables = {}
-            if fmt == _FORMAT_U8:
+            if fmt == _FORMAT_U8 or fmt == _FORMAT_BRICKS and "sh_scale_0" in z.files:
                 tables = {"sh_scale": [t(f"sh_scale_{lvl}") for lvl in range(levels)],
                           "sh_offset": [t(f"sh_offset_{lvl}") for lvl in range(levels)]}
+            if fmt == _FORMAT_BRICKS:
+                want = ["resolutions"] + [f"{k}_{lvl}" for lvl in range(levels) for k in ("table", "pool", "sh")]
+                missing = [k for k in want if k not in z.files]
+                if missing:
+                    raise ValueError(f"{path}: baked-grid format {fmt} without its arrays {missing}")
+                return cls.from_bricks([t(f"table_{lvl}") for lvl in range(levels)],
+                                       [t(f"pool_{lvl}") for lvl in range(levels)],
+                                       [tuple(int(n) for n in r) for r in z["resolutions"]],
+                                       [t(f"sh_{lvl}") for lvl in range(levels)], t("occupancy"),
+                                       (tuple(bounds[0]), tuple(bounds[1])), int(z["degree"]), float(z["rgb_padding"]),
+                                       int(z["block"]), **tables)
             return cls([t(f"density_{lvl}") for lvl in range(levels)], [t(f"index_{lvl}") for lvl in range(levels)],
                        [t(f"sh_{lvl}") for lvl in range(levels)], t("occupancy"),
                        (tuple(bounds[0]), tuple(bounds[1])), int(z["degree"]), float(z["rgb_padding"]), int(z["block"]),
                        **tables)
+
+
+def _slab_layers(ty: int, tx: int, slab_bytes: int) -> int:
+    """Brick layers per slab: as many as fit `slab_bytes` of dense cells, at least one."""
+    return max(1, int(slab_bytes) // (ty * tx * BRICK ** 3 * 8))
+
+
+def _empty_words(shape, device) -> torch.Tensor:
+    """[*shape, 2] int32 whose every word is (+0.0 bits, -1), the word of a point that is not kept."""
+    w = torch.empty(*shape, 2, dtype=torch.int32, device=device)
+    w[..., 0] = 0
+    w[..., 1] = -1
+    return w
+
+
+def _brick_slab(cells: torch.Tensor, z0: int, z1: int, t) -> torch.Tensor:
+    """Brick layers [z0, z1) of dense cells [nz, ny, nx, 2] as [z1 - z0, ty, tx, 8, 8, 8, 2] (a view of a padded
+    copy), points past the lattice holding (0, -1)."""
+    nz, ny, nx = cells.shape[:3]
+    pad = _empty_words(((z1 - z0) * BRICK, t[1] * BRICK, t[2] * BRICK), cells.device)
+    zs = cells[z0 * BRICK:min(z1 * BRICK, nz)]
+    pad[:zs.shape[0], :ny, :nx] = zs
+    return pad.view(z1 - z0, BRICK, t[1], BRICK, t[2], BRICK, 2).permute(0, 2, 4, 1, 3, 5, 6)
 
 
 class _GridRender(torch.autograd.Function):

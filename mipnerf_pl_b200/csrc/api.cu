@@ -146,8 +146,9 @@ int check_rays(const mipnerf_b200_rays* r) {
 }
 
 // The grid description of mipnerf_b200_grid_render, its backward and mipnerf_b200_grid_visibility (`g` checked
-// non-NULL by the caller).
-int check_grid(const mipnerf_b200_grid* g) {
+// non-NULL by the caller).  With `bricks` (mipnerf_b200_grid_render_bricks, checked non-NULL by the caller) the
+// cells are the bricks: every levels[l].cells must be NULL and every bricks->table[l] set.
+int check_grid(const mipnerf_b200_grid* g, const mipnerf_b200_grid_bricks* bricks = nullptr) {
   if (g->num_levels < 1 || g->num_levels > MIPNERF_B200_GRID_MAX_LEVELS)
     return fail(MIPNERF_B200_EINVAL, "num_levels=%d: need 1..%d", g->num_levels, MIPNERF_B200_GRID_MAX_LEVELS);
   if (g->degree < 0 || g->degree > 3) return fail(MIPNERF_B200_EINVAL, "degree=%d: need 0..3", g->degree);
@@ -162,12 +163,31 @@ int check_grid(const mipnerf_b200_grid* g) {
   const int32_t* n0 = &g->levels[0].nx;
   for (int l = 0; l < g->num_levels; ++l) {
     const mipnerf_b200_grid_level& lv = g->levels[l];
-    if (!lv.cells) return fail(MIPNERF_B200_EINVAL, "level %d: cells is NULL", l);
+    if (!bricks && !lv.cells) return fail(MIPNERF_B200_EINVAL, "level %d: cells is NULL", l);
+    if (bricks && lv.cells)
+      return fail(MIPNERF_B200_EINVAL, "level %d: levels[%d].cells is set; the cells are read from bricks", l, l);
+    if (bricks && !bricks->table[l]) return fail(MIPNERF_B200_EINVAL, "level %d: bricks->table[%d] is NULL", l, l);
     const int32_t n[3] = {lv.nx, lv.ny, lv.nz};
     for (int a = 0; a < 3; ++a)
       if (n[a] < 2 || (int64_t)(n[a] - 1) << l != (int64_t)n0[a] - 1)
         return fail(MIPNERF_B200_EINVAL, "level %d: %d x %d x %d points, need >= 2 per axis and (n_0 - 1) / 2^%d + 1",
                     l, lv.nx, lv.ny, lv.nz, l);
+  }
+  return MIPNERF_B200_OK;
+}
+
+// The uint8 rows of mipnerf_b200_grid_render_u8 and mipnerf_b200_grid_render_bricks (`sh` checked non-NULL by the
+// caller): no levels[l].sh, finite scale / offset entries in use.
+int check_sh_u8(const mipnerf_b200_grid* g, const mipnerf_b200_grid_sh_u8* sh) {
+  const int nc = (g->degree + 1) * (g->degree + 1);
+  for (int l = 0; l < g->num_levels; ++l) {
+    if (g->levels[l].sh)
+      return fail(MIPNERF_B200_EINVAL, "level %d: levels[%d].sh is set; the uint8 rows are read from sh->rows", l, l);
+    for (int k = 0; k < nc; ++k)
+      for (int ch = 0; ch < 3; ++ch)
+        if (!std::isfinite(sh->scale[l][k][ch]) || !std::isfinite(sh->offset[l][k][ch]))
+          return fail(MIPNERF_B200_EINVAL, "level %d coefficient %d channel %d: scale=%g offset=%g, need finite", l, k,
+                      ch, sh->scale[l][k][ch], sh->offset[l][k][ch]);
   }
   return MIPNERF_B200_OK;
 }
@@ -2079,17 +2099,25 @@ int mipnerf_b200_grid_render_u8(const mipnerf_b200_grid* g, const mipnerf_b200_g
   if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
   if ((rc = check_grid(g))) return rc;
   if (!sh) return fail(MIPNERF_B200_EINVAL, "sh is NULL");
-  const int nc = (g->degree + 1) * (g->degree + 1);
-  for (int l = 0; l < g->num_levels; ++l) {
-    if (g->levels[l].sh)
-      return fail(MIPNERF_B200_EINVAL, "level %d: levels[%d].sh is set; the uint8 rows are read from sh->rows", l, l);
-    for (int k = 0; k < nc; ++k)
-      for (int ch = 0; ch < 3; ++ch)
-        if (!std::isfinite(sh->scale[l][k][ch]) || !std::isfinite(sh->offset[l][k][ch]))
-          return fail(MIPNERF_B200_EINVAL, "level %d coefficient %d channel %d: scale=%g offset=%g, need finite", l, k,
-                      ch, sh->scale[l][k][ch], sh->offset[l][k][ch]);
-  }
+  if ((rc = check_sh_u8(g, sh))) return rc;
   CUDA_TRY(mipnerf::launch_grid_render_u8(*g, *sh, *rays, step, white_bkgd, rgb, distance, acc, (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_grid_render_bricks(const mipnerf_b200_grid* g, const mipnerf_b200_grid_bricks* bricks,
+                                    const mipnerf_b200_grid_sh_u8* sh_u8, const mipnerf_b200_rays* rays, float step,
+                                    int white_bkgd, float* rgb, float* distance, float* acc, void* stream) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_rays(rays))) return rc;
+  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
+  if (rays->num_rays > 0 && (!rgb || !distance || !acc)) return fail(MIPNERF_B200_EINVAL, "rgb / distance / acc is NULL");
+  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
+  if (!bricks) return fail(MIPNERF_B200_EINVAL, "bricks is NULL");
+  if ((rc = check_grid(g, bricks))) return rc;
+  if (sh_u8 && (rc = check_sh_u8(g, sh_u8))) return rc;
+  CUDA_TRY(mipnerf::launch_grid_render_bricks(*g, *bricks, sh_u8, *rays, step, white_bkgd, rgb, distance, acc,
+                                              (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

@@ -12,7 +12,8 @@
 //     density is 0 on the cell's lattice points widened by one point of that level, so every skipped sample, and any
 //     sample a rounding error away from the cell, interpolates to exactly 0 at every level: skipping is bit-exact.
 //   * Density at the level(s) picked by the cone footprint is trilinear over the packed (density, SH row) lattice
-//     points (one 8-byte load per corner).  Colour is evaluated only where the density is non-zero: each kept corner's
+//     points (one 8-byte load per corner), read from the dense cells or, in mipnerf_b200_grid_render_bricks, from
+//     8^3-point bricks through a brick table.  Colour is evaluated only where the density is non-zero: each kept corner's
 //     raw colour Y(viewdir) . c, blended with the corner weights and the level weights, then the model's sigmoid.
 #include <cuda_runtime.h>
 #include <math.h>
@@ -70,9 +71,74 @@ __device__ int64_t first_past(float thr, float near, float dt, int64_t k0, int64
   return k;
 }
 
+// Cell readers: how level_density reads the 8-byte (density bits, SH row) words of one level.  `cells.level(g, l)` is
+// level l's reader, and `.cell(lv, i)` (lv = g.lv[l], i the cell's low corner, 0 <= i <= n - 2 per axis) the cell,
+// whose `(dx, dy, dz)` is the word of corner i + (dx, dy, dz).  DenseCells reads GLevel::cells, the [nz, ny, nx]
+// array.  BrickCells reads the 8^3-point bricks of mipnerf_b200_grid_render_bricks.  Both run the one march below.
+struct DenseCells {
+  struct Cell {
+    const int2* p;
+    int64_t sy, sz;
+    __device__ __forceinline__ int2 operator()(int dx, int dy, int dz) const { return __ldg(p + dx + dy * sy + dz * sz); }
+  };
+  struct Level {
+    __device__ __forceinline__ Cell cell(const GLevel& l, const int (&i)[3]) const {
+      const int64_t base = ((int64_t)i[2] * l.n[1] + i[1]) * l.n[0] + i[0];
+      return {l.cells + base, l.n[0], (int64_t)l.n[0] * l.n[1]};
+    }
+  };
+  __device__ __forceinline__ Level level(const GParams&, int) const { return {}; }
+};
+
+// Lattice point (i, j, k) is point (i & 7, j & 7, k & 7) of brick (i >> 3, j >> 3, k >> 3); a brick's table entry is
+// its id in the pool, or -1 for a brick not stored, whose words all read (+0.0 bits, -1).  Along each axis the cell's
+// two corners share a brick unless the low corner is the brick's last point (i & 7 == 7), so 7 of 8 cells per axis
+// lie in one brick.  The cell therefore looks up the low corner's brick once and each other corner's only when that
+// corner crosses a brick face on an axis where the cell does: a predicated load, not a branch, so the common cell costs
+// one table load and a warp whose threads disagree does not diverge.  The kernel takes this by value as a
+// __grid_constant__ parameter.
+struct BrickCells {
+  mipnerf_b200_grid_bricks t;
+  struct Cell {
+    const int* table;
+    const int2* pool;
+    int o[3];      // the low corner's local point in its brick
+    bool nx[3];    // whether the high corner is in the next brick along the axis
+    int64_t bs[3];  // table strides (1, tx, tx * ty)
+    int64_t b0;    // the low corner's table entry
+    int id0;
+    __device__ __forceinline__ int2 operator()(int dx, int dy, int dz) const {
+      int id = id0;
+      if ((dx && nx[0]) || (dy && nx[1]) || (dz && nx[2]))
+        id = __ldg(table + b0 + (dx && nx[0] ? bs[0] : 0) + (dy && nx[1] ? bs[1] : 0) + (dz && nx[2] ? bs[2] : 0));
+      const int local = ((((o[2] + dz) & 7) << 3 | ((o[1] + dy) & 7)) << 3) | ((o[0] + dx) & 7);
+      return id >= 0 ? __ldg(pool + (int64_t)id * 512 + local) : make_int2(0, -1);
+    }
+  };
+  struct Level {
+    const int* table;
+    const int2* pool;
+    __device__ __forceinline__ Cell cell(const GLevel& l, const int (&i)[3]) const {
+      Cell c;
+      c.table = table, c.pool = pool;
+      const int64_t tx = (l.n[0] + 7) >> 3, ty = (l.n[1] + 7) >> 3;
+      c.bs[0] = 1, c.bs[1] = tx, c.bs[2] = tx * ty;
+#pragma unroll
+      for (int a = 0; a < 3; ++a) c.o[a] = i[a] & 7, c.nx[a] = c.o[a] == 7;
+      c.b0 = ((int64_t)(i[2] >> 3) * ty + (i[1] >> 3)) * tx + (i[0] >> 3);
+      c.id0 = __ldg(table + c.b0);
+      return c;
+    }
+  };
+  __device__ __forceinline__ Level level(const GParams&, int l) const {
+    return {t.table[l], reinterpret_cast<const int2*>(t.pool[l])};
+  }
+};
+
 // Trilinear density of one level at position x: also the corner rows and weights, for the colour.
-__device__ __forceinline__ float level_density(const GLevel& l, const float (&lo)[3], const float (&x)[3],
-                                               int (&row)[8], float (&wc)[8]) {
+template <class CellLevel>
+__device__ __forceinline__ float level_density(const GLevel& l, const CellLevel cells, const float (&lo)[3],
+                                               const float (&x)[3], int (&row)[8], float (&wc)[8]) {
   int i[3];
   float f[3];
 #pragma unroll
@@ -81,13 +147,12 @@ __device__ __forceinline__ float level_density(const GLevel& l, const float (&lo
     i[a] = min((int)u, l.n[a] - 2);
     f[a] = u - (float)i[a];
   }
-  const int64_t base = ((int64_t)i[2] * l.n[1] + i[1]) * l.n[0] + i[0];
-  const int64_t sy = l.n[0], sz = (int64_t)l.n[0] * l.n[1];
+  const auto cell = cells.cell(l, i);
   float sigma = 0.f;
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
     const int dx = c & 1, dy = (c >> 1) & 1, dz = c >> 2;
-    const int2 v = __ldg(l.cells + base + dx + dy * sy + dz * sz);
+    const int2 v = cell(dx, dy, dz);
     wc[c] = (dx ? f[0] : 1.f - f[0]) * (dy ? f[1] : 1.f - f[1]) * (dz ? f[2] : 1.f - f[2]);
     row[c] = v.y;
     sigma += wc[c] * __int_as_float(v.x);
@@ -275,13 +340,17 @@ struct Blend {
   float w_a[8], w_b[8];
 };
 
-__device__ __forceinline__ float blend_density(const GParams& g, float radius, float t, const float (&x)[3], Blend& b) {
+template <class Cells>
+__device__ __forceinline__ float blend_density(const GParams& g, const Cells& cells, float radius, float t,
+                                               const float (&x)[3], Blend& b) {
   float lam = log2f(kSqrt3 * radius * t / g.s0_max);
   lam = fminf(fmaxf(lam, 0.f), (float)(g.num_levels - 1));  // NaN -> 0
   b.la = min((int)lam, g.num_levels - 1);
   b.f = b.la == g.num_levels - 1 ? 0.f : lam - (float)b.la;
-  float sigma = level_density(g.lv[b.la], g.lo, x, b.row_a, b.w_a);
-  if (b.f > 0.f) sigma = (1.f - b.f) * sigma + b.f * level_density(g.lv[b.la + 1], g.lo, x, b.row_b, b.w_b);
+  float sigma = level_density(g.lv[b.la], cells.level(g, b.la), g.lo, x, b.row_a, b.w_a);
+  if (b.f > 0.f)
+    sigma = (1.f - b.f) * sigma +
+            b.f * level_density(g.lv[b.la + 1], cells.level(g, b.la + 1), g.lo, x, b.row_b, b.w_b);
   return sigma;
 }
 
@@ -308,9 +377,9 @@ __device__ __forceinline__ void composite(Composite& s, float alpha, const float
 }
 
 // The forward march of one ray: every sample with non-zero density composited, up to the one that leaves T < 1e-4.
-template <int NC, class Rows>
-__device__ __forceinline__ void march(const GParams& g, const Rows& rows, const RayMarch& m, const float (&y)[16],
-                                      Composite& s) {
+template <int NC, class Rows, class Cells>
+__device__ __forceinline__ void march(const GParams& g, const Rows& rows, const Cells& cells, const RayMarch& m,
+                                      const float (&y)[16], Composite& s) {
   for (int64_t k = m.k0; k < m.k1;) {
     float t, x[3];
     if (!sample_at(g, m, k, t, x)) {
@@ -319,7 +388,7 @@ __device__ __forceinline__ void march(const GParams& g, const Rows& rows, const 
     }
     if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
     Blend b;
-    const float sigma = blend_density(g, m.radius, t, x, b);
+    const float sigma = blend_density(g, cells, m.radius, t, x, b);
     ++k;
     if (!(sigma != 0.f)) continue;
     const float alpha = 1.f - expf(-sigma * m.delta);
@@ -332,18 +401,18 @@ __device__ __forceinline__ void march(const GParams& g, const Rows& rows, const 
   }
 }
 
-template <int NC, class Rows>
+template <int NC, class Rows, class Cells>
 __global__ void __launch_bounds__(kGridThreads)
     grid_render_kernel(const GParams g, const mipnerf_b200_rays rays, float step, int white_bkgd,
                        float* __restrict__ rgb_out, float* __restrict__ dist_out, float* __restrict__ acc_out,
-                       const __grid_constant__ Rows rows) {
+                       const __grid_constant__ Rows rows, const __grid_constant__ Cells cells) {
   const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
   if (r >= rays.num_rays) return;
   RayMarch m;
   float y[16];
   ray_setup(g, rays, r, step, m, y);
   Composite s;
-  march<NC>(g, rows, m, y, s);
+  march<NC>(g, rows, cells, m, y, s);
   const float bg = white_bkgd ? 1.f - s.acc : 0.f;
   rgb_out[3 * r] = s.c[0] + bg;
   rgb_out[3 * r + 1] = s.c[1] + bg;
@@ -405,7 +474,7 @@ __global__ void __launch_bounds__(kGridThreads)
   float y[16];
   ray_setup(g, rays, r, step, m, y);
   Composite total;
-  march<NC>(g, F32Rows{}, m, y, total);
+  march<NC>(g, F32Rows{}, DenseCells{}, m, y, total);
   if (!(total.dist >= m.near && total.dist <= m.far)) g_dist = 0.f;  // the clamp passes the gradient inside, inclusive
 
   Composite s;
@@ -417,7 +486,7 @@ __global__ void __launch_bounds__(kGridThreads)
     }
     if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
     Blend b;
-    const float sigma = blend_density(g, m.radius, t, x, b);
+    const float sigma = blend_density(g, DenseCells{}, m.radius, t, x, b);
     ++k;
     // a zero density still has a gradient; it reaches parameters only through kept corners
     const bool zero = !(sigma != 0.f);
@@ -487,7 +556,7 @@ __global__ void __launch_bounds__(kGridThreads)
     }
     if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
     Blend b;
-    const float sigma = blend_density(g, m.radius, t, x, b);
+    const float sigma = blend_density(g, DenseCells{}, m.radius, t, x, b);
     ++k;
     if (!(sigma != 0.f)) continue;
     const float alpha = 1.f - expf(-sigma * m.delta);
@@ -534,15 +603,17 @@ GParams make_params(const mipnerf_b200_grid& grid) {
 
 namespace {
 
-template <class Rows>
+template <class Rows, class Cells>
 cudaError_t launch_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step, int white_bkgd,
-                          float* rgb, float* distance, float* acc, const Rows& rows, KernelId id, cudaStream_t st) {
+                          float* rgb, float* distance, float* acc, const Rows& rows, const Cells& cells, KernelId id,
+                          cudaStream_t st) {
   if (rays.num_rays == 0) return cudaSuccess;
   const GParams g = make_params(grid);
   const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
   LaunchScope scope(id, st);
-#define MIPNERF_GRID_FWD(NC) \
-  grid_render_kernel<NC, Rows><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc, rows)
+#define MIPNERF_GRID_FWD(NC)                                                                                           \
+  grid_render_kernel<NC, Rows, Cells><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc, \
+                                                                       rows, cells)
   switch (grid.degree) {
     case 0: MIPNERF_GRID_FWD(1); break;
     case 1: MIPNERF_GRID_FWD(4); break;
@@ -557,13 +628,25 @@ cudaError_t launch_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays
 
 cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
                                int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st) {
-  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, F32Rows{}, kKernGridRender, st);
+  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, F32Rows{}, DenseCells{}, kKernGridRender,
+                       st);
 }
 
 cudaError_t launch_grid_render_u8(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_sh_u8& sh,
                                   const mipnerf_b200_rays& rays, float step, int white_bkgd, float* rgb,
                                   float* distance, float* acc, cudaStream_t st) {
-  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, U8Rows{sh}, kKernGridRenderU8, st);
+  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, U8Rows{sh}, DenseCells{}, kKernGridRenderU8,
+                       st);
+}
+
+cudaError_t launch_grid_render_bricks(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks& bricks,
+                                      const mipnerf_b200_grid_sh_u8* sh, const mipnerf_b200_rays& rays, float step,
+                                      int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st) {
+  if (sh)
+    return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, U8Rows{*sh}, BrickCells{bricks},
+                         kKernGridRenderBricks, st);
+  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, F32Rows{}, BrickCells{bricks},
+                       kKernGridRenderBricks, st);
 }
 
 cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,

@@ -8,6 +8,7 @@
 #include "draws.h"
 
 struct mipnerf_b200_grid;  // include/mipnerf_b200.h
+struct mipnerf_b200_grid_bricks;
 struct mipnerf_b200_grid_grads;
 struct mipnerf_b200_grid_sh_u8;
 struct mipnerf_b200_rays;
@@ -77,6 +78,10 @@ cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200
 cudaError_t launch_grid_render_u8(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_sh_u8& sh,
                                   const mipnerf_b200_rays& rays, float step, int white_bkgd, float* rgb,
                                   float* distance, float* acc, cudaStream_t st);
+// sh NULL: fp32 rows (levels[l].sh); otherwise the uint8 rows of *sh
+cudaError_t launch_grid_render_bricks(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks& bricks,
+                                      const mipnerf_b200_grid_sh_u8* sh, const mipnerf_b200_rays& rays, float step,
+                                      int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st);
 cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
                                         int white_bkgd, const float* d_rgb, const float* d_distance,
                                         const float* d_acc, const mipnerf_b200_grid_grads& grads, cudaStream_t st);

@@ -3,14 +3,15 @@ render the spheric video path from the grid.
 
     python tools/bake_grid.py --ckpt last.ckpt --out GRID.npz [--resolution 257] [--levels 1] [--threshold 0.01]
         [--degree 2] [--bounds -1.5 -1.5 -1.5 1.5 1.5 1.5] [--precision bf16] [--prune DATA_DIR]
-        [--weight-threshold 1e-5] [--quantize] [--frames DIR] [--size 800]
+        [--weight-threshold 1e-5] [--quantize] [--sparse] [--frames DIR] [--size 800]
 
 Level l has (n - 1) / 2^l + 1 points per axis (n - 1 divisible by 2^(levels - 1)).  Lattice points farther than one
 point from any point of density > threshold are dropped (density 0).  With --prune, the kept points that no pixel of
 the Blender scene's train split sees (largest blending weight times colour coefficient <= --weight-threshold over
 every training ray, `mp.prune_grid`) are dropped as well, before the grid is saved.  With --quantize, the SH rows are
 stored as uint8 with a per-level, per-coefficient affine code (`BakedGrid.quantize`, after any pruning; the .npz is
-then format 2).  With --frames, the 120 poses of
+then format 2).  With --sparse, each level's cells keep only their non-empty bricks of 8^3 points
+(`BakedGrid.sparsify`, last, after any pruning and quantization; lossless; the .npz is then format 3).  With --frames, the 120 poses of
 `metrics.spheric_path()` are rendered from the grid with `render_baked_frame` and written with `save_images`
 (<idx>_rgb.png, _dist.png, _acc.png).  A saved grid renders without the checkpoint: `mp.BakedGrid.load(path)`.
 """
@@ -43,6 +44,7 @@ def main(argv=None):
                     help="prune by visibility from the train split of this Blender scene")
     ap.add_argument("--weight-threshold", type=float, default=mp.baked.DEFAULT_WEIGHT_THRESHOLD)
     ap.add_argument("--quantize", action="store_true", help="store the SH rows in 8 bits (after --prune)")
+    ap.add_argument("--sparse", action="store_true", help="keep only the non-empty 8^3 bricks of the cells (last)")
     ap.add_argument("--frames", default=None, metavar="DIR", help="render the spheric path from the grid into DIR")
     ap.add_argument("--size", type=int, default=800, help="frame height and width for --frames")
     ap.add_argument("--device", default="cuda:0")
@@ -70,6 +72,14 @@ def main(argv=None):
         grid = grid.quantize()
         torch.cuda.synchronize()
         print(f"quantized the SH rows to 8 bits: {summary(grid)}, in {time.perf_counter() - t0:.2f} s")
+    if args.sparse:
+        print(f"before sparsify: {summary(grid)}")
+        t0 = time.perf_counter()
+        grid = grid.sparsify()
+        torch.cuda.synchronize()
+        stored = [f"{int(p.shape[0])}/{t.numel()}" for t, p in grid.bricks]
+        print(f"sparsified the cells into 8^3 bricks (stored / table entries per level {stored}): {summary(grid)}, in "
+              f"{time.perf_counter() - t0:.2f} s")
     grid.save(args.out)
     print(f"{args.out}: written")
     if args.frames:
