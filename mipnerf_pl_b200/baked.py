@@ -41,6 +41,10 @@ Sparse cells (`BakedGrid.sparsify`, the occupied blocks PlenOctrees and SNeRG st
 of each level, fp32 or quantized rows alike; `densify` restores the dense grid bit for bit.  A sparse grid is a
 viewer format, the last step of bake -> prune -> fine-tune -> quantize -> sparsify: it renders
 (mipnerf_b200_grid_render_bricks) and saves, and is not pruned, trained or (de)quantized.
+
+Streamed bakes (`bake_grid(sparse=True)`, `sparse_grid_structure`) write the sparse layout directly, walking each
+level in z-slabs of brick layers, so that a bake at 1025^3 or 2049^3 never holds a level's whole lattice; the result
+equals the dense bake followed by `sparsify()` in every array.
 """
 from __future__ import annotations
 
@@ -92,6 +96,24 @@ def _cell_matrix(n_cells: int, n_points: int, block: int, scale: int, device) ->
     return ((p >= first) & (p <= last)).to(torch.float32)
 
 
+def _keep_mask(density: torch.Tensor, threshold: float) -> torch.Tensor:
+    """The kept points of fp32 densities [nz, ny, nx]: the 3x3x3 dilation of density > threshold, nothing kept past
+    the array's ends."""
+    return torch.nn.functional.max_pool3d((density > threshold).to(torch.float32)[None, None], 3, 1, 1)[0, 0] > 0
+
+
+def _occupancy_counts(nonzero: torch.Tensor, z0: int, nz: int, o, block: int, scale: int) -> torch.Tensor:
+    """Per macro cell [oz, oy, ox] fp32, how many of the 0/1 points `nonzero` (lattice layers [z0, z0 + its depth) of a
+    level of nz layers and point spacing `scale` finest cells) lie on the cell's lattice points widened by one point.
+    Every count is an exact integer below 2^24, so `> 0` of a sum of such counts is exact."""
+    dev = nonzero.device
+    ax, ay = (_cell_matrix(o[2 - a], nonzero.shape[2 - a], block, scale, dev) for a in range(2))
+    az = _cell_matrix(o[0], nz, block, scale, dev)[:, z0:z0 + nonzero.shape[0]]
+    t = torch.einsum("kji,ai->kja", nonzero, ax)
+    t = torch.einsum("kja,bj->kba", t, ay)
+    return torch.einsum("kba,ck->cba", t, az)
+
+
 @torch.no_grad()
 def grid_structure(densities: Sequence[torch.Tensor], threshold: float, block: int = DEFAULT_BLOCK):
     """The mask, index and occupancy construction from the density grids of every level (no model; any device) ->
@@ -114,7 +136,7 @@ def grid_structure(densities: Sequence[torch.Tensor], threshold: float, block: i
         if tuple(dens.shape) != want:
             raise ValueError(f"level {lvl}: grid {tuple(dens.shape)}, need {want} nested in level 0's {n0}")
         d = dens.to(torch.float32)
-        keep = torch.nn.functional.max_pool3d((d > threshold).to(torch.float32)[None, None], 3, 1, 1)[0, 0] > 0
+        keep = _keep_mask(d, threshold)
         bd = torch.where(keep, d, torch.zeros((), device=dev))
         idx = torch.full(bd.shape, -1, dtype=torch.int32, device=dev)
         idx[keep] = torch.arange(int(keep.sum()), dtype=torch.int32, device=dev)
@@ -133,14 +155,78 @@ def grid_occupancy(baked_densities: Sequence[torch.Tensor], block: int = DEFAULT
     o = [-(-(n - 1) // block) for n in n0]  # (oz, oy, ox)
     occ = torch.zeros(o, dtype=torch.float32, device=dev)
     for lvl, bd in enumerate(baked_densities):
-        want = tuple(bd.shape)
-        nz = (bd != 0).to(torch.float32)
-        s = 1 << lvl
-        ax, ay, az = (_cell_matrix(o[2 - a], want[2 - a], block, s, dev) for a in range(3))
-        t = torch.einsum("kji,ai->kja", nz, ax)
-        t = torch.einsum("kja,bj->kba", t, ay)
-        occ += torch.einsum("kba,ck->cba", t, az)
+        occ += _occupancy_counts((bd != 0).to(torch.float32), 0, bd.shape[0], o, block, 1 << lvl)
     return (occ > 0).to(torch.uint8)
+
+
+_MAX_ROWS = 2 ** 31 - 1  # SH row ids are int32
+
+
+@torch.no_grad()
+def sparse_grid_structure(density_fn, resolution: Resolution, levels: int = 1, threshold: float = DEFAULT_THRESHOLD,
+                          block: int = DEFAULT_BLOCK, slab: Optional[int] = None):
+    """`grid_structure` followed by the dense constructor and `sparsify()`, streamed: each level is walked in z-slabs
+    of `slab` brick layers (lattice layers [8 z0, 8 z1); None: the whole level), so that no array the size of a
+    level's lattice is ever held.  `density_fn(level, z0, z1)` returns that level's densities on lattice layers [z0,
+    z1) as [z1 - z0, ny, nx] (level l of `level_resolutions(resolution, levels)`).  Returns (tables, pools, positions,
+    occupancy): per level the int32 brick table and pool of `sparsify`, the int64 lattice positions (x fastest, z
+    slowest) of the kept points in SH-row order, and the uint8 occupancy of `grid_occupancy`, every array bit for bit
+    as the dense path gives it.  A level whose kept points would not fit int32 row ids is refused."""
+    res = level_resolutions(resolution, levels)
+    scale_max = 1 << (len(res) - 1)
+    if int(block) < 1 or int(block) % scale_max:
+        raise ValueError(f"block {block}: need a positive multiple of 2^(levels - 1) = {scale_max}")
+    if slab is not None and int(slab) < 1:
+        raise ValueError(f"slab {slab}: need >= 1 brick layer, or None for the whole level")
+    o = tuple(-(-(n - 1) // int(block)) for n in res[0][::-1])
+    occ = None
+    tables, pools, positions = [], [], []
+    for lvl, (nx, ny, nz) in enumerate(res):
+        t = (-(-nz // BRICK), -(-ny // BRICK), -(-nx // BRICK))
+        step = t[0] if slab is None else int(slab)
+        tabs, bricks, pos = [], [], []
+        rows = count = 0
+        for b0 in range(0, t[0], step):
+            b1 = min(b0 + step, t[0])
+            z0, z1 = b0 * BRICK, min(b1 * BRICK, nz)
+            # The halo: the keep mask's 3x3x3 dilation reads density > threshold one layer beyond the slab on each
+            # side, clipped at the lattice ends (where max_pool3d's padding keeps nothing, as on the whole level).
+            # The occupancy needs no halo: each slab adds its own points' counts to every macro cell whose widened
+            # lattice points hold them, and the cell is occupied iff any slab's count is non-zero.
+            h0, h1 = max(z0 - 1, 0), min(z1 + 1, nz)
+            d = density_fn(lvl, h0, h1)
+            if tuple(d.shape) != (h1 - h0, ny, nx):
+                raise ValueError(f"density_fn({lvl}, {h0}, {h1}): shape {tuple(d.shape)}, need {(h1 - h0, ny, nx)}")
+            d = d.to(torch.float32)
+            keep = _keep_mask(d, threshold)[z0 - h0:z1 - h0]
+            d = d[z0 - h0:z1 - h0]
+            dev = d.device
+            k = int(keep.sum())
+            if rows + k > _MAX_ROWS:
+                raise ValueError(f"level {lvl}: more than {_MAX_ROWS} kept points, beyond int32 SH row ids; use a "
+                                 f"coarser resolution or a higher threshold")
+            pos.append(keep.reshape(-1).nonzero().reshape(-1) + z0 * ny * nx)
+            idx = torch.full(keep.shape, -1, dtype=torch.int32, device=dev)
+            idx[keep] = torch.arange(rows, rows + k, dtype=torch.int32, device=dev)
+            rows += k
+            bd = torch.where(keep, d, torch.zeros((), device=dev))
+            del d, keep
+            counts = _occupancy_counts((bd != 0).to(torch.float32), z0, nz, o, int(block), 1 << lvl)
+            occ = counts > 0 if occ is None else occ | (counts > 0)
+            b = _brick_slab(torch.stack([bd.view(torch.int32), idx], dim=-1), 0, b1 - b0, t)
+            del bd, idx
+            tab, stored, count = _number_bricks(b, count)
+            tabs.append(tab)
+            # each slab's stored bricks stay a tensor of their own and are joined once per level: one copy per brick
+            # and a transient of one pool, where growing one buffer by doubling copies up to twice and peaks at three
+            # pools, and a count pass then a fill pass would query every density twice
+            bricks.append(b[stored])
+            del b
+        tables.append(torch.cat(tabs))
+        pools.append(torch.cat(bricks))
+        del bricks
+        positions.append(torch.cat(pos))
+    return tables, pools, positions, occ.to(torch.uint8)
 
 
 class BakedGrid:
@@ -533,28 +619,7 @@ class BakedGrid:
         if self.quantized:
             raise ValueError("BakedGrid.quantize: the grid is already quantized")
         self._sync()
-        nc = (self.degree + 1) ** 2
-        rows, scales, offsets = [], [], []
-        for lvl, c in enumerate(self.sh):
-            c = c.detach()
-            if not bool(torch.isfinite(c).all()):
-                raise ValueError(f"BakedGrid.quantize: level {lvl} has non-finite SH coefficients")
-            if c.shape[0] == 0:
-                scale = offset = torch.zeros(nc, 3, device=c.device)
-                q = torch.empty(0, nc, 3, dtype=torch.uint8, device=c.device)
-            else:
-                offset, hi = c.amin(dim=0), c.amax(dim=0)
-                # a tensor divisor: CUDA torch turns a Python-scalar divisor into a multiply by its reciprocal, which
-                # is not the correctly rounded quotient the CPU gives
-                scale = (hi - offset) / torch.full_like(hi, 255.0)
-                if not bool(torch.isfinite(scale).all()):
-                    raise ValueError(f"BakedGrid.quantize: level {lvl}: a column's range overflows fp32")
-                live = scale > 0
-                code = torch.round((c - offset) / torch.where(live, scale, torch.ones((), device=c.device)))
-                q = torch.where(live, code.clamp(0, 255), torch.zeros((), device=c.device)).to(torch.uint8)
-            rows.append(q)
-            scales.append(scale)
-            offsets.append(offset)
+        rows, scales, offsets = zip(*[_quantize_rows(c.detach(), lvl) for lvl, c in enumerate(self.sh)])
         return BakedGrid([self.density(lvl) for lvl in range(self.levels)],
                          [self.index(lvl) for lvl in range(self.levels)], rows, self.occupancy.clone(), self.bounds,
                          self.degree, self.rgb_padding, self.block, scales, offsets)
@@ -592,11 +657,7 @@ class BakedGrid:
             count = 0
             for z0 in range(0, t[0], step):  # the table: stored bricks numbered in raster order
                 z1 = min(z0 + step, t[0])
-                b = _brick_slab(c, z0, z1, t)
-                stored = ((b[..., 0] != 0) | (b[..., 1] != -1)).flatten(3).any(-1)
-                ids = torch.cumsum(stored.reshape(-1), 0).view(stored.shape) - 1 + count
-                table[z0:z1] = torch.where(stored, ids, torch.full((), -1, device=c.device)).to(torch.int32)
-                count += int(stored.sum())
+                table[z0:z1], _, count = _number_bricks(_brick_slab(c, z0, z1, t), count)
             pool = torch.empty(count, BRICK, BRICK, BRICK, 2, dtype=torch.int32, device=c.device)
             for z0 in range(0, t[0], step):  # the pool, filled slab by slab
                 z1 = min(z0 + step, t[0])
@@ -680,6 +741,35 @@ class BakedGrid:
                        **tables)
 
 
+@torch.no_grad()
+def _quantize_rows(c: torch.Tensor, lvl: int, chunk_rows: int = 1 << 16):
+    """The 8-bit codec of one level's fp32 SH rows [M, nc, 3] (`BakedGrid.quantize`) -> (uint8 rows [M, nc, 3],
+    scale [nc, 3], offset [nc, 3]).  The checks, column extremes and codes run `chunk_rows` rows at a time (a minimum
+    or maximum of chunk extremes is the column's, exactly), so that the transient memory is a few fp32 chunks rather
+    than copies of the rows."""
+    nc = c.shape[1]
+    chunks = [c[s:s + chunk_rows] for s in range(0, c.shape[0], chunk_rows)]
+    if not all(bool(torch.isfinite(x).all()) for x in chunks):
+        raise ValueError(f"BakedGrid.quantize: level {lvl} has non-finite SH coefficients")
+    if c.shape[0] == 0:
+        scale = offset = torch.zeros(nc, 3, device=c.device)
+        return torch.empty(0, nc, 3, dtype=torch.uint8, device=c.device), scale, offset
+    offset = torch.stack([x.amin(dim=0) for x in chunks]).amin(dim=0)
+    hi = torch.stack([x.amax(dim=0) for x in chunks]).amax(dim=0)
+    # a tensor divisor: CUDA torch turns a Python-scalar divisor into a multiply by its reciprocal, which is not the
+    # correctly rounded quotient the CPU gives
+    scale = (hi - offset) / torch.full_like(hi, 255.0)
+    if not bool(torch.isfinite(scale).all()):
+        raise ValueError(f"BakedGrid.quantize: level {lvl}: a column's range overflows fp32")
+    live = scale > 0
+    div = torch.where(live, scale, torch.ones((), device=c.device))
+    q = torch.empty(c.shape, dtype=torch.uint8, device=c.device)
+    for s in range(0, c.shape[0], chunk_rows):
+        code = torch.round((c[s:s + chunk_rows] - offset) / div)
+        q[s:s + chunk_rows] = torch.where(live, code.clamp(0, 255), torch.zeros((), device=c.device)).to(torch.uint8)
+    return q, scale, offset
+
+
 def _slab_layers(ty: int, tx: int, slab_bytes: int) -> int:
     """Brick layers per slab: as many as fit `slab_bytes` of dense cells, at least one."""
     return max(1, int(slab_bytes) // (ty * tx * BRICK ** 3 * 8))
@@ -701,6 +791,16 @@ def _brick_slab(cells: torch.Tensor, z0: int, z1: int, t) -> torch.Tensor:
     zs = cells[z0 * BRICK:min(z1 * BRICK, nz)]
     pad[:zs.shape[0], :ny, :nx] = zs
     return pad.view(z1 - z0, BRICK, t[1], BRICK, t[2], BRICK, 2).permute(0, 2, 4, 1, 3, 5, 6)
+
+
+def _number_bricks(bricks: torch.Tensor, count: int):
+    """The table entries of a slab of bricks [z, ty, tx, 8, 8, 8, 2] (`_brick_slab`) whose stored bricks are numbered
+    from `count` in raster order -> (int32 table slab [z, ty, tx], stored mask, count after the slab).  A brick is
+    stored iff one of its words is not (+0.0 bits, -1)."""
+    stored = ((bricks[..., 0] != 0) | (bricks[..., 1] != -1)).flatten(3).any(-1)
+    ids = torch.cumsum(stored.reshape(-1), 0).view(stored.shape) - 1 + count
+    table = torch.where(stored, ids, torch.full((), -1, device=bricks.device)).to(torch.int32)
+    return table, stored, count + int(stored.sum())
 
 
 class _GridRender(torch.autograd.Function):
@@ -740,30 +840,72 @@ class _GridRender(torch.autograd.Function):
 @torch.no_grad()
 def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: float = DEFAULT_THRESHOLD,
               degree: int = 2, n_theta: int = 8, bounds=DEFAULT_BOUNDS, block: int = DEFAULT_BLOCK,
-              slab_points: int = 1 << 20) -> BakedGrid:
+              slab_points: int = 1 << 20, sparse: bool = False, quantize: bool = False,
+              stream_points: int = 1 << 24) -> BakedGrid:
     """Bake `model` into a `levels`-level grid over `bounds` (level l: (n_0 - 1) / 2^l + 1 points per axis): the
     density of `field.density_grid` at its default voxel variance, the keep mask, index and occupancy of
     `grid_structure`, and the raw SH colour of the kept points' voxel Gaussians (`field.bake_sh(raw=True)`, degree
-    0..3, in slabs of `slab_points`), on the model's device."""
+    0..3, in slabs of `slab_points`), on the model's device.
+
+    `quantize`: the result of `.quantize()` on that grid.  `sparse`: the result of `.sparsify()` on it (after
+    `quantize`), bit for bit in every array, but baked without ever holding an array the size of a level's lattice:
+    `sparse_grid_structure` walks each level in z-slabs of brick layers, querying `density_grid(z_range=...)` on
+    each slab plus one layer of halo, then the kept points' SH rows are baked as above (quantized level by level once
+    a level's fp32 rows are all baked).  A slab is L = max(1, stream_points // (512 ty tx)) brick layers, with (tx,
+    ty) = ceil((nx, ny) / 8) of level 0 (coarser levels' slabs are smaller).  With P = (8 L + 2) (8 ty) (8 tx) the
+    points of level 0's slab padded to bricks with its halo, Q = min(P, max(2^22, nx ny)) the points of one density
+    query, M the kept points of all levels, M_l and B_l the kept points and stored bricks of level l, and nc = (degree
+    + 1)^2, the memory held at once beyond the returned grid, the model and the queries' workspace is at most
+
+        8 M + max(64 P + 28 Q + max_l (8 M_l + 4096 B_l),
+                  (72 + 12 nc) slab_points + [quantize] 12 nc (max_l M_l + 2^19))
+
+    bytes: per slab the densities, masks, cells and padded bricks, the positions of the kept points until their rows
+    are baked (8 M), one level's positions and pool twice while their slabs are joined, and one SH query's points and
+    output (or with `quantize` one level's fp32 rows and the codec's temporaries of 2^16 rows).  The dense bake holds
+    at least 20 bytes per point of level 0's whole lattice at once."""
     if not 0 <= int(degree) <= 3:
         raise ValueError(f"degree {degree}: need 0..3")
     res = level_resolutions(resolution, levels)
-    dens = [density_grid(model, r, bounds) for r in res]
-    baked, indices, occ = grid_structure(dens, threshold, block)
-    dev = dens[0].device
-    sh = []
-    for r, bd, idx in zip(res, baked, indices):
-        (xs, ys, zs), _ = lattice_axes(r, bounds, dev)
-        flat = (idx.reshape(-1) >= 0).nonzero().reshape(-1)
-        var = torch.tensor(voxel_variance(r, bounds), device=dev)
-        out = torch.empty(flat.numel(), (int(degree) + 1) ** 2, 3, device=dev)
-        nx, ny = r[0], r[1]
-        for s in range(0, flat.numel(), slab_points):
-            p = flat[s:s + slab_points]
-            means = torch.stack([xs[p % nx], ys[(p // nx) % ny], zs[p // (nx * ny)]], dim=-1)
-            out[s:s + len(p)] = bake_sh(model, means, var.expand(len(p), 3), degree, n_theta, raw=True)
-        sh.append(out)
-    return BakedGrid(baked, indices, sh, occ, bounds, degree, float(model.rgb_padding), block)
+    if not sparse:
+        dens = [density_grid(model, r, bounds) for r in res]
+        baked, indices, occ = grid_structure(dens, threshold, block)
+        sh = [_bake_rows(model, r, (idx.reshape(-1) >= 0).nonzero().reshape(-1), bounds, degree, n_theta, slab_points)
+              for r, idx in zip(res, indices)]
+        grid = BakedGrid(baked, indices, sh, occ, bounds, degree, float(model.rgb_padding), block)
+        return grid.quantize() if quantize else grid
+    tx, ty = -(-res[0][0] // BRICK), -(-res[0][1] // BRICK)
+    slab = max(1, int(stream_points) // (BRICK ** 3 * ty * tx))
+    tables, pools, positions, occ = sparse_grid_structure(
+        lambda lvl, z0, z1: density_grid(model, res[lvl], bounds, z_range=(z0, z1)), resolution, levels, threshold,
+        block, slab)
+    sh, scales, offsets = [], [], []
+    for lvl, r in enumerate(res):
+        rows = _bake_rows(model, r, positions[lvl], bounds, degree, n_theta, slab_points)
+        positions[lvl] = None
+        if quantize:
+            rows, scale, offset = _quantize_rows(rows, lvl)
+            scales.append(scale)
+            offsets.append(offset)
+        sh.append(rows)
+    return BakedGrid.from_bricks(tables, pools, res, sh, occ, bounds, degree, float(model.rgb_padding), block,
+                                 scales if quantize else None, offsets if quantize else None)
+
+
+def _bake_rows(model, resolution, flat: torch.Tensor, bounds, degree: int, n_theta: int,
+               slab_points: int) -> torch.Tensor:
+    """The raw SH rows [len(flat), (degree + 1)^2, 3] of the lattice points at int64 positions `flat` (x fastest) of
+    a level's lattice, `bake_sh(raw=True)` of their voxel Gaussians in calls of `slab_points` points."""
+    dev = flat.device
+    (xs, ys, zs), _ = lattice_axes(resolution, bounds, dev)
+    var = torch.tensor(voxel_variance(resolution, bounds), device=dev)
+    out = torch.empty(flat.numel(), (int(degree) + 1) ** 2, 3, device=dev)
+    nx, ny = resolution[0], resolution[1]
+    for s in range(0, flat.numel(), slab_points):
+        p = flat[s:s + slab_points]
+        means = torch.stack([xs[p % nx], ys[(p // nx) % ny], zs[p // (nx * ny)]], dim=-1)
+        out[s:s + len(p)] = bake_sh(model, means, var.expand(len(p), 3), degree, n_theta, raw=True)
+    return out
 
 
 @torch.no_grad()

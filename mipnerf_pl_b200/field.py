@@ -50,27 +50,31 @@ def lattice_axes(resolution: Resolution, bounds=DEFAULT_BOUNDS, device="cuda"):
 
 @torch.no_grad()
 def density_grid(model, resolution: Resolution, bounds=DEFAULT_BOUNDS, variance=None,
-                 slab_points: int = 1 << 22) -> torch.Tensor:
+                 slab_points: int = 1 << 22, z_range: Optional[Tuple[int, int]] = None) -> torch.Tensor:
     """Density (softplus(raw + density_bias)) of `model` on a lattice -> [nz, ny, nx] on the model's device.  Point
     (i, j, k) sits at lo + (i, j, k) * step; `variance` (a float or one per axis) is the diagonal covariance of every
     query, by default step**2 / 12 per axis; 0 gives a point-sampled grid.  Queried in z-slabs of at most
-    `slab_points` points, so that the memory beyond the grid stays bounded.  Under no_grad: no graph, even on an
-    autograd model."""
+    `slab_points` points, so that the memory beyond the grid stays bounded.  `z_range` (z0, z1): only lattice layers
+    [z0, z1), as [z1 - z0, ny, nx], equal bit for bit to those rows of the whole grid (the points are the same and
+    the queries do not depend on how the points are batched).  Under no_grad: no graph, even on an autograd model."""
     dev = next(model.parameters()).device
     nx, ny, nz = _resolution(resolution)
+    z0, z1 = (0, nz) if z_range is None else (int(z_range[0]), int(z_range[1]))
+    if not 0 <= z0 <= z1 <= nz:
+        raise ValueError(f"z_range {z_range!r}: need 0 <= z0 <= z1 <= nz = {nz}")
     (xs, ys, zs), step = lattice_axes((nx, ny, nz), bounds, dev)
     var = step.astype(np.float32) ** 2 / np.float32(12) if variance is None else np.broadcast_to(
         np.asarray(variance, dtype=np.float32), (3,))
     covs_row = torch.tensor(np.asarray(var, dtype=np.float32), device=dev)
-    out = torch.empty(nz, ny, nx, device=dev)
+    out = torch.empty(z1 - z0, ny, nx, device=dev)
     slab = max(1, slab_points // (nx * ny))
     yy, xx = torch.meshgrid(ys, xs, indexing="ij")
-    for z0 in range(0, nz, slab):
-        z = zs[z0:z0 + slab]
+    for s in range(z0, z1, slab):
+        z = zs[s:min(s + slab, z1)]
         means = torch.stack([xx.expand(len(z), ny, nx), yy.expand(len(z), ny, nx),
                              z[:, None, None].expand(len(z), ny, nx)], dim=-1)
         covs = covs_row.expand(len(z), ny, nx, 3)
-        out[z0:z0 + len(z)] = model.query_density(means, covs)
+        out[s - z0:s - z0 + len(z)] = model.query_density(means, covs)
     return out
 
 
