@@ -589,6 +589,15 @@ int mipnerf_b200_grid_render_backward(const mipnerf_b200_grid* grid, const mipne
 int mipnerf_b200_grid_visibility(const mipnerf_b200_grid* grid, const mipnerf_b200_rays* rays, float step,
                                  float* const* max_weight, void* stream);
 
+/* mipnerf_b200_grid_visibility on a grid whose cells are `bricks` (every levels[l].cells NULL, every bricks->table[l]
+ * non-NULL, as for mipnerf_b200_grid_render_bricks): the same march and scores, so max_weight equals, bit for bit, the
+ * dense call's on the cells the bricks encode.  The SH rows are not read, so levels[l].sh may be NULL on a grid whose
+ * rows are not baked yet (the streamed bake prunes before it bakes them); max_weight[l] is required for every level
+ * whose bricks->pool[l] is non-NULL.  No allocation, no synchronisation. */
+int mipnerf_b200_grid_visibility_bricks(const mipnerf_b200_grid* grid, const mipnerf_b200_grid_bricks* bricks,
+                                        const mipnerf_b200_rays* rays, float step, float* const* max_weight,
+                                        void* stream);
+
 /* Hardware self-test of the wgmma building blocks (descriptor / swizzle / accumulator-fragment conventions):
  * d[128,n] = a[128,k] . b[n,k]^T, 16-bit operands (precision BF16|FP16), fp32 accumulate; n in {128, 256}.
  * variant bit 0: B through a pre-swizzled image + cp.async.bulk (needs `scratch`); bit 1: A in registers (the RS form

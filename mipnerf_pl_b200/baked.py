@@ -44,7 +44,10 @@ viewer format, the last step of bake -> prune -> fine-tune -> quantize -> sparsi
 
 Streamed bakes (`bake_grid(sparse=True)`, `sparse_grid_structure`) write the sparse layout directly, walking each
 level in z-slabs of brick layers, so that a bake at 1025^3 or 2049^3 never holds a level's whole lattice; the result
-equals the dense bake followed by `sparsify()` in every array.
+equals the dense bake followed by `sparsify()` in every array.  `bake_grid(prune=bank)` prunes inside the bake: the
+visibility runs on the structure (cells and occupancy, on the bricks with `sparse`) before any SH row exists, so only
+the surviving points' rows are baked; the result equals `prune_grid` of the unpruned bake, then `quantize` and
+`sparsify`.
 """
 from __future__ import annotations
 
@@ -434,18 +437,9 @@ class BakedGrid:
         """Level `level`'s [nz, ny, nx, 2] cells rebuilt from a sparse grid's bricks, in slabs of brick layers."""
         table, pool = self.bricks[level]
         nz, ny, nx = self._resolutions[level][::-1]
-        tz, ty, tx = table.shape
         cells = torch.empty(nz, ny, nx, 2, dtype=torch.int32, device=table.device)
-        step = _slab_layers(ty, tx, slab_bytes)
-        for z0 in range(0, tz, step):
-            z1 = min(z0 + step, tz)
-            tab = table[z0:z1]
-            b = _empty_words((z1 - z0, ty, tx, BRICK, BRICK, BRICK), table.device)
-            stored = tab >= 0
-            b[stored] = pool[tab[stored].long()]
-            dense = b.permute(0, 3, 1, 4, 2, 5, 6).reshape((z1 - z0) * BRICK, ty * BRICK, tx * BRICK, 2)
-            zn = min(z1 * BRICK, nz) - z0 * BRICK
-            cells[z0 * BRICK:z0 * BRICK + zn] = dense[:zn, :ny, :nx]
+        for z0, slab in _cell_slabs(table, pool, self._resolutions[level], _slab_layers(*table.shape[1:], slab_bytes)):
+            cells[z0:z0 + slab.shape[0]] = slab
         return cells
 
     @property
@@ -793,6 +787,76 @@ def _brick_slab(cells: torch.Tensor, z0: int, z1: int, t) -> torch.Tensor:
     return pad.view(z1 - z0, BRICK, t[1], BRICK, t[2], BRICK, 2).permute(0, 2, 4, 1, 3, 5, 6)
 
 
+def _cell_slabs(table: torch.Tensor, pool: torch.Tensor, resolution, step: int):
+    """A level's dense cells rebuilt from its bricks (table [tz, ty, tx], pool [num_bricks, 8, 8, 8, 2], `resolution`
+    (nx, ny, nz)), `step` brick layers at a time: yields (z0, cells [zn, ny, nx, 2] of lattice layers [z0, z0 + zn))."""
+    nz, ny, nx = resolution[::-1]
+    tz, ty, tx = table.shape
+    for b0 in range(0, tz, step):
+        b1 = min(b0 + step, tz)
+        tab = table[b0:b1]
+        b = _empty_words((b1 - b0, ty, tx, BRICK, BRICK, BRICK), table.device)
+        stored = tab >= 0
+        b[stored] = pool[tab[stored].long()]
+        dense = b.permute(0, 3, 1, 4, 2, 5, 6).reshape((b1 - b0) * BRICK, ty * BRICK, tx * BRICK, 2)
+        zn = min(b1 * BRICK, nz) - b0 * BRICK
+        yield b0 * BRICK, dense[:zn, :ny, :nx]
+
+
+_PRUNE_CHUNK = 1 << 10  # _prune_bricks: bricks rewritten at once
+
+
+@torch.no_grad()
+def _prune_bricks(tables, pools, positions, resolutions, scores, weight_threshold: float, block: int,
+                  slab: Optional[int] = None):
+    """`BakedGrid.prune(scores, weight_threshold).sparsify()` on the structure `sparse_grid_structure` returns (per
+    level the brick table, pool and kept positions, and the scores [M_l] of the kept points in SH-row order) ->
+    (tables, pools, positions, occupancy), every array bit for bit as that path gives it.  A kept point survives iff
+    its score is > weight_threshold, and the survivors are renumbered in row order (x fastest already).  A dropped
+    point's word becomes (+0.0 bits, -1), a brick left with only such words is dropped, and the stored bricks stay in
+    raster order.  The occupancy is rebuilt from the pruned bricks in slabs of `slab` brick layers (None: the whole
+    level).  The lists `pools`, `positions` and `scores` are consumed: each pool is rewritten in place, and each level's
+    entries are released once its pruned arrays exist, so that a level's pool is held twice only while it is
+    compacted."""
+    o = tuple(-(-(n - 1) // int(block)) for n in resolutions[0][::-1])
+    out_tables, out_pools, out_positions = [], [], []
+    for lvl, table in enumerate(tables):
+        pool = pools[lvl]
+        keep = scores[lvl] > float(weight_threshold)
+        scores[lvl] = None
+        rowmap = torch.cumsum(keep, 0, dtype=torch.int32) - 1  # the new row of a surviving old row
+        rowmap[~keep] = -1
+        out_positions.append(positions[lvl][keep])
+        positions[lvl] = None
+        del keep
+        ids, count = [], 0
+        for s in range(0, pool.shape[0], _PRUNE_CHUNK):
+            w = pool[s:s + _PRUNE_CHUNK]
+            row = w[..., 1]
+            live = row >= 0
+            new = torch.full_like(row, -1)
+            new[live] = rowmap[row[live].long()]
+            w[..., 0].masked_fill_(live & (new < 0), 0)
+            w[..., 1] = new
+            tab, _, count = _number_bricks(w[None, None], count)
+            ids.append(tab.reshape(-1))
+        del rowmap
+        if pool.shape[0]:
+            ids = torch.cat(ids)  # the new id of each old brick, -1 for a brick left empty
+            out_pools.append(pool[ids >= 0])
+            out_tables.append(torch.where(table >= 0, ids[table.clamp(min=0).long()], table))
+        else:
+            out_pools.append(pool)
+            out_tables.append(table.clone())
+        pools[lvl] = pool = None
+    occ = torch.zeros(o, dtype=torch.bool, device=tables[0].device)
+    for lvl, (table, pool, r) in enumerate(zip(out_tables, out_pools, resolutions)):
+        for z0, cells in _cell_slabs(table, pool, r, table.shape[0] if slab is None else int(slab)):
+            occ |= _occupancy_counts((cells[..., 0].view(torch.float32) != 0).to(torch.float32), z0, r[2], o,
+                                     int(block), 1 << lvl) > 0
+    return out_tables, out_pools, out_positions, occ.to(torch.uint8)
+
+
 def _number_bricks(bricks: torch.Tensor, count: int):
     """The table entries of a slab of bricks [z, ty, tx, 8, 8, 8, 2] (`_brick_slab`) whose stored bricks are numbered
     from `count` in raster order -> (int32 table slab [z, ty, tx], stored mask, count after the slab).  A brick is
@@ -841,7 +905,8 @@ class _GridRender(torch.autograd.Function):
 def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: float = DEFAULT_THRESHOLD,
               degree: int = 2, n_theta: int = 8, bounds=DEFAULT_BOUNDS, block: int = DEFAULT_BLOCK,
               slab_points: int = 1 << 20, sparse: bool = False, quantize: bool = False,
-              stream_points: int = 1 << 24) -> BakedGrid:
+              stream_points: int = 1 << 24, prune=None,
+              weight_threshold: float = DEFAULT_WEIGHT_THRESHOLD) -> BakedGrid:
     """Bake `model` into a `levels`-level grid over `bounds` (level l: (n_0 - 1) / 2^l + 1 points per axis): the
     density of `field.density_grid` at its default voxel variance, the keep mask, index and occupancy of
     `grid_structure`, and the raw SH colour of the kept points' voxel Gaussians (`field.bake_sh(raw=True)`, degree
@@ -863,13 +928,40 @@ def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: f
     bytes: per slab the densities, masks, cells and padded bricks, the positions of the kept points until their rows
     are baked (8 M), one level's positions and pool twice while their slabs are joined, and one SH query's points and
     output (or with `quantize` one level's fp32 rows and the codec's temporaries of 2^16 rows).  The dense bake holds
-    at least 20 bytes per point of level 0's whole lattice at once."""
+    at least 20 bytes per point of level 0's whole lattice at once.
+
+    `prune` (a `DeviceRayBank`, or None): the result of `prune_grid(grid, prune, weight_threshold)` on the unquantized
+    dense grid, then `quantize` and `sparse` as above (bake -> prune -> quantize -> sparsify), bit for bit in every
+    array; the visibility runs at `default_step()`.  The visibility and the prune run on the structure, before any SH
+    row is baked, so only the surviving points' rows are queried.  With `sparse` the visibility reads the bricks
+    (mipnerf_b200_grid_visibility_bricks) and no array the size of a level's lattice is held either.  With M' and B'_l
+    the kept points and stored bricks of level l before the prune (M, M_l and B_l above are after it), R = min(2^20,
+    the bank's pixels) the rays of one visibility batch, and D = 4096 sum_l (B'_l - B_l) the bricks the prune drops,
+    the memory held at once beyond the returned grid, the model, the bank and the queries' workspace is at most
+
+        12 M' + D + max(64 P + 28 Q + max_l (8 M'_l + 4096 B'_l),  68 R,  24 max_l M'_l + 4096 max_l B'_l + 2^24,
+                        (72 + 12 nc) slab_points + [quantize] 12 nc (max_l M_l + 2^19))
+
+    bytes: the positions and fp32 scores of all kept points, held until the prune, and the pools of the bricks it
+    drops; then the structure pass as above; one batch of rays (68 bytes a ray); one level's pool twice while it is
+    compacted, with its new row numbers, new positions and the rewrite of 2^10 bricks at a time; and the SH rows of
+    the survivors as above."""
     if not 0 <= int(degree) <= 3:
         raise ValueError(f"degree {degree}: need 0..3")
     res = level_resolutions(resolution, levels)
     if not sparse:
         dens = [density_grid(model, r, bounds) for r in res]
         baked, indices, occ = grid_structure(dens, threshold, block)
+        if prune is not None:
+            # neither the visibility nor the prune reads the rows: degree-0 zero rows stand in for them
+            zeros = [torch.zeros(int((i >= 0).sum()), 1, 3, device=i.device) for i in indices]
+            rowless = BakedGrid(baked, indices, zeros, occ, bounds, 0, float(model.rgb_padding), block)
+            del dens, zeros, baked, indices
+            rowless = prune_grid(rowless, prune, weight_threshold)
+            baked = [rowless.density(lvl) for lvl in range(len(res))]
+            indices = [rowless.index(lvl) for lvl in range(len(res))]
+            occ = rowless.occupancy
+            del rowless
         sh = [_bake_rows(model, r, (idx.reshape(-1) >= 0).nonzero().reshape(-1), bounds, degree, n_theta, slab_points)
               for r, idx in zip(res, indices)]
         grid = BakedGrid(baked, indices, sh, occ, bounds, degree, float(model.rgb_padding), block)
@@ -879,6 +971,10 @@ def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: f
     tables, pools, positions, occ = sparse_grid_structure(
         lambda lvl, z0, z1: density_grid(model, res[lvl], bounds, z_range=(z0, z1)), resolution, levels, threshold,
         block, slab)
+    if prune is not None:
+        scores = _bricks_visibility(tables, pools, res, occ, [p.numel() for p in positions], bounds, block, prune)
+        tables, pools, positions, occ = _prune_bricks(tables, pools, positions, res, scores, weight_threshold, block,
+                                                      slab)
     sh, scales, offsets = [], [], []
     for lvl, r in enumerate(res):
         rows = _bake_rows(model, r, positions[lvl], bounds, degree, n_theta, slab_points)
@@ -890,6 +986,31 @@ def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: f
         sh.append(rows)
     return BakedGrid.from_bricks(tables, pools, res, sh, occ, bounds, degree, float(model.rgb_padding), block,
                                  scales if quantize else None, offsets if quantize else None)
+
+
+@torch.no_grad()
+def _bricks_visibility(tables, pools, resolutions, occupancy: torch.Tensor, kept: Sequence[int], bounds, block: int,
+                       bank, batch_size: int = 1 << 20) -> List[torch.Tensor]:
+    """`prune_grid`'s scores (per level fp32 [kept[l]] in SH-row order, over every pixel of `bank` in batches of
+    `batch_size`, at `default_step()`) on a sparse structure whose SH rows are not baked yet, on
+    mipnerf_b200_grid_visibility_bricks, which reads no row."""
+    dev = occupancy.device
+    rowless = BakedGrid.from_bricks(tables, pools, resolutions, [torch.empty(0, 1, 3, device=dev)] * len(tables),
+                                    occupancy, bounds, 0, 0.0, block)
+    g, b = rowless._struct(), rowless._bricks_struct()
+    scores = [torch.zeros(int(m), device=dev) for m in kept]
+    ptrs = (C.c_void_p * len(scores))(*[t.data_ptr() if t.numel() else None for t in scores])
+    step = rowless.default_step()
+    for s in range(0, bank.num_pixels, int(batch_size)):
+        rays, _ = bank.rays(torch.arange(s, min(s + int(batch_size), bank.num_pixels), device=bank.device))
+        if rays.origins.device != dev:
+            raise ValueError(f"rays on {rays.origins.device}, grid on {dev}")
+        rs, _keep = _rays_struct(rays.origins.reshape(-1, 3), rays.directions.reshape(-1, 3),
+                                 rays.viewdirs.reshape(-1, 3), rays.radii.reshape(-1), rays.near.reshape(-1),
+                                 rays.far.reshape(-1))
+        _call(dev, "grid_visibility_bricks", _cabi.lib().mipnerf_b200_grid_visibility_bricks, C.byref(g), C.byref(b),
+              C.byref(rs), step, ptrs)
+    return scores
 
 
 def _bake_rows(model, resolution, flat: torch.Tensor, bounds, degree: int, n_theta: int,

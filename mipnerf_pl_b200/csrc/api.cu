@@ -146,7 +146,8 @@ int check_rays(const mipnerf_b200_rays* r) {
 }
 
 // The grid description of mipnerf_b200_grid_render, its backward and mipnerf_b200_grid_visibility (`g` checked
-// non-NULL by the caller).  With `bricks` (mipnerf_b200_grid_render_bricks, checked non-NULL by the caller) the
+// non-NULL by the caller).  With `bricks` (mipnerf_b200_grid_render_bricks and mipnerf_b200_grid_visibility_bricks,
+// checked non-NULL by the caller) the
 // cells are the bricks: every levels[l].cells must be NULL and every bricks->table[l] set.
 int check_grid(const mipnerf_b200_grid* g, const mipnerf_b200_grid_bricks* bricks = nullptr) {
   if (g->num_levels < 1 || g->num_levels > MIPNERF_B200_GRID_MAX_LEVELS)
@@ -2152,6 +2153,26 @@ int mipnerf_b200_grid_visibility(const mipnerf_b200_grid* g, const mipnerf_b200_
     if (g->levels[l].sh && !max_weight[l])
       return fail(MIPNERF_B200_EINVAL, "level %d has kept points: max_weight[%d] is NULL", l, l);
   CUDA_TRY(mipnerf::launch_grid_visibility(*g, *rays, step, max_weight, (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_grid_visibility_bricks(const mipnerf_b200_grid* g, const mipnerf_b200_grid_bricks* bricks,
+                                        const mipnerf_b200_rays* rays, float step, float* const* max_weight,
+                                        void* stream) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_rays(rays))) return rc;
+  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
+  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
+  if (!bricks) return fail(MIPNERF_B200_EINVAL, "bricks is NULL");
+  if ((rc = check_grid(g, bricks))) return rc;
+  if (!max_weight) return fail(MIPNERF_B200_EINVAL, "max_weight is NULL");
+  // a level may have kept points wherever it stores a brick: its rows need not be baked yet, so levels[l].sh cannot
+  // tell
+  for (int l = 0; l < g->num_levels; ++l)
+    if (bricks->pool[l] && !max_weight[l])
+      return fail(MIPNERF_B200_EINVAL, "level %d stores bricks: max_weight[%d] is NULL", l, l);
+  CUDA_TRY(mipnerf::launch_grid_visibility_bricks(*g, *bricks, *rays, step, max_weight, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

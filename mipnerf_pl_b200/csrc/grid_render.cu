@@ -539,9 +539,12 @@ __device__ __forceinline__ void level_visibility(float* __restrict__ max_weight,
 // compositing arithmetic on T (w_k = T_k alpha_k exactly as `composite` forms it) and the same stop after the sample
 // that leaves T < 1e-4; no colour is evaluated.  A maximum does not depend on the order of its updates, so the result
 // is bit for bit the same across runs, across any split of the rays into calls, and under any permutation of the rays.
+// With BrickCells (mipnerf_b200_grid_visibility_bricks) every corner reads the word the dense cells hold, so the scores
+// equal the dense kernel's on the densified grid bit for bit.
+template <class Cells>
 __global__ void __launch_bounds__(kGridThreads)
     grid_visibility_kernel(const GParams g, const mipnerf_b200_rays rays, float step,
-                           const __grid_constant__ GMaxWeight max_weight) {
+                           const __grid_constant__ GMaxWeight max_weight, const __grid_constant__ Cells cells) {
   const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
   if (r >= rays.num_rays) return;
   RayMarch m;
@@ -556,7 +559,7 @@ __global__ void __launch_bounds__(kGridThreads)
     }
     if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
     Blend b;
-    const float sigma = blend_density(g, DenseCells{}, m.radius, t, x, b);
+    const float sigma = blend_density(g, cells, m.radius, t, x, b);
     ++k;
     if (!(sigma != 0.f)) continue;
     const float alpha = 1.f - expf(-sigma * m.delta);
@@ -668,16 +671,32 @@ cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mip
   return cudaGetLastError();
 }
 
-cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
-                                   float* const* max_weight, cudaStream_t st) {
+namespace {
+
+template <class Cells>
+cudaError_t launch_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
+                              float* const* max_weight, const Cells& cells, KernelId id, cudaStream_t st) {
   if (rays.num_rays == 0) return cudaSuccess;
   const GParams g = make_params(grid);
   GMaxWeight mw{};
   for (int l = 0; l < grid.num_levels; ++l) mw.w[l] = max_weight[l];
   const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
-  LaunchScope scope(kKernGridVisibility, st);
-  grid_visibility_kernel<<<blocks, kGridThreads, 0, st>>>(g, rays, step, mw);
+  LaunchScope scope(id, st);
+  grid_visibility_kernel<Cells><<<blocks, kGridThreads, 0, st>>>(g, rays, step, mw, cells);
   return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
+                                   float* const* max_weight, cudaStream_t st) {
+  return launch_visibility(grid, rays, step, max_weight, DenseCells{}, kKernGridVisibility, st);
+}
+
+cudaError_t launch_grid_visibility_bricks(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks& bricks,
+                                          const mipnerf_b200_rays& rays, float step, float* const* max_weight,
+                                          cudaStream_t st) {
+  return launch_visibility(grid, rays, step, max_weight, BrickCells{bricks}, kKernGridVisibilityBricks, st);
 }
 
 }  // namespace mipnerf

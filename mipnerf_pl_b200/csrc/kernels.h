@@ -87,6 +87,9 @@ cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mip
                                         const float* d_acc, const mipnerf_b200_grid_grads& grads, cudaStream_t st);
 cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
                                    float* const* max_weight, cudaStream_t st);
+cudaError_t launch_grid_visibility_bricks(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks& bricks,
+                                          const mipnerf_b200_rays& rays, float step, float* const* max_weight,
+                                          cudaStream_t st);
 
 // ---- metrics.cu ----
 size_t image_metrics_scratch_bytes(int height, int width, int channels);
