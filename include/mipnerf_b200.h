@@ -598,6 +598,28 @@ int mipnerf_b200_grid_visibility_bricks(const mipnerf_b200_grid* grid, const mip
                                         const mipnerf_b200_rays* rays, float step, float* const* max_weight,
                                         void* stream);
 
+/* The total-variation prior of a baked grid (Plenoxels), for fine-tuning.  Per level l, on that level's own lattice:
+ * for each kept point p (SH row r, lattice position points[l][r] = i + nx (j + ny k), r < num_points[l] = M_l) and
+ * each axis a, q = p + e_a is its forward neighbour, and
+ *   density:  D_a(p) = s(q) - sigma(p), s(q) = sigma(q) (the cell's density) when q is kept, 0 when it is dropped
+ *             (the value the renderer interpolates there);
+ *   SH:       D_a c_{k,ch}(p) = c_{k,ch}(q) - c_{k,ch}(p) when q is kept, 0 when q is dropped (it has no row);
+ *   both are 0 where q lies outside the lattice.
+ * Point p's terms are tv_density[l][r] = sqrt(eps + sum_a D_a(p)^2) and tv_sh[l][r] = sum_{k,ch} sqrt(eps + sum_a
+ * (D_a c_{k,ch}(p))^2) (the k, ch sum in row order).  TV_density and TV_sh are their sums over every level's kept
+ * points divided by M = sum_l M_l (0 when M = 0); that normalisation is the caller's.
+ * With `grads`, the call WRITES (does not add) grads->density[l][r] = weights[0] * d(sum of density terms) /
+ * dsigma(p) and grads->sh[l][r] = weights[1] * d(sum of SH terms) / dc(p), the sums over every kept point of the
+ * level.  `weights` is a device array of 2 fp32 (read only with grads).  Each entry is a fixed-order sum formed by one
+ * thread, so the gradient is bit-reproducible.  Every output may be NULL: tv_density, tv_sh and grads themselves, and
+ * any of their per-level pointers; a level whose outputs are all NULL is not read.  eps > 0 and finite.  The density
+ * is read from levels[l].cells, the coefficients from levels[l].sh (required, with points[l], where M_l > 0).
+ * points and num_points are host arrays of num_levels entries, points[l] a device int64 [M_l] array.  Every row id
+ * in the cells must be < M_l.  No allocation, no synchronisation. */
+int mipnerf_b200_grid_tv(const mipnerf_b200_grid* grid, const int64_t* const* points, const int64_t* num_points,
+                         float eps, float* const* tv_density, float* const* tv_sh, const float* weights,
+                         const mipnerf_b200_grid_grads* grads, void* stream);
+
 /* Hardware self-test of the wgmma building blocks (descriptor / swizzle / accumulator-fragment conventions):
  * d[128,n] = a[128,k] . b[n,k]^T, 16-bit operands (precision BF16|FP16), fp32 accumulate; n in {128, 256}.
  * variant bit 0: B through a pre-swizzled image + cp.async.bulk (needs `scratch`); bit 1: A in registers (the RS form

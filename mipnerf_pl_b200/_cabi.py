@@ -193,6 +193,8 @@ _SIGNATURES = {
     "mipnerf_b200_grid_visibility": (C.c_int, [C.POINTER(Grid), C.POINTER(RaysStruct), C.c_float, C.POINTER(_V), _V]),
     "mipnerf_b200_grid_visibility_bricks": (C.c_int, [C.POINTER(Grid), C.POINTER(GridBricks), C.POINTER(RaysStruct),
                                                       C.c_float, C.POINTER(_V), _V]),
+    "mipnerf_b200_grid_tv": (C.c_int, [C.POINTER(Grid), C.POINTER(_V), _i64p, C.c_float, C.POINTER(_V), C.POINTER(_V),
+                                       _V, C.POINTER(GridGrads), _V]),
     "mipnerf_b200_selftest_umma": (C.c_int, [_V, _V, _V, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),
     "mipnerf_b200_profile_enable": (C.c_int, [C.c_int]),
     "mipnerf_b200_profile_num_kernels": (C.c_int, []),

@@ -71,6 +71,9 @@ FINETUNE_LR_DENSITY = 0.1
 FINETUNE_LR_SH = 0.01
 # prune_grid's visibility threshold (README, "Pruning a baked grid by visibility")
 DEFAULT_WEIGHT_THRESHOLD = 1e-5
+# the epsilon inside every square root of BakedGrid.total_variation: it keeps the gradient finite where a point's
+# differences are all 0, and adds sqrt(TV_EPS) per point and term, far below any difference a grid resolves
+TV_EPS = 1e-8
 _FORMAT = 1
 _FORMAT_U8 = 2  # a quantized grid: uint8 SH rows plus per-level scale / offset
 _FORMAT_BRICKS = 3  # a sparse grid: per-level brick table and pool, fp32 or uint8 rows
@@ -360,18 +363,45 @@ class BakedGrid:
             return self
         if self.kept_density is not None:
             return self
-        kd, pos = [], []
+        kd, pos = [], self._row_positions()
+        for lvl, p in enumerate(pos):
+            kd.append(self.cells[lvl].view(-1, 2)[p, 0].view(torch.float32).requires_grad_(True))
+            self.sh[lvl].requires_grad_(True)
+        self.kept_density, self._kept_pos = kd, pos
+        self._synced = [t._version for t in kd]
+        return self
+
+    def _row_positions(self) -> List[torch.Tensor]:
+        """Per level the int64 lattice position (x fastest) of each SH row, [M_l] in row order; a trainable grid's are
+        built once, in `requires_grad_`."""
+        if self.kept_density is not None:
+            return self._kept_pos
+        pos = []
         for lvl in range(self.levels):
             idx = self.cells[lvl][..., 1].reshape(-1)
             flat = (idx >= 0).nonzero().reshape(-1)
             p = torch.empty_like(flat)
             p[idx[flat].long()] = flat  # the lattice position of row r
             pos.append(p)
-            kd.append(self.cells[lvl].view(-1, 2)[p, 0].view(torch.float32).requires_grad_(True))
-            self.sh[lvl].requires_grad_(True)
-        self.kept_density, self._kept_pos = kd, pos
-        self._synced = [t._version for t in kd]
-        return self
+        return pos
+
+    def total_variation(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(TV_density, TV_sh) as 0-dim fp32 tensors: the total-variation prior of Plenoxels on each level's own
+        lattice, on mipnerf_b200_grid_tv.  For each kept point p and axis a, with q = p + e_a its forward neighbour,
+        D_a = sigma(q) - sigma(p) (a dropped q reads 0, the density the renderer interpolates there) and D_a c_{k,ch} =
+        c_{k,ch}(q) - c_{k,ch}(p) (0 where q is dropped: a dropped point has no row); both are 0 where q lies outside
+        the lattice.  TV_density = (1/M) sum_l sum_p sqrt(TV_EPS + sum_a D_a^2) and TV_sh = (1/M) sum_l sum_p
+        sum_{k,ch} sqrt(TV_EPS + sum_a (D_a c_{k,ch})^2), M the kept points of all levels (both 0 when M = 0).  On a
+        trainable grid in grad mode both are differentiable in `parameters()`; the gradient is bit-reproducible.  A
+        trainable grid is synced first.  Not on a sparse or quantized grid: fine-tune before `quantize` and
+        `sparsify`."""
+        self._refuse_sparse("total_variation")
+        self._refuse_quantized("total_variation")
+        if self.kept_density is None or not torch.is_grad_enabled():
+            with torch.no_grad():
+                return _tv_terms(self, self._row_positions())
+        self._sync()
+        return _GridTV.apply(self, *self.parameters())
 
     @property
     def trainable(self) -> bool:
@@ -901,6 +931,60 @@ class _GridRender(torch.autograd.Function):
         return (None, None, None, None, *grads)
 
 
+def _tv_launch(grid: BakedGrid, pos, terms=None, weights=None, grads=None) -> None:
+    """mipnerf_b200_grid_tv on a dense fp32 grid: per-level terms (a pair of lists of [M_l] tensors) and / or the
+    weighted gradient (a list [density_0, sh_0, ...] with the shapes of `parameters()`, `weights` a device fp32 [2])."""
+    g = grid._struct()
+    dev = _dev(grid.cells[0])
+    n = grid.levels
+    ptrs = lambda ts: (C.c_void_p * n)(*[t.data_ptr() if t.numel() else None for t in ts])  # noqa: E731
+    gg = None
+    if grads is not None:
+        gg = _cabi.GridGrads()
+        for lvl in range(n):
+            if grads[2 * lvl + 1].numel():
+                gg.density[lvl], gg.sh[lvl] = grads[2 * lvl].data_ptr(), grads[2 * lvl + 1].data_ptr()
+    _call(dev, "grid_tv", _cabi.lib().mipnerf_b200_grid_tv, C.byref(g), ptrs(pos),
+          (C.c_int64 * n)(*[p.numel() for p in pos]), TV_EPS, None if terms is None else ptrs(terms[0]),
+          None if terms is None else ptrs(terms[1]), None if weights is None else weights.data_ptr(),
+          None if gg is None else C.byref(gg))
+
+
+def _tv_terms(grid: BakedGrid, pos) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(TV_density, TV_sh): the per-point terms summed level by level, in level order, over M."""
+    terms = ([torch.empty(p.numel(), device=grid.device) for p in pos],
+             [torch.empty(p.numel(), device=grid.device) for p in pos])
+    m = sum(p.numel() for p in pos)
+    if m == 0:
+        return torch.zeros((), device=grid.device), torch.zeros((), device=grid.device)
+    _tv_launch(grid, pos, terms=terms)
+    return tuple(torch.stack([t.sum() for t in ts]).sum() / m for ts in terms)
+
+
+class _GridTV(torch.autograd.Function):
+    """BakedGrid.total_variation of a trainable grid: the forward launches for the per-point terms and sums them; the
+    backward launches once for the gradient of both sums, weighted by the cotangents over M on the device."""
+
+    @staticmethod
+    def forward(ctx, grid, *params):
+        ctx.grid = grid
+        # the parameters the kernel reads: an in-place update before the backward raises autograd's version error
+        ctx.save_for_backward(*params)
+        return _tv_terms(grid, grid._kept_pos)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_density, d_sh):
+        params = ctx.saved_tensors
+        grid = ctx.grid
+        grads = [torch.zeros_like(p, memory_format=torch.contiguous_format) for p in params]
+        m = sum(p.numel() for p in grid._kept_pos)
+        if m:
+            weights = torch.stack([d_density, d_sh]).to(torch.float32) / m
+            _tv_launch(grid, grid._kept_pos, weights=weights, grads=grads)
+        return (None, *grads)
+
+
 @torch.no_grad()
 def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: float = DEFAULT_THRESHOLD,
               degree: int = 2, n_theta: int = 8, bounds=DEFAULT_BOUNDS, block: int = DEFAULT_BLOCK,
@@ -1061,12 +1145,18 @@ def prune_grid(grid: BakedGrid, bank, weight_threshold: float = DEFAULT_WEIGHT_T
 
 def finetune_grid(grid: BakedGrid, bank, steps: int, batch_size: int = 8192, lr_density: float = FINETUNE_LR_DENSITY,
                   lr_sh: float = FINETUNE_LR_SH, white_bkgd: bool = True, step: Optional[float] = None,
-                  generator: Optional[torch.Generator] = None) -> List[float]:
+                  generator: Optional[torch.Generator] = None, tv_density: float = 0.0,
+                  tv_sh: float = 0.0) -> List[float]:
     """Fine-tune a baked grid's kept densities and SH rows against a `DeviceRayBank`'s pixels (PlenOctrees / SNeRG
     style): per step a random batch, `grid.render`, the MSE against the targets, its backward through the grid ray
-    marcher, and one `FusedAdam` step (`lr_density` for the densities, `lr_sh` for the SH rows).  Makes the grid
-    trainable if it is not; returns the per-step losses."""
+    marcher, and one `FusedAdam` step (`lr_density` for the densities, `lr_sh` for the SH rows).  With `tv_density` or
+    `tv_sh` > 0 the loss is MSE + tv_density TV_density + tv_sh TV_sh (`BakedGrid.total_variation`, Plenoxels' prior);
+    with both 0 nothing else is launched.  Makes the grid trainable if it is not; returns the per-step MSE, without the
+    prior, so that runs with different weights compare directly."""
     from .train import FusedAdam
+    tv_density, tv_sh = float(tv_density), float(tv_sh)
+    if not (tv_density >= 0 and tv_sh >= 0):
+        raise ValueError(f"tv_density={tv_density}, tv_sh={tv_sh}: need weights >= 0")
     grid.requires_grad_(True)
     params = [p for p in grid.parameters() if p.numel()]  # a level without kept points has nothing to train
     opt = FusedAdam([{"params": [p for p in params if p.dim() == 1], "lr": float(lr_density)},
@@ -1076,9 +1166,13 @@ def finetune_grid(grid: BakedGrid, bank, steps: int, batch_size: int = 8192, lr_
         rays, target = bank.sample(batch_size, generator)
         rgb, _, _ = grid.render(rays, white_bkgd, step)
         loss = torch.mean((rgb - target) ** 2)
+        total = loss
+        if tv_density or tv_sh:
+            tv_d, tv_s = grid.total_variation()
+            total = loss + tv_density * tv_d + tv_sh * tv_s
         for p in params:
             p.grad = None
-        loss.backward()
+        total.backward()
         opt.step()
         losses.append(loss.detach())
     return torch.stack(losses).tolist() if losses else []

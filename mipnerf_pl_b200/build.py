@@ -12,7 +12,8 @@ OBJ = os.path.join(HERE, "build")
 OUT = os.path.join(HERE, "libmipnerf_b200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
-SOURCES = ["api.cu", "ray_kernels.cu", "linear_f32.cu", "mlp_tc.cu", "profile.cu", "tc_selftest.cu", "train_kernels.cu", "linear_tc.cu", "metrics.cu", "train_t16.cu", "isosurface.cu", "grid_render.cu"]
+SOURCES = ["api.cu", "ray_kernels.cu", "linear_f32.cu", "mlp_tc.cu", "profile.cu", "tc_selftest.cu", "train_kernels.cu", "linear_tc.cu", "metrics.cu", "train_t16.cu", "isosurface.cu", "grid_render.cu",
+           "grid_tv.cu"]
 
 
 def _nvcc() -> str:

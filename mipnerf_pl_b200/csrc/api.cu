@@ -145,7 +145,8 @@ int check_rays(const mipnerf_b200_rays* r) {
   return MIPNERF_B200_OK;
 }
 
-// The grid description of mipnerf_b200_grid_render, its backward and mipnerf_b200_grid_visibility (`g` checked
+// The grid description of mipnerf_b200_grid_render, its backward, mipnerf_b200_grid_visibility and
+// mipnerf_b200_grid_tv (`g` checked
 // non-NULL by the caller).  With `bricks` (mipnerf_b200_grid_render_bricks and mipnerf_b200_grid_visibility_bricks,
 // checked non-NULL by the caller) the
 // cells are the bricks: every levels[l].cells must be NULL and every bricks->table[l] set.
@@ -2173,6 +2174,30 @@ int mipnerf_b200_grid_visibility_bricks(const mipnerf_b200_grid* g, const mipner
     if (bricks->pool[l] && !max_weight[l])
       return fail(MIPNERF_B200_EINVAL, "level %d stores bricks: max_weight[%d] is NULL", l, l);
   CUDA_TRY(mipnerf::launch_grid_visibility_bricks(*g, *bricks, *rays, step, max_weight, (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_grid_tv(const mipnerf_b200_grid* g, const int64_t* const* points, const int64_t* num_points,
+                         float eps, float* const* tv_density, float* const* tv_sh, const float* weights,
+                         const mipnerf_b200_grid_grads* grads, void* stream) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_grid(g))) return rc;
+  if (!(eps > 0.f) || !std::isfinite(eps)) return fail(MIPNERF_B200_EINVAL, "eps=%g: need a finite eps > 0", eps);
+  if (!points || !num_points) return fail(MIPNERF_B200_EINVAL, "points / num_points is NULL");
+  if (grads && !weights) return fail(MIPNERF_B200_EINVAL, "grads is set: weights is NULL");
+  for (int l = 0; l < g->num_levels; ++l) {
+    const mipnerf_b200_grid_level& lv = g->levels[l];
+    const int64_t m = num_points[l], n = (int64_t)lv.nx * lv.ny * lv.nz;
+    if (m < 0 || m > n)
+      return fail(MIPNERF_B200_EINVAL, "level %d: num_points=%lld, need 0..%lld (the lattice's points)", l,
+                  (long long)m, (long long)n);
+    if (m > 0 && (!lv.sh || !points[l]))
+      return fail(MIPNERF_B200_EINVAL, "level %d has %lld kept points: levels[%d].sh / points[%d] is NULL", l,
+                  (long long)m, l, l);
+  }
+  CUDA_TRY(mipnerf::launch_grid_tv(*g, points, num_points, eps, tv_density, tv_sh, weights, grads,
+                                   (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

@@ -91,6 +91,11 @@ cudaError_t launch_grid_visibility_bricks(const mipnerf_b200_grid& grid, const m
                                           const mipnerf_b200_rays& rays, float step, float* const* max_weight,
                                           cudaStream_t st);
 
+// ---- grid_tv.cu (total-variation prior of a baked grid; arguments checked by the caller) ----
+cudaError_t launch_grid_tv(const mipnerf_b200_grid& grid, const int64_t* const* points, const int64_t* num_points,
+                           float eps, float* const* tv_density, float* const* tv_sh, const float* weights,
+                           const mipnerf_b200_grid_grads* grads, cudaStream_t st);
+
 // ---- metrics.cu ----
 size_t image_metrics_scratch_bytes(int height, int width, int channels);
 cudaError_t launch_image_metrics(const float* pred, const float* target, int height, int width, int channels,
