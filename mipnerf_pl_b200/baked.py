@@ -245,18 +245,14 @@ class BakedGrid:
                  occupancy: torch.Tensor, bounds=DEFAULT_BOUNDS, degree: int = 2, rgb_padding: float = 0.001,
                  block: int = DEFAULT_BLOCK, sh_scale: Optional[Sequence[torch.Tensor]] = None,
                  sh_offset: Optional[Sequence[torch.Tensor]] = None):
-        if not 0 <= int(degree) <= 3:
-            raise ValueError(f"degree {degree}: need 0..3")
-        if not (len(densities) == len(indices) == len(sh)) or not 1 <= len(densities) <= MAX_LEVELS:
-            raise ValueError(f"{len(densities)} / {len(indices)} / {len(sh)} levels: need the same count, 1..{MAX_LEVELS}")
         cells = []
         for lvl, (d, i, c) in enumerate(zip(densities, indices, sh)):
             if d.shape != i.shape or d.dim() != 3:
                 raise ValueError(f"level {lvl}: density {tuple(d.shape)}, index {tuple(i.shape)}, sh {tuple(c.shape)}")
             # (density bits, row) per lattice point: the kernel reads one 8-byte word per corner
             cells.append(torch.stack([_f32(d).view(torch.int32), i.to(torch.int32)], dim=-1).contiguous())
-        self._setup(cells, None, [tuple(c.shape[2::-1]) for c in cells], sh, occupancy, bounds, degree, rgb_padding,
-                    block, sh_scale, sh_offset)
+        self._setup((densities, indices, sh), "", cells, None, [tuple(c.shape[2::-1]) for c in cells], sh, occupancy,
+                    bounds, degree, rgb_padding, block, sh_scale, sh_offset)
 
     @classmethod
     def from_bricks(cls, tables: Sequence[torch.Tensor], pools: Sequence[torch.Tensor],
@@ -267,11 +263,6 @@ class BakedGrid:
         """A sparse grid from its bricks (the layout of `sparsify`): per level an int32 table [tz, ty, tx] (t = ceil(n
         / 8) of `resolutions[l]` = (nx, ny, nz)) and an int32 pool [num_bricks, 8, 8, 8, 2]; the other arguments as
         for the dense constructor.  Every table entry must be -1 or a brick id below num_bricks."""
-        if not 0 <= int(degree) <= 3:
-            raise ValueError(f"degree {degree}: need 0..3")
-        if not (len(tables) == len(pools) == len(resolutions) == len(sh)) or not 1 <= len(tables) <= MAX_LEVELS:
-            raise ValueError(f"{len(tables)} / {len(pools)} / {len(resolutions)} / {len(sh)} levels of tables / pools / "
-                             f"resolutions / sh: need the same count, 1..{MAX_LEVELS}")
         bricks, res = [], []
         for lvl, (t, p, r) in enumerate(zip(tables, pools, resolutions)):
             r = tuple(int(n) for n in r)
@@ -286,13 +277,19 @@ class BakedGrid:
             bricks.append((t.contiguous(), p.contiguous()))
             res.append(r)
         grid = cls.__new__(cls)
-        grid._setup(None, bricks, res, sh, occupancy, bounds, degree, rgb_padding, block, sh_scale, sh_offset)
+        grid._setup((tables, pools, resolutions, sh), " of tables / pools / resolutions / sh", None, bricks, res, sh,
+                    occupancy, bounds, degree, rgb_padding, block, sh_scale, sh_offset)
         return grid
 
-    def _setup(self, cells, bricks, resolutions, sh, occupancy, bounds, degree, rgb_padding, block, sh_scale,
-               sh_offset) -> None:
+    def _setup(self, per_level, names, cells, bricks, resolutions, sh, occupancy, bounds, degree,
+               rgb_padding, block, sh_scale, sh_offset) -> None:
         """The constructors' shared part: `cells` (dense) or `bricks` (sparse, per level (table, pool)), one of them
-        None, with the (nx, ny, nz) of each level."""
+        None, with the (nx, ny, nz) of each level; the per-level arguments `per_level` (`names`) need one count."""
+        if not 0 <= int(degree) <= 3:
+            raise ValueError(f"degree {degree}: need 0..3")
+        counts = [len(a) for a in per_level]
+        if len(set(counts)) != 1 or not 1 <= counts[0] <= MAX_LEVELS:
+            raise ValueError(f"{' / '.join(map(str, counts))} levels{names}: need the same count, 1..{MAX_LEVELS}")
         self.degree = int(degree)
         self.rgb_padding = float(rgb_padding)
         self.block = int(block)
@@ -536,12 +533,8 @@ class BakedGrid:
     def _render(self, rays: Rays, white_bkgd: bool, step: Optional[float]):
         """((rgb, distance, acc), the fp32 ray fields the launch read, the step it used)."""
         dev = _dev(self.sh[0])
-        o = rays.origins.reshape(-1, 3)
-        if o.device != dev:
-            raise ValueError(f"rays on {o.device}, grid on {dev}")
-        n = o.shape[0]
-        rs, keep = _rays_struct(o, rays.directions.reshape(-1, 3), rays.viewdirs.reshape(-1, 3), rays.radii.reshape(-1),
-                                rays.near.reshape(-1), rays.far.reshape(-1))
+        rs, keep = _grid_rays(rays, dev)
+        n = rs.num_rays
         g = self._struct()
         rgb = torch.empty(n, 3, device=dev)
         dist = torch.empty(n, device=dev)
@@ -571,9 +564,6 @@ class BakedGrid:
         self._refuse_sparse("visibility")
         self._refuse_quantized("visibility")
         dev = _dev(self.cells[0])
-        o = rays.origins.reshape(-1, 3)
-        if o.device != dev:
-            raise ValueError(f"rays on {o.device}, grid on {dev}")
         if out is None:
             out = [torch.zeros(m, device=dev) for m in self.kept]
         else:
@@ -582,13 +572,21 @@ class BakedGrid:
                     t.dtype != torch.float32 or t.device != dev or tuple(t.shape) != (m,) or not t.is_contiguous()
                     for t, m in zip(out, self.kept)):
                 raise ValueError(f"out: need {self.levels} contiguous fp32 tensors of shapes {self.kept} on {dev}")
-        rs, _ = _rays_struct(o, rays.directions.reshape(-1, 3), rays.viewdirs.reshape(-1, 3), rays.radii.reshape(-1),
-                             rays.near.reshape(-1), rays.far.reshape(-1))
-        g = self._struct()
-        ptrs = (C.c_void_p * self.levels)(*[t.data_ptr() if t.numel() else None for t in out])
-        st = self.default_step() if step is None else float(step)
-        _call(dev, "grid_visibility", _cabi.lib().mipnerf_b200_grid_visibility, C.byref(g), C.byref(rs), st, ptrs)
+        self._visibility(rays, step, out)
         return out
+
+    def _visibility(self, rays: Rays, step: Optional[float], out: Sequence[torch.Tensor]) -> None:
+        """`visibility`'s launch into `out`, on dense cells or (mipnerf_b200_grid_visibility_bricks) bricks.  It reads
+        no SH row, so `out` may be sized for rows not baked yet."""
+        dev = _dev(self.sh[0])
+        rs, keep = _grid_rays(rays, dev)
+        g, mw = self._struct(), _level_ptrs(out)
+        st = self.default_step() if step is None else float(step)
+        if self.sparse:
+            _call(dev, "grid_visibility_bricks", _cabi.lib().mipnerf_b200_grid_visibility_bricks, C.byref(g),
+                  C.byref(self._bricks_struct()), C.byref(rs), st, mw)
+        else:
+            _call(dev, "grid_visibility", _cabi.lib().mipnerf_b200_grid_visibility, C.byref(g), C.byref(rs), st, mw)
 
     @torch.no_grad()
     def prune(self, max_weight: Sequence[torch.Tensor], weight_threshold: float) -> "BakedGrid":
@@ -617,8 +615,7 @@ class BakedGrid:
             dens.append(torch.where(kept & ~keep, torch.zeros((), device=d.device), d))
             indices.append(idx)
             sh.append(self.sh[lvl].detach()[old[keep].long()])  # x-fastest order of the kept points
-        return BakedGrid(dens, indices, sh, grid_occupancy(dens, self.block), self.bounds, self.degree,
-                         self.rgb_padding, self.block)
+        return self._derive(dense=(dens, indices), sh=sh, occupancy=grid_occupancy(dens, self.block))
 
     def _refuse_sparse(self, what: str) -> None:
         if self.sparse:
@@ -644,9 +641,7 @@ class BakedGrid:
             raise ValueError("BakedGrid.quantize: the grid is already quantized")
         self._sync()
         rows, scales, offsets = zip(*[_quantize_rows(c.detach(), lvl) for lvl, c in enumerate(self.sh)])
-        return BakedGrid([self.density(lvl) for lvl in range(self.levels)],
-                         [self.index(lvl) for lvl in range(self.levels)], rows, self.occupancy.clone(), self.bounds,
-                         self.degree, self.rgb_padding, self.block, scales, offsets)
+        return self._derive(sh=rows, sh_tables=(scales, offsets))
 
     @torch.no_grad()
     def dequantize(self) -> "BakedGrid":
@@ -657,9 +652,7 @@ class BakedGrid:
         if not self.quantized:
             raise ValueError("BakedGrid.dequantize: the grid is not quantized (fp32 rows)")
         rows = [q.to(torch.float32) * s + o for q, s, o in zip(self.sh, self.sh_scale, self.sh_offset)]
-        return BakedGrid([self.density(lvl) for lvl in range(self.levels)],
-                         [self.index(lvl) for lvl in range(self.levels)], rows, self.occupancy.clone(), self.bounds,
-                         self.degree, self.rgb_padding, self.block)
+        return self._derive(sh=rows, sh_tables=(None, None))
 
     @torch.no_grad()
     def sparsify(self, slab_bytes: int = _SLAB_BYTES) -> "BakedGrid":
@@ -690,11 +683,7 @@ class BakedGrid:
                 pool[tab[stored].long()] = _brick_slab(c, z0, z1, t)[stored]
             tables.append(table)
             pools.append(pool)
-        q = self.quantized
-        return BakedGrid.from_bricks(tables, pools, self.resolutions, [s.detach().clone() for s in self.sh],
-                                     self.occupancy.clone(), self.bounds, self.degree, self.rgb_padding, self.block,
-                                     [s.clone() for s in self.sh_scale] if q else None,
-                                     [o.clone() for o in self.sh_offset] if q else None)
+        return self._derive(bricks=(tables, pools))
 
     @torch.no_grad()
     def densify(self, slab_bytes: int = _SLAB_BYTES) -> "BakedGrid":
@@ -702,12 +691,24 @@ class BakedGrid:
         layers; `self` is left as it is."""
         if not self.sparse:
             raise ValueError("BakedGrid.densify: the grid is not sparse (dense cells)")
-        q = self.quantized
         cells = [self._dense_cells(lvl, slab_bytes) for lvl in range(self.levels)]
-        return BakedGrid([c[..., 0].view(torch.float32) for c in cells], [c[..., 1] for c in cells],
-                         [s.clone() for s in self.sh], self.occupancy.clone(), self.bounds, self.degree,
-                         self.rgb_padding, self.block, [s.clone() for s in self.sh_scale] if q else None,
-                         [o.clone() for o in self.sh_offset] if q else None)
+        return self._derive(dense=([c[..., 0].view(torch.float32) for c in cells], [c[..., 1] for c in cells]))
+
+    def _derive(self, dense=None, bricks=None, sh=None, sh_tables=None, occupancy=None) -> "BakedGrid":
+        """A new grid with this grid's bounds, degree, rgb_padding and block, and a copy of each other part not given:
+        cells (`dense` = (densities, indices) or `bricks` = (tables, pools), per level), SH rows, quantization tables
+        (`sh_tables` = (sh_scale, sh_offset), (None, None) for fp32 rows) and occupancy."""
+        if dense is None and bricks is None:
+            dense = ([self.density(lvl) for lvl in range(self.levels)], [self.index(lvl) for lvl in range(self.levels)])
+        if sh_tables is None:
+            q = self.quantized
+            sh_tables = ([s.clone() for s in self.sh_scale], [o.clone() for o in self.sh_offset]) if q else (None, None)
+        shared = ([s.detach().clone() for s in self.sh] if sh is None else sh,
+                  self.occupancy.clone() if occupancy is None else occupancy, self.bounds, self.degree,
+                  self.rgb_padding, self.block, *sh_tables)
+        if bricks is not None:
+            return BakedGrid.from_bricks(*bricks, self.resolutions, *shared)
+        return BakedGrid(*dense, *shared)
 
     def save(self, path: str) -> None:
         """One .npz: per level density, index and sh, plus occupancy, bounds, degree, rgb_padding and block (format
@@ -897,6 +898,29 @@ def _number_bricks(bricks: torch.Tensor, count: int):
     return table, stored, count + int(stored.sum())
 
 
+def _grid_rays(rays: Rays, dev: torch.device):
+    """(RaysStruct, keep) of flat `rays` (`_rays_struct`) for a launch on the grid's device `dev`."""
+    o = rays.origins.reshape(-1, 3)
+    if o.device != dev:
+        raise ValueError(f"rays on {o.device}, grid on {dev}")
+    return _rays_struct(o, rays.directions.reshape(-1, 3), rays.viewdirs.reshape(-1, 3), rays.radii.reshape(-1),
+                        rays.near.reshape(-1), rays.far.reshape(-1))
+
+
+def _level_ptrs(ts: Sequence[torch.Tensor]):
+    """The per-level pointer array of tensors `ts`, NULL for an empty one."""
+    return (C.c_void_p * len(ts))(*[t.data_ptr() if t.numel() else None for t in ts])
+
+
+def _grid_grads(grads: Sequence[torch.Tensor]) -> "_cabi.GridGrads":
+    """The GridGrads of gradients in `parameters()` order, NULL for a level without kept points."""
+    gg = _cabi.GridGrads()
+    for lvl in range(len(grads) // 2):
+        if grads[2 * lvl + 1].numel():
+            gg.density[lvl], gg.sh[lvl] = grads[2 * lvl].data_ptr(), grads[2 * lvl + 1].data_ptr()
+    return gg
+
+
 class _GridRender(torch.autograd.Function):
     """BakedGrid.render of a trainable grid: the forward is the no-grad launch; the backward zeroes one gradient per
     parameter and adds mipnerf_b200_grid_render_backward into them."""
@@ -919,15 +943,11 @@ class _GridRender(torch.autograd.Function):
         grid = ctx.grid
         dev = _dev(grid.cells[0])
         grads = [torch.zeros_like(p, memory_format=torch.contiguous_format) for p in params]
-        gg = _cabi.GridGrads()
-        for lvl in range(grid.levels):
-            if grads[2 * lvl + 1].numel():
-                gg.density[lvl], gg.sh[lvl] = grads[2 * lvl].data_ptr(), grads[2 * lvl + 1].data_ptr()
         cot = [None if t is None else _f32(t) for t in (d_rgb, d_dist, d_acc)]
         rs = _cabi.RaysStruct(*[t.data_ptr() for t in rays_keep], ctx.num_rays)
         _call(dev, "grid_render_backward", _cabi.lib().mipnerf_b200_grid_render_backward, C.byref(grid._struct()),
               C.byref(rs), ctx.step, int(ctx.white_bkgd), *[None if t is None else t.data_ptr() for t in cot],
-              C.byref(gg))
+              C.byref(_grid_grads(grads)))
         return (None, None, None, None, *grads)
 
 
@@ -936,18 +956,10 @@ def _tv_launch(grid: BakedGrid, pos, terms=None, weights=None, grads=None) -> No
     weighted gradient (a list [density_0, sh_0, ...] with the shapes of `parameters()`, `weights` a device fp32 [2])."""
     g = grid._struct()
     dev = _dev(grid.cells[0])
-    n = grid.levels
-    ptrs = lambda ts: (C.c_void_p * n)(*[t.data_ptr() if t.numel() else None for t in ts])  # noqa: E731
-    gg = None
-    if grads is not None:
-        gg = _cabi.GridGrads()
-        for lvl in range(n):
-            if grads[2 * lvl + 1].numel():
-                gg.density[lvl], gg.sh[lvl] = grads[2 * lvl].data_ptr(), grads[2 * lvl + 1].data_ptr()
-    _call(dev, "grid_tv", _cabi.lib().mipnerf_b200_grid_tv, C.byref(g), ptrs(pos),
-          (C.c_int64 * n)(*[p.numel() for p in pos]), TV_EPS, None if terms is None else ptrs(terms[0]),
-          None if terms is None else ptrs(terms[1]), None if weights is None else weights.data_ptr(),
-          None if gg is None else C.byref(gg))
+    terms = (None, None) if terms is None else [_level_ptrs(t) for t in terms]
+    _call(dev, "grid_tv", _cabi.lib().mipnerf_b200_grid_tv, C.byref(g), _level_ptrs(pos),
+          (C.c_int64 * grid.levels)(*[p.numel() for p in pos]), TV_EPS, *terms,
+          None if weights is None else weights.data_ptr(), None if grads is None else C.byref(_grid_grads(grads)))
 
 
 def _tv_terms(grid: BakedGrid, pos) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -1056,7 +1068,11 @@ def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: f
         lambda lvl, z0, z1: density_grid(model, res[lvl], bounds, z_range=(z0, z1)), resolution, levels, threshold,
         block, slab)
     if prune is not None:
-        scores = _bricks_visibility(tables, pools, res, occ, [p.numel() for p in positions], bounds, block, prune)
+        rowless = BakedGrid.from_bricks(tables, pools, res, [torch.empty(0, 1, 3, device=occ.device)] * len(res), occ,
+                                        bounds, 0, 0.0, block)
+        scores = [torch.zeros(p.numel(), device=occ.device) for p in positions]
+        _sweep_bank(rowless, prune, rowless.default_step(), scores)
+        del rowless  # _prune_bricks releases the pools level by level
         tables, pools, positions, occ = _prune_bricks(tables, pools, positions, res, scores, weight_threshold, block,
                                                       slab)
     sh, scales, offsets = [], [], []
@@ -1070,31 +1086,6 @@ def bake_grid(model, resolution: Resolution = 257, levels: int = 1, threshold: f
         sh.append(rows)
     return BakedGrid.from_bricks(tables, pools, res, sh, occ, bounds, degree, float(model.rgb_padding), block,
                                  scales if quantize else None, offsets if quantize else None)
-
-
-@torch.no_grad()
-def _bricks_visibility(tables, pools, resolutions, occupancy: torch.Tensor, kept: Sequence[int], bounds, block: int,
-                       bank, batch_size: int = 1 << 20) -> List[torch.Tensor]:
-    """`prune_grid`'s scores (per level fp32 [kept[l]] in SH-row order, over every pixel of `bank` in batches of
-    `batch_size`, at `default_step()`) on a sparse structure whose SH rows are not baked yet, on
-    mipnerf_b200_grid_visibility_bricks, which reads no row."""
-    dev = occupancy.device
-    rowless = BakedGrid.from_bricks(tables, pools, resolutions, [torch.empty(0, 1, 3, device=dev)] * len(tables),
-                                    occupancy, bounds, 0, 0.0, block)
-    g, b = rowless._struct(), rowless._bricks_struct()
-    scores = [torch.zeros(int(m), device=dev) for m in kept]
-    ptrs = (C.c_void_p * len(scores))(*[t.data_ptr() if t.numel() else None for t in scores])
-    step = rowless.default_step()
-    for s in range(0, bank.num_pixels, int(batch_size)):
-        rays, _ = bank.rays(torch.arange(s, min(s + int(batch_size), bank.num_pixels), device=bank.device))
-        if rays.origins.device != dev:
-            raise ValueError(f"rays on {rays.origins.device}, grid on {dev}")
-        rs, _keep = _rays_struct(rays.origins.reshape(-1, 3), rays.directions.reshape(-1, 3),
-                                 rays.viewdirs.reshape(-1, 3), rays.radii.reshape(-1), rays.near.reshape(-1),
-                                 rays.far.reshape(-1))
-        _call(dev, "grid_visibility_bricks", _cabi.lib().mipnerf_b200_grid_visibility_bricks, C.byref(g), C.byref(b),
-              C.byref(rs), step, ptrs)
-    return scores
 
 
 def _bake_rows(model, resolution, flat: torch.Tensor, bounds, degree: int, n_theta: int,
@@ -1137,10 +1128,19 @@ def prune_grid(grid: BakedGrid, bank, weight_threshold: float = DEFAULT_WEIGHT_T
     if int(batch_size) < 1:
         raise ValueError(f"batch_size {batch_size}: need >= 1")
     scores = [torch.zeros(m, device=grid.device) for m in grid.kept]
+    grid._refuse_sparse("visibility")
+    grid._refuse_quantized("visibility")
+    _sweep_bank(grid, bank, step, scores, batch_size)
+    return grid.prune(scores, weight_threshold)
+
+
+def _sweep_bank(grid: BakedGrid, bank, step: Optional[float], scores: List[torch.Tensor],
+                batch_size: int = 1 << 20) -> None:
+    """Raise `scores` (per level [M_l] in SH-row order) in place to the visibility scores of every pixel of a
+    `DeviceRayBank`, in id order and batches of `batch_size`, on dense cells or bricks (`BakedGrid._visibility`)."""
     for s in range(0, bank.num_pixels, int(batch_size)):
         rays, _ = bank.rays(torch.arange(s, min(s + int(batch_size), bank.num_pixels), device=bank.device))
-        grid.visibility(rays, step, scores)
-    return grid.prune(scores, weight_threshold)
+        grid._visibility(rays, step, scores)
 
 
 def finetune_grid(grid: BakedGrid, bank, steps: int, batch_size: int = 8192, lr_density: float = FINETUNE_LR_DENSITY,

@@ -11,6 +11,7 @@
 #include "../../include/mipnerf_b200.h"
 #include "kernels.h"
 #include "mlp_tc.h"
+#include "profile.h"
 
 namespace {
 
@@ -192,6 +193,22 @@ int check_sh_u8(const mipnerf_b200_grid* g, const mipnerf_b200_grid_sh_u8* sh) {
                       ch, sh->scale[l][k][ch], sh->offset[l][k][ch]);
   }
   return MIPNERF_B200_OK;
+}
+
+// The shared prologue of the entry points that march rays through a grid, in the order they refuse: grid, rays,
+// viewdirs, the outputs (`out`: {rgb, distance, acc} of an entry point that renders, NULL for the others), the step,
+// the bricks (`bricks`: the bricks argument of a _bricks entry point, NULL for the dense ones), then check_grid.
+int check_march(const mipnerf_b200_grid* g, const mipnerf_b200_rays* rays, float* const* out, float step,
+                const mipnerf_b200_grid_bricks* const* bricks) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_rays(rays))) return rc;
+  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
+  if (out && rays->num_rays > 0 && (!out[0] || !out[1] || !out[2]))
+    return fail(MIPNERF_B200_EINVAL, "rgb / distance / acc is NULL");
+  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
+  if (bricks && !*bricks) return fail(MIPNERF_B200_EINVAL, "bricks is NULL");
+  return check_grid(g, bricks ? *bricks : nullptr);
 }
 
 mipnerf_b200_rays offset_rays(const mipnerf_b200_rays& r, int64_t off, int64_t count) {
@@ -2080,13 +2097,10 @@ int mipnerf_b200_isosurface_normals(const float* grid, int nx, int ny, int nz, c
 int mipnerf_b200_grid_render(const mipnerf_b200_grid* g, const mipnerf_b200_rays* rays, float step, int white_bkgd,
                              float* rgb, float* distance, float* acc, void* stream) {
   int rc;
-  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
-  if ((rc = check_rays(rays))) return rc;
-  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
-  if (rays->num_rays > 0 && (!rgb || !distance || !acc)) return fail(MIPNERF_B200_EINVAL, "rgb / distance / acc is NULL");
-  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
-  if ((rc = check_grid(g))) return rc;
-  CUDA_TRY(mipnerf::launch_grid_render(*g, *rays, step, white_bkgd, rgb, distance, acc, (cudaStream_t)stream));
+  float* const out[3] = {rgb, distance, acc};
+  if ((rc = check_march(g, rays, out, step, nullptr))) return rc;
+  CUDA_TRY(mipnerf::launch_grid_render(*g, nullptr, nullptr, *rays, step, white_bkgd, rgb, distance, acc,
+                                       mipnerf::kKernGridRender, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 
@@ -2094,15 +2108,12 @@ int mipnerf_b200_grid_render_u8(const mipnerf_b200_grid* g, const mipnerf_b200_g
                                 const mipnerf_b200_rays* rays, float step, int white_bkgd, float* rgb, float* distance,
                                 float* acc, void* stream) {
   int rc;
-  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
-  if ((rc = check_rays(rays))) return rc;
-  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
-  if (rays->num_rays > 0 && (!rgb || !distance || !acc)) return fail(MIPNERF_B200_EINVAL, "rgb / distance / acc is NULL");
-  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
-  if ((rc = check_grid(g))) return rc;
+  float* const out[3] = {rgb, distance, acc};
+  if ((rc = check_march(g, rays, out, step, nullptr))) return rc;
   if (!sh) return fail(MIPNERF_B200_EINVAL, "sh is NULL");
   if ((rc = check_sh_u8(g, sh))) return rc;
-  CUDA_TRY(mipnerf::launch_grid_render_u8(*g, *sh, *rays, step, white_bkgd, rgb, distance, acc, (cudaStream_t)stream));
+  CUDA_TRY(mipnerf::launch_grid_render(*g, nullptr, sh, *rays, step, white_bkgd, rgb, distance, acc,
+                                       mipnerf::kKernGridRenderU8, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 
@@ -2110,16 +2121,11 @@ int mipnerf_b200_grid_render_bricks(const mipnerf_b200_grid* g, const mipnerf_b2
                                     const mipnerf_b200_grid_sh_u8* sh_u8, const mipnerf_b200_rays* rays, float step,
                                     int white_bkgd, float* rgb, float* distance, float* acc, void* stream) {
   int rc;
-  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
-  if ((rc = check_rays(rays))) return rc;
-  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
-  if (rays->num_rays > 0 && (!rgb || !distance || !acc)) return fail(MIPNERF_B200_EINVAL, "rgb / distance / acc is NULL");
-  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
-  if (!bricks) return fail(MIPNERF_B200_EINVAL, "bricks is NULL");
-  if ((rc = check_grid(g, bricks))) return rc;
+  float* const out[3] = {rgb, distance, acc};
+  if ((rc = check_march(g, rays, out, step, &bricks))) return rc;
   if (sh_u8 && (rc = check_sh_u8(g, sh_u8))) return rc;
-  CUDA_TRY(mipnerf::launch_grid_render_bricks(*g, *bricks, sh_u8, *rays, step, white_bkgd, rgb, distance, acc,
-                                              (cudaStream_t)stream));
+  CUDA_TRY(mipnerf::launch_grid_render(*g, bricks, sh_u8, *rays, step, white_bkgd, rgb, distance, acc,
+                                       mipnerf::kKernGridRenderBricks, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 
@@ -2127,11 +2133,7 @@ int mipnerf_b200_grid_render_backward(const mipnerf_b200_grid* g, const mipnerf_
                                       int white_bkgd, const float* d_rgb, const float* d_distance, const float* d_acc,
                                       const mipnerf_b200_grid_grads* grads, void* stream) {
   int rc;
-  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
-  if ((rc = check_rays(rays))) return rc;
-  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
-  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
-  if ((rc = check_grid(g))) return rc;
+  if ((rc = check_march(g, rays, nullptr, step, nullptr))) return rc;
   if (!grads) return fail(MIPNERF_B200_EINVAL, "grads is NULL");
   for (int l = 0; l < g->num_levels; ++l)
     if (g->levels[l].sh && (!grads->density[l] || !grads->sh[l]))
@@ -2144,16 +2146,13 @@ int mipnerf_b200_grid_render_backward(const mipnerf_b200_grid* g, const mipnerf_
 int mipnerf_b200_grid_visibility(const mipnerf_b200_grid* g, const mipnerf_b200_rays* rays, float step,
                                  float* const* max_weight, void* stream) {
   int rc;
-  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
-  if ((rc = check_rays(rays))) return rc;
-  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
-  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
-  if ((rc = check_grid(g))) return rc;
+  if ((rc = check_march(g, rays, nullptr, step, nullptr))) return rc;
   if (!max_weight) return fail(MIPNERF_B200_EINVAL, "max_weight is NULL");
   for (int l = 0; l < g->num_levels; ++l)
     if (g->levels[l].sh && !max_weight[l])
       return fail(MIPNERF_B200_EINVAL, "level %d has kept points: max_weight[%d] is NULL", l, l);
-  CUDA_TRY(mipnerf::launch_grid_visibility(*g, *rays, step, max_weight, (cudaStream_t)stream));
+  CUDA_TRY(mipnerf::launch_grid_visibility(*g, nullptr, *rays, step, max_weight, mipnerf::kKernGridVisibility,
+                                           (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 
@@ -2161,19 +2160,15 @@ int mipnerf_b200_grid_visibility_bricks(const mipnerf_b200_grid* g, const mipner
                                         const mipnerf_b200_rays* rays, float step, float* const* max_weight,
                                         void* stream) {
   int rc;
-  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
-  if ((rc = check_rays(rays))) return rc;
-  if (rays->num_rays > 0 && !rays->viewdirs) return fail(MIPNERF_B200_EINVAL, "rays->viewdirs is NULL");
-  if (!(step > 0.f) || !std::isfinite(step)) return fail(MIPNERF_B200_EINVAL, "step=%g: need a finite step > 0", step);
-  if (!bricks) return fail(MIPNERF_B200_EINVAL, "bricks is NULL");
-  if ((rc = check_grid(g, bricks))) return rc;
+  if ((rc = check_march(g, rays, nullptr, step, &bricks))) return rc;
   if (!max_weight) return fail(MIPNERF_B200_EINVAL, "max_weight is NULL");
   // a level may have kept points wherever it stores a brick: its rows need not be baked yet, so levels[l].sh cannot
   // tell
   for (int l = 0; l < g->num_levels; ++l)
     if (bricks->pool[l] && !max_weight[l])
       return fail(MIPNERF_B200_EINVAL, "level %d stores bricks: max_weight[%d] is NULL", l, l);
-  CUDA_TRY(mipnerf::launch_grid_visibility_bricks(*g, *bricks, *rays, step, max_weight, (cudaStream_t)stream));
+  CUDA_TRY(mipnerf::launch_grid_visibility(*g, bricks, *rays, step, max_weight, mipnerf::kKernGridVisibilityBricks,
+                                           (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

@@ -602,54 +602,30 @@ GParams make_params(const mipnerf_b200_grid& grid) {
   return g;
 }
 
+unsigned grid_blocks(int64_t num_rays) { return (unsigned)((num_rays + kGridThreads - 1) / kGridThreads); }
+
 }  // namespace
 
-namespace {
-
-template <class Rows, class Cells>
-cudaError_t launch_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step, int white_bkgd,
-                          float* rgb, float* distance, float* acc, const Rows& rows, const Cells& cells, KernelId id,
-                          cudaStream_t st) {
+cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
+                               const mipnerf_b200_grid_sh_u8* sh, const mipnerf_b200_rays& rays, float step,
+                               int white_bkgd, float* rgb, float* distance, float* acc, int id, cudaStream_t st) {
   if (rays.num_rays == 0) return cudaSuccess;
   const GParams g = make_params(grid);
-  const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
   LaunchScope scope(id, st);
-#define MIPNERF_GRID_FWD(NC)                                                                                           \
-  grid_render_kernel<NC, Rows, Cells><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, rgb, distance, acc, \
-                                                                       rows, cells)
-  switch (grid.degree) {
-    case 0: MIPNERF_GRID_FWD(1); break;
-    case 1: MIPNERF_GRID_FWD(4); break;
-    case 2: MIPNERF_GRID_FWD(9); break;
-    default: MIPNERF_GRID_FWD(16);
-  }
-#undef MIPNERF_GRID_FWD
+  // the cells and the rows: levels[l].cells and the fp32 levels[l].sh, or the bricks and the uint8 rows given
+  const auto launch = [&](const auto& rows, const auto& cells) {
+    using Rows = std::decay_t<decltype(rows)>;
+    using Cells = std::decay_t<decltype(cells)>;
+    with_sh_coeffs(grid.degree, [&](auto nc) {
+      grid_render_kernel<decltype(nc)::value, Rows, Cells><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
+          g, rays, step, white_bkgd, rgb, distance, acc, rows, cells);
+    });
+  };
+  if (bricks && sh) launch(U8Rows{*sh}, BrickCells{*bricks});
+  else if (bricks) launch(F32Rows{}, BrickCells{*bricks});
+  else if (sh) launch(U8Rows{*sh}, DenseCells{});
+  else launch(F32Rows{}, DenseCells{});
   return cudaGetLastError();
-}
-
-}  // namespace
-
-cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
-                               int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st) {
-  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, F32Rows{}, DenseCells{}, kKernGridRender,
-                       st);
-}
-
-cudaError_t launch_grid_render_u8(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_sh_u8& sh,
-                                  const mipnerf_b200_rays& rays, float step, int white_bkgd, float* rgb,
-                                  float* distance, float* acc, cudaStream_t st) {
-  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, U8Rows{sh}, DenseCells{}, kKernGridRenderU8,
-                       st);
-}
-
-cudaError_t launch_grid_render_bricks(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks& bricks,
-                                      const mipnerf_b200_grid_sh_u8* sh, const mipnerf_b200_rays& rays, float step,
-                                      int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st) {
-  if (sh)
-    return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, U8Rows{*sh}, BrickCells{bricks},
-                         kKernGridRenderBricks, st);
-  return launch_render(grid, rays, step, white_bkgd, rgb, distance, acc, F32Rows{}, BrickCells{bricks},
-                       kKernGridRenderBricks, st);
 }
 
 cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
@@ -657,46 +633,29 @@ cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mip
                                         const float* d_acc, const mipnerf_b200_grid_grads& grads, cudaStream_t st) {
   if (rays.num_rays == 0 || (!d_rgb && !d_distance && !d_acc)) return cudaSuccess;
   const GParams g = make_params(grid);
-  const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
   LaunchScope scope(kKernGridRenderBackward, st);
-#define MIPNERF_GRID_BWD(NC) \
-  grid_render_backward_kernel<NC><<<blocks, kGridThreads, 0, st>>>(g, rays, step, white_bkgd, d_rgb, d_distance, d_acc, grads)
-  switch (grid.degree) {
-    case 0: MIPNERF_GRID_BWD(1); break;
-    case 1: MIPNERF_GRID_BWD(4); break;
-    case 2: MIPNERF_GRID_BWD(9); break;
-    default: MIPNERF_GRID_BWD(16);
-  }
-#undef MIPNERF_GRID_BWD
+  with_sh_coeffs(grid.degree, [&](auto nc) {
+    grid_render_backward_kernel<decltype(nc)::value><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
+        g, rays, step, white_bkgd, d_rgb, d_distance, d_acc, grads);
+  });
   return cudaGetLastError();
 }
 
-namespace {
-
-template <class Cells>
-cudaError_t launch_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
-                              float* const* max_weight, const Cells& cells, KernelId id, cudaStream_t st) {
+cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
+                                   const mipnerf_b200_rays& rays, float step, float* const* max_weight, int id,
+                                   cudaStream_t st) {
   if (rays.num_rays == 0) return cudaSuccess;
   const GParams g = make_params(grid);
   GMaxWeight mw{};
   for (int l = 0; l < grid.num_levels; ++l) mw.w[l] = max_weight[l];
-  const unsigned blocks = (unsigned)((rays.num_rays + kGridThreads - 1) / kGridThreads);
   LaunchScope scope(id, st);
-  grid_visibility_kernel<Cells><<<blocks, kGridThreads, 0, st>>>(g, rays, step, mw, cells);
+  const auto launch = [&](const auto& cells) {
+    grid_visibility_kernel<std::decay_t<decltype(cells)>><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
+        g, rays, step, mw, cells);
+  };
+  if (bricks) launch(BrickCells{*bricks});
+  else launch(DenseCells{});
   return cudaGetLastError();
-}
-
-}  // namespace
-
-cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
-                                   float* const* max_weight, cudaStream_t st) {
-  return launch_visibility(grid, rays, step, max_weight, DenseCells{}, kKernGridVisibility, st);
-}
-
-cudaError_t launch_grid_visibility_bricks(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks& bricks,
-                                          const mipnerf_b200_rays& rays, float step, float* const* max_weight,
-                                          cudaStream_t st) {
-  return launch_visibility(grid, rays, step, max_weight, BrickCells{bricks}, kKernGridVisibilityBricks, st);
 }
 
 }  // namespace mipnerf

@@ -178,12 +178,8 @@ cudaError_t launch_grid_tv(const mipnerf_b200_grid& grid, const int64_t* const* 
   }
   if (blocks == 0) return cudaSuccess;
   LaunchScope scope(kKernGridTv, st);
-  switch (grid.degree) {
-    case 0: grid_tv_kernel<1><<<(unsigned)blocks, kTvThreads, 0, st>>>(P); break;
-    case 1: grid_tv_kernel<4><<<(unsigned)blocks, kTvThreads, 0, st>>>(P); break;
-    case 2: grid_tv_kernel<9><<<(unsigned)blocks, kTvThreads, 0, st>>>(P); break;
-    default: grid_tv_kernel<16><<<(unsigned)blocks, kTvThreads, 0, st>>>(P);
-  }
+  with_sh_coeffs(grid.degree,
+                 [&](auto nc) { grid_tv_kernel<decltype(nc)::value><<<(unsigned)blocks, kTvThreads, 0, st>>>(P); });
   return cudaGetLastError();
 }
 

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <type_traits>
 
 #include "draws.h"
 
@@ -72,24 +73,23 @@ cudaError_t launch_isosurface_emit(const float* grid, int nx, int ny, int nz, co
 cudaError_t launch_isosurface_normals(const float* grid, int nx, int ny, int nz, const float* step, float iso,
                                       const void* scratch, float* normals, cudaStream_t st);
 
-// ---- grid_render.cu (ray marching through a baked grid; arguments checked by the caller) ----
-cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
-                               int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st);
-cudaError_t launch_grid_render_u8(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_sh_u8& sh,
-                                  const mipnerf_b200_rays& rays, float step, int white_bkgd, float* rgb,
-                                  float* distance, float* acc, cudaStream_t st);
-// sh NULL: fp32 rows (levels[l].sh); otherwise the uint8 rows of *sh
-cudaError_t launch_grid_render_bricks(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks& bricks,
-                                      const mipnerf_b200_grid_sh_u8* sh, const mipnerf_b200_rays& rays, float step,
-                                      int white_bkgd, float* rgb, float* distance, float* acc, cudaStream_t st);
+// ---- grid_render.cu (ray marching through a baked grid; arguments checked by the caller; id: a KernelId) ----
+cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
+                               const mipnerf_b200_grid_sh_u8* sh, const mipnerf_b200_rays& rays, float step,
+                               int white_bkgd, float* rgb, float* distance, float* acc, int id, cudaStream_t st);
 cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
                                         int white_bkgd, const float* d_rgb, const float* d_distance,
                                         const float* d_acc, const mipnerf_b200_grid_grads& grads, cudaStream_t st);
-cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
-                                   float* const* max_weight, cudaStream_t st);
-cudaError_t launch_grid_visibility_bricks(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks& bricks,
-                                          const mipnerf_b200_rays& rays, float step, float* const* max_weight,
-                                          cudaStream_t st);
+cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
+                                   const mipnerf_b200_rays& rays, float step, float* const* max_weight, int id,
+                                   cudaStream_t st);
+template <class F>  // f(std::integral_constant<int, NC>{}), NC = (degree + 1)^2 for degree 0..3: the grid kernels' NC
+void with_sh_coeffs(int degree, F&& f) {
+  if (degree == 0) return f(std::integral_constant<int, 1>{});
+  if (degree == 1) return f(std::integral_constant<int, 4>{});
+  if (degree == 2) return f(std::integral_constant<int, 9>{});
+  f(std::integral_constant<int, 16>{});
+}
 
 // ---- grid_tv.cu (total-variation prior of a baked grid; arguments checked by the caller) ----
 cudaError_t launch_grid_tv(const mipnerf_b200_grid& grid, const int64_t* const* points, const int64_t* num_points,

@@ -255,6 +255,89 @@ def test_cabi_refusals(lib, case):
     assert _cabi.last_error(), case
 
 
+MARCHING = ["grid_render", "grid_render_u8", "grid_render_bricks", "grid_render_backward", "grid_visibility",
+            "grid_visibility_bricks"]
+_RENDERS, _BRICKS = MARCHING[:3], ("grid_render_bricks", "grid_visibility_bricks")
+
+
+def _march_refusal(lib, name, faults):
+    """The message `name` refuses a valid argument set with `faults` applied; a fault an entry point has no argument
+    for is not applied."""
+    g, r = _valid_args()
+    step, out = 0.01, [0xC000, 0xD000, 0xE000]
+    bricks, sh = _cabi.GridBricks(), _cabi.GridShU8()
+    for lvl in range(2):
+        if name in _BRICKS:
+            g.levels[lvl].cells = None
+            bricks.table[lvl], bricks.pool[lvl] = 0x10000 + lvl, 0x20000 + lvl
+        if name in ("grid_render_u8", "grid_render_bricks"):
+            g.levels[lvl].sh = None
+            sh.rows[lvl] = 0x30000 + lvl
+    grads, mw = _cabi.GridGrads(), (C.c_void_p * 2)(0xF000, 0xF100)
+    grads.density[:2], grads.sh[:2] = [0x40000, 0x40100], [0x50000, 0x50100]
+    gp, rp, bp, sp, gr = C.byref(g), C.byref(r), C.byref(bricks), C.byref(sh), C.byref(grads)
+    for f in faults:
+        if f == "grid":
+            gp = None
+        elif f == "origins":
+            r.origins = None
+        elif f == "viewdirs":
+            r.viewdirs = None
+        elif f == "num_rays":
+            r.num_rays = -1
+        elif f == "rgb":
+            out[0] = None
+        elif f == "step":
+            step = 0.0
+        elif f == "bricks":
+            bp = None
+        elif f == "degree":
+            g.degree = 4
+        elif f == "sh":
+            sp = None
+        elif f == "grads":
+            gr = None
+        elif f == "max_weight":
+            mw = None
+    call = {"grid_render": lambda: lib.mipnerf_b200_grid_render(gp, rp, step, 1, *out, None),
+            "grid_render_u8": lambda: lib.mipnerf_b200_grid_render_u8(gp, sp, rp, step, 1, *out, None),
+            "grid_render_bricks": lambda: lib.mipnerf_b200_grid_render_bricks(gp, bp, None, rp, step, 1, *out, None),
+            "grid_render_backward": lambda: lib.mipnerf_b200_grid_render_backward(gp, rp, step, 1, 0x60000, None,
+                                                                                  None, gr, None),
+            "grid_visibility": lambda: lib.mipnerf_b200_grid_visibility(gp, rp, step, mw, None),
+            "grid_visibility_bricks": lambda: lib.mipnerf_b200_grid_visibility_bricks(gp, bp, rp, step, mw, None)}[name]
+    assert call() == _cabi.EINVAL, (name, faults)
+    return _cabi.last_error()
+
+
+STEP_MSG = "step=0: need a finite step > 0"
+DEGREE_MSG = "degree=4: need 0..3"
+
+
+@pytest.mark.parametrize("faults,want", [
+    (("grid", "origins"), {n: "grid is NULL" for n in MARCHING}),
+    (("num_rays", "grid"), {n: "grid is NULL" for n in MARCHING}),
+    (("origins", "viewdirs"), {n: "a ray field is NULL" for n in MARCHING}),
+    (("num_rays", "viewdirs"), {n: "num_rays=-1" for n in MARCHING}),
+    (("viewdirs", "rgb"), {n: "rays->viewdirs is NULL" for n in MARCHING}),
+    (("bricks", "viewdirs"), {n: "rays->viewdirs is NULL" for n in MARCHING}),
+    (("rgb", "step"), {n: "rgb / distance / acc is NULL" if n in _RENDERS else STEP_MSG for n in MARCHING}),
+    (("step", "bricks"), {n: STEP_MSG for n in MARCHING}),
+    (("bricks", "degree"), {n: "bricks is NULL" if n in _BRICKS else DEGREE_MSG for n in MARCHING}),
+    (("degree", "sh"), {n: DEGREE_MSG for n in MARCHING}),
+    (("degree", "grads"), {n: DEGREE_MSG for n in MARCHING}),
+    (("degree", "max_weight"), {n: DEGREE_MSG for n in MARCHING}),
+    (("sh", "max_weight"), {**{n: None for n in MARCHING}, "grid_render_u8": "sh is NULL",
+                            "grid_visibility": "max_weight is NULL", "grid_visibility_bricks": "max_weight is NULL"}),
+])
+def test_marching_refusal_order(lib, faults, want):
+    """Every entry point that marches rays refuses the first of two faults in one order: grid, rays, viewdirs, the
+    outputs, the step, bricks, the grid description, then what the entry point checks on its own."""
+    for name in MARCHING:
+        if want[name] is not None:
+            assert _march_refusal(lib, name, faults) == want[name], (name, faults)
+
+
 def test_kernel_registered_with_profiler(lib):
     names = [lib.mipnerf_b200_profile_kernel_name(k).decode() for k in range(lib.mipnerf_b200_profile_num_kernels())]
     assert names[-1] == "grid_render"

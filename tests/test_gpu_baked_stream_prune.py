@@ -3,8 +3,6 @@ fp16x3, fp32), mipnerf_b200_grid_visibility_bricks against the dense visibility 
 grids of test_gpu_baked.py, `bake_grid(prune=bank)` against `prune_grid(bake_grid(...), bank)` (then `.quantize()`,
 `.sparsify()`) in every array (65^3 and 129^3, 1 and 3 levels, degrees 0 and 2, dense and streamed), and the streamed
 pruned bake's peak memory against `bake_grid`'s docstring bound."""
-import ctypes as C
-
 import pytest
 import torch
 
@@ -15,10 +13,8 @@ from test_gpu_baked_stream import CASES, DEV, PRECISIONS, assert_same_grid, mode
 pytestmark = pytest.mark.gpu
 
 import mipnerf_pl_b200 as mp  # noqa: E402
-from mipnerf_pl_b200 import _cabi  # noqa: E402
 from mipnerf_pl_b200.baked import _bake_rows  # noqa: E402
 from mipnerf_pl_b200.field import DEFAULT_BOUNDS  # noqa: E402
-from mipnerf_pl_b200.ops import _call, _rays_struct  # noqa: E402
 
 _BANKS = {}
 
@@ -48,11 +44,7 @@ def test_bake_sh_rows_do_not_depend_on_their_call(precision, degree):
 def brick_scores(sparse, rays):
     """mipnerf_b200_grid_visibility_bricks on a sparse grid's bricks, every max_weight passed."""
     out = [torch.zeros(m, device=DEV) for m in sparse.kept]
-    rs, _keep = _rays_struct(rays.origins.reshape(-1, 3), rays.directions.reshape(-1, 3), rays.viewdirs.reshape(-1, 3),
-                             rays.radii.reshape(-1), rays.near.reshape(-1), rays.far.reshape(-1))
-    ptrs = (C.c_void_p * sparse.levels)(*[t.data_ptr() if t.numel() else None for t in out])
-    _call(torch.device(DEV), "grid_visibility_bricks", _cabi.lib().mipnerf_b200_grid_visibility_bricks,
-          C.byref(sparse._struct()), C.byref(sparse._bricks_struct()), C.byref(rs), sparse.default_step(), ptrs)
+    sparse._visibility(rays, None, out)
     return out
 
 
