@@ -140,6 +140,26 @@ int mipnerf_b200_forward_rng(const mipnerf_b200_config* cfg, const mipnerf_b200_
                              int precision, mipnerf_b200_level_out* outs, void* workspace,
                              size_t workspace_bytes, void* stream);
 
+/* Levels 1 .. num_levels - 1 of mipnerf_b200_forward's loop, run exactly as that loop runs them, with the caller's
+ * fenceposts t_prev [B,N+1] and weights w_prev [B,N] in place of level 0's outputs (e.g. mipnerf_b200_grid_proposal's
+ * weights at sample_along_rays' fenceposts: level 0's MLP is not run).  `outs` has cfg->num_levels - 1 entries, outs[k]
+ * for level k + 1.  Draws as the forward's: `u_jitter` (required when randomized) is level l's inverse-CDF jitter for
+ * every level, outs[k].density_normal the density noise of level k + 1; the _rng form draws stream 1 + l (jitter) and
+ * 32 + l (density noise) of `rng`.  So with t_prev / w_prev = a forward's outs[0].t_samples / weights, every output
+ * equals that forward's levels >= 1 bit for bit.  The workspace is mipnerf_b200_workspace_bytes', the precisions and
+ * num_samples the forward's.  num_levels < 2: MIPNERF_B200_EINVAL.  The refusals, in order: the config, num_levels, the
+ * weights, the rays, outs, t_prev / w_prev, then the forward's. */
+int mipnerf_b200_forward_proposed(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
+                                  const mipnerf_b200_rays* rays, const float* t_prev, const float* w_prev,
+                                  int randomized, const float* u_jitter, int white_bkgd, int precision,
+                                  mipnerf_b200_level_out* outs, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+int mipnerf_b200_forward_proposed_rng(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
+                                      const mipnerf_b200_rays* rays, const float* t_prev, const float* w_prev,
+                                      const mipnerf_b200_rng* rng, int white_bkgd, int precision,
+                                      mipnerf_b200_level_out* outs, void* workspace, size_t workspace_bytes,
+                                      void* stream);
+
 /* The uniforms those kernels draw: out[num_rays, ncols] for `stream_id` (0: t_rand in [0,1); >= 1: u_jitter in
  * [0, 1/ncols - eps)).  forward(t_rand = stream 0, u_jitter = stream 1+level) reproduces forward_rng bit for bit. */
 int mipnerf_b200_philox_uniform(const mipnerf_b200_rng* rng, int stream_id, int64_t num_rays, int ncols, float* out,
@@ -597,6 +617,24 @@ int mipnerf_b200_grid_visibility(const mipnerf_b200_grid* grid, const mipnerf_b2
 int mipnerf_b200_grid_visibility_bricks(const mipnerf_b200_grid* grid, const mipnerf_b200_grid_bricks* bricks,
                                         const mipnerf_b200_rays* rays, float step, float* const* max_weight,
                                         void* stream);
+
+/* Proposal weights from a baked grid's density (mip-NeRF 360's proposal sampling): the level-0 weights of a forward at
+ * the caller's fenceposts t_samples [B, N+1], for mipnerf_b200_forward_proposed.  Per ray and interval i, in fp32:
+ *   t_mid = fl(fl(t_i + t_{i+1}) * 0.5), x = fl(o + fl(t_mid d)) per axis, delta_i = fl(fl(t_{i+1} - t_i) |d|) with
+ *   |d| = fl(sqrt(fl(fl(dx dx + dy dy) + dz dz))) (every operation rounded once, as the renderer's sample lattice);
+ *   sigma_i = the renderer's density at x: 0 outside [lo, hi], else levels floor(lambda) and floor(lambda) + 1 blended
+ *   by lambda = clamp(log2(sqrt(3) radii t_mid / s_0), 0, L - 1), each trilinear over its lattice (0 at dropped points);
+ *   s_i = fl(sigma_i delta_i), w_i = fl(fl(1 - exp(-s_i)) exp(-S_i)), S_i = sum_{j<i} s_j accumulated in order in fp32:
+ *   volumetric_rendering's weights (models/mip.py:366-401), every interval weighted (no early stop).
+ * Midpoints in empty macro cells are not looked up (their density is exactly 0), so the weights equal those of the
+ * grid with every macro cell occupied bit for bit.  bricks NULL: the cells are levels[l].cells; otherwise the cells
+ * are `bricks` (as mipnerf_b200_grid_render_bricks: every levels[l].cells NULL, every bricks->table[l] set), with the
+ * same weights bit for bit as the dense cells they encode.  No SH row and no viewdir is read.  The refusals, in order:
+ * grid NULL, the rays, t_samples / weights NULL, num_samples outside 1..256, bricks' cells, then the grid.  No
+ * allocation, no synchronisation. */
+int mipnerf_b200_grid_proposal(const mipnerf_b200_grid* grid, const mipnerf_b200_grid_bricks* bricks,
+                               const mipnerf_b200_rays* rays, const float* t_samples, int num_samples, float* weights,
+                               void* stream);
 
 /* The total-variation prior of a baked grid (Plenoxels), for fine-tuning.  Per level l, on that level's own lattice:
  * for each kept point p (SH row r, lattice position points[l][r] = i + nx (j + ny k), r < num_points[l] = M_l) and

@@ -20,7 +20,7 @@ from .metrics import eval_errors, ssim, evaluate, render_path, spheric_path, sav
 from .field import (density_grid, isosurface, extract_mesh, mesh_colors, voxel_variance, write_ply, sh_basis,
                     sphere_quadrature, bake_sh, eval_sh, mesh_sh)
 from .baked import (BakedGrid, bake_grid, finetune_grid, grid_occupancy, grid_structure, prune_grid,
-                    render_baked_frame, sparse_grid_structure)
+                    render_baked_frame, render_proposed_frame, sparse_grid_structure)
 
 __all__ = [
     "Rays", "Rays_keys", "namedtuple_map", "rearrange_render_image", "blender_rays", "spheric_pose",
@@ -34,5 +34,5 @@ __all__ = [
     "render_path", "spheric_path", "save_images", "density_grid", "isosurface", "extract_mesh", "write_ply",
     "mesh_colors", "voxel_variance", "sh_basis", "sphere_quadrature", "bake_sh", "eval_sh", "mesh_sh",
     "BakedGrid", "bake_grid", "finetune_grid", "grid_occupancy", "grid_structure", "prune_grid", "render_baked_frame",
-    "sparse_grid_structure",
+    "render_proposed_frame", "sparse_grid_structure",
 ]

@@ -118,6 +118,11 @@ _SIGNATURES = {
                                        _V, _V, C.c_int, C.c_int, C.POINTER(LevelOut), _V, C.c_size_t, _V]),
     "mipnerf_b200_forward_rng": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), C.POINTER(RaysStruct), C.POINTER(Rng),
                                            C.c_int, C.c_int, C.POINTER(LevelOut), _V, C.c_size_t, _V]),
+    "mipnerf_b200_forward_proposed": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), C.POINTER(RaysStruct), _V, _V,
+                                                C.c_int, _V, C.c_int, C.c_int, C.POINTER(LevelOut), _V, C.c_size_t, _V]),
+    "mipnerf_b200_forward_proposed_rng": (C.c_int, [C.POINTER(Config), C.POINTER(Weights), C.POINTER(RaysStruct), _V,
+                                                    _V, C.POINTER(Rng), C.c_int, C.c_int, C.POINTER(LevelOut), _V,
+                                                    C.c_size_t, _V]),
     "mipnerf_b200_philox_uniform": (C.c_int, [C.POINTER(Rng), C.c_int, C.c_int64, C.c_int, _V, _V]),
     "mipnerf_b200_philox_normal": (C.c_int, [C.POINTER(Rng), C.c_int, C.c_int64, C.c_int, _V, _V]),
     "mipnerf_b200_distloss": (C.c_int, [_V, _V, C.c_int64, C.c_int, _V, _V]),
@@ -193,6 +198,8 @@ _SIGNATURES = {
     "mipnerf_b200_grid_visibility": (C.c_int, [C.POINTER(Grid), C.POINTER(RaysStruct), C.c_float, C.POINTER(_V), _V]),
     "mipnerf_b200_grid_visibility_bricks": (C.c_int, [C.POINTER(Grid), C.POINTER(GridBricks), C.POINTER(RaysStruct),
                                                       C.c_float, C.POINTER(_V), _V]),
+    "mipnerf_b200_grid_proposal": (C.c_int, [C.POINTER(Grid), C.POINTER(GridBricks), C.POINTER(RaysStruct), _V,
+                                             C.c_int, _V, _V]),
     "mipnerf_b200_grid_tv": (C.c_int, [C.POINTER(Grid), C.POINTER(_V), _i64p, C.c_float, C.POINTER(_V), C.POINTER(_V),
                                        _V, C.POINTER(GridGrads), _V]),
     "mipnerf_b200_selftest_umma": (C.c_int, [_V, _V, _V, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),

@@ -589,6 +589,26 @@ class BakedGrid:
             _call(dev, "grid_visibility", _cabi.lib().mipnerf_b200_grid_visibility, C.byref(g), C.byref(rs), st, mw)
 
     @torch.no_grad()
+    def proposal(self, rays: Rays, t_samples: torch.Tensor) -> torch.Tensor:
+        """Proposal weights [B, N] of flat `rays` at fenceposts `t_samples` [B, N+1] (1 <= N <= 256), on
+        mipnerf_b200_grid_proposal: per interval, the grid's density at its midpoint under the renderer's level blend,
+        composited as volumetric_rendering's weights with no early stop.  What `MipNerf.forward_proposed` resamples
+        level 1 from.  Dense, sparse, quantized and trainable grids (synced first); no gradient."""
+        dev = _dev(self.sh[0])
+        rs, keep = _grid_rays(rays, dev)
+        b = rs.num_rays
+        if t_samples.dim() != 2 or t_samples.shape[0] != b or not 2 <= t_samples.shape[1] <= 257:
+            raise ValueError(f"t_samples {tuple(t_samples.shape)}: need [B = {b}, N + 1] with 1 <= N <= 256")
+        if t_samples.device != dev:
+            raise ValueError(f"t_samples on {t_samples.device}, grid on {dev}")
+        t = _f32(t_samples)
+        n = t.shape[1] - 1
+        out = torch.empty(b, n, device=dev)
+        _call(dev, "grid_proposal", _cabi.lib().mipnerf_b200_grid_proposal, C.byref(self._struct()),
+              C.byref(self._bricks_struct()) if self.sparse else None, C.byref(rs), t.data_ptr(), n, out.data_ptr())
+        return out
+
+    @torch.no_grad()
     def prune(self, max_weight: Sequence[torch.Tensor], weight_threshold: float) -> "BakedGrid":
         """A new, non-trainable grid that keeps the points kept here whose score in `max_weight` (per level [M_l] in
         SH-row order, as `visibility` returns) is > `weight_threshold`; `self` is left as it is.  A point pruned away
@@ -1118,6 +1138,23 @@ def render_baked_frame(grid: BakedGrid, c2w, height: int = 800, width: int = 800
     counts = [(shard_rows(height, world, r)[1] - shard_rows(height, world, r)[0]) * width for r in range(world)]
     full = gather_rows(local, counts, group)
     return full[:, 0:3].reshape(height, width, 3), full[:, 3].reshape(height, width), full[:, 4].reshape(height, width)
+
+
+@torch.no_grad()
+def render_proposed_frame(model, grid: BakedGrid, c2w, height: int = 800, width: int = 800, white_bkgd: bool = True,
+                          camera_angle_x: float = BLENDER_CAMERA_ANGLE_X, near: float = 2.0, far: float = 6.0,
+                          world: int = 1, rank: int = 0, group=None, device=None):
+    """One frame of `model.forward_proposed(rays, grid, False, white_bkgd)` (the MLP's fine level, placed by the
+    grid's proposal weights), with `render.render_frame`'s rays and row sharding: (fine_rgb [H,W,3], distance [H,W]) on
+    every rank."""
+    dev = device or next(model.parameters()).device
+    r0, r1 = shard_rows(height, world, rank)
+    rays = generate_rays(c2w, height, width, camera_angle_x, near, far, rows=(r0, r1), device=dev)
+    ret = model.forward_proposed(rays, grid, False, white_bkgd)
+    local = torch.cat([ret[-1][0], ret[-1][1][:, None]], dim=1)  # [rows*W, 4]
+    counts = [(shard_rows(height, world, r)[1] - shard_rows(height, world, r)[0]) * width for r in range(world)]
+    full = gather_rows(local, counts, group)
+    return full[:, 0:3].reshape(height, width, 3), full[:, 3].reshape(height, width)
 
 
 def prune_grid(grid: BakedGrid, bank, weight_threshold: float = DEFAULT_WEIGHT_THRESHOLD, step: Optional[float] = None,

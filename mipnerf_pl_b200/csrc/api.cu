@@ -348,36 +348,48 @@ int mipnerf_b200_pack_weights(const mipnerf_b200_config* cfg, const mipnerf_b200
 }
 
 // randomized with density_noise > 0 (models/mip_nerf.py:232-233): the injected-noise entry points need the normals too
+// (outs[l - first] is level l's output)
 static int check_density_normals(const mipnerf_b200_config* cfg, int randomized, const mipnerf_b200_rng* rng,
-                                 const mipnerf_b200_level_out* outs, int64_t num_rays) {
+                                 const mipnerf_b200_level_out* outs, int64_t num_rays, int first = 0) {
   if (!randomized || !(cfg->density_noise > 0.f) || rng || num_rays == 0) return MIPNERF_B200_OK;
-  for (int l = 0; l < cfg->num_levels; ++l)
-    if (!outs[l].density_normal)
+  for (int l = first; l < cfg->num_levels; ++l)
+    if (!outs[l - first].density_normal)
       return fail(MIPNERF_B200_EINVAL,
                   "randomized=1 with density_noise > 0 needs outs[%d].density_normal (injected noise) or the _rng "
-                  "entry point (in-kernel Philox)", l);
+                  "entry point (in-kernel Philox)", l - first);
   return MIPNERF_B200_OK;
 }
 
+// The level loop of mipnerf_b200_forward(_rng).  With `proposal` = {t_prev, w_prev} (mipnerf_b200_forward_proposed) it
+// starts at level 1 with those in place of level 0's outputs, and outs[l - 1] is level l's output.
 static int forward_impl(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
                         const mipnerf_b200_rays* rays, int randomized, const float* t_rand,
                         const float* u_jitter, const mipnerf_b200_rng* rng, int white_bkgd, int precision,
-                        mipnerf_b200_level_out* outs, void* workspace, size_t workspace_bytes, void* stream) {
+                        mipnerf_b200_level_out* outs, void* workspace, size_t workspace_bytes, void* stream,
+                        const float* const* proposal = nullptr) {
   Dims d;
   int rc;
   if ((rc = check_config(cfg, &d))) return rc;
+  const int first = proposal ? 1 : 0;
+  if (proposal && cfg->num_levels < 2)
+    return fail(MIPNERF_B200_EINVAL, "num_levels=%d: a forward from proposal weights needs >= 2 levels",
+                cfg->num_levels);
   if ((rc = check_weights(cfg, d, w))) return rc;
   if ((rc = check_rays(rays))) return rc;
   if (!outs) return fail(MIPNERF_B200_EINVAL, "outs is NULL");
+  if (proposal && rays->num_rays > 0 && (!proposal[0] || !proposal[1]))
+    return fail(MIPNERF_B200_EINVAL, "t_prev / w_prev is NULL");
   if (cfg->use_viewdirs && rays->num_rays > 0 && !rays->viewdirs)
     return fail(MIPNERF_B200_EINVAL, "use_viewdirs but rays.viewdirs is NULL");
-  if (randomized && !rng && (!t_rand || (cfg->num_levels > 1 && !u_jitter)))
-    return fail(MIPNERF_B200_EINVAL,
-                "randomized=1 needs t_rand and u_jitter (injected noise) or the _rng entry point (in-kernel Philox)");
-  for (int l = 0; l < cfg->num_levels; ++l)
-    if (rays->num_rays > 0 && (!outs[l].comp_rgb || !outs[l].distance || !outs[l].acc))
-      return fail(MIPNERF_B200_EINVAL, "outs[%d] misses comp_rgb/distance/acc", l);
-  if ((rc = check_density_normals(cfg, randomized, rng, outs, rays->num_rays))) return rc;
+  if (randomized && !rng && ((!proposal && !t_rand) || (cfg->num_levels > 1 && !u_jitter)))
+    return fail(MIPNERF_B200_EINVAL, proposal ? "randomized=1 needs u_jitter (injected noise) or the _rng entry point "
+                                                "(in-kernel Philox)"
+                                              : "randomized=1 needs t_rand and u_jitter (injected noise) or the _rng "
+                                                "entry point (in-kernel Philox)");
+  for (int l = first; l < cfg->num_levels; ++l)
+    if (rays->num_rays > 0 && (!outs[l - first].comp_rgb || !outs[l - first].distance || !outs[l - first].acc))
+      return fail(MIPNERF_B200_EINVAL, "outs[%d] misses comp_rgb/distance/acc", l - first);
+  if ((rc = check_density_normals(cfg, randomized, rng, outs, rays->num_rays, first))) return rc;
   const size_t need = mipnerf_b200_workspace_bytes(cfg, rays->num_rays, precision);
   if (rays->num_rays > 0 && (!workspace || workspace_bytes < need))
     return fail(MIPNERF_B200_EWORKSPACE, "workspace %zu < %zu bytes", workspace_bytes, need);
@@ -388,7 +400,7 @@ static int forward_impl(const mipnerf_b200_config* cfg, const mipnerf_b200_weigh
   if (precision != MIPNERF_B200_FP32) {
     if ((rc = check_tc(cfg, w, precision, "forward"))) return rc;
     cudaError_t e = mipnerf::tc_forward(cfg, w, rays, randomized, t_rand, u_jitter, rng, white_bkgd, precision,
-                                        outs, workspace, workspace_bytes, st);
+                                        outs, workspace, workspace_bytes, st, nullptr, 0, 0, proposal);
     if (e != cudaSuccess) return fail(MIPNERF_B200_ECUDA, "tc_forward: %s", cudaGetErrorString(e));
     return MIPNERF_B200_OK;
   }
@@ -399,16 +411,18 @@ static int forward_impl(const mipnerf_b200_config* cfg, const mipnerf_b200_weigh
     const Fp32Scratch s = carve_fp32(cfg, d, cnt, workspace);
     if (cfg->use_viewdirs)
       CUDA_TRY(mipnerf::launch_pos_enc(rc_.viewdirs, s.venc, cnt, 0, cfg->deg_view, 1, st));
-    const float *t_prev = nullptr, *w_prev = nullptr;
-    for (int l = 0; l < cfg->num_levels; ++l) {
-      float* t_cur = outs[l].t_samples ? outs[l].t_samples + off * (n + 1) : s.t[l & 1];
-      float* w_cur = outs[l].weights ? outs[l].weights + off * n : s.w[l & 1];
+    const float* t_prev = proposal ? proposal[0] + off * (n + 1) : nullptr;
+    const float* w_prev = proposal ? proposal[1] + off * n : nullptr;
+    for (int l = first; l < cfg->num_levels; ++l) {
+      const mipnerf_b200_level_out& o = outs[l - first];
+      float* t_cur = o.t_samples ? o.t_samples + off * (n + 1) : s.t[l & 1];
+      float* w_cur = o.weights ? o.weights + off * n : s.w[l & 1];
       if (l == 0) {
         CUDA_TRY(mipnerf::launch_coarse_t(rc_.near, rc_.far, mipnerf::level_draws(randomized, t_rand, rng, off, 0, n + 1),
                                           t_cur, cnt, n, randomized, cfg->disparity, st));
       } else {
         CUDA_TRY(mipnerf::launch_resample(t_prev, w_prev, mipnerf::level_draws(randomized, u_jitter, rng, off, 1 + l, n + 1),
-                                          t_cur, outs[l].inds ? outs[l].inds + off * (n + 1) : nullptr, cnt, n, n + 1,
+                                          t_cur, o.inds ? o.inds + off * (n + 1) : nullptr, cnt, n, n + 1,
                                           randomized, 1, cfg->resample_padding, st));
       }
       CUDA_TRY(mipnerf::launch_ipe_from_t(rc_.origins, rc_.directions, rc_.radii, t_cur, s.enc, cnt, n,
@@ -418,9 +432,9 @@ static int forward_impl(const mipnerf_b200_config* cfg, const mipnerf_b200_weigh
                                  s.raw_density, st)))
         return rc;
       CUDA_TRY(mipnerf::launch_add_density_noise(                                   // models/mip_nerf.py:232-233
-          s.raw_density, mipnerf::density_noise_draws(cfg, randomized, outs[l].density_normal, rng, off, l, n), cnt, n, st));
+          s.raw_density, mipnerf::density_noise_draws(cfg, randomized, o.density_normal, rng, off, l, n), cnt, n, st));
       CUDA_TRY(mipnerf::launch_composite(s.raw_rgb, s.raw_density, t_cur, rc_.directions,
-                                         outs[l].comp_rgb + off * 3, outs[l].distance + off, outs[l].acc + off,
+                                         o.comp_rgb + off * 3, o.distance + off, o.acc + off,
                                          w_cur, cnt, n, white_bkgd, 1, cfg->density_bias, rgb_scale,
                                          cfg->rgb_padding, st));
       t_prev = t_cur;
@@ -445,6 +459,27 @@ int mipnerf_b200_forward_rng(const mipnerf_b200_config* cfg, const mipnerf_b200_
   if (!rng) return fail(MIPNERF_B200_EINVAL, "rng is NULL");
   return forward_impl(cfg, w, rays, 1, nullptr, nullptr, rng, white_bkgd, precision, outs, workspace,
                       workspace_bytes, stream);
+}
+
+int mipnerf_b200_forward_proposed(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
+                                  const mipnerf_b200_rays* rays, const float* t_prev, const float* w_prev,
+                                  int randomized, const float* u_jitter, int white_bkgd, int precision,
+                                  mipnerf_b200_level_out* outs, void* workspace, size_t workspace_bytes,
+                                  void* stream) {
+  const float* const proposal[2] = {t_prev, w_prev};
+  return forward_impl(cfg, w, rays, randomized, nullptr, u_jitter, nullptr, white_bkgd, precision, outs, workspace,
+                      workspace_bytes, stream, proposal);
+}
+
+int mipnerf_b200_forward_proposed_rng(const mipnerf_b200_config* cfg, const mipnerf_b200_weights* w,
+                                      const mipnerf_b200_rays* rays, const float* t_prev, const float* w_prev,
+                                      const mipnerf_b200_rng* rng, int white_bkgd, int precision,
+                                      mipnerf_b200_level_out* outs, void* workspace, size_t workspace_bytes,
+                                      void* stream) {
+  if (!rng) return fail(MIPNERF_B200_EINVAL, "rng is NULL");
+  const float* const proposal[2] = {t_prev, w_prev};
+  return forward_impl(cfg, w, rays, 1, nullptr, nullptr, rng, white_bkgd, precision, outs, workspace,
+                      workspace_bytes, stream, proposal);
 }
 
 int mipnerf_b200_philox_normal(const mipnerf_b200_rng* rng, int level, int64_t num_rays, int num_samples, float* out,
@@ -2169,6 +2204,20 @@ int mipnerf_b200_grid_visibility_bricks(const mipnerf_b200_grid* g, const mipner
       return fail(MIPNERF_B200_EINVAL, "level %d stores bricks: max_weight[%d] is NULL", l, l);
   CUDA_TRY(mipnerf::launch_grid_visibility(*g, bricks, *rays, step, max_weight, mipnerf::kKernGridVisibilityBricks,
                                            (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_grid_proposal(const mipnerf_b200_grid* g, const mipnerf_b200_grid_bricks* bricks,
+                               const mipnerf_b200_rays* rays, const float* t_samples, int num_samples, float* weights,
+                               void* stream) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_rays(rays))) return rc;
+  if (rays->num_rays > 0 && (!t_samples || !weights)) return fail(MIPNERF_B200_EINVAL, "t_samples / weights is NULL");
+  if (num_samples < 1 || num_samples > 256)
+    return fail(MIPNERF_B200_EINVAL, "num_samples=%d: need 1..256", num_samples);
+  if ((rc = check_grid(g, bricks))) return rc;
+  CUDA_TRY(mipnerf::launch_grid_proposal(*g, bricks, *rays, t_samples, num_samples, weights, (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

@@ -309,17 +309,23 @@ __device__ __forceinline__ bool sample_at(const GParams& g, const RayMarch& m, i
   return inside;
 }
 
-// For dt > 0: if x lies in an empty macro cell, move k to the first sample past the cell's exit t (at least k + 1) and
-// return true.
-__device__ __forceinline__ bool skip_empty(const GParams& g, const RayMarch& m, const float (&x)[3], int64_t& k) {
+// Whether the macro cell of an inside position x is occupied; c is the cell.
+__device__ __forceinline__ bool occupied(const GParams& g, const float (&x)[3], int (&c)[3]) {
   const GLevel& l0 = g.lv[0];
-  int c[3];
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
     const int i = (int)fminf(fmaxf((x[a] - g.lo[a]) * l0.inv_s[a], 0.f), (float)(l0.n[a] - 2));
     c[a] = i / g.block;
   }
-  if (__ldg(g.occ + ((int64_t)c[2] * g.on[1] + c[1]) * g.on[0] + c[0])) return false;
+  return __ldg(g.occ + ((int64_t)c[2] * g.on[1] + c[1]) * g.on[0] + c[0]);
+}
+
+// For dt > 0: if x lies in an empty macro cell, move k to the first sample past the cell's exit t (at least k + 1) and
+// return true.
+__device__ __forceinline__ bool skip_empty(const GParams& g, const RayMarch& m, const float (&x)[3], int64_t& k) {
+  const GLevel& l0 = g.lv[0];
+  int c[3];
+  if (occupied(g, x, c)) return false;
   float t_exit = INFINITY;
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
@@ -571,6 +577,50 @@ __global__ void __launch_bounds__(kGridThreads)
   }
 }
 
+// Proposal weights of the caller's intervals (mipnerf_b200_grid_proposal), one thread per ray.  Interval i is sampled
+// at its midpoint with blend_density, and its weight is volumetric_rendering's (1 - exp(-s_i)) exp(-sum_{j<i} s_j),
+// s_i = sigma_i delta_i, with every interval weighted: no stop.  A midpoint in an empty macro cell has density exactly
+// 0 at every level (the occupancy rule skip_empty relies on), so its lookup is skipped and s_i = 0 exactly: the result
+// equals the all-occupied grid's bit for bit.  No SH row is read.
+template <class Cells>
+__global__ void __launch_bounds__(kGridThreads)
+    grid_proposal_kernel(const GParams g, const mipnerf_b200_rays rays, const float* __restrict__ t_samples,
+                         int num_samples, float* __restrict__ weights, const __grid_constant__ Cells cells) {
+  const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
+  if (r >= rays.num_rays) return;
+  float o[3], d[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) o[a] = __ldg(rays.origins + 3 * r + a), d[a] = __ldg(rays.directions + 3 * r + a);
+  const float radius = __ldg(rays.radii + r);
+  const float dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
+  const float* t = t_samples + r * (num_samples + 1);
+  float* w = weights + r * num_samples;
+  float depth = 0.f;  // sum_{j<i} s_j
+  float t0 = __ldg(t);
+  for (int i = 0; i < num_samples; ++i) {
+    const float t1 = __ldg(t + i + 1);
+    const float tm = __fmul_rn(__fadd_rn(t0, t1), 0.5f);
+    const float delta = __fmul_rn(__fsub_rn(t1, t0), dn);
+    t0 = t1;
+    float x[3];
+    bool inside = true;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      x[a] = __fadd_rn(o[a], __fmul_rn(tm, d[a]));
+      inside = inside && x[a] >= g.lo[a] && x[a] <= g.hi[a];
+    }
+    float sigma = 0.f;
+    int c[3];
+    if (inside && occupied(g, x, c)) {
+      Blend b;
+      sigma = blend_density(g, cells, radius, tm, x, b);
+    }
+    const float s = __fmul_rn(sigma, delta);
+    w[i] = __fmul_rn(__fsub_rn(1.f, expf(-s)), expf(-depth));
+    depth = __fadd_rn(depth, s);
+  }
+}
+
 GParams make_params(const mipnerf_b200_grid& grid) {
   GParams g{};
   g.num_levels = grid.num_levels;
@@ -652,6 +702,21 @@ cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_
   const auto launch = [&](const auto& cells) {
     grid_visibility_kernel<std::decay_t<decltype(cells)>><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
         g, rays, step, mw, cells);
+  };
+  if (bricks) launch(BrickCells{*bricks});
+  else launch(DenseCells{});
+  return cudaGetLastError();
+}
+
+cudaError_t launch_grid_proposal(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
+                                 const mipnerf_b200_rays& rays, const float* t_samples, int num_samples,
+                                 float* weights, cudaStream_t st) {
+  if (rays.num_rays == 0) return cudaSuccess;
+  const GParams g = make_params(grid);
+  LaunchScope scope(kKernGridProposal, st);
+  const auto launch = [&](const auto& cells) {
+    grid_proposal_kernel<std::decay_t<decltype(cells)>><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
+        g, rays, t_samples, num_samples, weights, cells);
   };
   if (bricks) launch(BrickCells{*bricks});
   else launch(DenseCells{});

@@ -83,6 +83,10 @@ cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mip
 cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
                                    const mipnerf_b200_rays& rays, float step, float* const* max_weight, int id,
                                    cudaStream_t st);
+// bricks NULL: the dense cells
+cudaError_t launch_grid_proposal(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
+                                 const mipnerf_b200_rays& rays, const float* t_samples, int num_samples,
+                                 float* weights, cudaStream_t st);
 template <class F>  // f(std::integral_constant<int, NC>{}), NC = (degree + 1)^2 for degree 0..3: the grid kernels' NC
 void with_sh_coeffs(int degree, F&& f) {
   if (degree == 0) return f(std::integral_constant<int, 1>{});

@@ -1915,7 +1915,7 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
                        int randomized, const float* t_rand, const float* u_jitter, const mipnerf_b200_rng* rng,
                        int white_bkgd, int precision, mipnerf_b200_level_out* outs, void* workspace,
                        size_t workspace_bytes, cudaStream_t st, const TcTrainDump* dump, int64_t ray_base,
-                       int given_t) {
+                       int given_t, const float* const* proposal) {
   const uint8_t* img = static_cast<const uint8_t*>(w->packed);
   SmallUpload small(img, st);  // biases / heads -> constant bank, ordered against other streams' forwards
   cudaError_t e = small.error();
@@ -1937,19 +1937,22 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
       if (!array) d.ray_base += ray_base;
       return d;
     };
-    const float *t_prev = nullptr, *w_prev = nullptr;
-    for (int l = 0; l < c->num_levels; ++l) {
-      float* t_cur = outs[l].t_samples ? outs[l].t_samples + off * (n + 1) : s.t[l & 1];
-      float* w_cur = outs[l].weights ? outs[l].weights + off * n : s.w[l & 1];
+    const int first = proposal ? 1 : 0;
+    const float* t_prev = proposal ? proposal[0] + off * (n + 1) : nullptr;
+    const float* w_prev = proposal ? proposal[1] + off * n : nullptr;
+    for (int l = first; l < c->num_levels; ++l) {
+      const mipnerf_b200_level_out& o = outs[l - first];
+      float* t_cur = o.t_samples ? o.t_samples + off * (n + 1) : s.t[l & 1];
+      float* w_cur = o.weights ? o.weights + off * n : s.w[l & 1];
       const Draws jit = draws(u_jitter, 1 + l);  // one stream per level
-      int64_t* inds = outs[l].inds ? outs[l].inds + off * (n + 1) : nullptr;
+      int64_t* inds = o.inds ? o.inds + off * (n + 1) : nullptr;
       LevelParams p{};
       p.wimage = img;
       p.origins = origins, p.directions = directions, p.radii = radii;
       p.t = t_cur;
       p.view_bias = s.vbias;
       p.t_mode = given_t ? 0 : (l == 0 ? 1 : 2);  // 0: the caller's fenceposts in outs[l].t_samples
-      p.vb_mode = l == 0 ? 1 : 0;  // level 0 leaves the per-ray bias in s.vbias for the later levels
+      p.vb_mode = l == first ? 1 : 0;  // the first level leaves the per-ray bias in s.vbias for the later levels
       p.near = rays->near + off, p.far = rays->far + off;
       p.t_rand = draws(t_rand, 0);
       p.disparity = c->disparity;
@@ -1964,16 +1967,16 @@ cudaError_t tc_forward(const mipnerf_b200_config* c, const mipnerf_b200_weights*
         p.raw_rgb_keep = dump->raw_rgb[l], p.raw_density_keep = dump->raw_density[l];
         p.dump_tiles = cnt;
       }
-      p.comp_rgb = outs[l].comp_rgb + off * 3;
-      p.distance = outs[l].distance + off;
-      p.acc = outs[l].acc + off;
+      p.comp_rgb = o.comp_rgb + off * 3;
+      p.distance = o.distance + off;
+      p.acc = o.acc + off;
       p.weights = w_cur;
       p.num_rays = cnt;
       p.white_bkgd = white_bkgd;
       p.disable_integration = c->disable_integration;
       p.density_bias = c->density_bias, p.rgb_scale = rgb_scale, p.rgb_padding = c->rgb_padding;
-      p.dnoise = density_noise_draws(c, randomized, outs[l].density_normal, rng, off, l, n);
-      if (!outs[l].density_normal) p.dnoise.ray_base += ray_base;
+      p.dnoise = density_noise_draws(c, randomized, o.density_normal, rng, off, l, n);
+      if (!o.density_normal) p.dnoise.ray_base += ray_base;
       // the split precisions' training forward dumps the lo halves as well (kTrain); bf16x3 is the one that trains
       if (dump && is_x3(precision))
         e = fmt_of(precision) == MIPNERF_B200_BF16 ? launch_level_t<1, true, 1, kModeForward, true>(p, st)

@@ -97,9 +97,12 @@ cudaError_t tc_forward(const mipnerf_b200_config* cfg, const mipnerf_b200_weight
                        const mipnerf_b200_rays* rays, int randomized, const float* t_rand,
                        const float* u_jitter, const mipnerf_b200_rng* rng, int white_bkgd, int precision,
                        mipnerf_b200_level_out* outs, void* workspace, size_t workspace_bytes, cudaStream_t st,
-                       const TcTrainDump* dump = nullptr, int64_t ray_base = 0, int given_t = 0);
+                       const TcTrainDump* dump = nullptr, int64_t ray_base = 0, int given_t = 0,
+                       const float* const* proposal = nullptr);
 // given_t != 0: every level reads its fenceposts from outs[l].t_samples instead of generating them (sampling /
 // resampling skipped; the backward pass of MipNerf.forward re-evaluates the MLP where the forward did)
+// proposal = {t_prev [B,N+1], w_prev [B,N]}: the loop starts at level 1, resampling those in place of level 0's
+// outputs; outs[l - 1] is level l's output, and level 1 computes the per-ray view bias level 0 would have
 // the uniforms of one launch (see mlp_tc.cu)
 Draws level_draws(int randomized, const float* array, const mipnerf_b200_rng* rng, int64_t off, int stream, int ncols);
 // the density-noise normals of one launch of `level` (inactive unless randomized and cfg->density_noise > 0)

@@ -196,11 +196,12 @@ class LevelOutputs(list):
     pixels: Optional[torch.Tensor] = None
 
 
-def _level_outputs(b: int, n: int, levels: int, dev, normals, return_inds: bool):
+def _level_outputs(b: int, n: int, levels: int, dev, normals, return_inds: bool, first: int = 0):
     """(LevelOutputs, LevelOut array) of a call on b rays with n samples per level, in one allocation: the pixel outputs
     (comp_rgb | distance | acc = 5 floats per ray) of all levels first, so that a caller that only wants pixels reads
     them back with ONE contiguous copy (`.pixels`, [levels, 5*B]); then weights / fenceposts per level.  `normals`: the
-    density normals handed to the library, one tensor or None per level."""
+    density normals handed to the library, one tensor or None per level.  `first`: the model level of entry 0 (1 for
+    `forward_proposed`, whose levels all resample and so all have inds)."""
     flat = torch.empty(levels * b * (5 + n + n + 1), device=dev)
     ret = LevelOutputs()
     ret.pixels = flat[:levels * 5 * b].view(levels, 5 * b) if b > 0 else flat[:0].view(levels, 0)
@@ -214,7 +215,7 @@ def _level_outputs(b: int, n: int, levels: int, dev, normals, return_inds: bool)
         q = tail + lvl * (2 * n + 1) * b
         w = flat[q:q + n * b].view(b, n)
         t = flat[q + n * b:q + (2 * n + 1) * b].view(b, n + 1)
-        inds = torch.empty(b, n + 1, device=dev, dtype=torch.int64) if (return_inds and lvl > 0) else None
+        inds = torch.empty(b, n + 1, device=dev, dtype=torch.int64) if (return_inds and lvl + first > 0) else None
         outs[lvl] = _cabi.LevelOut(comp.data_ptr(), dist.data_ptr(), acc.data_ptr(), w.data_ptr(), t.data_ptr(),
                                    _ptr(inds), _ptr(normals[lvl]))
         ret.append((comp, dist, acc, w, t, inds) if return_inds else (comp, dist, acc, w, t))
@@ -340,6 +341,64 @@ class MipNerf(torch.nn.Module):
         if self._builds_graph():
             return _forward_with_grad(self, rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds)
         return self._forward(rays, randomized, white_bkgd, t_rand, u_jitter, density_normal, return_inds)[0]
+
+    @torch.no_grad()
+    def forward_proposed(self, rays: Rays, grid, randomized: bool, white_bkgd: bool, *,
+                         t_rand: Optional[torch.Tensor] = None, u_jitter: Optional[torch.Tensor] = None,
+                         density_normal=None, return_inds: bool = False):
+        """`forward` with level 0's MLP replaced by a baked grid's proposal (mip-NeRF 360's proposal sampling) ->
+        levels 1..L-1 of `forward`'s list, in its tuple format.  Level 0's fenceposts are the library's
+        `sample_along_rays` (t_rand, or Philox stream 0 of `next_rng()` when randomized with no draws given), its
+        weights `grid.proposal(rays, t_samples)` (`BakedGrid.proposal`); the later levels resample from those on the
+        unchanged level kernels, with `forward`'s draws (u_jitter; density_normal is one tensor per level as for
+        `forward`, level 0's unused).  Inference only: no graph, also on an autograd model."""
+        if self.num_levels < 2:
+            raise ValueError(f"forward_proposed: num_levels={self.num_levels}; the proposal replaces level 0 of a "
+                             "model with at least 2 levels")
+        if self.ray_shape != 'cone':
+            raise NotImplementedError(f"forward_proposed: ray_shape={self.ray_shape!r}")  # models/mip.py:97-98
+        if self.use_viewdirs and not self._append_identity:
+            raise RuntimeError("append_identity=False: view encoding width does not match view_layers "
+                               "(same failure as the reference)")
+        dev = _dev(rays.origins)
+        b, n = rays.origins.shape[0], self.num_samples
+        rs, keep = _rays_struct(rays.origins, rays.directions, rays.viewdirs, rays.radii, rays.near, rays.far)
+        rng, t_rand, u_jitter, normals = self._noise(randomized, b, dev, t_rand, u_jitter, density_normal)
+        lib = _cabi.lib()
+        t0 = torch.empty(b, n + 1, device=dev)
+        if rng is not None:
+            t_rand = torch.empty(b, n + 1, device=dev)
+            _call(dev, "philox_uniform", lib.mipnerf_b200_philox_uniform, C.byref(rng), 0, b, n + 1, t_rand.data_ptr())
+        _call(dev, "sample_along_rays", lib.mipnerf_b200_sample_along_rays, C.byref(rs), n, int(bool(randomized)),
+              int(bool(self.disparity)), _ptr(t_rand), t0.data_ptr(), None, None)
+        return self._forward_from(rays, t0, grid.proposal(rays, t0), randomized, white_bkgd, rng, u_jitter, normals,
+                                  return_inds)
+
+    def _forward_from(self, rays: Rays, t_prev: torch.Tensor, w_prev: torch.Tensor, randomized: bool,
+                      white_bkgd: bool, rng, u_jitter, normals, return_inds: bool):
+        """Levels 1..L-1 of `forward` from level-0 fenceposts t_prev [B,N+1] and weights w_prev [B,N]
+        (mipnerf_b200_forward_proposed(_rng)); rng / u_jitter / normals as `_noise` returns them."""
+        dev = _dev(rays.origins)
+        b, n = rays.origins.shape[0], self.num_samples
+        prec = _cabi.PRECISIONS[self.precision]
+        cfg = self._config()
+        rs, keep = _rays_struct(rays.origins, rays.directions, rays.viewdirs, rays.radii, rays.near, rays.far)
+        t_prev, w_prev = _f32(t_prev), _f32(w_prev)
+        if tuple(t_prev.shape) != (b, n + 1) or tuple(w_prev.shape) != (b, n):
+            raise ValueError(f"t_prev {tuple(t_prev.shape)} / w_prev {tuple(w_prev.shape)}: need [{b}, {n + 1}] / "
+                             f"[{b}, {n}]")
+        ws, wkeep = self.mlp._weights_struct(cfg, prec, dev)
+        ret, outs = _level_outputs(b, n, self.num_levels - 1, dev, normals[1:], return_inds, first=1)
+        lib = _cabi.lib()
+        scratch = _Workspace.get(dev, lib.mipnerf_b200_workspace_bytes(C.byref(cfg), b, prec))
+        args = (C.byref(cfg), C.byref(ws), C.byref(rs), t_prev.data_ptr(), w_prev.data_ptr())
+        if rng is not None:
+            _call(dev, "MipNerf.forward_proposed", lib.mipnerf_b200_forward_proposed_rng, *args, C.byref(rng),
+                  int(bool(white_bkgd)), prec, outs, scratch.data_ptr(), scratch.numel())
+        else:
+            _call(dev, "MipNerf.forward_proposed", lib.mipnerf_b200_forward_proposed, *args, int(bool(randomized)),
+                  _ptr(u_jitter), int(bool(white_bkgd)), prec, outs, scratch.data_ptr(), scratch.numel())
+        return ret
 
     def _builds_graph(self) -> bool:
         """`forward` and the queries return outputs with a grad_fn: autograd=True, grad mode on, and some MLP
