@@ -263,6 +263,25 @@ int mipnerf_b200_backward(const mipnerf_b200_config* cfg, const mipnerf_b200_wei
 int mipnerf_b200_distloss_backward(const float* weights, const float* samples, int64_t num_rays, int num_samples,
                                    const float* grad_out, float scale, float* d_weights, void* stream);
 
+/* mip-NeRF 360's interlevel loss, which trains proposal weights to cover the fine weights.  Per ray: fine fenceposts
+ * t [B, n+1] and weights w [B, n], proposal fenceposts t_hat [B, n_hat+1] and weights w_hat [B, n_hat], n, n_hat >= 1
+ * (neither needs to be sorted).  With C_0 = 0, C_{k+1} = C_k + w_hat_k (M = n_hat), for fine interval i:
+ *   lo_i = clamp(#{k : t_hat_k <= t_i} - 1, 0, M),  hi_i = clamp(#{k : t_hat_k < t_{i+1}}, 0, M)  (exact fp32
+ *   comparisons; for sorted fenceposts, the proposal intervals that overlap fine interval i),
+ *   bound_i = C_{hi_i} - C_{lo_i} (0 when hi_i <= lo_i),
+ *   per_ray_loss[r] = sum_i max(0, w_i - bound_i)^2 / (w_i + FLT_EPSILON),
+ * in fp64, rounded once to fp32.  The result is bit for bit the same across runs and across any split of the rays into
+ * calls.  The refusals, in order: num_rays < 0, a NULL tensor when num_rays > 0, then n or n_hat < 1. */
+int mipnerf_b200_interlevel_loss(const float* t, const float* w, int n, const float* t_hat, const float* w_hat,
+                                 int n_hat, int64_t num_rays, float* per_ray_loss, void* stream);
+/* Its gradient with respect to w_hat (t, w and t_hat are constants: the paper's stop-gradient), written:
+ *   d_w_hat[r, j] = grad_out[0] * scale * sum_{i : lo_i <= j < hi_i} -2 max(0, w_i - bound_i) / (w_i + FLT_EPSILON)
+ * (grad_out: device scalar, NULL = 1; the mean over rays is scale = 1/num_rays), the sum in fp64 in increasing i.  The
+ * same determinism and refusals as the loss, with d_w_hat in place of per_ray_loss.  No synchronisation. */
+int mipnerf_b200_interlevel_loss_backward(const float* t, const float* w, int n, const float* t_hat,
+                                          const float* w_hat, int n_hat, int64_t num_rays, const float* grad_out,
+                                          float scale, float* d_w_hat, void* stream);
+
 /* Stand-alone tensor-core linear layer  y[m,n] = act(x[m,k] . weight[n,k]^T + bias)  (wgmma, 16-bit operands, fp32
  * accumulate; n in {128,256}, k in {96,128,256}): the GEMM the training step uses for its forward and dgrad passes in
  * BF16 / FP16 mode.  `scratch` receives the packed weight image (n * ceil(k/64) * 128 bytes). */
@@ -635,6 +654,23 @@ int mipnerf_b200_grid_visibility_bricks(const mipnerf_b200_grid* grid, const mip
 int mipnerf_b200_grid_proposal(const mipnerf_b200_grid* grid, const mipnerf_b200_grid_bricks* bricks,
                                const mipnerf_b200_rays* rays, const float* t_samples, int num_samples, float* weights,
                                void* stream);
+
+/* The derivative of sum_{r,i} d_weights[r,i] w[r,i], w = mipnerf_b200_grid_proposal's weights (same grid, rays and
+ * t_samples [B, num_samples+1]), with respect to the kept points' densities, ADDED into grads->density (the caller
+ * zeroes it; required for every level whose levels[l].sh is non-NULL).  grads->sh is not read.  Dense fp32 cells only
+ * (levels[l].cells): a trainable grid is dense.  Per ray, with g_i = d_weights[r,i], s_i = sigma_i delta_i and S_i =
+ * sum_{j<i} s_j, so that w_i = e^{-S_i} - e^{-S_{i+1}}:
+ *   dL/ds_k = g_k e^{-S_{k+1}} - sum_{i>k} g_i w_i,   dL/dsigma_k = delta_k dL/ds_k,
+ * each w_i recomputed with the forward's fp32 expressions and the suffix formed as total - prefix, then scattered
+ * through the level blend and trilinear weights into the kept corners.  A midpoint outside the bounds or in an empty
+ * macro cell (which the forward does not look up) gets no gradient.  So the gradient can raise density only at kept
+ * points whose midpoints fall in occupied macro cells: empty space stays empty.  The scatter is fp32 atomic adds:
+ * reproducible to round-off, not bit for bit.  The refusals, in order: grid NULL, the rays, t_samples / d_weights /
+ * grads NULL (when num_rays > 0), num_samples outside 1..256, the grid, then a NULL grads->density[l] (when
+ * num_rays > 0).  No allocation, no synchronisation. */
+int mipnerf_b200_grid_proposal_backward(const mipnerf_b200_grid* grid, const mipnerf_b200_rays* rays,
+                                        const float* t_samples, int num_samples, const float* d_weights,
+                                        const mipnerf_b200_grid_grads* grads, void* stream);
 
 /* The total-variation prior of a baked grid (Plenoxels), for fine-tuning.  Per level l, on that level's own lattice:
  * for each kept point p (SH row r, lattice position points[l][r] = i + nx (j + ny k), r < num_points[l] = M_l) and

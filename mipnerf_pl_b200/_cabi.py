@@ -138,6 +138,9 @@ _SIGNATURES = {
                                         C.POINTER(Rng), _V, C.c_int, C.c_int, C.POINTER(LevelCotangent),
                                         C.POINTER(LinearGrad), C.c_int, C.c_int, _V, C.c_size_t, _V]),
     "mipnerf_b200_distloss_backward": (C.c_int, [_V, _V, C.c_int64, C.c_int, _V, C.c_float, _V, _V]),
+    "mipnerf_b200_interlevel_loss": (C.c_int, [_V, _V, C.c_int, _V, _V, C.c_int, C.c_int64, _V, _V]),
+    "mipnerf_b200_interlevel_loss_backward": (C.c_int, [_V, _V, C.c_int, _V, _V, C.c_int, C.c_int64, _V, C.c_float,
+                                                        _V, _V]),
     "mipnerf_b200_linear_tc": (C.c_int, [_V, _V, _V, _V, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),
     "mipnerf_b200_wgrad_tc_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "mipnerf_b200_wgrad_tc": (C.c_int, [_V, C.c_int, _V, C.c_int, _V, C.c_int, C.c_int, C.c_int64, _V, _V, C.c_int, _V,
@@ -200,6 +203,8 @@ _SIGNATURES = {
                                                       C.c_float, C.POINTER(_V), _V]),
     "mipnerf_b200_grid_proposal": (C.c_int, [C.POINTER(Grid), C.POINTER(GridBricks), C.POINTER(RaysStruct), _V,
                                              C.c_int, _V, _V]),
+    "mipnerf_b200_grid_proposal_backward": (C.c_int, [C.POINTER(Grid), C.POINTER(RaysStruct), _V, C.c_int, _V,
+                                                      C.POINTER(GridGrads), _V]),
     "mipnerf_b200_grid_tv": (C.c_int, [C.POINTER(Grid), C.POINTER(_V), _i64p, C.c_float, C.POINTER(_V), C.POINTER(_V),
                                        _V, C.POINTER(GridGrads), _V]),
     "mipnerf_b200_selftest_umma": (C.c_int, [_V, _V, _V, C.c_int, C.c_int, C.c_int, C.c_int, _V, C.c_size_t, _V]),

@@ -588,12 +588,26 @@ class BakedGrid:
         else:
             _call(dev, "grid_visibility", _cabi.lib().mipnerf_b200_grid_visibility, C.byref(g), C.byref(rs), st, mw)
 
-    @torch.no_grad()
-    def proposal(self, rays: Rays, t_samples: torch.Tensor) -> torch.Tensor:
+    def proposal(self, rays: Rays, t_samples: torch.Tensor, differentiable: bool = False) -> torch.Tensor:
         """Proposal weights [B, N] of flat `rays` at fenceposts `t_samples` [B, N+1] (1 <= N <= 256), on
         mipnerf_b200_grid_proposal: per interval, the grid's density at its midpoint under the renderer's level blend,
         composited as volumetric_rendering's weights with no early stop.  What `MipNerf.forward_proposed` resamples
-        level 1 from.  Dense, sparse, quantized and trainable grids (synced first); no gradient."""
+        level 1 from.  Dense, sparse, quantized and trainable grids (synced first); no gradient.  With
+        `differentiable`, on a trainable grid in grad mode, the weights carry a graph in `kept_density`
+        (mipnerf_b200_grid_proposal_backward, what `finetune_proposal` trains through): the SH rows get no gradient,
+        and rays or fenceposts that require grad are refused, as they have none.  Anywhere else `differentiable`
+        changes nothing."""
+        if not differentiable or self.kept_density is None or not torch.is_grad_enabled():
+            with torch.no_grad():
+                return self._proposal(rays, t_samples)[0]
+        if t_samples.requires_grad or any(isinstance(f, torch.Tensor) and f.requires_grad for f in rays):
+            raise ValueError("BakedGrid.proposal: rays or t_samples that require grad; the grid has no gradient for "
+                             "them")
+        self._sync()
+        return _GridProposal.apply(self, rays, t_samples, *self.parameters())
+
+    def _proposal(self, rays: Rays, t_samples: torch.Tensor):
+        """(weights, the fp32 ray fields the launch read, the fp32 fenceposts it read)."""
         dev = _dev(self.sh[0])
         rs, keep = _grid_rays(rays, dev)
         b = rs.num_rays
@@ -606,7 +620,7 @@ class BakedGrid:
         out = torch.empty(b, n, device=dev)
         _call(dev, "grid_proposal", _cabi.lib().mipnerf_b200_grid_proposal, C.byref(self._struct()),
               C.byref(self._bricks_struct()) if self.sparse else None, C.byref(rs), t.data_ptr(), n, out.data_ptr())
-        return out
+        return out, keep, t
 
     @torch.no_grad()
     def prune(self, max_weight: Sequence[torch.Tensor], weight_threshold: float) -> "BakedGrid":
@@ -971,6 +985,38 @@ class _GridRender(torch.autograd.Function):
         return (None, None, None, None, *grads)
 
 
+class _GridProposal(torch.autograd.Function):
+    """BakedGrid.proposal of a trainable grid: the forward is the no-grad launch; the backward zeroes one gradient per
+    kept density and adds mipnerf_b200_grid_proposal_backward into them.  The SH rows get None."""
+
+    @staticmethod
+    def forward(ctx, grid, rays, t_samples, *params):
+        out, rays_keep, t = grid._proposal(rays, t_samples)
+        ctx.grid, ctx.num_rays = grid, out.shape[0]
+        # the densities and the ray fields and fenceposts the kernel reads: an in-place update of any of them before the
+        # backward raises autograd's version error
+        ctx.save_for_backward(*params[0::2], t, *rays_keep)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_weights):
+        grid = ctx.grid
+        saved = ctx.saved_tensors
+        dens, t, rays_keep = saved[:grid.levels], saved[grid.levels], saved[grid.levels + 1:]
+        dev = _dev(grid.cells[0])
+        grads = [torch.zeros_like(d, memory_format=torch.contiguous_format) for d in dens]
+        gg = _cabi.GridGrads()
+        for lvl, g in enumerate(grads):
+            if g.numel():
+                gg.density[lvl] = g.data_ptr()
+        gw = _f32(d_weights)
+        rs = _cabi.RaysStruct(*[x.data_ptr() for x in rays_keep], ctx.num_rays)
+        _call(dev, "grid_proposal_backward", _cabi.lib().mipnerf_b200_grid_proposal_backward, C.byref(grid._struct()),
+              C.byref(rs), t.data_ptr(), t.shape[1] - 1, gw.data_ptr(), C.byref(gg))
+        return (None, None, None, *[x for g in grads for x in (g, None)])
+
+
 def _tv_launch(grid: BakedGrid, pos, terms=None, weights=None, grads=None) -> None:
     """mipnerf_b200_grid_tv on a dense fp32 grid: per-level terms (a pair of lists of [M_l] tensors) and / or the
     weighted gradient (a list [density_0, sh_0, ...] with the shapes of `parameters()`, `weights` a device fp32 [2])."""
@@ -1210,6 +1256,39 @@ def finetune_grid(grid: BakedGrid, bank, steps: int, batch_size: int = 8192, lr_
         for p in params:
             p.grad = None
         total.backward()
+        opt.step()
+        losses.append(loss.detach())
+    return torch.stack(losses).tolist() if losses else []
+
+
+def finetune_proposal(grid: BakedGrid, model, bank, steps: int, batch_size: int = 8192,
+                      lr_density: float = FINETUNE_LR_DENSITY, generator: Optional[torch.Generator] = None) -> List[float]:
+    """Fine-tune a baked grid's kept densities as the proposal of `model` (`MipNerf.forward_proposed`), with mip-NeRF
+    360's interlevel loss.  Per step: a random batch of a `DeviceRayBank`'s rays; level 0's randomized fenceposts t_hat
+    as `forward_proposed` draws them; the proposal weights w_hat = `grid.proposal(rays, t_hat, differentiable=True)`,
+    with their graph; `model`'s later levels from (t_hat, w_hat) under no_grad; `ops.interlevel_loss` of the last
+    level's (t, w) against (t_hat, w_hat), its backward through mipnerf_b200_grid_proposal_backward, and one
+    `FusedAdam` step (`lr_density`) on the kept densities only.  The SH rows and the kept set never change, and the model is not trained.  The loss
+    can raise density only at kept points whose samples fall in occupied macro cells: the proposal weights have no
+    gradient in empty space, so fine weight behind a hole the bake left stays uncovered.  Makes the grid trainable if
+    it is not, and refuses what `forward_proposed` refuses; returns the per-step losses."""
+    from .ops import interlevel_loss
+    from .train import FusedAdam
+    model._check_proposed("finetune_proposal")
+    grid.requires_grad_(True)
+    params = [d for d in grid.kept_density if d.numel()]  # a level without kept points has nothing to train
+    opt = FusedAdam([{"params": params, "lr": float(lr_density)}])
+    losses = []
+    for _ in range(int(steps)):
+        rays, _ = bank.sample(batch_size, generator)
+        t_hat, rng, u_jitter, normals = model._proposal_fenceposts(rays, True, None, None, None)
+        w_hat = grid.proposal(rays, t_hat, differentiable=True)
+        with torch.no_grad():
+            fine = model._forward_from(rays, t_hat, w_hat.detach(), True, True, rng, u_jitter, normals, False)[-1]
+        loss = interlevel_loss(fine[4], fine[3], t_hat, w_hat)
+        for p in params:
+            p.grad = None
+        loss.backward()
         opt.step()
         losses.append(loss.detach())
     return torch.stack(losses).tolist() if losses else []

@@ -1445,6 +1445,35 @@ int mipnerf_b200_distloss_backward(const float* weights, const float* samples, i
   return MIPNERF_B200_OK;
 }
 
+// The interlevel loss entry points' refusals, in order: num_rays, the NULL tensors (`out`: per_ray_loss or d_w_hat),
+// then n and n_hat.
+static int check_interlevel(const float* t, const float* w, int n, const float* t_hat, const float* w_hat, int n_hat,
+                            int64_t num_rays, const float* out) {
+  if (num_rays < 0) return fail(MIPNERF_B200_EINVAL, "num_rays=%lld: need >= 0", (long long)num_rays);
+  if (num_rays > 0 && (!t || !w || !t_hat || !w_hat || !out)) return fail(MIPNERF_B200_EINVAL, "NULL tensor");
+  if (n < 1 || n_hat < 1) return fail(MIPNERF_B200_EINVAL, "n=%d, n_hat=%d: need >= 1", n, n_hat);
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_interlevel_loss(const float* t, const float* w, int n, const float* t_hat, const float* w_hat,
+                                 int n_hat, int64_t num_rays, float* per_ray_loss, void* stream) {
+  int rc;
+  if ((rc = check_interlevel(t, w, n, t_hat, w_hat, n_hat, num_rays, per_ray_loss))) return rc;
+  CUDA_TRY(mipnerf::launch_interlevel_loss(t, w, n, t_hat, w_hat, n_hat, num_rays, per_ray_loss,
+                                           (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_interlevel_loss_backward(const float* t, const float* w, int n, const float* t_hat,
+                                          const float* w_hat, int n_hat, int64_t num_rays, const float* grad_out,
+                                          float scale, float* d_w_hat, void* stream) {
+  int rc;
+  if ((rc = check_interlevel(t, w, n, t_hat, w_hat, n_hat, num_rays, d_w_hat))) return rc;
+  CUDA_TRY(mipnerf::launch_interlevel_loss_backward(t, w, n, t_hat, w_hat, n_hat, num_rays, grad_out, scale, d_w_hat,
+                                                    (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
 size_t mipnerf_b200_image_metrics_scratch_bytes(int height, int width, int channels) {
   if (height < 1 || width < 1 || channels < 1) return 0;
   return mipnerf::image_metrics_scratch_bytes(height, width, channels);
@@ -2218,6 +2247,26 @@ int mipnerf_b200_grid_proposal(const mipnerf_b200_grid* g, const mipnerf_b200_gr
     return fail(MIPNERF_B200_EINVAL, "num_samples=%d: need 1..256", num_samples);
   if ((rc = check_grid(g, bricks))) return rc;
   CUDA_TRY(mipnerf::launch_grid_proposal(*g, bricks, *rays, t_samples, num_samples, weights, (cudaStream_t)stream));
+  return MIPNERF_B200_OK;
+}
+
+int mipnerf_b200_grid_proposal_backward(const mipnerf_b200_grid* g, const mipnerf_b200_rays* rays,
+                                        const float* t_samples, int num_samples, const float* d_weights,
+                                        const mipnerf_b200_grid_grads* grads, void* stream) {
+  int rc;
+  if (!g) return fail(MIPNERF_B200_EINVAL, "grid is NULL");
+  if ((rc = check_rays(rays))) return rc;
+  if (rays->num_rays > 0 && (!t_samples || !d_weights || !grads))
+    return fail(MIPNERF_B200_EINVAL, "t_samples / d_weights / grads is NULL");
+  if (num_samples < 1 || num_samples > 256)
+    return fail(MIPNERF_B200_EINVAL, "num_samples=%d: need 1..256", num_samples);
+  if ((rc = check_grid(g))) return rc;
+  if (rays->num_rays == 0) return MIPNERF_B200_OK;
+  for (int l = 0; l < g->num_levels; ++l)
+    if (g->levels[l].sh && !grads->density[l])
+      return fail(MIPNERF_B200_EINVAL, "level %d has kept points: grads->density[%d] is NULL", l, l);
+  CUDA_TRY(mipnerf::launch_grid_proposal_backward(*g, *rays, t_samples, num_samples, d_weights, *grads,
+                                                  (cudaStream_t)stream));
   return MIPNERF_B200_OK;
 }
 

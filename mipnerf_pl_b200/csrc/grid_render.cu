@@ -577,6 +577,44 @@ __global__ void __launch_bounds__(kGridThreads)
   }
 }
 
+// One ray of the proposal kernels: origin, direction, radius and |d|, rounded as the header states.
+struct ProposalRay {
+  float o[3], d[3];
+  float radius, dn;
+};
+
+__device__ __forceinline__ void proposal_ray(const mipnerf_b200_rays& rays, int64_t r, ProposalRay& p) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a) p.o[a] = __ldg(rays.origins + 3 * r + a), p.d[a] = __ldg(rays.directions + 3 * r + a);
+  p.radius = __ldg(rays.radii + r);
+  p.dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(p.d[0], p.d[0]), __fmul_rn(p.d[1], p.d[1])),
+                              __fmul_rn(p.d[2], p.d[2])));
+}
+
+// Interval [t0, t1] of a proposal ray: its delta, and the density at its midpoint under the level blend.  A midpoint
+// outside the bounds or in an empty macro cell is not looked up (density 0, `looked_up` false, `b` unset).
+template <class Cells>
+__device__ __forceinline__ float proposal_density(const GParams& g, const Cells& cells, const ProposalRay& p, float t0,
+                                                  float t1, float& delta, Blend& b, bool& looked_up) {
+  const float tm = __fmul_rn(__fadd_rn(t0, t1), 0.5f);
+  delta = __fmul_rn(__fsub_rn(t1, t0), p.dn);
+  float x[3];
+  bool inside = true;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    x[a] = __fadd_rn(p.o[a], __fmul_rn(tm, p.d[a]));
+    inside = inside && x[a] >= g.lo[a] && x[a] <= g.hi[a];
+  }
+  float sigma = 0.f;
+  int c[3];
+  looked_up = false;
+  if (inside && occupied(g, x, c)) {
+    looked_up = true;
+    sigma = blend_density(g, cells, p.radius, tm, x, b);
+  }
+  return sigma;
+}
+
 // Proposal weights of the caller's intervals (mipnerf_b200_grid_proposal), one thread per ray.  Interval i is sampled
 // at its midpoint with blend_density, and its weight is volumetric_rendering's (1 - exp(-s_i)) exp(-sum_{j<i} s_j),
 // s_i = sigma_i delta_i, with every interval weighted: no stop.  A midpoint in an empty macro cell has density exactly
@@ -588,36 +626,78 @@ __global__ void __launch_bounds__(kGridThreads)
                          int num_samples, float* __restrict__ weights, const __grid_constant__ Cells cells) {
   const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
   if (r >= rays.num_rays) return;
-  float o[3], d[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) o[a] = __ldg(rays.origins + 3 * r + a), d[a] = __ldg(rays.directions + 3 * r + a);
-  const float radius = __ldg(rays.radii + r);
-  const float dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
+  ProposalRay p;
+  proposal_ray(rays, r, p);
   const float* t = t_samples + r * (num_samples + 1);
   float* w = weights + r * num_samples;
   float depth = 0.f;  // sum_{j<i} s_j
   float t0 = __ldg(t);
   for (int i = 0; i < num_samples; ++i) {
     const float t1 = __ldg(t + i + 1);
-    const float tm = __fmul_rn(__fadd_rn(t0, t1), 0.5f);
-    const float delta = __fmul_rn(__fsub_rn(t1, t0), dn);
+    float delta;
+    Blend b;
+    bool looked_up;
+    const float sigma = proposal_density(g, cells, p, t0, t1, delta, b, looked_up);
     t0 = t1;
-    float x[3];
-    bool inside = true;
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      x[a] = __fadd_rn(o[a], __fmul_rn(tm, d[a]));
-      inside = inside && x[a] >= g.lo[a] && x[a] <= g.hi[a];
-    }
-    float sigma = 0.f;
-    int c[3];
-    if (inside && occupied(g, x, c)) {
-      Blend b;
-      sigma = blend_density(g, cells, radius, tm, x, b);
-    }
     const float s = __fmul_rn(sigma, delta);
     w[i] = __fmul_rn(__fsub_rn(1.f, expf(-s)), expf(-depth));
     depth = __fadd_rn(depth, s);
+  }
+}
+
+// The gradient of grid_proposal_kernel's weights with respect to the densities (mipnerf_b200_grid_proposal_backward),
+// dense fp32 cells, one thread per ray.  With g_i = d_weights[i], s_i = sigma_i delta_i and S_i = sum_{j<i} s_j, w_i =
+// e^{-S_i} - e^{-S_{i+1}}, so dL/ds_k = g_k e^{-S_{k+1}} - sum_{i>k} g_i w_i and dL/dsigma_k = delta_k dL/ds_k.  Pass 1
+// recomputes every w_i with the forward's fp32 expressions and sums g_i w_i; pass 2 walks the intervals again with the
+// same arithmetic, so its prefix sum reaches the total bit for bit, and takes the suffix as total - prefix, as
+// grid_render_backward_kernel does.  An interval the forward does not look up (midpoint outside the bounds or in an
+// empty macro cell) gets no gradient; the others scatter through the level blend and the trilinear weights into the
+// kept corners (level_scatter, density only).
+__global__ void __launch_bounds__(kGridThreads)
+    grid_proposal_backward_kernel(const GParams g, const mipnerf_b200_rays rays, const float* __restrict__ t_samples,
+                                  int num_samples, const float* __restrict__ d_weights,
+                                  const __grid_constant__ mipnerf_b200_grid_grads grads) {
+  const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
+  if (r >= rays.num_rays) return;
+  ProposalRay p;
+  proposal_ray(rays, r, p);
+  const float* t = t_samples + r * (num_samples + 1);
+  const float* gw = d_weights + r * num_samples;
+  float total = 0.f, depth = 0.f;
+  float t0 = __ldg(t);
+  for (int i = 0; i < num_samples; ++i) {
+    const float t1 = __ldg(t + i + 1);
+    float delta;
+    Blend b;
+    bool looked_up;
+    const float s = __fmul_rn(proposal_density(g, DenseCells{}, p, t0, t1, delta, b, looked_up), delta);
+    t0 = t1;
+    const float w = __fmul_rn(__fsub_rn(1.f, expf(-s)), expf(-depth));
+    depth = __fadd_rn(depth, s);
+    total = __fmaf_rn(__ldg(gw + i), w, total);
+  }
+  const float y[16] = {};
+  const float d_raw[3] = {};
+  float prefix = 0.f;
+  depth = 0.f;
+  t0 = __ldg(t);
+  for (int i = 0; i < num_samples; ++i) {
+    const float t1 = __ldg(t + i + 1);
+    float delta;
+    Blend b;
+    bool looked_up;
+    const float s = __fmul_rn(proposal_density(g, DenseCells{}, p, t0, t1, delta, b, looked_up), delta);
+    t0 = t1;
+    const float w = __fmul_rn(__fsub_rn(1.f, expf(-s)), expf(-depth));
+    depth = __fadd_rn(depth, s);  // S_{i+1}
+    const float gi = __ldg(gw + i);
+    prefix = __fmaf_rn(gi, w, prefix);
+    if (!looked_up) continue;
+    const float d_sigma = delta * (gi * expf(-depth) - (total - prefix));
+    if (d_sigma == 0.f) continue;
+    level_scatter<1>(grads.density[b.la], nullptr, b.row_a, b.w_a, b.f > 0.f ? 1.f - b.f : 1.f, y, d_sigma, d_raw,
+                     false);
+    if (b.f > 0.f) level_scatter<1>(grads.density[b.la + 1], nullptr, b.row_b, b.w_b, b.f, y, d_sigma, d_raw, false);
   }
 }
 
@@ -720,6 +800,17 @@ cudaError_t launch_grid_proposal(const mipnerf_b200_grid& grid, const mipnerf_b2
   };
   if (bricks) launch(BrickCells{*bricks});
   else launch(DenseCells{});
+  return cudaGetLastError();
+}
+
+cudaError_t launch_grid_proposal_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays,
+                                          const float* t_samples, int num_samples, const float* d_weights,
+                                          const mipnerf_b200_grid_grads& grads, cudaStream_t st) {
+  if (rays.num_rays == 0) return cudaSuccess;
+  const GParams g = make_params(grid);
+  LaunchScope scope(kKernGridProposalBackward, st);
+  grid_proposal_backward_kernel<<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(g, rays, t_samples, num_samples,
+                                                                                     d_weights, grads);
   return cudaGetLastError();
 }
 

@@ -22,6 +22,12 @@ cudaError_t launch_distloss(const float* weights, const float* t, float* out, in
 // d_w[r,i] = grad_out * scale * ((2/3) (t_{i+1} - t_i) w_i + 2 S_i),  S_i = sum_j w_j |m_i - m_j|  (grad_out NULL = 1)
 cudaError_t launch_distloss_backward(const float* weights, const float* t, const float* grad_out, float scale,
                                      float* d_w, int64_t num_rays, int n, cudaStream_t st);
+// mip-NeRF 360's interlevel loss per ray (include/mipnerf_b200.h) and its gradient in w_hat, written (grad_out NULL = 1)
+cudaError_t launch_interlevel_loss(const float* t, const float* w, int n, const float* t_hat, const float* w_hat,
+                                   int m, int64_t num_rays, float* out, cudaStream_t st);
+cudaError_t launch_interlevel_loss_backward(const float* t, const float* w, int n, const float* t_hat,
+                                            const float* w_hat, int m, int64_t num_rays, const float* grad_out,
+                                            float scale, float* d_w_hat, cudaStream_t st);
 cudaError_t launch_generate_rays(const float* c2w_host, int height, int width, float focal, float near_v,
                                  float far_v, int row0, int rows, float* origins, float* directions,
                                  float* viewdirs, float* radii, float* near_o, float* far_o, cudaStream_t st);
@@ -87,6 +93,10 @@ cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_
 cudaError_t launch_grid_proposal(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
                                  const mipnerf_b200_rays& rays, const float* t_samples, int num_samples,
                                  float* weights, cudaStream_t st);
+// dense fp32 cells; adds into grads.density only
+cudaError_t launch_grid_proposal_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays,
+                                          const float* t_samples, int num_samples, const float* d_weights,
+                                          const mipnerf_b200_grid_grads& grads, cudaStream_t st);
 template <class F>  // f(std::integral_constant<int, NC>{}), NC = (degree + 1)^2 for degree 0..3: the grid kernels' NC
 void with_sh_coeffs(int degree, F&& f) {
   if (degree == 0) return f(std::integral_constant<int, 1>{});

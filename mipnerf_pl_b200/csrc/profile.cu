@@ -30,7 +30,8 @@ const char* const kNames[kKernCount] = {"coarse_t",  "cast_rays", "ipe",        
                                         "generate_rays", "distloss", "ray_prologue",
                                         "render_backward", "dgrad_f32", "wgrad_f32", "adam", "linear_tc", "wgrad_tc",
                                         "image_metrics", "density_tc", "isosurface", "radiance_tc",
-                                        "radiance_dirs_tc", "radiance_pairs", "grid_proposal", "grid_tv", "grid_visibility_bricks",
+                                        "radiance_dirs_tc", "radiance_pairs", "interlevel_loss", "grid_proposal_backward",
+                                        "grid_proposal", "grid_tv", "grid_visibility_bricks",
                                         "grid_render_bricks", "grid_render_backward", "grid_render_u8",
                                         "grid_visibility", "grid_render"};
 

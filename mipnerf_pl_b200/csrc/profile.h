@@ -33,6 +33,8 @@ enum KernelId : int {
   kKernRadianceTc,   // radiance mode of the wgmma level kernel (IPE + per-point view term + the whole MLP)
   kKernRadianceDirsTc,  // view-accumulator mode of the wgmma level kernel (IPE + the MLP up to the view layer's GEMM)
   kKernRadiancePairs,   // per-(point, direction) view layer + colour head (+ projection) of a shared direction set
+  kKernInterlevelLoss,  // mip-NeRF 360's interlevel loss of proposal weights, and its gradient
+  kKernGridProposalBackward,  // gradient of a baked grid's proposal weights with respect to its densities
   kKernGridProposal,   // proposal weights of a baked grid at a forward's level-0 intervals
   kKernGridTv,         // total-variation terms and gradient of a baked grid's kept points
   kKernGridVisibilityBricks,  // grid_visibility on a baked grid whose cells are 8^3-point bricks

@@ -315,6 +315,108 @@ __global__ void distloss_backward_kernel(const float* __restrict__ weights, cons
 }
 
 // ---------------------------------------------------------------------------------------------
+// Interlevel loss (mip-NeRF 360's proposal loss), per ray: fine fenceposts t [N+1] and weights w [N], proposal
+// fenceposts t^ [M+1] and weights w^ [M].  Fine interval i is bounded by the proposal weight of the proposal
+// intervals it overlaps,
+//   lo_i = clamp(#{k : t^_k <= t_i} - 1, 0, M),  hi_i = clamp(#{k : t^_k < t_{i+1}}, 0, M),
+//   bound_i = sum_{lo_i <= k < hi_i} w^_k  (= C^_{hi_i} - C^_{lo_i}, 0 when hi_i <= lo_i),
+// and loss = sum_i max(0, w_i - bound_i)^2 / (w_i + eps).  The counts are exact fp32 comparisons over all M + 1
+// proposal fenceposts, so they are defined for unsorted input too; bound_i and the loss are fp64.  Warp per ray, lane
+// l owning fine intervals l, l + 32, ...; nothing is shared between rays and every sum has a fixed order, so the
+// result is bit for bit the same across runs and across any split of the rays into calls.
+// ---------------------------------------------------------------------------------------------
+constexpr double kInterlevelEps = 1.1920928955078125e-07;  // FLT_EPSILON
+
+// max(0, w_i - bound_i) of fine interval [t0, t1] of weight wi, and its proposal range [lo, hi).
+__device__ __forceinline__ double interlevel_excess(const float* __restrict__ t_hat, const float* __restrict__ w_hat,
+                                                    int m, float t0, float t1, double wi, int& lo, int& hi) {
+  int le = 0, lt = 0;
+  for (int k = 0; k <= m; ++k) {
+    const float th = __ldg(t_hat + k);
+    le += th <= t0;
+    lt += th < t1;
+  }
+  lo = min(max(le - 1, 0), m);
+  hi = min(lt, m);
+  double bound = 0.0;
+  for (int k = lo; k < hi; ++k) bound += (double)__ldg(w_hat + k);
+  return fmax(0.0, wi - bound);
+}
+
+__global__ void interlevel_loss_kernel(const float* __restrict__ t, const float* __restrict__ w, int n,
+                                       const float* __restrict__ t_hat, const float* __restrict__ w_hat, int m,
+                                       int64_t num_rays, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t ray = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (ray >= num_rays) return;
+  const float* tr = t + ray * (n + 1);
+  const float* wr = w + ray * n;
+  const float* thr = t_hat + ray * (m + 1);
+  const float* whr = w_hat + ray * m;
+  double v = 0.0;
+  for (int i = lane; i < n; i += 32) {
+    const double wi = __ldg(wr + i);
+    int lo, hi;
+    const double e = interlevel_excess(thr, whr, m, __ldg(tr + i), __ldg(tr + i + 1), wi, lo, hi);
+    v += e * e / (wi + kInterlevelEps);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if (lane == 0) out[ray] = (float)v;
+}
+
+// Its gradient with respect to w^ (t, w and t^ are constants: the stop-gradient of mip-NeRF 360):
+//   d loss / d w^_j = sum_{i : lo_i <= j < hi_i} g_i,  g_i = -2 max(0, w_i - bound_i) / (w_i + eps).
+// Lane l owns proposal weights j0 + 32 p + l (p < kInterlevelLanesJ) of a pass over 32 kInterlevelLanesJ of them; per
+// pass the lanes form g_i for 32 fine intervals at a time and broadcast them in order of i, so each d w^_j is an fp64
+// sum in increasing i.  M above 32 kInterlevelLanesJ takes more passes, each recomputing the g_i.
+constexpr int kInterlevelLanesJ = 8;
+
+__global__ void interlevel_loss_backward_kernel(const float* __restrict__ t, const float* __restrict__ w, int n,
+                                                const float* __restrict__ t_hat, const float* __restrict__ w_hat,
+                                                int m, int64_t num_rays, const float* __restrict__ grad_out,
+                                                float scale, float* __restrict__ d_w_hat) {
+  const int lane = threadIdx.x & 31;
+  const int64_t ray = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (ray >= num_rays) return;
+  const float* tr = t + ray * (n + 1);
+  const float* wr = w + ray * n;
+  const float* thr = t_hat + ray * (m + 1);
+  const float* whr = w_hat + ray * m;
+  const double up = (double)(grad_out ? __ldg(grad_out) : 1.0f) * (double)scale;
+  for (int j0 = 0; j0 < m; j0 += 32 * kInterlevelLanesJ) {
+    double acc[kInterlevelLanesJ];
+#pragma unroll
+    for (int p = 0; p < kInterlevelLanesJ; ++p) acc[p] = 0.0;
+    for (int i0 = 0; i0 < n; i0 += 32) {
+      const int i = i0 + lane;
+      double g = 0.0;
+      int lo = 0, hi = 0;
+      if (i < n) {
+        const double wi = __ldg(wr + i);
+        g = -2.0 * interlevel_excess(thr, whr, m, __ldg(tr + i), __ldg(tr + i + 1), wi, lo, hi) / (wi + kInterlevelEps);
+      }
+      const int cnt = min(32, n - i0);
+      for (int s = 0; s < cnt; ++s) {
+        const double gs = __shfl_sync(0xffffffffu, g, s);
+        const int ls = __shfl_sync(0xffffffffu, lo, s), hs = __shfl_sync(0xffffffffu, hi, s);
+        if (gs == 0.0) continue;  // the same for every lane
+#pragma unroll
+        for (int p = 0; p < kInterlevelLanesJ; ++p) {
+          const int j = j0 + 32 * p + lane;
+          if (j >= ls && j < hs) acc[p] += gs;
+        }
+      }
+    }
+#pragma unroll
+    for (int p = 0; p < kInterlevelLanesJ; ++p) {
+      const int j = j0 + 32 * p + lane;
+      if (j < m) d_w_hat[ray * m + j] = (float)(up * acc[p]);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Blender-style pinhole rays for rows [row0, row0+rows) of an H x W frame, straight into HBM
 // (datasets/datasets.py:214-263, render_video.py:29-105): one thread per pixel.
 //   camera dir = ((x - W/2 + .5)/f, -(y - H/2 + .5)/f, -1);  direction = R . dir;  origin = c2w[:,3]
@@ -459,6 +561,24 @@ cudaError_t launch_distloss_backward(const float* weights, const float* t, const
   if (num_rays == 0) return cudaSuccess;
   LaunchScope scope(kKernDistloss, st);
   distloss_backward_kernel<<<blocks_for(num_rays, 4), 128, 0, st>>>(weights, t, grad_out, scale, d_w, num_rays, n);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_interlevel_loss(const float* t, const float* w, int n, const float* t_hat, const float* w_hat,
+                                   int m, int64_t num_rays, float* out, cudaStream_t st) {
+  if (num_rays == 0) return cudaSuccess;
+  LaunchScope scope(kKernInterlevelLoss, st);
+  interlevel_loss_kernel<<<blocks_for(num_rays, 4), 128, 0, st>>>(t, w, n, t_hat, w_hat, m, num_rays, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_interlevel_loss_backward(const float* t, const float* w, int n, const float* t_hat,
+                                            const float* w_hat, int m, int64_t num_rays, const float* grad_out,
+                                            float scale, float* d_w_hat, cudaStream_t st) {
+  if (num_rays == 0) return cudaSuccess;
+  LaunchScope scope(kKernInterlevelLoss, st);
+  interlevel_loss_backward_kernel<<<blocks_for(num_rays, 4), 128, 0, st>>>(t, w, n, t_hat, w_hat, m, num_rays,
+                                                                          grad_out, scale, d_w_hat);
   return cudaGetLastError();
 }
 

@@ -352,14 +352,26 @@ class MipNerf(torch.nn.Module):
         weights `grid.proposal(rays, t_samples)` (`BakedGrid.proposal`); the later levels resample from those on the
         unchanged level kernels, with `forward`'s draws (u_jitter; density_normal is one tensor per level as for
         `forward`, level 0's unused).  Inference only: no graph, also on an autograd model."""
+        t0, rng, u_jitter, normals = self._proposal_fenceposts(rays, randomized, t_rand, u_jitter, density_normal)
+        return self._forward_from(rays, t0, grid.proposal(rays, t0), randomized, white_bkgd, rng, u_jitter, normals,
+                                  return_inds)
+
+    def _check_proposed(self, what: str) -> None:
+        """The refusals of a model whose level 0 a proposal replaces (`forward_proposed`, `finetune_proposal`)."""
         if self.num_levels < 2:
-            raise ValueError(f"forward_proposed: num_levels={self.num_levels}; the proposal replaces level 0 of a "
+            raise ValueError(f"{what}: num_levels={self.num_levels}; the proposal replaces level 0 of a "
                              "model with at least 2 levels")
         if self.ray_shape != 'cone':
-            raise NotImplementedError(f"forward_proposed: ray_shape={self.ray_shape!r}")  # models/mip.py:97-98
+            raise NotImplementedError(f"{what}: ray_shape={self.ray_shape!r}")  # models/mip.py:97-98
         if self.use_viewdirs and not self._append_identity:
             raise RuntimeError("append_identity=False: view encoding width does not match view_layers "
                                "(same failure as the reference)")
+
+    def _proposal_fenceposts(self, rays: Rays, randomized: bool, t_rand, u_jitter, density_normal):
+        """Level 0's fenceposts of a forward whose level 0 a proposal replaces -> (t0 [B,N+1], rng, u_jitter, normals):
+        the library's `sample_along_rays` with t_rand, or Philox stream 0 of `next_rng()` when randomized with no
+        draws given; the rest as `_noise` returns them, for `_forward_from`."""
+        self._check_proposed("forward_proposed")
         dev = _dev(rays.origins)
         b, n = rays.origins.shape[0], self.num_samples
         rs, keep = _rays_struct(rays.origins, rays.directions, rays.viewdirs, rays.radii, rays.near, rays.far)
@@ -371,8 +383,7 @@ class MipNerf(torch.nn.Module):
             _call(dev, "philox_uniform", lib.mipnerf_b200_philox_uniform, C.byref(rng), 0, b, n + 1, t_rand.data_ptr())
         _call(dev, "sample_along_rays", lib.mipnerf_b200_sample_along_rays, C.byref(rs), n, int(bool(randomized)),
               int(bool(self.disparity)), _ptr(t_rand), t0.data_ptr(), None, None)
-        return self._forward_from(rays, t0, grid.proposal(rays, t0), randomized, white_bkgd, rng, u_jitter, normals,
-                                  return_inds)
+        return t0, rng, u_jitter, normals
 
     def _forward_from(self, rays: Rays, t_prev: torch.Tensor, w_prev: torch.Tensor, randomized: bool,
                       white_bkgd: bool, rng, u_jitter, normals, return_inds: bool):

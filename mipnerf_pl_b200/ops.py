@@ -272,3 +272,59 @@ def distloss(weight, samples):
     if torch.is_grad_enabled() and weight.requires_grad:
         return _DistLoss.apply(weight, samples)
     return _distloss_value(_f32(weight), _f32(samples))
+
+
+def _interlevel_check(t, w, t_hat, w_hat):
+    """interlevel_loss's shape and device refusals."""
+    shapes = [tuple(x.shape) for x in (t, w, t_hat, w_hat)]
+    if not (all(len(s) == 2 for s in shapes) and len({s[0] for s in shapes}) == 1 and shapes[1][1] >= 1
+            and shapes[0][1] == shapes[1][1] + 1 and shapes[3][1] >= 1 and shapes[2][1] == shapes[3][1] + 1):
+        raise ValueError(f"interlevel_loss: t {shapes[0]}, w {shapes[1]}, t_hat {shapes[2]}, w_hat {shapes[3]}: need "
+                         "[B, N+1], [B, N], [B, M+1], [B, M] with N, M >= 1")
+    devs = {x.device for x in (t, w, t_hat, w_hat)}
+    if len(devs) != 1:
+        raise ValueError(f"interlevel_loss: tensors on {sorted(str(d) for d in devs)}; need one device")
+
+
+def _interlevel_value(t, w, t_hat, w_hat) -> torch.Tensor:
+    dev = _dev(w)
+    b, n = w.shape
+    out = torch.empty(b, device=dev)
+    _call(dev, "interlevel_loss", _cabi.lib().mipnerf_b200_interlevel_loss, t.data_ptr(), w.data_ptr(), n,
+          t_hat.data_ptr(), w_hat.data_ptr(), w_hat.shape[1], b, out.data_ptr())
+    return out.mean()
+
+
+class _InterlevelLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, t, w, t_hat, w_hat):
+        args = [_f32(x) for x in (t, w, t_hat, w_hat)]
+        ctx.save_for_backward(*args)
+        ctx.w_hat_dtype = w_hat.dtype
+        return _interlevel_value(*args)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        t, w, t_hat, w_hat = ctx.saved_tensors
+        b, n = w.shape
+        d_w_hat = torch.empty_like(w_hat)
+        g = _f32(grad_out).reshape(1)
+        _call(w.device, "interlevel_loss_backward", _cabi.lib().mipnerf_b200_interlevel_loss_backward, t.data_ptr(),
+              w.data_ptr(), n, t_hat.data_ptr(), w_hat.data_ptr(), w_hat.shape[1], b, g.data_ptr(), 1.0 / max(b, 1),
+              d_w_hat.data_ptr())
+        return None, None, None, d_w_hat.to(ctx.w_hat_dtype)
+
+
+def interlevel_loss(t, w, t_hat, w_hat):
+    """mip-NeRF 360's interlevel loss, the mean over rays of sum_i max(0, w_i - bound_i)^2 / (w_i + eps): fine
+    fenceposts t [B,N+1] and weights w [B,N], proposal fenceposts t_hat [B,M+1] and weights w_hat [B,M], bound_i the
+    proposal weight of the proposal intervals that overlap fine interval i (`mipnerf_b200_interlevel_loss`).  It
+    penalises fine weight the proposal does not cover.  Differentiable with respect to `w_hat` when it requires grad
+    (`mipnerf_b200_interlevel_loss_backward`); t, w and t_hat are constants, the paper's stop-gradient.  Deterministic:
+    the value and the gradient are bit for bit the same across runs."""
+    _interlevel_check(t, w, t_hat, w_hat)
+    _dev(w)
+    if torch.is_grad_enabled() and w_hat.requires_grad:
+        return _InterlevelLoss.apply(t, w, t_hat, w_hat)
+    return _interlevel_value(*[_f32(x) for x in (t, w, t_hat, w_hat)])
