@@ -946,12 +946,16 @@ def _level_ptrs(ts: Sequence[torch.Tensor]):
     return (C.c_void_p * len(ts))(*[t.data_ptr() if t.numel() else None for t in ts])
 
 
-def _grid_grads(grads: Sequence[torch.Tensor]) -> "_cabi.GridGrads":
-    """The GridGrads of gradients in `parameters()` order, NULL for a level without kept points."""
+def _grid_grads(grads: Sequence[Optional[torch.Tensor]]) -> "_cabi.GridGrads":
+    """The GridGrads of gradients in `parameters()` order, NULL for a level without kept points.  An SH gradient of
+    None leaves that level's `sh` NULL: density-only gradients."""
     gg = _cabi.GridGrads()
     for lvl in range(len(grads) // 2):
-        if grads[2 * lvl + 1].numel():
-            gg.density[lvl], gg.sh[lvl] = grads[2 * lvl].data_ptr(), grads[2 * lvl + 1].data_ptr()
+        density, sh = grads[2 * lvl], grads[2 * lvl + 1]
+        if density.numel():
+            gg.density[lvl] = density.data_ptr()
+            if sh is not None:
+                gg.sh[lvl] = sh.data_ptr()
     return gg
 
 
@@ -1005,16 +1009,12 @@ class _GridProposal(torch.autograd.Function):
         saved = ctx.saved_tensors
         dens, t, rays_keep = saved[:grid.levels], saved[grid.levels], saved[grid.levels + 1:]
         dev = _dev(grid.cells[0])
-        grads = [torch.zeros_like(d, memory_format=torch.contiguous_format) for d in dens]
-        gg = _cabi.GridGrads()
-        for lvl, g in enumerate(grads):
-            if g.numel():
-                gg.density[lvl] = g.data_ptr()
+        grads = [x for d in dens for x in (torch.zeros_like(d, memory_format=torch.contiguous_format), None)]
         gw = _f32(d_weights)
         rs = _cabi.RaysStruct(*[x.data_ptr() for x in rays_keep], ctx.num_rays)
         _call(dev, "grid_proposal_backward", _cabi.lib().mipnerf_b200_grid_proposal_backward, C.byref(grid._struct()),
-              C.byref(rs), t.data_ptr(), t.shape[1] - 1, gw.data_ptr(), C.byref(gg))
-        return (None, None, None, *[x for g in grads for x in (g, None)])
+              C.byref(rs), t.data_ptr(), t.shape[1] - 1, gw.data_ptr(), C.byref(_grid_grads(grads)))
+        return (None, None, None, *grads)
 
 
 def _tv_launch(grid: BakedGrid, pos, terms=None, weights=None, grads=None) -> None:

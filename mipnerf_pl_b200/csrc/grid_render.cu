@@ -2,7 +2,11 @@
 // mipnerf_pl_b200/baked.py, which owns the other half of the memory layout read here).
 //
 // One thread per ray, rays in the caller's (pixel) order, so that neighbouring threads walk neighbouring paths through
-// the same cache lines.  Per ray:
+// the same cache lines.  Every kernel walks its ray with one of two loops, each written once:
+//   * walk_samples, the march over the sample lattice of a step: the render, both passes of its backward, and the
+//     visibility scores.  Each caller composites the samples it is handed and keeps its own rule for zero density.
+//   * walk_intervals, over the caller's fenceposts: the proposal weights and both passes of their backward.
+// Per ray of walk_samples:
 //   * K, dt, t_k, delta and the sample positions o + t_k d are computed with explicitly rounded fp32 operations, so a
 //     host restatement reproduces them exactly (tests/grid_render_ref.py).
 //   * The sample range is first clipped to the bounds grown by a margin far above the rounding of those positions;
@@ -241,26 +245,49 @@ __device__ __forceinline__ void sh_basis(float x, float y, float z, float (&b)[1
   b[15] = -0.5900435899266435f * x * (xx - 3.f * yy);
 }
 
-// One ray's sample lattice, clipped to the samples inside the bounds grown by a margin.
-struct RayMarch {
+// One ray's origin, direction, cone radius and |d|, rounded as mipnerf_b200.h states.  Both walks start here; the
+// interval walk reads nothing else of the ray (no viewdirs, near or far).
+struct Ray {
   float o[3], d[3];
-  float radius, near, far;
+  float radius, dn;
+};
+
+__device__ __forceinline__ void load_ray(const mipnerf_b200_rays& rays, int64_t r, Ray& p) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a) p.o[a] = __ldg(rays.origins + 3 * r + a), p.d[a] = __ldg(rays.directions + 3 * r + a);
+  p.radius = __ldg(rays.radii + r);
+  p.dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(p.d[0], p.d[0]), __fmul_rn(p.d[1], p.d[1])),
+                              __fmul_rn(p.d[2], p.d[2])));
+}
+
+// Position x = o + t d of a ray, each coordinate fl(o + fl(t d)); whether x is inside the bounds.
+__device__ __forceinline__ bool ray_point(const GParams& g, const Ray& p, float t, float (&x)[3]) {
+  bool inside = true;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    x[a] = __fadd_rn(p.o[a], __fmul_rn(t, p.d[a]));
+    inside = inside && x[a] >= g.lo[a] && x[a] <= g.hi[a];
+  }
+  return inside;
+}
+
+// One ray's sample lattice, clipped to the samples inside the bounds grown by a margin.
+struct RayMarch : Ray {
+  float near, far;
   float dt, delta;
   int64_t k0, k1;
 };
 
 __device__ __forceinline__ void ray_setup(const GParams& g, const mipnerf_b200_rays& rays, int64_t r, float step,
                                           RayMarch& m, float (&y)[16]) {
-#pragma unroll
-  for (int a = 0; a < 3; ++a) m.o[a] = __ldg(rays.origins + 3 * r + a), m.d[a] = __ldg(rays.directions + 3 * r + a);
-  m.radius = __ldg(rays.radii + r), m.near = __ldg(rays.near + r), m.far = __ldg(rays.far + r);
+  load_ray(rays, r, m);
+  m.near = __ldg(rays.near + r), m.far = __ldg(rays.far + r);
   sh_basis(__ldg(rays.viewdirs + 3 * r), __ldg(rays.viewdirs + 3 * r + 1), __ldg(rays.viewdirs + 3 * r + 2), y);
   const float(&o)[3] = m.o;
   const float(&d)[3] = m.d;
-  const float near = m.near, far = m.far;
+  const float near = m.near, far = m.far, dn = m.dn;
 
   // the sample lattice, every operation rounded as the contract states
-  const float dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
   const float span = __fsub_rn(far, near);
   const float kf = ceilf(__fdiv_rn(__fmul_rn(span, dn), step));
   const int64_t K = kf >= 1.f ? (int64_t)fminf(kf, 4e18f) : 1;
@@ -295,18 +322,6 @@ __device__ __forceinline__ void ray_setup(const GParams& g, const mipnerf_b200_r
     }
   }
   m.k0 = k0, m.k1 = k1;
-}
-
-// Sample k's t and position; whether the position is inside the bounds.
-__device__ __forceinline__ bool sample_at(const GParams& g, const RayMarch& m, int64_t k, float& t, float (&x)[3]) {
-  t = sample_t(m.near, m.dt, k);
-  bool inside = true;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    x[a] = __fadd_rn(m.o[a], __fmul_rn(t, m.d[a]));
-    inside = inside && x[a] >= g.lo[a] && x[a] <= g.hi[a];
-  }
-  return inside;
 }
 
 // Whether the macro cell of an inside position x is occupied; c is the cell.
@@ -344,6 +359,13 @@ struct Blend {
   float f;  // weight of level la + 1; level la has 1 - f (1 when f == 0, and level la + 1 is not read)
   int row_a[8], row_b[8];
   float w_a[8], w_b[8];
+
+  // visit(l, row, wc, lw) for each level the blend reads: its corner rows and weights and its level weight.
+  template <class Visit>
+  __device__ __forceinline__ void levels(Visit&& visit) const {
+    visit(la, row_a, w_a, f > 0.f ? 1.f - f : 1.f);
+    if (f > 0.f) visit(la + 1, row_b, w_b, f);
+  }
 };
 
 template <class Cells>
@@ -365,8 +387,34 @@ template <int NC, class Rows>
 __device__ __forceinline__ void blend_raw(const GParams& g, const Rows& rows, const Blend& b, const float (&y)[16],
                                           float (&raw)[3]) {
   raw[0] = raw[1] = raw[2] = 0.f;
-  level_color<NC>(rows.level(g, b.la), b.row_a, b.w_a, y, b.f > 0.f ? 1.f - b.f : 1.f, raw);
-  if (b.f > 0.f) level_color<NC>(rows.level(g, b.la + 1), b.row_b, b.w_b, y, b.f, raw);
+  b.levels([&](int l, const int (&row)[8], const float (&wc)[8], float lw) {
+    level_color<NC>(rows.level(g, l), row, wc, y, lw, raw);
+  });
+}
+
+// The samples of a ray's march whose density is looked up, front to back: inside the bounds and, for dt > 0, not in
+// an empty macro cell.  keep(sigma, b) is the caller's rule for which of them it uses (its rule for zero density), and
+// visit(t, sigma, b) is called for those, with the sample's t, blended density and level blend; the walk goes on while
+// visit returns true.  The rule is a separate argument, and visit's result means "go on" rather than "stop", because
+// in that loop shape no kernel spills: with the rule inside visit or a "stop" result, ptxas (CUDA 12.9) gives the
+// degree-2 uint8 brick render a 16-byte stack frame at its 96 registers.
+template <class Cells, class Keep, class Visit>
+__device__ __forceinline__ void walk_samples(const GParams& g, const Cells& cells, const RayMarch& m, Keep&& keep,
+                                             Visit&& visit) {
+  for (int64_t k = m.k0; k < m.k1;) {
+    const float t = sample_t(m.near, m.dt, k);
+    float x[3];
+    if (!ray_point(g, m, t, x)) {
+      ++k;
+      continue;
+    }
+    if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
+    Blend b;
+    const float sigma = blend_density(g, cells, m.radius, t, x, b);
+    ++k;
+    if (!keep(sigma, b)) continue;
+    if (!visit(t, sigma, b)) break;
+  }
 }
 
 // Front-to-back compositing state: transmittance and the running sums of the outputs.
@@ -386,25 +434,16 @@ __device__ __forceinline__ void composite(Composite& s, float alpha, const float
 template <int NC, class Rows, class Cells>
 __device__ __forceinline__ void march(const GParams& g, const Rows& rows, const Cells& cells, const RayMarch& m,
                                       const float (&y)[16], Composite& s) {
-  for (int64_t k = m.k0; k < m.k1;) {
-    float t, x[3];
-    if (!sample_at(g, m, k, t, x)) {
-      ++k;
-      continue;
-    }
-    if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
-    Blend b;
-    const float sigma = blend_density(g, cells, m.radius, t, x, b);
-    ++k;
-    if (!(sigma != 0.f)) continue;
+  const auto nonzero = [](float sigma, const Blend&) { return sigma != 0.f; };
+  walk_samples(g, cells, m, nonzero, [&](float t, float sigma, const Blend& b) {
     const float alpha = 1.f - expf(-sigma * m.delta);
     float raw[3], c[3];
     blend_raw<NC>(g, rows, b, y, raw);
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) c[ch] = g.rgb_scale / (1.f + expf(-raw[ch])) - g.rgb_padding;
     composite(s, alpha, c, t);
-    if (s.T < kStopTransmittance) break;
-  }
+    return !(s.T < kStopTransmittance);
+  });
 }
 
 template <int NC, class Rows, class Cells>
@@ -450,16 +489,21 @@ __device__ __forceinline__ void level_scatter(float* __restrict__ gd, float* __r
   }
 }
 
-__device__ __forceinline__ bool any_kept(const int (&row)[8]) {
+// Whether a level the blend reads has a kept corner.
+__device__ __forceinline__ bool any_kept(const Blend& b) {
   bool any = false;
+  b.levels([&](int, const int (&row)[8], const float (&)[8], float) {
 #pragma unroll
-  for (int c = 0; c < 8; ++c) any = any || row[c] >= 0;
+    for (int c = 0; c < 8; ++c) any = any || row[c] >= 0;
+  });
   return any;
 }
 
 // The gradient of grid_render_kernel's outputs, one thread per ray.  Pass 1 is the forward march (its totals: the
-// foreground rgb, acc and the unclamped distance).  Pass 2 walks the same samples front to back with the same
-// compositing arithmetic, so the prefix sums it forms equal the totals bit for bit at the last composited sample.  With
+// foreground rgb, acc and the unclamped distance).  Pass 2 walks with march's walk_samples over the same cells, so it
+// is handed the same samples; it also keeps a zero density with a kept corner, but composites only the samples march
+// composites, with composite, and stops where march stops.  So the prefix sums it forms equal the totals bit for bit
+// at the last composited sample.  With
 // e_k = g_rgb . c_k + g_acc' + g_dist t_k (g_acc' = g_acc - sum g_rgb under a white background) and w_k = T_k alpha_k,
 // dL/dsigma_k = delta (T_{k+1} e_k - sum_{j > k} w_j e_j), the suffix being total - prefix, and dL/draw_k = w_k g_rgb
 // (1 + 2 rgb_padding) s (1 - s) for s the sigmoid of the raw colour.
@@ -484,19 +528,10 @@ __global__ void __launch_bounds__(kGridThreads)
   if (!(total.dist >= m.near && total.dist <= m.far)) g_dist = 0.f;  // the clamp passes the gradient inside, inclusive
 
   Composite s;
-  for (int64_t k = m.k0; k < m.k1;) {
-    float t, x[3];
-    if (!sample_at(g, m, k, t, x)) {
-      ++k;
-      continue;
-    }
-    if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
-    Blend b;
-    const float sigma = blend_density(g, DenseCells{}, m.radius, t, x, b);
-    ++k;
-    // a zero density still has a gradient; it reaches parameters only through kept corners
+  // a zero density still has a gradient; it reaches parameters only through kept corners
+  const auto has_gradient = [](float sigma, const Blend& b) { return sigma != 0.f || any_kept(b); };
+  walk_samples(g, DenseCells{}, m, has_gradient, [&](float t, float sigma, const Blend& b) {
     const bool zero = !(sigma != 0.f);
-    if (zero && !any_kept(b.row_a) && !(b.f > 0.f && any_kept(b.row_b))) continue;
     const float alpha = 1.f - expf(-sigma * m.delta);
     float raw[3], c[3], sg[3];
     blend_raw<NC>(g, F32Rows{}, b, y, raw);
@@ -516,12 +551,11 @@ __global__ void __launch_bounds__(kGridThreads)
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) d_raw[ch] = w * g_rgb[ch] * g.rgb_scale * sg[ch] * (1.f - sg[ch]);
     const bool color = !zero;  // w == 0 at a zero density
-    level_scatter<NC>(grads.density[b.la], grads.sh[b.la], b.row_a, b.w_a, b.f > 0.f ? 1.f - b.f : 1.f, y, d_sigma,
-                      d_raw, color);
-    if (b.f > 0.f)
-      level_scatter<NC>(grads.density[b.la + 1], grads.sh[b.la + 1], b.row_b, b.w_b, b.f, y, d_sigma, d_raw, color);
-    if (s.T < kStopTransmittance) break;
-  }
+    b.levels([&](int l, const int (&row)[8], const float (&wc)[8], float lw) {
+      level_scatter<NC>(grads.density[l], grads.sh[l], row, wc, lw, y, d_sigma, d_raw, color);
+    });
+    return !(s.T < kStopTransmittance);
+  });
 }
 
 // Raise one level's kept corners to their scores at a composited sample of blending weight w: corner c's score is
@@ -540,11 +574,11 @@ __device__ __forceinline__ void level_visibility(float* __restrict__ max_weight,
   }
 }
 
-// Per kept corner, the largest score over these rays (mipnerf_b200_grid_visibility), one thread per ray.  The march
-// is the forward's for density only: the same samples, skipping, level blend and trilinear weights, the same
-// compositing arithmetic on T (w_k = T_k alpha_k exactly as `composite` forms it) and the same stop after the sample
-// that leaves T < 1e-4; no colour is evaluated.  A maximum does not depend on the order of its updates, so the result
-// is bit for bit the same across runs, across any split of the rays into calls, and under any permutation of the rays.
+// Per kept corner, the largest score over these rays (mipnerf_b200_grid_visibility), one thread per ray.  It walks with
+// march's walk_samples and zero-density rule, for density only: it is handed the forward's samples, level blends and
+// trilinear weights, forms w_k = T_k alpha_k with composite's arithmetic on T, and stops after the sample that leaves
+// T < 1e-4; no colour is evaluated.  A maximum does not depend on the order of its updates, so the result is bit for
+// bit the same across runs, across any split of the rays into calls, and under any permutation of the rays.
 // With BrickCells (mipnerf_b200_grid_visibility_bricks) every corner reads the word the dense cells hold, so the scores
 // equal the dense kernel's on the densified grid bit for bit.
 template <class Cells>
@@ -557,54 +591,27 @@ __global__ void __launch_bounds__(kGridThreads)
   float y[16];
   ray_setup(g, rays, r, step, m, y);
   float T = 1.f;
-  for (int64_t k = m.k0; k < m.k1;) {
-    float t, x[3];
-    if (!sample_at(g, m, k, t, x)) {
-      ++k;
-      continue;
-    }
-    if (m.dt > 0.f && skip_empty(g, m, x, k)) continue;
-    Blend b;
-    const float sigma = blend_density(g, cells, m.radius, t, x, b);
-    ++k;
-    if (!(sigma != 0.f)) continue;
+  const auto nonzero = [](float sigma, const Blend&) { return sigma != 0.f; };
+  walk_samples(g, cells, m, nonzero, [&](float, float sigma, const Blend& b) {
     const float alpha = 1.f - expf(-sigma * m.delta);
     const float w = T * alpha;
-    level_visibility(max_weight.w[b.la], b.row_a, b.w_a, b.f > 0.f ? 1.f - b.f : 1.f, w);
-    if (b.f > 0.f) level_visibility(max_weight.w[b.la + 1], b.row_b, b.w_b, b.f, w);
+    b.levels([&](int l, const int (&row)[8], const float (&wc)[8], float lw) {
+      level_visibility(max_weight.w[l], row, wc, lw, w);
+    });
     T *= 1.f - alpha;
-    if (T < kStopTransmittance) break;
-  }
+    return !(T < kStopTransmittance);
+  });
 }
 
-// One ray of the proposal kernels: origin, direction, radius and |d|, rounded as the header states.
-struct ProposalRay {
-  float o[3], d[3];
-  float radius, dn;
-};
-
-__device__ __forceinline__ void proposal_ray(const mipnerf_b200_rays& rays, int64_t r, ProposalRay& p) {
-#pragma unroll
-  for (int a = 0; a < 3; ++a) p.o[a] = __ldg(rays.origins + 3 * r + a), p.d[a] = __ldg(rays.directions + 3 * r + a);
-  p.radius = __ldg(rays.radii + r);
-  p.dn = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(p.d[0], p.d[0]), __fmul_rn(p.d[1], p.d[1])),
-                              __fmul_rn(p.d[2], p.d[2])));
-}
-
-// Interval [t0, t1] of a proposal ray: its delta, and the density at its midpoint under the level blend.  A midpoint
-// outside the bounds or in an empty macro cell is not looked up (density 0, `looked_up` false, `b` unset).
+// Interval [t0, t1] of a ray: its delta, and the density at its midpoint under the level blend.  A midpoint outside
+// the bounds or in an empty macro cell is not looked up (density 0, `looked_up` false, `b` unset).
 template <class Cells>
-__device__ __forceinline__ float proposal_density(const GParams& g, const Cells& cells, const ProposalRay& p, float t0,
+__device__ __forceinline__ float proposal_density(const GParams& g, const Cells& cells, const Ray& p, float t0,
                                                   float t1, float& delta, Blend& b, bool& looked_up) {
   const float tm = __fmul_rn(__fadd_rn(t0, t1), 0.5f);
   delta = __fmul_rn(__fsub_rn(t1, t0), p.dn);
   float x[3];
-  bool inside = true;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    x[a] = __fadd_rn(p.o[a], __fmul_rn(tm, p.d[a]));
-    inside = inside && x[a] >= g.lo[a] && x[a] <= g.hi[a];
-  }
+  const bool inside = ray_point(g, p, tm, x);
   float sigma = 0.f;
   int c[3];
   looked_up = false;
@@ -615,10 +622,30 @@ __device__ __forceinline__ float proposal_density(const GParams& g, const Cells&
   return sigma;
 }
 
-// Proposal weights of the caller's intervals (mipnerf_b200_grid_proposal), one thread per ray.  Interval i is sampled
-// at its midpoint with blend_density, and its weight is volumetric_rendering's (1 - exp(-s_i)) exp(-sum_{j<i} s_j),
-// s_i = sigma_i delta_i, with every interval weighted: no stop.  A midpoint in an empty macro cell has density exactly
-// 0 at every level (the occupancy rule skip_empty relies on), so its lookup is skipped and s_i = 0 exactly: the result
+// The n intervals of a ray between its fenceposts t[0..n], front to back, with volumetric_rendering's weights and no
+// stop: s_i = fl(sigma_i delta_i) from proposal_density, w_i = fl(fl(1 - e^{-s_i}) e^{-S_i}) and S_{i+1} = fl(S_i +
+// s_i), S_0 = 0, every rounding as mipnerf_b200.h states.  visit(i, w_i, S_{i+1}, delta_i, looked_up, b) for each.
+template <class Cells, class Visit>
+__device__ __forceinline__ void walk_intervals(const GParams& g, const Cells& cells, const Ray& p, const float* t,
+                                               int n, Visit&& visit) {
+  float S = 0.f;
+  float t0 = __ldg(t);
+  for (int i = 0; i < n; ++i) {
+    const float t1 = __ldg(t + i + 1);
+    float delta;
+    Blend b;
+    bool looked_up;
+    const float s = __fmul_rn(proposal_density(g, cells, p, t0, t1, delta, b, looked_up), delta);
+    t0 = t1;
+    const float w = __fmul_rn(__fsub_rn(1.f, expf(-s)), expf(-S));
+    S = __fadd_rn(S, s);
+    visit(i, w, S, delta, looked_up, b);
+  }
+}
+
+// Proposal weights of the caller's intervals (mipnerf_b200_grid_proposal), one thread per ray: walk_intervals' w_i.
+// Interval i is sampled at its midpoint with blend_density.  A midpoint in an empty macro cell has density exactly 0
+// at every level (the occupancy rule skip_empty relies on), so its lookup is skipped and s_i = 0 exactly: the result
 // equals the all-occupied grid's bit for bit.  No SH row is read.
 template <class Cells>
 __global__ void __launch_bounds__(kGridThreads)
@@ -626,79 +653,49 @@ __global__ void __launch_bounds__(kGridThreads)
                          int num_samples, float* __restrict__ weights, const __grid_constant__ Cells cells) {
   const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
   if (r >= rays.num_rays) return;
-  ProposalRay p;
-  proposal_ray(rays, r, p);
-  const float* t = t_samples + r * (num_samples + 1);
-  float* w = weights + r * num_samples;
-  float depth = 0.f;  // sum_{j<i} s_j
-  float t0 = __ldg(t);
-  for (int i = 0; i < num_samples; ++i) {
-    const float t1 = __ldg(t + i + 1);
-    float delta;
-    Blend b;
-    bool looked_up;
-    const float sigma = proposal_density(g, cells, p, t0, t1, delta, b, looked_up);
-    t0 = t1;
-    const float s = __fmul_rn(sigma, delta);
-    w[i] = __fmul_rn(__fsub_rn(1.f, expf(-s)), expf(-depth));
-    depth = __fadd_rn(depth, s);
-  }
+  Ray p;
+  load_ray(rays, r, p);
+  float* out = weights + r * num_samples;
+  walk_intervals(g, cells, p, t_samples + r * (num_samples + 1), num_samples,
+                 [&](int i, float w, float, float, bool, const Blend&) { out[i] = w; });
 }
 
 // The gradient of grid_proposal_kernel's weights with respect to the densities (mipnerf_b200_grid_proposal_backward),
 // dense fp32 cells, one thread per ray.  With g_i = d_weights[i], s_i = sigma_i delta_i and S_i = sum_{j<i} s_j, w_i =
-// e^{-S_i} - e^{-S_{i+1}}, so dL/ds_k = g_k e^{-S_{k+1}} - sum_{i>k} g_i w_i and dL/dsigma_k = delta_k dL/ds_k.  Pass 1
-// recomputes every w_i with the forward's fp32 expressions and sums g_i w_i; pass 2 walks the intervals again with the
-// same arithmetic, so its prefix sum reaches the total bit for bit, and takes the suffix as total - prefix, as
-// grid_render_backward_kernel does.  An interval the forward does not look up (midpoint outside the bounds or in an
-// empty macro cell) gets no gradient; the others scatter through the level blend and the trilinear weights into the
-// kept corners (level_scatter, density only).
+// e^{-S_i} - e^{-S_{i+1}}, so dL/ds_k = g_k e^{-S_{k+1}} - sum_{i>k} g_i w_i and dL/dsigma_k = delta_k dL/ds_k.  Both
+// passes are the forward's walk_intervals, so they are handed the forward's w_i.  Pass 1 sums g_i w_i; pass 2 sums
+// them again in the same order, so its prefix sum reaches the total bit for bit, and takes the suffix as total -
+// prefix, as grid_render_backward_kernel does.  An interval the forward does not look up (midpoint outside the bounds
+// or in an empty macro cell) gets no gradient; the others scatter through the level blend and the trilinear weights
+// into the kept corners (level_scatter, density only).
 __global__ void __launch_bounds__(kGridThreads)
     grid_proposal_backward_kernel(const GParams g, const mipnerf_b200_rays rays, const float* __restrict__ t_samples,
                                   int num_samples, const float* __restrict__ d_weights,
                                   const __grid_constant__ mipnerf_b200_grid_grads grads) {
   const int64_t r = (int64_t)blockIdx.x * kGridThreads + threadIdx.x;
   if (r >= rays.num_rays) return;
-  ProposalRay p;
-  proposal_ray(rays, r, p);
+  Ray p;
+  load_ray(rays, r, p);
   const float* t = t_samples + r * (num_samples + 1);
   const float* gw = d_weights + r * num_samples;
-  float total = 0.f, depth = 0.f;
-  float t0 = __ldg(t);
-  for (int i = 0; i < num_samples; ++i) {
-    const float t1 = __ldg(t + i + 1);
-    float delta;
-    Blend b;
-    bool looked_up;
-    const float s = __fmul_rn(proposal_density(g, DenseCells{}, p, t0, t1, delta, b, looked_up), delta);
-    t0 = t1;
-    const float w = __fmul_rn(__fsub_rn(1.f, expf(-s)), expf(-depth));
-    depth = __fadd_rn(depth, s);
+  float total = 0.f;
+  walk_intervals(g, DenseCells{}, p, t, num_samples, [&](int i, float w, float, float, bool, const Blend&) {
     total = __fmaf_rn(__ldg(gw + i), w, total);
-  }
+  });
   const float y[16] = {};
   const float d_raw[3] = {};
   float prefix = 0.f;
-  depth = 0.f;
-  t0 = __ldg(t);
-  for (int i = 0; i < num_samples; ++i) {
-    const float t1 = __ldg(t + i + 1);
-    float delta;
-    Blend b;
-    bool looked_up;
-    const float s = __fmul_rn(proposal_density(g, DenseCells{}, p, t0, t1, delta, b, looked_up), delta);
-    t0 = t1;
-    const float w = __fmul_rn(__fsub_rn(1.f, expf(-s)), expf(-depth));
-    depth = __fadd_rn(depth, s);  // S_{i+1}
-    const float gi = __ldg(gw + i);
-    prefix = __fmaf_rn(gi, w, prefix);
-    if (!looked_up) continue;
-    const float d_sigma = delta * (gi * expf(-depth) - (total - prefix));
-    if (d_sigma == 0.f) continue;
-    level_scatter<1>(grads.density[b.la], nullptr, b.row_a, b.w_a, b.f > 0.f ? 1.f - b.f : 1.f, y, d_sigma, d_raw,
-                     false);
-    if (b.f > 0.f) level_scatter<1>(grads.density[b.la + 1], nullptr, b.row_b, b.w_b, b.f, y, d_sigma, d_raw, false);
-  }
+  walk_intervals(g, DenseCells{}, p, t, num_samples,
+                 [&](int i, float w, float S, float delta, bool looked_up, const Blend& b) {
+                   const float gi = __ldg(gw + i);
+                   prefix = __fmaf_rn(gi, w, prefix);
+                   if (!looked_up) return;
+                   const float d_sigma = delta * (gi * expf(-S) - (total - prefix));
+                   if (d_sigma == 0.f) return;
+                   b.levels([&](int l, const int (&row)[8], const float (&wc)[8], float lw) {
+                     level_scatter<1>(grads.density[l], nullptr, row, wc, lw, y, d_sigma, d_raw, false);
+                   });
+                 });
 }
 
 GParams make_params(const mipnerf_b200_grid& grid) {
@@ -734,84 +731,87 @@ GParams make_params(const mipnerf_b200_grid& grid) {
 
 unsigned grid_blocks(int64_t num_rays) { return (unsigned)((num_rays + kGridThreads - 1) / kGridThreads); }
 
+// The prologue every launcher below shares: nothing to launch for no rays; otherwise launch(g, blocks) with `grid`'s
+// kernel parameters and the grid size of num_rays, timed under profiler id `id`.  Returns the launch's error.
+template <class Launch>
+cudaError_t launch_rays(const mipnerf_b200_grid& grid, int64_t num_rays, int id, cudaStream_t st, Launch&& launch) {
+  if (num_rays == 0) return cudaSuccess;
+  const GParams g = make_params(grid);
+  LaunchScope scope(id, st);
+  launch(g, grid_blocks(num_rays));
+  return cudaGetLastError();
+}
+
+// f(cells) with the cell reader of the nullable `bricks`: BrickCells over them, or DenseCells for levels[l].cells.
+template <class F>
+void with_cells(const mipnerf_b200_grid_bricks* bricks, F&& f) {
+  if (bricks) return f(BrickCells{*bricks});
+  f(DenseCells{});
+}
+
 }  // namespace
 
 cudaError_t launch_grid_render(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
                                const mipnerf_b200_grid_sh_u8* sh, const mipnerf_b200_rays& rays, float step,
                                int white_bkgd, float* rgb, float* distance, float* acc, int id, cudaStream_t st) {
-  if (rays.num_rays == 0) return cudaSuccess;
-  const GParams g = make_params(grid);
-  LaunchScope scope(id, st);
-  // the cells and the rows: levels[l].cells and the fp32 levels[l].sh, or the bricks and the uint8 rows given
-  const auto launch = [&](const auto& rows, const auto& cells) {
-    using Rows = std::decay_t<decltype(rows)>;
-    using Cells = std::decay_t<decltype(cells)>;
-    with_sh_coeffs(grid.degree, [&](auto nc) {
-      grid_render_kernel<decltype(nc)::value, Rows, Cells><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
-          g, rays, step, white_bkgd, rgb, distance, acc, rows, cells);
+  return launch_rays(grid, rays.num_rays, id, st, [&](const GParams& g, unsigned blocks) {
+    // the rows: the fp32 levels[l].sh, or the uint8 rows given
+    const auto launch = [&](const auto& rows, const auto& cells) {
+      using Rows = std::decay_t<decltype(rows)>;
+      using Cells = std::decay_t<decltype(cells)>;
+      with_sh_coeffs(grid.degree, [&](auto nc) {
+        grid_render_kernel<decltype(nc)::value, Rows, Cells><<<blocks, kGridThreads, 0, st>>>(
+            g, rays, step, white_bkgd, rgb, distance, acc, rows, cells);
+      });
+    };
+    with_cells(bricks, [&](const auto& cells) {
+      if (sh) launch(U8Rows{*sh}, cells);
+      else launch(F32Rows{}, cells);
     });
-  };
-  if (bricks && sh) launch(U8Rows{*sh}, BrickCells{*bricks});
-  else if (bricks) launch(F32Rows{}, BrickCells{*bricks});
-  else if (sh) launch(U8Rows{*sh}, DenseCells{});
-  else launch(F32Rows{}, DenseCells{});
-  return cudaGetLastError();
+  });
 }
 
 cudaError_t launch_grid_render_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays, float step,
                                         int white_bkgd, const float* d_rgb, const float* d_distance,
                                         const float* d_acc, const mipnerf_b200_grid_grads& grads, cudaStream_t st) {
-  if (rays.num_rays == 0 || (!d_rgb && !d_distance && !d_acc)) return cudaSuccess;
-  const GParams g = make_params(grid);
-  LaunchScope scope(kKernGridRenderBackward, st);
-  with_sh_coeffs(grid.degree, [&](auto nc) {
-    grid_render_backward_kernel<decltype(nc)::value><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
-        g, rays, step, white_bkgd, d_rgb, d_distance, d_acc, grads);
+  if (!d_rgb && !d_distance && !d_acc) return cudaSuccess;
+  return launch_rays(grid, rays.num_rays, kKernGridRenderBackward, st, [&](const GParams& g, unsigned blocks) {
+    with_sh_coeffs(grid.degree, [&](auto nc) {
+      grid_render_backward_kernel<decltype(nc)::value><<<blocks, kGridThreads, 0, st>>>(
+          g, rays, step, white_bkgd, d_rgb, d_distance, d_acc, grads);
+    });
   });
-  return cudaGetLastError();
 }
 
 cudaError_t launch_grid_visibility(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
                                    const mipnerf_b200_rays& rays, float step, float* const* max_weight, int id,
                                    cudaStream_t st) {
-  if (rays.num_rays == 0) return cudaSuccess;
-  const GParams g = make_params(grid);
-  GMaxWeight mw{};
-  for (int l = 0; l < grid.num_levels; ++l) mw.w[l] = max_weight[l];
-  LaunchScope scope(id, st);
-  const auto launch = [&](const auto& cells) {
-    grid_visibility_kernel<std::decay_t<decltype(cells)>><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
-        g, rays, step, mw, cells);
-  };
-  if (bricks) launch(BrickCells{*bricks});
-  else launch(DenseCells{});
-  return cudaGetLastError();
+  return launch_rays(grid, rays.num_rays, id, st, [&](const GParams& g, unsigned blocks) {
+    GMaxWeight mw{};
+    for (int l = 0; l < grid.num_levels; ++l) mw.w[l] = max_weight[l];
+    with_cells(bricks, [&](const auto& cells) {
+      grid_visibility_kernel<std::decay_t<decltype(cells)>><<<blocks, kGridThreads, 0, st>>>(g, rays, step, mw, cells);
+    });
+  });
 }
 
 cudaError_t launch_grid_proposal(const mipnerf_b200_grid& grid, const mipnerf_b200_grid_bricks* bricks,
                                  const mipnerf_b200_rays& rays, const float* t_samples, int num_samples,
                                  float* weights, cudaStream_t st) {
-  if (rays.num_rays == 0) return cudaSuccess;
-  const GParams g = make_params(grid);
-  LaunchScope scope(kKernGridProposal, st);
-  const auto launch = [&](const auto& cells) {
-    grid_proposal_kernel<std::decay_t<decltype(cells)>><<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(
-        g, rays, t_samples, num_samples, weights, cells);
-  };
-  if (bricks) launch(BrickCells{*bricks});
-  else launch(DenseCells{});
-  return cudaGetLastError();
+  return launch_rays(grid, rays.num_rays, kKernGridProposal, st, [&](const GParams& g, unsigned blocks) {
+    with_cells(bricks, [&](const auto& cells) {
+      grid_proposal_kernel<std::decay_t<decltype(cells)>><<<blocks, kGridThreads, 0, st>>>(
+          g, rays, t_samples, num_samples, weights, cells);
+    });
+  });
 }
 
 cudaError_t launch_grid_proposal_backward(const mipnerf_b200_grid& grid, const mipnerf_b200_rays& rays,
                                           const float* t_samples, int num_samples, const float* d_weights,
                                           const mipnerf_b200_grid_grads& grads, cudaStream_t st) {
-  if (rays.num_rays == 0) return cudaSuccess;
-  const GParams g = make_params(grid);
-  LaunchScope scope(kKernGridProposalBackward, st);
-  grid_proposal_backward_kernel<<<grid_blocks(rays.num_rays), kGridThreads, 0, st>>>(g, rays, t_samples, num_samples,
-                                                                                     d_weights, grads);
-  return cudaGetLastError();
+  return launch_rays(grid, rays.num_rays, kKernGridProposalBackward, st, [&](const GParams& g, unsigned blocks) {
+    grid_proposal_backward_kernel<<<blocks, kGridThreads, 0, st>>>(g, rays, t_samples, num_samples, d_weights, grads);
+  });
 }
 
 }  // namespace mipnerf
